@@ -2,7 +2,7 @@
 """Benchmark of the WCT inference hot path (BASELINE.json metric: 512x512 five-level
 stylised frames/sec), one process per GPU.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path (WCT.predict semantics: encode style, then
 [encode -> WCT -> decode] x relu5_1..relu1_1, wct_tf semantics, alpha=0.8) over one batch
@@ -13,7 +13,7 @@ no work is shared or cached between frames).
   value   frames/s, inputs (uint8 frames) already resident in HBM, CUDA-event timed
   e2e     frames/s through the public API (WCT.predict_batch) with PINNED HOST uint8
           buffers: H2D of contents+styles and D2H of the uint8 results inside the timed region
-  roofline  the dominant kernel = conv_tc2_kernel (tcgen05 implicit-GEMM conv): EXECUTED algorithmic conv
+  roofline  the dominant kernel = conv_tc2_kernel (wgmma implicit-GEMM conv): EXECUTED algorithmic conv
           FLOPs (2*taps*Cin*Cout per output pixel; 4 taps for the convs that absorbed an UpSampling2D) /
           CUDA-event time of those launches, vs the measured bf16 peak; per-level tensor-pipe fractions and
           covariance-only HBM GB/s beside it (north_star)
@@ -22,6 +22,10 @@ no work is shared or cached between frames).
 
 --impl reference: TensorFlow 1.x / Keras 2.0.9 are not installable offline, so the
 reference arm is the oracle port run on all host threads (kind "port").
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step returned (the uint8 stylised frames)
+for a fixed, seeded subset of its frames as DIR/stylized_frames.npy (float32 [k,512,512,3]) and the frame indices as
+DIR/stylized_frame_index.npy (float64).  Inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -62,7 +66,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d.get("hbm_gbs", 6650.0), tf=d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)),
                     source="MEASURED_PEAKS.json (bf16_tflops_sustained)")
-    return dict(hbm_gbs=6650.0, tf=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16/FP16 -- not measured here
+    return dict(hbm_gbs=3350.0, tf=989.0, source="H100 SXM data sheet (dense FP16)")
 
 
 class ClockSampler(object):
@@ -133,11 +138,11 @@ def make_config(world, B, adain, groups, scaling, global_batch):
     cfg = {"workload": WORKLOAD if not adain else WORKLOAD.replace("wct_tf semantics", "AdaIN (configs[4])"),
            "frames_per_gpu_per_step": B, "global_batch": global_batch, "parallelism": "frame-sharded dp%d" % world,
            "style": "one distinct style per frame, re-encoded every step (no caching)",
-           "l2": "two input sets alternate; per-step activation working set (>5 GB) >> 126 MB L2",
-           "precision": "fp32-class: split-fp16 pairs (22-23 bits, power-of-two scaled weights) x3 products on tcgen05, "
-                        "fp32 accumulate (TMEM chunks of 4 k-iterations summed in registers)",
+           "l2": "two input sets alternate; per-step activation working set (>5 GB) >> 50 MB L2",
+           "precision": "fp32-class: split-fp16 pairs (22-23 bits, power-of-two scaled weights) x3 products on wgmma, "
+                        "fp32 accumulate (chunks of 4 k-iterations summed in registers)",
            "transform": "whitening / colouring matrices per frame and level from the frame's own covariances: coupled Newton-Schulz "
-                        "on tcgen05 where the 1e-5 threshold provably keeps every eigenvalue (all matrices of this synthetic "
+                        "on wgmma where the 1e-5 threshold provably keeps every eigenvalue (all matrices of this synthetic "
                         "workload: k = C), Jacobi eigendecomposition otherwise",
            "streams": "%d sub-batch group(s) per step, each a (content, style) stream pair" % groups}
     if scaling == "strong":
@@ -204,8 +209,9 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--batch", type=int, default=30, help="frames per GPU per step (30 = two sub-batches of 15: at most 15 eigensolver clusters of 8 CTAs are co-resident on a B200)")
-    ap.add_argument("--impl", type=str, default="b200")
+    ap.add_argument("--batch", type=int, default=30, help="frames per GPU per step (two sub-batches of 15 by default: each sub-batch "
+                    "runs one eigensolver cluster of 8 CTAs per frame where the fast path does not apply)")
+    ap.add_argument("--impl", type=str, default="cuda")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--adain", action="store_true", help="config 5: AdaIN instead of WCT")
     ap.add_argument("--scaling", choices=["weak", "strong"], default="weak",
@@ -220,6 +226,8 @@ def main():
     ap.add_argument("--no-fuse-pool", action="store_true", help="tuning: separate maxpool2 kernels after conv1_2/2_2/3_4/4_4")
     ap.add_argument("--no-roofline", action="store_true", help="skip the per-kernel profiling steps")
     ap.add_argument("--jacobi-tolq", type=float, default=0.0, help="tuning: eigensolver predicted-convergence level (0 = library default)")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write a seeded sample of the last timed step's output frames to DIR/*.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -296,8 +304,9 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         n0 = eng.launches
         e0.record()
+        last = None
         for i in range(steps):
-            fn(i)
+            last = fn(i)
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1)
@@ -306,14 +315,23 @@ def main():
             t = torch.tensor([ms], device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             ms = float(t.item())
-        return ms, launches
+        return ms, launches, last
 
+    assert args.steps >= 1, "--steps must be >= 1"
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    ms_total, launches = timed(step_resident, args.steps, args.warmup)
+    ms_total, launches, last_out = timed(step_resident, args.steps, args.warmup)
     clocks = sampler.stop() if rank == 0 else None
-    ms_e2e, _ = timed(step_e2e, args.steps, max(3, args.warmup // 2))
+    if args.dump_outputs and rank == 0:
+        # the last timed step's frames (uint8, what step_resident hands back), a fixed seeded subset of <= 8 frames:
+        # 8 x 512 x 512 x 3 float32 = 24 MB
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        idx = np.sort(np.random.default_rng(1234).choice(B, size=min(B, 8), replace=False))
+        np.save(os.path.join(args.dump_outputs, "stylized_frames.npy"), last_out[torch.from_numpy(idx).to(dev)].cpu().numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "stylized_frame_index.npy"), idx.astype(np.float64))
+    del last_out
+    ms_e2e, _, _ = timed(step_e2e, args.steps, max(3, args.warmup // 2))
     eng.check_device()
 
     pk = peaks()
@@ -349,15 +367,10 @@ def main():
         conv_fl = sum(v["flops"] for v in conv.values())
         step_prof_ms = sum(v["ms"] for v in prof.values())
         achieved_tf = conv_fl / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
-        traffic, traffic_of = None, ("not captured for this build: needs one `ncu --set full` launch of conv_tc2_kernel at the "
-                                     "bench batch (profiles/r02_conv_traffic.json)")
-        tp = os.path.join(ROOT, "profiles", "r02_conv_traffic.json")
-        if os.path.exists(tp):
-            tj = json.load(open(tp))
-            traffic, traffic_of = tj.get("dram_bytes_per_launch"), tj.get("of")
+        traffic, traffic_of = None, "not measured (DRAM bytes per conv launch need a hardware-counter profile)"
         roofline = {"bound": "tensor", "achieved": achieved_tf, "peak": pk["tf"], "unit": "TFLOP/s",
                     "frac": achieved_tf / pk["tf"], "traffic": traffic, "traffic_of": traffic_of,
-                    "kernel": "conv_tc2_kernel (tcgen05 kind::f16, split-fp16 x3: 3 MMAs per algorithmic MAC -> ceiling 1/3 of the "
+                    "kernel": "conv_tc2_kernel (wgmma f16, split-fp16 x3: 3 MMAs per algorithmic MAC -> ceiling 1/3 of the "
                               "bf16 peak); flops counted = EXECUTED 2*taps*Cin*Cout per output pixel (taps = 4 in the UP2 convs)",
                     "tensor_pipe_frac": 3.0 * achieved_tf / pk["tf"],
                     "peak_source": pk["source"] + " of measured",
@@ -425,7 +438,7 @@ def main():
                                                 c_all, s_one)
             sharded_inputs = [(torch.from_numpy(frames(GB, 1000 + 1000 * j)).to(dev), torch.from_numpy(frames(1, 7 + 1000 * j)).to(dev))
                               for j in range(2)]
-            sharded_ms, _ = timed(sharded_step, max(3, args.steps // 2), 3)     # sharded compute + NCCL gather, event timed, max over ranks
+            sharded_ms, _, _ = timed(sharded_step, max(3, args.steps // 2), 3)     # sharded compute + NCCL gather, event timed, max over ranks
             sharded_ms /= max(3, args.steps // 2)
         else:
             for _ in range(3):

@@ -1,5 +1,5 @@
 /*
- * libwctb200 -- C-ABI of the B200-native WCT inference hot path.
+ * libwctb200 -- C-ABI of the H100-native (sm_90a) WCT inference hot path.
  *
  * The reference (eridgd/WCT-TF) has no native boundary: its operator surface is
  * Python (`WCT.predict` wct.py:70, `WCTModel` model.py:33, `wct_np/wct_tf/adain`
@@ -14,7 +14,7 @@
  *     the caller (e.g. `torch.Tensor.data_ptr()`), kept alive until `stream` is synced;
  *   - asynchronous on `stream` (a `cudaStream_t` passed as void*; 0 = default stream);
  *     the caller selects the device (`cudaSetDevice`) before the call;
- *   - no CPU fallback: without an sm_100 device the kernels fail with WCTB200_ECUDA.
+ *   - no CPU fallback: without an sm_90 device the kernels fail with WCTB200_ECUDA.
  *
  * Activation format "SPF16" (split-pair fp16, reflect-padded NHWC):
  *   one allocation of `wctb200_act_bytes(N,H,W,C)` bytes holding two fp16 planes
@@ -45,7 +45,7 @@ extern "C" {
 
 #define WCTB200_OK       0
 #define WCTB200_EINVAL  -1   /* bad argument / unsupported shape */
-#define WCTB200_ECUDA   -2   /* CUDA runtime / driver error (incl. no sm_100 device) */
+#define WCTB200_ECUDA   -2   /* CUDA runtime / driver error (incl. no sm_90 device) */
 #define WCTB200_EWS     -3   /* workspace too small */
 #define WCTB200_EDEVICE -4   /* a kernel flagged an internal error (pipeline timeout) */
 
@@ -62,7 +62,7 @@ extern "C" {
 WCTB200_API int         wctb200_abi_version(void);
 WCTB200_API const char* wctb200_last_error(void);
 /* Synchronises `stream` and returns WCTB200_EDEVICE if any kernel since the last
- * call recorded an internal error (mbarrier timeout in the tcgen05 pipeline). */
+ * call recorded an internal error (mbarrier timeout in a TMA / wgmma pipeline). */
 WCTB200_API int         wctb200_check_device(void* stream);
 
 /* ---- SPF16 activations ---------------------------------------------------- */
@@ -112,7 +112,7 @@ WCTB200_API int wctb200_prep_conv_weights(const float* w_hwio, int taps, int Cin
  * pixel; [4 parities][2 planes][Cout][4*Cin].  Buffer size: wctb200_conv_weight_bytes(16, Cin, Cout). */
 WCTB200_API int wctb200_prep_conv_weights_up2(const float* w_hwio, int Cin, int Cout, void* w_up2, void* stream);
 
-/* Conv2DReflect 3x3 (+bias, optional ReLU) on tensor cores (tcgen05, split-fp16 x3):
+/* Conv2DReflect 3x3 (+bias, optional ReLU) on tensor cores (wgmma, split-fp16 x3):
  * replaces `Lambda(pad_reflect) -> Conv2D(valid)` of vgg_normalised.py:28-40 and
  * model.py:291.  Cin, Cout multiples of 64.  in/out: SPF16 [N,H,W,Cin] -> [N,H,W,Cout]
  * ([N,ceil(H/2),ceil(W/2),Cout] with WCTB200_POOL2). */

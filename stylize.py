@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Command line front end with the flag surface of the reference's stylize.py (flags at stylize.py:14-37, the
 content x style loop at stylize.py:70-119, output naming ``<content>_<style><ext>``): the TF session behind
-``WCT.predict`` is replaced by the B200 engine.
+``WCT.predict`` is replaced by the H100 engine.
 
   python stylize.py --checkpoints DIR5 DIR4 ... --relu-targets relu5_1 relu4_1 ... --vgg-path vgg_normalised.t7 \
       --content-path IN --style-path STYLE --out-path OUT --alpha 0.8

@@ -25,8 +25,8 @@ CASES = [
     ("c64_a10", 64, (24, 20), (16, 28), 1.0, 0, 1),
     ("c64_a06", 64, (24, 20), (16, 28), 0.6, 0, 2),
     ("c128_a08_dead", 128, (20, 20), (24, 18), 0.8, 9, 3),
-    ("c256_a08", 256, (18, 18), (17, 20), 0.8, 0, 4),
-    ("c512_a08_dead", 512, (24, 24), (23, 26), 0.8, 40, 5),
+    ("c256_a08", 256, (14, 14), (13, 16), 0.8, 0, 4),        # sizes keep every file under 1 MB
+    ("c512_a08_dead", 512, (10, 10), (9, 12), 0.8, 40, 5),
 ]
 
 
@@ -39,10 +39,12 @@ def features(rng, c, hw, dead):
     return x.reshape(1, h, w, c).astype(np.float32)
 
 
-def main():
+def main(only=None):
     ref = ref_ops.load_reference_ops()
-    assert ref is not None, "/root/reference/ops.py not found: run in the build container"
+    assert ref is not None, "the reference's ops.py was not found"
     for name, c, hwc, hws, alpha, dead, seed in CASES:
+        if only and name not in only:
+            continue
         rng = np.random.default_rng(seed)
         content = features(rng, c, hwc, dead)
         style = features(rng, c, hws, 0)
@@ -72,6 +74,36 @@ def coral_golden():
     print("coral golden", out.shape, out.mean())
 
 
+def t7_golden():
+    """What the reference's torchfile.py (force_8bytes_long=True, vgg_normalised.py:16) reads back from the .t7 that
+    tests/t7_writer.py writes for make_synthetic_weights(5, relu_targets=["relu3_1"]): module names, shapes, sums and the
+    first 64 values of every convolution's weight and bias."""
+    import importlib.util
+    import tempfile
+    from tests.t7_writer import write_vgg_t7
+    from wct_tf_b200 import weights as W
+    ref_dir = os.environ.get("WCT_TF_REFERENCE", "reference")          # a checkout of eridgd/WCT-TF
+    spec = importlib.util.spec_from_file_location("_ref_torchfile", os.path.join(ref_dir, "torchfile.py"))
+    tf = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(tf)
+    w = W.make_synthetic_weights(5, relu_targets=["relu3_1"])
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "vgg_normalised.t7")
+        write_vgg_t7(path, w["vgg"])
+        net = tf.load(path, force_8bytes_long=True)
+    convs = [m for m in net.modules if m._typename == b"nn.SpatialConvolution"]
+    out = {"names": np.array([m.name.decode() if m.name is not None else "" for m in convs])}
+    for i, m in enumerate(convs):
+        wt, b = np.asarray(m.weight), np.asarray(m.bias)
+        out["w%d_shape" % i], out["w%d_sum" % i], out["w%d_head" % i] = np.array(wt.shape), np.float64(wt.astype(np.float64).sum()), wt.reshape(-1)[:64]
+        out["b%d_sum" % i], out["b%d_head" % i] = np.float64(b.astype(np.float64).sum()), b.reshape(-1)[:64]
+    np.savez_compressed(os.path.join(HERE, "t7_reference_parse.npz"), **out)
+    print("t7 golden", len(convs), "convolutions")
+
+
 if __name__ == "__main__":
-    main()
-    coral_golden()
+    # python tests/golden/make_golden.py [case names...]: regenerate only those wct_np cases
+    main(sys.argv[1:])
+    if len(sys.argv) == 1:
+        coral_golden()
+        t7_golden()

@@ -1,7 +1,7 @@
 """GPU experiment (TEST INFRASTRUCTURE, run by hand under gpurun): which part of the encoder's excess over fp32 noise
 is the SPF16 storage and which is the tensor-core path?  Runs the shared encoder to relu5_1 / relu4_1 three ways and
 compares each with the fp64 oracle on the same image:
-  tc     the product path (tcgen05 split-fp16 x3, chunked TMEM accumulation)
+  tc     the product path (wgmma split-fp16 x3, chunked register accumulation)
   ref    wctb200_conv3x3_ref: plain fp32 FFMA on CUDA cores, same SPF16 storage between layers
   cpu32  the oracle in fp32 (torch-CPU), the reference's arithmetic
 Usage: python tests/noise_split_gpu.py [size]"""

@@ -158,7 +158,7 @@ def test_split_style_prepare_and_apply_equals_combined_level():
 @pytest.mark.parametrize("shape", [(1, 8, 32, 64), (2, 9, 40, 64), (1, 16, 33, 128), (1, 12, 20, 256), (2, 8, 8, 512),
                                    (1, 70, 130, 64), (1, 3, 2, 128)])
 def test_covariance_kernels(shape):
-    """Stage A of the transform (ops.py:43-45,105-108): per-channel mean and fc fc^T/(HW-1) on tcgen05
+    """Stage A of the transform (ops.py:43-45,105-108): per-channel mean and fc fc^T/(HW-1) on wgmma
     (MN-major operands, centred in shared memory)."""
     rng = np.random.default_rng(3)
     n, h, w, c = shape

@@ -178,19 +178,15 @@ def test_t7_reader_against_reference_torchfile(tmp_path):
     for a, b in zip(ours, w["vgg"]):
         assert np.array_equal(a["weight"], b["weight"]) and np.array_equal(a["bias"], b["bias"])
     assert [l["name"] for l in t7.load_vgg_t7(path, deepest="relu2_1")][-1] == "conv2_1"    # stops at the target (vgg_normalised.py:48)
-    ref_path = "/root/reference/torchfile.py"
-    if os.path.exists(ref_path):
-        import importlib.util
-        spec = importlib.util.spec_from_file_location("_ref_torchfile", ref_path)
-        tf = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(tf)
-        net = tf.load(path, force_8bytes_long=True)
-        convs = [m for m in net.modules if m._typename == b"nn.SpatialConvolution"]
-        assert len(convs) == len(ours)
-        for m, o in zip(convs, ours):
-            assert np.array_equal(np.asarray(m.weight), o["weight"]) and np.array_equal(np.asarray(m.bias), o["bias"])
-        names = [m.name.decode() for m in net.modules[1:] if m._typename == b"nn.SpatialConvolution"]
-        assert names == [l["name"] for l in ours[1:]]
+    # what the reference's torchfile.py read back from this same file (tests/golden/make_golden.py:t7_golden)
+    ref = np.load(os.path.join(os.path.dirname(__file__), "golden", "t7_reference_parse.npz"))
+    assert len(ref["names"]) == len(ours)
+    for i, o in enumerate(ours):
+        assert tuple(ref["w%d_shape" % i]) == o["weight"].shape
+        assert np.array_equal(ref["w%d_head" % i], o["weight"].reshape(-1)[:64])
+        assert np.array_equal(ref["b%d_head" % i], o["bias"].reshape(-1)[:64])
+        assert ref["w%d_sum" % i] == o["weight"].astype(np.float64).sum() and ref["b%d_sum" % i] == o["bias"].astype(np.float64).sum()
+    assert [str(n) for n in ref["names"][1:]] == [l["name"] for l in ours[1:]]
     # and through the public loader: checkpoints stay .npz
     ck = str(tmp_path / "dec.npz")
     W.save_weights(ck, w)

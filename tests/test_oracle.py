@@ -1,6 +1,6 @@
 """CPU tests: pin the oracle restatement against the reference's own outputs
-(committed golden vectors made by tests/golden/make_golden.py from
-/root/reference/ops.py:92-140) and check its internal consistency."""
+(committed golden vectors made by tests/golden/make_golden.py from the
+reference's ops.py:92-140) and check its internal consistency."""
 import glob
 import os
 
@@ -27,15 +27,6 @@ def test_wct_np_restatement_matches_reference_golden(path):
     out64 = ref_ops.wct_np(g["content"].astype(np.float64), g["style"].astype(np.float64), float(g["alpha"]))
     assert np.abs(out64 - g["out_ref_fp64"]).max() <= 1e-6
     assert ref_ops.spectral_gap_ok(g["wc"]) and ref_ops.spectral_gap_ok(g["ws"])
-
-
-def test_live_reference_import_if_present():
-    ref = ref_ops.load_reference_ops()
-    if ref is None:
-        pytest.skip("/root/reference not present (GPU box)")
-    g = np.load(GOLDEN[0])
-    out = ref.wct_np(g["content"], g["style"], float(g["alpha"]))
-    assert np.array_equal(out, g["out_ref_fp32"])
 
 
 def test_np_vs_tf_semantics_differ_only_as_documented():
@@ -94,7 +85,17 @@ PIPE_GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden",
 def load_pipeline_fixture(path):
     from tests.golden.make_pipeline_golden import weight_checksum
     from wct_tf_b200.weights import make_synthetic_weights
-    g = np.load(path)
+    g = dict(np.load(path))
+    # a large fixture stores every 8th element of some arrays (files stay under 1 MB): NaN elsewhere, compared with nanmax;
+    # the reference's full-resolution fp32-vs-fp64 noise is then stored as out_ref_noise
+    for key in [k for k in g if k.endswith("_every8")]:
+        name = key[:-len("_every8")]
+        shape = tuple(int(v) for v in g.pop(name + "_shape"))
+        full = np.full(int(np.prod(shape)), np.nan)
+        full[::8] = g.pop(key)
+        g[name] = full.reshape(shape)
+    if "out_ref_noise" not in g:
+        g["out_ref_noise"] = np.abs(g["out_ref_fp32"] - g["out_ref_fp64"]).max()
     targets = [str(t) for t in g["relu_targets"]]
     w = make_synthetic_weights(int(g["seed"]), relu_targets=targets)
     assert abs(weight_checksum(w) - float(g["wsum"])) <= 1e-9 * float(g["wsum"]), "synthetic weight generator drifted"
@@ -104,7 +105,7 @@ def load_pipeline_fixture(path):
 def swap_kwargs(g):
     """--swap5 arguments of a fixture (older fixtures carry no patch / stride: the reference's defaults 3 / 1)."""
     kw = dict(swap5=bool(g["swap5"]), ss_alpha=float(g["ss_alpha"]))
-    if "ss_patch_size" in g.files:
+    if "ss_patch_size" in g:
         kw.update(ss_patch_size=int(g["ss_patch_size"]), ss_stride=int(g["ss_stride"]))
     return kw
 
@@ -126,26 +127,8 @@ def test_oracle_pipeline_matches_reference_code_fixture(path):
     if not adain:
         assert [(i["k_c"], i["k_s"]) for i in info] == [tuple(r) for r in g["k"].tolist()]
     o32 = nets.pipeline(g["content"], g["style"], w, targets, alpha=alpha, adain=adain, semantics="tf", dtype=np.float32, **swap)
-    noise = np.abs(g["out_ref_fp32"] - g["out_ref_fp64"]).max()     # the reference code's own fp32 rounding (chained levels amplify it)
-    assert np.abs(o32 - g["out_ref_fp32"]).max() <= max(1e-4, 4 * noise)
-
-
-def test_reference_code_live_reproduces_fixture_if_present(tmp_path):
-    if not os.path.exists("/root/reference/model.py"):
-        pytest.skip("reference tree not mounted")
-    from tests.golden import np_tf1
-    from tests.t7_writer import write_vgg_t7
-    path = [p for p in PIPE_GOLDEN if "wct_31_11_odd" in p][0]
-    g, targets, w = load_pipeline_fixture(path)
-    t7 = str(tmp_path / "vgg.t7")
-    write_vgg_t7(t7, w["vgg"])
-    dec = {l["name"]: (l["kernel"], l["bias"]) for t in targets for l in w["decoders"][t]}
-    with np_tf1.reference_modules() as ref:
-        out, levels = np_tf1.run_reference(ref, g["content"][None] / 255.0, g["style"][None] / 255.0, t7, dec, targets,
-                                           float(g["alpha"]), bool(g["adain"]), np.float64, swap5=bool(g["swap5"]),
-                                           ss_alpha=float(g["ss_alpha"]))
-    assert np.abs(out - g["out_ref_fp64"]).max() <= 1e-12
-    assert "tensorflow" not in __import__("sys").modules or not hasattr(__import__("sys").modules["tensorflow"], "placeholder_with_default")
+    noise = g["out_ref_noise"]     # the reference code's own fp32 rounding (chained levels amplify it)
+    assert np.nanmax(np.abs(o32 - g["out_ref_fp32"])) <= max(1e-4, 4 * noise)
 
 
 # ---------------------------------------------------------------------------

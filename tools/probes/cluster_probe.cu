@@ -1,5 +1,5 @@
 // How many clusters of size S (512 threads, 128 KB smem per CTA: the k_jacobi<512> footprint) are co-resident
-// on this GPU, and where do they land?   nvcc -gencode arch=compute_100a,code=sm_100a -o cluster_probe cluster_probe.cu
+// on this GPU, and where do they land?   nvcc -gencode arch=compute_90a,code=sm_90a -o cluster_probe cluster_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <cooperative_groups.h>

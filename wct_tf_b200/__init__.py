@@ -1,4 +1,4 @@
-"""wct_tf_b200 -- B200-native multi-level WCT stylisation engine (inference hot path of eridgd/WCT-TF)."""
+"""wct_tf_b200 -- H100-native (sm_90a) multi-level WCT stylisation engine (inference hot path of eridgd/WCT-TF)."""
 __version__ = "0.1.0"
 
 from .model import WCTModel, RELU_TARGETS_ALL  # noqa: F401

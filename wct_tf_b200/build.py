@@ -1,4 +1,4 @@
-"""Build libwctb200.so in-tree with nvcc for sm_100a (no GPU needed: cross-compiles)."""
+"""Build libwctb200.so in-tree with nvcc for sm_90a (H100; no GPU needed: cross-compiles)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libwctb200.so")
 SOURCES = ["capi.cu", "layers.cu", "conv_tc.cu", "cov_tc.cu", "wct.cu", "image_ops.cu", "conv_tail_tc.cu", "conv_head_tc.cu", "matfun_tc.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 NVCC_FLAGS += os.environ.get("WCTB_NVCC_EXTRA", "").split()      # experiments, e.g. -DWCTB_MBAR_TEST_WAIT
 
@@ -49,7 +49,7 @@ def build(force=False, verbose=False):
         if verbose and out:
             print(out.decode())
     if relink:
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC"]
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC"]
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s" % r.stdout.decode())

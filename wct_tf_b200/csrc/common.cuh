@@ -1,4 +1,4 @@
-// Shared device/host helpers for libwctb200 (sm_100a only).
+// Shared device/host helpers for libwctb200 (sm_90a only).
 #pragma once
 
 #include <cuda.h>
@@ -93,7 +93,7 @@ struct alignas(16) Half8 { __half2 v[4]; };
 
 // two fp32 -> (hi pair, lo pair).  cvt.rn.satfinite.f16x2.f32 (F2FP.SATFINITE.F16.F32.PACK_AB) converts, saturates to
 // +-65504 and packs two values in ONE instruction: 6 instructions per pair instead of the 11 of two clamped scalar splits
-// (the conv epilogue is instruction bound on every short-K layer, profiles/r02_ncu_conv_epilogue.txt)
+// (the conv epilogue is instruction bound on the short-K layers)
 __device__ __forceinline__ void split2(float a, float b, __half2& hi, __half2& lo) {
     unsigned int h, l;
     asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(b), "f"(a));       // a -> low half, b -> high half
@@ -245,23 +245,16 @@ __device__ __forceinline__ void store_tile_rows(const float (&acc)[NACC], const 
 }
 
 // ---------------------------------------------------------------------------
-// packed fp32 pairs: fma.rn.f32x2 does two FMAs per instruction on sm_100 (same FMA-pipe time, half the issue slots)
+// fp32 pairs: sm_90 has no packed fp32 FMA, so a pair is two scalar fmaf (round-to-nearest, same result per element)
 // ---------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack2(float a, float b) {
-    f32x2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pack2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+struct alignas(16) f32x2x2 { f32x2 x, y; };       // a float4 viewed as two pairs
 
 // ---------------------------------------------------------------------------
-// PTX wrappers: mbarrier / TMA / tcgen05 (sm_100a)
+// PTX wrappers: mbarrier / TMA / wgmma (sm_90a)
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -326,92 +319,102 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* map, uin
         : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---- warpgroup MMA (sm_90a): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 inputs, fp32 accumulators in registers.
+// Issued by all 128 threads of a warpgroup (4 consecutive warps starting at a multiple of 4).  Accumulator fragment of
+// thread t of the warpgroup: rows 16*(t/32) + (t%32)/4 (+8), columns 8j + 2*(t%4) (+1), d[4j..4j+3] =
+// (r, c), (r, c+1), (r+8, c), (r+8, c+1)  (PTX ISA, "wgmma .m64nNk16 register fragment D").
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// register budget of a warpgroup (producer warpgroups give theirs to the MMA warpgroups)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA window
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16 inputs, fp32 accumulate), issued by ONE thread
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread retire
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128B-swizzled shared-memory operand descriptor (tile rows are 128 bytes =
-// 64 fp16 of K; 8-row groups 1024 B apart).  Bit layout: cute::UMMA::SmemDescriptor.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// K-major, 128B-swizzled shared-memory operand descriptor (tile rows are 128 bytes = 64 fp16 of K; 8-row groups
+// 1024 B apart; the tile base is 1024-byte aligned).  Bit layout: sm_90 GMMA descriptor (start >> 4 at [0,14),
+// LBO >> 4 at [16,30), SBO >> 4 at [32,46), layout type at [62,64): 1 = SWIZZLE_128B).  A 16-wide k-step inside the
+// 128-byte row advances the start address by 32 bytes.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address  [0,14)
-    d |= (uint64_t)1 << 16;                       // LBO (unused for swizzled K-major) [16,30)
-    d |= (uint64_t)(1024 >> 4) << 32;             // SBO = 1024 B   [32,46)
-    d |= (uint64_t)1 << 46;                       // descriptor version = 1 (sm_100)
-    d |= (uint64_t)2 << 61;                       // layout type = SWIZZLE_128B
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;                       // LBO (unused for swizzled K-major)
+    d |= (uint64_t)(1024 >> 4) << 32;             // SBO = 1024 B
+    d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
     return d;
 }
-// kind::f16 instruction descriptor: fp16 x fp16 -> fp32, K-major A and B, M x N tile.
-// Bit layout: cute::UMMA::InstrDescriptor.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-    return (1u << 4)                      // c_format = F32
-           | (0u << 7) | (0u << 10)       // a_format = b_format = F16
-           | (0u << 15) | (0u << 16)      // a_major = b_major = K
-           | ((uint32_t)(N >> 3) << 17)   // n_dim
-           | ((uint32_t)(M >> 4) << 24);  // m_dim
-}
-// MN-major SWIZZLE_128B operand (used when the contraction index is the slow one: covariance X^T X, Gram G^T G):
-// 64 MN elements (128 B) per row, rows = K; LBO = stride between 64-wide MN groups (8 KB: the next slice / the lo plane),
-// SBO = stride between 8-row K groups (1 KB)  (cute::UMMA canonical layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte
-// units; strides probed on B200, profiles/r01_cov_mn_major_probe.txt)
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr) {
+// MN-major SWIZZLE_128B operand (used when the contraction index is the slow one: covariance X^T X, true products A B):
+// 64 MN elements (128 B) per row, rows = K; LBO = stride between 64-wide MN groups (8 KB: the next slice),
+// SBO = stride between 8-row K groups (1 KB)  (canonical layout ((64,n),(8,k)) : ((1,LBO),(64,SBO)) in elements)
+__device__ __forceinline__ uint64_t gmma_desc_mn_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)((8192 >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((1024 >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-__host__ __device__ constexpr uint32_t umma_idesc_f16_mn(int M, int N) {
-    return (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
+
+// TA / TB: 0 = K-major operand, 1 = MN-major (transposed) operand
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+
+// accumulator fragments of a 64-row warpgroup slice -> row-major fp32 tile in shared memory (tile[row * pitch + col])
+template <int R>
+__device__ __forceinline__ void frag_to_tile(const float (&d)[R], float* tile, int pitch, int row0, int t) {
+    const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+    const int c = 2 * (t & 3);
+#pragma unroll
+    for (int j = 0; j < R / 4; ++j) {
+        *reinterpret_cast<float2*>(tile + r * pitch + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(tile + (r + 8) * pitch + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
 }
 #endif  // __CUDACC__
 

@@ -7,12 +7,12 @@
 // 128-byte K-major row  [hi k=0..31 | lo k=0..31]  in the 128B-swizzled layout the MMA expects.  With
 //     B rows  0..63  = [w_hi | w_hi]        ->  D[:,  0:64 ) = x_hi w_hi + x_lo w_hi
 //     B rows 64..127 = [w_lo |  0  ]        ->  D[:, 64:128) = x_hi w_lo
-// one tcgen05.mma (M = 128, N = 128) per 16-wide k-step -- 4 per 128-pixel tile -- computes all three split products.
-//   warp 0    : MMA issuer, owns the TMEM allocation (2 buffers x 128 columns)
-//   warps 1-4 : producers (global -> split fp16 -> swizzled smem, fence.proxy.async, mbarrier)
-//   warps 5-8 : epilogue (tcgen05.ld, undo the scales, bias, ReLU, split, coalesced stores incl. the halo cells)
-// Two CTAs per SM.  The SIMT kernel (layers.cu k_conv_head) spent 1728 FMAs per pixel and ran at 31 TFLOP/s; this one is
-// bound by its 258 B/pixel of output.
+// one wgmma (M = 64, N = 128) per 16-wide k-step and 64-pixel half -- 8 per 128-pixel tile -- computes all three split products.
+//   warps 0-3 : producers (global -> split fp16 -> swizzled smem, fence.proxy.async, mbarrier)
+//   warps 4-7 : one warpgroup: wgmma, the two column halves summed into an fp32 tile in shared memory, then the epilogue
+//               (undo the scales, bias, ReLU, split, coalesced stores incl. the halo cells)
+// Two CTAs per SM.  The SIMT kernel (layers.cu k_conv_head) spends 1728 FMAs per pixel; this one is bound by its
+// 258 B/pixel of output.
 #include "common.cuh"
 
 namespace wctb {
@@ -21,11 +21,13 @@ struct HeadCfg {
     static constexpr int A_BYTES = 128 * 128;              // one tile: 128 pixels x 128 B
     static constexpr int STAGES = 2;
     static constexpr int B_BYTES = 128 * 128;              // 128 rows (n) x 64 fp16 (k)
-    static constexpr int STG_BYTES = 4 * 8192;
+    static constexpr int PITCH = 68;                       // fp32 tile [128 pixels][64 channels] (+4: conflict-free row reads)
+    static constexpr int TILE_BYTES = 128 * PITCH * 4;
+    static constexpr int STG_BYTES = 4 * 8192;             // per-epilogue-warp store staging, aliased with the fp32 tile
+    static constexpr int EPI_BYTES = TILE_BYTES > STG_BYTES ? TILE_BYTES : STG_BYTES;
     static constexpr int AUX_BYTES = 512;                  // barriers + bias[64]
-    static constexpr int SMEM_BYTES = STAGES * A_BYTES + B_BYTES + STG_BYTES + AUX_BYTES + 1024;
-    static constexpr int THREADS = 288;
-    static constexpr int TMEM_COLS = 256;
+    static constexpr int SMEM_BYTES = STAGES * A_BYTES + B_BYTES + EPI_BYTES + AUX_BYTES + 1024;
+    static constexpr int THREADS = 256;
 };
 
 struct HeadParams {
@@ -47,15 +49,13 @@ conv_head_tc_kernel(const HeadParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* bsm = smem + Cfg::STAGES * Cfg::A_BYTES;
-    uint8_t* stg = bsm + Cfg::B_BYTES;
-    uint8_t* aux = stg + Cfg::STG_BYTES;
+    uint8_t* epi = bsm + Cfg::B_BYTES;
+    float* ctile = reinterpret_cast<float*>(epi);
+    uint8_t* aux = epi + Cfg::EPI_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tfull = empty + Cfg::STAGES;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_slot + 1);
-    float* s_oscale = reinterpret_cast<float*>(tmem_slot + 2);
+    volatile int* abort_flag = reinterpret_cast<volatile int*>(empty + Cfg::STAGES);
+    float* s_oscale = reinterpret_cast<float*>(empty + Cfg::STAGES) + 1;
     float* sbias = reinterpret_cast<float*>(aux + 256);
 
     const int warp = threadIdx.x >> 5;
@@ -69,16 +69,11 @@ conv_head_tc_kernel(const HeadParams p) {
     if (threadIdx.x == 0) {
         for (int s = 0; s < Cfg::STAGES; ++s) {
             mbar_init(&full[s], 4);          // one arrival per producer warp
-            mbar_init(&empty[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&tfull[b], 1);
-            mbar_init(&tempty[b], 4);
+            mbar_init(&empty[s], 4);         // one arrival per consumer warp
         }
         *abort_flag = 0;
         fence_barrier_init();
     }
-    if (warp == 0) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
 
     // ---- B operand (all threads): power-of-two weight scale, split, swizzled K-major rows ----
     float m = 0.f;
@@ -119,37 +114,12 @@ conv_head_tc_kernel(const HeadParams p) {
         *reinterpret_cast<Half8*>(bsm + row * 128 + ((c ^ (row & 7)) * 16)) = v;
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const unsigned int HW = (unsigned int)p.H * (unsigned int)p.W;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16(128, 128);
-            const uint64_t b_desc = umma_desc_sw128(smem_u32(bsm));
-            uint32_t tg = 0;
-            for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++tg) {
-                const int s = tg % Cfg::STAGES, b = tg & 1;
-                mbar_wait(&tempty[b], ((tg >> 1) & 1) ^ 1u, abort_flag, p.err, 0x420u + b);
-                mbar_wait(&full[s], (tg / Cfg::STAGES) & 1, abort_flag, p.err, 0x230u + s);
-                tc_fence_after();
-                const uint64_t a_desc = umma_desc_sw128(smem_u32(smem + s * Cfg::A_BYTES));
-                const uint32_t tacc = tmem_base + (uint32_t)(b * 128);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t ko = (uint64_t)(k * 32 >> 4);
-                    umma_f16(tacc, a_desc + ko, b_desc + ko, idesc, k == 0 ? 0u : 1u);
-                }
-                umma_commit(&empty[s]);
-                umma_commit(&tfull[b]);
-            }
-        }
-        __syncwarp();
-    } else if (warp <= 4) {
+    if (warp < 4) {
         // ---- producers: one pixel per thread ----
-        const int i = (warp - 1) * 32 + lane;              // row of the A tile
+        const int i = warp * 32 + lane;                    // row of the A tile
         uint32_t tg = 0;
         for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++tg) {
             const int s = tg % Cfg::STAGES;
@@ -190,48 +160,72 @@ conv_head_tc_kernel(const HeadParams p) {
             __syncwarp();
             if (lane == 0) mbar_arrive(&full[s]);
         }
-    } else {
-        // ---- epilogue ----
-        const int g = warp & 3;                            // TMEM lane quadrant (warps 5,6,7,8 -> 1,2,3,0)
-        const ActGeom go(p.N, p.H, p.W, 64);
-        const float osc = *s_oscale;
-        uint8_t* wstg = stg + (warp - 5) * 8192;
-        uint32_t tg = 0;
-        for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++tg) {
-            const int b = tg & 1;
-            mbar_wait(&tfull[b], (tg >> 1) & 1, abort_flag, p.err, 0x320u + b);
-            tc_fence_after();
-            const uint32_t tsrc = tmem_base + ((uint32_t)(g * 32) << 16) + (uint32_t)(b * 128);
-            float acc[64];
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 16) {           // 16-column loads: 2 CTAs/SM leave ~110 registers per thread
-                uint32_t r0[16], r1[16];
-                tmem_ld16(tsrc + c0, r0);
-                tmem_ld16(tsrc + 64 + c0, r1);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 16; ++j) acc[c0 + j] = __uint_as_float(r0[j]) + __uint_as_float(r1[j]);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[b]);
-            const long long q = (long long)tile * 128 + g * 32 + lane;
-            int flags = -1;
-            unsigned int ppos = 0;
-            if (q < p.total_px && !*abort_flag) {
-                const unsigned int n = (unsigned int)(q / HW);
-                const unsigned int r = (unsigned int)(q - (long long)n * HW);
-                const int y = (int)(r / (unsigned int)p.W);
-                const int x = (int)(r - (unsigned int)y * (unsigned int)p.W);
-                flags = halo_flags(go, y, x);
-                ppos = (n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
-            }
-            store_tile_rows<64>(acc, osc, sbias, true, wstg, lane, ppos, flags, p.out, go, 0);
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+
+    // ---- consumer warpgroup (warps 4-7): wgmma per 64-row half, D[:, 0:64) + D[:, 64:128) -> fp32 tile -> epilogue ----
+    const int t = threadIdx.x - 128;
+    const int fr = 16 * (t >> 5) + ((t & 31) >> 2), fc = 2 * (t & 3);
+    const ActGeom go(p.N, p.H, p.W, 64);
+    const float osc = *s_oscale;
+    uint8_t* wstg = epi + (warp - 4) * 8192;
+    const uint64_t b_desc = gmma_desc_sw128(smem_u32(bsm));
+    uint32_t tg = 0;
+    for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++tg) {
+        const int s = tg % Cfg::STAGES;
+        mbar_wait(&full[s], (tg / Cfg::STAGES) & 1, abort_flag, p.err, 0x230u + s);
+        asm volatile("bar.sync 1, 128;" ::: "memory");             // previous tile's staging buffers are free
+#pragma unroll 1
+        for (int h = 0; h < 2; ++h) {
+            float d[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) d[i] = 0.f;
+            const uint64_t a_desc = gmma_desc_sw128(smem_u32(smem + s * Cfg::A_BYTES + h * 8192));
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t ko = (uint64_t)(k * 32 >> 4);
+                wgmma_m64n128k16<0, 0>(d, a_desc + ko, b_desc + ko, k == 0 ? 0u : 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_fence(d);
+            // columns [0,64) = x_hi w_hi + x_lo w_hi, [64,128) = x_hi w_lo of the same channels
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int r = 64 * h + fr;
+                *reinterpret_cast<float2*>(ctile + r * Cfg::PITCH + 8 * j + fc) =
+                    make_float2(d[4 * j] + d[4 * (j + 8)], d[4 * j + 1] + d[4 * (j + 8) + 1]);
+                *reinterpret_cast<float2*>(ctile + (r + 8) * Cfg::PITCH + 8 * j + fc) =
+                    make_float2(d[4 * j + 2] + d[4 * (j + 8) + 2], d[4 * j + 3] + d[4 * (j + 8) + 3]);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+        asm volatile("bar.sync 1, 128;" ::: "memory");             // fp32 tile complete
+        float acc[64];
+        {
+            const float4* src4 = reinterpret_cast<const float4*>(ctile + t * Cfg::PITCH);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const float4 v = src4[j];
+                acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
+            }
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");             // tile read: the staging buffers may be written
+        const long long q = (long long)tile * 128 + t;
+        int flags = -1;
+        unsigned int ppos = 0;
+        if (q < p.total_px && !*abort_flag) {
+            const unsigned int n = (unsigned int)(q / HW);
+            const unsigned int r = (unsigned int)(q - (long long)n * HW);
+            const int y = (int)(r / (unsigned int)p.W);
+            const int x = (int)(r - (unsigned int)y * (unsigned int)p.W);
+            flags = halo_flags(go, y, x);
+            ppos = (n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
+        }
+        store_tile_rows<64>(acc, osc, sbias, true, wstg, lane, ppos, flags, p.out, go, 0);
+    }
 }
 
 int g_conv_head_tc = 1;          // 0: the SIMT kernel of layers.cu (wctb200_debug_set_conv_head_tc)

@@ -11,12 +11,13 @@
 // Tiling.  A CTA owns a vertical strip of <= 126 output columns (a row tile is 128 consecutive padded positions: the strip
 // plus one neighbour column on either side) and walks DOWN a chunk of 32 output rows; the P rows live in a 3-row ring in
 // shared memory, so no partial product is computed twice vertically (2 extra rows per 32) and 2 of 128 columns horizontally.
-//   warp 0   : TMA producer (one 128 x 64 fp16 box per plane per row, 128B swizzle)
-//   warp 1   : MMA issuer: a_hi * [b_hi | b_lo] (N = 64) then a_lo * b_hi (N = 32) into a 64-column TMEM buffer (2 buffers)
-//   warps 2-5: tcgen05.ld -> P ring (fp32) -> gather / scale / bias / clip -> coalesced fp32 stores
-// Two CTAs per SM (100 KB of shared memory, 128 TMEM columns each): the gather of one overlaps the MMAs of the other.
-// Precision: split-fp16 x3 like the big convs (weights scaled by a power of two so their lo plane stays out of the fp16
-// subnormals); the K = 64 partial sums are accumulated in TMEM, the 9-term gather in fp32 registers.
+//   warp 4   : TMA producer (one 128 x 64 fp16 box per plane per row, 128B swizzle)
+//   warps 0-3: one warpgroup: wgmma (a_hi + a_lo) * [b_hi | b_lo] (N = 64, two m64 halves) into registers -> P ring (fp32)
+//              -> gather / scale / bias / clip -> fp32 stores
+// Two CTAs per SM (100 KB of shared memory each): the gather of one overlaps the MMAs of the other.
+// Precision: split-fp16 products like the big convs (weights scaled by a power of two so their lo plane stays out of the fp16
+// subnormals; the a_lo b_lo term rides along); the K = 64 partial sums are accumulated by the tensor core, the 9-term
+// gather in fp32 registers.
 #include "common.cuh"
 
 namespace wctb {
@@ -34,8 +35,7 @@ struct TailCfg {
     static constexpr int AUX_BYTES = 256;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + B_BYTES + RING_BYTES + AUX_BYTES + 1024;
     static constexpr int ROWS = 32;                        // output rows per work item
-    static constexpr int THREADS = 192;
-    static constexpr int TMEM_COLS = 128;                  // 2 buffers x 64 columns
+    static constexpr int THREADS = 160;
 };
 
 struct TailParams {
@@ -92,11 +92,8 @@ conv_tail_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     uint8_t* aux = reinterpret_cast<uint8_t*>(ring) + Cfg::RING_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tfull = empty + Cfg::STAGES;
-    uint64_t* tempty = tfull + 2;
-    uint64_t* bfull = tempty + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bfull + 1);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_slot + 1);
+    uint64_t* bfull = empty + Cfg::STAGES;
+    volatile int* abort_flag = reinterpret_cast<volatile int*>(bfull + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -109,11 +106,7 @@ conv_tail_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     if (threadIdx.x == 0) {
         for (int s = 0; s < Cfg::STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&tfull[b], 1);
-            mbar_init(&tempty[b], 4);
+            mbar_init(&empty[s], 4);         // one arrival per consumer warp
         }
         mbar_init(bfull, 1);
         *abort_flag = 0;
@@ -121,11 +114,7 @@ conv_tail_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
         tma_prefetch_desc(&mapA);
         tma_prefetch_desc(&mapB);
     }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const long long HpWp = (long long)p.Hp * p.Wp;
 
     // work item -> (image n, strip s, row chunk): chunk fastest so CTAs running together read neighbouring rows
@@ -139,7 +128,7 @@ conv_tail_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
         return min(Cfg::ROWS, p.H - py0) + 2;             // P rows: padded rows py0 .. py0 + nrows - 1
     };
 
-    if (warp == 0) {
+    if (warp == 4) {
         if (lane == 0) {
             mbar_arrive_expect_tx(bfull, Cfg::B_BYTES);
             tma_load_3d(bsm, &mapB, bfull, 0, 0, 0);
@@ -160,105 +149,101 @@ conv_tail_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
                 }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc64 = umma_idesc_f16(128, 64);
-            constexpr uint32_t idesc32 = umma_idesc_f16(128, 32);
-            mbar_wait(bfull, 0u, abort_flag, p.err, 0x210u);
-            tc_fence_after();
-            const uint64_t b_desc = umma_desc_sw128(smem_u32(bsm));       // 64 rows: b_hi then b_lo; the first 32 alone = b_hi
-            uint32_t sg = 0, rg = 0;
-            for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
-                int n, px0, py0;
-                const int nrows = item_rows(item, n, px0, py0);
-                for (int r = 0; r < nrows; ++r, ++rg) {
-                    const int b = rg & 1;
-                    mbar_wait(&tempty[b], ((rg >> 1) & 1) ^ 1u, abort_flag, p.err, 0x410u + b);
-                    tc_fence_after();
-                    const uint32_t tacc = tmem_base + (uint32_t)(b * 64);
+        return;
+    }
+
+    // ---- consumer warpgroup (warps 0-3): wgmma, P rows into the ring, gather ----
+    const int t = threadIdx.x;                             // 0..127
+    const int pos = t;                                     // position inside the row tile (gather)
+    const float isc = __ldg(p.inv_scale);
+    const float b0 = __ldg(p.bias), b1 = __ldg(p.bias + 1), b2 = __ldg(p.bias + 2);
+    const bool clip = (p.flags & WCTB200_CLIP01) != 0;
+    // fragment coordinates: rows fr, fr + 8 (+64 for the second half), columns 8j + fc (+1)
+    const int fr = 16 * (t >> 5) + ((t & 31) >> 2);
+    const int fc = 2 * (t & 3);
+    mbar_wait(bfull, 0u, abort_flag, p.err, 0x210u);
+    const uint64_t b_desc = gmma_desc_sw128(smem_u32(bsm));       // 64 rows: b_hi then b_lo
+    uint32_t sg = 0;
+    for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
+        int n, px0, py0;
+        const int nrows = item_rows(item, n, px0, py0);
+        const int x = px0 + pos - 1;                       // output column of this thread (interior coordinates)
+        const bool col_ok = pos >= 1 && pos <= p.ow && x < p.W;
+        for (int r = 0; r < nrows; ++r) {
+            // (a_hi + a_lo) x [b_hi | b_lo]: columns [0,32) = a b_hi, [32,64) = a b_lo (this includes the a_lo b_lo term)
+            float acc[2][32];
 #pragma unroll
-                    for (int plane = 0; plane < 2; ++plane, ++sg) {
-                        const int s = sg % Cfg::STAGES;
-                        mbar_wait(&full[s], (sg / Cfg::STAGES) & 1, abort_flag, p.err, 0x220u + s);
-                        tc_fence_after();
-                        const uint64_t a_desc = umma_desc_sw128(smem_u32(smem + s * Cfg::STAGE_BYTES));
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t ko = (uint64_t)(k * 32 >> 4);
-                            if (plane == 0) umma_f16(tacc, a_desc + ko, b_desc + ko, idesc64, k == 0 ? 0u : 1u);
-                            else umma_f16(tacc, a_desc + ko, b_desc + ko, idesc32, 1u);
-                        }
-                        umma_commit(&empty[s]);
-                    }
-                    umma_commit(&tfull[b]);
+                for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+            const int s0 = sg % Cfg::STAGES, s1 = (sg + 1) % Cfg::STAGES;
+            mbar_wait(&full[s0], (sg / Cfg::STAGES) & 1, abort_flag, p.err, 0x220u + s0);
+            mbar_wait(&full[s1], ((sg + 1) / Cfg::STAGES) & 1, abort_flag, p.err, 0x220u + s1);
+            const uint32_t a_hi = smem_u32(smem + s0 * Cfg::STAGE_BYTES);
+            const uint32_t a_lo = smem_u32(smem + s1 * Cfg::STAGE_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint64_t ko = (uint64_t)(k * 32 >> 4);
+                    wgmma_m64n64k16<0, 0>(acc[h], gmma_desc_sw128(a_hi + h * 8192) + ko, b_desc + ko, k == 0 ? 0u : 1u);
+                    wgmma_m64n64k16<0, 0>(acc[h], gmma_desc_sw128(a_lo + h * 8192) + ko, b_desc + ko, 1u);
                 }
             }
-        }
-        __syncwarp();
-    } else {
-        const int g = warp & 3;                                // TMEM lane quadrant of this warp
-        const int pos = g * 32 + lane;                         // position inside the row tile
-        const float isc = __ldg(p.inv_scale);
-        const float b0 = __ldg(p.bias), b1 = __ldg(p.bias + 1), b2 = __ldg(p.bias + 2);
-        const bool clip = (p.flags & WCTB200_CLIP01) != 0;
-        uint32_t rg = 0;
-        for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
-            int n, px0, py0;
-            const int nrows = item_rows(item, n, px0, py0);
-            const int x = px0 + pos - 1;                       // output column of this thread (interior coordinates)
-            const bool col_ok = pos >= 1 && pos <= p.ow && x < p.W;
-            for (int r = 0; r < nrows; ++r, ++rg) {
-                const int b = rg & 1;
-                mbar_wait(&tfull[b], (rg >> 1) & 1, abort_flag, p.err, 0x310u + b);
-                tc_fence_after();
-                const uint32_t tsrc = tmem_base + ((uint32_t)(g * 32) << 16) + (uint32_t)(b * 64);
-                uint32_t r0[32], r1[32];
-                tmem_ld32(tsrc, r0);                           // a_hi b_hi + a_lo b_hi
-                tmem_ld32(tsrc + 32, r1);                      // a_hi b_lo
-                tmem_ld_wait();
-                float* slot = ring + (r % 3) * Cfg::RING_ROW + pos;
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_fence(acc[0]);
+            acc_fence(acc[1]);
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(&empty[s0]);
+                mbar_arrive(&empty[s1]);
+            }
+            sg += 2;
+            float* slot = ring + (r % 3) * Cfg::RING_ROW;
 #pragma unroll
-                for (int j = 0; j < Cfg::NJ; ++j) slot[j * 128] = __uint_as_float(r0[j]) + __uint_as_float(r1[j]);
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[b]);
-                asm volatile("bar.sync 1, 128;" ::: "memory");           // P row r complete
-                if (r >= 2) {
-                    if (col_ok && !*abort_flag) {
-                        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                        for (int ky = 0; ky < 3; ++ky) {
-                            const float* row = ring + ((r - 2 + ky) % 3) * Cfg::RING_ROW + pos - 1;
+                for (int j = 0; j < 4; ++j)
 #pragma unroll
-                            for (int kx = 0; kx < 3; ++kx) {
-                                const float* q = row + ((ky * 3 + kx) * 3) * 128 + kx;
-                                a0 += q[0];
-                                a1 += q[128];
-                                a2 += q[256];
-                            }
-                        }
-                        a0 = fmaf(a0, isc, b0);
-                        a1 = fmaf(a1, isc, b1);
-                        a2 = fmaf(a2, isc, b2);
-                        if (clip) {
-                            a0 = fminf(fmaxf(a0, 0.f), 1.f);
-                            a1 = fminf(fmaxf(a1, 0.f), 1.f);
-                            a2 = fminf(fmaxf(a2, 0.f), 1.f);
-                        }
-                        float* d = p.img + (((long long)n * p.H + (py0 + r - 2)) * p.W + x) * 3;
-                        d[0] = a0;
-                        d[1] = a1;
-                        d[2] = a2;
+                    for (int q = 0; q < 4; ++q) {
+                        const int col = 8 * j + fc + (q & 1);                  // P column (tap*3 + co)
+                        const int prow = 64 * h + fr + 8 * (q >> 1);           // position
+                        if (col < Cfg::NJ) slot[col * 128 + prow] = acc[h][4 * j + q] + acc[h][4 * (j + 4) + q];
                     }
-                    asm volatile("bar.sync 1, 128;" ::: "memory");       // ring slot (r+1)%3 may be overwritten
+            asm volatile("bar.sync 1, 128;" ::: "memory");           // P row r complete
+            if (r >= 2) {
+                if (col_ok && !*abort_flag) {
+                    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+#pragma unroll
+                    for (int ky = 0; ky < 3; ++ky) {
+                        const float* row = ring + ((r - 2 + ky) % 3) * Cfg::RING_ROW + pos - 1;
+#pragma unroll
+                        for (int kx = 0; kx < 3; ++kx) {
+                            const float* q = row + ((ky * 3 + kx) * 3) * 128 + kx;
+                            a0 += q[0];
+                            a1 += q[128];
+                            a2 += q[256];
+                        }
+                    }
+                    a0 = fmaf(a0, isc, b0);
+                    a1 = fmaf(a1, isc, b1);
+                    a2 = fmaf(a2, isc, b2);
+                    if (clip) {
+                        a0 = fminf(fmaxf(a0, 0.f), 1.f);
+                        a1 = fminf(fmaxf(a1, 0.f), 1.f);
+                        a2 = fminf(fmaxf(a2, 0.f), 1.f);
+                    }
+                    float* d = p.img + (((long long)n * p.H + (py0 + r - 2)) * p.W + x) * 3;
+                    d[0] = a0;
+                    d[1] = a1;
+                    d[2] = a2;
                 }
+                asm volatile("bar.sync 1, 128;" ::: "memory");       // ring slot (r+1)%3 may be overwritten
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 int g_conv_tail_tc = 1;          // 0: always the SIMT kernels of layers.cu (wctb200_debug_set_conv_tail_tc)

@@ -1,5 +1,5 @@
 // Conv2DReflect 3x3, the 1x1 "apply" of the feature transform, and UpSampling2D+Conv2DReflect as ONE conv,
-// all as an implicit GEMM on the 5th-gen tensor cores.
+// all as an implicit GEMM on the tensor cores (Hopper wgmma, TMA-fed).
 //
 //   reference: Lambda(pad_reflect) -> Conv2D(valid) (+ReLU)   ops.py:12-19,
 //              vgg_normalised.py:28-40, model.py:291; the whitening/colouring
@@ -26,17 +26,16 @@
 // halo: its producer is launched with WCTB200_HALO_EDGE.
 //
 // Precision.  fp32-class accuracy from fp16 tensor-core inputs: x = x_hi + x_lo,
-//   x*w ~= x_hi*w_hi + x_hi*w_lo + x_lo*w_hi     (3 x tcgen05.mma kind::f16, fp32 accumulate in TMEM)
+//   x*w ~= x_hi*w_hi + x_hi*w_lo + x_lo*w_hi     (3 x wgmma f16 x f16, fp32 accumulate in registers)
 // the dropped lo*lo term is 2^-22 relative.  Weights are stored SCALED by a per-layer power of two
 // (max|w| -> [512,1024), undone exactly in the epilogue): He-initialised / trained conv weights are ~1e-2, so the
 // unscaled lo plane (~5e-6) fell into the fp16 subnormals and kept only ~16 bits of the weight -- measured as
-// 8x the reference's own fp32 noise on the free-running 5-level image (profiles/r02_noise_split.txt).
+// 8x the reference's own fp32 noise on the free-running 5-level image (tests/noise_split_cpu.py).
 //
-// Structure (persistent CTAs, 192 threads):
-//   warp 0   : TMA producer   (cp.async.bulk.tensor 3-D, 128B swizzle, mbarrier complete_tx)
-//   warp 1   : MMA issuer     (one elected thread, tcgen05.mma / tcgen05.commit), owns TMEM alloc
-//   warps 2-5: epilogue       (tcgen05.ld 32x32b -> *scale +bias, ReLU -> split fp16 -> 16-byte stores
-//                              of the interior pixel AND the halo cells that mirror it)
+// Structure (persistent CTAs, 384 threads):
+//   warp 8   : TMA producer   (cp.async.bulk.tensor 3-D, 128B swizzle, mbarrier complete_tx; warps 9-11 idle)
+//   warps 0-7: two wgmma warpgroups (64 tile rows each), then the epilogue (*scale +bias, ReLU -> split fp16 ->
+//              16-byte stores of the interior pixel AND the halo cells that mirror it)
 #include "common.cuh"
 
 namespace wctb {
@@ -63,19 +62,20 @@ struct ConvParams {
 };
 
 // ===========================================================================
-// v2: persistent CTAs + chunked accumulation drained into registers
-//
-//   * grid = #SMs, every CTA walks a static tile list (cout tile fastest, so CTAs running
-//     together share activation tiles in L2 and the whole weight tensor stays L2 resident);
-//   * the accumulator ring: TMEM holds NBUF buffers of BN fp32 columns.  The MMA warp
-//     accumulates CH k-iterations (CH*4*3 tcgen05.mma) into one buffer starting from zero,
-//     commits it, and moves on to the next buffer; the epilogue warps drain each finished
-//     buffer with tcgen05.ld and ADD IT INTO REGISTERS with round-to-nearest FADDs.
-//     The tensor core adds into its fp32 accumulator with truncation (measured: -1.2e-5
-//     relative bias at K=4608 when everything is accumulated in TMEM); short chunks summed
-//     in registers bring the conv back to fp32-class error, and the drain of chunk i
-//     overlaps the MMAs of chunk i+1 (also across tiles: the epilogue of tile t overlaps
-//     the main loop of tile t+1).
+// Persistent CTAs, warp-specialised (384 threads):
+//   warps 0-7: two consumer warpgroups.  Warpgroup w multiplies rows [64w, 64w + 64) of the 128-position tile with
+//              wgmma (m64 x N x k16, both operands K-major from the 128B-swizzled stages, fp32 accumulators in registers)
+//              and then both run the epilogue;
+//   warps 8-11: producer warpgroup; one thread issues the TMA loads.  setmaxnreg moves registers from it to the
+//              consumers (the register file is allocated in whole warpgroups: 288 threads would cap every thread at 168).
+//   * grid = #SMs x oversubscription, every CTA walks a static tile list (cout tile fastest, so CTAs running together
+//     share activation tiles in L2 and the whole weight tensor stays L2 resident);
+//   * chunked accumulation: CH k-iterations accumulate into register chunks that start from zero (one for a_hi b_hi, one
+//     for the two small cross products) and are then added into the running sum with round-to-nearest FADDs.  The tensor
+//     core adds into its fp32 accumulator with truncation; short chunks summed in registers keep the conv at fp32-class
+//     error for K up to 4608;
+//   * epilogue: the fp32 tile goes through shared memory (a wgmma fragment spreads one row over 4 lanes) so that each
+//     epilogue thread owns one output position and 64 consecutive channels: scale/bias/ReLU/(pool)/split/coalesced stores.
 // ===========================================================================
 template <int BN, bool FUSE_>
 struct Conv2Cfg {
@@ -84,24 +84,24 @@ struct Conv2Cfg {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-    static constexpr int STAGES = BN == 64 ? 4 : (BN == 128 ? 3 : 2);
-    // FUSE: the products a_hi*b_hi and a_hi*b_lo share the A operand, and the two weight planes sit back to back in a
-    // stage, so ONE tcgen05.mma with N = 2*BN computes both into adjacent accumulator column ranges (summed when the
-    // chunk is drained); a_lo*b_hi follows with N = BN into the first range.  8 instead of 12 MMAs per k-iteration and
-    // half the A-operand shared-memory reads per flop (timeline probe: ~80 cycles per MMA regardless of N <= 128).
-    static constexpr bool FUSE = FUSE_ && BN <= 128;
-    static constexpr int ACC_COLS = FUSE ? 2 * BN : BN;         // TMEM columns of one accumulation buffer
-    static constexpr int NBUF = 512 / ACC_COLS >= 4 ? 4 : 2;
-    static constexpr int TMEM_COLS = NBUF * ACC_COLS;           // 512 / 512 / 512
-    static constexpr int CH = 4;                                // k-iterations per accumulation chunk
-    // (8 epilogue warps -- two per TMEM lane quadrant, 32-channel staging, 64-byte stores -- were measured in round 2:
-    //  slower on every short-K layer, e.g. UP2 64->64 841 -> 1002 us; profiles/r02_conv_layer_bench.txt)
-    static constexpr int EPI_WARPS = BN == 256 ? 8 : 4;
-    static constexpr int THREADS = 64 + 32 * EPI_WARPS;
-    static constexpr int NACC = BN / (EPI_WARPS / 4);           // accumulators per epilogue thread (<= 128)
+    static constexpr int STAGES = BN == 64 ? 3 : 2;
+    // FUSE (BN = 64): the products a_hi*b_hi and a_hi*b_lo share the A operand and the two weight planes sit back to back
+    // in a stage, so ONE wgmma with N = 2*BN computes both into adjacent accumulator column ranges (summed when the chunk
+    // is added up); a_lo*b_hi follows with N = BN into the first range.  2 instead of 3 wgmma per k-step.
+    static constexpr bool FUSE = FUSE_ && BN == 64;
+    static constexpr int CHUNK_REGS = FUSE ? BN : BN / 2;       // per-thread fp32 registers of one accumulation chunk
+    static constexpr int SUM_REGS = BN / 2;                     // per-thread fp32 registers of the m64 x BN running sum
+    static constexpr int CH = 2;                                // k-iterations per accumulation chunk
+    static constexpr int CONSUMERS = 256;
+    static constexpr int THREADS = CONSUMERS + 128;
+    static constexpr int EPI_WARPS = BN / 16;                   // 64 channels per epilogue thread
+    static constexpr int NACC = 64;
+    static constexpr int PITCH = BN + 4;                        // fp32 tile row pitch (conflict-free float4 row reads)
+    static constexpr int TILE_BYTES = BM * PITCH * 4;
+    static constexpr int STG_BYTES = EPI_WARPS * 8192;          // per-epilogue-warp store staging (coalesced stores)
+    static constexpr int EPI_BYTES = TILE_BYTES > STG_BYTES ? TILE_BYTES : STG_BYTES;   // the two alias
     static constexpr int AUX_BYTES = 256 + BN * 4;
-    static constexpr int STG_BYTES = BN <= 128 ? 4 * 8192 : 0;  // per-epilogue-warp store staging (coalesced stores)
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + STG_BYTES + 1024;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + EPI_BYTES + 1024;
 };
 
 struct TileCoord {
@@ -148,6 +148,34 @@ __device__ __forceinline__ TileCoord tile_coord(const ConvParams& p, int tile, i
     return t;
 }
 
+// One pipeline stage (BK = 64: four 16-wide k-steps) of split-fp16 products into the chunk accumulators:
+// `ch` takes a_hi b_hi (FUSE: a_hi [b_hi | b_lo]), `cx` the small cross terms a_hi b_lo + a_lo b_hi (FUSE: a_lo b_hi), so
+// that the truncating adds of the cross terms never touch the large a_hi b_hi sum.
+// NP = 3: all three products (default), 2: without a_lo b_hi, 1: a_hi b_hi only (experiment knob).
+// NP is a template argument so that the wgmma sequence has no branches between its instructions.
+template <class Cfg, int NP>
+__device__ __forceinline__ void conv_stage_mma(float (&ch)[Cfg::CHUNK_REGS], float (&cx)[Cfg::SUM_REGS], uint64_t a_hi,
+                                               uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
+#pragma unroll
+    for (int k = 0; k < Cfg::BK / 16; ++k) {
+        const uint64_t ko = (uint64_t)(k * 32 >> 4);
+        const uint32_t acc_in = (first && k == 0) ? 0u : 1u;
+        if constexpr (Cfg::FUSE) {
+            // [b_hi | b_lo] is one 2*BN-row K-major tile: columns [0,BN) += a_hi b_hi, [BN,2BN) += a_hi b_lo
+            wgmma_m64n128k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
+            if (NP >= 3) wgmma_m64n64k16<0, 0>(cx, a_lo + ko, b_hi + ko, acc_in);
+        } else if constexpr (Cfg::CHUNK_REGS == 64) {
+            wgmma_m64n128k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
+            if (NP >= 2) wgmma_m64n128k16<0, 0>(cx, a_hi + ko, b_lo + ko, acc_in);
+            if (NP >= 3) wgmma_m64n128k16<0, 0>(cx, a_lo + ko, b_hi + ko, 1u);
+        } else {
+            wgmma_m64n64k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
+            if (NP >= 2) wgmma_m64n64k16<0, 0>(cx, a_hi + ko, b_lo + ko, acc_in);
+            if (NP >= 3) wgmma_m64n64k16<0, 0>(cx, a_lo + ko, b_hi + ko, 1u);
+        }
+    }
+}
+
 template <int BN, bool FUSE_>
 __global__ void __launch_bounds__(Conv2Cfg<BN, FUSE_>::THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
@@ -158,11 +186,10 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     uint8_t* aux = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tfull = empty + Cfg::STAGES;
-    uint64_t* tempty = tfull + Cfg::NBUF;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + Cfg::NBUF);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_slot + 1);
+    volatile int* abort_flag = reinterpret_cast<volatile int*>(empty + Cfg::STAGES);
     float* sbias = reinterpret_cast<float*>(aux + 256);
+    uint8_t* epi = aux + Cfg::AUX_BYTES;                 // fp32 tile, then (aliased) the per-warp store staging buffers
+    float* ctile = reinterpret_cast<float*>(epi);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -175,29 +202,22 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     if (threadIdx.x == 0) {
         for (int s = 0; s < Cfg::STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
-        }
-        for (int b = 0; b < Cfg::NBUF; ++b) {
-            mbar_init(&tfull[b], 1);
-            mbar_init(&tempty[b], Cfg::EPI_WARPS);
+            mbar_init(&empty[s], Cfg::CONSUMERS / 32);      // one arrival per consumer warp
         }
         *abort_flag = 0;
         fence_barrier_init();
         tma_prefetch_desc(&mapA);
         tma_prefetch_desc(&mapB);
     }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int ksl = p.Cin / Cfg::BK;
     const int kiters = p.taps * ksl;
     const int nchunks = (kiters + Cfg::CH - 1) / Cfg::CH;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= Cfg::CONSUMERS / 32) {
+        setmaxnreg_dec<40>();
+        if (warp == Cfg::CONSUMERS / 32 && lane == 0) {
             uint32_t itg = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
@@ -230,222 +250,176 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16(Cfg::BM, BN);
-            constexpr uint32_t idesc2 = umma_idesc_f16(Cfg::BM, Cfg::FUSE ? 2 * BN : BN);
-            uint32_t itg = 0, cg_ = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                for (int c = 0; c < nchunks; ++c, ++cg_) {
-                    const int b = cg_ % Cfg::NBUF;
-                    const uint32_t bph = (cg_ / Cfg::NBUF) & 1;
-                    mbar_wait(&tempty[b], bph ^ 1u, abort_flag, p.err, 0x400u + b);   // epilogue drained this buffer
-                    tc_fence_after();
-                    const uint32_t tacc = tmem_base + (uint32_t)(b * Cfg::ACC_COLS);
-                    const int it_end = min(kiters, (c + 1) * Cfg::CH);
-                    for (int it = c * Cfg::CH; it < it_end; ++it, ++itg) {
-                        const int s = itg % Cfg::STAGES;
-                        const uint32_t ph = (itg / Cfg::STAGES) & 1;
-                        mbar_wait(&full[s], ph, abort_flag, p.err, 0x200u + s);
-                        tc_fence_after();
-                        const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
-                        const uint64_t a_hi = umma_desc_sw128(st);
-                        const uint64_t a_lo = umma_desc_sw128(st + Cfg::A_BYTES);
-                        const uint64_t b_hi = umma_desc_sw128(st + 2 * Cfg::A_BYTES);
-                        const uint64_t b_lo = umma_desc_sw128(st + 2 * Cfg::A_BYTES + Cfg::B_BYTES);
-                        const bool first = (it == c * Cfg::CH);
+        return;
+    }
+
+    // ---- consumer warpgroups ----
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;                            // rows [64 wg, 64 wg + 64) of the tile
+    const int t = threadIdx.x & 127;
+    const int e = warp;                                  // epilogue warp: rows 32 (e & 3) .. +31, channels 64 (e >> 2) .. +63
+    const int g = e & 3;
+    const int colbase = (e >> 2) * Cfg::NACC;
+    constexpr int ETHREADS = 32 * Cfg::EPI_WARPS;
+    const bool up2 = p.mode == CONV_UP2;
+    ActGeom go(p.N, up2 ? 2 * p.H : (p.pool ? (p.H + 1) / 2 : p.H), up2 ? 2 * p.W : (p.pool ? (p.W + 1) / 2 : p.W), p.Cout);
+    go.edge = (p.flags & WCTB200_HALO_EDGE) ? 1 : 0;
+    const bool relu = (p.flags & WCTB200_RELU) != 0;
+    const float wsc = p.wscale ? __ldg(p.wscale) : 1.f;
+    uint32_t itg = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
+        float sum[Cfg::SUM_REGS];
 #pragma unroll
-                        for (int k = 0; k < Cfg::BK / 16; ++k) {
-                            const uint64_t ko = (uint64_t)(k * 32 >> 4);
-                            if (Cfg::FUSE) {
-                                // [b_hi | b_lo] is one 2*BN-row K-major tile: columns [0,BN) += a_hi b_hi, [BN,2BN) += a_hi b_lo
-                                umma_f16(tacc, a_hi + ko, b_hi + ko, idesc2, (first && k == 0) ? 0u : 1u);
-                                if (p.products >= 3) umma_f16(tacc, a_lo + ko, b_hi + ko, idesc, 1u);
-                            } else {
-                                umma_f16(tacc, a_hi + ko, b_hi + ko, idesc, (first && k == 0) ? 0u : 1u);
-                                if (p.products >= 2) umma_f16(tacc, a_hi + ko, b_lo + ko, idesc, 1u);
-                                if (p.products >= 3) umma_f16(tacc, a_lo + ko, b_hi + ko, idesc, 1u);
-                            }
-                        }
-                        umma_commit(&empty[s]);
-                    }
-                    umma_commit(&tfull[b]);
-                }
+        for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
+        int it = 0;
+        for (int c = 0; c < nchunks; ++c) {
+            float ch[Cfg::CHUNK_REGS], cx[Cfg::SUM_REGS];
+#pragma unroll
+            for (int i = 0; i < Cfg::CHUNK_REGS; ++i) ch[i] = 0.f;
+#pragma unroll
+            for (int i = 0; i < Cfg::SUM_REGS; ++i) cx[i] = 0.f;
+            const int it_end = min(kiters, (c + 1) * Cfg::CH);
+            for (; it < it_end; ++it, ++itg) {
+                const int s = itg % Cfg::STAGES;
+                const uint32_t ph = (itg / Cfg::STAGES) & 1;
+                mbar_wait(&full[s], ph, abort_flag, p.err, 0x200u + s);
+                const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
+                const uint64_t a_hi = gmma_desc_sw128(st + wg * (Cfg::A_BYTES / 2));
+                const uint64_t a_lo = gmma_desc_sw128(st + Cfg::A_BYTES + wg * (Cfg::A_BYTES / 2));
+                const uint64_t b_hi = gmma_desc_sw128(st + 2 * Cfg::A_BYTES);
+                const uint64_t b_lo = gmma_desc_sw128(st + 2 * Cfg::A_BYTES + Cfg::B_BYTES);
+                const bool first = (it == c * Cfg::CH);
+                wgmma_fence();
+                if (p.products >= 3) conv_stage_mma<Cfg, 3>(ch, cx, a_hi, a_lo, b_hi, b_lo, first);
+                else if (p.products == 2) conv_stage_mma<Cfg, 2>(ch, cx, a_hi, a_lo, b_hi, b_lo, first);
+                else conv_stage_mma<Cfg, 1>(ch, cx, a_hi, a_lo, b_hi, b_lo, first);
+                wgmma_commit();
+                wgmma_wait<0>();
+                acc_fence(ch);
+                acc_fence(cx);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);   // stage may be refilled
+            }
+            if constexpr (Cfg::FUSE) {
+#pragma unroll
+                for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] += ch[i] + (ch[Cfg::SUM_REGS + i] + cx[i]);
+            } else {
+#pragma unroll
+                for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] += ch[i] + cx[i];
             }
         }
-        __syncwarp();
-    } else {
-        // ---- epilogue warps: drain chunks into registers, then bias/ReLU/split/store ----
-        const int e = warp - 2;
-        const int g = warp & 3;                              // TMEM lane quadrant of this warp
-        const int colbase = (e >> 2) * Cfg::NACC;            // BN=256: warps 6..9 take the upper half
-        const int et = threadIdx.x - 64;                     // 0 .. 32*EPI_WARPS-1
-        constexpr int ETHREADS = 32 * Cfg::EPI_WARPS;
-        const bool up2 = p.mode == CONV_UP2;
-        ActGeom go(p.N, up2 ? 2 * p.H : (p.pool ? (p.H + 1) / 2 : p.H), up2 ? 2 * p.W : (p.pool ? (p.W + 1) / 2 : p.W), p.Cout);
-        go.edge = (p.flags & WCTB200_HALO_EDGE) ? 1 : 0;
-        const bool relu = (p.flags & WCTB200_RELU) != 0;
-        const float wsc = p.wscale ? __ldg(p.wscale) : 1.f;
-        uint32_t cg_ = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
-            // stage this tile's bias slice (named barrier 1: epilogue warps only)
-            asm volatile("bar.sync 1, %0;" ::"r"(ETHREADS) : "memory");
-            for (int i = et; i < BN; i += ETHREADS) sbias[i] = p.bias ? p.bias[(long long)(p.mode == CONV_APPLY ? tc.set : 0) * p.Cout + tc.n0 + i] : 0.f;   // UP2: set = weight parity class, ONE bias
-            asm volatile("bar.sync 1, %0;" ::"r"(ETHREADS) : "memory");
 
-            float acc[Cfg::NACC];
+        // ---- fp32 tile through shared memory: epilogue thread = one row (position), 64 channels ----
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // previous tile's staging buffers are free
+        frag_to_tile(sum, ctile, Cfg::PITCH, 64 * wg, t);
+        for (int i = threadIdx.x; i < BN; i += Cfg::CONSUMERS)
+            sbias[i] = p.bias ? p.bias[(long long)(p.mode == CONV_APPLY ? tc.set : 0) * p.Cout + tc.n0 + i] : 0.f;   // UP2: set = weight parity class, ONE bias
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");
+        float acc[Cfg::NACC];
+        if (e < Cfg::EPI_WARPS) {
+            const float4* src = reinterpret_cast<const float4*>(ctile + (g * 32 + lane) * Cfg::PITCH + colbase);
 #pragma unroll
-            for (int i = 0; i < Cfg::NACC; ++i) acc[i] = 0.f;
-            for (int c = 0; c < nchunks; ++c, ++cg_) {
-                const int b = cg_ % Cfg::NBUF;
-                const uint32_t bph = (cg_ / Cfg::NBUF) & 1;
-                mbar_wait(&tfull[b], bph, abort_flag, p.err, 0x300u + b);
-                tc_fence_after();
-                const uint32_t tsrc = tmem_base + ((uint32_t)(g * 32) << 16) + (uint32_t)(b * Cfg::ACC_COLS + colbase);
-                if (Cfg::FUSE) {
-#pragma unroll
-                    for (int c0 = 0; c0 < Cfg::NACC; c0 += 32) {
-                        uint32_t r0[32], r1[32];
-                        tmem_ld32(tsrc + c0, r0);               // a_hi b_hi + a_lo b_hi
-                        tmem_ld32(tsrc + BN + c0, r1);          // a_hi b_lo
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(r0[j]) + __uint_as_float(r1[j]);
-                    }
-                } else {
-#pragma unroll
-                    for (int c0 = 0; c0 < Cfg::NACC; c0 += 64) {
-                        uint32_t r0[32], r1[32];
-                        tmem_ld32(tsrc + c0, r0);
-                        if (c0 + 32 < Cfg::NACC) tmem_ld32(tsrc + c0 + 32, r1);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(r0[j]);
-                        if (c0 + 32 < Cfg::NACC) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) acc[c0 + 32 + j] += __uint_as_float(r1[j]);
-                        }
-                    }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[b]);      // buffer may be overwritten
+            for (int j = 0; j < Cfg::NACC / 4; ++j) {
+                const float4 v = src[j];
+                acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
             }
-            if (Cfg::STG_BYTES > 0 && p.pool) {
-                // ---- MaxPooling2D 2x2/2 'same' (vgg_normalised.py:41-42) on the raw accumulators: max commutes with the
-                // monotone  *scale + bias -> ReLU -> split  that follows.  Tile rows 0..63 = image row 2i, 64..127 = row 2i+1.
-                // Work split: the two lanes of a horizontal pixel pair share the pooled pixel's channels (16-channel blocks:
-                // lane parity l owns channels 8l..8l+7 of each block), and the warps of the two image rows share them by halves
-                // (upper-row warps keep the lower half of the channel range, lower-row warps the upper half), so every lane of
-                // all four warps finishes and stores NACC/4 channels of one pooled pixel.
-                constexpr int NH = Cfg::NACC / 2;            // channels per half
-                constexpr int Q = Cfg::NACC / 4;             // channels a lane finishes
-                const int tpos = g * 32 + lane;
-                const int xloc = tpos & 63;
-                const int hv = tpos >> 6;                    // 0: image row 2i, 1: row 2i+1
-                const int lp = lane & 1;
-                const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
-                const unsigned int n = (unsigned int)tc.p0 / hpwp;
-                const int yy0 = (int)(((unsigned int)tc.p0 - n * hpwp) / (unsigned int)p.Wp);   // padded row of image row 2i
-                const int x = 64 * tc.cls + xloc;
-                const bool valid = (yy0 - 1 + hv) < p.H && x < p.W;
-                if (__any_sync(0xffffffffu, !valid)) {       // ragged right / bottom edge only
-                    const float ninf = __int_as_float(0xff800000);
+        }
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // tile read: the staging buffers may be written
+        if (e >= Cfg::EPI_WARPS) continue;
+
+        if (p.pool) {
+            // ---- MaxPooling2D 2x2/2 'same' (vgg_normalised.py:41-42) on the raw accumulators: max commutes with the
+            // monotone  *scale + bias -> ReLU -> split  that follows.  Tile rows 0..63 = image row 2i, 64..127 = row 2i+1.
+            // Work split: the two lanes of a horizontal pixel pair share the pooled pixel's channels (16-channel blocks:
+            // lane parity l owns channels 8l..8l+7 of each block), and the warps of the two image rows share them by halves
+            // (upper-row warps keep the lower half of the channel range, lower-row warps the upper half), so every lane of
+            // the two warps finishes and stores NACC/4 channels of one pooled pixel.
+            constexpr int NH = Cfg::NACC / 2;            // channels per half
+            constexpr int Q = Cfg::NACC / 4;             // channels a lane finishes
+            const int tpos = g * 32 + lane;
+            const int xloc = tpos & 63;
+            const int hv = tpos >> 6;                    // 0: image row 2i, 1: row 2i+1
+            const int lp = lane & 1;
+            const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
+            const unsigned int n = (unsigned int)tc.p0 / hpwp;
+            const int yy0 = (int)(((unsigned int)tc.p0 - n * hpwp) / (unsigned int)p.Wp);   // padded row of image row 2i
+            const int x = 64 * tc.cls + xloc;
+            const bool valid = (yy0 - 1 + hv) < p.H && x < p.W;
+            if (__any_sync(0xffffffffu, !valid)) {       // ragged right / bottom edge only
+                const float ninf = __int_as_float(0xff800000);
 #pragma unroll
-                    for (int j = 0; j < Cfg::NACC; ++j) acc[j] = valid ? acc[j] : ninf;
-                }
-                // horizontal: m[h][k] = max over the pixel pair of channel  h*NH + (k>>3)*16 + lp*8 + (k&7)
-                float keep[Q], send[Q];
-#pragma unroll
-                for (int k = 0; k < Q; ++k) {
-                    const int c0 = (k >> 3) * 16 + (k & 7);
-                    float mh[2];
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const float a0 = acc[h * NH + c0], a1 = acc[h * NH + c0 + 8];
-                        const float mine = lp ? a1 : a0;
-                        const float other = lp ? a0 : a1;    // the neighbour lane's channel, this lane's pixel
-                        mh[h] = fmaxf(mine, __shfl_xor_sync(0xffffffffu, other, 1));
-                    }
-                    keep[k] = hv ? mh[1] : mh[0];
-                    send[k] = hv ? mh[0] : mh[1];
-                }
-                // vertical: hand the other half over to the warp of the other image row (same lane = same pixel column)
-                uint8_t* stg_all = aux + Cfg::AUX_BYTES;
-                {
-                    float* xb = reinterpret_cast<float*>(stg_all + e * 8192) + lane;
-#pragma unroll
-                    for (int k = 0; k < Q; ++k) xb[k * 32] = send[k];
-                }
-                asm volatile("bar.sync 1, %0;" ::"r"(ETHREADS) : "memory");
-                {
-                    const float* pb = reinterpret_cast<const float*>(stg_all + (e ^ 2) * 8192) + lane;   // TMEM quadrant g ^ 2
-#pragma unroll
-                    for (int k = 0; k < Q; ++k) keep[k] = fmaxf(keep[k], pb[k * 32]);
-                }
-                const int xe = x & ~1;                       // the even column of the pair
-                if (xe < p.W && yy0 - 1 < p.H && !*abort_flag) {
-                    const int yo = (yy0 - 1) >> 1, xo = xe >> 1;
-                    const int flags = halo_flags(go, yo, xo);
-                    const unsigned int ppos = (n * (unsigned int)go.Hp + (unsigned int)(yo + 1)) * (unsigned int)go.Wp + (unsigned int)(xo + 1);
-                    const int cb = colbase + hv * NH + lp * 8;   // first channel this lane stores
-#pragma unroll
-                    for (int q = 0; q < Q / 8; ++q) {
-                        float v[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float t = fmaf(keep[q * 8 + j], wsc, sbias[cb + q * 16 + j]);
-                            v[j] = relu ? fmaxf(t, 0.f) : t;
-                        }
-                        Half8 hi, lo;
-                        split8(v, hi, lo);
-                        store8_at(p.out, go, ppos, flags, tc.n0 + cb + q * 16, hi, lo);
-                    }
-                }
-                continue;
+                for (int j = 0; j < Cfg::NACC; ++j) acc[j] = valid ? acc[j] : ninf;
             }
-            // ---- store: interior pixel + the halo cells that mirror it ----
-            // (32-bit position arithmetic: P < 2^31 is checked by the launcher; 64-bit divisions cost ~60 instructions each)
-            const unsigned int pos = (unsigned int)tc.p0 + (unsigned int)(g * 32 + lane);
-            int flags = -1;                                      // < 0: nothing to store for this row
-            unsigned int ppos = 0;
-            if (pos < (unsigned int)tc.p_end) {
-                const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
-                const unsigned int n = pos / hpwp;
-                const unsigned int r = pos - n * hpwp;
-                const int yy = (int)(r / (unsigned int)p.Wp);
-                const int xx = (int)(r - (unsigned int)yy * (unsigned int)p.Wp);
-                if (yy >= 1 && yy <= p.H && xx >= 1 && xx <= p.W && !*abort_flag) {
-                    int y = yy - 1, x = xx - 1;
-                    if (up2) { y = 2 * y + (tc.cls >> 1); x = 2 * x + (tc.cls & 1); }
-                    flags = halo_flags(go, y, x);
-                    ppos = ((unsigned int)n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
-                }
-            }
-            if (Cfg::STG_BYTES > 0) {
-                uint8_t* stg = aux + Cfg::AUX_BYTES + e * 8192;
-                store_tile_rows<Cfg::NACC>(acc, wsc, sbias + colbase, relu, stg, lane, ppos, flags, p.out, go, tc.n0 + colbase);
-            } else if (flags >= 0) {
+            // horizontal: m[h][k] = max over the pixel pair of channel  h*NH + (k>>3)*16 + lp*8 + (k&7)
+            float keep[Q], send[Q];
 #pragma unroll
-                for (int q = 0; q < Cfg::NACC / 8; ++q) {
+            for (int k = 0; k < Q; ++k) {
+                const int c0 = (k >> 3) * 16 + (k & 7);
+                float mh[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float a0 = acc[h * NH + c0], a1 = acc[h * NH + c0 + 8];
+                    const float mine = lp ? a1 : a0;
+                    const float other = lp ? a0 : a1;    // the neighbour lane's channel, this lane's pixel
+                    mh[h] = fmaxf(mine, __shfl_xor_sync(0xffffffffu, other, 1));
+                }
+                keep[k] = hv ? mh[1] : mh[0];
+                send[k] = hv ? mh[0] : mh[1];
+            }
+            // vertical: hand the other half over to the warp of the other image row (same lane = same pixel column)
+            {
+                float* xb = reinterpret_cast<float*>(epi + e * 8192) + lane;
+#pragma unroll
+                for (int k = 0; k < Q; ++k) xb[k * 32] = send[k];
+            }
+            asm volatile("bar.sync 2, %0;" ::"r"(ETHREADS) : "memory");
+            {
+                const float* pb = reinterpret_cast<const float*>(epi + (e ^ 2) * 8192) + lane;   // rows of the other image row
+#pragma unroll
+                for (int k = 0; k < Q; ++k) keep[k] = fmaxf(keep[k], pb[k * 32]);
+            }
+            const int xe = x & ~1;                       // the even column of the pair
+            if (xe < p.W && yy0 - 1 < p.H && !*abort_flag) {
+                const int yo = (yy0 - 1) >> 1, xo = xe >> 1;
+                const int flags = halo_flags(go, yo, xo);
+                const unsigned int ppos = (n * (unsigned int)go.Hp + (unsigned int)(yo + 1)) * (unsigned int)go.Wp + (unsigned int)(xo + 1);
+                const int cb = colbase + hv * NH + lp * 8;   // first channel this lane stores
+#pragma unroll
+                for (int q = 0; q < Q / 8; ++q) {
                     float v[8];
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
-                        const float t = fmaf(acc[q * 8 + j], wsc, sbias[colbase + q * 8 + j]);
-                        v[j] = relu ? fmaxf(t, 0.f) : t;
+                        const float tt = fmaf(keep[q * 8 + j], wsc, sbias[cb + q * 16 + j]);
+                        v[j] = relu ? fmaxf(tt, 0.f) : tt;
                     }
                     Half8 hi, lo;
                     split8(v, hi, lo);
-                    store8_at(p.out, go, ppos, flags, tc.n0 + colbase + q * 8, hi, lo);
+                    store8_at(p.out, go, ppos, flags, tc.n0 + cb + q * 16, hi, lo);
                 }
             }
+            continue;
         }
+        // ---- store: interior pixel + the halo cells that mirror it ----
+        // (32-bit position arithmetic: P < 2^31 is checked by the launcher; 64-bit divisions cost ~60 instructions each)
+        const unsigned int pos = (unsigned int)tc.p0 + (unsigned int)(g * 32 + lane);
+        int flags = -1;                                      // < 0: nothing to store for this row
+        unsigned int ppos = 0;
+        if (pos < (unsigned int)tc.p_end) {
+            const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
+            const unsigned int n = pos / hpwp;
+            const unsigned int r = pos - n * hpwp;
+            const int yy = (int)(r / (unsigned int)p.Wp);
+            const int xx = (int)(r - (unsigned int)yy * (unsigned int)p.Wp);
+            if (yy >= 1 && yy <= p.H && xx >= 1 && xx <= p.W && !*abort_flag) {
+                int y = yy - 1, x = xx - 1;
+                if (up2) { y = 2 * y + (tc.cls >> 1); x = 2 * x + (tc.cls & 1); }
+                flags = halo_flags(go, y, x);
+                ppos = ((unsigned int)n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
+            }
+        }
+        store_tile_rows<Cfg::NACC>(acc, wsc, sbias + colbase, relu, epi + e * 8192, lane, ppos, flags, p.out, go, tc.n0 + colbase);
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------
@@ -511,7 +485,7 @@ static int launch2_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtens
 
 int g_conv_products = 3;     // experiment knob (wctb200_debug_set_conv_products): split-fp16 products per MAC
 int g_conv_fuse = -1;        // -1 auto, 0 never, 1 whenever the tile allows (wctb200_debug_set_conv_fuse)
-int g_conv_bn_override = 0;  // test/tuning hook: force the N tile (64/128/256)
+int g_conv_bn_override = 0;  // test/tuning hook: force the N tile (64/128; 256 runs as 128)
 
 // mode CONV_3X3  : in [N,H,W,Cin], w_split [2][Cout][9*Cin],          out [N,H,W,Cout]
 // mode CONV_APPLY: in [N,H,W,Cin], w_split [nsets][2][Cout][Cin],     out [N,H,W,Cout]   (per-image weight sets)
@@ -532,9 +506,9 @@ int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, con
 
     const bool pool = (flags & WCTB200_POOL2) != 0;
     WCTB_REQUIRE(!pool || (mode == CONV_3X3 && (H + 1) / 2 >= 2 && (W + 1) / 2 >= 2), "conv: POOL2 needs the 3x3 mode and a pooled output >= 2x2");
-    int BN = Cout % 128 == 0 ? 128 : 64;   // 256-wide tiles leave only 2 pipeline stages: measured slower
-    if (g_conv_bn_override && Cout % g_conv_bn_override == 0) BN = g_conv_bn_override;
-    if (pool && BN > 128) BN = 128;        // the pooling epilogue works on the 4-warp layouts
+    // N tile: at most 128 (a 64 x 256 fp32 chunk plus the running sum would not fit a warpgroup's registers)
+    int BN = Cout % 128 == 0 ? 128 : 64;
+    if (g_conv_bn_override && Cout % g_conv_bn_override == 0) BN = g_conv_bn_override > 128 ? 128 : g_conv_bn_override;
 
     CUtensorMap mA, mB;
     int rc = make_tensor_map_3d(&mA, in, (uint64_t)Cin, (uint64_t)gi.P, 2, (uint64_t)Cin * 2, (uint64_t)gi.plane * 2, 128);
@@ -569,14 +543,10 @@ int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, con
     const int n_tiles = Cout / BN;
     const int total = m_tiles * n_tiles * (mode == CONV_UP2 ? 4 : 1);
     switch (BN) {
-        // fused [b_hi|b_lo] MMAs (Conv2Cfg::FUSE): always at BN=64 (4 TMEM buffers stay); at BN=128 the ring shrinks to 2
-        // buffers, which only pays for long K loops (measured: Cin=128 -9 %, Cin>=256 +3..5 %)
+        // fused [b_hi|b_lo] wgmma (Conv2Cfg::FUSE) at BN=64 unless switched off; at BN=128 it would need N = 256
         case 64: return g_conv_fuse == 0 ? launch2_bn<64, false>(mA, mB, mA64, p, total, n_tiles, st)
                                          : launch2_bn<64, true>(mA, mB, mA64, p, total, n_tiles, st);
-        case 128: return (g_conv_fuse == 1 || (g_conv_fuse < 0 && (long long)taps * Cin >= 9 * 256))
-                             ? launch2_bn<128, true>(mA, mB, mA64, p, total, n_tiles, st)
-                             : launch2_bn<128, false>(mA, mB, mA64, p, total, n_tiles, st);
-        default: return launch2_bn<256, false>(mA, mB, mA64, p, total, n_tiles, st);
+        default: return launch2_bn<128, false>(mA, mB, mA64, p, total, n_tiles, st);
     }
 }
 

@@ -4,22 +4,22 @@
 // The features are SPF16 [pixel][channel]: for the product X^T X the contraction index K is the
 // PIXEL, so both operands are "MN-major" (for a fixed k the 64 channels of a slice are the 128
 // contiguous bytes of a row).  A TMA box of 64 pixels x 64 channels lands as the canonical
-// MN-major SWIZZLE_128B tile (8-pixel groups of 1024 B), and tcgen05.mma reads A and B from the
-// same staged tiles with a_major = b_major = MN.  The tensor map is built over the INTERIOR of the
+// MN-major SWIZZLE_128B tile (8-pixel groups of 1024 B), and wgmma reads A and B from the
+// same staged tiles with both operands transposed (MN-major).  The tensor map is built over the INTERIOR of the
 // reflect-padded plane (base pointer at pixel (0,0), padded strides, dims W x H): boxes that stick
 // out at a ragged edge are zero-filled by TMA and add nothing to the sums, halo cells are never read.
 //
 // Centring (ops.py:44,49,106: fc = f - mean BEFORE the product).  Round 1 ran three extra passes for it (channel sums,
 // a centred SPF16 copy written to HBM, the product over the copy).  Now a tiny pre-kernel estimates a per-channel SHIFT t
-// (the mean of <= 1024 strided pixels; the exact mean when HW <= 1024), eight worker warps subtract t from every staged
-// tile IN SHARED MEMORY (hi+lo -> fp32 -> minus t -> re-split, zero-filled out-of-range pixels stay zero) before the MMA warp
-// may read it, and accumulate s = sum_p (x_p - t) on the way.  The finalize kernel forms
+// (the mean of <= 1024 strided pixels; the exact mean when HW <= 1024), the two consumer warpgroups subtract t from every
+// staged tile IN SHARED MEMORY (hi+lo -> fp32 -> minus t -> re-split, zero-filled out-of-range pixels stay zero) before
+// their wgmma read it, and accumulate s = sum_p (x_p - t) on the way.  The finalize kernel forms
 //     cov = (S - s s^T / HW) / (HW - 1),   mean = t + s / HW
 // in fp64: exact algebra for ANY t, and with t within sigma/32 of the mean the subtracted term is ~1e-3 of S, so nothing
 // cancels (the fully uncentred form, t = 0, was measured in round 1: it produced a spurious eigenvalue above the 1e-5 cut).
 //
-// Determinism.  Products in fp32 (split-fp16 x3), drained from TMEM every 128 pixels into registers (the tensor core
-// accumulates with truncation and the diagonals are all-positive sums).  Every CTA writes its partial block and partial sums
+// Determinism.  Products in fp32 (split-fp16 x3), a fresh register accumulator every 128 pixels added into the running sum
+// (the tensor core accumulates with truncation and the diagonals are all-positive sums).  Every CTA writes its partial block and partial sums
 // to its OWN slot; the finalize kernel adds the slots in a fixed order.  The split of an image into CTAs depends on (C, H, W)
 // only -- not on the batch size or the SM count -- so a frame's covariance is bit-identical whatever batch or GPU it is in
 // (tests: 2-GPU shards == 1 GPU, batch == single frames).
@@ -48,10 +48,10 @@ struct CovCfg {
     static constexpr int STAGE = 2 * OPER;                  // A + B (off-diagonal block pair); a diagonal pair uses OPER, C = 64 two SLICEs
     static constexpr int RING_BYTES = 3 * STAGE;            // 192 KB of tiles in flight whatever the stage size: 3 / 6 / 12 stages
     static constexpr int STAGES = 12;                       // barrier slots (the deepest ring)
-    static constexpr int NBUF = 4;
-    static constexpr int CH = 2;                            // 64-pixel tiles per TMEM accumulation chunk (24 truncating adds)
-    static constexpr int THREADS = 320;                     // producer, MMA, 8 worker warps (centring + TMEM drains)
-    static constexpr int RED_BYTES = 32 * 128 * 4;          // worker warps: [32 row groups][128 channels] partial sums
+    static constexpr int CH = 2;                            // 64-pixel tiles per register accumulation chunk (24 truncating adds)
+    static constexpr int CONSUMERS = 256;                   // two warpgroups: centring + wgmma
+    static constexpr int THREADS = CONSUMERS + 128;         // + producer warpgroup
+    static constexpr int RED_BYTES = 32 * 128 * 4;          // consumers: [32 row groups][128 channels] partial sums
     static constexpr int SMEM_BYTES = RING_BYTES + 512 + RED_BYTES + 1024;
 };
 
@@ -72,11 +72,7 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
     uint8_t* aux = smem + Cfg::RING_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* ready = empty + Cfg::STAGES;
-    uint64_t* tfull = ready + Cfg::STAGES;
-    uint64_t* tempty = tfull + Cfg::NBUF;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + Cfg::NBUF);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_slot + 1);
+    volatile int* abort_flag = reinterpret_cast<volatile int*>(empty + Cfg::STAGES);
     float* red = reinterpret_cast<float*>(aux + 512);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -99,26 +95,21 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
     const bool dup = (p.C == 64);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); mbar_init(&ready[s], 8); }
-        for (int b = 0; b < Cfg::NBUF; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], 8); }
+        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], Cfg::CONSUMERS / 32); }
         *abort_flag = 0;
         fence_barrier_init();
         tma_prefetch_desc(&mapX);
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int nchunks = (ntiles + Cfg::CH - 1) / Cfg::CH;
     // One stage holds exactly what one tile needs, so the ring is 3 (off-diagonal pair), 6 (diagonal pair) or 12 (C = 64)
-    // stages deep: the C <= 128 levels are HBM-latency bound, with 3 stages of 16 KB in flight a CTA could not pull more than
-    // ~27 GB/s (measured 0.34 of the HBM rate)
+    // stages deep: the C <= 128 levels are HBM-latency bound and want many tiles in flight
     const uint32_t stage_bytes = dup ? 2 * Cfg::SLICE : (diag ? Cfg::OPER : Cfg::STAGE);
     const int nst = min(Cfg::RING_BYTES / (int)stage_bytes, p.max_stages);
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= Cfg::CONSUMERS / 32) {
+        setmaxnreg_dec<40>();
+        if (warp == Cfg::CONSUMERS / 32 && lane == 0) {
             // (stage index, barrier phase and tile coordinates advance incrementally: runtime div/mod cost ~40 instructions each)
             int s = 0, ty = t0 / p.tiles_x, tx = t0 - ty * p.tiles_x;
             uint32_t ph = 0;
@@ -144,197 +135,153 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
                 }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16_mn(128, 128);
-            int it = 0, s = 0;
-            uint32_t ph = 0;
-            for (int c = 0; c < nchunks; ++c) {
-                const int b = c % Cfg::NBUF;
-                mbar_wait(&tempty[b], ((c / Cfg::NBUF) & 1) ^ 1u, abort_flag, p.err, 0x540u + b);
-                tc_fence_after();
-                const uint32_t tacc = tmem_base + (uint32_t)(b * 128);
-                const int it_end = min(ntiles, (c + 1) * Cfg::CH);
-                for (; it < it_end; ++it, ++s) {
-                    if (s == nst) { s = 0; ph ^= 1u; }
-                    mbar_wait(&ready[s], ph, abort_flag, p.err, 0x520u + s);   // tile landed AND centred
-                    tc_fence_after();
-                    const uint32_t a0 = smem_u32(smem + s * stage_bytes);
-                    const uint32_t b0 = diag ? a0 : a0 + Cfg::OPER;
-                    const bool first = (it == c * Cfg::CH);
+        return;
+    }
+
+    // ---- two consumer warpgroups (warps 0-7).  All 256 threads centre each staged tile (x -> x - shift in place, sums of
+    // the shifted values); then warpgroup w multiplies accumulator rows [64w, 64w + 64) (channels of block bi) with all 128
+    // columns (block bj) by wgmma with both operands MN-major.
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int ct = threadIdx.x;           // 0..255
+    const int chunk = ct & 7;             // logical 16-byte chunk of a 128-byte row = channels chunk*8 .. +7 of the slice
+    const int rg = ct >> 3;               // rows rg and rg+32 of every 64-pixel slice
+    const int pchunk = (chunk ^ (rg & 7)) << 4;      // SWIZZLE_128B: physical chunk = logical ^ (row & 7); row & 7 == rg & 7
+    const int nops = dup ? 1 : (diag ? 1 : 2);
+    const int nsl = dup ? 1 : 2;
+    const bool want_sums = dup || diag;   // every channel block has exactly one diagonal pair
+    float sh[2][2][8], sums[2][8], acc[64];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {           // 64 pixels = 4 x UMMA_K(16): 16 rows of 128 B = 2048 B per step
-                        const uint32_t ko = k * 2048;
-                        if (dup) {
-                            const uint64_t d = umma_desc_mn_sw128(a0 + ko);   // [hi | lo] x [hi | lo]^T
-                            umma_f16(tacc, d, d, idesc, (first && k == 0) ? 0u : 1u);
-                            continue;
-                        }
-                        const uint64_t a_hi = umma_desc_mn_sw128(a0 + ko);
-                        const uint64_t a_lo = umma_desc_mn_sw128(a0 + 2 * Cfg::SLICE + ko);
-                        const uint64_t b_hi = umma_desc_mn_sw128(b0 + ko);
-                        const uint64_t b_lo = umma_desc_mn_sw128(b0 + 2 * Cfg::SLICE + ko);
-                        umma_f16(tacc, a_hi, b_lo, idesc, (first && k == 0) ? 0u : 1u);
-                        umma_f16(tacc, a_lo, b_hi, idesc, 1u);
-                        umma_f16(tacc, a_hi, b_hi, idesc, 1u);
-                    }
-                    umma_commit(&empty[s]);
-                }
-                umma_commit(&tfull[b]);
-            }
+    for (int op = 0; op < 2; ++op)
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl) {
+            const int blk = op == 0 ? bi : bj;
+            const int c0 = dup ? chunk * 8 : blk * 128 + sl * 64 + chunk * 8;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) sh[op][sl][j] = (op < nops && sl < nsl) ? __ldg(p.shift + (long long)img * p.C + c0 + j) : 0.f;
         }
-        __syncwarp();
-    } else {
-        // ---- 8 worker warps (2..9).  All of them centre the staged tiles (x -> x - shift in place, sums of the shifted
-        // values); in between they drain the finished TMEM chunks into registers: warps 2-5 own accumulator columns 0..63,
-        // warps 6-9 columns 64..127 (a warp may only read the TMEM lanes of its quadrant, warp & 3).  One warp per
-        // scheduler for the centring (the first version: warps 6-9 only) ran at the latency of its own instruction chain
-        // and capped the kernel at 0.34 of the HBM rate.
-        const int ct = threadIdx.x - 64;      // 0..255
-        const int chunk = ct & 7;             // logical 16-byte chunk of a 128-byte row = channels chunk*8 .. +7 of the slice
-        const int rg = ct >> 3;               // rows rg and rg+32 of every 64-pixel slice
-        const int pchunk = (chunk ^ (rg & 7)) << 4;      // SWIZZLE_128B: physical chunk = logical ^ (row & 7); row & 7 == rg & 7
-        const int nops = dup ? 1 : (diag ? 1 : 2);
-        const int nsl = dup ? 1 : 2;
-        const bool want_sums = dup || diag;   // every channel block has exactly one diagonal pair
-        const int g = warp & 3;               // TMEM lane quadrant
-        const int chalf = warp >= 6 ? 1 : 0;  // accumulator column half drained by this warp
-        float sh[2][2][8], sums[2][8], acc[64];
 #pragma unroll
-        for (int op = 0; op < 2; ++op)
+    for (int sl = 0; sl < 2; ++sl)
 #pragma unroll
-            for (int sl = 0; sl < 2; ++sl) {
-                const int blk = op == 0 ? bi : bj;
-                const int c0 = dup ? chunk * 8 : blk * 128 + sl * 64 + chunk * 8;
+        for (int j = 0; j < 8; ++j) sums[sl][j] = 0.f;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) sh[op][sl][j] = (op < nops && sl < nsl) ? __ldg(p.shift + (long long)img * p.C + c0 + j) : 0.f;
-            }
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int s = 0, ty = t0 / p.tiles_x, tx = t0 - ty * p.tiles_x;
+    uint32_t ph = 0;
+    int it = 0;
+    for (int c = 0; c < nchunks; ++c) {
+        float chk[64];
 #pragma unroll
-        for (int sl = 0; sl < 2; ++sl)
+        for (int i = 0; i < 64; ++i) chk[i] = 0.f;
+        const int it_end = min(ntiles, (c + 1) * Cfg::CH);
+        for (; it < it_end; ++it, ++s, ++tx) {
+            if (s == nst) { s = 0; ph ^= 1u; }
+            if (tx == p.tiles_x) { tx = 0; ++ty; }
+            mbar_wait(&full[s], ph, abort_flag, p.err, 0x550u + s);
+            uint8_t* st = smem + s * stage_bytes;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) sums[sl][j] = 0.f;
+            for (int op = 0; op < 2; ++op) {
+                if (op >= nops) break;
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-        int drained = 0;
-        auto drain = [&](int c) {
-            const int b = c % Cfg::NBUF;
-            mbar_wait(&tfull[b], (c / Cfg::NBUF) & 1, abort_flag, p.err, 0x530u + b);
-            tc_fence_after();
-            const uint32_t tsrc = tmem_base + ((uint32_t)(g * 32) << 16) + (uint32_t)(b * 128 + chalf * 64);
-            uint32_t r0[32], r1[32];
-            tmem_ld32(tsrc, r0);
-            tmem_ld32(tsrc + 32, r1);
-            tmem_ld_wait();
+                for (int sl = 0; sl < 2; ++sl) {
+                    if (sl >= nsl) break;
+                    uint8_t* hi_base = dup ? st : st + op * Cfg::OPER + sl * Cfg::SLICE;
+                    uint8_t* lo_base = dup ? st + Cfg::SLICE : st + op * Cfg::OPER + (2 + sl) * Cfg::SLICE;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] += __uint_as_float(r0[j]);
+                    for (int k = 0; k < 2; ++k) {
+                        const int r = rg + 32 * k;
+                        const int x = tx * 32 + (r & 31), y = ty * 2 + (r >> 5);
+                        if (x < p.W && y < p.H) {           // out-of-range pixels were zero-filled by TMA and must stay zero
+                            const int off = r * 128 + pchunk;
+                            const Half8 h = *reinterpret_cast<const Half8*>(hi_base + off);
+                            const Half8 l = *reinterpret_cast<const Half8*>(lo_base + off);
+                            float v[8];
+                            merge8(h, l, v);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) acc[32 + j] += __uint_as_float(r1[j]);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[b]);
-        };
-        // fence.proxy.async (generic-proxy writes -> visible to the tensor core) is expensive: measured ~2100 cycles per tile
-        // whatever the number of centring warps or the ring depth (ncu: tensor pipe 13 % active, 2.2 TB/s).  The workers
-        // therefore centre a GROUP of tiles per fence: 4 when the ring is 12 deep, 2 when 6, 1 when 3.
-        const int T = nst >= 12 ? 4 : (nst >= 6 ? 2 : 1);
-        int s = 0, ty = t0 / p.tiles_x, tx = t0 - ty * p.tiles_x;
-        uint32_t ph = 0;
-        for (int it0 = 0; it0 < ntiles; it0 += T) {
-            const int it1 = min(it0 + T, ntiles);
-            const int s_first = s;
-            for (int it = it0; it < it1; ++it, ++s, ++tx) {
-                if (s == nst) { s = 0; ph ^= 1u; }
-                if (tx == p.tiles_x) { tx = 0; ++ty; }
-                mbar_wait(&full[s], ph, abort_flag, p.err, 0x550u + s);
-                uint8_t* st = smem + s * stage_bytes;
+                            for (int j = 0; j < 8; ++j) v[j] -= sh[op][sl][j];
+                            if (op == 0) {
 #pragma unroll
-                for (int op = 0; op < 2; ++op) {
-                    if (op >= nops) break;
-#pragma unroll
-                    for (int sl = 0; sl < 2; ++sl) {
-                        if (sl >= nsl) break;
-                        uint8_t* hi_base = dup ? st : st + op * Cfg::OPER + sl * Cfg::SLICE;
-                        uint8_t* lo_base = dup ? st + Cfg::SLICE : st + op * Cfg::OPER + (2 + sl) * Cfg::SLICE;
-#pragma unroll
-                        for (int k = 0; k < 2; ++k) {
-                            const int r = rg + 32 * k;
-                            const int x = tx * 32 + (r & 31), y = ty * 2 + (r >> 5);
-                            if (x < p.W && y < p.H) {           // out-of-range pixels were zero-filled by TMA and must stay zero
-                                const int off = r * 128 + pchunk;
-                                const Half8 h = *reinterpret_cast<const Half8*>(hi_base + off);
-                                const Half8 l = *reinterpret_cast<const Half8*>(lo_base + off);
-                                float v[8];
-                                merge8(h, l, v);
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) v[j] -= sh[op][sl][j];
-                                if (op == 0) {
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) sums[sl][j] += v[j];
-                                }
-                                Half8 nh, nl;
-                                split8(v, nh, nl);
-                                *reinterpret_cast<Half8*>(hi_base + off) = nh;
-                                *reinterpret_cast<Half8*>(lo_base + off) = nl;
+                                for (int j = 0; j < 8; ++j) sums[sl][j] += v[j];
                             }
+                            Half8 nh, nl;
+                            split8(v, nh, nl);
+                            *reinterpret_cast<Half8*>(hi_base + off) = nh;
+                            *reinterpret_cast<Half8*>(lo_base + off) = nl;
                         }
                     }
                 }
             }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-                int sa = s_first == nst ? 0 : s_first;
-                for (int it = it0; it < it1; ++it) {
-                    mbar_arrive(&ready[sa]);
-                    if (++sa == nst) sa = 0;
+            fence_proxy_async();                                   // generic-proxy writes -> visible to the tensor core
+            asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // the whole tile is centred
+            const uint32_t a0 = smem_u32(st);
+            const uint32_t b0 = diag ? a0 : a0 + Cfg::OPER;
+            const bool first = (it == c * Cfg::CH);
+            wgmma_fence();
+            if (dup) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {            // 64 pixels = 4 x k16: 16 rows of 128 B = 2048 B per step
+                    const uint32_t ko = k * 2048;
+                    // [hi | lo] x [hi | lo]^T: warpgroup w takes the rows of plane w
+                    wgmma_m64n128k16<1, 1>(chk, gmma_desc_mn_sw128(a0 + wg * Cfg::SLICE + ko), gmma_desc_mn_sw128(a0 + ko),
+                                           (first && k == 0) ? 0u : 1u);
+                }
+            } else {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint32_t ko = k * 2048;
+                    const uint64_t a_hi = gmma_desc_mn_sw128(a0 + wg * Cfg::SLICE + ko);
+                    const uint64_t a_lo = gmma_desc_mn_sw128(a0 + 2 * Cfg::SLICE + wg * Cfg::SLICE + ko);
+                    const uint64_t b_hi = gmma_desc_mn_sw128(b0 + ko);
+                    const uint64_t b_lo = gmma_desc_mn_sw128(b0 + 2 * Cfg::SLICE + ko);
+                    wgmma_m64n128k16<1, 1>(chk, a_hi, b_lo, (first && k == 0) ? 0u : 1u);
+                    wgmma_m64n128k16<1, 1>(chk, a_lo, b_hi, 1u);
+                    wgmma_m64n128k16<1, 1>(chk, a_hi, b_hi, 1u);
                 }
             }
-            // every tile of the chunks up to (it1-1) / CH is centred now: drain the chunks BEFORE that one
-            {
-                const int cdone = (it1 - 1) / Cfg::CH;
-                while (drained < cdone) drain(drained++);
-            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_fence(chk);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
         }
-        while (drained < nchunks) drain(drained++);
-        // ---- this CTA's partial block -> its own slot ----
-        const int m = g * 32 + lane;          // accumulator row
-        if (!*abort_flag) {
-            if (dup) {
-                // accumulator rows m and m+64 both belong to channel m & 63, columns j and 64+j to channel j: the four
-                // (row half, column half) quadrants go to four slots, the finalize kernel adds them
-                float* dst = p.part + (((long long)img * p.nslots + split * 4 + (m >> 6) * 2 + chalf) * p.C + (m & 63)) * p.C;
 #pragma unroll
-                for (int j = 0; j < 64; j += 4)
-                    *reinterpret_cast<float4*>(dst + j) = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
-            } else {
-                float* dst = p.part + (((long long)img * p.nslots + split) * p.C + bi * 128 + m) * p.C + bj * 128 + chalf * 64;
+        for (int i = 0; i < 64; ++i) acc[i] += chk[i];
+    }
+    // ---- this CTA's partial block -> its own slot.  Fragment: rows m, m + 8; columns 8j + 2 (lane & 3) (+1) ----
+    const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int cl = 2 * (lane & 3);
+    if (!*abort_flag) {
 #pragma unroll
-                for (int j = 0; j < 64; j += 4)
-                    *reinterpret_cast<float4*>(dst + j) = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
-            }
-        }
-        if (want_sums) {
-            // fixed-order reduction over the 32 row groups, then one partial per (image, split, channel)
+        for (int j = 0; j < 16; ++j) {
 #pragma unroll
-            for (int sl = 0; sl < 2; ++sl)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) red[rg * 128 + sl * 64 + chunk * 8 + j] = sums[sl][j];
-        }
-        asm volatile("bar.sync 2, 256;" ::: "memory");
-        if (want_sums) {
-            const int nch = dup ? 64 : 128;
-            if (ct < nch && !*abort_flag) {
-                float a = 0.f;
-#pragma unroll
-                for (int r = 0; r < 32; ++r) a += red[r * 128 + ct];
-                p.psum[((long long)img * p.ksplit + split) * p.C + (dup ? 0 : bi * 128) + ct] = a;
+            for (int h = 0; h < 2; ++h) {
+                const int mm = m + 8 * h, col = 8 * j + cl;
+                float* dst;
+                if (dup)   // rows m and m+64 both belong to channel m & 63, columns j and 64+j to channel j: quadrant -> slot
+                    dst = p.part + (((long long)img * p.nslots + split * 4 + (mm >> 6) * 2 + (col >> 6)) * p.C + (mm & 63)) * p.C + (col & 63);
+                else
+                    dst = p.part + (((long long)img * p.nslots + split) * p.C + bi * 128 + mm) * p.C + bj * 128 + col;
+                *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
+    if (want_sums) {
+        // fixed-order reduction over the 32 row groups, then one partial per (image, split, channel)
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) red[rg * 128 + sl * 64 + chunk * 8 + j] = sums[sl][j];
+    }
+    asm volatile("bar.sync 2, 256;" ::: "memory");
+    if (want_sums) {
+        const int nch = dup ? 64 : 128;
+        if (ct < nch && !*abort_flag) {
+            float a = 0.f;
+#pragma unroll
+            for (int r = 0; r < 32; ++r) a += red[r * 128 + ct];
+            p.psum[((long long)img * p.ksplit + split) * p.C + (dup ? 0 : bi * 128) + ct] = a;
+        }
+    }
 }
 
 // shift[n][c] = mean of <= ~1024 strided interior pixels (all pixels when HW <= 1024): fixed-order reduction.
@@ -445,8 +392,7 @@ int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, fl
     const int npairs = p.nb * (p.nb + 1) / 2;
     const int tiles_img = p.tiles_x * p.tiles_y;
     // Split of one image into CTAs: a function of (C, H, W) ONLY (batch- and device-invariant results).  Up to 64 tiles
-    // (4096 pixels) per CTA keeps the ~5 us of TMEM/barrier set-up per CTA below 20 % and still gives a single
-    // 512x512 frame 64 CTAs per block pair.
+    // (4096 pixels) per CTA keeps the per-CTA set-up small and still gives a single 512x512 frame 64 CTAs per block pair.
     int tps = 64;
     if (tiles_img < 64 * 8) tps = (tiles_img + 7) / 8;        // small maps: 8 splits
     if (tps < 8) tps = 8;

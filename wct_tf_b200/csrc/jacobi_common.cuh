@@ -5,7 +5,7 @@
 namespace wctb {
 
 // ---- register-blocked pair rotation: operands live in registers as PACKED fp32 pairs
-// (fma.rn.f32x2: two FMAs per instruction on sm_100), column norms are cached ----
+// (as fp32 pairs), column norms are cached ----
 // single-MUFU approximations (the CUDA intrinsics wrap these in range/denormal fix-ups: measured 25 FMUL +
 // 12 FSETP + 7 MUFU per rotation in the SASS of the previous version)
 __device__ __forceinline__ float rsqrt_ap(float x) {

@@ -202,8 +202,7 @@ k_conv_head(const float* __restrict__ img, int N, int H, int W, const float* __r
         const int xs = (int)(t % segs) * 4; t /= segs;
         const int y = (int)(t % (unsigned)H);
         const int n = (int)(t / (unsigned)H);
-        // accumulators as packed fp32 pairs (fma.rn.f32x2): the kernel is issue bound (ncu: IPC 2.7, FMA pipe 43 %,
-        // "not selected" the top stall), and a packed FMA does two channels per issue slot
+        // accumulators as fp32 pairs (two channels each)
         f32x2 acc[4][4];
 #pragma unroll
         for (int p = 0; p < 4; ++p)
@@ -229,8 +228,8 @@ k_conv_head(const float* __restrict__ img, int N, int H, int W, const float* __r
 #pragma unroll
                 for (int ci = 0; ci < 3; ++ci) {
                     const int k = (ky * 3 + kx) * 3 + ci;
-                    const ulonglong2 w0 = *reinterpret_cast<const ulonglong2*>(sw + (k * 2) * 32 + g * 4);       // channels 0..3 as two pairs
-                    const ulonglong2 w1 = *reinterpret_cast<const ulonglong2*>(sw + (k * 2 + 1) * 32 + g * 4);   // channels 4..7
+                    const f32x2x2 w0 = *reinterpret_cast<const f32x2x2*>(sw + (k * 2) * 32 + g * 4);       // channels 0..3 as two pairs
+                    const f32x2x2 w1 = *reinterpret_cast<const f32x2x2*>(sw + (k * 2 + 1) * 32 + g * 4);   // channels 4..7
 #pragma unroll
                     for (int p = 0; p < 4; ++p) {
                         const f32x2 v = in[p + kx][ci];
@@ -407,7 +406,7 @@ k_conv_tail_tiled(const __half* __restrict__ in, ActGeom gi, const float* __rest
     }
     f32x2 acc[8][3];                                  // packed pairs: (even, odd) channel partial sums, added at the end
 #pragma unroll
-    for (int p = 0; p < 8; ++p) acc[p][0] = acc[p][1] = acc[p][2] = 0ull;
+    for (int p = 0; p < 8; ++p) acc[p][0] = acc[p][1] = acc[p][2] = pack2(0.f, 0.f);
 
     for (int c0 = 0; c0 < gi.C; c0 += TT_CH) {
         asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -427,15 +426,15 @@ k_conv_tail_tiled(const __half* __restrict__ in, ActGeom gi, const float* __rest
             const float4* wg = swt + (c0 / 4 + g) * 3;
 #pragma unroll
             for (int kx = 0; kx < 3; ++kx) {
-                ulonglong2 a[10];                     // float4 viewed as two packed fp32 pairs
-                const ulonglong2* col = reinterpret_cast<const ulonglong2*>(sact) + (g * TT_PH + warp * 8) * TT_PW + lane + kx;
+                f32x2x2 a[10];                     // float4 viewed as two packed fp32 pairs
+                const f32x2x2* col = reinterpret_cast<const f32x2x2*>(sact) + (g * TT_PH + warp * 8) * TT_PW + lane + kx;
 #pragma unroll
                 for (int r = 0; r < 10; ++r) a[r] = col[r * TT_PW];
 #pragma unroll
                 for (int ky = 0; ky < 3; ++ky) {
 #pragma unroll
                     for (int o = 0; o < 3; ++o) {
-                        const ulonglong2 wv = *reinterpret_cast<const ulonglong2*>(wg + (ky * 3 + kx) * C4 * 3 + o);
+                        const f32x2x2 wv = *reinterpret_cast<const f32x2x2*>(wg + (ky * 3 + kx) * C4 * 3 + o);
 #pragma unroll
                         for (int p = 0; p < 8; ++p) acc[p][o] = fma2(a[p + ky].y, wv.y, fma2(a[p + ky].x, wv.x, acc[p][o]));
                     }

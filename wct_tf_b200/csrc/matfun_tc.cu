@@ -8,10 +8,10 @@
 // product form) that consists of nothing but C x C x C products -- tensor-core work instead of ~1.7 M plane rotations:
 //       Y_0 = A / s,  Z_0 = I                  (s = ||A||_F >= lambda_max)
 //       T   = (3 I - Z Y) / 2 ;   Y <- Y T ;   Z <- T Z          ->   Y -> (A/s)^1/2 ,  Z -> (A/s)^-1/2
-// The products are TRUE products (A operand K-major, B operand MN-major through the tcgen05 descriptors): although every
+// The products are TRUE products (A operand K-major, B operand MN-major through the wgmma descriptors): although every
 // iterate is symmetric in exact arithmetic, using rows for columns destabilises the iteration.  All operands live in HBM/L2 as split-fp16 planes [matrix][hi|lo][C][C]; a product is one launch of
-// `ns_gemm_kernel` (the TMA / tcgen05 / TMEM pipeline of conv_tc.cu: a_hi [b_hi|b_lo] + a_lo b_hi, chunked drain into fp32
-// registers), batched over the matrices of a level.  The residual max|I - Z Y| falls out of the first product of an
+// `ns_gemm_kernel` (the TMA / wgmma pipeline of conv_tc.cu: a_hi b_hi + a_hi b_lo + a_lo b_hi, chunks of 4 k-iterations
+// summed in fp32 registers), batched over the matrices of a level.  The residual max|I - Z Y| falls out of the first product of an
 // iteration; a matrix that reaches `tol` is skipped by every later launch (`conv_iter`), so the launch count is fixed and
 // nothing synchronises with the host.
 //
@@ -20,8 +20,7 @@
 // ||A^-1/2||_F^2 = ||Z||_F^2 / s, so  s / ||Z||_F^2 - eps_eig > thresh * 1.01  implies  lambda_min(cov) > thresh, i.e. k = C.
 // Everything else -- rank-deficient or ill-conditioned covariances, eigenvalues near the threshold -- is left to the Jacobi
 // eigensolver, whose kernels skip the matrices flagged here (`ok`).  Measured accuracy of the products (split-fp16 x3):
-// the transformed features move by ~4e-5 (values up to 5) against the eigendecomposition in float64
-// (profiles/r02_matfun_accuracy.txt); the parity gate is 1e-3.
+// tests/test_gpu_transform.py holds the transformed features to 1e-3 of the eigendecomposition in float64.
 #include <math.h>
 
 #include "common.cuh"
@@ -36,15 +35,16 @@ struct NsCfg {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;      // 64 KB
-    static constexpr int STAGES = 3;
-    static constexpr int ACC_COLS = 2 * BN;                            // [a_hi b_hi + a_lo b_hi | a_hi b_lo]
-    static constexpr int NBUF = 2;
-    static constexpr int TMEM_COLS = NBUF * ACC_COLS;                  // 512
+    static constexpr int STAGES = 2;
     static constexpr int CH = 4;                                       // k-iterations per accumulation chunk
-    static constexpr int THREADS = 192;
+    static constexpr int CONSUMERS = 256;                              // two wgmma warpgroups (64 rows each)
+    static constexpr int THREADS = CONSUMERS + 128;                    // + producer warpgroup
     static constexpr int AUX_BYTES = 512;
-    static constexpr int STG_BYTES = 4 * 8192;                         // per-epilogue-warp transposition buffer (coalesced row stores)
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + STG_BYTES + 1024;
+    static constexpr int PITCH = BN + 4;
+    static constexpr int TILE_BYTES = BM * PITCH * 4;                  // fp32 tile, aliased with the store staging buffers
+    static constexpr int STG_BYTES = 8 * 8192;                         // per-warp transposition buffer (coalesced row stores)
+    static constexpr int EPI_BYTES = TILE_BYTES > STG_BYTES ? TILE_BYTES : STG_BYTES;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + EPI_BYTES + 1024;
 };
 
 struct NsState {                 // per matrix
@@ -79,11 +79,10 @@ ns_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     uint8_t* aux = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tfull = empty + Cfg::STAGES;
-    uint64_t* tempty = tfull + Cfg::NBUF;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + Cfg::NBUF);
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(tmem_slot + 1);
-    float* red = reinterpret_cast<float*>(aux + 256);          // [4] epilogue partials
+    volatile int* abort_flag = reinterpret_cast<volatile int*>(empty + Cfg::STAGES);
+    float* red = reinterpret_cast<float*>(aux + 256);          // [8] epilogue partials
+    uint8_t* epi = aux + Cfg::AUX_BYTES;
+    float* ctile = reinterpret_cast<float*>(epi);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -96,22 +95,14 @@ ns_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     if (threadIdx.x == 0) {
         for (int s = 0; s < Cfg::STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
-        }
-        for (int b = 0; b < Cfg::NBUF; ++b) {
-            mbar_init(&tfull[b], 1);
-            mbar_init(&tempty[b], 4);
+            mbar_init(&empty[s], Cfg::CONSUMERS / 32);
         }
         *abort_flag = 0;
         fence_barrier_init();
         tma_prefetch_desc(&mapA);
         tma_prefetch_desc(&mapB);
     }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int kiters = p.n / Cfg::BK;
     const int nchunks = (kiters + Cfg::CH - 1) / Cfg::CH;
@@ -121,8 +112,9 @@ ns_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     // mode-1 product of iteration `it` itself: `it > conv_iter` is false for every reader of this launch either way)
     auto skipped = [&](int b) { return p.it > *reinterpret_cast<volatile int*>(&p.state[b].conv_iter); };
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= Cfg::CONSUMERS / 32) {
+        setmaxnreg_dec<40>();
+        if (warp == Cfg::CONSUMERS / 32 && lane == 0) {
             uint32_t itg = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int b = tile / tpm, r = tile - b * tpm;
@@ -147,173 +139,166 @@ ns_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // A K-major (rows of A), B MN-major (rows of B are the contraction index): TRUE products A B.  (Using B's rows as
-            // columns -- legitimate for exactly symmetric B -- makes the iteration unstable: the iterates only commute up to
-            // rounding, and the transposed products diverge after reaching ~1e-4; tools/ns_emulation.py.)
-            constexpr uint32_t idesc = umma_idesc_f16(Cfg::BM, Cfg::BN) | (1u << 16);
-            constexpr uint32_t idesc2 = umma_idesc_f16(Cfg::BM, 2 * Cfg::BN) | (1u << 16);
-            uint32_t itg = 0, cg_ = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                if (skipped(tile / tpm)) continue;
-                for (int c = 0; c < nchunks; ++c, ++cg_) {
-                    const int bb = cg_ % Cfg::NBUF;
-                    mbar_wait(&tempty[bb], ((cg_ / Cfg::NBUF) & 1) ^ 1u, abort_flag, p.err, 0x450u + bb);
-                    tc_fence_after();
-                    const uint32_t tacc = tmem_base + (uint32_t)(bb * Cfg::ACC_COLS);
-                    const int it_end = min(kiters, (c + 1) * Cfg::CH);
-                    for (int ki = c * Cfg::CH; ki < it_end; ++ki, ++itg) {
-                        const int s = itg % Cfg::STAGES;
-                        mbar_wait(&full[s], (itg / Cfg::STAGES) & 1, abort_flag, p.err, 0x250u + s);
-                        tc_fence_after();
-                        const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
-                        const uint64_t a_hi = umma_desc_sw128(st);
-                        const uint64_t a_lo = umma_desc_sw128(st + Cfg::A_BYTES);
-                        const bool first = (ki == c * Cfg::CH);
-#pragma unroll
-                        for (int k = 0; k < Cfg::BK / 16; ++k) {
-                            const uint64_t ko = (uint64_t)(k * 32 >> 4);
-                            const uint64_t b_hi = umma_desc_mn_sw128(st + 2 * Cfg::A_BYTES + k * 2048);   // 16 k-rows of 128 B per step
-                            umma_f16(tacc, a_hi + ko, b_hi, idesc2, (first && k == 0) ? 0u : 1u);        // N = 256: [b_hi | b_lo]
-                            umma_f16(tacc, a_lo + ko, b_hi, idesc, 1u);
-                        }
-                        umma_commit(&empty[s]);
-                    }
-                    umma_commit(&tfull[bb]);
-                }
-            }
-        }
-        __syncwarp();
-    } else {
-        const int e = warp - 2;
-        const int g = warp & 3;
-        uint32_t cg_ = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const int b = tile / tpm, r = tile - b * tpm;
-            if (skipped(b)) continue;
-            const int mi = r / p.tiles_m, ni = r - mi * p.tiles_m;
-            float acc[Cfg::BN];
-#pragma unroll
-            for (int i = 0; i < Cfg::BN; ++i) acc[i] = 0.f;
-            for (int c = 0; c < nchunks; ++c, ++cg_) {
-                const int bb = cg_ % Cfg::NBUF;
-                mbar_wait(&tfull[bb], (cg_ / Cfg::NBUF) & 1, abort_flag, p.err, 0x350u + bb);
-                tc_fence_after();
-                const uint32_t tsrc = tmem_base + ((uint32_t)(g * 32) << 16) + (uint32_t)(bb * Cfg::ACC_COLS);
-#pragma unroll
-                for (int c0 = 0; c0 < Cfg::BN; c0 += 32) {
-                    uint32_t r0[32], r1[32];
-                    tmem_ld32(tsrc + c0, r0);
-                    tmem_ld32(tsrc + Cfg::BN + c0, r1);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(r0[j]) + __uint_as_float(r1[j]);
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[bb]);
-            }
-            // ---- epilogue: this thread owns row `row`, columns [col0, col0 + 128) ----
-            const int row = mi * Cfg::BM + g * 32 + lane;
-            const int col0 = ni * Cfg::BN;
-            const int dj = row - col0;                               // diagonal element sits at acc[dj] when 0 <= dj < 128
-            float rmax = 0.f, zz = 0.f;
-            if (p.mode == 1) {
-#pragma unroll
-                for (int j = 0; j < Cfg::BN; ++j) {
-                    const float d = (j == dj) ? 1.f : 0.f;
-                    rmax = fmaxf(rmax, fabsf(acc[j] - d));           // |I - Z Y|
-                    acc[j] = fmaf(-0.5f, acc[j], 1.5f * d);          // T = (3 I - Z Y) / 2
-                }
-            }
-            // the fp32 result and ||Z||_F^2 are only needed from the FINAL iterate: the mode-1 product of this very iteration
-            // (earlier in stream order) has set conv_iter = it for a matrix whose residual passed
-            const bool final_it = *reinterpret_cast<volatile int*>(&p.state[b].conv_iter) == p.it;
-            const bool f32 = final_it && p.f32_rule != 0 && ((p.f32_rule == 1) == (b < p.n_first));
-            const float fs = f32 ? p.state[b].f32_scale : 0.f;
-            // Row-major stores through a per-warp transposition buffer: a thread owns a ROW of the tile, so direct stores
-            // would put 32 lanes on 32 different rows (ncu: 32 half-filled sectors per request, lg_throttle).  64 columns at a
-            // time go through 8 KB of shared memory (XOR-swizzled 16-byte chunks) and leave as full 128 / 256-byte row segments.
-            uint8_t* stg = aux + Cfg::AUX_BYTES + e * 8192;
-            const int rowbase = mi * Cfg::BM + g * 32;
-            if (!*abort_flag) {
-#pragma unroll
-                for (int h = 0; h < Cfg::BN / 64; ++h) {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        Half8 hi, lo;
-                        split8(acc + h * 64 + q * 8, hi, lo);
-                        const int slot = q ^ (lane & 7);
-                        *reinterpret_cast<Half8*>(stg + (lane * 8 + slot) * 16) = hi;
-                        *reinterpret_cast<Half8*>(stg + 4096 + (lane * 8 + slot) * 16) = lo;
-                    }
-                    __syncwarp();
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int rr = j * 4 + (lane >> 3), c = lane & 7;
-                        const int slot = c ^ (rr & 7);
-                        const Half8 hi = *reinterpret_cast<const Half8*>(stg + (rr * 8 + slot) * 16);
-                        const Half8 lo = *reinterpret_cast<const Half8*>(stg + 4096 + (rr * 8 + slot) * 16);
-                        __half* o = p.out_split + ((long long)(b * 2) * p.n + rowbase + rr) * p.n + col0 + h * 64 + c * 8;
-                        *reinterpret_cast<Half8*>(o) = hi;
-                        *reinterpret_cast<Half8*>(o + (long long)p.n * p.n) = lo;
-                    }
-                    __syncwarp();
-                    if (f32) {                                   // warp-uniform (one matrix per tile)
-#pragma unroll
-                        for (int q = 0; q < 16; ++q) {
-                            const float* a4 = acc + h * 64 + q * 4;
-                            const int slot = q ^ (lane & 15);
-                            *reinterpret_cast<float4*>(stg + (lane * 16 + slot) * 16) = make_float4(a4[0] * fs, a4[1] * fs, a4[2] * fs, a4[3] * fs);
-                        }
-                        __syncwarp();
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const int rr = j * 2 + (lane >> 4), c = lane & 15;
-                            const int slot = c ^ (rr & 15);
-                            const float4 v = *reinterpret_cast<const float4*>(stg + (rr * 16 + slot) * 16);
-                            *reinterpret_cast<float4*>(p.out_f32 + ((long long)b * p.n + rowbase + rr) * p.n + col0 + h * 64 + c * 4) = v;
-                        }
-                        __syncwarp();
-                    }
-                }
-            }
-            if (p.want_zz && final_it) {
-#pragma unroll
-                for (int j = 0; j < Cfg::BN; ++j) zz = fmaf(acc[j], acc[j], zz);
-#pragma unroll
-                for (int o = 16; o >= 1; o >>= 1) zz += __shfl_xor_sync(0xffffffffu, zz, o);
-                if (lane == 0) red[e] = zz;
-            }
-            if (p.mode == 1) {
-#pragma unroll
-                for (int o = 16; o >= 1; o >>= 1) rmax = fmaxf(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
-                if (lane == 0) atomicMax(&p.state[b].resid_bits, __float_as_uint(rmax));     // order independent
-            }
-            __threadfence();
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (e == 0 && lane == 0) {
-                if (p.want_zz && final_it) p.zz_slots[(long long)b * tpm + r] = (red[0] + red[1]) + (red[2] + red[3]);   // fixed order
-                if (p.mode == 1) {
-                    const int done = atomicAdd(&p.state[b].tiles_done, 1);
-                    if (done == tpm - 1) {                           // last tile of this matrix in this launch
-                        __threadfence();
-                        const float res = __uint_as_float(atomicAdd(&p.state[b].resid_bits, 0u));
-                        p.state[b].last_resid = res;
-                        p.state[b].resid_bits = 0u;
-                        p.state[b].tiles_done = 0;
-                        if (res < p.tol) p.state[b].conv_iter = p.it;
-                    }
-                }
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");           // red[] is reused by the next tile
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+
+    // ---- consumer warpgroups: rows [64 wg, 64 wg + 64) of the tile; then the epilogue, one row and 64 columns per thread ----
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int t = threadIdx.x & 127;
+    const int e = warp;
+    const int g = e & 3;
+    const int colbase = (e >> 2) * 64;
+    uint32_t itg = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int b = tile / tpm, r = tile - b * tpm;
+        if (skipped(b)) continue;
+        const int mi = r / p.tiles_m, ni = r - mi * p.tiles_m;
+        float sum[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+        int ki = 0;
+        for (int c = 0; c < nchunks; ++c) {
+            float ch[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) ch[i] = 0.f;
+            const int it_end = min(kiters, (c + 1) * Cfg::CH);
+            for (; ki < it_end; ++ki, ++itg) {
+                const int s = itg % Cfg::STAGES;
+                mbar_wait(&full[s], (itg / Cfg::STAGES) & 1, abort_flag, p.err, 0x250u + s);
+                // A K-major (rows of A), B MN-major (rows of B are the contraction index): TRUE products A B.  (Using B's rows
+                // as columns -- legitimate for exactly symmetric B -- makes the iteration unstable: the iterates only commute
+                // up to rounding, and the transposed products diverge after reaching ~1e-4; tools/ns_emulation.py.)
+                const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
+                const uint64_t a_hi = gmma_desc_sw128(st + wg * (Cfg::A_BYTES / 2));
+                const uint64_t a_lo = gmma_desc_sw128(st + Cfg::A_BYTES + wg * (Cfg::A_BYTES / 2));
+                const bool first = (ki == c * Cfg::CH);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < Cfg::BK / 16; ++k) {
+                    const uint64_t ko = (uint64_t)(k * 32 >> 4);
+                    const uint64_t b_hi = gmma_desc_mn_sw128(st + 2 * Cfg::A_BYTES + k * 2048);          // 16 k-rows of 128 B per step
+                    const uint64_t b_lo = gmma_desc_mn_sw128(st + 2 * Cfg::A_BYTES + 16384 + k * 2048);
+                    wgmma_m64n128k16<0, 1>(ch, a_hi + ko, b_hi, (first && k == 0) ? 0u : 1u);
+                    wgmma_m64n128k16<0, 1>(ch, a_hi + ko, b_lo, 1u);
+                    wgmma_m64n128k16<0, 1>(ch, a_lo + ko, b_hi, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                acc_fence(ch);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);
+            }
+#pragma unroll
+            for (int i = 0; i < 64; ++i) sum[i] += ch[i];
+        }
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // staging buffers of the previous tile are free
+        frag_to_tile(sum, ctile, Cfg::PITCH, 64 * wg, t);
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");
+        float acc[64];
+        {
+            const float4* src = reinterpret_cast<const float4*>(ctile + (g * 32 + lane) * Cfg::PITCH + colbase);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const float4 v = src[j];
+                acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
+            }
+        }
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // tile read: the staging buffers may be written
+
+        // ---- epilogue: this thread owns row `row`, columns [col0, col0 + 64) ----
+        const int row = mi * Cfg::BM + g * 32 + lane;
+        const int col0 = ni * Cfg::BN + colbase;
+        const int dj = row - col0;                               // diagonal element sits at acc[dj] when 0 <= dj < 64
+        float rmax = 0.f, zz = 0.f;
+        if (p.mode == 1) {
+#pragma unroll
+            for (int j = 0; j < 64; ++j) {
+                const float d = (j == dj) ? 1.f : 0.f;
+                rmax = fmaxf(rmax, fabsf(acc[j] - d));           // |I - Z Y|
+                acc[j] = fmaf(-0.5f, acc[j], 1.5f * d);          // T = (3 I - Z Y) / 2
+            }
+        }
+        // the fp32 result and ||Z||_F^2 are only needed from the FINAL iterate: the mode-1 product of this very iteration
+        // (earlier in stream order) has set conv_iter = it for a matrix whose residual passed
+        const bool final_it = *reinterpret_cast<volatile int*>(&p.state[b].conv_iter) == p.it;
+        const bool f32 = final_it && p.f32_rule != 0 && ((p.f32_rule == 1) == (b < p.n_first));
+        const float fs = f32 ? p.state[b].f32_scale : 0.f;
+        // Row-major stores through a per-warp transposition buffer: a thread owns a ROW of the tile, so direct stores
+        // would put 32 lanes on 32 different rows.  The 64 columns go through 8 KB of shared memory (XOR-swizzled 16-byte
+        // chunks) and leave as full 128 / 256-byte row segments.
+        uint8_t* stg = epi + e * 8192;
+        const int rowbase = mi * Cfg::BM + g * 32;
+        if (!*abort_flag) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                Half8 hi, lo;
+                split8(acc + q * 8, hi, lo);
+                const int slot = q ^ (lane & 7);
+                *reinterpret_cast<Half8*>(stg + (lane * 8 + slot) * 16) = hi;
+                *reinterpret_cast<Half8*>(stg + 4096 + (lane * 8 + slot) * 16) = lo;
+            }
+            __syncwarp();
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int rr = j * 4 + (lane >> 3), c = lane & 7;
+                const int slot = c ^ (rr & 7);
+                const Half8 hi = *reinterpret_cast<const Half8*>(stg + (rr * 8 + slot) * 16);
+                const Half8 lo = *reinterpret_cast<const Half8*>(stg + 4096 + (rr * 8 + slot) * 16);
+                __half* o = p.out_split + ((long long)(b * 2) * p.n + rowbase + rr) * p.n + col0 + c * 8;
+                *reinterpret_cast<Half8*>(o) = hi;
+                *reinterpret_cast<Half8*>(o + (long long)p.n * p.n) = lo;
+            }
+            __syncwarp();
+            if (f32) {                                   // warp-uniform (one matrix per tile)
+#pragma unroll
+                for (int q = 0; q < 16; ++q) {
+                    const float* a4 = acc + q * 4;
+                    const int slot = q ^ (lane & 15);
+                    *reinterpret_cast<float4*>(stg + (lane * 16 + slot) * 16) = make_float4(a4[0] * fs, a4[1] * fs, a4[2] * fs, a4[3] * fs);
+                }
+                __syncwarp();
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int rr = j * 2 + (lane >> 4), c = lane & 15;
+                    const int slot = c ^ (rr & 15);
+                    const float4 v = *reinterpret_cast<const float4*>(stg + (rr * 16 + slot) * 16);
+                    *reinterpret_cast<float4*>(p.out_f32 + ((long long)b * p.n + rowbase + rr) * p.n + col0 + c * 4) = v;
+                }
+                __syncwarp();
+            }
+        }
+        if (p.want_zz && final_it) {
+#pragma unroll
+            for (int j = 0; j < 64; ++j) zz = fmaf(acc[j], acc[j], zz);
+#pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) zz += __shfl_xor_sync(0xffffffffu, zz, o);
+            if (lane == 0) red[e] = zz;
+        }
+        if (p.mode == 1) {
+#pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) rmax = fmaxf(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
+            if (lane == 0) atomicMax(&p.state[b].resid_bits, __float_as_uint(rmax));     // order independent
+        }
+        __threadfence();
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");
+        if (e == 0 && lane == 0) {
+            if (p.want_zz && final_it)                                                   // fixed order
+                p.zz_slots[(long long)b * tpm + r] = ((red[0] + red[1]) + (red[2] + red[3])) + ((red[4] + red[5]) + (red[6] + red[7]));
+            if (p.mode == 1) {
+                const int done = atomicAdd(&p.state[b].tiles_done, 1);
+                if (done == tpm - 1) {                           // last tile of this matrix in this launch
+                    __threadfence();
+                    const float res = __uint_as_float(atomicAdd(&p.state[b].resid_bits, 0u));
+                    p.state[b].last_resid = res;
+                    p.state[b].resid_bits = 0u;
+                    p.state[b].tiles_done = 0;
+                    if (res < p.tol) p.state[b].conv_iter = p.it;
+                }
+            }
+        }
+        // (red[] is rewritten only after the next tile's three consumer barriers)
+    }
 }
 
 // s = ||A + eps I||_F, Y0 = (A + eps I)/s and Z0 = I as split planes, state reset.  Two launches of NS_INIT_BLOCKS blocks per

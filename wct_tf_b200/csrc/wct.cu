@@ -5,7 +5,7 @@
 // Stage B  C x C symmetric eigendecomposition: one-sided (Hestenes) Jacobi, one pair per warp,
 //          columns staged in shared memory, a thread-block CLUSTER of C/64 CTAs per matrix
 // Stage C  W_c = E_c D_c^-1/2 E_c^T, C_s = E_s D_s^1/2 E_s^T, T = C_s W_c, M = aT + (1-a)I, bias
-// Stage D  out = M x + bias : the 1-tap mode of the tcgen05 conv kernel (conv_tc.cu) with a
+// Stage D  out = M x + bias : the 1-tap mode of the wgmma conv kernel (conv_tc.cu) with a
 //          per-frame weight set, so the apply GEMM runs on the tensor cores.
 #include <cooperative_groups.h>
 
@@ -99,7 +99,7 @@ template <int HP>
 __device__ __forceinline__ void rot_regs2(f32x2 (&x0)[HP], f32x2 (&y0)[HP], float& a0, float& b0, f32x2 (&x1)[HP],
                                           f32x2 (&y1)[HP], float& a1, float& b1, float tol2, float tolq2, float null2,
                                           float& flag) {
-    f32x2 d00 = 0ull, d01 = 0ull, d10 = 0ull, d11 = 0ull;
+    f32x2 d00 = pack2(0.f, 0.f), d01 = d00, d10 = d00, d11 = d00;
 #pragma unroll
     for (int i = 0; i < HP; ++i) {
         if (i & 1) { d01 = fma2(x0[i], y0[i], d01); d11 = fma2(x1[i], y1[i], d11); }
@@ -141,11 +141,11 @@ __device__ __forceinline__ void load_col(const float* __restrict__ c, int lane, 
     for (int v = 0; v < Cfg::NV; ++v) {
         const int off = (v * 32 + lane) * Cfg::VEC;
         if (Cfg::VEC == 4) {
-            const ulonglong2 a = *reinterpret_cast<const ulonglong2*>(c + off);
+            const f32x2x2 a = *reinterpret_cast<const f32x2x2*>(c + off);
             r[v * 2] = a.x;
             r[v * 2 + 1] = a.y;
         } else {
-            r[v] = *reinterpret_cast<const unsigned long long*>(c + off);
+            r[v] = *reinterpret_cast<const f32x2*>(c + off);
         }
     }
 }
@@ -155,8 +155,8 @@ __device__ __forceinline__ void store_col(float* __restrict__ c, int lane, const
 #pragma unroll
     for (int v = 0; v < Cfg::NV; ++v) {
         const int off = (v * 32 + lane) * Cfg::VEC;
-        if (Cfg::VEC == 4) *reinterpret_cast<ulonglong2*>(c + off) = make_ulonglong2(r[v * 2], r[v * 2 + 1]);
-        else *reinterpret_cast<unsigned long long*>(c + off) = r[v];
+        if (Cfg::VEC == 4) *reinterpret_cast<f32x2x2*>(c + off) = f32x2x2{r[v * 2], r[v * 2 + 1]};
+        else *reinterpret_cast<f32x2*>(c + off) = r[v];
     }
 }
 
@@ -274,7 +274,7 @@ k_jacobi(float* __restrict__ Gall, float* __restrict__ conv_ws, int* __restrict_
             for (int c = warp * 4; c < warp * 4 + 4; ++c) {
                 f32x2 v[HP];
                 load_col<NN>(cols + c * NN, lane, v);
-                f32x2 q = 0ull;
+                f32x2 q = pack2(0.f, 0.f);
 #pragma unroll
                 for (int i = 0; i < HP; ++i) q = fma2(v[i], v[i], q);
                 float q0, q1;
@@ -643,7 +643,7 @@ static int launch_sums(const __half* act, ActGeom g, double* sum, double* sumsq,
 }
 
 // cross-phase schedule of k_jacobi: 2^lg warp groups, started `stagger` cycles apart (wctb200_debug_set_jacobi)
-// -1 = auto: measured best on B200 (tools/jacobi_bench.py): C=512 -> 4 groups 300 cycles apart (6.76 ms vs 7.80 ms for
+// -1 = auto: chosen by measurement (tools/jacobi_bench.py): C=512 -> 4 groups 300 cycles apart (6.76 ms vs 7.80 ms for
 // one group), smaller matrices -> 2 groups 600 cycles apart.
 int g_jacobi_lg = -1;
 int g_jacobi_stagger = -1;

@@ -6,11 +6,11 @@
 #ifdef __cplusplus
 extern "C" {
 #endif
-/* force the conv output-channel tile (64/128/256; 0 = built-in heuristic) */
+/* force the conv output-channel tile (64/128; 256 runs as 128; 0 = built-in heuristic) */
 WCTB200_API int wctb200_debug_set_conv_bn(int bn);
 /* CTAs per SM in the persistent conv grid (default 4; 1 = exactly one CTA per SM) */
 WCTB200_API int wctb200_debug_set_conv_oversub(int k);
-/* fuse the a_hi*b_hi and a_hi*b_lo products into one N = 2*tile MMA: -1 auto (default), 0 never, 1 always */
+/* fuse the a_hi*b_hi and a_hi*b_lo products into one N = 2*tile MMA at the 64-wide tile: -1 / 1 on (default), 0 off */
 WCTB200_API int wctb200_debug_set_conv_fuse(int mode);
 /* Jacobi cross-phase schedule: 2^lg_groups warp groups (0..4) started stagger_cycles apart; negative = per-size default */
 WCTB200_API int wctb200_debug_set_jacobi(int lg_groups, int stagger_cycles);

@@ -2,7 +2,7 @@
 
 Host side of the hot path ``WCT.predict`` (wct.py:70-106): PyTorch is used only
 for device memory, streams and H2D/D2H copies; every arithmetic step is a
-hand-written sm_100a kernel behind the C-ABI (include/wctb200.h).
+hand-written sm_90a kernel behind the C-ABI (include/wctb200.h).
 """
 from __future__ import annotations
 

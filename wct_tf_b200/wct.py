@@ -1,7 +1,7 @@
 """``WCT`` -- drop-in for the reference inference wrapper (wct.py:14-106).
 
 Same constructor and ``predict`` signature; the TF session is replaced by the
-sm_100a engine (engine.py -> libwctb200.so).  Differences, all explicit:
+sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``checkpoints`` / ``vgg_path`` may be file paths (``.npz`` bundles, see
     weights.py) OR ``weights=`` may pass an in-memory weights dict (the offline
     build has no .t7 / TF checkpoints, so benchmarks use synthetic weights);
@@ -32,7 +32,7 @@ def _torch_device(device):
         if re.match(r"^\d+$", device.strip()):          # a bare ordinal, as the CLI help advertises
             return "cuda:%s" % device.strip()
         if device.strip().lower() in ("/cpu:0", "cpu"):
-            raise ValueError("the B200 engine has no CPU path (device=%r)" % (device,))
+            raise ValueError("the CUDA engine has no CPU path (device=%r)" % (device,))
     return device
 
 
