@@ -172,6 +172,24 @@ WCTB200_API int wctb200_wct_style_prepare(const void* style, int Ns, int Hs, int
 WCTB200_API int wctb200_wct_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns,
                       float alpha, float eps_cov, float eps_eig, float thresh, int readd_content_mean,
                       void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
+/* Spatial control (WCT paper, section 4): a label map splits each content frame into regions and region r takes style r.
+ * Per (frame, region r < R) with at least 2 pixels the transform is wctb200_wct_apply's (same semantics flags) restricted
+ * to the region's pixels: mean, covariance and whitening over those pixels only, colouring with style r.  Every other
+ * pixel -- labels >= R, and regions with fewer than 2 pixels -- keeps its content feature bit for bit (interior and halo).
+ * labels: device uint8 [Nc][Hc][Wc], at the level's feature resolution (wctb200_labels_resize_nearest).
+ * states: HOST array of R device pointers, each a state of wctb200_wct_style_prepare with Ns = 1 (styles may have any size).
+ * R in 1..8, else WCTB200_EINVAL.  ws: device scratch of wctb200_wct_regions_workspace_bytes(C, Nc, R, Hc, Wc).
+ * k_out (device int32 [2*(Nc*R + R)], may be NULL): [k_c x Nc*R | k_s x R | sweeps_c x Nc*R | sweeps_s x R], entry
+ * n*R + r for frame n / region r; k_c = -1 (and 0 sweeps) for a skipped (frame, region).
+ * With R = 1 and every label 0 the output is byte-identical to wctb200_wct_apply's. */
+WCTB200_API size_t wctb200_wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc);
+WCTB200_API int wctb200_wct_apply_regions(const void* content, int Nc, int Hc, int Wc, int C, const uint8_t* labels, int R,
+                              const void* const* states, float alpha, float eps_cov, float eps_eig, float thresh,
+                              int readd_content_mean, void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
+/* Label map resampling for spatial control: src device uint8 [N][Hm][Wm] -> dst [N][Hf][Wf] by proportional nearest
+ * sampling in integer arithmetic, dst[y][x] = src[((2y+1)*Hm) / (2*Hf)][((2x+1)*Wm) / (2*Wf)] (no divisibility needed). */
+WCTB200_API int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst,
+                                  void* stream);
 /* AdaIN (ops.py:282-294): biased per-channel moments of content and style,
  * y = (x-mc)*rsqrt(vc+eps)*sqrt(vs)+ms, out = alpha*y + (1-alpha)*x. */
 WCTB200_API int wctb200_adain_level(const void* content, int Nc, int Hc, int Wc,
@@ -197,6 +215,10 @@ WCTB200_API int wctb200_style_swap_level(const void* content, int Hc, int Wc, co
  * (ops.py:43-45,105-108), fp32 outputs. */
 WCTB200_API int wctb200_covariance(const void* act, int N, int H, int W, int C, float eps_cov, float* mean, float* cov,
                        void* stream);
+/* The same per (image, region): labels device uint8 [N][H][W], R in 1..8; mean [N*R][C], cov [N*R][C][C] over the pixels
+ * labelled r (entry n*R + r), counts device int32 [N*R] = those pixels; cov = I where a region has fewer than 2 pixels. */
+WCTB200_API int wctb200_covariance_regions(const void* act, int N, int H, int W, int C, const uint8_t* labels, int R,
+                               float eps_cov, float* mean, float* cov, int32_t* counts, void* stream);
 /*
  * symmetric eigen-decomposition of `count` CxC fp32 matrices by one-sided Jacobi.
  * a: [count][C][C] symmetric (overwritten: column i becomes s_i * u_i, u_i the unit eigenvector, s_i within 2e-4 relative of

@@ -6,6 +6,10 @@ content x style loop at stylize.py:70-119, output naming ``<content>_<style><ext
   python stylize.py --checkpoints DIR5 DIR4 ... --relu-targets relu5_1 relu4_1 ... --vgg-path vgg_normalised.t7 \
       --content-path IN --style-path STYLE --out-path OUT --alpha 0.8
 
+Spatial control: ``--content-mask MASK --mask-styles S0 S1 ...`` splits the content by an 8-bit grayscale mask (gray value
+v -> region v*R // 256 for R styles: a black/white mask with two styles gives background / foreground) and region r takes
+style r; the output is ``<content>_<s0>+<s1>...<ext>``.
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -43,7 +47,13 @@ _FLAGS = [
     # not in the reference
     (("--synthetic-weights",), dict(type=int, default=None, help="seeded random weights (no model files needed)")),
     (("--semantics",), dict(type=str, default="tf", choices=["tf", "np"], help="wct_tf (the reference graph) or wct_np eps/blend rules")),
+    (("--content-mask",), dict(type=str, default=None, help="8-bit grayscale region mask: gray v -> region v*R//256 (R = #--mask-styles)")),
+    (("--mask-styles",), dict(nargs="+", type=str, default=None, help="one style image per mask region (with --content-mask)")),
 ]
+
+# flags that do not combine with --content-mask
+_MASK_EXCLUDES = [("style_path", "--style-path"), ("adain", "--adain"), ("swap5", "--swap5"), ("concat", "--concat"),
+                  ("random", "-r/--random")]
 
 
 def build_parser():
@@ -51,6 +61,34 @@ def build_parser():
     for names, kw in _FLAGS:
         parser.add_argument(*names, **kw)
     return parser
+
+
+def parse_args(argv=None):
+    parser = build_parser()
+    args = parser.parse_args(argv)
+    if args.content_mask is not None:
+        if not args.mask_styles:
+            parser.error("--content-mask needs --mask-styles")
+        if len(args.mask_styles) > 8:
+            parser.error("--mask-styles takes at most 8 styles")
+        for attr, flag in _MASK_EXCLUDES:
+            if getattr(args, attr):
+                parser.error("--content-mask does not combine with %s" % flag)
+    elif args.mask_styles:
+        parser.error("--mask-styles needs --content-mask")
+    return args
+
+
+def read_mask(path, R):
+    """8-bit grayscale mask file -> uint8 region labels: gray value v -> region v*R // 256."""
+    from PIL import Image
+    gray = np.asarray(Image.open(path).convert("L"), dtype=np.int64)
+    return ((gray * R) // 256).astype(np.uint8)
+
+
+def mask_output_name(content_path, style_paths):
+    stem, ext = os.path.splitext(os.path.basename(content_path))
+    return "{}_{}{}".format(stem, "+".join(os.path.splitext(os.path.basename(p))[0] for p in style_paths), ext)
 
 
 def _listing(path, io):
@@ -90,12 +128,44 @@ def make_model(args):
                ss_patch_size=args.ss_patch_size, ss_stride=args.ss_stride, weights=weights, semantics=args.semantics, verbose=True)
 
 
-def main(argv=None):
-    args = build_parser().parse_args(argv)
-    from wct_tf_b200 import device_image as dimg
+def _stylize_masked(model, content_dev, styles_dev, labels, args):
+    kw = dict(alpha=args.alpha, return_device=True, content_mask=labels)
+    result = model.predict_batch(content_dev, styles_dev, **kw)
+    for _ in range(args.passes - 1):
+        result = model.predict_batch(result, styles_dev, **kw)
+    return result[0]
+
+
+def main_masked(args, model, io, dimg, t_start):
+    """--content-mask: every content image, split by the mask, with region r in style r."""
+    labels = read_mask(args.content_mask, len(args.mask_styles))
+    os.makedirs(args.out_path, exist_ok=True)
+    device = model.engine.device
+    written = 0
+    for content_path in _listing(args.content_path, io):
+        content_dev = dimg.to_device(io.get_img(content_path), device)
+        if args.content_size > 0:
+            content_dev = dimg.resize_to(content_dev, args.content_size)
+        styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device) for p in args.mask_styles]
+        result = _stylize_masked(model, content_dev, styles_dev, labels, args)
+        target = os.path.join(args.out_path, mask_output_name(content_path, args.mask_styles))
+        io.save_img(target, dimg.to_host(result))
+        written += 1
+        print("{}: Wrote stylized output image to {}".format(written, target))
+    print("Finished stylizing {} outputs in {}s".format(written, time.time() - t_start))
+    return written
+
+
+def main(argv=None, model_factory=make_model, image_ops=None):
+    args = parse_args(argv)
     from wct_tf_b200 import imageio as io
+    if image_ops is None:
+        from wct_tf_b200 import device_image as image_ops
+    dimg = image_ops
     t_start = time.time()
-    model = make_model(args)
+    model = model_factory(args)
+    if args.content_mask is not None:
+        return main_masked(args, model, io, dimg, t_start)
     styles = _listing(args.style_path, io)
     if os.path.isdir(args.style_path) and args.random > 0:
         styles = list(np.random.choice(styles, args.random))

@@ -49,6 +49,10 @@ SIGNATURES = {
     "wctb200_adain_level": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _vp, _vp, _sz, _vp]),
     "wctb200_covariance": (_i, [_vp, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
     "wctb200_jacobi_eigh": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
+    "wctb200_wct_regions_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "wctb200_wct_apply_regions": (_i, [_vp, _i, _i, _i, _i, _vp, _i, C.POINTER(_vp), _f, _f, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_labels_resize_nearest": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "wctb200_covariance_regions": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp]),
     "wctb200_style_swap_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i]),
     "wctb200_style_swap_level": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _vp, _sz, _vp]),
 }
@@ -93,6 +97,11 @@ def load():
         raise WctB200Error("libwctb200 ABI version mismatch")
     _lib = lib
     return lib
+
+
+def pointer_array(ptrs):
+    """Host array of device pointers (``const void* const*`` arguments, e.g. the style states of wct_apply_regions)."""
+    return (_vp * len(ptrs))(*[int(p) for p in ptrs])
 
 
 def check(rc):

@@ -110,6 +110,11 @@ int launch_wct_style_prepare(const __half*, int, int, int, int, float, float, fl
 int launch_wct_apply(const __half*, int, int, int, int, const void*, int, float, float, float, float, int, __half*, int32_t*,
                      void*, size_t, cudaStream_t);
 int launch_covariance(const __half*, int, int, int, int, float, float*, float*, cudaStream_t);
+size_t wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc);
+int launch_wct_apply_regions(const __half*, int, int, int, int, const uint8_t*, int, const void* const*, float, float, float, float,
+                             int, __half*, int32_t*, void*, size_t, cudaStream_t);
+int launch_labels_resize(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, cudaStream_t st);
+int launch_covariance_regions(const __half*, int, int, int, int, const uint8_t*, int, float, float*, float*, int*, cudaStream_t);
 int launch_jacobi(float*, int, int, float*, int*, cudaStream_t, const int* skip);
 int launch_eig_post(const float*, const float*, float*, int, int, float, float, int, float*, float*, int*, cudaStream_t, const int* skip);
 extern int g_conv_bn_override;
@@ -298,6 +303,26 @@ int wctb200_wct_apply(const void* content, int Nc, int Hc, int Wc, int C, const 
     return launch_wct_apply(HCP(content), Nc, Hc, Wc, C, state, Ns, alpha, eps_cov, eps_eig, thresh, readd_content_mean,
                             HP(out), k_out, ws, ws_bytes, ST(stream));
 }
+size_t wctb200_wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc) {
+    if (C < 8 || Nc < 1 || R < 1 || R > 8 || Hc < 2 || Wc < 2) return 0;
+    return wct_regions_workspace_bytes(C, Nc, R, Hc, Wc);
+}
+int wctb200_wct_apply_regions(const void* content, int Nc, int Hc, int Wc, int C, const uint8_t* labels, int R,
+                              const void* const* states, float alpha, float eps_cov, float eps_eig, float thresh,
+                              int readd_content_mean, void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(content && labels && states && out && ws, "wct_apply_regions: null pointer");
+    WCTB_REQUIRE(R >= 1 && R <= 8, "wct_apply_regions: R=%d not in 1..8", R);
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "wct_apply_regions: bad geometry");
+    return launch_wct_apply_regions(HCP(content), Nc, Hc, Wc, C, labels, R, states, alpha, eps_cov, eps_eig, thresh,
+                                    readd_content_mean, HP(out), k_out, ws, ws_bytes, ST(stream));
+}
+int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, void* stream) {
+    WCTB_REQUIRE(src && dst, "labels_resize_nearest: null pointer");
+    WCTB_REQUIRE(N >= 1 && Hm >= 1 && Wm >= 1 && Hf >= 1 && Wf >= 1 && Hm <= (1 << 15) && Wm <= (1 << 15) && Hf <= (1 << 15) &&
+                     Wf <= (1 << 15),
+                 "labels_resize_nearest: bad geometry N=%d %dx%d -> %dx%d", N, Hm, Wm, Hf, Wf);
+    return launch_labels_resize(src, N, Hm, Wm, Hf, Wf, dst, ST(stream));
+}
 int wctb200_adain_level(const void* content, int Nc, int Hc, int Wc, const void* style, int Ns, int Hs, int Ws, int C,
                         float alpha, float eps, void* out, void* ws, size_t ws_bytes, void* stream) {
     WCTB_REQUIRE(content && style && out && ws, "adain_level: null pointer");
@@ -309,6 +334,13 @@ int wctb200_adain_level(const void* content, int Nc, int Hc, int Wc, const void*
 int wctb200_covariance(const void* act, int N, int H, int W, int C, float eps_cov, float* mean, float* cov, void* stream) {
     WCTB_REQUIRE(act && mean && cov && geom_ok(N, H, W, C), "covariance: bad arguments");
     return launch_covariance(HCP(act), N, H, W, C, eps_cov, mean, cov, ST(stream));
+}
+
+int wctb200_covariance_regions(const void* act, int N, int H, int W, int C, const uint8_t* labels, int R, float eps_cov,
+                               float* mean, float* cov, int32_t* counts, void* stream) {
+    WCTB_REQUIRE(act && labels && mean && cov && counts && geom_ok(N, H, W, C), "covariance_regions: bad arguments");
+    WCTB_REQUIRE(R >= 1 && R <= 8, "covariance_regions: R=%d not in 1..8", R);
+    return launch_covariance_regions(HCP(act), N, H, W, C, labels, R, eps_cov, mean, cov, counts, ST(stream));
 }
 
 int wctb200_jacobi_eigh(float* a, int C, int count, float* sigma, int32_t* sweeps, void* stream) {

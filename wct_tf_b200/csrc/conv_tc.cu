@@ -59,7 +59,19 @@ struct ConvParams {
     const float* wscale;  // device scalar: 1 / (power-of-two scale the weights were stored with), or nullptr (= 1)
     __half* out;          // SPF16, Cout channels; UP2: [N, 2H, 2W, Cout]
     unsigned int* err;
+    // regions apply (conv_tc2_kernel<.., REG = true>, spatial control): weight/bias set = image * R + region
+    const __half* in;     // the input activation (pixels outside every styled region are copied from it)
+    const uint8_t* labels;// [N][H][W] region label per pixel
+    const int* counts;    // [N*R] pixels per (image, region); a region with fewer than 2 pixels keeps its input
+    const uint16_t* amask;// [m_tiles]: bit r set when the tile holds a pixel of region r, bit R when it holds a kept pixel
+    int R;
 };
+
+// region a pixel takes in the regions apply: its label, or R (keep the input) for labels >= R and regions of < 2 pixels
+__device__ __forceinline__ int region_of(const uint8_t* labels, const int* counts, int R, int n, int H, int W, int y, int x) {
+    const int l = labels[((long long)n * H + y) * W + x];
+    return (l < R && counts[n * R + l] >= 2) ? l : R;
+}
 
 // ===========================================================================
 // Persistent CTAs, warp-specialised (384 threads):
@@ -176,7 +188,10 @@ __device__ __forceinline__ void conv_stage_mma(float (&ch)[Cfg::CHUNK_REGS], flo
     }
 }
 
-template <int BN, bool FUSE_>
+// REG (spatial control, CONV_APPLY only): every tile runs one mainloop + epilogue pass per region present in it (its own
+// weight set, stores only the rows of that region), then copies the rows to keep; a tile inside one region costs what the
+// plain apply costs.
+template <int BN, bool FUSE_, bool REG = false>
 __global__ void __launch_bounds__(Conv2Cfg<BN, FUSE_>::THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                 const __grid_constant__ CUtensorMap mapA64, const ConvParams p, const int total_tiles, const int n_tiles) {
@@ -221,6 +236,10 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             uint32_t itg = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
+                unsigned todo = 1u;                      // passes over the tile (REG: one per region present)
+                if constexpr (REG) todo = p.amask[tile / n_tiles] & ((1u << p.R) - 1u);
+                for (; todo; todo &= todo - 1u) {
+                const int set = REG ? (tile / n_tiles) / p.tiles_per_image * p.R + (__ffs(todo) - 1) : tc.set;
                 for (int it = 0; it < kiters; ++it, ++itg) {
                     const int s = itg % Cfg::STAGES;
                     const uint32_t ph = (itg / Cfg::STAGES) & 1;
@@ -244,9 +263,10 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                         tma_load_3d(st, &mapA, &full[s], ks * Cfg::BK, row, 0);
                         tma_load_3d(st + Cfg::A_BYTES, &mapA, &full[s], ks * Cfg::BK, row, 1);
                     }
-                    tma_load_3d(st + 2 * Cfg::A_BYTES, &mapB, &full[s], tap * p.Cin + ks * Cfg::BK, tc.n0, tc.set * 2);
+                    tma_load_3d(st + 2 * Cfg::A_BYTES, &mapB, &full[s], tap * p.Cin + ks * Cfg::BK, tc.n0, set * 2);
                     tma_load_3d(st + 2 * Cfg::A_BYTES + Cfg::B_BYTES, &mapB, &full[s], tap * p.Cin + ks * Cfg::BK,
-                                tc.n0, tc.set * 2 + 1);
+                                tc.n0, set * 2 + 1);
+                }
                 }
             }
         }
@@ -269,6 +289,11 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     uint32_t itg = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
+        unsigned todo = 1u;
+        if constexpr (REG) todo = p.amask[tile / n_tiles] & ((1u << p.R) - 1u);
+        for (; todo; todo &= todo - 1u) {
+        const int region = __ffs(todo) - 1;
+        const int set = REG ? (tile / n_tiles) / p.tiles_per_image * p.R + region : tc.set;
         float sum[Cfg::SUM_REGS];
 #pragma unroll
         for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
@@ -314,7 +339,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // previous tile's staging buffers are free
         frag_to_tile(sum, ctile, Cfg::PITCH, 64 * wg, t);
         for (int i = threadIdx.x; i < BN; i += Cfg::CONSUMERS)
-            sbias[i] = p.bias ? p.bias[(long long)(p.mode == CONV_APPLY ? tc.set : 0) * p.Cout + tc.n0 + i] : 0.f;   // UP2: set = weight parity class, ONE bias
+            sbias[i] = p.bias ? p.bias[(long long)(p.mode == CONV_APPLY ? set : 0) * p.Cout + tc.n0 + i] : 0.f;   // UP2: set = weight parity class, ONE bias
         asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");
         float acc[Cfg::NACC];
         if (e < Cfg::EPI_WARPS) {
@@ -416,9 +441,36 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 if (up2) { y = 2 * y + (tc.cls >> 1); x = 2 * x + (tc.cls & 1); }
                 flags = halo_flags(go, y, x);
                 ppos = ((unsigned int)n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
+                if (REG && region_of(p.labels, p.counts, p.R, (int)n, p.H, p.W, y, x) != region) flags = -1;   // another pass stores it
             }
         }
         store_tile_rows<Cfg::NACC>(acc, wsc, sbias + colbase, relu, epi + e * 8192, lane, ppos, flags, p.out, go, tc.n0 + colbase);
+        }
+        if constexpr (REG) {
+            // rows to keep: the input pixel (hi and lo bytes) goes to the interior cell and the halo cells that mirror it
+            if (((p.amask[tile / n_tiles] >> p.R) & 1u) && e < Cfg::EPI_WARPS && !*abort_flag) {
+                const unsigned int pos = (unsigned int)tc.p0 + (unsigned int)(g * 32 + lane);
+                if (pos < (unsigned int)tc.p_end) {
+                    const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
+                    const unsigned int n = pos / hpwp;
+                    const unsigned int r = pos - n * hpwp;
+                    const int yy = (int)(r / (unsigned int)p.Wp);
+                    const int xx = (int)(r - (unsigned int)yy * (unsigned int)p.Wp);
+                    if (yy >= 1 && yy <= p.H && xx >= 1 && xx <= p.W &&
+                        region_of(p.labels, p.counts, p.R, (int)n, p.H, p.W, yy - 1, xx - 1) == p.R) {
+                        const int flags = halo_flags(go, yy - 1, xx - 1);
+                        const long long plane = (long long)p.P * p.Cin;
+#pragma unroll
+                        for (int q = 0; q < Cfg::NACC / 8; ++q) {
+                            const int c0 = tc.n0 + colbase + q * 8;
+                            const Half8 hi = *reinterpret_cast<const Half8*>(p.in + (long long)pos * p.Cin + c0);
+                            const Half8 lo = *reinterpret_cast<const Half8*>(p.in + plane + (long long)pos * p.Cin + c0);
+                            store8_at(p.out, go, pos, flags, c0, hi, lo);
+                        }
+                    }
+                }
+            }
+        }
     }
 }
 
@@ -467,18 +519,18 @@ int make_tensor_map_3d(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d
 
 int g_conv_oversub = 4;
 
-template <int BN, bool FUSE_>
+template <int BN, bool FUSE_, bool REG = false>
 static int launch2_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mA64, const ConvParams& p, int total_tiles,
                       int n_tiles, cudaStream_t st) {
     using Cfg = Conv2Cfg<BN, FUSE_>;
-    WCTB_ENSURE_SMEM((conv_tc2_kernel<BN, FUSE_>), Cfg::SMEM_BYTES);
+    WCTB_ENSURE_SMEM((conv_tc2_kernel<BN, FUSE_, REG>), Cfg::SMEM_BYTES);
     // Over-subscribed persistent grid: with g_conv_oversub x #SMs CTAs (1 resident per SM) the
     // hardware block scheduler hands queued CTAs to whichever SMs are free, so a conv launched
     // while the Jacobi clusters of the other stream hold half the SMs still balances its tiles
     // (a grid of exactly #SMs would run as two unbalanced waves).
     int grid = device_sm_count() * (g_conv_oversub > 0 ? g_conv_oversub : 1);
     if (grid > total_tiles) grid = total_tiles;
-    conv_tc2_kernel<BN, FUSE_><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(mA, mB, mA64, p, total_tiles, n_tiles);
+    conv_tc2_kernel<BN, FUSE_, REG><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(mA, mB, mA64, p, total_tiles, n_tiles);
     WCTB_CHECK_LAUNCH("conv_tc2_kernel");
     return 0;
 }
@@ -491,8 +543,14 @@ int g_conv_bn_override = 0;  // test/tuning hook: force the N tile (64/128; 256 
 // mode CONV_APPLY: in [N,H,W,Cin], w_split [nsets][2][Cout][Cin],     out [N,H,W,Cout]   (per-image weight sets)
 // mode CONV_UP2  : in [N,H,W,Cin] (edge halo), w_split [4][2][Cout][4*Cin], out [N,2H,2W,Cout]
 // mode CONV_TAPS : in [N,H,W,Cin], w_split [2][Cout][kw*kw*Cin],      out [N,H,W,Cout]: top-left anchored kw x kw correlation
-int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
-                   const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw) {
+// regions (spatial control, CONV_APPLY with C = Cin = Cout): w_split [N*R][2][C][C], bias [N*R][C]; labels / counts / amask
+// as in ConvParams
+static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
+                        const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw,
+                        const uint8_t* labels, const int* counts, const uint16_t* amask, int R) {
+    const bool reg = labels != nullptr;
+    WCTB_REQUIRE(!reg || (mode == CONV_APPLY && Cin == Cout && nsets == N * R && flags == 0), "conv: bad regions apply");
+    if (reg) nsets = N;                                   // per-image tiling; the region picks the set inside an image
     WCTB_REQUIRE(N >= 1 && H >= 2 && W >= 2, "conv: bad geometry N=%d H=%d W=%d", N, H, W);
     WCTB_REQUIRE(Cin % 64 == 0 && Cout % 64 == 0 && Cin >= 64 && Cout >= 64, "conv: Cin=%d Cout=%d must be multiples of 64", Cin, Cout);
     WCTB_REQUIRE(mode == CONV_3X3 || mode == CONV_APPLY || mode == CONV_UP2 || mode == CONV_TAPS, "conv: bad mode %d", mode);
@@ -502,7 +560,7 @@ int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, con
     WCTB_REQUIRE(gi.P < (1ll << 31) - 4096, "conv: too many padded positions (%lld)", gi.P);
     WCTB_REQUIRE(mode != CONV_UP2 || ActGeom(N, 2 * H, 2 * W, Cout).P < (1ll << 31), "conv: too many output positions");
     const int taps = mode == CONV_3X3 ? 9 : (mode == CONV_UP2 ? 4 : (mode == CONV_TAPS ? kw * kw : 1));
-    const int wsets = mode == CONV_UP2 ? 4 : nsets;
+    const int wsets = mode == CONV_UP2 ? 4 : (reg ? N * R : nsets);
 
     const bool pool = (flags & WCTB200_POOL2) != 0;
     WCTB_REQUIRE(!pool || (mode == CONV_3X3 && (H + 1) / 2 >= 2 && (W + 1) / 2 >= 2), "conv: POOL2 needs the 3x3 mode and a pooled output >= 2x2");
@@ -539,15 +597,41 @@ int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, con
     p.wscale = wscale;
     p.out = out;
     p.err = device_error_word();
+    p.in = in;
+    p.labels = labels;
+    p.counts = counts;
+    p.amask = amask;
+    p.R = R;
+    if (reg) {
+        p.per_image = 1;
+        p.nsets = N;
+    }
     const int m_tiles = pool ? N * p.pool_ho * p.pool_tx : (p.per_image ? N * p.tiles_per_image : cdiv(gi.P, 128));
     const int n_tiles = Cout / BN;
     const int total = m_tiles * n_tiles * (mode == CONV_UP2 ? 4 : 1);
+    if (reg) {
+        switch (BN) {
+            case 64: return g_conv_fuse == 0 ? launch2_bn<64, false, true>(mA, mB, mA64, p, total, n_tiles, st)
+                                             : launch2_bn<64, true, true>(mA, mB, mA64, p, total, n_tiles, st);
+            default: return launch2_bn<128, false, true>(mA, mB, mA64, p, total, n_tiles, st);
+        }
+    }
     switch (BN) {
         // fused [b_hi|b_lo] wgmma (Conv2Cfg::FUSE) at BN=64 unless switched off; at BN=128 it would need N = 256
         case 64: return g_conv_fuse == 0 ? launch2_bn<64, false>(mA, mB, mA64, p, total, n_tiles, st)
                                          : launch2_bn<64, true>(mA, mB, mA64, p, total, n_tiles, st);
         default: return launch2_bn<128, false>(mA, mB, mA64, p, total, n_tiles, st);
     }
+}
+
+int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
+                   const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw) {
+    return conv_tc_impl(mode, in, N, H, W, Cin, w_split, nsets, wscale, bias, Cout, flags, out, st, kw, nullptr, nullptr, nullptr, 1);
+}
+// out = M_{n,r} x + bias_{n,r} for the pixels of region r of image n, out = x for the rest (wct.cu: launch_wct_apply_regions)
+int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const uint8_t* labels,
+                              const int* counts, const uint16_t* amask, int R, __half* out, cudaStream_t st) {
+    return conv_tc_impl(CONV_APPLY, in, N, H, W, C, w_split, N * R, nullptr, bias, C, 0, out, st, 3, labels, counts, amask, R);
 }
 
 }  // namespace wctb

@@ -36,10 +36,14 @@ struct CovParams {
     int nb;                      // 128-channel blocks (C=64: 1 block, rows duplicated)
     int nslots;                  // partial slots per image: ksplit (C=64: 4*ksplit)
     int max_stages;              // cap on the ring depth (probe knob; 12 = no cap)
-    const float* shift;          // [N][C]
-    float* part;                 // [N][nslots][C][C] fp32 partial products (upper block triangle)
+    const float* shift;          // [N][C]   (regions: [N*R][C])
+    float* part;                 // [N][nslots][C][C] fp32 partial products (upper block triangle)   (regions: [N*R]...)
     float* psum;                 // [N][ksplit][C] fp32 partial sums of (x - shift)
     unsigned int* err;
+    // spatial control (cov_tc_kernel<true>): problem z = image * R + region covers the pixels labelled `region` only
+    const uint8_t* labels;       // [N][H][W] region label per pixel
+    const uint16_t* tmask;       // [N][tiles_y * tiles_x]: bit r set when the 32 x 2 tile holds a pixel labelled r
+    int R;
 };
 
 struct CovCfg {
@@ -64,6 +68,10 @@ __device__ __forceinline__ void tma_load_5d_cov(void* smem_dst, const void* map,
         : "memory");
 }
 
+// MASK = false: one problem per image (blockIdx.y = image).  MASK = true (spatial control): blockIdx.y = image * R + region;
+// producer and consumers skip the tiles without a pixel of the region (each tile is read once per region present in it),
+// and the centring step writes zeros for the staged pixels of other regions, exactly as for out-of-range pixels.
+template <bool MASK>
 __global__ void __launch_bounds__(CovCfg::THREADS, 1)
 cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
     using Cfg = CovCfg;
@@ -84,7 +92,10 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
     while (rem >= p.nb - bi) { rem -= p.nb - bi; ++bi; }
     const int bj = bi + rem;
     const bool diag = (bi == bj);
-    const int img = blockIdx.y;
+    const int prob = blockIdx.y;                     // output slot: image (MASK: image * R + region)
+    const int img = MASK ? prob / p.R : prob;
+    const int reg = MASK ? prob - img * p.R : 0;
+    const uint16_t* tmask = MASK ? p.tmask + (long long)img * p.tiles_x * p.tiles_y : nullptr;
     const int tiles_img = p.tiles_x * p.tiles_y;
     const int t0 = split * p.tiles_per_split;
     const int t1 = min(t0 + p.tiles_per_split, tiles_img);
@@ -113,15 +124,17 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
             // (stage index, barrier phase and tile coordinates advance incrementally: runtime div/mod cost ~40 instructions each)
             int s = 0, ty = t0 / p.tiles_x, tx = t0 - ty * p.tiles_x;
             uint32_t ph = 0;
-            for (int it = 0; it < ntiles; ++it, ++s, ++tx) {
-                if (s == nst) { s = 0; ph ^= 1u; }
+            for (int it = 0; it < ntiles; ++it, ++tx) {
                 if (tx == p.tiles_x) { tx = 0; ++ty; }
+                if (MASK && !((tmask[t0 + it] >> reg) & 1u)) continue;
+                if (s == nst) { s = 0; ph ^= 1u; }
                 mbar_wait(&empty[s], ph ^ 1u, abort_flag, p.err, 0x510u + s);
                 uint8_t* st = smem + s * stage_bytes;
                 mbar_arrive_expect_tx(&full[s], stage_bytes);
                 if (dup) {
                     tma_load_5d_cov(st, &mapX, &full[s], 0, tx * 32, ty * 2, img, 0);                  // rows 0..63   : hi
                     tma_load_5d_cov(st + Cfg::SLICE, &mapX, &full[s], 0, tx * 32, ty * 2, img, 1);     // rows 64..127 : lo
+                    ++s;
                     continue;
                 }
                 for (int op = 0; op < (diag ? 1 : 2); ++op) {
@@ -133,6 +146,7 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
                                             ty * 2, img, pl);
                     }
                 }
+                ++s;
             }
         }
         return;
@@ -158,7 +172,7 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
             const int blk = op == 0 ? bi : bj;
             const int c0 = dup ? chunk * 8 : blk * 128 + sl * 64 + chunk * 8;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) sh[op][sl][j] = (op < nops && sl < nsl) ? __ldg(p.shift + (long long)img * p.C + c0 + j) : 0.f;
+            for (int j = 0; j < 8; ++j) sh[op][sl][j] = (op < nops && sl < nsl) ? __ldg(p.shift + (long long)prob * p.C + c0 + j) : 0.f;
         }
 #pragma unroll
     for (int sl = 0; sl < 2; ++sl)
@@ -168,84 +182,125 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     int s = 0, ty = t0 / p.tiles_x, tx = t0 - ty * p.tiles_x;
     uint32_t ph = 0;
-    int it = 0;
-    for (int c = 0; c < nchunks; ++c) {
-        float chk[64];
+    // one staged tile: centre it in shared memory, then multiply it into `chk` (first: the chunk starts from zero)
+    auto tile = [&](float (&chk)[64], bool first) {
+        mbar_wait(&full[s], ph, abort_flag, p.err, 0x550u + s);
+        uint8_t* st = smem + s * stage_bytes;
+        bool keep[2] = {true, true};                 // MASK: the pixel carries this CTA's region label
+        if (MASK) {
 #pragma unroll
-        for (int i = 0; i < 64; ++i) chk[i] = 0.f;
-        const int it_end = min(ntiles, (c + 1) * Cfg::CH);
-        for (; it < it_end; ++it, ++s, ++tx) {
-            if (s == nst) { s = 0; ph ^= 1u; }
-            if (tx == p.tiles_x) { tx = 0; ++ty; }
-            mbar_wait(&full[s], ph, abort_flag, p.err, 0x550u + s);
-            uint8_t* st = smem + s * stage_bytes;
+            for (int k = 0; k < 2; ++k) {
+                const int r = rg + 32 * k;
+                const int x = tx * 32 + (r & 31), y = ty * 2 + (r >> 5);
+                keep[k] = x < p.W && y < p.H && p.labels[((long long)img * p.H + y) * p.W + x] == reg;
+            }
+        }
 #pragma unroll
-            for (int op = 0; op < 2; ++op) {
-                if (op >= nops) break;
+        for (int op = 0; op < 2; ++op) {
+            if (op >= nops) break;
 #pragma unroll
-                for (int sl = 0; sl < 2; ++sl) {
-                    if (sl >= nsl) break;
-                    uint8_t* hi_base = dup ? st : st + op * Cfg::OPER + sl * Cfg::SLICE;
-                    uint8_t* lo_base = dup ? st + Cfg::SLICE : st + op * Cfg::OPER + (2 + sl) * Cfg::SLICE;
+            for (int sl = 0; sl < 2; ++sl) {
+                if (sl >= nsl) break;
+                uint8_t* hi_base = dup ? st : st + op * Cfg::OPER + sl * Cfg::SLICE;
+                uint8_t* lo_base = dup ? st + Cfg::SLICE : st + op * Cfg::OPER + (2 + sl) * Cfg::SLICE;
 #pragma unroll
-                    for (int k = 0; k < 2; ++k) {
-                        const int r = rg + 32 * k;
-                        const int x = tx * 32 + (r & 31), y = ty * 2 + (r >> 5);
-                        if (x < p.W && y < p.H) {           // out-of-range pixels were zero-filled by TMA and must stay zero
-                            const int off = r * 128 + pchunk;
-                            const Half8 h = *reinterpret_cast<const Half8*>(hi_base + off);
-                            const Half8 l = *reinterpret_cast<const Half8*>(lo_base + off);
-                            float v[8];
-                            merge8(h, l, v);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) v[j] -= sh[op][sl][j];
-                            if (op == 0) {
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) sums[sl][j] += v[j];
-                            }
-                            Half8 nh, nl;
-                            split8(v, nh, nl);
-                            *reinterpret_cast<Half8*>(hi_base + off) = nh;
-                            *reinterpret_cast<Half8*>(lo_base + off) = nl;
+                for (int k = 0; k < 2; ++k) {
+                    const int r = rg + 32 * k;
+                    const int x = tx * 32 + (r & 31), y = ty * 2 + (r >> 5);
+                    if (x < p.W && y < p.H) {           // out-of-range pixels were zero-filled by TMA and must stay zero
+                        const int off = r * 128 + pchunk;
+                        if (MASK && !keep[k]) {         // another region's pixel: TMA loaded it, overwrite with zeros
+                            const Half8 z = {};
+                            *reinterpret_cast<Half8*>(hi_base + off) = z;
+                            *reinterpret_cast<Half8*>(lo_base + off) = z;
+                            continue;
                         }
+                        const Half8 h = *reinterpret_cast<const Half8*>(hi_base + off);
+                        const Half8 l = *reinterpret_cast<const Half8*>(lo_base + off);
+                        float v[8];
+                        merge8(h, l, v);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) v[j] -= sh[op][sl][j];
+                        if (op == 0) {
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) sums[sl][j] += v[j];
+                        }
+                        Half8 nh, nl;
+                        split8(v, nh, nl);
+                        *reinterpret_cast<Half8*>(hi_base + off) = nh;
+                        *reinterpret_cast<Half8*>(lo_base + off) = nl;
                     }
                 }
             }
-            fence_proxy_async();                                   // generic-proxy writes -> visible to the tensor core
-            asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // the whole tile is centred
-            const uint32_t a0 = smem_u32(st);
-            const uint32_t b0 = diag ? a0 : a0 + Cfg::OPER;
-            const bool first = (it == c * Cfg::CH);
-            wgmma_fence();
-            if (dup) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {            // 64 pixels = 4 x k16: 16 rows of 128 B = 2048 B per step
-                    const uint32_t ko = k * 2048;
-                    // [hi | lo] x [hi | lo]^T: warpgroup w takes the rows of plane w
-                    wgmma_m64n128k16<1, 1>(chk, gmma_desc_mn_sw128(a0 + wg * Cfg::SLICE + ko), gmma_desc_mn_sw128(a0 + ko),
-                                           (first && k == 0) ? 0u : 1u);
-                }
-            } else {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint32_t ko = k * 2048;
-                    const uint64_t a_hi = gmma_desc_mn_sw128(a0 + wg * Cfg::SLICE + ko);
-                    const uint64_t a_lo = gmma_desc_mn_sw128(a0 + 2 * Cfg::SLICE + wg * Cfg::SLICE + ko);
-                    const uint64_t b_hi = gmma_desc_mn_sw128(b0 + ko);
-                    const uint64_t b_lo = gmma_desc_mn_sw128(b0 + 2 * Cfg::SLICE + ko);
-                    wgmma_m64n128k16<1, 1>(chk, a_hi, b_lo, (first && k == 0) ? 0u : 1u);
-                    wgmma_m64n128k16<1, 1>(chk, a_lo, b_hi, 1u);
-                    wgmma_m64n128k16<1, 1>(chk, a_hi, b_hi, 1u);
-                }
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            acc_fence(chk);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[s]);
         }
+        fence_proxy_async();                                   // generic-proxy writes -> visible to the tensor core
+        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // the whole tile is centred
+        const uint32_t a0 = smem_u32(st);
+        const uint32_t b0 = diag ? a0 : a0 + Cfg::OPER;
+        wgmma_fence();
+        if (dup) {
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] += chk[i];
+            for (int k = 0; k < 4; ++k) {            // 64 pixels = 4 x k16: 16 rows of 128 B = 2048 B per step
+                const uint32_t ko = k * 2048;
+                // [hi | lo] x [hi | lo]^T: warpgroup w takes the rows of plane w
+                wgmma_m64n128k16<1, 1>(chk, gmma_desc_mn_sw128(a0 + wg * Cfg::SLICE + ko), gmma_desc_mn_sw128(a0 + ko),
+                                       (first && k == 0) ? 0u : 1u);
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint32_t ko = k * 2048;
+                const uint64_t a_hi = gmma_desc_mn_sw128(a0 + wg * Cfg::SLICE + ko);
+                const uint64_t a_lo = gmma_desc_mn_sw128(a0 + 2 * Cfg::SLICE + wg * Cfg::SLICE + ko);
+                const uint64_t b_hi = gmma_desc_mn_sw128(b0 + ko);
+                const uint64_t b_lo = gmma_desc_mn_sw128(b0 + 2 * Cfg::SLICE + ko);
+                wgmma_m64n128k16<1, 1>(chk, a_hi, b_lo, (first && k == 0) ? 0u : 1u);
+                wgmma_m64n128k16<1, 1>(chk, a_lo, b_hi, 1u);
+                wgmma_m64n128k16<1, 1>(chk, a_hi, b_hi, 1u);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(chk);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+        if (++s == nst) { s = 0; ph ^= 1u; }
+    };
+    if constexpr (!MASK) {
+        int it = 0;
+        for (int c = 0; c < nchunks; ++c) {
+            float chk[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) chk[i] = 0.f;
+            const int it_end = min(ntiles, (c + 1) * Cfg::CH);
+            for (; it < it_end; ++it, ++tx) {
+                if (tx == p.tiles_x) { tx = 0; ++ty; }
+                tile(chk, it == c * Cfg::CH);
+            }
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] += chk[i];
+        }
+    } else {
+        // chunks of CH tiles of THIS region (the tiles without it are skipped): with every label equal to the region the
+        // chunks, and so the rounding, are those of the unmasked kernel
+        float chk[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) chk[i] = 0.f;
+        int done = 0;
+        for (int it = 0; it < ntiles; ++it, ++tx) {
+            if (tx == p.tiles_x) { tx = 0; ++ty; }
+            if (!((tmask[t0 + it] >> reg) & 1u)) continue;
+            tile(chk, done == 0);
+            if (++done == Cfg::CH) {
+#pragma unroll
+                for (int i = 0; i < 64; ++i) acc[i] += chk[i];
+                done = 0;
+            }
+        }
+        if (done) {
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] += chk[i];
+        }
     }
     // ---- this CTA's partial block -> its own slot.  Fragment: rows m, m + 8; columns 8j + 2 (lane & 3) (+1) ----
     const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2);
@@ -258,9 +313,9 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
                 const int mm = m + 8 * h, col = 8 * j + cl;
                 float* dst;
                 if (dup)   // rows m and m+64 both belong to channel m & 63, columns j and 64+j to channel j: quadrant -> slot
-                    dst = p.part + (((long long)img * p.nslots + split * 4 + (mm >> 6) * 2 + (col >> 6)) * p.C + (mm & 63)) * p.C + (col & 63);
+                    dst = p.part + (((long long)prob * p.nslots + split * 4 + (mm >> 6) * 2 + (col >> 6)) * p.C + (mm & 63)) * p.C + (col & 63);
                 else
-                    dst = p.part + (((long long)img * p.nslots + split) * p.C + bi * 128 + mm) * p.C + bj * 128 + col;
+                    dst = p.part + (((long long)prob * p.nslots + split) * p.C + bi * 128 + mm) * p.C + bj * 128 + col;
                 *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
             }
         }
@@ -279,65 +334,101 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
             float a = 0.f;
 #pragma unroll
             for (int r = 0; r < 32; ++r) a += red[r * 128 + ct];
-            p.psum[((long long)img * p.ksplit + split) * p.C + (dup ? 0 : bi * 128) + ct] = a;
+            p.psum[((long long)prob * p.ksplit + split) * p.C + (dup ? 0 : bi * 128) + ct] = a;
         }
     }
 }
 
 // shift[n][c] = mean of <= ~1024 strided interior pixels (all pixels when HW <= 1024): fixed-order reduction.
 // grid (C/64, N): one CTA per 64 channels of an image (a single CTA per image took 180 us at C = 512);
-// 256 threads = 8 channel groups x 32 pixel lanes
+// 256 threads = 8 channel groups x 32 pixel lanes.
+// MASK (spatial control): grid (C/64, N*R); problem z = n*R + r takes the mean of the sampled pixels labelled r, or of the
+// whole sample when it holds none of them.  A frame-wide shift alone is not enough: a region mean far from t cancels in
+// S - s s^T / n.  With every label equal to r the additions are those of the unmasked kernel.
+template <bool MASK>
 __global__ void __launch_bounds__(256)
-k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __restrict__ shift) {
+k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __restrict__ shift, const uint8_t* __restrict__ labels,
+               int R) {
     __shared__ float red[32][64];
+    __shared__ float red_all[MASK ? 32 : 1][64];
+    __shared__ int red_n[MASK ? 32 : 1];
     const int grp = threadIdx.x & 7, rl = threadIdx.x >> 3;
     const int c0 = blockIdx.x * 64 + grp * 8;
-    const int n = blockIdx.y;
+    const int n = MASK ? blockIdx.y / R : blockIdx.y;
+    const int reg = MASK ? blockIdx.y - n * R : 0;
     const long long HW = (long long)g.H * g.W;
     const long long ns = (HW + stride - 1) / stride;
-    float s[8];
+    float s[8], sa[8];
+    int cnt = 0;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s[j] = 0.f;
+    for (int j = 0; j < 8; ++j) { s[j] = 0.f; sa[j] = 0.f; }
 #pragma unroll 4
     for (long long k = rl; k < ns; k += 32) {
         const long long q = k * stride;
         const int y = (int)(q / g.W), x = (int)(q - (long long)y * g.W);
         float v[8];
         load8(act, g, ((long long)n * g.Hp + y + 1) * g.Wp + x + 1, c0, v);
+        if (MASK) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) sa[j] += v[j];
+            if (labels[(long long)n * HW + q] != reg) continue;
+            ++cnt;
+        }
 #pragma unroll
         for (int j = 0; j < 8; ++j) s[j] += v[j];
     }
 #pragma unroll
-    for (int j = 0; j < 8; ++j) red[rl][grp * 8 + j] = s[j];
+    for (int j = 0; j < 8; ++j) {
+        red[rl][grp * 8 + j] = s[j];
+        if (MASK) red_all[rl][grp * 8 + j] = sa[j];
+    }
+    if (MASK && grp == 0) red_n[rl] = cnt;
     __syncthreads();
     if (threadIdx.x < 64) {
-        float a = 0.f;
+        float a = 0.f, aa = 0.f;
+        int m = 0;
 #pragma unroll
-        for (int r = 0; r < 32; ++r) a += red[r][threadIdx.x];
-        shift[(long long)n * g.C + blockIdx.x * 64 + threadIdx.x] = a / (float)ns;
+        for (int r = 0; r < 32; ++r) {
+            a += red[r][threadIdx.x];
+            if (MASK) { aa += red_all[r][threadIdx.x]; m += red_n[r]; }
+        }
+        float t = a / (float)ns;
+        if (MASK) t = m > 0 ? a / (float)m : aa / (float)ns;
+        shift[(long long)blockIdx.y * g.C + blockIdx.x * 64 + threadIdx.x] = t;
     }
 }
 
 // dsum[n][c] = sum over splits of psum (fp64, fixed order); mean = shift + dsum / HW
+// (spatial control: `counts` [problems] replaces HW; a problem without pixels keeps its shift as the mean)
 __global__ void k_cov_sums(const float* __restrict__ psum, const float* __restrict__ shift, int C, int ksplit, long long HW,
-                           int total, double* __restrict__ dsum, float* __restrict__ mean) {
+                           int total, double* __restrict__ dsum, float* __restrict__ mean, const int* __restrict__ counts = nullptr) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const int n = i / C, c = i - n * C;
+    const long long cnt = counts ? (long long)counts[n] : HW;
     double a = 0.0;
     for (int s = 0; s < ksplit; ++s) a += (double)psum[((long long)n * ksplit + s) * C + c];
     dsum[i] = a;
-    mean[i] = (float)((double)shift[i] + a / (double)HW);
+    mean[i] = cnt > 0 ? (float)((double)shift[i] + a / (double)cnt) : shift[i];
 }
 
 // G = (sum_slots part - s s^T / HW) / (HW - 1) + eps_cov * I   (ops.py:45,50,108,121), exactly symmetric
+// (spatial control: `counts` [problems] replaces HW; a problem with fewer than 2 pixels gets G = I, a well-posed
+//  placeholder whose transform is never applied)
 __global__ void k_cov_finalize(const float* __restrict__ part, const double* __restrict__ dsum, int C, int nslots, long long HW,
-                               float eps_cov, int count, float* __restrict__ G, float* __restrict__ A0) {
+                               float eps_cov, int count, float* __restrict__ G, float* __restrict__ A0,
+                               const int* __restrict__ counts = nullptr) {
     const long long total = (long long)count * C * C;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
         const int j = (int)(t % C);
         const int i = (int)((t / C) % C);
         const long long n = t / ((long long)C * C);
+        if (counts && counts[n] < 2) {
+            G[t] = i == j ? 1.f : 0.f;
+            if (A0) A0[t] = G[t];
+            continue;
+        }
+        const long long cnt = counts ? (long long)counts[n] : HW;
         // every (min,max) entry lies in a stored upper block: reading it for both (i,j) and (j,i) makes G exactly symmetric
         const long long e = (i <= j) ? (long long)i * C + j : (long long)j * C + i;
         const float* pp = part + n * nslots * (long long)C * C + e;
@@ -353,8 +444,8 @@ __global__ void k_cov_finalize(const float* __restrict__ part, const double* __r
         }
         for (; s < nslots; ++s) v0 += (double)pp[(long long)s * cc];
         double v = (v0 + v1) + (v2 + v3);
-        v -= dsum[n * C + i] * dsum[n * C + j] / (double)HW;
-        float r = (float)(v / (double)(HW - 1));
+        v -= dsum[n * C + i] * dsum[n * C + j] / (double)cnt;
+        float r = (float)(v / (double)(cnt - 1));
         if (i == j) r += eps_cov;
         G[t] = r;
         if (A0) A0[t] = r;          // pristine copy: the Jacobi kernel overwrites G, the Rayleigh quotients need A
@@ -370,7 +461,11 @@ int g_cov_max_stages = 12;   // probe knob (wctb200_debug_set_cov_stages)
 
 // Means and covariance (+ eps_cov I) of a feature batch: mean [N][C], G [N][C][C] (and a copy A0 if not null), fp32.
 // dsum: [N][C] fp64 scratch (caller's workspace); partial products live in the per-stream scratch cache.
-int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, float* G, float* A0, double* dsum, cudaStream_t st) {
+// Spatial control (labels != nullptr): one problem per (image, region), z = n * R + r, over the pixels labelled r:
+// outputs [N*R][...]; counts [N*R] = pixels per problem and tmask [N][tiles] = regions present per 32 x 2 tile
+// (k_region_scan, wct.cu).
+static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mean, float* G, float* A0, double* dsum,
+                         const uint8_t* labels, int R, const int* counts, const uint16_t* tmask, cudaStream_t st) {
     static PFN_encodeTiledC enc = nullptr;
     if (!enc) {
         void* ptr = nullptr;
@@ -384,6 +479,8 @@ int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, fl
     }
     WCTB_REQUIRE(g.C == 64 || (g.C % 128 == 0 && g.C <= 2048), "covariance: C=%d must be 64 or a multiple of 128 (<= 2048)", g.C);
     const long long HW = (long long)g.H * g.W;
+    const bool masked = labels != nullptr;
+    const int nprob = masked ? g.N * R : g.N;
     CovParams p;
     p.C = g.C; p.W = g.W; p.H = g.H; p.N = g.N;
     p.tiles_x = (g.W + 31) / 32;
@@ -399,9 +496,9 @@ int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, fl
     p.tiles_per_split = tps;
     p.ksplit = (tiles_img + tps - 1) / tps;
     p.nslots = g.C == 64 ? 4 * p.ksplit : p.ksplit;
-    // scratch: shift [N][C] | psum [N][ksplit][C] | part [N][nslots][C][C]
-    const size_t n_shift = (size_t)g.N * g.C, n_psum = (size_t)g.N * p.ksplit * g.C;
-    const size_t n_part = (size_t)g.N * p.nslots * g.C * g.C;
+    // scratch: shift [P][C] | psum [P][ksplit][C] | part [P][nslots][C][C]   (P problems)
+    const size_t n_shift = (size_t)nprob * g.C, n_psum = (size_t)nprob * p.ksplit * g.C;
+    const size_t n_part = (size_t)nprob * p.nslots * g.C * g.C;
     float* scratch = nullptr;
     { int rc0 = scratch_alloc(reinterpret_cast<void**>(&scratch), (n_shift + n_psum + n_part + 64) * sizeof(float), st, 0); if (rc0) return rc0; }
     float* shift = scratch;
@@ -410,10 +507,14 @@ int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, fl
     p.shift = shift; p.psum = psum; p.part = part;
     p.err = device_error_word();
     p.max_stages = g_cov_max_stages;
+    p.labels = labels;
+    p.tmask = tmask;
+    p.R = masked ? R : 1;
     // (blocks below the diagonal are never written -- and never read: k_cov_finalize only touches (min,max) entries)
 
     const int stride = HW <= 1024 ? 1 : (int)(HW / 1024);
-    k_sample_shift<<<dim3((unsigned)(g.C / 64), (unsigned)g.N), 256, 0, st>>>(act, g, stride, shift);
+    if (masked) k_sample_shift<true><<<dim3((unsigned)(g.C / 64), (unsigned)nprob), 256, 0, st>>>(act, g, stride, shift, labels, R);
+    else k_sample_shift<false><<<dim3((unsigned)(g.C / 64), (unsigned)g.N), 256, 0, st>>>(act, g, stride, shift, nullptr, 1);
     WCTB_CHECK_LAUNCH("k_sample_shift");
 
     // tensor map over the interior pixels only (see header comment)
@@ -431,17 +532,30 @@ int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, fl
         set_error("cov_tc: cuTensorMapEncodeTiled failed (%d)", (int)r);
         return WCTB200_ECUDA;
     }
-    WCTB_ENSURE_SMEM(cov_tc_kernel, CovCfg::SMEM_BYTES);
-    dim3 grid((unsigned)(npairs * p.ksplit), (unsigned)g.N);
-    cov_tc_kernel<<<grid, CovCfg::THREADS, CovCfg::SMEM_BYTES, st>>>(mX, p);
+    dim3 grid((unsigned)(npairs * p.ksplit), (unsigned)nprob);
+    if (masked) {
+        WCTB_ENSURE_SMEM(cov_tc_kernel<true>, CovCfg::SMEM_BYTES);
+        cov_tc_kernel<true><<<grid, CovCfg::THREADS, CovCfg::SMEM_BYTES, st>>>(mX, p);
+    } else {
+        WCTB_ENSURE_SMEM(cov_tc_kernel<false>, CovCfg::SMEM_BYTES);
+        cov_tc_kernel<false><<<grid, CovCfg::THREADS, CovCfg::SMEM_BYTES, st>>>(mX, p);
+    }
     WCTB_CHECK_LAUNCH("cov_tc_kernel");
-    k_cov_sums<<<cdiv((long long)g.N * g.C, 256), 256, 0, st>>>(psum, shift, g.C, p.ksplit, HW, g.N * g.C, dsum, mean);
+    k_cov_sums<<<cdiv((long long)nprob * g.C, 256), 256, 0, st>>>(psum, shift, g.C, p.ksplit, HW, nprob * g.C, dsum, mean, counts);
     WCTB_CHECK_LAUNCH("k_cov_sums");
-    const long long tot = (long long)g.N * g.C * g.C;
+    const long long tot = (long long)nprob * g.C * g.C;
     k_cov_finalize<<<(unsigned)(cdiv(tot, 256) > 4096 ? 4096 : cdiv(tot, 256)), 256, 0, st>>>(part, dsum, g.C, p.nslots, HW,
-                                                                                               eps_cov, g.N, G, A0);
+                                                                                               eps_cov, nprob, G, A0, counts);
     WCTB_CHECK_LAUNCH("k_cov_finalize");
     return 0;
+}
+
+int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, float* G, float* A0, double* dsum, cudaStream_t st) {
+    return mean_cov_impl(act, g, eps_cov, mean, G, A0, dsum, nullptr, 1, nullptr, nullptr, st);
+}
+int launch_mean_cov_regions(const __half* act, ActGeom g, const uint8_t* labels, int R, const int* counts, const uint16_t* tmask,
+                            float eps_cov, float* mean, float* G, float* A0, double* dsum, cudaStream_t st) {
+    return mean_cov_impl(act, g, eps_cov, mean, G, A0, dsum, labels, R, counts, tmask, st);
 }
 
 }  // namespace wctb

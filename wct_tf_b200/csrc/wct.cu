@@ -477,12 +477,12 @@ __global__ void k_eig_post(const float* __restrict__ Gall, const float* __restri
 __global__ void __launch_bounds__(256)
 k_outer_gemm(const float* __restrict__ A, long long sa, const float* __restrict__ B, long long sb,
              const float* __restrict__ d, long long sd, float* __restrict__ Cm, long long sc, int n,
-             const int* __restrict__ skip = nullptr) {
+             const int* __restrict__ skip = nullptr, int amod = 0) {
     if (skip && skip[blockIdx.z]) return;      // this output was produced by the matrix-function fast path
     __shared__ __align__(16) float As[16][64];
     __shared__ __align__(16) float Bs[16][64];
     const int z = blockIdx.z;
-    const float* a = A + (long long)z * sa;
+    const float* a = A + (long long)(amod ? z % amod : z) * sa;     // amod: A cycles through amod matrices (regions: style z % R)
     const float* b = B + (long long)z * sb;
     const float* dd = d ? d + (long long)z * sd : nullptr;
     const int i0 = blockIdx.x * 64, j0 = blockIdx.y * 64;
@@ -525,7 +525,7 @@ k_outer_gemm(const float* __restrict__ A, long long sa, const float* __restrict_
 
 // M = alpha*T + (1-alpha)*I  -> split-fp16 GEMM operand [frame][2][C][C] (row = output channel)
 // bias = alpha*ms - M*mc + (1-alpha)*readd*mc                       (ops.py:80-83 / 131-133)
-//   one warp per (frame, output channel)
+//   one warp per (frame, output channel); style mean z % Ns (Ns == 1: shared; regions: problem z = frame*R + r, Ns = R)
 __global__ void k_finalize_transform(const float* __restrict__ T, int C, int Nc, int Ns, float alpha, int readd,
                                      const float* __restrict__ mean_c, const float* __restrict__ mean_s,
                                      __half* __restrict__ Msplit, float* __restrict__ bias) {
@@ -535,7 +535,7 @@ __global__ void k_finalize_transform(const float* __restrict__ T, int C, int Nc,
     if (row >= C) return;
     const float* t = T + ((long long)z * C + row) * C;
     const float* mc = mean_c + (long long)z * C;
-    const float* ms = mean_s + (long long)(Ns == 1 ? 0 : z) * C;
+    const float* ms = mean_s + (long long)(Ns == 1 ? 0 : z % Ns) * C;
     __half* mh = Msplit + (((long long)z * 2 + 0) * C + row) * C;
     __half* ml = Msplit + (((long long)z * 2 + 1) * C + row) * C;
     float dot = 0.f;
@@ -933,6 +933,229 @@ int launch_adain_level(const __half* content, int Nc, int Hc, int Wc, const __ha
     k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(content, gc, scale, shift, out);
     WCTB_CHECK_LAUNCH("k_affine_apply");
     return 0;
+}
+
+// ---------------------------------------------------------------------------
+// Spatial control (WCT paper, section 4): a label map splits every frame into regions and region r takes style r.  Per
+// (frame, region) the transform is the reference's own, restricted to the region's pixels; labels >= R, and regions with
+// fewer than 2 pixels at a level, keep the content feature.
+// ---------------------------------------------------------------------------
+// proportional nearest sampling of an Hm x Wm label map onto an Hf x Wf grid, integer arithmetic (no divisibility needed):
+//   dst[y][x] = src[((2y+1) Hm) / (2 Hf)][((2x+1) Wm) / (2 Wf)]
+__global__ void k_labels_resize(const uint8_t* __restrict__ src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* __restrict__ dst) {
+    const long long total = (long long)N * Hf * Wf;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % Wf);
+        const long long t = i / Wf;
+        const int y = (int)(t % Hf);
+        const int n = (int)(t / Hf);
+        const int sy = (int)(((2ll * y + 1) * Hm) / (2ll * Hf)), sx = (int)(((2ll * x + 1) * Wm) / (2ll * Wf));
+        dst[i] = src[((long long)n * Hm + sy) * Wm + sx];
+    }
+}
+int launch_labels_resize(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, cudaStream_t st) {
+    const long long total = (long long)N * Hf * Wf;
+    long long blocks = (total + 255) / 256;
+    if (blocks > device_sm_count() * 16ll) blocks = device_sm_count() * 16ll;
+    k_labels_resize<<<(unsigned)blocks, 256, 0, st>>>(src, N, Hm, Wm, Hf, Wf, dst);
+    WCTB_CHECK_LAUNCH("k_labels_resize");
+    return 0;
+}
+
+// one warp per 32 x 2 covariance tile (cov_tc.cu): tmask[n][tile] = regions present (bit r, r < R), counts[n*R + r] += pixels
+// (integer counts: order-independent).  grid (cdiv(tiles, 8), N), 256 threads.  counts must be zeroed.
+__global__ void __launch_bounds__(256)
+k_region_scan(const uint8_t* __restrict__ labels, int H, int W, int R, int tiles_x, int tiles, int* __restrict__ counts,
+              uint16_t* __restrict__ tmask) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int t = blockIdx.x * 8 + warp, n = blockIdx.y;
+    if (t >= tiles) return;
+    const int ty = t / tiles_x, tx = t - ty * tiles_x;
+    const int x = tx * 32 + lane;
+    int l[2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        const int y = ty * 2 + k;
+        l[k] = (x < W && y < H) ? labels[((long long)n * H + y) * W + x] : 255;
+    }
+    unsigned bits = 0;
+    for (int r = 0; r < R; ++r) {
+        const int c = __popc(__ballot_sync(0xffffffffu, l[0] == r)) + __popc(__ballot_sync(0xffffffffu, l[1] == r));
+        if (c) {
+            bits |= 1u << r;
+            if (lane == 0) atomicAdd(&counts[n * R + r], c);
+        }
+    }
+    if (lane == 0) tmask[(long long)n * tiles + t] = (uint16_t)bits;
+}
+
+// per 128-position tile of the regions apply (conv_tc.cu, per-image tiling over the padded plane): bit r for every region
+// whose pixels the tile transforms, bit R when it holds a pixel that keeps its input.  One warp per tile.
+__global__ void __launch_bounds__(256)
+k_region_apply_tiles(const uint8_t* __restrict__ labels, const int* __restrict__ counts, int N, int H, int W, int R,
+                     int tiles_per_image, uint16_t* __restrict__ amask) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long t = (long long)blockIdx.x * 8 + warp;
+    if (t >= (long long)N * tiles_per_image) return;
+    const int n = (int)(t / tiles_per_image), mt = (int)(t - (long long)n * tiles_per_image);
+    const int Wp = W + 2;
+    const long long HpWp = (long long)(H + 2) * Wp;
+    unsigned bits = 0;
+    for (int k = lane; k < 128; k += 32) {
+        const long long r = (long long)mt * 128 + k;
+        if (r >= HpWp) break;
+        const int yy = (int)(r / Wp), xx = (int)(r - (long long)yy * Wp);
+        if (yy < 1 || yy > H || xx < 1 || xx > W) continue;
+        const int l = labels[((long long)n * H + yy - 1) * W + xx - 1];
+        bits |= 1u << ((l < R && counts[n * R + l] >= 2) ? l : R);
+    }
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    if (lane == 0) amask[t] = (uint16_t)bits;
+}
+
+// k_out of the regions apply: [k_c x Nc*R | k_s x R | sweeps_c x Nc*R | sweeps_s x R], k_c = -1 for a skipped (frame, region)
+__global__ void k_regions_kout(const int* __restrict__ kc, const int* __restrict__ counts, const int* __restrict__ ks, int np, int R,
+                               int32_t* __restrict__ k_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < np) {
+        k_out[i] = counts[i] < 2 ? -1 : kc[i];
+        k_out[np + R + i] = counts[i] < 2 ? 0 : kc[np + i];
+    }
+    if (i < R) {
+        k_out[np + i] = ks[2 * i];
+        k_out[2 * np + R + i] = ks[2 * i + 1];
+    }
+}
+
+struct RegionWs {
+    size_t base, mean_s, Cs, ks, counts, tmask, amask, total;
+    int tiles_x, tiles, tiles_per_image;
+};
+static RegionWs regions_layout(int C, int Nc, int R, int Hc, int Wc) {
+    RegionWs L;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.tiles_x = (Wc + 31) / 32;
+    L.tiles = L.tiles_x * ((Hc + 1) / 2);
+    L.tiles_per_image = cdiv((long long)(Hc + 2) * (Wc + 2), 128);
+    L.base = take(wct_layout(C, Nc * R, 0).total);   // the per-(frame, region) transform, as wct_apply's for Nc*R frames
+    L.mean_s = take((size_t)R * C * 4);                // the R style states, gathered
+    L.Cs = take((size_t)R * C * C * 4);
+    L.ks = take((size_t)R * 2 * 4);
+    L.counts = take((size_t)Nc * R * 4);
+    L.tmask = take((size_t)Nc * L.tiles * 2);
+    L.amask = take((size_t)Nc * L.tiles_per_image * 2);
+    L.total = o;
+    return L;
+}
+size_t wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc) { return regions_layout(C, Nc, R, Hc, Wc).total; }
+
+int launch_mean_cov_regions(const __half* act, ActGeom g, const uint8_t* labels, int R, const int* counts, const uint16_t* tmask,
+                            float eps_cov, float* mean, float* G, float* A0, double* dsum, cudaStream_t st);
+int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias,
+                              const uint8_t* labels, const int* counts, const uint16_t* amask, int R, __half* out, cudaStream_t st);
+
+static int region_scan(const uint8_t* labels, int N, int H, int W, int R, int* counts, uint16_t* tmask, cudaStream_t st) {
+    const int tiles_x = (W + 31) / 32, tiles = tiles_x * ((H + 1) / 2);
+    WCTB_CUDA(cudaMemsetAsync(counts, 0, (size_t)N * R * 4, st));
+    k_region_scan<<<dim3((unsigned)cdiv(tiles, 8), (unsigned)N), 256, 0, st>>>(labels, H, W, R, tiles_x, tiles, counts, tmask);
+    WCTB_CHECK_LAUNCH("k_region_scan");
+    return 0;
+}
+
+int launch_wct_apply_regions(const __half* content, int Nc, int Hc, int Wc, int C, const uint8_t* labels, int R,
+                             const void* const* states, float alpha, float eps_cov, float eps_eig, float thresh, int readd,
+                             __half* out, int32_t* k_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_apply_regions: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(R >= 1 && R <= 8, "wct_apply_regions: R=%d not in 1..8", R);
+    const RegionWs RL = regions_layout(C, Nc, R, Hc, Wc);
+    if (ws_bytes < RL.total) {
+        set_error("wct_apply_regions: workspace %zu < %zu bytes", ws_bytes, RL.total);
+        return WCTB200_EWS;
+    }
+    const int np = Nc * R;
+    const WctWs L = wct_layout(C, np, 0);
+    uint8_t* w = static_cast<uint8_t*>(ws) + RL.base;
+    uint8_t* rw = static_cast<uint8_t*>(ws);
+    float* mean_s = reinterpret_cast<float*>(rw + RL.mean_s);
+    float* Cs = reinterpret_cast<float*>(rw + RL.Cs);
+    int* ks = reinterpret_cast<int*>(rw + RL.ks);
+    int* counts = reinterpret_cast<int*>(rw + RL.counts);
+    uint16_t* tmask = reinterpret_cast<uint16_t*>(rw + RL.tmask);
+    uint16_t* amask = reinterpret_cast<uint16_t*>(rw + RL.amask);
+    double* dsum = reinterpret_cast<double*>(w + L.dsum);
+    float* mean = reinterpret_cast<float*>(w + L.mean);
+    float* G = reinterpret_cast<float*>(w + L.G);
+    float* sigma = reinterpret_cast<float*>(w + L.sigma);
+    float* dvec = reinterpret_cast<float*>(w + L.dvec);
+    float* Wcm = reinterpret_cast<float*>(w + L.Wc);
+    float* T = reinterpret_cast<float*>(w + L.T);
+    __half* Msplit = reinterpret_cast<__half*>(w + L.Msplit);
+    float* bias = reinterpret_cast<float*>(w + L.bias);
+    float* conv = reinterpret_cast<float*>(w + L.conv);
+    int* kc = reinterpret_cast<int*>(w + L.kcount);
+    float* A0 = reinterpret_cast<float*>(w + L.A0);
+    float* lam = reinterpret_cast<float*>(w + L.lam);
+    int* ok = reinterpret_cast<int*>(w + L.ok);
+    const long long CC = (long long)C * C;
+    // gather the R style states (each from wct_style_prepare with Ns = 1: [C] mean_s | [C][C] C_s | k_s, sweeps)
+    size_t off_cs, off_k;
+    style_state_offsets(C, 1, &off_cs, &off_k);
+    for (int r = 0; r < R; ++r) {
+        WCTB_REQUIRE(states[r], "wct_apply_regions: style state %d is null", r);
+        const uint8_t* sp = static_cast<const uint8_t*>(states[r]);
+        WCTB_CUDA(cudaMemcpyAsync(mean_s + (long long)r * C, sp, (size_t)C * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(Cs + r * CC, sp + off_cs, (size_t)CC * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(ks + 2 * r, sp + off_k, 2 * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)np * 2 * 4, st));
+    int rc = region_scan(labels, Nc, Hc, Wc, R, counts, tmask, st);
+    if (rc) return rc;
+    // per (frame, region): masked covariance; then the content side of wct_apply over Nc*R matrices, style z % R
+    rc = launch_mean_cov_regions(content, ActGeom(Nc, Hc, Wc, C), labels, R, counts, tmask, eps_cov, mean, G, A0, dsum, st);
+    if (rc) return rc;
+    rc = launch_matfun_ns(A0, C, np, /*n_first=*/np, thresh, eps_eig, Wcm, ok, kc, st);
+    if (rc < 0) return rc;
+    rc = launch_jacobi(G, C, np, conv, kc + np, st, ok);
+    if (rc) return rc;
+    rc = launch_eig_post(G, A0, lam, C, np, thresh, eps_eig, np, sigma, dvec, kc, st, ok);
+    if (rc) return rc;
+    dim3 gg((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)np);
+    k_outer_gemm<<<gg, 256, 0, st>>>(G, CC, G, CC, dvec, C, Wcm, CC, C, ok);
+    WCTB_CHECK_LAUNCH("k_outer_gemm(Wc)");
+    k_outer_gemm<<<gg, 256, 0, st>>>(Cs, CC, Wcm, CC, nullptr, 0, T, CC, C, nullptr, R);   // T = C_s(z % R) W_c(z)
+    WCTB_CHECK_LAUNCH("k_outer_gemm(T)");
+    dim3 gf((unsigned)cdiv(C, 8), (unsigned)np);
+    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, np, R, alpha, readd, mean, mean_s, Msplit, bias);
+    WCTB_CHECK_LAUNCH("k_finalize_transform");
+    // out = M_{n,r} x + bias_{n,r} per pixel of region r; every other pixel keeps its input bytes
+    const long long napply = (long long)Nc * RL.tiles_per_image;
+    k_region_apply_tiles<<<(unsigned)cdiv(napply, 8), 256, 0, st>>>(labels, counts, Nc, Hc, Wc, R, RL.tiles_per_image, amask);
+    WCTB_CHECK_LAUNCH("k_region_apply_tiles");
+    rc = launch_conv_apply_regions(content, Nc, Hc, Wc, C, Msplit, bias, labels, counts, amask, R, out, st);
+    if (rc) return rc;
+    if (k_out) {
+        k_regions_kout<<<(unsigned)cdiv(np > R ? np : R, 256), 256, 0, st>>>(kc, counts, ks, np, R, k_out);
+        WCTB_CHECK_LAUNCH("k_regions_kout");
+    }
+    return 0;
+}
+
+// test hook: means, covariances (+ eps_cov I) and pixel counts per (image, region): mean [N*R][C], cov [N*R][C][C],
+// counts [N*R]; a region with fewer than 2 pixels gets cov = I
+int launch_covariance_regions(const __half* act, int N, int H, int W, int C, const uint8_t* labels, int R, float eps_cov,
+                              float* mean_out, float* cov_out, int* counts, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || (C % 128 == 0 && C >= 128), "covariance_regions: C=%d must be 64 or a multiple of 128", C);
+    WCTB_REQUIRE(R >= 1 && R <= 8, "covariance_regions: R=%d not in 1..8", R);
+    const int tiles = ((W + 31) / 32) * ((H + 1) / 2);
+    uint8_t* scratch = nullptr;
+    const size_t dsum_bytes = align_up((size_t)N * R * C * sizeof(double), 256);
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&scratch), dsum_bytes + (size_t)N * tiles * 2, st, 1); if (rc0) return rc0; }
+    double* dsum = reinterpret_cast<double*>(scratch);
+    uint16_t* tmask = reinterpret_cast<uint16_t*>(scratch + dsum_bytes);
+    int rc = region_scan(labels, N, H, W, R, counts, tmask, st);
+    if (rc) return rc;
+    return launch_mean_cov_regions(act, ActGeom(N, H, W, C), labels, R, counts, tmask, eps_cov, mean_out, cov_out, nullptr, dsum, st);
 }
 
 // ---------------------------------------------------------------------------

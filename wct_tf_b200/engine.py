@@ -318,9 +318,38 @@ class Engine(object):
                    flops=2.0 * C * C * 2 * content.N * hwc, bytes_=4.0 * C * 2 * content.N * hwc)
         return out, kbuf
 
+    def labels_resize(self, labels, H, W):
+        """Device uint8 label maps [N,Hm,Wm] -> [N,H,W] by proportional nearest sampling (spatial control)."""
+        out = torch.empty((labels.shape[0], H, W), dtype=torch.uint8, device=self.device)
+        self._call("labels_resize", 1, self.lib.wctb200_labels_resize_nearest, labels.data_ptr(), labels.shape[0], labels.shape[1],
+                   labels.shape[2], H, W, out.data_ptr(), self._stream())
+        return out
+
+    def wct_apply_regions(self, content, labels, states, alpha, want_info=False):
+        """Spatial control on one level: region r of each frame (``labels`` [N,H,W] at the feature resolution) takes the
+        style whose state is ``states[r]``; labels >= R and regions of < 2 pixels keep the content feature."""
+        st = self._stream()
+        sem = SEMANTICS[self.semantics]
+        C, N, R = content.C, content.N, len(states)
+        out = self._act(N, content.H, content.W, C)
+        nbytes = self.lib.wctb200_wct_regions_workspace_bytes(C, N, R, content.H, content.W)
+        key = (self._group, "regions", C, N, R)        # grow-only: the levels of a call differ in H x W
+        ws = self._ws.get(key)
+        if ws is None or ws.numel() < nbytes:
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            self._ws[key] = ws
+        kbuf = torch.empty(2 * (N * R + R), dtype=torch.int32, device=self.device) if want_info else None
+        hwc = content.H * content.W
+        self._call("wct_regions[C%d]" % C, 12 + self._matfun_launches(C), self.lib.wctb200_wct_apply_regions, content.ptr, N,
+                   content.H, content.W, C, labels.data_ptr(), R, _capi.pointer_array([s.data_ptr() for s in states]),
+                   float(alpha), sem["eps_cov"], sem["eps_eig"], sem["thresh"], sem["readd"], out.ptr,
+                   kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel(), st,
+                   flops=2.0 * C * C * 2 * N * hwc, bytes_=4.0 * C * 2 * N * hwc)
+        return out, kbuf
+
     # ------------------------------------------------------------------ pipeline
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
-                ss_patch_size=3, ss_stride=1):
+                ss_patch_size=3, ss_stride=1, labels=None, region_styles=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3], Ns in {1, N}.
         Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -328,8 +357,25 @@ class Engine(object):
         With ``self.groups`` = G > 1 the batch is cut into G sub-batches whose level chains are
         enqueued on G independent stream pairs: frames are independent (wct.py:97-103), and the
         eigendecompositions are latency bound on a few SMs, so one group's Jacobi clusters overlap the
-        other groups' convolutions (same arithmetic per frame; only the schedule changes)."""
+        other groups' convolutions (same arithmetic per frame; only the schedule changes).
+
+        Spatial control: ``labels`` is a cuda uint8 label map [N|1,Hm,Wm] of any resolution and ``region_styles`` a list of
+        R (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes; ``style_u8`` is ignored.  At every level the map is resampled
+        to the feature grid and region r of a frame is transformed against style r (WCT only); labels >= R keep the
+        content feature.  The R styles are encoded and prepared once per call."""
         N = content_u8.shape[0]
+        if labels is not None:
+            if adain or swap5:
+                raise ValueError("spatial control (labels) works with WCT only: not with adain or swap5")
+            R = len(region_styles) if region_styles is not None else 0
+            if not 1 <= R <= 8:
+                raise ValueError("spatial control needs 1..8 region styles, got %d" % R)
+            if labels.dim() == 2:
+                labels = labels.unsqueeze(0)
+            if labels.dtype != torch.uint8 or labels.dim() != 3 or labels.shape[0] not in (1, N):
+                raise ValueError("labels must be uint8 [Hm,Wm] or [N,Hm,Wm]")
+            labels = labels.expand(N, -1, -1).contiguous()
+            return self._stylize_regions(content_u8, labels, list(region_styles), alpha, want_info, capture)
         swap5 = bool(swap5) and "relu5_1" in [l.relu_target for l in self.model.levels]    # model.py:148: only relu5_1 swaps
         if swap5:
             if N != 1 or style_u8.shape[0] != 1:
@@ -376,6 +422,46 @@ class Engine(object):
             return out
         return self._stylize_one(content_u8, style_u8, alpha, adain, want_info, capture)
 
+    def _stylize_regions(self, content_u8, labels, region_styles, alpha, want_info, capture):
+        """``stylize`` with a label map: the R style sides run once and are shared by every sub-batch group."""
+        N = content_u8.shape[0]
+        main = torch.cuda.current_stream(self.device)
+        G = min(self.groups, N) if (capture is None and not want_info) else 1
+        self._group = 1 if G > 1 else 0
+        try:
+            sides = [self._style_side(s, True, main) for s in region_styles]
+        finally:
+            self._group = 0
+        if G == 1:
+            out = self._stylize_one(content_u8, None, alpha, False, want_info, capture, region=(labels, sides))
+        else:
+            bounds = [(g * N) // G for g in range(G + 1)]
+            outs = []
+            for g in range(G):
+                if g not in self._group_streams:
+                    prio = -1 if (self.group_priorities and g == 0) else 0
+                    self._group_streams[g] = torch.cuda.Stream(device=self.device, priority=prio)
+                gs = self._group_streams[g]
+                gs.wait_stream(main)
+                self._group = g + 1
+                try:
+                    with torch.cuda.stream(gs):
+                        lo, hi = bounds[g], bounds[g + 1]
+                        outs.append(self._stylize_one(content_u8[lo:hi], None, alpha, False, False, None,
+                                                      region=(labels[lo:hi], sides)))
+                finally:
+                    self._group = 0
+            for g in range(G):
+                main.wait_stream(self._group_streams[g])
+            out = torch.cat(outs, dim=0)
+            for g in range(G):
+                self._group_streams[g].wait_stream(main)
+        for side in {id(sd["side"]): sd["side"] for sd in sides}.values():
+            if side is not main:
+                side.wait_stream(main)         # the style states are recycled only after every level used them
+                main.wait_stream(side)
+        return out
+
     def _style_side(self, style_u8, split, main):
         """Style side of one call (model.py:70-72: ONE encoder pass emitting every target; ops.py:48-55,76 per level when
         ``split``): enqueued on this group's style stream when overlap is on.  Returns the states / events / features."""
@@ -405,25 +491,37 @@ class Engine(object):
         return dict(states=states, events=events, feats=feats, side=side)
 
     def _stylize_one(self, content_u8, style_u8, alpha, adain, want_info, capture, swap5=False, ss_alpha=0.6, shared_style=None,
-                     ss_patch=3, ss_stride=1):
+                     ss_patch=3, ss_stride=1, region=None):
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
-        assert content_u8.dtype == torch.uint8 and style_u8.dtype == torch.uint8
-        assert style_u8.shape[0] in (1, N)
+        main = torch.cuda.current_stream(self.device)
+        if region is None:
+            assert content_u8.dtype == torch.uint8 and style_u8.dtype == torch.uint8
+            assert style_u8.shape[0] in (1, N)
         content = torch.empty(content_u8.shape, dtype=torch.float32, device=self.device)
         self._call("u8_to_f32", 1, lib.wctb200_image_u8_to_f32, content_u8.data_ptr(), content_u8.numel(), content.data_ptr(), st)
-        main = torch.cuda.current_stream(self.device)
         split = not adain and not swap5        # WCT: style side on its own stream; AdaIN / style swap: keep it inline
-        ss = shared_style if (shared_style is not None and split) else self._style_side(style_u8, split, main)
+        if region is not None:                 # spatial control: (labels [N,Hm,Wm], the R style sides of _stylize_regions)
+            labels, sides = region
+            ss = sides[0]
+            n_style = 1
+        else:
+            ss = shared_style if (shared_style is not None and split) else self._style_side(style_u8, split, main)
+            n_style = style_u8.shape[0]
         side, style_states, style_events, style_feats = ss["side"], ss["states"], ss["events"], ss["feats"]
         infos = []
         x = content
         nlev = len(self.model.levels)
-        n_style = style_u8.shape[0]
         for lvl in self.model.levels:
             self._tag = lvl.relu_target
             cf, _ = self.encode(x, lvl.relu_target)
-            if swap5 and lvl.relu_target == "relu5_1":     # model.py:148-152: style swap wins over AdaIN / WCT at relu5_1
+            if region is not None:
+                for sd in sides:
+                    if sd["side"] is not main:
+                        main.wait_event(sd["events"][lvl.relu_target])
+                lab = self.labels_resize(labels, cf.H, cf.W)
+                f, kbuf = self.wct_apply_regions(cf, lab, [sd["states"][lvl.relu_target] for sd in sides], alpha, want_info)
+            elif swap5 and lvl.relu_target == "relu5_1":     # model.py:148-152: style swap wins over AdaIN / WCT at relu5_1
                 f, kbuf = self.style_swap(cf, style_feats[lvl.relu_target], ss_alpha, want_info, ss_patch, ss_stride)
             elif split:
                 if side is not main:
@@ -441,7 +539,7 @@ class Engine(object):
             if capture is not None:
                 capture.setdefault("level_output", []).append(x)
         self._tag = None
-        if side is not main and shared_style is None:
+        if side is not main and shared_style is None and region is None:
             side.wait_stream(main)             # buffers handed across streams may be recycled only after both are done
             main.wait_stream(side)
         if want_info:

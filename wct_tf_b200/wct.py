@@ -8,7 +8,8 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``device`` accepts the reference's TF strings ('/gpu:0') and torch strings;
   * ``swap5=True`` (style-swap at relu5_1, ops.py:145-278) honours ``ss_patch_size`` / ``ss_stride``; with a stride the
     content is centre-cropped so that the patches tile its relu5_1 encoding, as wct.py:84-90 does;
-  * ``predict_batch`` is new: a batch of frames per call (frames are independent).
+  * ``predict_batch`` is new: a batch of frames per call (frames are independent);
+  * ``content_mask`` is new: spatial control (WCT paper, section 4), a label map whose region r takes style r.
 """
 from __future__ import annotations
 
@@ -66,8 +67,29 @@ class WCT(object):
         """wct.py:66-68"""
         return np.uint8(np.clip(image, 0, 1) * 255)
 
+    @staticmethod
+    def check_mask(content_mask, n_frames, styles):
+        """Host-side validation of a spatial-control call: uint8 mask [Hm,Wm] (shared) or [N,Hm,Wm], and a list of
+        1..8 uint8 [Hs,Ws,3] style images (one per region, any sizes).  Returns (mask as uint8 [1|N,Hm,Wm], styles)."""
+        m = content_mask.cpu() if isinstance(content_mask, torch.Tensor) else torch.from_numpy(np.asarray(content_mask))
+        if m.dtype != torch.uint8:
+            raise ValueError("content_mask must be uint8, got %s" % (m.dtype,))
+        if m.dim() == 2:
+            m = m.unsqueeze(0)
+        if m.dim() != 3 or m.shape[0] not in (1, n_frames) or m.shape[1] < 1 or m.shape[2] < 1:
+            raise ValueError("content_mask must be [Hm,Wm] or [N,Hm,Wm] with N = %d frames, got %s" % (n_frames, tuple(m.shape)))
+        if isinstance(styles, (np.ndarray, torch.Tensor)) and styles.ndim == 3:
+            styles = [styles]
+        styles = list(styles)
+        if not 1 <= len(styles) <= 8:
+            raise ValueError("a content mask needs 1..8 region styles, got %d" % len(styles))
+        for s in styles:
+            if s.dtype not in (np.uint8, torch.uint8) or s.ndim not in (3, 4) or s.shape[-1] != 3 or (s.ndim == 4 and s.shape[0] != 1):
+                raise ValueError("each region style must be one uint8 [Hs,Ws,3] image")
+        return m.contiguous(), styles
+
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
-                      passes=1, return_device=False):
+                      passes=1, return_device=False, content_mask=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -76,9 +98,18 @@ class WCT(object):
         ``passes`` > 1 repeats the stylisation on the previous OUTPUT like stylize.py:102-104 (``--passes``), but keeps the
         intermediate frames on the device: each pass still ends in the uint8 quantisation of wct.py:66-68 and restarts from
         /255 (wct.py:60-64), so the result is bit-identical to calling predict once per pass; style swap only acts in the
-        first pass, as in stylize_video.py:117-121.  ``return_device=True`` returns the uint8 cuda tensor instead of a host copy."""
+        first pass, as in stylize_video.py:117-121.  ``return_device=True`` returns the uint8 cuda tensor instead of a host copy.
+
+        ``content_mask`` (spatial control): uint8 label map [Hm,Wm] shared by every frame, or [N,Hm,Wm]; ``styles`` is then
+        a list of R (1..8) uint8 [Hs,Ws,3] images of any sizes, and region r of each frame takes style r.  The mask may have
+        any resolution: every level samples it to its feature grid.  Labels >= R leave that region unstyled.  WCT only."""
         eng = self.engine
         dev = eng.device
+        if content_mask is not None:
+            if adain or swap5:
+                raise ValueError("content_mask works with WCT only: not with adain or swap5")
+            n = 1 if np.ndim(contents) == 3 else contents.shape[0]
+            mask, region_styles = self.check_mask(content_mask, n, styles)
 
         def to_dev(a):
             if isinstance(a, np.ndarray):
@@ -100,7 +131,17 @@ class WCT(object):
                     contents = center_crop_to(contents, H, W)
         with torch.cuda.device(dev):
             c = to_dev(contents)
-            s = to_dev(styles)
+            if content_mask is not None:
+                lab = mask.to(dev, non_blocking=True)
+                rs = [to_dev(x) for x in region_styles]
+
+                def one_pass(x):
+                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs)
+            else:
+                s = to_dev(styles)
+
+                def one_pass(x):
+                    return eng.stylize(x, s, alpha=alpha, adain=adain)
             if swap5:
                 # one pair per call like the reference graph (ops.py:146); frames of a batch are swapped one by one
                 outs = [eng.stylize(c[i:i + 1], s[i:i + 1] if s.shape[0] > 1 else s, alpha=alpha, adain=adain, swap5=True,
@@ -108,10 +149,10 @@ class WCT(object):
                         for i in range(c.shape[0])]
                 out_f = outs[0] if len(outs) == 1 else torch.cat(outs, dim=0)
             else:
-                out_f = eng.stylize(c, s, alpha=alpha, adain=adain)
+                out_f = one_pass(c)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
-                out_f = eng.stylize(out_dev, s, alpha=alpha, adain=adain)
+                out_f = one_pass(out_dev)
                 out_dev = eng.to_u8(out_f)
             if return_device:
                 eng.check_device()            # synchronises; raises WctB200Error if a kernel recorded a pipeline time-out
@@ -131,10 +172,15 @@ class WCT(object):
             return out_u8, out_f.cpu().numpy()
         return out_u8
 
-    def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False):
-        '''Stylize a single content/style pair (wct.py:70-106).'''
+    def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None):
+        '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
+        is a list of R region styles and region r of the content takes style r.'''
         s = time.time()
-        out = self.predict_batch(np.asarray(content), np.asarray(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha)
+        if content_mask is not None:
+            out = self.predict_batch(np.asarray(content), [np.asarray(x) for x in style], alpha=alpha, adain=adain, swap5=swap5,
+                                     content_mask=content_mask)
+        else:
+            out = self.predict_batch(np.asarray(content), np.asarray(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
