@@ -1,18 +1,80 @@
 """Per-layer conv micro-benchmark: every conv shape of the 512x512 pipeline (3x3 layers and the UP2 layers that absorbed an
-UpSampling2D), default dispatch vs fused MMA off.  TFLOP/s = EXECUTED algorithmic flops (2*taps*Cin*Cout per output pixel)."""
-import os, sys
+UpSampling2D), default dispatch vs fused MMA off.  TFLOP/s = EXECUTED algorithmic flops (2*taps*Cin*Cout per output pixel).
+
+  python tools/conv_bench.py [BATCH] [--fixed]
+
+--fixed: the per-tile cost that does not scale with K = 9*Cin (epilogue, tile hand-over, pipeline fill), from pairs of
+3x3 convs with the same output shape and Cout whose Cin differs by 2x: they run the same tiles and the same epilogue, and
+the second has twice the k-iterations, so  fixed = 2 t(Cin) - t(2 Cin)  and  mainloop(Cin) = t(2 Cin) - t(Cin).  Both are
+turned into SM-microseconds per 128 x BN tile (time x #SMs / tiles) and into SM clocks at the clock read after timing."""
+import os, subprocess, sys
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from wct_tf_b200 import _capi
 from tests import gpu_util as U
 
-B = int(sys.argv[1]) if len(sys.argv) > 1 else 8
+ARGS = [a for a in sys.argv[1:] if not a.startswith("--")]
+B = int(ARGS[0]) if ARGS else 8
+FIXED = "--fixed" in sys.argv
 # (output H=W, Cin, Cout, up2)
 SHAPES = [(512, 64, 64, 0), (256, 64, 128, 0), (256, 128, 128, 0), (256, 128, 64, 0), (128, 128, 256, 0), (128, 256, 256, 0),
           (128, 256, 128, 0), (64, 256, 512, 0), (64, 512, 512, 0), (64, 512, 256, 0), (32, 512, 512, 0),
           (64, 512, 512, 1), (128, 256, 256, 1), (256, 128, 128, 1), (512, 64, 64, 1)]
 CFGS = [("default", -1), ("nofuse", 0), ("fuse", 1)]
+# --fixed: (output H=W, Cin, Cout); each shape is timed at Cin and at 2*Cin
+FIXED_PAIRS = [(512, 64, 64), (256, 64, 128), (256, 128, 64), (128, 256, 256)]
 lib = U.lib()
+
+
+def conv_ms(hw, cin, cout, reps=20):
+    """CUDA-event time of one default-dispatch 3x3 conv (+ReLU) at batch B, random ReLU'd input."""
+    x = torch.randn(B, hw, hw, cin, device="cuda").relu_()
+    xin = torch.empty(lib.wctb200_act_bytes(B, hw, hw, cin), dtype=torch.uint8, device="cuda")
+    _capi.check(lib.wctb200_act_from_f32(x.data_ptr(), B, hw, hw, cin, xin.data_ptr(), U.stream()))
+    del x
+    k = (torch.randn(3, 3, cin, cout, device="cuda") * (2.0 / (9 * cin)) ** 0.5).contiguous()
+    bias = torch.zeros(cout, device="cuda")
+    ws = torch.empty(lib.wctb200_conv_weight_bytes(9, cin, cout), dtype=torch.uint8, device="cuda")
+    _capi.check(lib.wctb200_prep_conv_weights(k.data_ptr(), 9, cin, cout, ws.data_ptr(), U.stream()))
+    out = torch.empty(lib.wctb200_act_bytes(B, hw, hw, cout), dtype=torch.uint8, device="cuda")
+    def run():
+        _capi.check(lib.wctb200_conv3x3(xin.data_ptr(), B, hw, hw, cin, ws.data_ptr(), bias.data_ptr(), cout, 1, out.data_ptr(), U.stream()))
+    for _ in range(3): run()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps): run()
+    e1.record(); torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def sm_clock_mhz():
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader,nounits", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30)
+        return float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        return float("nan")
+
+
+if FIXED:
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    print("%-20s %9s %9s %7s %10s %10s %9s %9s %7s   (batch %d, %d SMs, 3x3 + ReLU, default dispatch)" % (
+        "HxW Cin->Cout", "t(Cin)", "t(2Cin)", "tiles", "fixed/tile", "main/tile", "fixed clk", "main clk", "fixed%",
+        B, sms))
+    for hw, cin, cout in FIXED_PAIRS:
+        t1 = conv_ms(hw, cin, cout)
+        t2 = conv_ms(hw, 2 * cin, cout)
+        mhz = sm_clock_mhz()
+        bn = 128 if cout % 128 == 0 else 64
+        tiles = -(-(B * (hw + 2) * (hw + 2)) // 128) * (cout // bn)
+        fixed_us = (2 * t1 - t2) * 1e3 * sms / tiles       # SM-microseconds per tile
+        main_us = (t2 - t1) * 1e3 * sms / tiles
+        print("%-20s %7.1fus %7.1fus %7d %8.3fus %8.3fus %9.0f %9.0f %6.1f%%   (SM clock %.0f MHz after timing)" % (
+            "%dx%d %d->%d" % (hw, hw, cin, cout), t1 * 1e3, t2 * 1e3, tiles, fixed_us, main_us, fixed_us * mhz,
+            main_us * mhz, 100.0 * (2 * t1 - t2) / t1, mhz), flush=True)
+    _capi.check(lib.wctb200_check_device(U.stream()))
+    sys.exit(0)
+
 print("%-24s" % "HxW Cin->Cout" + "".join("%18s" % c[0] for c in CFGS) + "   (executed TFLOP/s, batch %d)" % B)
 for hw, cin, cout, up2 in SHAPES:
     hin = hw // 2 if up2 else hw

@@ -33,9 +33,11 @@
 // 8x the reference's own fp32 noise on the free-running 5-level image (tests/noise_split_cpu.py).
 //
 // Structure (persistent CTAs, 384 threads):
-//   warp 8   : TMA producer   (cp.async.bulk.tensor 3-D, 128B swizzle, mbarrier complete_tx; warps 9-11 idle)
-//   warps 0-7: two wgmma warpgroups (64 tile rows each), then the epilogue (*scale +bias, ReLU -> split fp16 ->
-//              16-byte stores of the interior pixel AND the halo cells that mirror it)
+//   warp 8    : TMA producer   (cp.async.bulk.tensor 3-D, 128B swizzle, mbarrier complete_tx)
+//   warps 0-7 : two wgmma warpgroups (64 tile rows each); each hands its finished fp32 tile rows over in shared memory and
+//               goes straight on to the next tile's mainloop
+//   warps 9-11: the epilogue (*scale +bias, ReLU -> split fp16 -> 16-byte stores of the interior pixel AND the halo cells
+//               that mirror it), overlapped with the next tile's mainloop
 #include "common.cuh"
 
 namespace wctb {
@@ -76,18 +78,25 @@ __device__ __forceinline__ int region_of(const uint8_t* labels, const int* count
 // ===========================================================================
 // Persistent CTAs, warp-specialised (384 threads):
 //   warps 0-7: two consumer warpgroups.  Warpgroup w multiplies rows [64w, 64w + 64) of the 128-position tile with
-//              wgmma (m64 x N x k16, both operands K-major from the 128B-swizzled stages, fp32 accumulators in registers)
-//              and then both run the epilogue;
-//   warps 8-11: producer warpgroup; one thread issues the TMA loads.  setmaxnreg moves registers from it to the
-//              consumers (the register file is allocated in whole warpgroups: 288 threads would cap every thread at 168).
+//              wgmma (m64 x N x k16, both operands K-major from the 128B-swizzled stages, fp32 accumulators in registers),
+//              writes its rows of the fp32 tile to shared memory and returns to the mainloop;
+//   warps 8-11: producer warpgroup; lane 0 of warp 8 issues the TMA loads, warps 9-11 run the epilogue of the tile the
+//              consumers handed over while those already multiply the next one.  setmaxnreg moves registers from this
+//              warpgroup to the consumers (the register file is allocated in whole warpgroups: 288 threads would cap every
+//              thread at 168).
 //   * grid = #SMs x oversubscription, every CTA walks a static tile list (cout tile fastest, so CTAs running together
 //     share activation tiles in L2 and the whole weight tensor stays L2 resident);
 //   * chunked accumulation: CH k-iterations accumulate into register chunks that start from zero (one for a_hi b_hi, one
 //     for the two small cross products) and are then added into the running sum with round-to-nearest FADDs.  The tensor
 //     core adds into its fp32 accumulator with truncation; short chunks summed in registers keep the conv at fp32-class
 //     error for K up to 4608;
-//   * epilogue: the fp32 tile goes through shared memory (a wgmma fragment spreads one row over 4 lanes) so that each
-//     epilogue thread owns one output position and 64 consecutive channels: scale/bias/ReLU/(pool)/split/coalesced stores.
+//   * tile hand-off: one fp32 tile buffer in shared memory and two mbarriers.  Every consumer warp arrives on tile_full
+//     after writing its fragment rows; every epilogue warp arrives on tile_empty after its last read.  A consumer waits
+//     on tile_empty only before writing the NEXT tile, a whole mainloop later, so the epilogue runs in the shadow of the
+//     mainloop as long as it is the shorter of the two;
+//   * epilogue: 8 lanes per output position, 8 consecutive channels per lane read straight from the fp32 tile:
+//     scale/bias/ReLU/(pool)/split, then 16-byte stores; the 8 lanes of a position write its 128 contiguous bytes per
+//     plane, so the stores stay coalesced without a staging buffer.
 // ===========================================================================
 template <int BN, bool FUSE_>
 struct Conv2Cfg {
@@ -106,14 +115,14 @@ struct Conv2Cfg {
     static constexpr int CH = 2;                                // k-iterations per accumulation chunk
     static constexpr int CONSUMERS = 256;
     static constexpr int THREADS = CONSUMERS + 128;
-    static constexpr int EPI_WARPS = BN / 16;                   // 64 channels per epilogue thread
-    static constexpr int NACC = 64;
-    static constexpr int PITCH = BN + 4;                        // fp32 tile row pitch (conflict-free float4 row reads)
+    static constexpr int EPI_WARPS = 3;                         // warps 9-11 of the producer warpgroup
+    static constexpr int NB = BN / 64;                          // 64-channel blocks of a tile row
+    // fp32 tile row pitch: BN + 8 makes the consumers' float2 fragment writes conflict free (a half-warp's 4 rows land
+    // 8 banks apart); the epilogue reads 256 contiguous bytes of one row per 8 lanes, which no pitch affects
+    static constexpr int PITCH = BN + 8;
     static constexpr int TILE_BYTES = BM * PITCH * 4;
-    static constexpr int STG_BYTES = EPI_WARPS * 8192;          // per-epilogue-warp store staging (coalesced stores)
-    static constexpr int EPI_BYTES = TILE_BYTES > STG_BYTES ? TILE_BYTES : STG_BYTES;   // the two alias
-    static constexpr int AUX_BYTES = 256 + BN * 4;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + EPI_BYTES + 1024;
+    static constexpr int AUX_BYTES = 256 + 2 * BN * 4;          // mbarriers + abort flag, then the bias of two passes
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + TILE_BYTES + 1024;
 };
 
 struct TileCoord {
@@ -188,6 +197,144 @@ __device__ __forceinline__ void conv_stage_mma(float (&ch)[Cfg::CHUNK_REGS], flo
     }
 }
 
+// 8 consecutive fp32 of a tile row.  Lanes 4-7 of each 8-lane group read their two 16-byte halves in the opposite order, so
+// each 16-byte load of the 8 lanes (one shared-memory phase) covers all 32 banks once.
+__device__ __forceinline__ void tile_load8(const float* src, int c, float (&v)[8]) {
+    const float4* s = reinterpret_cast<const float4*>(src);
+    const int sw = (c >> 2) & 1;
+    const float4 a = s[sw], b = s[sw ^ 1];
+    const float4 l = sw ? b : a, h = sw ? a : b;
+    v[0] = l.x; v[1] = l.y; v[2] = l.z; v[3] = l.w;
+    v[4] = h.x; v[5] = h.y; v[6] = h.z; v[7] = h.w;
+}
+
+// *scale + bias, ReLU, split: 8 channels of one output position
+__device__ __forceinline__ void finish8(const float (&a)[8], float wsc, const float* sb, bool relu, Half8& hi, Half8& lo) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const float t = fmaf(a[j], wsc, sb[j]);
+        v[j] = relu ? fmaxf(t, 0.f) : t;
+    }
+    split8(v, hi, lo);
+}
+
+// Where row `row` of a 128-position tile goes: returns its halo flags and sets its padded output position, or returns -1
+// when nothing is stored (halo / junk row of the padded tiling, a pixel of another region, an aborted pipeline).
+// REG: the pass stores the pixels of region `want` (R: the pixels that keep their input).
+// (32-bit position arithmetic: P < 2^31 is checked by the launcher; 64-bit divisions cost ~60 instructions each)
+template <bool REG>
+__device__ __forceinline__ int row_target(const ConvParams& p, const ActGeom& go, const TileCoord& tc, int row, int want,
+                                          volatile int* abort_flag, unsigned int& ppos) {
+    ppos = 0;
+    const unsigned int pos = (unsigned int)tc.p0 + (unsigned int)row;
+    if (pos >= (unsigned int)tc.p_end) return -1;
+    const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
+    const unsigned int n = pos / hpwp;
+    const unsigned int r = pos - n * hpwp;
+    const int yy = (int)(r / (unsigned int)p.Wp);
+    const int xx = (int)(r - (unsigned int)yy * (unsigned int)p.Wp);
+    if (yy < 1 || yy > p.H || xx < 1 || xx > p.W || *abort_flag) return -1;
+    int y = yy - 1, x = xx - 1;
+    if (p.mode == CONV_UP2) { y = 2 * y + (tc.cls >> 1); x = 2 * x + (tc.cls & 1); }
+    if (REG && region_of(p.labels, p.counts, p.R, (int)n, p.H, p.W, y, x) != want) return -1;
+    ppos = ((unsigned int)n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
+    return halo_flags(go, y, x);
+}
+
+// Epilogue of one pass, run by epilogue warp ew (of Cfg::EPI_WARPS).  The work is split into units of 4 positions x 64
+// channels (8 lanes per position, 8 channels per lane); unit u = (32-row chunk * 8 + j) * NB + 64-channel block goes to
+// warp u % EPI_WARPS.  The lane of a chunk row computes that row's target once; the 8 lanes storing it take it by shuffle.
+// KEEP (REG only): copy the input pixels of the rows to keep (hi and lo bytes) instead of finishing the fp32 tile.
+template <class Cfg, bool REG, bool KEEP>
+__device__ __forceinline__ void epi_rows(const ConvParams& p, const ActGeom& go, const TileCoord& tc, const float* ctile,
+                                         const float* sb, float wsc, bool relu, int want, int ew, int lane,
+                                         volatile int* abort_flag) {
+    constexpr int U = 8 * Cfg::NB;                       // units per 32-row chunk
+    const int c = lane & 7;
+#pragma unroll 1
+    for (int chunk = 0; chunk < Cfg::BM / 32; ++chunk) {
+        unsigned int pp;
+        const int fl = row_target<REG>(p, go, tc, chunk * 32 + lane, want, abort_flag, pp);
+        for (int v = ((ew - chunk * U) % Cfg::EPI_WARPS + Cfg::EPI_WARPS) % Cfg::EPI_WARPS; v < U; v += Cfg::EPI_WARPS) {
+            const int j = v / Cfg::NB, b = v - j * Cfg::NB;
+            const int r = j * 4 + (lane >> 3);
+            const unsigned int q = __shfl_sync(0xffffffffu, pp, r);
+            const int f = __shfl_sync(0xffffffffu, fl, r);
+            if (f < 0) continue;
+            const int ch = b * 64 + c * 8;               // channel within the tile
+            Half8 hi, lo;
+            if (KEEP) {
+                const __half* src = p.in + (long long)q * p.Cin + tc.n0 + ch;   // APPLY: input and output positions agree
+                hi = *reinterpret_cast<const Half8*>(src);
+                lo = *reinterpret_cast<const Half8*>(src + (long long)p.P * p.Cin);
+            } else {
+                float a[8], bb[8];
+                tile_load8(ctile + (chunk * 32 + r) * Cfg::PITCH + ch, c, a);
+                tile_load8(sb + ch, c, bb);
+                finish8(a, wsc, bb, relu, hi, lo);
+            }
+            store8_at(p.out, go, q, f, tc.n0 + ch, hi, lo);
+        }
+    }
+}
+
+// POOL2 epilogue: MaxPooling2D 2x2/2 'same' (vgg_normalised.py:41-42) on the raw accumulators, which commutes with the
+// monotone  *scale + bias -> ReLU -> split  that follows.  Tile rows 0..63 = image row 2i, 64..127 = row 2i+1, so pooled
+// pixel k of the tile is the max of rows 2k, 2k+1, 64+2k, 65+2k; cells past the right / bottom edge are left out.
+// Units of 4 pooled pixels x 64 channels; lane k computes pooled pixel k's target.
+template <class Cfg>
+__device__ __forceinline__ void epi_pool(const ConvParams& p, const ActGeom& go, const TileCoord& tc, const float* ctile,
+                                         const float* sb, float wsc, bool relu, int ew, int lane, volatile int* abort_flag) {
+    const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
+    const unsigned int n = (unsigned int)tc.p0 / hpwp;
+    const int yy0 = (int)(((unsigned int)tc.p0 - n * hpwp) / (unsigned int)p.Wp);   // padded row of image row 2i
+    const bool lower = yy0 < p.H;                        // image row 2i+1 exists
+    unsigned int pp = 0;
+    int fl = -1;
+    {
+        const int x = 64 * tc.cls + 2 * lane;
+        if (x < p.W && yy0 - 1 < p.H && !*abort_flag) {
+            const int yo = (yy0 - 1) >> 1, xo = x >> 1;
+            fl = halo_flags(go, yo, xo);
+            pp = (n * (unsigned int)go.Hp + (unsigned int)(yo + 1)) * (unsigned int)go.Wp + (unsigned int)(xo + 1);
+        }
+    }
+    const int c = lane & 7;
+    for (int v = ew; v < 8 * Cfg::NB; v += Cfg::EPI_WARPS) {
+        const int j = v / Cfg::NB, b = v - j * Cfg::NB;
+        const int k = j * 4 + (lane >> 3);
+        const unsigned int q = __shfl_sync(0xffffffffu, pp, k);
+        const int f = __shfl_sync(0xffffffffu, fl, k);
+        if (f < 0) continue;
+        const bool right = 64 * tc.cls + 2 * k + 1 < p.W;
+        const int ch = b * 64 + c * 8;
+        const float* s = ctile + 2 * k * Cfg::PITCH + ch;
+        float m[8], a[8];
+        tile_load8(s, c, m);
+        if (right) {
+            tile_load8(s + Cfg::PITCH, c, a);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) m[i] = fmaxf(m[i], a[i]);
+        }
+        if (lower) {
+            tile_load8(s + 64 * Cfg::PITCH, c, a);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) m[i] = fmaxf(m[i], a[i]);
+            if (right) {
+                tile_load8(s + 65 * Cfg::PITCH, c, a);
+#pragma unroll
+                for (int i = 0; i < 8; ++i) m[i] = fmaxf(m[i], a[i]);
+            }
+        }
+        float bb[8];
+        tile_load8(sb + ch, c, bb);
+        Half8 hi, lo;
+        finish8(m, wsc, bb, relu, hi, lo);
+        store8_at(p.out, go, q, f, tc.n0 + ch, hi, lo);
+    }
+}
+
 // REG (spatial control, CONV_APPLY only): every tile runs one mainloop + epilogue pass per region present in it (its own
 // weight set, stores only the rows of that region), then copies the rows to keep; a tile inside one region costs what the
 // plain apply costs.
@@ -201,10 +348,11 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     uint8_t* aux = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty = full + Cfg::STAGES;
-    volatile int* abort_flag = reinterpret_cast<volatile int*>(empty + Cfg::STAGES);
-    float* sbias = reinterpret_cast<float*>(aux + 256);
-    uint8_t* epi = aux + Cfg::AUX_BYTES;                 // fp32 tile, then (aliased) the per-warp store staging buffers
-    float* ctile = reinterpret_cast<float*>(epi);
+    uint64_t* tile_full = empty + Cfg::STAGES;           // the fp32 tile is written (one arrival per consumer warp)
+    uint64_t* tile_empty = tile_full + 1;                // the fp32 tile is read (one arrival per epilogue warp)
+    volatile int* abort_flag = reinterpret_cast<volatile int*>(tile_empty + 1);
+    float* sbias = reinterpret_cast<float*>(aux + 256);  // [2][BN]: bias of the pass (by pass parity)
+    float* ctile = reinterpret_cast<float*>(aux + Cfg::AUX_BYTES);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -219,6 +367,8 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], Cfg::CONSUMERS / 32);      // one arrival per consumer warp
         }
+        mbar_init(tile_full, Cfg::CONSUMERS / 32);
+        mbar_init(tile_empty, Cfg::EPI_WARPS);
         *abort_flag = 0;
         fence_barrier_init();
         tma_prefetch_desc(&mapA);
@@ -230,9 +380,16 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const int kiters = p.taps * ksl;
     const int nchunks = (kiters + Cfg::CH - 1) / Cfg::CH;
 
+    // register split, checked with ptxas -v to spill nothing: the consumers of BN = 128 need more than 200 and the epilogue
+    // warps more than 56 (REG: 80).  setmaxnreg.inc only receives what the other warpgroups released, so the split must
+    // stay within the 3 x 128 x 168 registers the CTA was launched with, or the consumers wait for registers forever.
+    constexpr int EPI_REGS = REG ? (BN == 128 ? 88 : 104) : 72;
+    constexpr int MMA_REGS = REG ? (BN == 128 ? 208 : 200) : 216;
+    static_assert(2 * 128 * MMA_REGS + 128 * EPI_REGS <= 3 * 128 * 168, "setmaxnreg split exceeds the CTA's registers");
     if (warp >= Cfg::CONSUMERS / 32) {
-        setmaxnreg_dec<40>();
-        if (warp == Cfg::CONSUMERS / 32 && lane == 0) {
+        setmaxnreg_dec<EPI_REGS>();
+        if (warp == Cfg::CONSUMERS / 32) {
+            if (lane != 0) return;
             uint32_t itg = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
@@ -269,31 +426,53 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 }
                 }
             }
+            return;
+        }
+
+        // ---- epilogue warps 9-11: the same tile list and passes as the consumers, one tile hand-off per pass ----
+        const int ew = warp - Cfg::CONSUMERS / 32 - 1;
+        const bool up2 = p.mode == CONV_UP2;
+        ActGeom go(p.N, up2 ? 2 * p.H : (p.pool ? (p.H + 1) / 2 : p.H), up2 ? 2 * p.W : (p.pool ? (p.W + 1) / 2 : p.W), p.Cout);
+        go.edge = (p.flags & WCTB200_HALO_EDGE) ? 1 : 0;
+        const bool relu = (p.flags & WCTB200_RELU) != 0;
+        const float wsc = p.wscale ? __ldg(p.wscale) : 1.f;
+        uint32_t pass = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
+            const int mt = tile / n_tiles;
+            unsigned todo = 1u;
+            if constexpr (REG) todo = p.amask[mt] & ((1u << p.R) - 1u);
+            for (; todo; todo &= todo - 1u, ++pass) {
+                const int region = __ffs(todo) - 1;
+                const int set = REG ? mt / p.tiles_per_image * p.R + region : tc.set;
+                // bias of this pass into the buffer of its parity: that buffer was last read two passes ago, before every
+                // epilogue warp passed the previous pass's barrier
+                float* sb = sbias + (pass & 1) * BN;
+                for (int i = threadIdx.x - (Cfg::CONSUMERS + 32); i < BN; i += 32 * Cfg::EPI_WARPS)
+                    sb[i] = p.bias ? __ldg(p.bias + (long long)(p.mode == CONV_APPLY ? set : 0) * p.Cout + tc.n0 + i) : 0.f;   // UP2: set = weight parity class, ONE bias
+                mbar_wait(tile_full, pass & 1, abort_flag, p.err, 0x301u);
+                asm volatile("bar.sync 1, %0;" ::"r"(32 * Cfg::EPI_WARPS) : "memory");
+                if (p.pool) epi_pool<Cfg>(p, go, tc, ctile, sb, wsc, relu, ew, lane, abort_flag);
+                else epi_rows<Cfg, REG, false>(p, go, tc, ctile, sb, wsc, relu, region, ew, lane, abort_flag);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(tile_empty);  // the consumers may write the next tile
+            }
+            if constexpr (REG) {
+                if ((p.amask[mt] >> p.R) & 1u) epi_rows<Cfg, REG, true>(p, go, tc, ctile, sbias, wsc, relu, p.R, ew, lane, abort_flag);
+            }
         }
         return;
     }
 
     // ---- consumer warpgroups ----
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<MMA_REGS>();
     const int wg = warp >> 2;                            // rows [64 wg, 64 wg + 64) of the tile
     const int t = threadIdx.x & 127;
-    const int e = warp;                                  // epilogue warp: rows 32 (e & 3) .. +31, channels 64 (e >> 2) .. +63
-    const int g = e & 3;
-    const int colbase = (e >> 2) * Cfg::NACC;
-    constexpr int ETHREADS = 32 * Cfg::EPI_WARPS;
-    const bool up2 = p.mode == CONV_UP2;
-    ActGeom go(p.N, up2 ? 2 * p.H : (p.pool ? (p.H + 1) / 2 : p.H), up2 ? 2 * p.W : (p.pool ? (p.W + 1) / 2 : p.W), p.Cout);
-    go.edge = (p.flags & WCTB200_HALO_EDGE) ? 1 : 0;
-    const bool relu = (p.flags & WCTB200_RELU) != 0;
-    const float wsc = p.wscale ? __ldg(p.wscale) : 1.f;
-    uint32_t itg = 0;
+    uint32_t itg = 0, pass = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
         unsigned todo = 1u;
         if constexpr (REG) todo = p.amask[tile / n_tiles] & ((1u << p.R) - 1u);
-        for (; todo; todo &= todo - 1u) {
-        const int region = __ffs(todo) - 1;
-        const int set = REG ? (tile / n_tiles) / p.tiles_per_image * p.R + region : tc.set;
+        for (; todo; todo &= todo - 1u, ++pass) {
         float sum[Cfg::SUM_REGS];
 #pragma unroll
         for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
@@ -335,141 +514,12 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             }
         }
 
-        // ---- fp32 tile through shared memory: epilogue thread = one row (position), 64 channels ----
-        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // previous tile's staging buffers are free
+        // ---- hand the fp32 tile to the epilogue warps (row-major in shared memory: a wgmma fragment spreads one row
+        // over 4 lanes); the previous tile must have been read, which it normally was during this mainloop ----
+        mbar_wait(tile_empty, (pass & 1) ^ 1u, abort_flag, p.err, 0x300u);
         frag_to_tile(sum, ctile, Cfg::PITCH, 64 * wg, t);
-        for (int i = threadIdx.x; i < BN; i += Cfg::CONSUMERS)
-            sbias[i] = p.bias ? p.bias[(long long)(p.mode == CONV_APPLY ? set : 0) * p.Cout + tc.n0 + i] : 0.f;   // UP2: set = weight parity class, ONE bias
-        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");
-        float acc[Cfg::NACC];
-        if (e < Cfg::EPI_WARPS) {
-            const float4* src = reinterpret_cast<const float4*>(ctile + (g * 32 + lane) * Cfg::PITCH + colbase);
-#pragma unroll
-            for (int j = 0; j < Cfg::NACC / 4; ++j) {
-                const float4 v = src[j];
-                acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.z; acc[4 * j + 3] = v.w;
-            }
-        }
-        asm volatile("bar.sync 1, %0;" ::"r"(Cfg::CONSUMERS) : "memory");   // tile read: the staging buffers may be written
-        if (e >= Cfg::EPI_WARPS) continue;
-
-        if (p.pool) {
-            // ---- MaxPooling2D 2x2/2 'same' (vgg_normalised.py:41-42) on the raw accumulators: max commutes with the
-            // monotone  *scale + bias -> ReLU -> split  that follows.  Tile rows 0..63 = image row 2i, 64..127 = row 2i+1.
-            // Work split: the two lanes of a horizontal pixel pair share the pooled pixel's channels (16-channel blocks:
-            // lane parity l owns channels 8l..8l+7 of each block), and the warps of the two image rows share them by halves
-            // (upper-row warps keep the lower half of the channel range, lower-row warps the upper half), so every lane of
-            // the two warps finishes and stores NACC/4 channels of one pooled pixel.
-            constexpr int NH = Cfg::NACC / 2;            // channels per half
-            constexpr int Q = Cfg::NACC / 4;             // channels a lane finishes
-            const int tpos = g * 32 + lane;
-            const int xloc = tpos & 63;
-            const int hv = tpos >> 6;                    // 0: image row 2i, 1: row 2i+1
-            const int lp = lane & 1;
-            const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
-            const unsigned int n = (unsigned int)tc.p0 / hpwp;
-            const int yy0 = (int)(((unsigned int)tc.p0 - n * hpwp) / (unsigned int)p.Wp);   // padded row of image row 2i
-            const int x = 64 * tc.cls + xloc;
-            const bool valid = (yy0 - 1 + hv) < p.H && x < p.W;
-            if (__any_sync(0xffffffffu, !valid)) {       // ragged right / bottom edge only
-                const float ninf = __int_as_float(0xff800000);
-#pragma unroll
-                for (int j = 0; j < Cfg::NACC; ++j) acc[j] = valid ? acc[j] : ninf;
-            }
-            // horizontal: m[h][k] = max over the pixel pair of channel  h*NH + (k>>3)*16 + lp*8 + (k&7)
-            float keep[Q], send[Q];
-#pragma unroll
-            for (int k = 0; k < Q; ++k) {
-                const int c0 = (k >> 3) * 16 + (k & 7);
-                float mh[2];
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const float a0 = acc[h * NH + c0], a1 = acc[h * NH + c0 + 8];
-                    const float mine = lp ? a1 : a0;
-                    const float other = lp ? a0 : a1;    // the neighbour lane's channel, this lane's pixel
-                    mh[h] = fmaxf(mine, __shfl_xor_sync(0xffffffffu, other, 1));
-                }
-                keep[k] = hv ? mh[1] : mh[0];
-                send[k] = hv ? mh[0] : mh[1];
-            }
-            // vertical: hand the other half over to the warp of the other image row (same lane = same pixel column)
-            {
-                float* xb = reinterpret_cast<float*>(epi + e * 8192) + lane;
-#pragma unroll
-                for (int k = 0; k < Q; ++k) xb[k * 32] = send[k];
-            }
-            asm volatile("bar.sync 2, %0;" ::"r"(ETHREADS) : "memory");
-            {
-                const float* pb = reinterpret_cast<const float*>(epi + (e ^ 2) * 8192) + lane;   // rows of the other image row
-#pragma unroll
-                for (int k = 0; k < Q; ++k) keep[k] = fmaxf(keep[k], pb[k * 32]);
-            }
-            const int xe = x & ~1;                       // the even column of the pair
-            if (xe < p.W && yy0 - 1 < p.H && !*abort_flag) {
-                const int yo = (yy0 - 1) >> 1, xo = xe >> 1;
-                const int flags = halo_flags(go, yo, xo);
-                const unsigned int ppos = (n * (unsigned int)go.Hp + (unsigned int)(yo + 1)) * (unsigned int)go.Wp + (unsigned int)(xo + 1);
-                const int cb = colbase + hv * NH + lp * 8;   // first channel this lane stores
-#pragma unroll
-                for (int q = 0; q < Q / 8; ++q) {
-                    float v[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float tt = fmaf(keep[q * 8 + j], wsc, sbias[cb + q * 16 + j]);
-                        v[j] = relu ? fmaxf(tt, 0.f) : tt;
-                    }
-                    Half8 hi, lo;
-                    split8(v, hi, lo);
-                    store8_at(p.out, go, ppos, flags, tc.n0 + cb + q * 16, hi, lo);
-                }
-            }
-            continue;
-        }
-        // ---- store: interior pixel + the halo cells that mirror it ----
-        // (32-bit position arithmetic: P < 2^31 is checked by the launcher; 64-bit divisions cost ~60 instructions each)
-        const unsigned int pos = (unsigned int)tc.p0 + (unsigned int)(g * 32 + lane);
-        int flags = -1;                                      // < 0: nothing to store for this row
-        unsigned int ppos = 0;
-        if (pos < (unsigned int)tc.p_end) {
-            const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
-            const unsigned int n = pos / hpwp;
-            const unsigned int r = pos - n * hpwp;
-            const int yy = (int)(r / (unsigned int)p.Wp);
-            const int xx = (int)(r - (unsigned int)yy * (unsigned int)p.Wp);
-            if (yy >= 1 && yy <= p.H && xx >= 1 && xx <= p.W && !*abort_flag) {
-                int y = yy - 1, x = xx - 1;
-                if (up2) { y = 2 * y + (tc.cls >> 1); x = 2 * x + (tc.cls & 1); }
-                flags = halo_flags(go, y, x);
-                ppos = ((unsigned int)n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
-                if (REG && region_of(p.labels, p.counts, p.R, (int)n, p.H, p.W, y, x) != region) flags = -1;   // another pass stores it
-            }
-        }
-        store_tile_rows<Cfg::NACC>(acc, wsc, sbias + colbase, relu, epi + e * 8192, lane, ppos, flags, p.out, go, tc.n0 + colbase);
-        }
-        if constexpr (REG) {
-            // rows to keep: the input pixel (hi and lo bytes) goes to the interior cell and the halo cells that mirror it
-            if (((p.amask[tile / n_tiles] >> p.R) & 1u) && e < Cfg::EPI_WARPS && !*abort_flag) {
-                const unsigned int pos = (unsigned int)tc.p0 + (unsigned int)(g * 32 + lane);
-                if (pos < (unsigned int)tc.p_end) {
-                    const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
-                    const unsigned int n = pos / hpwp;
-                    const unsigned int r = pos - n * hpwp;
-                    const int yy = (int)(r / (unsigned int)p.Wp);
-                    const int xx = (int)(r - (unsigned int)yy * (unsigned int)p.Wp);
-                    if (yy >= 1 && yy <= p.H && xx >= 1 && xx <= p.W &&
-                        region_of(p.labels, p.counts, p.R, (int)n, p.H, p.W, yy - 1, xx - 1) == p.R) {
-                        const int flags = halo_flags(go, yy - 1, xx - 1);
-                        const long long plane = (long long)p.P * p.Cin;
-#pragma unroll
-                        for (int q = 0; q < Cfg::NACC / 8; ++q) {
-                            const int c0 = tc.n0 + colbase + q * 8;
-                            const Half8 hi = *reinterpret_cast<const Half8*>(p.in + (long long)pos * p.Cin + c0);
-                            const Half8 lo = *reinterpret_cast<const Half8*>(p.in + plane + (long long)pos * p.Cin + c0);
-                            store8_at(p.out, go, pos, flags, c0, hi, lo);
-                        }
-                    }
-                }
-            }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(tile_full);
         }
     }
 }
