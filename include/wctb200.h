@@ -191,7 +191,9 @@ WCTB200_API int wctb200_wct_apply_regions(const void* content, int Nc, int Hc, i
 WCTB200_API int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst,
                                   void* stream);
 /* AdaIN (ops.py:282-294): biased per-channel moments of content and style,
- * y = (x-mc)*rsqrt(vc+eps)*sqrt(vs)+ms, out = alpha*y + (1-alpha)*x. */
+ * y = (x-mc)*rsqrt(vc+eps)*sqrt(vs)+ms, out = alpha*y + (1-alpha)*x.  The moments are summed centred on a sampled
+ * per-channel shift, in a split of each frame that depends on C, H and W only: a frame's output is bit-identical
+ * whatever batch it runs in. */
 WCTB200_API int wctb200_adain_level(const void* content, int Nc, int Hc, int Wc,
                         const void* style, int Ns, int Hs, int Ws, int C,
                         float alpha, float eps, void* out, void* ws, size_t ws_bytes, void* stream);

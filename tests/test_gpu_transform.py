@@ -131,6 +131,59 @@ def test_adain_level(c, alpha):
         assert np.abs(got[i:i + 1] - ref).max() <= 2e-5 * (1 + np.abs(ref).max())
 
 
+ADAIN_MEANS = (0.3, 5.0, 30.0)
+ADAIN_STDS = (1.0, 0.1, 0.03)
+
+
+def _adain_features(shape, rng):
+    """Channel c takes mean x std combination c % 11 of ADAIN_MEANS x ADAIN_STDS; combination 9 is a constant channel
+    (var = 0: eps governs) and 10 an all-zero channel."""
+    n, h, w, c = shape
+    x = rng.standard_normal(shape)
+    for ch in range(c):
+        k = ch % 11
+        if k < 9:
+            x[..., ch] = ADAIN_MEANS[k // 3] + ADAIN_STDS[k % 3] * x[..., ch]
+        else:
+            x[..., ch] = 29.71 if k == 9 else 0.0
+    return x.astype(np.float32)
+
+
+@pytest.mark.parametrize("alpha", [1.0, 0.6])
+@pytest.mark.parametrize("shape", [(1, 256, 256, 64), (2, 128, 128, 128), (1, 64, 64, 256), (3, 32, 32, 512), (1, 37, 53, 64)],
+                         ids=lambda s: "x".join(map(str, s)))
+def test_adain_level_moments_at_numeric_edges(shape, alpha):
+    """AdaIN vs the two-pass float64 oracle on channels with large means and small spreads (where sum x^2 / HW - mean^2
+    cancels), a constant channel and an all-zero one, at level-sized maps.  Per channel c:
+        max |got - ref| <= 1e-5 max |ref_c| + 1e-4 alpha sqrt(var_s,c)
+    (the SPF16 rounding of the output, plus a 1e-5-class error on the normalised part)."""
+    n, h, w, c = shape
+    rng = np.random.default_rng(sum(shape))
+    content = _adain_features(shape, rng)
+    ns = n if n == 2 else 1
+    style = (rng.uniform(0.0, 3.0, c) + rng.uniform(0.2, 2.0, c) * rng.standard_normal((ns, h // 2 + 3, w // 2 + 5, c)))
+    style = style.astype(np.float32)
+    cin, sin = U.act_from_numpy(content), U.act_from_numpy(style)
+    out = U.act_alloc(n, h, w, c)
+    ws = torch.empty(U.lib().wctb200_wct_workspace_bytes(c, n, ns), dtype=torch.uint8, device="cuda")
+    _capi.check(U.lib().wctb200_adain_level(cin.data_ptr(), n, h, w, sin.data_ptr(), ns, style.shape[1], style.shape[2], c, alpha,
+                                            1e-5, out.data_ptr(), ws.data_ptr(), ws.numel(), U.stream()))
+    U.check_device()
+    got = U.act_to_numpy(out, n, h, w, c)
+    worst = (0.0, None)
+    for i in range(n):
+        s64 = U.split_repr(style[i if ns > 1 else 0][None])
+        ref = ref_ops.adain(U.split_repr(content[i:i + 1]), s64, alpha)
+        err = np.abs(got[i:i + 1] - ref).max(axis=(0, 1, 2))
+        tol = 1e-5 * np.abs(ref).max(axis=(0, 1, 2)) + 1e-4 * alpha * np.sqrt(s64.var(axis=(0, 1, 2)))
+        r = err / tol
+        if r.max() > worst[0]:
+            ch = int(r.argmax())
+            worst = (float(r.max()), (i, ch, ch % 11, float(err[ch]), float(tol[ch])))
+    print("worst err / tol %.3g at (frame, channel, combination, err, tol) %s" % worst)
+    assert worst[0] <= 1.0, worst
+
+
 def test_split_style_prepare_and_apply_equals_combined_level():
     """wctb200_wct_style_prepare + wctb200_wct_apply (two-stream form) == wctb200_wct_level."""
     g = np.load(GOLDEN[3])
@@ -160,9 +213,21 @@ def test_split_style_prepare_and_apply_equals_combined_level():
 def test_covariance_kernels(shape):
     """Stage A of the transform (ops.py:43-45,105-108): per-channel mean and fc fc^T/(HW-1) on wgmma
     (MN-major operands, centred in shared memory)."""
+    _covariance_case(shape, 0.3)
+
+
+@pytest.mark.parametrize("offset", [0.3, 30.0])
+@pytest.mark.parametrize("shape", [(1, 256, 256, 64), (1, 512, 512, 64)], ids=lambda s: "x".join(map(str, s)))
+def test_covariance_level_sizes_with_offset(shape, offset):
+    """relu1_1-sized maps (HW = 262 144 at 512 x 512: full split-K, 64 tiles per CTA) with small and large channel means: the
+    sampled shift must keep S - s s^T / HW free of cancellation."""
+    _covariance_case(shape, offset)
+
+
+def _covariance_case(shape, offset):
     rng = np.random.default_rng(3)
     n, h, w, c = shape
-    x = np.maximum(rng.standard_normal(shape) @ (rng.standard_normal((c, c)) / np.sqrt(c)) + 0.3, 0).astype(np.float32)
+    x = np.maximum(rng.standard_normal(shape) @ (rng.standard_normal((c, c)) / np.sqrt(c)) + offset, 0).astype(np.float32)
     lib = U.lib()
     buf = U.act_from_numpy(x)
     mean = torch.empty((n, c), dtype=torch.float32, device="cuda")
@@ -177,6 +242,34 @@ def test_covariance_kernels(shape):
         # tensor-core chunks add with truncation: ~24 adds x 2^-24 on the all-positive diagonal sums
         assert np.abs(got - ref).max() <= 1.5e-6 * max(1.0, np.abs(ref).max()), np.abs(got - ref).max()
         assert np.array_equal(got, got.T)
+
+
+@pytest.mark.parametrize("sem", ["tf", "np"])
+@pytest.mark.parametrize("flat", ["content", "style"])
+@pytest.mark.parametrize("c", [64, 256])
+def test_wct_level_constant_frame(c, flat, sem):
+    """A constant map (a black video frame at relu1_1: every channel at its bias) has a zero covariance, so k = 0 on that
+    side and the transform degenerates to a blend with the means.  The output must be finite, match the oracle's blend,
+    and k_out must carry the oracle's counts."""
+    rng = np.random.default_rng(c + (flat == "style"))
+    mix = rng.standard_normal((c, c)) / np.sqrt(c)
+    content = np.maximum(rng.standard_normal((1, 24, 32, c)) @ mix + 0.3, 0).astype(np.float32)
+    style = np.maximum(rng.standard_normal((1, 20, 28, c)) @ mix.T + 0.3, 0).astype(np.float32)
+    level = rng.uniform(0.0, 2.0, c).astype(np.float32)
+    if flat == "content":
+        content[:] = level
+    else:
+        style[:] = level
+    alpha = 0.7
+    got, k = _run_wct(content, style, alpha, sem)
+    fn = ref_ops.wct_tf if sem == "tf" else ref_ops.wct_np
+    ref, info = fn(U.split_repr(content), U.split_repr(style), alpha, return_info=True)
+    assert (info["k_c"] == 0) == (flat == "content") and (info["k_s"] == 0) == (flat == "style")
+    assert ref_ops.spectral_gap_ok(info["ws"] if flat == "content" else info["wc"])
+    assert (k[0], k[1]) == (info["k_c"], info["k_s"]), (k, info["k_c"], info["k_s"])
+    err = np.abs(got - ref).max()
+    print("constant %s, %s semantics, C=%d: k %s, max-abs vs oracle %.2e" % (flat, sem, c, k[:2], err))
+    assert err <= 2e-5 * (1 + np.abs(ref).max()), err
 
 
 def test_jacobi_rank_deficient_null_space_stays_below_threshold():

@@ -340,8 +340,8 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
 }
 
 // shift[n][c] = mean of <= ~1024 strided interior pixels (all pixels when HW <= 1024): fixed-order reduction.
-// grid (C/64, N): one CTA per 64 channels of an image (a single CTA per image took 180 us at C = 512);
-// 256 threads = 8 channel groups x 32 pixel lanes.
+// grid (cdiv(C, 64), N): one CTA per 64 channels of an image (a single CTA per image took 180 us at C = 512);
+// 256 threads = 8 channel groups x 32 pixel lanes (groups past C idle: AdaIN takes any multiple of 8 channels).
 // MASK (spatial control): grid (C/64, N*R); problem z = n*R + r takes the mean of the sampled pixels labelled r, or of the
 // whole sample when it holds none of them.  A frame-wide shift alone is not enough: a region mean far from t cancels in
 // S - s s^T / n.  With every label equal to r the additions are those of the unmasked kernel.
@@ -358,12 +358,13 @@ k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __r
     const int reg = MASK ? blockIdx.y - n * R : 0;
     const long long HW = (long long)g.H * g.W;
     const long long ns = (HW + stride - 1) / stride;
+    const long long nk = c0 < g.C ? ns : 0;
     float s[8], sa[8];
     int cnt = 0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) { s[j] = 0.f; sa[j] = 0.f; }
 #pragma unroll 4
-    for (long long k = rl; k < ns; k += 32) {
+    for (long long k = rl; k < nk; k += 32) {
         const long long q = k * stride;
         const int y = (int)(q / g.W), x = (int)(q - (long long)y * g.W);
         float v[8];
@@ -384,7 +385,7 @@ k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __r
     }
     if (MASK && grp == 0) red_n[rl] = cnt;
     __syncthreads();
-    if (threadIdx.x < 64) {
+    if (threadIdx.x < 64 && blockIdx.x * 64 + threadIdx.x < g.C) {
         float a = 0.f, aa = 0.f;
         int m = 0;
 #pragma unroll
@@ -459,6 +460,17 @@ typedef CUresult (*PFN_encodeTiledC)(CUtensorMap*, CUtensorMapDataType, cuuint32
 
 int g_cov_max_stages = 12;   // probe knob (wctb200_debug_set_cov_stages)
 
+static inline int shift_stride(long long HW) { return HW <= 1024 ? 1 : (int)(HW / 1024); }
+
+// shift [N][C] of a feature batch (k_sample_shift): the centring point of the covariance and of AdaIN's moments (wct.cu).
+// A function of the frame alone.
+int launch_sample_shift(const __half* act, ActGeom g, float* shift, cudaStream_t st) {
+    k_sample_shift<false><<<dim3((unsigned)cdiv(g.C, 64), (unsigned)g.N), 256, 0, st>>>(act, g, shift_stride((long long)g.H * g.W),
+                                                                                        shift, nullptr, 1);
+    WCTB_CHECK_LAUNCH("k_sample_shift");
+    return 0;
+}
+
 // Means and covariance (+ eps_cov I) of a feature batch: mean [N][C], G [N][C][C] (and a copy A0 if not null), fp32.
 // dsum: [N][C] fp64 scratch (caller's workspace); partial products live in the per-stream scratch cache.
 // Spatial control (labels != nullptr): one problem per (image, region), z = n * R + r, over the pixels labelled r:
@@ -512,10 +524,13 @@ static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mea
     p.R = masked ? R : 1;
     // (blocks below the diagonal are never written -- and never read: k_cov_finalize only touches (min,max) entries)
 
-    const int stride = HW <= 1024 ? 1 : (int)(HW / 1024);
-    if (masked) k_sample_shift<true><<<dim3((unsigned)(g.C / 64), (unsigned)nprob), 256, 0, st>>>(act, g, stride, shift, labels, R);
-    else k_sample_shift<false><<<dim3((unsigned)(g.C / 64), (unsigned)g.N), 256, 0, st>>>(act, g, stride, shift, nullptr, 1);
-    WCTB_CHECK_LAUNCH("k_sample_shift");
+    if (masked) {
+        k_sample_shift<true><<<dim3((unsigned)(g.C / 64), (unsigned)nprob), 256, 0, st>>>(act, g, shift_stride(HW), shift, labels, R);
+        WCTB_CHECK_LAUNCH("k_sample_shift");
+    } else {
+        int rc = launch_sample_shift(act, g, shift, st);
+        if (rc) return rc;
+    }
 
     // tensor map over the interior pixels only (see header comment)
     CUtensorMap mX;

@@ -1,7 +1,7 @@
 // Whiten-colour transform (ops.py:24-140) and AdaIN (ops.py:282-294) for one relu level,
 // batched over frames.
 //
-// Stage A  channel sums / covariance        HBM-bound streaming kernels (fp32 FFMA, fp64 combine)
+// Stage A  channel moments / covariance     HBM-bound streaming kernels (fp32 FFMA, fp64 combine)
 // Stage B  C x C symmetric eigendecomposition: one-sided (Hestenes) Jacobi, one pair per warp,
 //          columns staged in shared memory, a thread-block CLUSTER of C/64 CTAs per matrix
 // Stage C  W_c = E_c D_c^-1/2 E_c^T, C_s = E_s D_s^1/2 E_s^T, T = C_s W_c, M = aT + (1-a)I, bias
@@ -17,63 +17,83 @@ namespace cg = cooperative_groups;
 namespace wctb {
 
 // ---------------------------------------------------------------------------
-// Stage A.1: per-channel sums (and sums of squares) over the interior pixels
-//   grid (chunks, problems); 256 threads; thread = (row lane, 8-channel group)
+// Stage A.1 (AdaIN): per-channel moments over the interior pixels, centred on the shift t of k_sample_shift (cov_tc.cu)
+//   grid (slices, frames); 256 threads; thread = (row lane, 8-channel group).  A slice is moments_slice(C) pixels, up to
+//   32 per thread: the split of a frame depends on C and H x W only, never on the batch, so neither does any rounding.
+//   Each CTA writes sum (x - t) and sum (x - t)^2 of its slice to its OWN slot [frame][slice][2][C]; k_moments_finalize
+//   adds the slots in a fixed order.  Centring first keeps the sum of squares free of cancellation: a channel with a large
+//   mean and a small spread (a flat region of the frame) would lose its variance in sum x^2 / HW - mean^2.
 // ---------------------------------------------------------------------------
-template <bool SQ>
+static inline int moments_slice(int C) { return 32 * (256 / (C / 8)); }
+
 __global__ void __launch_bounds__(256)
-k_chan_sums(const __half* __restrict__ act, ActGeom g, int chunk_pix, double* __restrict__ sum, double* __restrict__ sumsq) {
+k_chan_moments(const __half* __restrict__ act, ActGeom g, const float* __restrict__ shift, int slice, float* __restrict__ part) {
     __shared__ float red[256 * 8];
-    __shared__ float red2[SQ ? 256 * 8 : 8];
+    __shared__ float red2[256 * 8];
     const int cgs = g.C / 8;
     const int rows = 256 / cgs;                 // pixel rows handled per iteration (C <= 2048)
     const int grp = threadIdx.x % cgs;
     const int rl = threadIdx.x / cgs;
     const int n = blockIdx.y;
     const long long HW = (long long)g.H * g.W;
-    const long long q0 = (long long)blockIdx.x * chunk_pix;
-    const long long q1 = min(q0 + chunk_pix, HW);
+    const long long q0 = (long long)blockIdx.x * slice;
+    const long long q1 = min(q0 + slice, HW);
     float s[8], s2[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) { s[j] = 0.f; s2[j] = 0.f; }
     if (rl < rows) {
+        float t[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) t[j] = shift[(long long)n * g.C + grp * 8 + j];
         for (long long q = q0 + rl; q < q1; q += rows) {
             const int y = (int)((unsigned)q / (unsigned)g.W), x = (int)((unsigned)q - (unsigned)y * (unsigned)g.W);
             float v[8];
             load8(act, g, ((long long)n * g.Hp + y + 1) * g.Wp + x + 1, grp * 8, v);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                s[j] += v[j];
-                if (SQ) s2[j] = fmaf(v[j], v[j], s2[j]);
+                const float d = v[j] - t[j];
+                s[j] += d;
+                s2[j] = fmaf(d, d, s2[j]);
             }
         }
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         red[threadIdx.x * 8 + j] = s[j];
-        if (SQ) red2[threadIdx.x * 8 + j] = s2[j];
+        red2[threadIdx.x * 8 + j] = s2[j];
     }
     __syncthreads();
-    // thread t < C reduces channel t over the row lanes
+    // thread t < C reduces channel t over the row lanes, in order
+    float* slot = part + ((long long)n * gridDim.x + blockIdx.x) * 2 * g.C;
     for (int c = threadIdx.x; c < g.C; c += 256) {
         const int gq = c / 8, j = c % 8;
         float a = 0.f, a2 = 0.f;
         for (int r = 0; r < rows; ++r) {
             a += red[(r * cgs + gq) * 8 + j];
-            if (SQ) a2 += red2[(r * cgs + gq) * 8 + j];
+            a2 += red2[(r * cgs + gq) * 8 + j];
         }
-        atomicAdd(&sum[(long long)n * g.C + c], (double)a);
-        if (SQ) atomicAdd(&sumsq[(long long)n * g.C + c], (double)a2);
+        slot[c] = a;
+        slot[g.C + c] = a2;
     }
 }
 
-__global__ void k_mean_finalize(const double* __restrict__ sum, const double* __restrict__ sumsq, long long HW, int total,
-                                float* __restrict__ mean, float* __restrict__ var) {
+// mean = t + s / HW, var = S / HW - (s / HW)^2 (biased, tf.nn.moments) with s, S the slot sums of k_chan_moments added in
+// slot order in fp64
+__global__ void k_moments_finalize(const float* __restrict__ part, const float* __restrict__ shift, int C, int nslices, long long HW,
+                                   int total, float* __restrict__ mean, float* __restrict__ var) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const double m = sum[i] / (double)HW;
-    mean[i] = (float)m;
-    if (var) var[i] = (float)fmax(sumsq[i] / (double)HW - m * m, 0.0);   // biased variance (tf.nn.moments)
+    const int n = i / C, c = i - n * C;
+    const float* p = part + (long long)n * nslices * 2 * C + c;
+    double s = 0.0, S = 0.0;
+#pragma unroll 8
+    for (int b = 0; b < nslices; ++b) {
+        s += (double)p[(long long)b * 2 * C];
+        S += (double)p[(long long)b * 2 * C + C];
+    }
+    const double m = s / (double)HW;
+    mean[i] = (float)((double)shift[i] + m);
+    var[i] = (float)fmax(S / (double)HW - m * m, 0.0);
 }
 
 // ---------------------------------------------------------------------------
@@ -555,20 +575,20 @@ __global__ void k_finalize_transform(const float* __restrict__ T, int C, int Nc,
 // ---------------------------------------------------------------------------
 // AdaIN (ops.py:282-294): per-(frame,channel) affine map
 // ---------------------------------------------------------------------------
-__global__ void k_adain_coeffs(const float* __restrict__ mean_c, const float* __restrict__ var_c,
-                               const float* __restrict__ mean_s, const float* __restrict__ var_s, int C, int Nc, int Ns,
-                               float alpha, float eps, float* __restrict__ scale, float* __restrict__ shift) {
+// inv = rsqrt(vc + eps) * sqrt(vs) (batch_normalization with scale = sqrt(style_var)) and the style mean of each content frame
+__global__ void k_adain_coeffs(const float* __restrict__ var_c, const float* __restrict__ mean_s, const float* __restrict__ var_s,
+                               int C, int Nc, int Ns, float eps, float* __restrict__ inv, float* __restrict__ ms) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= Nc * C) return;
     const int z = i / C, c = i % C;
     const int si = (Ns == 1 ? 0 : z) * C + c;
-    const float inv = rsqrtf(var_c[i] + eps) * sqrtf(var_s[si]);   // batch_normalization(scale=sqrt(style_var))
-    // y = (x - mc)*inv + ms ; out = alpha*y + (1-alpha)*x
-    scale[i] = alpha * inv + (1.f - alpha);
-    shift[i] = alpha * (mean_s[si] - mean_c[i] * inv);
+    inv[i] = rsqrtf(var_c[i] + eps) * sqrtf(var_s[si]);
+    ms[i] = mean_s[si];
 }
-__global__ void k_affine_apply(const __half* __restrict__ in, ActGeom g, const float* __restrict__ scale,
-                               const float* __restrict__ shift, __half* __restrict__ out) {
+// y = (x - mc) * inv + ms, out = alpha * y + (1 - alpha) * x.  Centred first, as tf.nn.batch_normalization is: folded into
+// x * scale + shift, the shift of a channel with a large mean and a small spread is the difference of two large fp32 terms.
+__global__ void k_affine_apply(const __half* __restrict__ in, ActGeom g, const float* __restrict__ mean_c,
+                               const float* __restrict__ inv, const float* __restrict__ ms, float alpha, __half* __restrict__ out) {
     const int cgs = g.C / 8;
     const long long total = (long long)g.N * g.H * g.W * cgs;
     for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < (unsigned)total; i += gridDim.x * blockDim.x) {
@@ -579,10 +599,11 @@ __global__ void k_affine_apply(const __half* __restrict__ in, ActGeom g, const f
         const int n = (int)(pix / (unsigned)g.H);
         float v[8];
         load8(in, g, ((long long)n * g.Hp + y + 1) * g.Wp + x + 1, c0, v);
-        const float* sc = scale + (long long)n * g.C + c0;
-        const float* sh = shift + (long long)n * g.C + c0;
+        const float* mc = mean_c + (long long)n * g.C + c0;
+        const float* iv = inv + (long long)n * g.C + c0;
+        const float* m_s = ms + (long long)n * g.C + c0;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = fmaf(v[j], sc[j], sh[j]);
+        for (int j = 0; j < 8; ++j) v[j] = fmaf(alpha, fmaf(v[j] - mc[j], iv[j], m_s[j]), (1.f - alpha) * v[j]);
         Half8 hi, lo;
         split8(v, hi, lo);
         store8_with_halo(out, g, n, y, x, c0, hi, lo);
@@ -595,15 +616,14 @@ __global__ void k_affine_apply(const __half* __restrict__ in, ActGeom g, const f
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 struct WctWs {
-    size_t sum, sumsq, dsum, mean, var, G, A0, lam, sigma, dvec, Wc, Cs, T, Msplit, bias, conv, kcount, ok, scale, shift, total;
+    size_t shift, dsum, mean, var, G, A0, lam, sigma, dvec, Wc, Cs, T, Msplit, bias, conv, kcount, ok, inv, ms, total;
 };
 static WctWs wct_layout(int C, int Nc, int Ns) {
     WctWs w;
     const size_t np = (size_t)Nc + Ns;
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
-    w.sum = take(np * C * 8);          // AdaIN: fp64 sums / sums of squares (contiguous: one memset clears both)
-    w.sumsq = take(np * C * 8);
+    w.shift = take(np * C * 4);        // AdaIN: centring shift of the channel moments (k_sample_shift)
     w.dsum = take(np * C * 8);         // WCT: fp64 sums of the shifted features (cov_tc.cu)
     w.mean = take(np * C * 4);
     w.var = take(np * C * 4);
@@ -620,25 +640,26 @@ static WctWs wct_layout(int C, int Nc, int Ns) {
     w.conv = take(np * 16 * 4);
     w.kcount = take(np * 2 * 4);
     w.ok = take(np * 4);               // matrices whose W / C_s came from the matrix-function fast path (matfun_tc.cu)
-    w.scale = take((size_t)Nc * C * 4);
-    w.shift = take((size_t)Nc * C * 4);
+    w.inv = take((size_t)Nc * C * 4);  // AdaIN: rsqrt(vc + eps) sqrt(vs) and the style mean, per (frame, channel)
+    w.ms = take((size_t)Nc * C * 4);
     w.total = o;
     return w;
 }
 size_t wct_workspace_bytes(int C, int Nc, int Ns) { return wct_layout(C, Nc, Ns).total; }
 
-template <bool SQ>
-static int launch_sums(const __half* act, ActGeom g, double* sum, double* sumsq, cudaStream_t st) {
+int launch_sample_shift(const __half* act, ActGeom g, float* shift, cudaStream_t st);   // cov_tc.cu
+
+// per-channel mean and biased variance of a feature batch: shift, slot partials (`part`: [N][slices][2][C]), fixed-order finalize
+static int launch_moments(const __half* act, ActGeom g, float* shift, float* part, float* mean, float* var, cudaStream_t st) {
     const long long HW = (long long)g.H * g.W;
-    // enough blocks to fill the chip (~4 per SM) even for small feature maps, at most 1024 px per block
-    long long chunk = (HW * g.N + 591) / 592;
-    const int rows = 256 / (g.C / 8) > 0 ? 256 / (g.C / 8) : 1;
-    chunk = (chunk + rows - 1) / rows * rows;
-    if (chunk < rows) chunk = rows;
-    if (chunk > 1024) chunk = 1024;
-    dim3 grid((unsigned)cdiv(HW, chunk), (unsigned)g.N);
-    k_chan_sums<SQ><<<grid, 256, 0, st>>>(act, g, chunk, sum, sumsq);
-    WCTB_CHECK_LAUNCH("k_chan_sums");
+    const int slice = moments_slice(g.C);
+    const int nslices = cdiv(HW, slice);
+    int rc = launch_sample_shift(act, g, shift, st);
+    if (rc) return rc;
+    k_chan_moments<<<dim3((unsigned)nslices, (unsigned)g.N), 256, 0, st>>>(act, g, shift, slice, part);
+    WCTB_CHECK_LAUNCH("k_chan_moments");
+    k_moments_finalize<<<cdiv((long long)g.N * g.C, 256), 256, 0, st>>>(part, shift, g.C, nslices, HW, g.N * g.C, mean, var);
+    WCTB_CHECK_LAUNCH("k_moments_finalize");
     return 0;
 }
 
@@ -906,31 +927,28 @@ int launch_adain_level(const __half* content, int Nc, int Hc, int Wc, const __ha
         return WCTB200_EWS;
     }
     uint8_t* w = static_cast<uint8_t*>(ws);
-    double* sum = reinterpret_cast<double*>(w + L.sum);
-    double* sumsq = reinterpret_cast<double*>(w + L.sumsq);
+    float* shift = reinterpret_cast<float*>(w + L.shift);
     float* mean = reinterpret_cast<float*>(w + L.mean);
     float* var = reinterpret_cast<float*>(w + L.var);
-    float* scale = reinterpret_cast<float*>(w + L.scale);
-    float* shift = reinterpret_cast<float*>(w + L.shift);
-    WCTB_CUDA(cudaMemsetAsync(w + L.sum, 0, L.dsum - L.sum, st));
+    float* inv = reinterpret_cast<float*>(w + L.inv);
+    float* ms = reinterpret_cast<float*>(w + L.ms);
+    // slot partials of both sides in the per-stream scratch (their count depends on H x W, the workspace size does not)
+    const size_t part_c = (size_t)Nc * cdiv((long long)Hc * Wc, moments_slice(C)) * 2 * C;
+    const size_t part_s = (size_t)Ns * cdiv((long long)Hs * Ws, moments_slice(C)) * 2 * C;
+    float* part = nullptr;
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&part), (part_c + part_s) * sizeof(float), st, 5); if (rc0) return rc0; }
     ActGeom gc(Nc, Hc, Wc, C), gs(Ns, Hs, Ws, C);
-    int rc = launch_sums<true>(content, gc, sum, sumsq, st);
+    int rc = launch_moments(content, gc, shift, part, mean, var, st);
     if (rc) return rc;
-    rc = launch_sums<true>(style, gs, sum + (long long)Nc * C, sumsq + (long long)Nc * C, st);
+    const long long oc = (long long)Nc * C;
+    rc = launch_moments(style, gs, shift + oc, part + part_c, mean + oc, var + oc, st);
     if (rc) return rc;
-    k_mean_finalize<<<cdiv((long long)Nc * C, 256), 256, 0, st>>>(sum, sumsq, (long long)Hc * Wc, Nc * C, mean, var);
-    WCTB_CHECK_LAUNCH("k_mean_finalize(c)");
-    k_mean_finalize<<<cdiv((long long)Ns * C, 256), 256, 0, st>>>(sum + (long long)Nc * C, sumsq + (long long)Nc * C,
-                                                                  (long long)Hs * Ws, Ns * C, mean + (long long)Nc * C,
-                                                                  var + (long long)Nc * C);
-    WCTB_CHECK_LAUNCH("k_mean_finalize(s)");
-    k_adain_coeffs<<<cdiv((long long)Nc * C, 256), 256, 0, st>>>(mean, var, mean + (long long)Nc * C, var + (long long)Nc * C, C,
-                                                                 Nc, Ns, alpha, eps, scale, shift);
+    k_adain_coeffs<<<cdiv(oc, 256), 256, 0, st>>>(var, mean + oc, var + oc, C, Nc, Ns, eps, inv, ms);
     WCTB_CHECK_LAUNCH("k_adain_coeffs");
     const long long total = (long long)Nc * Hc * Wc * (C / 8);
     long long blocks = (total + 255) / 256;
     if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
-    k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(content, gc, scale, shift, out);
+    k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(content, gc, mean, inv, ms, alpha, out);
     WCTB_CHECK_LAUNCH("k_affine_apply");
     return 0;
 }

@@ -255,7 +255,7 @@ class Engine(object):
         out = self._act(content.N, content.H, content.W, content.C)
         ws = self._workspace(content.C, content.N, style.N)
         if adain:
-            self._call("adain_level[C%d]" % content.C, 6, self.lib.wctb200_adain_level, content.ptr, content.N, content.H,
+            self._call("adain_level[C%d]" % content.C, 8, self.lib.wctb200_adain_level, content.ptr, content.N, content.H,
                        content.W, style.ptr, style.N, style.H, style.W, content.C, float(alpha), 1e-5, out.ptr,
                        ws.data_ptr(), ws.numel(), st,
                        bytes_=4.0 * content.C * (2 * content.N * content.H * content.W + style.N * style.H * style.W))
