@@ -1,21 +1,30 @@
 """Per-layer conv micro-benchmark: every conv shape of the 512x512 pipeline (3x3 layers and the UP2 layers that absorbed an
 UpSampling2D), default dispatch vs fused MMA off.  TFLOP/s = EXECUTED algorithmic flops (2*taps*Cin*Cout per output pixel).
 
-  python tools/conv_bench.py [BATCH] [--fixed]
+  python tools/conv_bench.py [BATCH] [--fixed] [--products N] [--digest]
 
 --fixed: the per-tile cost that does not scale with K = 9*Cin (epilogue, tile hand-over, pipeline fill), from pairs of
 3x3 convs with the same output shape and Cout whose Cin differs by 2x: they run the same tiles and the same epilogue, and
 the second has twice the k-iterations, so  fixed = 2 t(Cin) - t(2 Cin)  and  mainloop(Cin) = t(2 Cin) - t(Cin).  Both are
-turned into SM-microseconds per 128 x BN tile (time x #SMs / tiles) and into SM clocks at the clock read after timing."""
-import os, subprocess, sys
+turned into SM-microseconds per 128 x BN tile (time x #SMs / tiles) and into SM clocks at the clock read after timing.
+
+--products N: split-fp16 products per MAC (wctb200_debug_set_conv_products: 3 = default, 1 = a_hi b_hi only).  N = 1 cuts
+the tensor work 3x and leaves the operand traffic as it is, so the ratio of the two times tells a feed-bound mainloop from a
+tensor-bound one.
+
+--digest: seeded inputs, and a SHA-256 of each shape's default-dispatch output bytes (both planes, halo included), so that
+two builds can be compared output for output."""
+import hashlib, os, subprocess, sys
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from wct_tf_b200 import _capi
 from tests import gpu_util as U
 
-ARGS = [a for a in sys.argv[1:] if not a.startswith("--")]
-B = int(ARGS[0]) if ARGS else 8
 FIXED = "--fixed" in sys.argv
+DIGEST = "--digest" in sys.argv
+PRODUCTS = int(sys.argv[sys.argv.index("--products") + 1]) if "--products" in sys.argv else 3
+ARGS = [a for i, a in enumerate(sys.argv[1:]) if not a.startswith("--") and sys.argv[i] != "--products"]
+B = int(ARGS[0]) if ARGS else 8
 # (output H=W, Cin, Cout, up2)
 SHAPES = [(512, 64, 64, 0), (256, 64, 128, 0), (256, 128, 128, 0), (256, 128, 64, 0), (128, 128, 256, 0), (128, 256, 256, 0),
           (128, 256, 128, 0), (64, 256, 512, 0), (64, 512, 512, 0), (64, 512, 256, 0), (32, 512, 512, 0),
@@ -24,6 +33,7 @@ CFGS = [("default", -1), ("nofuse", 0), ("fuse", 1)]
 # --fixed: (output H=W, Cin, Cout); each shape is timed at Cin and at 2*Cin
 FIXED_PAIRS = [(512, 64, 64), (256, 64, 128), (256, 128, 64), (128, 256, 256)]
 lib = U.lib()
+assert lib.wctb200_debug_set_conv_products(PRODUCTS) == PRODUCTS, "--products takes 1, 2 or 3"
 
 
 def conv_ms(hw, cin, cout, reps=20):
@@ -75,8 +85,11 @@ if FIXED:
     _capi.check(lib.wctb200_check_device(U.stream()))
     sys.exit(0)
 
-print("%-24s" % "HxW Cin->Cout" + "".join("%18s" % c[0] for c in CFGS) + "   (executed TFLOP/s, batch %d)" % B)
-for hw, cin, cout, up2 in SHAPES:
+print("%-24s" % "HxW Cin->Cout" + "".join("%18s" % c[0] for c in CFGS) + "   (executed TFLOP/s, batch %d, %d products)" % (
+    B, PRODUCTS))
+for si, (hw, cin, cout, up2) in enumerate(SHAPES):
+    if DIGEST:
+        torch.manual_seed(1000 + si)
     hin = hw // 2 if up2 else hw
     x = torch.randn(B, hin, hin, cin, device="cuda").relu_()
     xin = torch.empty(lib.wctb200_act_bytes(B, hin, hin, cin), dtype=torch.uint8, device="cuda")
@@ -88,7 +101,7 @@ for hw, cin, cout, up2 in SHAPES:
         _capi.check(lib.wctb200_prep_conv_weights_up2(k.data_ptr(), cin, cout, ws.data_ptr(), U.stream()))
     else:
         _capi.check(lib.wctb200_prep_conv_weights(k.data_ptr(), 9, cin, cout, ws.data_ptr(), U.stream()))
-    out = torch.empty(lib.wctb200_act_bytes(B, hw, hw, cout), dtype=torch.uint8, device="cuda")
+    out = torch.zeros(lib.wctb200_act_bytes(B, hw, hw, cout), dtype=torch.uint8, device="cuda")
     flops = 2.0 * (4 if up2 else 9) * cin * cout * B * hw * hw
     row = "%-24s" % ("%dx%d %d->%d%s" % (hw, hw, cin, cout, " up2" if up2 else ""))
     for name, fuse in CFGS:
@@ -103,6 +116,11 @@ for hw, cin, cout, up2 in SHAPES:
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 10
         row += "%10.0f (%5.0fus)" % (flops / ms / 1e9, ms * 1e3)
+        if DIGEST and fuse == -1:
+            digest = hashlib.sha256(out.cpu().numpy().tobytes()).hexdigest()[:16]
+    if DIGEST:
+        row += "   sha256 %s" % digest
     print(row, flush=True)
 lib.wctb200_debug_set_conv_fuse(-1)
+lib.wctb200_debug_set_conv_products(3)
 _capi.check(lib.wctb200_check_device(U.stream()))

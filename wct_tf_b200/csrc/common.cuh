@@ -342,7 +342,11 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 // K-major, 128B-swizzled shared-memory operand descriptor (tile rows are 128 bytes = 64 fp16 of K; 8-row groups
 // 1024 B apart; the tile base is 1024-byte aligned).  Bit layout: sm_90 GMMA descriptor (start >> 4 at [0,14),
 // LBO >> 4 at [16,30), SBO >> 4 at [32,46), layout type at [62,64): 1 = SWIZZLE_128B).  A 16-wide k-step inside the
-// 128-byte row advances the start address by 32 bytes.
+// 128-byte row advances the start address by 32 bytes.  The swizzle follows the absolute shared-memory address, so an
+// operand may also start at any 128-byte row of a swizzled tile (the conv's column taps, 0..15 rows into a strip) with
+// the base-offset field [49,52) left 0.  Measured on an H100 with a wgmma m64n64k16 at row offsets 0..79 of a swizzled
+// tile: base offset 0 gave the exact product at every offset; (start >> 7) & 7 there was wrong at every offset that is
+// not a multiple of 8.  tests/test_gpu_conv_strip.py runs the conv at every row residue.
 __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);

@@ -10,10 +10,16 @@
 // NHWC tensor, viewed as a 2-D matrix [P = N*(H+2)*(W+2) padded positions][C].  For an
 // output position p (padded coordinates) and filter tap (ky,kx) the input row is simply
 // p + (ky-1)*(W+2) + (kx-1): each tap of a 128-position output tile is ONE dense
-// 128 x 64 TMA box at a shifted row coordinate (rows outside [0,P) are zero-filled by
+// 128 x 64 block of rows at a shifted row coordinate (rows outside [0,P) are zero-filled by
 // TMA and only feed halo/junk outputs, which the epilogue never stores).
 //
 //   D[128 pos][BN cout] = sum_{tap, cin-slice}  A_tap[128][64] * W_tap[BN][64]^T
+//
+// Activation strips.  The column taps kx = 0, 1, 2 of filter row ky read the same rows shifted by one, so ONE TMA box of
+// 128 + 2 rows per (filter row, 64-channel slice) feeds all three: column tap kx is a wgmma operand that starts kx rows
+// (128*kx bytes) into the 128B-swizzled strip.  A k-iteration then loads only its tap's weights; the strip is loaded once
+// per ncol k-iterations (3x3: 3, UP2: 2, TAPS: kw, APPLY: 1).  3x3 operand bytes per k-iteration: 64 KB -> 43 KB at
+// BN = 128, 48 KB -> 27 KB at BN = 64.
 //
 // UP2 (nearest x2 upsampling folded into the conv that follows it).  Output pixel (2i+a, 2j+b) of
 // conv3x3(reflect_pad(upsample2(L))) only ever reads the 2x2 low-resolution neighbourhood
@@ -50,6 +56,8 @@ struct ConvParams {
     int mode;             // ConvMode
     int taps;             // 9 (3x3), 1 (apply), 4 (up2: per output parity), kw*kw (taps)
     int kw;               // CONV_TAPS: filter width (top-left anchored kw x kw correlation, style-swap patches)
+    int ncol;             // column taps per filter row, all fed from one strip: 3 (3x3), 2 (up2), kw (taps), 1 (apply)
+    int strip_rows;       // rows of one strip box: 127 + ncol (pool: 66 per segment)
     int products;         // 3 (default): a_hi b_hi + a_hi b_lo + a_lo b_hi; 2: without a_lo b_hi; 1: a_hi b_hi only (experiment knob)
     int per_image;        // tiles never straddle images; weight/bias set = image index (APPLY with nsets > 1)
     int pool;             // CONV_3X3 + WCTB200_POOL2: M tile = 2 image rows x 64 columns, 2x2 max-pool in the epilogue
@@ -78,14 +86,18 @@ __device__ __forceinline__ int region_of(const uint8_t* labels, const int* count
 // ===========================================================================
 // Persistent CTAs, warp-specialised (384 threads):
 //   warps 0-7: two consumer warpgroups.  Warpgroup w multiplies rows [64w, 64w + 64) of the 128-position tile with
-//              wgmma (m64 x N x k16, both operands K-major from the 128B-swizzled stages, fp32 accumulators in registers),
-//              writes its rows of the fp32 tile to shared memory and returns to the mainloop;
+//              wgmma (m64 x N x k16, both operands K-major and 128B-swizzled, fp32 accumulators in registers), writes its
+//              rows of the fp32 tile to shared memory and returns to the mainloop;
 //   warps 8-11: producer warpgroup; lane 0 of warp 8 issues the TMA loads, warps 9-11 run the epilogue of the tile the
 //              consumers handed over while those already multiply the next one.  setmaxnreg moves registers from this
 //              warpgroup to the consumers (the register file is allocated in whole warpgroups: 288 threads would cap every
 //              thread at 168).
 //   * grid = #SMs x oversubscription, every CTA walks a static tile list (cout tile fastest, so CTAs running together
 //     share activation tiles in L2 and the whole weight tensor stays L2 resident);
+//   * two operand rings, each with its own full / empty mbarriers: the A ring holds activation strips (BN = 128: 2,
+//     BN = 64: 3), the B ring one tap's [b_hi | b_lo] per k-iteration (BN = 128: 2, BN = 64: 4).  k-iterations run in
+//     the order (filter row, channel slice, column tap), so a strip is released after its last column tap.  With one
+//     channel slice (Cin = 64) this is the tap order of a ring without strips, and the sums are the same bit for bit;
 //   * chunked accumulation: CH k-iterations accumulate into register chunks that start from zero (one for a_hi b_hi, one
 //     for the two small cross products) and are then added into the running sum with round-to-nearest FADDs.  The tensor
 //     core adds into its fp32 accumulator with truncation; short chunks summed in registers keep the conv at fp32-class
@@ -102,10 +114,18 @@ template <int BN, bool FUSE_>
 struct Conv2Cfg {
     static constexpr int BM = 128;
     static constexpr int BK = 64;
-    static constexpr int A_BYTES = BM * BK * 2;
+    // A ring: one strip per (filter row, 64-channel slice), both planes.  A plane holds the 128 + ncol - 1 rows that the
+    // filter row's column taps read (TAPS: ncol = kw <= 16) or, for POOL2, two segments of 64 + 2 rows, each segment
+    // starting on a 1024-byte swizzle atom; 144 rows cover every mode.
+    static constexpr int STRIP_ROWS = 144;
+    static constexpr int POOL_SEG_ROWS = 72;
+    static constexpr int PLANE_BYTES = STRIP_ROWS * 128;
+    static constexpr int STRIP_BYTES = 2 * PLANE_BYTES;
+    // B ring: one tap's [b_hi | b_lo] per k-iteration
     static constexpr int B_BYTES = BN * BK * 2;
-    static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-    static constexpr int STAGES = BN == 64 ? 3 : 2;
+    static constexpr int B_SLOT_BYTES = 2 * B_BYTES;
+    static constexpr int A_STAGES = BN == 64 ? 3 : 2;
+    static constexpr int B_STAGES = BN == 64 ? 4 : 2;
     // FUSE (BN = 64): the products a_hi*b_hi and a_hi*b_lo share the A operand and the two weight planes sit back to back
     // in a stage, so ONE wgmma with N = 2*BN computes both into adjacent accumulator column ranges (summed when the chunk
     // is added up); a_lo*b_hi follows with N = BN into the first range.  2 instead of 3 wgmma per k-step.
@@ -122,7 +142,10 @@ struct Conv2Cfg {
     static constexpr int PITCH = BN + 8;
     static constexpr int TILE_BYTES = BM * PITCH * 4;
     static constexpr int AUX_BYTES = 256 + 2 * BN * 4;          // mbarriers + abort flag, then the bias of two passes
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + TILE_BYTES + 1024;
+    static constexpr int RING_BYTES = A_STAGES * STRIP_BYTES + B_STAGES * B_SLOT_BYTES;
+    static constexpr int SMEM_BYTES = RING_BYTES + AUX_BYTES + TILE_BYTES + 1024;
+    static_assert(SMEM_BYTES <= 227 * 1024, "conv: shared memory exceeds the 227 KB opt-in limit");
+    static_assert(8 * (2 * A_STAGES + 2 * B_STAGES + 2) + 4 <= 256, "conv: mbarriers overflow the aux block");
 };
 
 struct TileCoord {
@@ -340,15 +363,18 @@ __device__ __forceinline__ void epi_pool(const ConvParams& p, const ActGeom& go,
 // plain apply costs.
 template <int BN, bool FUSE_, bool REG = false>
 __global__ void __launch_bounds__(Conv2Cfg<BN, FUSE_>::THREADS, 1)
-conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                const __grid_constant__ CUtensorMap mapA64, const ConvParams p, const int total_tiles, const int n_tiles) {
+conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const ConvParams p,
+                const int total_tiles, const int n_tiles) {
     using Cfg = Conv2Cfg<BN, FUSE_>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* aux = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
-    uint64_t* full = reinterpret_cast<uint64_t*>(aux);
-    uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tile_full = empty + Cfg::STAGES;           // the fp32 tile is written (one arrival per consumer warp)
+    uint8_t* bring = smem + Cfg::A_STAGES * Cfg::STRIP_BYTES;
+    uint8_t* aux = smem + Cfg::RING_BYTES;
+    uint64_t* fullA = reinterpret_cast<uint64_t*>(aux);
+    uint64_t* emptyA = fullA + Cfg::A_STAGES;
+    uint64_t* full = emptyA + Cfg::A_STAGES;             // B ring
+    uint64_t* empty = full + Cfg::B_STAGES;
+    uint64_t* tile_full = empty + Cfg::B_STAGES;         // the fp32 tile is written (one arrival per consumer warp)
     uint64_t* tile_empty = tile_full + 1;                // the fp32 tile is read (one arrival per epilogue warp)
     volatile int* abort_flag = reinterpret_cast<volatile int*>(tile_empty + 1);
     float* sbias = reinterpret_cast<float*>(aux + 256);  // [2][BN]: bias of the pass (by pass parity)
@@ -363,9 +389,13 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         if (s_prev_err != 0u) return;
     }
     if (threadIdx.x == 0) {
-        for (int s = 0; s < Cfg::STAGES; ++s) {
+        for (int s = 0; s < Cfg::A_STAGES; ++s) {
+            mbar_init(&fullA[s], 1);
+            mbar_init(&emptyA[s], Cfg::CONSUMERS / 32);     // one arrival per consumer warp
+        }
+        for (int s = 0; s < Cfg::B_STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], Cfg::CONSUMERS / 32);      // one arrival per consumer warp
+            mbar_init(&empty[s], Cfg::CONSUMERS / 32);
         }
         mbar_init(tile_full, Cfg::CONSUMERS / 32);
         mbar_init(tile_empty, Cfg::EPI_WARPS);
@@ -376,8 +406,12 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     }
     __syncthreads();
 
+    // k-iteration order: (filter row, channel slice, column tap), column tap innermost, so that one strip feeds ncol
+    // consecutive k-iterations
     const int ksl = p.Cin / Cfg::BK;
     const int kiters = p.taps * ksl;
+    const int ncol = REG ? 1 : p.ncol;                   // the regions apply is a 1x1 conv
+    const bool pool = !REG && p.pool;
     const int nchunks = (kiters + Cfg::CH - 1) / Cfg::CH;
 
     // register split, checked with ptxas -v to spill nothing: the consumers of BN = 128 need more than 200 and the epilogue
@@ -390,39 +424,53 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         setmaxnreg_dec<EPI_REGS>();
         if (warp == Cfg::CONSUMERS / 32) {
             if (lane != 0) return;
-            uint32_t itg = 0;
+            // the whole box counts towards the transaction bytes, rows zero-filled outside [0, P) included
+            const uint32_t strip_tx = (pool ? 4u : 2u) * (uint32_t)p.strip_rows * 128u;
+            uint32_t itg = 0, stg = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
                 unsigned todo = 1u;                      // passes over the tile (REG: one per region present)
                 if constexpr (REG) todo = p.amask[tile / n_tiles] & ((1u << p.R) - 1u);
                 for (; todo; todo &= todo - 1u) {
                 const int set = REG ? (tile / n_tiles) / p.tiles_per_image * p.R + (__ffs(todo) - 1) : tc.set;
+                int fr = 0, ks = 0, kx = 0;                  // filter row, channel slice, column tap of k-iteration it
                 for (int it = 0; it < kiters; ++it, ++itg) {
-                    const int s = itg % Cfg::STAGES;
-                    const uint32_t ph = (itg / Cfg::STAGES) & 1;
-                    mbar_wait(&empty[s], ph ^ 1u, abort_flag, p.err, 0x100u + s);
-                    const int tap = it / ksl;
-                    const int ks = it - tap * ksl;
-                    int off = 0;
-                    if (p.mode == CONV_3X3) off = (tap / 3 - 1) * p.Wp + (tap % 3 - 1);
-                    else if (p.mode == CONV_TAPS) off = (tap / p.kw) * p.Wp + (tap % p.kw);
-                    else if (p.mode == CONV_UP2) off = ((tap >> 1) - 1 + (tc.cls >> 1)) * p.Wp + ((tap & 1) - 1 + (tc.cls & 1));
-                    const int row = (int)(tc.p0 + off);
-                    uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-                    mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
-                    if (p.pool) {
-                        // two 64-position boxes per plane: the segment of image row 2i and the one below it
-                        tma_load_3d(st, &mapA64, &full[s], ks * Cfg::BK, row, 0);
-                        tma_load_3d(st + Cfg::A_BYTES / 2, &mapA64, &full[s], ks * Cfg::BK, row + p.Wp, 0);
-                        tma_load_3d(st + Cfg::A_BYTES, &mapA64, &full[s], ks * Cfg::BK, row, 1);
-                        tma_load_3d(st + Cfg::A_BYTES + Cfg::A_BYTES / 2, &mapA64, &full[s], ks * Cfg::BK, row + p.Wp, 1);
-                    } else {
-                        tma_load_3d(st, &mapA, &full[s], ks * Cfg::BK, row, 0);
-                        tma_load_3d(st + Cfg::A_BYTES, &mapA, &full[s], ks * Cfg::BK, row, 1);
+                    if (kx == 0) {
+                        // the strip of (fr, ks): the first row its column tap 0 reads
+                        const int sa = stg % Cfg::A_STAGES;
+                        mbar_wait(&emptyA[sa], ((stg / Cfg::A_STAGES) & 1) ^ 1u, abort_flag, p.err, 0x110u + sa);
+                        int off = 0;
+                        if (p.mode == CONV_3X3) off = (fr - 1) * p.Wp - 1;
+                        else if (p.mode == CONV_TAPS) off = fr * p.Wp;
+                        else if (p.mode == CONV_UP2) off = (fr - 1 + (tc.cls >> 1)) * p.Wp + (tc.cls & 1) - 1;
+                        const int row = (int)(tc.p0 + off);
+                        uint8_t* sp = smem + sa * Cfg::STRIP_BYTES;
+                        mbar_arrive_expect_tx(&fullA[sa], strip_tx);
+                        if (pool) {
+                            // two segments per plane: the one of image row 2i and the one below it
+                            constexpr int SEG = Cfg::POOL_SEG_ROWS * 128;
+                            tma_load_3d(sp, &mapA, &fullA[sa], ks * Cfg::BK, row, 0);
+                            tma_load_3d(sp + SEG, &mapA, &fullA[sa], ks * Cfg::BK, row + p.Wp, 0);
+                            tma_load_3d(sp + Cfg::PLANE_BYTES, &mapA, &fullA[sa], ks * Cfg::BK, row, 1);
+                            tma_load_3d(sp + Cfg::PLANE_BYTES + SEG, &mapA, &fullA[sa], ks * Cfg::BK, row + p.Wp, 1);
+                        } else {
+                            tma_load_3d(sp, &mapA, &fullA[sa], ks * Cfg::BK, row, 0);
+                            tma_load_3d(sp + Cfg::PLANE_BYTES, &mapA, &fullA[sa], ks * Cfg::BK, row, 1);
+                        }
                     }
-                    tma_load_3d(st + 2 * Cfg::A_BYTES, &mapB, &full[s], tap * p.Cin + ks * Cfg::BK, tc.n0, set * 2);
-                    tma_load_3d(st + 2 * Cfg::A_BYTES + Cfg::B_BYTES, &mapB, &full[s], tap * p.Cin + ks * Cfg::BK,
-                                tc.n0, set * 2 + 1);
+                    const int s = itg % Cfg::B_STAGES;
+                    const uint32_t ph = (itg / Cfg::B_STAGES) & 1;
+                    mbar_wait(&empty[s], ph ^ 1u, abort_flag, p.err, 0x100u + s);
+                    const int k0 = (fr * ncol + kx) * p.Cin + ks * Cfg::BK;
+                    uint8_t* sp = bring + s * Cfg::B_SLOT_BYTES;
+                    mbar_arrive_expect_tx(&full[s], Cfg::B_SLOT_BYTES);
+                    tma_load_3d(sp, &mapB, &full[s], k0, tc.n0, set * 2);
+                    tma_load_3d(sp + Cfg::B_BYTES, &mapB, &full[s], k0, tc.n0, set * 2 + 1);
+                    if (++kx == ncol) {
+                        kx = 0;
+                        ++stg;
+                        if (++ks == ksl) { ks = 0; ++fr; }
+                    }
                 }
                 }
             }
@@ -468,7 +516,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     setmaxnreg_inc<MMA_REGS>();
     const int wg = warp >> 2;                            // rows [64 wg, 64 wg + 64) of the tile
     const int t = threadIdx.x & 127;
-    uint32_t itg = 0, pass = 0;
+    uint32_t itg = 0, stg = 0, pass = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         unsigned todo = 1u;
         if constexpr (REG) todo = p.amask[tile / n_tiles] & ((1u << p.R) - 1u);
@@ -476,7 +524,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         float sum[Cfg::SUM_REGS];
 #pragma unroll
         for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
-        int it = 0;
+        int it = 0, kx = 0;
         for (int c = 0; c < nchunks; ++c) {
             float ch[Cfg::CHUNK_REGS], cx[Cfg::SUM_REGS];
 #pragma unroll
@@ -485,14 +533,18 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             for (int i = 0; i < Cfg::SUM_REGS; ++i) cx[i] = 0.f;
             const int it_end = min(kiters, (c + 1) * Cfg::CH);
             for (; it < it_end; ++it, ++itg) {
-                const int s = itg % Cfg::STAGES;
-                const uint32_t ph = (itg / Cfg::STAGES) & 1;
+                const int sa = stg % Cfg::A_STAGES;
+                if (kx == 0) mbar_wait(&fullA[sa], (stg / Cfg::A_STAGES) & 1, abort_flag, p.err, 0x210u + sa);
+                const int s = itg % Cfg::B_STAGES;
+                const uint32_t ph = (itg / Cfg::B_STAGES) & 1;
                 mbar_wait(&full[s], ph, abort_flag, p.err, 0x200u + s);
-                const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
-                const uint64_t a_hi = gmma_desc_sw128(st + wg * (Cfg::A_BYTES / 2));
-                const uint64_t a_lo = gmma_desc_sw128(st + Cfg::A_BYTES + wg * (Cfg::A_BYTES / 2));
-                const uint64_t b_hi = gmma_desc_sw128(st + 2 * Cfg::A_BYTES);
-                const uint64_t b_lo = gmma_desc_sw128(st + 2 * Cfg::A_BYTES + Cfg::B_BYTES);
+                // this warpgroup's operand rows: tile rows 64 wg .. (POOL2: the second segment), column tap kx kx rows further
+                const uint32_t sta = smem_u32(smem + sa * Cfg::STRIP_BYTES) + (wg * (pool ? Cfg::POOL_SEG_ROWS : 64) + kx) * 128;
+                const uint64_t a_hi = gmma_desc_sw128(sta);
+                const uint64_t a_lo = gmma_desc_sw128(sta + Cfg::PLANE_BYTES);
+                const uint32_t stb = smem_u32(bring + s * Cfg::B_SLOT_BYTES);
+                const uint64_t b_hi = gmma_desc_sw128(stb);
+                const uint64_t b_lo = gmma_desc_sw128(stb + Cfg::B_BYTES);
                 const bool first = (it == c * Cfg::CH);
                 wgmma_fence();
                 if (p.products >= 3) conv_stage_mma<Cfg, 3>(ch, cx, a_hi, a_lo, b_hi, b_lo, first);
@@ -503,7 +555,12 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 acc_fence(ch);
                 acc_fence(cx);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[s]);   // stage may be refilled
+                if (lane == 0) mbar_arrive(&empty[s]);   // slot may be refilled
+                if (++kx == ncol) {                    // last column tap of the strip
+                    kx = 0;
+                    ++stg;
+                    if (lane == 0) mbar_arrive(&emptyA[sa]);
+                }
             }
             if constexpr (Cfg::FUSE) {
 #pragma unroll
@@ -570,8 +627,8 @@ int make_tensor_map_3d(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d
 int g_conv_oversub = 4;
 
 template <int BN, bool FUSE_, bool REG = false>
-static int launch2_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mA64, const ConvParams& p, int total_tiles,
-                      int n_tiles, cudaStream_t st) {
+static int launch2_bn(const CUtensorMap& mA, const CUtensorMap& mB, const ConvParams& p, int total_tiles, int n_tiles,
+                      cudaStream_t st) {
     using Cfg = Conv2Cfg<BN, FUSE_>;
     WCTB_ENSURE_SMEM((conv_tc2_kernel<BN, FUSE_, REG>), Cfg::SMEM_BYTES);
     // Over-subscribed persistent grid: with g_conv_oversub x #SMs CTAs (1 resident per SM) the
@@ -580,7 +637,7 @@ static int launch2_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtens
     // (a grid of exactly #SMs would run as two unbalanced waves).
     int grid = device_sm_count() * (g_conv_oversub > 0 ? g_conv_oversub : 1);
     if (grid > total_tiles) grid = total_tiles;
-    conv_tc2_kernel<BN, FUSE_, REG><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(mA, mB, mA64, p, total_tiles, n_tiles);
+    conv_tc2_kernel<BN, FUSE_, REG><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(mA, mB, p, total_tiles, n_tiles);
     WCTB_CHECK_LAUNCH("conv_tc2_kernel");
     return 0;
 }
@@ -618,23 +675,24 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
     int BN = Cout % 128 == 0 ? 128 : 64;
     if (g_conv_bn_override && Cout % g_conv_bn_override == 0) BN = g_conv_bn_override > 128 ? 128 : g_conv_bn_override;
 
+    // one strip box per (filter row, channel slice) holds the rows of all its column taps
+    const int ncol = mode == CONV_3X3 ? 3 : (mode == CONV_UP2 ? 2 : (mode == CONV_TAPS ? kw : 1));
+    const int strip_rows = pool ? 64 + 2 : 127 + ncol;
     CUtensorMap mA, mB;
-    int rc = make_tensor_map_3d(&mA, in, (uint64_t)Cin, (uint64_t)gi.P, 2, (uint64_t)Cin * 2, (uint64_t)gi.plane * 2, 128);
+    int rc = make_tensor_map_3d(&mA, in, (uint64_t)Cin, (uint64_t)gi.P, 2, (uint64_t)Cin * 2, (uint64_t)gi.plane * 2,
+                                (uint32_t)strip_rows);
     if (rc) return rc;
     const uint64_t K = (uint64_t)taps * Cin;
     rc = make_tensor_map_3d(&mB, w_split, K, (uint64_t)Cout, (uint64_t)2 * wsets, K * 2, K * Cout * 2, (uint32_t)BN);
     if (rc) return rc;
-    CUtensorMap mA64 = mA;
-    if (pool) {
-        rc = make_tensor_map_3d(&mA64, in, (uint64_t)Cin, (uint64_t)gi.P, 2, (uint64_t)Cin * 2, (uint64_t)gi.plane * 2, 64);
-        if (rc) return rc;
-    }
 
     ConvParams p;
     p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.Hp = gi.Hp; p.Wp = gi.Wp; p.P = gi.P;
     p.mode = mode;
     p.taps = taps;
     p.kw = kw;
+    p.ncol = ncol;
+    p.strip_rows = strip_rows;
     p.products = (mode == CONV_3X3 || mode == CONV_UP2) ? g_conv_products : 3;    // the knob only touches the encoder / decoder convs
     p.nsets = nsets;
     p.per_image = nsets > 1 ? 1 : 0;
@@ -661,16 +719,16 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
     const int total = m_tiles * n_tiles * (mode == CONV_UP2 ? 4 : 1);
     if (reg) {
         switch (BN) {
-            case 64: return g_conv_fuse == 0 ? launch2_bn<64, false, true>(mA, mB, mA64, p, total, n_tiles, st)
-                                             : launch2_bn<64, true, true>(mA, mB, mA64, p, total, n_tiles, st);
-            default: return launch2_bn<128, false, true>(mA, mB, mA64, p, total, n_tiles, st);
+            case 64: return g_conv_fuse == 0 ? launch2_bn<64, false, true>(mA, mB, p, total, n_tiles, st)
+                                             : launch2_bn<64, true, true>(mA, mB, p, total, n_tiles, st);
+            default: return launch2_bn<128, false, true>(mA, mB, p, total, n_tiles, st);
         }
     }
     switch (BN) {
         // fused [b_hi|b_lo] wgmma (Conv2Cfg::FUSE) at BN=64 unless switched off; at BN=128 it would need N = 256
-        case 64: return g_conv_fuse == 0 ? launch2_bn<64, false>(mA, mB, mA64, p, total, n_tiles, st)
-                                         : launch2_bn<64, true>(mA, mB, mA64, p, total, n_tiles, st);
-        default: return launch2_bn<128, false>(mA, mB, mA64, p, total, n_tiles, st);
+        case 64: return g_conv_fuse == 0 ? launch2_bn<64, false>(mA, mB, p, total, n_tiles, st)
+                                         : launch2_bn<64, true>(mA, mB, p, total, n_tiles, st);
+        default: return launch2_bn<128, false>(mA, mB, p, total, n_tiles, st);
     }
 }
 
