@@ -186,6 +186,34 @@ WCTB200_API size_t wctb200_wct_regions_workspace_bytes(int C, int Nc, int R, int
 WCTB200_API int wctb200_wct_apply_regions(const void* content, int Nc, int Hc, int Wc, int C, const uint8_t* labels, int R,
                               const void* const* states, float alpha, float eps_cov, float eps_eig, float thresh,
                               int readd_content_mean, void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
+/* Style interpolation (WCT paper, section 4): the transform of wctb200_wct_apply (same semantics flags) against a weighted
+ * blend of K styles.  The transform is affine in the style statistics, so the blend runs on the states: frame n is coloured
+ * with C_w = sum_k w_k C_sk and shifted by m_w = sum_k w_k m_sk (an fp32 fmaf chain in k order), so that
+ *   out = sum_k w_k * wct_apply(states[k])   when a row sums to 1.
+ * The weights are used as given (no normalisation).  A one-hot row, or K = 1 with weight 1, is byte-identical to
+ * wctb200_wct_apply with that state.
+ * states: HOST array of K device pointers, each a state of wctb200_wct_style_prepare with Ns = 1 (styles may have any size).
+ * weights: DEVICE fp32 [Nw][K], Nw = 1 (one row for every frame) or Nw = Nc (row n for frame n).
+ * K in 1..8, Nw in {1, Nc}, else WCTB200_EINVAL (also for a null state).  ws: device scratch of
+ * wctb200_wct_blend_workspace_bytes(C, Nc, K, Nw).  k_out (device int32 [2*(Nc+K)], may be NULL):
+ * [k_c x Nc | k_s x K | sweeps_c x Nc | sweeps_s x K]. */
+WCTB200_API size_t wctb200_wct_blend_workspace_bytes(int C, int Nc, int K, int Nw);
+WCTB200_API int wctb200_wct_apply_blend(const void* content, int Nc, int Hc, int Wc, int C,
+                            const void* const* states, int K, const float* weights, int Nw,
+                            float alpha, float eps_cov, float eps_eig, float thresh, int readd_content_mean,
+                            void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
+/* AdaIN against a weighted blend of K styles: the moments of each style, then per (frame, channel)
+ * y = (x-mc)*rsqrt(vc+eps)*sum_k w_k sqrt(v_sk) + sum_k w_k m_sk, out = alpha*y + (1-alpha)*x, so that
+ *   out = sum_k w_k * adain_level(styles[k])   when a row sums to 1.
+ * styles: HOST array of K device pointers, style k SPF16 [1,Hs[k],Ws[k],C]; Hs, Ws: HOST int arrays of K.  weights as for
+ * wctb200_wct_apply_blend (DEVICE fp32 [Nw][K], Nw in {1, Nc}, used as given).  K in 1..8, else WCTB200_EINVAL.
+ * ws: device scratch of wctb200_adain_blend_workspace_bytes(C, Nc, K).  K = 1 with weight 1 is byte-identical to
+ * wctb200_adain_level with Ns = 1. */
+WCTB200_API size_t wctb200_adain_blend_workspace_bytes(int C, int Nc, int K);
+WCTB200_API int wctb200_adain_blend(const void* content, int Nc, int Hc, int Wc, int C,
+                        const void* const* styles, const int* Hs, const int* Ws, int K,
+                        const float* weights, int Nw, float alpha, float eps,
+                        void* out, void* ws, size_t ws_bytes, void* stream);
 /* Label map resampling for spatial control: src device uint8 [N][Hm][Wm] -> dst [N][Hf][Wf] by proportional nearest
  * sampling in integer arithmetic, dst[y][x] = src[((2y+1)*Hm) / (2*Hf)][((2x+1)*Wm) / (2*Wf)] (no divisibility needed). */
 WCTB200_API int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst,

@@ -10,6 +10,10 @@ Spatial control: ``--content-mask MASK --mask-styles S0 S1 ...`` splits the cont
 v -> region v*R // 256 for R styles: a black/white mask with two styles gives background / foreground) and region r takes
 style r; the output is ``<content>_<s0>+<s1>...<ext>``.
 
+Style interpolation: ``--interp-styles S0 S1 ... --interp-weights w0 w1 ...`` stylises with the weighted blend of 1..8
+styles (weights >= 0, normalised to sum 1; WCT or ``--adain``); the output is ``<content>_<s0>-<w0>+<s1>-<w1>...<ext>``
+with the normalised weights.
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -49,11 +53,16 @@ _FLAGS = [
     (("--semantics",), dict(type=str, default="tf", choices=["tf", "np"], help="wct_tf (the reference graph) or wct_np eps/blend rules")),
     (("--content-mask",), dict(type=str, default=None, help="8-bit grayscale region mask: gray v -> region v*R//256 (R = #--mask-styles)")),
     (("--mask-styles",), dict(nargs="+", type=str, default=None, help="one style image per mask region (with --content-mask)")),
+    (("--interp-styles",), dict(nargs="+", type=str, default=None, help="1..8 style images to blend (with --interp-weights)")),
+    (("--interp-weights",), dict(nargs="+", type=float, default=None, help="one weight >= 0 per --interp-styles entry (normalised)")),
 ]
 
 # flags that do not combine with --content-mask
 _MASK_EXCLUDES = [("style_path", "--style-path"), ("adain", "--adain"), ("swap5", "--swap5"), ("concat", "--concat"),
                   ("random", "-r/--random")]
+# flags that do not combine with --interp-styles
+_INTERP_EXCLUDES = [("style_path", "--style-path"), ("random", "-r/--random"), ("swap5", "--swap5"), ("concat", "--concat"),
+                    ("content_mask", "--content-mask")]
 
 
 def build_parser():
@@ -66,6 +75,7 @@ def build_parser():
 def parse_args(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
+    check_interp_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
@@ -77,6 +87,44 @@ def parse_args(argv=None):
     elif args.mask_styles:
         parser.error("--mask-styles needs --content-mask")
     return args
+
+
+def check_interp_flags(parser, args, excludes=_INTERP_EXCLUDES):
+    """--interp-styles / --interp-weights: each needs the other, one weight per style, 1..8 styles, valid weights."""
+    if args.interp_styles is None and args.interp_weights is None:
+        return
+    if args.interp_styles is None:
+        parser.error("--interp-weights needs --interp-styles")
+    if args.interp_weights is None:
+        parser.error("--interp-styles needs --interp-weights")
+    if len(args.interp_styles) != len(args.interp_weights):
+        parser.error("--interp-styles and --interp-weights must have the same length")
+    if len(args.interp_styles) > 8:
+        parser.error("--interp-styles takes at most 8 styles")
+    for attr, flag in excludes:
+        if getattr(args, attr, None):
+            parser.error("--interp-styles does not combine with %s" % flag)
+    try:
+        normalized_weights(args.interp_weights)
+    except ValueError as e:
+        parser.error("--interp-weights: %s" % e)
+
+
+def normalized_weights(weights):
+    """One weight row -> float64 weights that sum to 1 (WCT.normalize_weights: finite, >= 0, positive sum)."""
+    from wct_tf_b200.wct import WCT
+    return WCT.normalize_weights(weights, 1, len(weights), dtype=np.float64)[0]
+
+
+def interp_label(style_paths, weights):
+    """``<s0>-<w0>+<s1>-<w1>...`` with the normalised weights printed with %g."""
+    return "+".join("{}-{:g}".format(os.path.splitext(os.path.basename(p))[0], w)
+                    for p, w in zip(style_paths, normalized_weights(weights)))
+
+
+def interp_output_name(content_path, style_paths, weights):
+    stem, ext = os.path.splitext(os.path.basename(content_path))
+    return "{}_{}{}".format(stem, interp_label(style_paths, weights), ext)
 
 
 def read_mask(path, R):
@@ -156,6 +204,28 @@ def main_masked(args, model, io, dimg, t_start):
     return written
 
 
+def main_interp(args, model, io, dimg, t_start):
+    """--interp-styles: every content image in the weighted blend of the styles."""
+    os.makedirs(args.out_path, exist_ok=True)
+    device = model.engine.device
+    kw = dict(alpha=args.alpha, adain=args.adain, return_device=True, style_weights=np.asarray(args.interp_weights, np.float64))
+    written = 0
+    for content_path in _listing(args.content_path, io):
+        content_dev = dimg.to_device(io.get_img(content_path), device)
+        if args.content_size > 0:
+            content_dev = dimg.resize_to(content_dev, args.content_size)
+        styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device) for p in args.interp_styles]
+        result = model.predict_batch(content_dev, styles_dev, **kw)
+        for _ in range(args.passes - 1):
+            result = model.predict_batch(result, styles_dev, **kw)
+        target = os.path.join(args.out_path, interp_output_name(content_path, args.interp_styles, args.interp_weights))
+        io.save_img(target, dimg.to_host(result[0]))
+        written += 1
+        print("{}: Wrote stylized output image to {}".format(written, target))
+    print("Finished stylizing {} outputs in {}s".format(written, time.time() - t_start))
+    return written
+
+
 def main(argv=None, model_factory=make_model, image_ops=None):
     args = parse_args(argv)
     from wct_tf_b200 import imageio as io
@@ -164,6 +234,8 @@ def main(argv=None, model_factory=make_model, image_ops=None):
     dimg = image_ops
     t_start = time.time()
     model = model_factory(args)
+    if args.interp_styles is not None:
+        return main_interp(args, model, io, dimg, t_start)
     if args.content_mask is not None:
         return main_masked(args, model, io, dimg, t_start)
     styles = _listing(args.style_path, io)

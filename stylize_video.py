@@ -7,6 +7,11 @@ style side of every level is computed once per batch), while a thread pool decod
 previous one, so the GPU never waits for PNG I/O.  ``--in-path`` may also be a directory of frames (then no ffmpeg is
 needed and the stylised frames are left in ``--out-path``); ffmpeg is used only when it is installed.
 Additions: ``--batch``, ``--synthetic-weights``, ``--adain``.
+
+Style interpolation: ``--interp-styles S0 S1 ...`` with ``--interp-weights w0 w1 ...`` stylises every frame with one fixed
+blend (output ``<clip>_<s0>-<w0>+<s1>-<w1>...``), and with ``--morph`` sweeps piecewise-linearly from S0 to the last style
+across the clip (``morph_weights``; output ``<clip>_morph_<s0>+<s1>...``).  A frame's weights depend on its index in the
+clip only, so ``--batch`` does not change a frame.
 """
 from __future__ import division, print_function
 
@@ -26,7 +31,9 @@ import numpy as np
 _VIDEO_FLAGS = [
     (("--in-path",), dict(type=str, required=True, help="video file, or a directory of frames")),
     (("--out-path",), dict(type=str, required=True, help="folder for the encoded videos / stylised frames")),
-    (("--style-path",), dict(type=str, required=True, help="style image, or a folder of them")),
+    (("--style-path",), dict(type=str, default=None, help="style image, or a folder of them (or --interp-styles)")),
+    (("--morph",), dict(action="store_true", default=False,
+                        help="with --interp-styles: sweep piecewise-linearly from the first style to the last across the clip")),
     (("--tmp-dir",), dict(type=str, dest="tmp_dir", default=None, help="where ffmpeg unpacks the frames")),
     (("--keep-tmp",), dict(action="store_true", default=False, help="keep the unpacked frames")),
     (("--batch",), dict(type=int, default=15, help="frames per predict_batch call (not in the reference)")),
@@ -34,7 +41,9 @@ _VIDEO_FLAGS = [
 ]
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
-           "--synthetic-weights")
+           "--synthetic-weights", "--interp-styles", "--interp-weights")
+# flags that do not combine with --interp-styles
+_INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat")]
 
 
 def build_parser():
@@ -48,6 +57,45 @@ def build_parser():
     return parser
 
 
+def parse_args(argv=None):
+    """One of --style-path or --interp-styles; with --interp-styles either --interp-weights (a fixed blend) or --morph."""
+    import stylize
+    parser = build_parser()
+    args = parser.parse_args(argv)
+    if args.morph:
+        if args.interp_styles is None:
+            parser.error("--morph needs --interp-styles")
+        if args.interp_weights is not None:
+            parser.error("--morph does not combine with --interp-weights")
+        if not 2 <= len(args.interp_styles) <= 8:
+            parser.error("--morph needs 2..8 --interp-styles")
+        for attr, flag in _INTERP_EXCLUDES:
+            if getattr(args, attr):
+                parser.error("--interp-styles does not combine with %s" % flag)
+    else:
+        if args.interp_styles is not None and args.interp_weights is None:
+            parser.error("--interp-styles needs --interp-weights or --morph")
+        stylize.check_interp_flags(parser, args, _INTERP_EXCLUDES)
+    if args.interp_styles is None and args.style_path is None:
+        parser.error("--style-path (or --interp-styles) is required")
+    return args
+
+
+def morph_weights(T, K):
+    """Weights [T, K] of a piecewise-linear sweep from style 0 to style K-1 over T frames (float64): frame t sits at
+    p = t (K-1) / (T-1) (0 when T = 1), between styles i = min(floor(p), K-2) and i+1 with w_i = 1 - f, w_i+1 = f, f = p - i."""
+    if K < 2:
+        raise ValueError("a morph needs at least 2 styles")
+    w = np.zeros((T, K), np.float64)
+    for t in range(T):
+        p = t * (K - 1) / (T - 1) if T > 1 else 0.0
+        i = min(int(np.floor(p)), K - 2)
+        f = p - i
+        w[t, i] = 1.0 - f
+        w[t, i + 1] = f
+    return w
+
+
 def frame_key(name):
     """frame_12.png sorts after frame_2.png (the reference iterates os.listdir order; ffmpeg numbers the frames)."""
     digits = ''.join(ch if ch.isdigit() else ' ' for ch in os.path.basename(name)).split()
@@ -59,36 +107,53 @@ def batches(seq, n):
         yield seq[i:i + n]
 
 
-def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device):
+def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device, weights=None):
     """All frames of one clip with one style (a uint8 CUDA tensor, already resized / cropped).  Frames of equal size are
     batched; the decode of batch i+1 and the PNG writes of batch i-1 overlap the GPU work of batch i.  Resize
     (``--content-size``), CORAL (``--keep-colors``), every pass and the ``--concat`` thumbnail run on the device
-    (wct_tf_b200.device_image); a frame crosses PCIe once in each direction."""
+    (wct_tf_b200.device_image); a frame crosses PCIe once in each direction.
+
+    Style interpolation: ``style_img`` is a list of K styles and ``weights`` a float64 [K] blend for every frame or [T, K],
+    row t for frame t of the clip, so a frame's weights do not depend on the batching."""
     def finish(out_f, frame_u8):
         io.save_img(out_f, frame_u8)
 
     def prep(frames_dev):
         return dimg.resize_to(frames_dev, args.content_size) if args.content_size > 0 else frames_dev
 
-    todo = list(batches(list(zip(in_files, out_files)), max(1, args.batch)))
+    def interp_kw(lo, hi):
+        if weights is None:
+            return {}
+        return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
+
+    def coral(style, fr):
+        if isinstance(style, list):
+            return [dimg.preserve_colors_np(s, fr) for s in style]
+        return dimg.preserve_colors_np(style, fr)
+
+    step = max(1, args.batch)
+    todo = list(batches(list(zip(in_files, out_files)), step))
     pending_loads = [pool.submit(io.get_img, f) for f, _ in todo[0]] if todo else []
     writes, count = [], 0
     for bi, group in enumerate(todo):
         frames = [f.result() for f in pending_loads]
         pending_loads = [pool.submit(io.get_img, f) for f, _ in todo[bi + 1]] if bi + 1 < len(todo) else []
         same = all(fr.shape == frames[0].shape for fr in frames) and not args.keep_colors and not args.swap5
+        first = bi * step                                      # clip index of the batch's first frame
         if same and len(frames) > 1:
             x = prep(dimg.to_device(np.stack(frames), device))
             # --passes (stylize_video.py:119-121) run back to back on the device
-            out = wct_model.predict_batch(x, style_img[None], alpha=args.alpha, adain=args.adain, passes=args.passes,
-                                          return_device=True)
+            out = wct_model.predict_batch(x, style_img if weights is not None else style_img[None], alpha=args.alpha,
+                                          adain=args.adain, passes=args.passes, return_device=True,
+                                          **interp_kw(first, first + len(frames)))
             results = [(out[i], style_img) for i in range(len(frames))]
         else:                                                  # per-frame styles (CORAL), style swap or ragged sizes
             results = []
-            for fr in frames:
+            for j, fr in enumerate(frames):
                 fr = prep(dimg.to_device(fr, device))
-                style_rgb = dimg.preserve_colors_np(style_img, fr) if args.keep_colors else style_img
-                kw = dict(alpha=args.alpha, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True)
+                style_rgb = coral(style_img, fr) if args.keep_colors else style_img
+                kw = dict(alpha=args.alpha, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True,
+                          **interp_kw(first + j, first + j + 1))
                 o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, **kw)
                 for _ in range(args.passes - 1):
                     o = wct_model.predict_batch(o, style_rgb, swap5=False, **kw)
@@ -110,7 +175,7 @@ def have_ffmpeg():
 def main(argv=None, wct_factory=None, image_ops=None):
     """``wct_factory`` / ``image_ops`` let the tests drive the frame logic with stand-ins for the engine and for
     wct_tf_b200.device_image; the CLI always uses the real ones."""
-    args = build_parser().parse_args(argv)
+    args = parse_args(argv)
     from wct_tf_b200 import imageio as io
     if image_ops is None:
         from wct_tf_b200 import device_image as image_ops
@@ -129,7 +194,10 @@ def main(argv=None, wct_factory=None, image_ops=None):
     else:
         wct_model = wct_factory(args)
 
-    style_files = io.get_files(args.style_path) if os.path.isdir(args.style_path) else [args.style_path]
+    if args.interp_styles is not None:
+        style_files = [None]                                   # one run with the blend of every --interp-styles image
+    else:
+        style_files = io.get_files(args.style_path) if os.path.isdir(args.style_path) else [args.style_path]
     os.makedirs(args.out_path, exist_ok=True)
     from_dir = os.path.isdir(args.in_path)
     tmp_dir = args.tmp_dir or os.path.join(args.out_path, '_____fns_frames_%s' % random.randint(0, 99999))
@@ -149,12 +217,27 @@ def main(argv=None, wct_factory=None, image_ops=None):
     with ThreadPoolExecutor(max_workers=8) as pool:
         for style_fullpath in style_files:                     # stylize_video.py:97
             device = wct_model.engine.device if hasattr(wct_model, "engine") else None
-            style_img = dimg.to_device(io.get_img(style_fullpath), device)
-            if args.style_size > 0:
-                style_img = dimg.resize_to(style_img, args.style_size)
-            if args.crop_size > 0:
-                style_img = dimg.center_crop(style_img, args.crop_size)
-            style_prefix = os.path.basename(os.path.splitext(style_fullpath)[0])
+
+            def load_style(path):
+                img = dimg.to_device(io.get_img(path), device)
+                if args.style_size > 0:
+                    img = dimg.resize_to(img, args.style_size)
+                if args.crop_size > 0:
+                    img = dimg.center_crop(img, args.crop_size)
+                return img
+            weights = None
+            if style_fullpath is None:
+                import stylize
+                style_img = [load_style(p) for p in args.interp_styles]
+                if args.morph:
+                    weights = morph_weights(len(in_files), len(args.interp_styles))
+                    style_prefix = "morph_" + "+".join(os.path.splitext(os.path.basename(p))[0] for p in args.interp_styles)
+                else:
+                    weights = np.asarray(args.interp_weights, np.float64)     # normalised by WCT.predict_batch
+                    style_prefix = stylize.interp_label(args.interp_styles, args.interp_weights)
+            else:
+                style_img = load_style(style_fullpath)
+                style_prefix = os.path.basename(os.path.splitext(style_fullpath)[0])
             out_v = os.path.join(args.out_path, '{}_{}{}'.format(clip, style_prefix, ext))
             frames_dir = os.path.join(args.out_path if from_dir else tmp_dir, '{}_{}_frames'.format(clip, style_prefix))
             if os.path.isfile(out_v):                          # stylize_video.py:108-110
@@ -162,7 +245,7 @@ def main(argv=None, wct_factory=None, image_ops=None):
                 continue
             os.makedirs(frames_dir, exist_ok=True)
             out_files = [os.path.join(frames_dir, os.path.splitext(os.path.basename(f))[0] + '.png') for f in in_files]
-            n = stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device)
+            n = stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device, weights)
             total += n
             print("Stylized {} frames with {} -> {}".format(n, style_prefix, frames_dir))
             # stylize_video.py:137-149 re-encodes "frame_%d.png".  Frames extracted by ffmpeg carry that name; a user-supplied

@@ -51,7 +51,12 @@ SIGNATURES = {
     "wctb200_jacobi_eigh": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
     "wctb200_wct_regions_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "wctb200_wct_apply_regions": (_i, [_vp, _i, _i, _i, _i, _vp, _i, C.POINTER(_vp), _f, _f, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
-    "wctb200_labels_resize_nearest": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "wctb200_wct_blend_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "wctb200_wct_apply_blend": (_i, [_vp, _i, _i, _i, _i, C.POINTER(_vp), _i, _vp, _i, _f, _f, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_adain_blend_workspace_bytes": (_sz, [_i, _i, _i]),
+    "wctb200_adain_blend": (_i, [_vp, _i, _i, _i, _i, C.POINTER(_vp), C.POINTER(_i), C.POINTER(_i), _i, _vp, _i, _f, _f, _vp, _vp,
+                                 _sz, _vp]),
+    "wctb200_labels_resize_nearest":(_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "wctb200_covariance_regions": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp]),
     "wctb200_style_swap_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i]),
     "wctb200_style_swap_level": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _vp, _sz, _vp]),
@@ -102,6 +107,11 @@ def load():
 def pointer_array(ptrs):
     """Host array of device pointers (``const void* const*`` arguments, e.g. the style states of wct_apply_regions)."""
     return (_vp * len(ptrs))(*[int(p) for p in ptrs])
+
+
+def int_array(vals):
+    """Host int array (``const int*`` arguments, e.g. the style sizes of adain_blend)."""
+    return (_i * len(vals))(*[int(v) for v in vals])
 
 
 def check(rc):

@@ -110,6 +110,12 @@ int launch_wct_style_prepare(const __half*, int, int, int, int, float, float, fl
 int launch_wct_apply(const __half*, int, int, int, int, const void*, int, float, float, float, float, int, __half*, int32_t*,
                      void*, size_t, cudaStream_t);
 int launch_covariance(const __half*, int, int, int, int, float, float*, float*, cudaStream_t);
+size_t wct_blend_workspace_bytes(int C, int Nc, int K, int Nw);
+int launch_wct_apply_blend(const __half*, int, int, int, int, const void* const*, int, const float*, int, float, float, float, float,
+                           int, __half*, int32_t*, void*, size_t, cudaStream_t);
+size_t adain_blend_workspace_bytes(int C, int Nc, int K);
+int launch_adain_blend(const __half*, int, int, int, int, const void* const*, const int*, const int*, int, const float*, int, float,
+                       float, __half*, void*, size_t, cudaStream_t);
 size_t wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc);
 int launch_wct_apply_regions(const __half*, int, int, int, int, const uint8_t*, int, const void* const*, float, float, float, float,
                              int, __half*, int32_t*, void*, size_t, cudaStream_t);
@@ -315,6 +321,34 @@ int wctb200_wct_apply_regions(const void* content, int Nc, int Hc, int Wc, int C
     WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "wct_apply_regions: bad geometry");
     return launch_wct_apply_regions(HCP(content), Nc, Hc, Wc, C, labels, R, states, alpha, eps_cov, eps_eig, thresh,
                                     readd_content_mean, HP(out), k_out, ws, ws_bytes, ST(stream));
+}
+size_t wctb200_wct_blend_workspace_bytes(int C, int Nc, int K, int Nw) {
+    if (C < 8 || Nc < 1 || K < 1 || K > 8 || (Nw != 1 && Nw != Nc)) return 0;
+    return wct_blend_workspace_bytes(C, Nc, K, Nw);
+}
+int wctb200_wct_apply_blend(const void* content, int Nc, int Hc, int Wc, int C, const void* const* states, int K, const float* weights,
+                            int Nw, float alpha, float eps_cov, float eps_eig, float thresh, int readd_content_mean, void* out,
+                            int32_t* k_out, void* ws, size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(content && states && weights && out && ws, "wct_apply_blend: null pointer");
+    WCTB_REQUIRE(K >= 1 && K <= 8, "wct_apply_blend: K=%d not in 1..8", K);
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "wct_apply_blend: bad geometry");
+    return launch_wct_apply_blend(HCP(content), Nc, Hc, Wc, C, states, K, weights, Nw, alpha, eps_cov, eps_eig, thresh,
+                                  readd_content_mean, HP(out), k_out, ws, ws_bytes, ST(stream));
+}
+size_t wctb200_adain_blend_workspace_bytes(int C, int Nc, int K) {
+    if (C < 8 || Nc < 1 || K < 1 || K > 8) return 0;
+    return adain_blend_workspace_bytes(C, Nc, K);
+}
+int wctb200_adain_blend(const void* content, int Nc, int Hc, int Wc, int C, const void* const* styles, const int* Hs, const int* Ws,
+                        int K, const float* weights, int Nw, float alpha, float eps, void* out, void* ws, size_t ws_bytes,
+                        void* stream) {
+    WCTB_REQUIRE(content && styles && Hs && Ws && weights && out && ws, "adain_blend: null pointer");
+    WCTB_REQUIRE(K >= 1 && K <= 8, "adain_blend: K=%d not in 1..8", K);
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "adain_blend: bad geometry");
+    for (int k = 0; k < K; ++k)
+        WCTB_REQUIRE(geom_ok(1, Hs[k], Ws[k], C), "adain_blend: bad geometry of style %d", k);
+    return launch_adain_blend(HCP(content), Nc, Hc, Wc, C, styles, Hs, Ws, K, weights, Nw, alpha, eps, HP(out), ws, ws_bytes,
+                              ST(stream));
 }
 int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, void* stream) {
     WCTB_REQUIRE(src && dst, "labels_resize_nearest: null pointer");

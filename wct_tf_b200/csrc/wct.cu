@@ -847,32 +847,17 @@ int launch_wct_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C,
     return 0;
 }
 
-int launch_wct_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha,
-                     float eps_cov, float eps_eig, float thresh, int readd, __half* out, int32_t* k_out, void* ws,
-                     size_t ws_bytes, cudaStream_t st) {
-    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_apply: C=%d not in {64,128,256,512}", C);
-    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "wct_apply: Ns must be 1 or Nc");
-    const WctWs L = wct_layout(C, Nc, 0);
-    if (ws_bytes < L.total) {
-        set_error("wct_apply: workspace %zu < %zu bytes", ws_bytes, L.total);
-        return WCTB200_EWS;
-    }
-    uint8_t* w = static_cast<uint8_t*>(ws);
-    size_t off_cs, off_k;
-    style_state_offsets(C, Ns, &off_cs, &off_k);
-    const uint8_t* sp = static_cast<const uint8_t*>(state);
-    const float* mean_s = reinterpret_cast<const float*>(sp);
-    const float* Cs = reinterpret_cast<const float*>(sp + off_cs);
-    const int* ks = reinterpret_cast<const int*>(sp + off_k);
+// Content side of the split transform (wct_apply, wct_apply_blend) in the workspace `w` of wct_layout(C, Nc, 0): means and
+// covariances of the Nc frames, then W_c = A^-1/2 by the matrix-function fast path or the eigensolver.  The kcount slot
+// receives [k_c x Nc | sweeps_c x Nc].
+static int wct_content_side(const __half* content, int Nc, int Hc, int Wc, int C, float eps_cov, float eps_eig, float thresh,
+                            uint8_t* w, const WctWs& L, cudaStream_t st) {
     double* dsum = reinterpret_cast<double*>(w + L.dsum);
     float* mean = reinterpret_cast<float*>(w + L.mean);
     float* G = reinterpret_cast<float*>(w + L.G);
     float* sigma = reinterpret_cast<float*>(w + L.sigma);
     float* dvec = reinterpret_cast<float*>(w + L.dvec);
     float* Wcm = reinterpret_cast<float*>(w + L.Wc);
-    float* T = reinterpret_cast<float*>(w + L.T);
-    __half* Msplit = reinterpret_cast<__half*>(w + L.Msplit);
-    float* bias = reinterpret_cast<float*>(w + L.bias);
     float* conv = reinterpret_cast<float*>(w + L.conv);
     int* kc = reinterpret_cast<int*>(w + L.kcount);
     const long long CC = (long long)C * C;
@@ -891,12 +876,49 @@ int launch_wct_apply(const __half* content, int Nc, int Hc, int Wc, int C, const
     dim3 gg((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc);
     k_outer_gemm<<<gg, 256, 0, st>>>(G, CC, G, CC, dvec, C, Wcm, CC, C, ok);
     WCTB_CHECK_LAUNCH("k_outer_gemm(Wc)");
+    return 0;
+}
+
+// Style side of the split transform after wct_content_side: T = C_s W_c, the split-fp16 operand M and the bias, then
+// out = M x + bias on the tensor cores.  C_s [Ns][C][C] and mean_s [Ns][C] with Ns == 1 (shared) or Ns == Nc (per frame).
+static int wct_colour_apply(const __half* content, int Nc, int Hc, int Wc, int C, const float* Cs, const float* mean_s, int Ns,
+                            float alpha, int readd, uint8_t* w, const WctWs& L, __half* out, cudaStream_t st) {
+    const float* mean = reinterpret_cast<const float*>(w + L.mean);
+    const float* Wcm = reinterpret_cast<const float*>(w + L.Wc);
+    float* T = reinterpret_cast<float*>(w + L.T);
+    __half* Msplit = reinterpret_cast<__half*>(w + L.Msplit);
+    float* bias = reinterpret_cast<float*>(w + L.bias);
+    const long long CC = (long long)C * C;
+    dim3 gg((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc);
     k_outer_gemm<<<gg, 256, 0, st>>>(Cs, Ns == 1 ? 0 : CC, Wcm, CC, nullptr, 0, T, CC, C);   // T = C_s W_c
     WCTB_CHECK_LAUNCH("k_outer_gemm(T)");
     dim3 gf((unsigned)cdiv(C, 8), (unsigned)Nc);
     k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean_s, Msplit, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform");
-    rc = launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, Msplit, Nc, nullptr, bias, C, 0, out, st);
+    return launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, Msplit, Nc, nullptr, bias, C, 0, out, st);
+}
+
+int launch_wct_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha,
+                     float eps_cov, float eps_eig, float thresh, int readd, __half* out, int32_t* k_out, void* ws,
+                     size_t ws_bytes, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_apply: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "wct_apply: Ns must be 1 or Nc");
+    const WctWs L = wct_layout(C, Nc, 0);
+    if (ws_bytes < L.total) {
+        set_error("wct_apply: workspace %zu < %zu bytes", ws_bytes, L.total);
+        return WCTB200_EWS;
+    }
+    uint8_t* w = static_cast<uint8_t*>(ws);
+    size_t off_cs, off_k;
+    style_state_offsets(C, Ns, &off_cs, &off_k);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    const float* mean_s = reinterpret_cast<const float*>(sp);
+    const float* Cs = reinterpret_cast<const float*>(sp + off_cs);
+    const int* ks = reinterpret_cast<const int*>(sp + off_k);
+    int* kc = reinterpret_cast<int*>(w + L.kcount);
+    int rc = wct_content_side(content, Nc, Hc, Wc, C, eps_cov, eps_eig, thresh, w, L, st);
+    if (rc) return rc;
+    rc = wct_colour_apply(content, Nc, Hc, Wc, C, Cs, mean_s, Ns, alpha, readd, w, L, out, st);
     if (rc) return rc;
     if (k_out) {
         // k_out: [k_c x Nc | k_s x Ns | sweeps_c x Nc | sweeps_s x Ns]  (same order as wct_level)
@@ -904,6 +926,113 @@ int launch_wct_apply(const __half* content, int Nc, int Hc, int Wc, int C, const
         WCTB_CUDA(cudaMemcpyAsync(k_out + Nc, ks, (size_t)Ns * 4, cudaMemcpyDeviceToDevice, st));
         WCTB_CUDA(cudaMemcpyAsync(k_out + Nc + Ns, kc + Nc, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
         WCTB_CUDA(cudaMemcpyAsync(k_out + 2 * Nc + Ns, ks + Ns, (size_t)Ns * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// Style interpolation (WCT paper, section 4): a weighted blend of K styles.  Both transforms are affine in the style
+// statistics, so for weights that sum to 1 the blend of the K outputs is the transform of the blended statistics:
+//   WCT    sum_k w_k (a (C_sk W_c (x - m_c) + m_sk) + (1 - a) base) = a (C_w W_c (x - m_c) + m_w) + (1 - a) base,
+//          C_w = sum_k w_k C_sk, m_w = sum_k w_k m_sk;
+//   AdaIN  the same with sigma_w = sum_k w_k sqrt(v_sk) and mu_w = sum_k w_k mu_sk.
+// The blend runs on the small per-style state; the content side and the tensor-core apply run once.
+// ---------------------------------------------------------------------------
+struct BlendSrc {
+    const float* Cs[8];
+    const float* ms[8];
+};
+
+// For every weight row (blockIdx.y of Nw rows of K): Cs_w = sum_k w[k] Cs_k and ms_w = sum_k w[k] ms_k, an fp32 fmaf chain
+// in k order that starts from the product w[0] S_0.  A one-hot row reproduces its style bit for bit.
+__global__ void __launch_bounds__(256)
+k_blend_styles(BlendSrc src, int K, const float* __restrict__ weights, int C, float* __restrict__ Cs, float* __restrict__ ms) {
+    const int row = blockIdx.y;
+    const long long CC4 = (long long)C * C / 4, n4 = CC4 + C / 4;
+    float wk[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) wk[k] = k < K ? weights[(long long)row * K + k] : 0.f;
+    float4* cs_out = reinterpret_cast<float4*>(Cs + (long long)row * C * C);
+    float4* ms_out = reinterpret_cast<float4*>(ms + (long long)row * C);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+        const bool is_cs = i < CC4;
+        const long long j = is_cs ? i : i - CC4;
+        float4 s = is_cs ? reinterpret_cast<const float4*>(src.Cs[0])[j] : reinterpret_cast<const float4*>(src.ms[0])[j];
+        float4 a = make_float4(__fmul_rn(wk[0], s.x), __fmul_rn(wk[0], s.y), __fmul_rn(wk[0], s.z), __fmul_rn(wk[0], s.w));
+#pragma unroll
+        for (int k = 1; k < 8; ++k) {
+            if (k < K) {
+                s = is_cs ? reinterpret_cast<const float4*>(src.Cs[k])[j] : reinterpret_cast<const float4*>(src.ms[k])[j];
+                a = make_float4(fmaf(wk[k], s.x, a.x), fmaf(wk[k], s.y, a.y), fmaf(wk[k], s.z, a.z), fmaf(wk[k], s.w, a.w));
+            }
+        }
+        if (is_cs) cs_out[j] = a;
+        else ms_out[j] = a;
+    }
+}
+
+struct BlendWs {
+    size_t base, Cs, ms, total;
+};
+static BlendWs blend_layout(int C, int Nc, int Nw) {
+    BlendWs L;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.base = take(wct_layout(C, Nc, 0).total);   // the content side and apply, as wct_apply's
+    L.Cs = take((size_t)Nw * C * C * 4);         // the blended style states, one per weight row
+    L.ms = take((size_t)Nw * C * 4);
+    L.total = o;
+    return L;
+}
+size_t wct_blend_workspace_bytes(int C, int Nc, int K, int Nw) {
+    (void)K;
+    return blend_layout(C, Nc, Nw).total;
+}
+
+int launch_wct_apply_blend(const __half* content, int Nc, int Hc, int Wc, int C, const void* const* states, int K,
+                           const float* weights, int Nw, float alpha, float eps_cov, float eps_eig, float thresh, int readd,
+                           __half* out, int32_t* k_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_apply_blend: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(K >= 1 && K <= 8, "wct_apply_blend: K=%d not in 1..8", K);
+    WCTB_REQUIRE(Nw == 1 || Nw == Nc, "wct_apply_blend: Nw=%d must be 1 or Nc=%d", Nw, Nc);
+    const BlendWs BL = blend_layout(C, Nc, Nw);
+    if (ws_bytes < BL.total) {
+        set_error("wct_apply_blend: workspace %zu < %zu bytes", ws_bytes, BL.total);
+        return WCTB200_EWS;
+    }
+    // each state from wct_style_prepare with Ns = 1: [C] mean_s | [C][C] C_s | k_s, sweeps
+    size_t off_cs, off_k;
+    style_state_offsets(C, 1, &off_cs, &off_k);
+    BlendSrc src = {};
+    for (int k = 0; k < K; ++k) {
+        WCTB_REQUIRE(states[k], "wct_apply_blend: style state %d is null", k);
+        const uint8_t* sp = static_cast<const uint8_t*>(states[k]);
+        src.ms[k] = reinterpret_cast<const float*>(sp);
+        src.Cs[k] = reinterpret_cast<const float*>(sp + off_cs);
+    }
+    const WctWs L = wct_layout(C, Nc, 0);
+    uint8_t* w = static_cast<uint8_t*>(ws) + BL.base;
+    float* Cs = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + BL.Cs);
+    float* ms = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + BL.ms);
+    int rc = wct_content_side(content, Nc, Hc, Wc, C, eps_cov, eps_eig, thresh, w, L, st);
+    if (rc) return rc;
+    const long long n4 = ((long long)C * C + C) / 4;
+    long long blocks = cdiv(n4, 256);
+    if (blocks > device_sm_count() * 4ll) blocks = device_sm_count() * 4ll;
+    k_blend_styles<<<dim3((unsigned)blocks, (unsigned)Nw), 256, 0, st>>>(src, K, weights, C, Cs, ms);
+    WCTB_CHECK_LAUNCH("k_blend_styles");
+    rc = wct_colour_apply(content, Nc, Hc, Wc, C, Cs, ms, Nw, alpha, readd, w, L, out, st);
+    if (rc) return rc;
+    if (k_out) {
+        // k_out: [k_c x Nc | k_s x K | sweeps_c x Nc | sweeps_s x K]
+        const int* kc = reinterpret_cast<const int*>(w + L.kcount);
+        WCTB_CUDA(cudaMemcpyAsync(k_out, kc, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(k_out + Nc + K, kc + Nc, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
+        for (int k = 0; k < K; ++k) {
+            const int* ks = reinterpret_cast<const int*>(static_cast<const uint8_t*>(states[k]) + off_k);
+            WCTB_CUDA(cudaMemcpyAsync(k_out + Nc + k, ks, 4, cudaMemcpyDeviceToDevice, st));
+            WCTB_CUDA(cudaMemcpyAsync(k_out + 2 * Nc + K + k, ks + 1, 4, cudaMemcpyDeviceToDevice, st));
+        }
     }
     return 0;
 }
@@ -945,6 +1074,89 @@ int launch_adain_level(const __half* content, int Nc, int Hc, int Wc, const __ha
     if (rc) return rc;
     k_adain_coeffs<<<cdiv(oc, 256), 256, 0, st>>>(var, mean + oc, var + oc, C, Nc, Ns, eps, inv, ms);
     WCTB_CHECK_LAUNCH("k_adain_coeffs");
+    const long long total = (long long)Nc * Hc * Wc * (C / 8);
+    long long blocks = (total + 255) / 256;
+    if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
+    k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(content, gc, mean, inv, ms, alpha, out);
+    WCTB_CHECK_LAUNCH("k_affine_apply");
+    return 0;
+}
+
+// AdaIN of a style blend: inv = rsqrt(vc + eps) * sum_k w_k sqrt(v_sk) and ms = sum_k w_k m_sk per (frame, channel), in k
+// order from the product w_0 S_0 (K = 1 with weight 1 gives k_adain_coeffs' values bit for bit).  Weight row z, or 0 if Nw == 1.
+__global__ void k_adain_blend_coeffs(const float* __restrict__ var_c, const float* __restrict__ mean_s, const float* __restrict__ var_s,
+                                     int C, int Nc, int K, const float* __restrict__ weights, int Nw, float eps,
+                                     float* __restrict__ inv, float* __restrict__ ms) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= Nc * C) return;
+    const int z = i / C, c = i % C;
+    const float* wr = weights + (long long)(Nw == 1 ? 0 : z) * K;
+    float s = __fmul_rn(wr[0], sqrtf(var_s[c])), m = __fmul_rn(wr[0], mean_s[c]);
+    for (int k = 1; k < K; ++k) {
+        s = fmaf(wr[k], sqrtf(var_s[(long long)k * C + c]), s);
+        m = fmaf(wr[k], mean_s[(long long)k * C + c], m);
+    }
+    inv[i] = rsqrtf(var_c[i] + eps) * s;
+    ms[i] = m;
+}
+
+struct AdainBlendWs {
+    size_t shift, mean, var, inv, ms, total;
+};
+static AdainBlendWs adain_blend_layout(int C, int Nc, int K) {
+    AdainBlendWs L;
+    const size_t np = (size_t)Nc + K;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.shift = take(np * C * 4);        // content frames then the K styles
+    L.mean = take(np * C * 4);
+    L.var = take(np * C * 4);
+    L.inv = take((size_t)Nc * C * 4);
+    L.ms = take((size_t)Nc * C * 4);
+    L.total = o;
+    return L;
+}
+size_t adain_blend_workspace_bytes(int C, int Nc, int K) { return adain_blend_layout(C, Nc, K).total; }
+
+int launch_adain_blend(const __half* content, int Nc, int Hc, int Wc, int C, const void* const* styles, const int* Hs, const int* Ws,
+                       int K, const float* weights, int Nw, float alpha, float eps, __half* out, void* ws, size_t ws_bytes,
+                       cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_blend: C=%d must be a multiple of 8 (<= 2048)", C);
+    WCTB_REQUIRE(K >= 1 && K <= 8, "adain_blend: K=%d not in 1..8", K);
+    WCTB_REQUIRE(Nw == 1 || Nw == Nc, "adain_blend: Nw=%d must be 1 or Nc=%d", Nw, Nc);
+    const AdainBlendWs L = adain_blend_layout(C, Nc, K);
+    if (ws_bytes < L.total) {
+        set_error("adain_blend: workspace %zu < %zu bytes", ws_bytes, L.total);
+        return WCTB200_EWS;
+    }
+    uint8_t* w = static_cast<uint8_t*>(ws);
+    float* shift = reinterpret_cast<float*>(w + L.shift);
+    float* mean = reinterpret_cast<float*>(w + L.mean);
+    float* var = reinterpret_cast<float*>(w + L.var);
+    float* inv = reinterpret_cast<float*>(w + L.inv);
+    float* ms = reinterpret_cast<float*>(w + L.ms);
+    // slot partials of the content and of every style in the per-stream scratch, as adain_level's
+    size_t part_off[9];
+    part_off[0] = (size_t)Nc * cdiv((long long)Hc * Wc, moments_slice(C)) * 2 * C;
+    for (int k = 0; k < K; ++k) {
+        WCTB_REQUIRE(styles[k], "adain_blend: style %d is null", k);
+        WCTB_REQUIRE(Hs[k] >= 2 && Ws[k] >= 2, "adain_blend: style %d is %dx%d", k, Hs[k], Ws[k]);
+        part_off[k + 1] = part_off[k] + (size_t)cdiv((long long)Hs[k] * Ws[k], moments_slice(C)) * 2 * C;
+    }
+    float* part = nullptr;
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&part), part_off[K] * sizeof(float), st, 5); if (rc0) return rc0; }
+    ActGeom gc(Nc, Hc, Wc, C);
+    int rc = launch_moments(content, gc, shift, part, mean, var, st);
+    if (rc) return rc;
+    const long long oc = (long long)Nc * C;
+    for (int k = 0; k < K; ++k) {
+        const long long o = oc + (long long)k * C;
+        rc = launch_moments(static_cast<const __half*>(styles[k]), ActGeom(1, Hs[k], Ws[k], C), shift + o, part + part_off[k], mean + o,
+                            var + o, st);
+        if (rc) return rc;
+    }
+    k_adain_blend_coeffs<<<cdiv(oc, 256), 256, 0, st>>>(var, mean + oc, var + oc, C, Nc, K, weights, Nw, eps, inv, ms);
+    WCTB_CHECK_LAUNCH("k_adain_blend_coeffs");
     const long long total = (long long)Nc * Hc * Wc * (C / 8);
     long long blocks = (total + 255) / 256;
     if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;

@@ -332,12 +332,7 @@ class Engine(object):
         sem = SEMANTICS[self.semantics]
         C, N, R = content.C, content.N, len(states)
         out = self._act(N, content.H, content.W, C)
-        nbytes = self.lib.wctb200_wct_regions_workspace_bytes(C, N, R, content.H, content.W)
-        key = (self._group, "regions", C, N, R)        # grow-only: the levels of a call differ in H x W
-        ws = self._ws.get(key)
-        if ws is None or ws.numel() < nbytes:
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            self._ws[key] = ws
+        ws = self._grow_workspace(("regions", C, N, R), self.lib.wctb200_wct_regions_workspace_bytes(C, N, R, content.H, content.W))
         kbuf = torch.empty(2 * (N * R + R), dtype=torch.int32, device=self.device) if want_info else None
         hwc = content.H * content.W
         self._call("wct_regions[C%d]" % C, 12 + self._matfun_launches(C), self.lib.wctb200_wct_apply_regions, content.ptr, N,
@@ -347,9 +342,48 @@ class Engine(object):
                    flops=2.0 * C * C * 2 * N * hwc, bytes_=4.0 * C * 2 * N * hwc)
         return out, kbuf
 
+    def _grow_workspace(self, key, nbytes):
+        """Grow-only scratch per (group, key): the levels of a call differ in size."""
+        key = (self._group,) + key
+        ws = self._ws.get(key)
+        if ws is None or ws.numel() < nbytes:
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            self._ws[key] = ws
+        return ws
+
+    def wct_apply_blend(self, content, states, weights, alpha, want_info=False):
+        """Style interpolation on one level: frame n takes the blend of the K style ``states`` with the weights of row n of
+        ``weights`` (cuda fp32 [1|N, K]; one row: every frame)."""
+        st = self._stream()
+        sem = SEMANTICS[self.semantics]
+        C, N, K, Nw = content.C, content.N, len(states), weights.shape[0]
+        out = self._act(N, content.H, content.W, C)
+        ws = self._grow_workspace(("blend", C, N, K, Nw), self.lib.wctb200_wct_blend_workspace_bytes(C, N, K, Nw))
+        kbuf = torch.empty(2 * (N + K), dtype=torch.int32, device=self.device) if want_info else None
+        hwc = content.H * content.W
+        self._call("wct_blend[C%d]" % C, 10 + self._matfun_launches(C), self.lib.wctb200_wct_apply_blend, content.ptr, N, content.H,
+                   content.W, C, _capi.pointer_array([s.data_ptr() for s in states]), K, weights.data_ptr(), Nw, float(alpha),
+                   sem["eps_cov"], sem["eps_eig"], sem["thresh"], sem["readd"], out.ptr, kbuf.data_ptr() if want_info else None,
+                   ws.data_ptr(), ws.numel(), st, flops=2.0 * C * C * 2 * N * hwc, bytes_=4.0 * C * 2 * N * hwc)
+        return out, kbuf
+
+    def adain_blend(self, content, styles, weights, alpha):
+        """AdaIN against the blend of the K style feature maps ``styles`` (each [1,Hs,Ws,C], any sizes) with the weights of
+        ``weights`` (cuda fp32 [1|N, K])."""
+        st = self._stream()
+        C, N, K, Nw = content.C, content.N, len(styles), weights.shape[0]
+        out = self._act(N, content.H, content.W, C)
+        ws = self._grow_workspace(("adain_blend", C, N, K), self.lib.wctb200_adain_blend_workspace_bytes(C, N, K))
+        hws = sum(s.H * s.W for s in styles)
+        self._call("adain_blend[C%d]" % C, 5 + 3 * K, self.lib.wctb200_adain_blend, content.ptr, N, content.H, content.W, C,
+                   _capi.pointer_array([s.ptr for s in styles]), _capi.int_array([s.H for s in styles]),
+                   _capi.int_array([s.W for s in styles]), K, weights.data_ptr(), Nw, float(alpha), 1e-5, out.ptr, ws.data_ptr(),
+                   ws.numel(), st, bytes_=4.0 * C * (2 * N * content.H * content.W + hws))
+        return out, None
+
     # ------------------------------------------------------------------ pipeline
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
-                ss_patch_size=3, ss_stride=1, labels=None, region_styles=None):
+                ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3], Ns in {1, N}.
         Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -362,8 +396,27 @@ class Engine(object):
         Spatial control: ``labels`` is a cuda uint8 label map [N|1,Hm,Wm] of any resolution and ``region_styles`` a list of
         R (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes; ``style_u8`` is ignored.  At every level the map is resampled
         to the feature grid and region r of a frame is transformed against style r (WCT only); labels >= R keep the
-        content feature.  The R styles are encoded and prepared once per call."""
+        content feature.  The R styles are encoded and prepared once per call.
+
+        Style interpolation: ``interp_styles`` is a list of K (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes and
+        ``interp_weights`` a cuda float32 [1|N, K] tensor; ``style_u8`` is ignored.  Frame n is stylised with the blend of
+        the K styles under weight row n (one row: every frame), which for a row that sums to 1 is the same blend of the K
+        single-style outputs at every level (WCT and AdaIN are affine in the style statistics).  The weights are used as
+        given.  The K styles are encoded (and, for WCT, prepared) once per call."""
         N = content_u8.shape[0]
+        if interp_styles is not None:
+            if labels is not None or swap5:
+                raise ValueError("style interpolation does not combine with spatial control (labels) or swap5")
+            K = len(interp_styles)
+            if not 1 <= K <= 8:
+                raise ValueError("style interpolation needs 1..8 styles, got %d" % K)
+            w = interp_weights
+            if (not isinstance(w, torch.Tensor) or w.dtype != torch.float32 or w.dim() != 2 or w.shape[0] not in (1, N)
+                    or w.shape[1] != K or w.device != self.device):
+                raise ValueError("interp_weights must be a float32 tensor [1|N, K] on %s" % self.device)
+            w = w.contiguous()
+            return self._stylize_multi(content_u8, list(interp_styles), alpha, adain, want_info, capture,
+                                       lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]))
         if labels is not None:
             if adain or swap5:
                 raise ValueError("spatial control (labels) works with WCT only: not with adain or swap5")
@@ -375,7 +428,8 @@ class Engine(object):
             if labels.dtype != torch.uint8 or labels.dim() != 3 or labels.shape[0] not in (1, N):
                 raise ValueError("labels must be uint8 [Hm,Wm] or [N,Hm,Wm]")
             labels = labels.expand(N, -1, -1).contiguous()
-            return self._stylize_regions(content_u8, labels, list(region_styles), alpha, want_info, capture)
+            return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
+                                       lambda lo, hi: ("regions", labels[lo:hi]))
         swap5 = bool(swap5) and "relu5_1" in [l.relu_target for l in self.model.levels]    # model.py:148: only relu5_1 swaps
         if swap5:
             if N != 1 or style_u8.shape[0] != 1:
@@ -385,8 +439,6 @@ class Engine(object):
         G = min(self.groups, N) if (capture is None and not want_info) else 1
         if G > 1:
             main = torch.cuda.current_stream(self.device)
-            bounds = [(g * N) // G for g in range(G + 1)]
-            outs = []
             shared = None
             if style_u8.shape[0] == 1 and not adain:
                 # ONE style for the whole batch (video, configs[2]): its encoder pass and eigendecompositions run once,
@@ -396,66 +448,61 @@ class Engine(object):
                     shared = self._style_side(style_u8, True, main)
                 finally:
                     self._group = 0
-            for g in range(G):
-                lo, hi = bounds[g], bounds[g + 1]
-                if g not in self._group_streams:
-                    # descending priority: group 0 runs "in the foreground", later groups fill the SMs it
-                    # leaves idle while its eigendecompositions are latency bound (self.group_priorities)
-                    prio = -1 if (self.group_priorities and g == 0) else 0
-                    self._group_streams[g] = torch.cuda.Stream(device=self.device, priority=prio)
-                gs = self._group_streams[g]
-                gs.wait_stream(main)
-                self._group = g + 1
-                try:
-                    with torch.cuda.stream(gs):
-                        sg = style_u8 if style_u8.shape[0] == 1 else style_u8[lo:hi]
-                        outs.append(self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, shared_style=shared))
-                finally:
-                    self._group = 0
-            for g in range(G):
-                main.wait_stream(self._group_streams[g])
-            out = torch.cat(outs, dim=0)
-            for g in range(G):                      # sub-batch buffers die here: their streams wait for the cat
-                self._group_streams[g].wait_stream(main)
+
+            def run(lo, hi):
+                sg = style_u8 if style_u8.shape[0] == 1 else style_u8[lo:hi]
+                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, shared_style=shared)
+            out = self._in_groups(N, G, main, run)
             if shared is not None and shared["side"] is not main:
                 shared["side"].wait_stream(main)    # the shared style states are recycled only after every group used them
             return out
         return self._stylize_one(content_u8, style_u8, alpha, adain, want_info, capture)
 
-    def _stylize_regions(self, content_u8, labels, region_styles, alpha, want_info, capture):
-        """``stylize`` with a label map: the R style sides run once and are shared by every sub-batch group."""
+    def _in_groups(self, N, G, main, run):
+        """Cut a batch of N frames into G sub-batches and enqueue ``run(lo, hi)`` for each on its own stream (group g + 1
+        owns its scratch); returns the concatenated outputs, ordered on ``main`` after every group."""
+        bounds = [(g * N) // G for g in range(G + 1)]
+        outs = []
+        for g in range(G):
+            lo, hi = bounds[g], bounds[g + 1]
+            if g not in self._group_streams:
+                # descending priority: group 0 runs "in the foreground", later groups fill the SMs it
+                # leaves idle while its eigendecompositions are latency bound (self.group_priorities)
+                prio = -1 if (self.group_priorities and g == 0) else 0
+                self._group_streams[g] = torch.cuda.Stream(device=self.device, priority=prio)
+            gs = self._group_streams[g]
+            gs.wait_stream(main)
+            self._group = g + 1
+            try:
+                with torch.cuda.stream(gs):
+                    outs.append(run(lo, hi))
+            finally:
+                self._group = 0
+        for g in range(G):
+            main.wait_stream(self._group_streams[g])
+        out = torch.cat(outs, dim=0)
+        for g in range(G):                      # sub-batch buffers die here: their streams wait for the cat
+            self._group_streams[g].wait_stream(main)
+        return out
+
+    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame):
+        """``stylize`` with several style images (spatial control, style interpolation): their style sides run once per
+        call and are shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the label
+        maps or weight rows)."""
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
+        split = not adain                      # AdaIN keeps its style features inline
         self._group = 1 if G > 1 else 0
         try:
-            sides = [self._style_side(s, True, main) for s in region_styles]
+            sides = [self._style_side(s, split, main) for s in styles]
         finally:
             self._group = 0
         if G == 1:
-            out = self._stylize_one(content_u8, None, alpha, False, want_info, capture, region=(labels, sides))
+            out = self._stylize_one(content_u8, None, alpha, adain, want_info, capture, multi=per_frame(0, N) + (sides,))
         else:
-            bounds = [(g * N) // G for g in range(G + 1)]
-            outs = []
-            for g in range(G):
-                if g not in self._group_streams:
-                    prio = -1 if (self.group_priorities and g == 0) else 0
-                    self._group_streams[g] = torch.cuda.Stream(device=self.device, priority=prio)
-                gs = self._group_streams[g]
-                gs.wait_stream(main)
-                self._group = g + 1
-                try:
-                    with torch.cuda.stream(gs):
-                        lo, hi = bounds[g], bounds[g + 1]
-                        outs.append(self._stylize_one(content_u8[lo:hi], None, alpha, False, False, None,
-                                                      region=(labels[lo:hi], sides)))
-                finally:
-                    self._group = 0
-            for g in range(G):
-                main.wait_stream(self._group_streams[g])
-            out = torch.cat(outs, dim=0)
-            for g in range(G):
-                self._group_streams[g].wait_stream(main)
+            out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, adain, False, None,
+                                                                               multi=per_frame(lo, hi) + (sides,)))
         for side in {id(sd["side"]): sd["side"] for sd in sides}.values():
             if side is not main:
                 side.wait_stream(main)         # the style states are recycled only after every level used them
@@ -491,18 +538,19 @@ class Engine(object):
         return dict(states=states, events=events, feats=feats, side=side)
 
     def _stylize_one(self, content_u8, style_u8, alpha, adain, want_info, capture, swap5=False, ss_alpha=0.6, shared_style=None,
-                     ss_patch=3, ss_stride=1, region=None):
+                     ss_patch=3, ss_stride=1, multi=None):
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
-        if region is None:
+        if multi is None:
             assert content_u8.dtype == torch.uint8 and style_u8.dtype == torch.uint8
             assert style_u8.shape[0] in (1, N)
         content = torch.empty(content_u8.shape, dtype=torch.float32, device=self.device)
         self._call("u8_to_f32", 1, lib.wctb200_image_u8_to_f32, content_u8.data_ptr(), content_u8.numel(), content.data_ptr(), st)
         split = not adain and not swap5        # WCT: style side on its own stream; AdaIN / style swap: keep it inline
-        if region is not None:                 # spatial control: (labels [N,Hm,Wm], the R style sides of _stylize_regions)
-            labels, sides = region
+        if multi is not None:
+            # ("regions", labels [N,Hm,Wm], R style sides) or ("interp", weight rows [1|N,K], K style sides): _stylize_multi
+            mode, per_frame, sides = multi
             ss = sides[0]
             n_style = 1
         else:
@@ -515,12 +563,17 @@ class Engine(object):
         for lvl in self.model.levels:
             self._tag = lvl.relu_target
             cf, _ = self.encode(x, lvl.relu_target)
-            if region is not None:
+            if multi is not None:
                 for sd in sides:
-                    if sd["side"] is not main:
+                    if split and sd["side"] is not main:     # AdaIN: the style features were encoded inline, before the groups
                         main.wait_event(sd["events"][lvl.relu_target])
-                lab = self.labels_resize(labels, cf.H, cf.W)
-                f, kbuf = self.wct_apply_regions(cf, lab, [sd["states"][lvl.relu_target] for sd in sides], alpha, want_info)
+                if mode == "regions":
+                    lab = self.labels_resize(per_frame, cf.H, cf.W)
+                    f, kbuf = self.wct_apply_regions(cf, lab, [sd["states"][lvl.relu_target] for sd in sides], alpha, want_info)
+                elif adain:
+                    f, kbuf = self.adain_blend(cf, [sd["feats"][lvl.relu_target] for sd in sides], per_frame, alpha)
+                else:
+                    f, kbuf = self.wct_apply_blend(cf, [sd["states"][lvl.relu_target] for sd in sides], per_frame, alpha, want_info)
             elif swap5 and lvl.relu_target == "relu5_1":     # model.py:148-152: style swap wins over AdaIN / WCT at relu5_1
                 f, kbuf = self.style_swap(cf, style_feats[lvl.relu_target], ss_alpha, want_info, ss_patch, ss_stride)
             elif split:
@@ -539,7 +592,7 @@ class Engine(object):
             if capture is not None:
                 capture.setdefault("level_output", []).append(x)
         self._tag = None
-        if side is not main and shared_style is None and region is None:
+        if side is not main and shared_style is None and multi is None:
             side.wait_stream(main)             # buffers handed across streams may be recycled only after both are done
             main.wait_stream(side)
         if want_info:

@@ -9,7 +9,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``swap5=True`` (style-swap at relu5_1, ops.py:145-278) honours ``ss_patch_size`` / ``ss_stride``; with a stride the
     content is centre-cropped so that the patches tile its relu5_1 encoding, as wct.py:84-90 does;
   * ``predict_batch`` is new: a batch of frames per call (frames are independent);
-  * ``content_mask`` is new: spatial control (WCT paper, section 4), a label map whose region r takes style r.
+  * ``content_mask`` is new: spatial control (WCT paper, section 4), a label map whose region r takes style r;
+  * ``style_weights`` is new: style interpolation (WCT paper, section 4), a weighted blend of 1..8 styles, shared by
+    every frame or one row per frame.
 """
 from __future__ import annotations
 
@@ -88,8 +90,43 @@ class WCT(object):
                 raise ValueError("each region style must be one uint8 [Hs,Ws,3] image")
         return m.contiguous(), styles
 
+    @staticmethod
+    def normalize_weights(style_weights, n_frames, K, dtype=np.float32):
+        """Host-side validation of interpolation weights: [K] (shared by every frame) or [N,K], finite, >= 0, every row with a
+        positive sum.  Each row is divided by its sum in float64 (a one-hot row stays exact), then cast to ``dtype``.
+        Returns [1|N, K]."""
+        w = style_weights.cpu().numpy() if isinstance(style_weights, torch.Tensor) else np.asarray(style_weights)
+        if w.dtype.kind not in "biuf":
+            raise ValueError("style_weights must be numeric, got %s" % (w.dtype,))
+        w = w.astype(np.float64)
+        if w.ndim == 1:
+            w = w[None]
+        if w.ndim != 2 or w.shape[1] != K or w.shape[0] not in (1, n_frames):
+            raise ValueError("style_weights must be [K] or [N,K] with K = %d styles and N = %d frames, got %s"
+                             % (K, n_frames, tuple(np.shape(style_weights))))
+        if not np.isfinite(w).all() or (w < 0).any():
+            raise ValueError("style_weights must be finite and >= 0")
+        s = w.sum(axis=1, keepdims=True)
+        if (s <= 0).any():
+            raise ValueError("every row of style_weights needs a positive sum")
+        return (w / s).astype(dtype)
+
+    @staticmethod
+    def check_interp(style_weights, n_frames, styles):
+        """Host-side validation of an interpolation call: a list of 1..8 uint8 [Hs,Ws,3] style images (any sizes) and their
+        weights (``normalize_weights``).  Returns (float32 weights [1|N, K], styles)."""
+        if isinstance(styles, (np.ndarray, torch.Tensor)) and styles.ndim == 3:
+            styles = [styles]
+        styles = list(styles)
+        if not 1 <= len(styles) <= 8:
+            raise ValueError("style interpolation needs 1..8 styles, got %d" % len(styles))
+        for s in styles:
+            if s.dtype not in (np.uint8, torch.uint8) or s.ndim not in (3, 4) or s.shape[-1] != 3 or (s.ndim == 4 and s.shape[0] != 1):
+                raise ValueError("each interpolated style must be one uint8 [Hs,Ws,3] image")
+        return WCT.normalize_weights(style_weights, n_frames, len(styles)), styles
+
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
-                      passes=1, return_device=False, content_mask=None):
+                      passes=1, return_device=False, content_mask=None, style_weights=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -102,13 +139,22 @@ class WCT(object):
 
         ``content_mask`` (spatial control): uint8 label map [Hm,Wm] shared by every frame, or [N,Hm,Wm]; ``styles`` is then
         a list of R (1..8) uint8 [Hs,Ws,3] images of any sizes, and region r of each frame takes style r.  The mask may have
-        any resolution: every level samples it to its feature grid.  Labels >= R leave that region unstyled.  WCT only."""
+        any resolution: every level samples it to its feature grid.  Labels >= R leave that region unstyled.  WCT only.
+
+        ``style_weights`` (style interpolation): ``styles`` is then a list of K (1..8) uint8 [Hs,Ws,3] images of any sizes
+        and ``style_weights`` their weights, [K] for every frame or [N,K] (row n for frame n); finite, >= 0, each row with a
+        positive sum, normalised to sum 1.  Frame n is stylised with the blend of the K styles, which equals the blend of
+        the K single-style results at every level.  WCT or AdaIN; not with ``content_mask`` or ``swap5``."""
         eng = self.engine
         dev = eng.device
+        n = 1 if np.ndim(contents) == 3 else contents.shape[0]
+        if style_weights is not None:
+            if content_mask is not None or swap5:
+                raise ValueError("style_weights does not combine with content_mask or swap5")
+            weights, interp_styles = self.check_interp(style_weights, n, styles)
         if content_mask is not None:
             if adain or swap5:
                 raise ValueError("content_mask works with WCT only: not with adain or swap5")
-            n = 1 if np.ndim(contents) == 3 else contents.shape[0]
             mask, region_styles = self.check_mask(content_mask, n, styles)
 
         def to_dev(a):
@@ -131,7 +177,13 @@ class WCT(object):
                     contents = center_crop_to(contents, H, W)
         with torch.cuda.device(dev):
             c = to_dev(contents)
-            if content_mask is not None:
+            if style_weights is not None:
+                w_dev = torch.from_numpy(weights).to(dev, non_blocking=True)
+                ist = [to_dev(x) for x in interp_styles]
+
+                def one_pass(x):
+                    return eng.stylize(x, None, alpha=alpha, adain=adain, interp_styles=ist, interp_weights=w_dev)
+            elif content_mask is not None:
                 lab = mask.to(dev, non_blocking=True)
                 rs = [to_dev(x) for x in region_styles]
 
@@ -172,11 +224,15 @@ class WCT(object):
             return out_u8, out_f.cpu().numpy()
         return out_u8
 
-    def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None):
+    def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
-        is a list of R region styles and region r of the content takes style r.'''
+        is a list of R region styles and region r of the content takes style r.  With ``style_weights`` ([K]), ``style`` is a
+        list of K styles and the content takes their weighted blend.'''
         s = time.time()
-        if content_mask is not None:
+        if style_weights is not None:
+            out = self.predict_batch(np.asarray(content), [np.asarray(x) for x in style], alpha=alpha, adain=adain, swap5=swap5,
+                                     style_weights=style_weights, content_mask=content_mask)
+        elif content_mask is not None:
             out = self.predict_batch(np.asarray(content), [np.asarray(x) for x in style], alpha=alpha, adain=adain, swap5=swap5,
                                      content_mask=content_mask)
         else:
