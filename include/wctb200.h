@@ -97,6 +97,14 @@ WCTB200_API int wctb200_rgb_moments_u8(const uint8_t* img, long long npix, unsig
 WCTB200_API int wctb200_coral_apply_u8(const uint8_t* src, long long npix, const double* A, const double* src_mean,
                                        const double* src_std, const double* tgt_mean, const double* tgt_std, uint8_t* dst,
                                        void* stream);
+/* Texture synthesis input (--noise, webcam.py:191-192 np.random.randint(0, 256, shape, np.uint8)): N frames of uniform random
+ * bytes, out device uint8 [N][H][W][C].  Frame n has the absolute index f = first_index + n; byte j of its H*W*C bytes
+ * (row-major HWC) is byte j % 16 of Philox4x32-10 (Random123) with counter (b_lo, b_hi, f_lo, f_hi), b = j / 16 (64-bit), and
+ * key (seed_lo, seed_hi), where the 16 bytes are x0..x3, each little-endian; a frame's last block is truncated at its end.
+ * A frame therefore depends only on (seed, f, H, W, C): not on N or on how a run is cut into calls.
+ * N, H, W >= 1, C in 1..4, first_index >= 0 and first_index + N representable, else WCTB200_EINVAL. */
+WCTB200_API int wctb200_noise_u8(uint8_t* out, int N, int H, int W, int C, unsigned long long seed, long long first_index,
+                                 void* stream);
 
 /* ---- encoder / decoder layers ---------------------------------------------- */
 /* Weight preparation (one-time, device side):

@@ -14,6 +14,10 @@ Style interpolation: ``--interp-styles S0 S1 ... --interp-weights w0 w1 ...`` st
 styles (weights >= 0, normalised to sum 1; WCT or ``--adain``); the output is ``<content>_<s0>-<w0>+<s1>-<w1>...<ext>``
 with the normalised weights.
 
+Texture synthesis: ``--noise [--noise-size H W] [--noise-count K] [--noise-seed S]`` replaces ``--content-path`` by K frames of
+seeded uniform noise made on the device (default one 512x512 frame, seed 0), stylised in one batch per style, blend or mask;
+the outputs are named as above with the content ``noise<S>-<i>.png``, e.g. ``noise0-3_starry.png``.
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -55,7 +59,14 @@ _FLAGS = [
     (("--mask-styles",), dict(nargs="+", type=str, default=None, help="one style image per mask region (with --content-mask)")),
     (("--interp-styles",), dict(nargs="+", type=str, default=None, help="1..8 style images to blend (with --interp-weights)")),
     (("--interp-weights",), dict(nargs="+", type=float, default=None, help="one weight >= 0 per --interp-styles entry (normalised)")),
+    # webcam.py:38; the three --noise-* flags are not in the reference.  Their defaults are filled in by parse_args, so that
+    # giving one without --noise can be told from leaving it out.
+    (("--noise",), dict(action="store_true", default=False, help="Synthesize textures from noise images")),
+    (("--noise-size",), dict(nargs=2, type=int, default=None, metavar=("H", "W"), help="size of the noise frames (default 512 512)")),
+    (("--noise-count",), dict(type=int, default=None, metavar="K", help="noise frames, one texture each (default 1)")),
+    (("--noise-seed",), dict(type=int, default=None, metavar="S", help="seed of the noise frames, 0 .. 2^64-1 (default 0)")),
 ]
+_NOISE_DEFAULTS = [("noise_size", [512, 512]), ("noise_count", 1), ("noise_seed", 0)]
 
 # flags that do not combine with --content-mask
 _MASK_EXCLUDES = [("style_path", "--style-path"), ("adain", "--adain"), ("swap5", "--swap5"), ("concat", "--concat"),
@@ -86,7 +97,28 @@ def parse_args(argv=None):
                 parser.error("--content-mask does not combine with %s" % flag)
     elif args.mask_styles:
         parser.error("--mask-styles needs --content-mask")
+    check_noise_flags(parser, args)
     return args
+
+
+def check_noise_flags(parser, args):
+    """--noise replaces the content images; the --noise-* flags need it, and get their defaults here."""
+    if not args.noise:
+        for attr, _ in _NOISE_DEFAULTS:
+            if getattr(args, attr) is not None:
+                parser.error("--%s needs --noise" % attr.replace("_", "-"))
+        return
+    if args.content_path is not None or args.content_size or args.keep_colors:
+        parser.error("--noise does not combine with --content-path, --content-size or --keep-colors")
+    for attr, default in _NOISE_DEFAULTS:
+        if getattr(args, attr) is None:
+            setattr(args, attr, default)
+    if min(args.noise_size) < 1:
+        parser.error("--noise-size must be positive")
+    if args.noise_count < 1:
+        parser.error("--noise-count must be >= 1")
+    if not 0 <= args.noise_seed < 2 ** 64:
+        parser.error("--noise-seed must be in 0 .. 2^64-1")
 
 
 def check_interp_flags(parser, args, excludes=_INTERP_EXCLUDES):
@@ -143,6 +175,26 @@ def _listing(path, io):
     return io.get_files(path) if os.path.isdir(path) else [path]
 
 
+def noise_names(seed, count):
+    """Content names of the --noise frames: ``noise<S>-<i>.png``."""
+    return ["noise{}-{}.png".format(seed, i) for i in range(count)]
+
+
+def _contents(args, io, dimg, device):
+    """Yields (names, content on the device): each image of --content-path alone ([its path], HxWx3), or with --noise the
+    K noise frames as one batch (``noise_names``, [K,H,W,3]) so that they are stylised in one call per style."""
+    if args.noise:
+        H, W = args.noise_size
+        yield noise_names(args.noise_seed, args.noise_count), dimg.noise_u8(args.noise_count, H, W, seed=args.noise_seed,
+                                                                           device=device)
+        return
+    for content_path in _listing(args.content_path, io):
+        content_dev = dimg.to_device(io.get_img(content_path), device)
+        if args.content_size > 0:
+            content_dev = dimg.resize_to(content_dev, args.content_size)
+        yield [content_path], content_dev
+
+
 def _prepare_style(path, args, io, dimg, content_dev, device):
     """stylize.py:86-95 on the device: decode on the host, then resize / crop / CORAL without leaving the GPU."""
     img = dimg.to_device(io.get_img(path), device)
@@ -161,7 +213,7 @@ def _stylize_pair(model, content_dev, style_dev, args):
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, style_dev, **kw)
-    return result[0]
+    return result
 
 
 def make_model(args):
@@ -181,7 +233,7 @@ def _stylize_masked(model, content_dev, styles_dev, labels, args):
     result = model.predict_batch(content_dev, styles_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, styles_dev, **kw)
-    return result[0]
+    return result
 
 
 def main_masked(args, model, io, dimg, t_start):
@@ -190,16 +242,14 @@ def main_masked(args, model, io, dimg, t_start):
     os.makedirs(args.out_path, exist_ok=True)
     device = model.engine.device
     written = 0
-    for content_path in _listing(args.content_path, io):
-        content_dev = dimg.to_device(io.get_img(content_path), device)
-        if args.content_size > 0:
-            content_dev = dimg.resize_to(content_dev, args.content_size)
+    for names, content_dev in _contents(args, io, dimg, device):
         styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device) for p in args.mask_styles]
-        result = _stylize_masked(model, content_dev, styles_dev, labels, args)
-        target = os.path.join(args.out_path, mask_output_name(content_path, args.mask_styles))
-        io.save_img(target, dimg.to_host(result))
-        written += 1
-        print("{}: Wrote stylized output image to {}".format(written, target))
+        results = _stylize_masked(model, content_dev, styles_dev, labels, args)
+        for name, result in zip(names, results):
+            target = os.path.join(args.out_path, mask_output_name(name, args.mask_styles))
+            io.save_img(target, dimg.to_host(result))
+            written += 1
+            print("{}: Wrote stylized output image to {}".format(written, target))
     print("Finished stylizing {} outputs in {}s".format(written, time.time() - t_start))
     return written
 
@@ -210,18 +260,16 @@ def main_interp(args, model, io, dimg, t_start):
     device = model.engine.device
     kw = dict(alpha=args.alpha, adain=args.adain, return_device=True, style_weights=np.asarray(args.interp_weights, np.float64))
     written = 0
-    for content_path in _listing(args.content_path, io):
-        content_dev = dimg.to_device(io.get_img(content_path), device)
-        if args.content_size > 0:
-            content_dev = dimg.resize_to(content_dev, args.content_size)
+    for names, content_dev in _contents(args, io, dimg, device):
         styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device) for p in args.interp_styles]
-        result = model.predict_batch(content_dev, styles_dev, **kw)
+        results = model.predict_batch(content_dev, styles_dev, **kw)
         for _ in range(args.passes - 1):
-            result = model.predict_batch(result, styles_dev, **kw)
-        target = os.path.join(args.out_path, interp_output_name(content_path, args.interp_styles, args.interp_weights))
-        io.save_img(target, dimg.to_host(result[0]))
-        written += 1
-        print("{}: Wrote stylized output image to {}".format(written, target))
+            results = model.predict_batch(results, styles_dev, **kw)
+        for name, result in zip(names, results):
+            target = os.path.join(args.out_path, interp_output_name(name, args.interp_styles, args.interp_weights))
+            io.save_img(target, dimg.to_host(result))
+            written += 1
+            print("{}: Wrote stylized output image to {}".format(written, target))
     print("Finished stylizing {} outputs in {}s".format(written, time.time() - t_start))
     return written
 
@@ -245,21 +293,20 @@ def main(argv=None, model_factory=make_model, image_ops=None):
 
     device = model.engine.device
     written = 0
-    for content_path in _listing(args.content_path, io):
-        stem, ext = os.path.splitext(os.path.basename(content_path))
-        content_dev = dimg.to_device(io.get_img(content_path), device)
-        if args.content_size > 0:
-            content_dev = dimg.resize_to(content_dev, args.content_size)
+    for names, content_dev in _contents(args, io, dimg, device):
         for style_path in styles:
             style_dev = _prepare_style(style_path, args, io, dimg, content_dev, device)
-            result = _stylize_pair(model, content_dev, style_dev, args)
-            if args.concat:
-                result = dimg.concat_with_style(style_dev, result)
-            target = os.path.join(args.out_path, "{}_{}{}".format(stem, os.path.splitext(os.path.basename(style_path))[0], ext))
-            io.save_img(target, result.cpu().numpy())
-            written += 1
-            print("{}: Wrote stylized output image to {}".format(written, target))
+            results = _stylize_pair(model, content_dev, style_dev, args)
+            for name, result in zip(names, results):
+                if args.concat:
+                    result = dimg.concat_with_style(style_dev, result)
+                stem, ext = os.path.splitext(os.path.basename(name))
+                target = os.path.join(args.out_path, "{}_{}{}".format(stem, os.path.splitext(os.path.basename(style_path))[0], ext))
+                io.save_img(target, dimg.to_host(result))
+                written += 1
+                print("{}: Wrote stylized output image to {}".format(written, target))
     print("Finished stylizing {} outputs in {}s".format(written, time.time() - t_start))
+    return written
 
 
 if __name__ == "__main__":

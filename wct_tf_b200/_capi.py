@@ -31,6 +31,7 @@ SIGNATURES = {
     "wctb200_resize_bilinear_u8": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "wctb200_rgb_moments_u8": (_i, [_vp, C.c_longlong, _vp, _vp]),
     "wctb200_coral_apply_u8": (_i, [_vp, C.c_longlong, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "wctb200_noise_u8": (_i, [_vp, _i, _i, _i, _i, C.c_ulonglong, C.c_longlong, _vp]),
     "wctb200_conv_weight_bytes": (_sz, [_i, _i, _i]),
     "wctb200_prep_conv_weights": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "wctb200_prep_conv_weights_up2": (_i, [_vp, _i, _i, _vp, _vp]),

@@ -1,4 +1,5 @@
 // extern "C" surface of libwctb200 (declared in include/wctb200.h).
+#include <limits.h>
 #include <stdarg.h>
 #include <string.h>
 
@@ -87,6 +88,7 @@ int launch_resize_u8(const uint8_t* src, int N, int Hs, int Ws, int C, int Hd, i
 int launch_rgb_moments(const uint8_t* img, long long npix, unsigned long long* sums, cudaStream_t st);
 int launch_coral_apply(const uint8_t* src, long long npix, const double* A, const double* sm, const double* ss, const double* tm,
                        const double* ts, uint8_t* dst, cudaStream_t st);
+int launch_noise_u8(uint8_t* out, int N, long long frame_bytes, unsigned long long seed, long long first_index, cudaStream_t st);
 int launch_act_from_f32(const float*, ActGeom, __half*, cudaStream_t);
 int launch_act_to_f32(const __half*, ActGeom, float*, cudaStream_t);
 int launch_prep_weights(const float*, int, int, int, __half*, cudaStream_t);
@@ -225,6 +227,14 @@ int wctb200_coral_apply_u8(const uint8_t* src, long long npix, const double* A, 
                            const double* tgt_mean, const double* tgt_std, uint8_t* dst, void* stream) {
     WCTB_REQUIRE(src && dst && A && src_mean && src_std && tgt_mean && tgt_std && npix >= 1, "coral_apply_u8: bad arguments");
     return launch_coral_apply(src, npix, A, src_mean, src_std, tgt_mean, tgt_std, dst, ST(stream));
+}
+int wctb200_noise_u8(uint8_t* out, int N, int H, int W, int C, unsigned long long seed, long long first_index, void* stream) {
+    WCTB_REQUIRE(out, "noise_u8: null pointer");
+    WCTB_REQUIRE(N >= 1 && H >= 1 && W >= 1 && C >= 1 && C <= 4, "noise_u8: bad geometry N=%d %dx%dx%d", N, H, W, C);
+    WCTB_REQUIRE((long long)H * W <= (1ll << 62) / C / N, "noise_u8: %d x %dx%dx%d bytes is too large", N, H, W, C);
+    WCTB_REQUIRE(first_index >= 0 && first_index <= LLONG_MAX - N, "noise_u8: first_index=%lld with N=%d is out of range",
+                 first_index, N);
+    return launch_noise_u8(out, N, (long long)H * W * C, seed, first_index, ST(stream));
 }
 
 size_t wctb200_conv_weight_bytes(int taps, int Cin, int Cout) {

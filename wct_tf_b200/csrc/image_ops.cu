@@ -16,6 +16,10 @@
 // per-pixel affine map out = (A ((x/255 - m_s) / s_s)) * s_t + m_t in double precision followed by the reference's
 // clip / *255 / truncation.  The 3x3 algebra in between (matSqrt through numpy's SVD, whose sign conventions the
 // reference's non-symmetric U sqrt(D) U depends on) stays on the host in wct_tf_b200/device_image.py.
+//
+// Noise (texture synthesis; reference: webcam.py:191-192 np.random.randint(0, 256, shape, np.uint8)).  Counter-based:
+// 16-byte block b of absolute frame f is Philox4x32-10(counter (b_lo, b_hi, f_lo, f_hi), key (seed_lo, seed_hi)), so every
+// byte is a pure function of (seed, f, position) whatever the launch shape or batch split.  Bound by its writes.
 #include "common.cuh"
 
 namespace wctb {
@@ -273,6 +277,59 @@ int launch_coral_apply(const uint8_t* src, long long npix, const double* A, cons
     }
     k_coral_apply<<<grid_for(npix, 256), 256, 0, st>>>(src, npix, P, dst);
     WCTB_CHECK_LAUNCH("k_coral_apply");
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// Noise
+// ---------------------------------------------------------------------------
+// Philox4x32-10 (Salmon et al., SC'11; the Random123 constants)
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, unsigned int k0, unsigned int k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const unsigned int hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+        const unsigned int hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+        k0 += 0x9E3779B9u;
+        k1 += 0xBB67AE85u;
+    }
+    return c;
+}
+
+// One thread per 16-byte block of a frame (frame_bytes = H*W*C).  A frame starts at out + n*frame_bytes, so its blocks share
+// one alignment: 16-byte stores where that is 16-aligned, four 4-byte stores where it is 4-aligned, bytes otherwise and for
+// the truncated last block of a frame.
+__global__ void k_noise_u8(uint8_t* __restrict__ out, long long N, long long frame_bytes, long long blocks_per_frame,
+                           unsigned int k0, unsigned int k1, unsigned long long first_index) {
+    const long long total = N * blocks_per_frame;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long n = i / blocks_per_frame;
+        const unsigned long long b = (unsigned long long)(i - n * blocks_per_frame);
+        const unsigned long long f = first_index + (unsigned long long)n;
+        const uint4 x = philox4x32_10(make_uint4((unsigned int)b, (unsigned int)(b >> 32), (unsigned int)f, (unsigned int)(f >> 32)),
+                                      k0, k1);
+        uint8_t* p = out + n * frame_bytes + (long long)b * 16;
+        const long long left = frame_bytes - (long long)b * 16;
+        const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+        if (left >= 16 && (a & 15) == 0) {
+            *reinterpret_cast<uint4*>(p) = x;
+        } else if (left >= 16 && (a & 3) == 0) {
+            unsigned int* q = reinterpret_cast<unsigned int*>(p);
+            q[0] = x.x; q[1] = x.y; q[2] = x.z; q[3] = x.w;
+        } else {
+            const int m = left < 16 ? (int)left : 16;
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+                if (j < m) p[j] = (uint8_t)((j < 4 ? x.x : j < 8 ? x.y : j < 12 ? x.z : x.w) >> (8 * (j & 3)));
+        }
+    }
+}
+
+int launch_noise_u8(uint8_t* out, int N, long long frame_bytes, unsigned long long seed, long long first_index, cudaStream_t st) {
+    const long long bpf = (frame_bytes + 15) / 16;
+    k_noise_u8<<<grid_for((long long)N * bpf, 256), 256, 0, st>>>(out, N, frame_bytes, bpf, (unsigned int)seed,
+                                                                   (unsigned int)(seed >> 32), (unsigned long long)first_index);
+    WCTB_CHECK_LAUNCH("k_noise_u8");
     return 0;
 }
 

@@ -3,6 +3,7 @@
 the ``--concat`` thumbnail stylize.py:107-111), operating on ``torch.uint8`` CUDA tensors HxWx3 (or NxHxWx3) through the C ABI
 (``wctb200_resize_bilinear_u8``, ``wctb200_rgb_moments_u8``, ``wctb200_coral_apply_u8``).  A decoded image goes to the GPU once
 and stays there through resize, crop, CORAL, every ``--passes`` round and the concat; only the finished frame comes back.
+``noise_u8`` makes the noise frames of texture synthesis (``--noise``) on the device (``wctb200_noise_u8``).
 
 There is no CPU fallback: the functions raise ``WctB200Error`` when the library or a CUDA device is missing.  The only host
 arithmetic is the 3x3 algebra of CORAL (the reference's ``matSqrt`` goes through ``np.linalg.svd`` and, as written, depends on
@@ -149,6 +150,25 @@ def preserve_colors_np(style_rgb, content_rgb):
     with torch.cuda.device(src.device):
         _capi.check(lib.wctb200_coral_apply_u8(src.data_ptr(), src.numel() // 3, keep[0][1], keep[1][1], keep[2][1], keep[3][1],
                                                keep[4][1], out.data_ptr(), _stream()))
+    return out
+
+
+def noise_u8(count, height, width, seed=0, first_index=0, device="cuda:0"):
+    """--noise (webcam.py:191-192, ``np.random.randint(0, 256, shape, np.uint8)``): ``count`` frames of uniform random bytes,
+    a uint8 CUDA tensor [count, height, width, 3] made on the device (``wctb200_noise_u8``) on the current stream.  Frame i
+    is a pure function of (seed, first_index + i, height, width): counter-based Philox4x32-10, so it does not depend on
+    ``count`` or on how a run is cut into calls.  ``seed``: 0 .. 2^64 - 1; ``first_index`` >= 0."""
+    if not torch.cuda.is_available():
+        raise _capi.WctB200Error("no CUDA device: the image steps have no CPU fallback")
+    count, height, width, seed, first_index = int(count), int(height), int(width), int(seed), int(first_index)
+    if count < 1 or height < 1 or width < 1:
+        raise ValueError("noise_u8: count, height and width must be >= 1, got %d, %d, %d" % (count, height, width))
+    if not 0 <= seed < 2 ** 64 or not 0 <= first_index < 2 ** 63:
+        raise ValueError("noise_u8: seed must be in [0, 2^64) and first_index in [0, 2^63)")
+    lib = _capi.load()
+    with torch.cuda.device(device):
+        out = torch.empty((count, height, width, 3), dtype=torch.uint8, device=device)
+        _capi.check(lib.wctb200_noise_u8(out.data_ptr(), count, height, width, 3, seed, first_index, _stream()))
     return out
 
 

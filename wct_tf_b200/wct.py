@@ -11,7 +11,8 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``predict_batch`` is new: a batch of frames per call (frames are independent);
   * ``content_mask`` is new: spatial control (WCT paper, section 4), a label map whose region r takes style r;
   * ``style_weights`` is new: style interpolation (WCT paper, section 4), a weighted blend of 1..8 styles, shared by
-    every frame or one row per frame.
+    every frame or one row per frame;
+  * ``synthesize`` is new: texture synthesis (WCT paper, section 4), the pipeline run on seeded noise made on the device.
 """
 from __future__ import annotations
 
@@ -223,6 +224,24 @@ class WCT(object):
         if return_float:
             return out_u8, out_f.cpu().numpy()
         return out_u8
+
+    def synthesize(self, styles, size, count=1, seed=0, first_index=0, **kw):
+        """Texture synthesis (WCT paper, section 4; the reference's ``--noise``, webcam.py:191-192): stylise ``count`` frames
+        of uniform noise made on the device into textures of the style.  ``size`` is (H, W) or one integer for a square.
+
+        Defined as ``predict_batch(noise_u8(count, H, W, seed, first_index), styles, **kw)`` and equal to it byte for byte;
+        ``kw`` is any ``predict_batch`` option (``alpha``, ``adain``, ``passes``, ``swap5`` / ``ss_alpha``, ``style_weights``
+        for texture mixing, ``content_mask`` for texture painting, ``return_device``, ``out``, ``return_float``), with the
+        same rules and rejections.
+
+        Texture i depends only on the seed, ``first_index + i`` and the size, the styles and options, and the weights: not
+        on ``count``, on how a run is cut into calls, or on the engine's sub-batch groups (the pipeline is batch-invariant,
+        tests/test_gpu_invariance.py).  ``synthesize(count=5)`` equals ``synthesize(count=2)`` followed by
+        ``synthesize(count=3, first_index=2)``."""
+        from .device_image import noise_u8
+        H, W = (size, size) if isinstance(size, (int, np.integer)) else size
+        noise = noise_u8(count, H, W, seed=seed, first_index=first_index, device=self.engine.device)
+        return self.predict_batch(noise, styles, **kw)
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
