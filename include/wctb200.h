@@ -180,6 +180,10 @@ WCTB200_API int wctb200_wct_style_prepare(const void* style, int Ns, int Hs, int
 WCTB200_API int wctb200_wct_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns,
                       float alpha, float eps_cov, float eps_eig, float thresh, int readd_content_mean,
                       void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
+/* Layout of a wctb200_wct_style_prepare state, so that a host can pack, unpack, save and load states without repeating
+ * the alignment rule: fp32 mean_s [Ns][C] at *off_mean (0), fp32 C_s [Ns][C][C] at *off_cs, int32 [k_s x Ns | sweeps_s x Ns]
+ * at *off_k.  Returns the total (= wctb200_wct_style_state_bytes), 0 for C < 8 or Ns < 1.  Any pointer may be NULL. */
+WCTB200_API size_t wctb200_wct_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_cs, size_t* off_k);
 /* Spatial control (WCT paper, section 4): a label map splits each content frame into regions and region r takes style r.
  * Per (frame, region r < R) with at least 2 pixels the transform is wctb200_wct_apply's (same semantics flags) restricted
  * to the region's pixels: mean, covariance and whitening over those pixels only, colouring with style r.  Every other
@@ -233,6 +237,26 @@ WCTB200_API int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm,
 WCTB200_API int wctb200_adain_level(const void* content, int Nc, int Hc, int Wc,
                         const void* style, int Ns, int Hs, int Ws, int C,
                         float alpha, float eps, void* out, void* ws, size_t ws_bytes, void* stream);
+/* Split form of wctb200_adain_level and wctb200_adain_blend: the style side is the biased per-channel moments of the style,
+ * which depend on the style features only, so a host can prepare them once and apply them to any number of calls.
+ * wctb200_adain_level is prepare followed by apply, and wctb200_adain_blend is K prepares followed by apply_blend, so
+ * the split form gives the same bytes.
+ *   state: device buffer of wctb200_adain_style_state_bytes(C, Ns) bytes, fp32 mean [Ns][C] at *off_mean (0) and var [Ns][C]
+ *   at *off_var (wctb200_adain_style_state_layout; 0 for C not a multiple of 8 or Ns < 1).
+ *   prepare: style SPF16 [Ns,Hs,Ws,C]; needs no workspace (it uses the library's per-stream scratch).
+ *   apply: content SPF16 [Nc,Hc,Wc,C] against a state of Ns in {1, Nc} styles (frame i takes style i, or the shared one).
+ *   apply_blend: states is a HOST array of K device pointers, each a state with Ns = 1; weights as for
+ *   wctb200_adain_blend (DEVICE fp32 [Nw][K], Nw in {1, Nc}, used as given).
+ * Both applies take a workspace of wctb200_wct_workspace_bytes(C, Nc, 0) bytes and only read the states.  A null state,
+ * Ns not in {1, Nc}, K outside 1..8 or Nw not in {1, Nc} is WCTB200_EINVAL. */
+WCTB200_API size_t wctb200_adain_style_state_bytes(int C, int Ns);
+WCTB200_API size_t wctb200_adain_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_var);
+WCTB200_API int wctb200_adain_style_prepare(const void* style, int Ns, int Hs, int Ws, int C, void* state, void* stream);
+WCTB200_API int wctb200_adain_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns,
+                        float alpha, float eps, void* out, void* ws, size_t ws_bytes, void* stream);
+WCTB200_API int wctb200_adain_apply_blend(const void* content, int Nc, int Hc, int Wc, int C,
+                              const void* const* states, int K, const float* weights, int Nw,
+                              float alpha, float eps, void* out, void* ws, size_t ws_bytes, void* stream);
 
 /*
  * wct_style_swap (ops.py:145-217) + style_swap (ops.py:219-278) for ONE content/style pair: whiten both encodings, take every
@@ -247,6 +271,33 @@ WCTB200_API size_t wctb200_style_swap_workspace_bytes(int C, int Hc, int Wc, int
 WCTB200_API int wctb200_style_swap_level(const void* content, int Hc, int Wc, const void* style, int Hs, int Ws, int C,
                              int patch, int stride, float alpha, float eps_cov, float thresh, void* out, int32_t* k_out,
                              void* ws, size_t ws_bytes, void* stream);
+/*
+ * Split form of wctb200_style_swap_level, batched over content frames.  The style side depends only on the style encoding,
+ * the patch and the stride, so it is prepared once into a state, and an apply swaps Nc >= 1 frames against it in one call.
+ * wctb200_style_swap_level is prepare followed by apply with Nc = 1.  Frame i of an apply is bit-identical to
+ * wctb200_style_swap_level on that frame alone.
+ *   state: device buffer of wctb200_style_swap_state_bytes(C, Hs, Ws, patch, stride) bytes (0 for a bad geometry) holding the
+ *   style mean and k_s, the whitened style encoding the gather reads, the per-tap norms and the split-fp16 patch filters,
+ *   and the colouring operand (C_s split) with its bias.  Its layout is private to the library; it is rebuilt from the style
+ *   encoding, not stored.
+ *   prepare: style SPF16 [1,Hs,Ws,C]; ws of wctb200_style_swap_prepare_workspace_bytes(C, Hs, Ws, patch, stride) bytes;
+ *   k_out (may be NULL): [k_s].
+ *   apply: content SPF16 [Nc,Hc,Wc,C]; out SPF16 [Nc,Hc,Wc,C]; ws of
+ *   wctb200_style_swap_apply_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride) bytes; k_out (may be NULL):
+ *   [k_c x Nc | k_s].  The apply only reads the state.
+ * A null state, Nc < 1, C not in {64,128,256,512}, a patch or stride outside 1..16, a map smaller than the patch, or a
+ * patch / stride that does not tile the content encoding ((ho-1)*stride + patch == Hc, and the same for Wc) is
+ * WCTB200_EINVAL.
+ */
+WCTB200_API size_t wctb200_style_swap_state_bytes(int C, int Hs, int Ws, int patch, int stride);
+WCTB200_API size_t wctb200_style_swap_prepare_workspace_bytes(int C, int Hs, int Ws, int patch, int stride);
+WCTB200_API int wctb200_style_swap_prepare(const void* style, int Hs, int Ws, int C, int patch, int stride,
+                               float eps_cov, float thresh, void* state, int32_t* k_out,
+                               void* ws, size_t ws_bytes, void* stream);
+WCTB200_API size_t wctb200_style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride);
+WCTB200_API int wctb200_style_swap_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state,
+                             int Hs, int Ws, int patch, int stride, float alpha, float eps_cov, float thresh,
+                             void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
 
 /* Stand-alone pieces of the transform, exposed for parity tests and profiling:
  * per-channel mean [N][C] and covariance [N][C][C] = fc fc^T/(HW-1) + eps_cov*I of a feature batch

@@ -18,6 +18,11 @@ Texture synthesis: ``--noise [--noise-size H W] [--noise-count K] [--noise-seed 
 seeded uniform noise made on the device (default one 512x512 frame, seed 0), stylised in one batch per style, blend or mask;
 the outputs are named as above with the content ``noise<S>-<i>.png``, e.g. ``noise0-3_starry.png``.
 
+Prepared styles: ``--style-path``, ``--interp-styles`` and ``--mask-styles`` also take ``.wctstyle`` files written by
+``prepare_styles.py`` (in a folder, the entries ending in ``.wctstyle``).  Each is read once per run and reused for every
+content, pass and noise batch.  A run's styles are all prepared or all images, and prepared styles take no ``--style-size``,
+``--crop-size`` or ``--keep-colors`` (their size and crop were fixed when they were prepared).
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -98,7 +103,53 @@ def parse_args(argv=None):
     elif args.mask_styles:
         parser.error("--mask-styles needs --content-mask")
     check_noise_flags(parser, args)
+    check_prepared_flags(parser, args)
     return args
+
+
+PREPARED_EXT = ".wctstyle"
+
+
+def is_prepared(path):
+    return str(path).endswith(PREPARED_EXT)
+
+
+def style_listing(path, io):
+    """A style path as a list: a file, or a folder's images (imageio.get_files) and its ``.wctstyle`` files."""
+    if not os.path.isdir(path):
+        return [path]
+    prepared = sorted(os.path.join(path, f) for f in os.listdir(path) if is_prepared(f))
+    return [p for p in io.get_files(path) if not is_prepared(p)] + prepared
+
+
+def check_prepared_flags(parser, args, flags=("style_size", "crop_size", "keep_colors")):
+    """A run's styles are all prepared (.wctstyle) or all images; prepared styles were sized and cropped when they were
+    prepared, and CORAL (--keep-colors) changes the style per content."""
+    from wct_tf_b200 import imageio as io
+    paths = []
+    if getattr(args, "style_path", None):
+        paths += style_listing(args.style_path, io) if os.path.isdir(args.style_path) else [args.style_path]
+    paths += list(getattr(args, "interp_styles", None) or []) + list(getattr(args, "mask_styles", None) or [])
+    kinds = set(is_prepared(p) for p in paths)
+    if True not in kinds:
+        return
+    if len(kinds) > 1:
+        parser.error("prepared styles (.wctstyle) and style images do not mix in one run")
+    for attr in flags:
+        if getattr(args, attr, None):
+            parser.error("prepared styles (.wctstyle) do not combine with --%s" % attr.replace("_", "-"))
+
+
+class PreparedStyles(object):
+    """Reads each ``.wctstyle`` file once per run (``model.load_style``) and hands out the same prepared style after."""
+
+    def __init__(self, model):
+        self.model, self.cache = model, {}
+
+    def get(self, path):
+        if path not in self.cache:
+            self.cache[path] = self.model.load_style(path)
+        return self.cache[path]
 
 
 def check_noise_flags(parser, args):
@@ -195,8 +246,11 @@ def _contents(args, io, dimg, device):
         yield [content_path], content_dev
 
 
-def _prepare_style(path, args, io, dimg, content_dev, device):
-    """stylize.py:86-95 on the device: decode on the host, then resize / crop / CORAL without leaving the GPU."""
+def _prepare_style(path, args, io, dimg, content_dev, device, prepared=None):
+    """stylize.py:86-95 on the device: decode on the host, then resize / crop / CORAL without leaving the GPU.  A
+    ``.wctstyle`` file gives its prepared style (``prepared``: the run's PreparedStyles)."""
+    if is_prepared(path):
+        return prepared.get(path)
     img = dimg.to_device(io.get_img(path), device)
     if args.style_size > 0:
         img = dimg.resize_to(img, args.style_size)
@@ -242,8 +296,9 @@ def main_masked(args, model, io, dimg, t_start):
     os.makedirs(args.out_path, exist_ok=True)
     device = model.engine.device
     written = 0
+    prepared = PreparedStyles(model)
     for names, content_dev in _contents(args, io, dimg, device):
-        styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device) for p in args.mask_styles]
+        styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device, prepared) for p in args.mask_styles]
         results = _stylize_masked(model, content_dev, styles_dev, labels, args)
         for name, result in zip(names, results):
             target = os.path.join(args.out_path, mask_output_name(name, args.mask_styles))
@@ -260,8 +315,9 @@ def main_interp(args, model, io, dimg, t_start):
     device = model.engine.device
     kw = dict(alpha=args.alpha, adain=args.adain, return_device=True, style_weights=np.asarray(args.interp_weights, np.float64))
     written = 0
+    prepared = PreparedStyles(model)
     for names, content_dev in _contents(args, io, dimg, device):
-        styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device) for p in args.interp_styles]
+        styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device, prepared) for p in args.interp_styles]
         results = model.predict_batch(content_dev, styles_dev, **kw)
         for _ in range(args.passes - 1):
             results = model.predict_batch(results, styles_dev, **kw)
@@ -286,20 +342,23 @@ def main(argv=None, model_factory=make_model, image_ops=None):
         return main_interp(args, model, io, dimg, t_start)
     if args.content_mask is not None:
         return main_masked(args, model, io, dimg, t_start)
-    styles = _listing(args.style_path, io)
+    styles = style_listing(args.style_path, io)
     if os.path.isdir(args.style_path) and args.random > 0:
         styles = list(np.random.choice(styles, args.random))
     os.makedirs(args.out_path, exist_ok=True)
 
     device = model.engine.device
     written = 0
+    prepared = PreparedStyles(model)
     for names, content_dev in _contents(args, io, dimg, device):
         for style_path in styles:
-            style_dev = _prepare_style(style_path, args, io, dimg, content_dev, device)
+            style_dev = _prepare_style(style_path, args, io, dimg, content_dev, device, prepared)
             results = _stylize_pair(model, content_dev, style_dev, args)
             for name, result in zip(names, results):
                 if args.concat:
-                    result = dimg.concat_with_style(style_dev, result)
+                    # a prepared style keeps its image on the host for this
+                    shown = dimg.to_device(style_dev.image[0], device) if is_prepared(style_path) else style_dev
+                    result = dimg.concat_with_style(shown, result)
                 stem, ext = os.path.splitext(os.path.basename(name))
                 target = os.path.join(args.out_path, "{}_{}{}".format(stem, os.path.splitext(os.path.basename(style_path))[0], ext))
                 io.save_img(target, dimg.to_host(result))

@@ -78,6 +78,7 @@ def parse_args(argv=None):
         stylize.check_interp_flags(parser, args, _INTERP_EXCLUDES)
     if args.interp_styles is None and args.style_path is None:
         parser.error("--style-path (or --interp-styles) is required")
+    stylize.check_prepared_flags(parser, args)
     return args
 
 
@@ -138,16 +139,19 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
     for bi, group in enumerate(todo):
         frames = [f.result() for f in pending_loads]
         pending_loads = [pool.submit(io.get_img, f) for f, _ in todo[bi + 1]] if bi + 1 < len(todo) else []
-        same = all(fr.shape == frames[0].shape for fr in frames) and not args.keep_colors and not args.swap5
+        same = all(fr.shape == frames[0].shape for fr in frames) and not args.keep_colors
         first = bi * step                                      # clip index of the batch's first frame
         if same and len(frames) > 1:
             x = prep(dimg.to_device(np.stack(frames), device))
-            # --passes (stylize_video.py:119-121) run back to back on the device
-            out = wct_model.predict_batch(x, style_img if weights is not None else style_img[None], alpha=args.alpha,
+            # --passes (stylize_video.py:119-121) run back to back on the device; a style swap acts in the first pass and
+            # swaps the whole batch against the one style in one call
+            swap_kw = dict(swap5=True, ss_alpha=args.ss_alpha) if args.swap5 else {}
+            one = weights is not None or not hasattr(style_img, "shape")   # a list of styles, or a prepared style
+            out = wct_model.predict_batch(x, style_img if one else style_img[None], alpha=args.alpha,
                                           adain=args.adain, passes=args.passes, return_device=True,
-                                          **interp_kw(first, first + len(frames)))
+                                          **dict(interp_kw(first, first + len(frames)), **swap_kw))
             results = [(out[i], style_img) for i in range(len(frames))]
-        else:                                                  # per-frame styles (CORAL), style swap or ragged sizes
+        else:                                                  # per-frame styles (CORAL) or ragged sizes
             results = []
             for j, fr in enumerate(frames):
                 fr = prep(dimg.to_device(fr, device))
@@ -160,6 +164,8 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 results.append((o[0], style_rgb))
         for (_, out_f), (o, srgb) in zip(group, results):
             if args.concat:                                    # stylize_video.py:125-128
+                if getattr(srgb, "image", None) is not None:   # a prepared style keeps its image on the host
+                    srgb = dimg.to_device(srgb.image[0], device)
                 o = dimg.concat_with_style(srgb, o)
             writes.append(pool.submit(finish, out_f, dimg.to_host(o)))
             count += 1
@@ -194,10 +200,12 @@ def main(argv=None, wct_factory=None, image_ops=None):
     else:
         wct_model = wct_factory(args)
 
+    import stylize
+    prepared = stylize.PreparedStyles(wct_model)
     if args.interp_styles is not None:
         style_files = [None]                                   # one run with the blend of every --interp-styles image
     else:
-        style_files = io.get_files(args.style_path) if os.path.isdir(args.style_path) else [args.style_path]
+        style_files = stylize.style_listing(args.style_path, io)
     os.makedirs(args.out_path, exist_ok=True)
     from_dir = os.path.isdir(args.in_path)
     tmp_dir = args.tmp_dir or os.path.join(args.out_path, '_____fns_frames_%s' % random.randint(0, 99999))
@@ -219,6 +227,8 @@ def main(argv=None, wct_factory=None, image_ops=None):
             device = wct_model.engine.device if hasattr(wct_model, "engine") else None
 
             def load_style(path):
+                if stylize.is_prepared(path):
+                    return prepared.get(path)                  # read once per run
                 img = dimg.to_device(io.get_img(path), device)
                 if args.style_size > 0:
                     img = dimg.resize_to(img, args.style_size)
@@ -227,7 +237,6 @@ def main(argv=None, wct_factory=None, image_ops=None):
                 return img
             weights = None
             if style_fullpath is None:
-                import stylize
                 style_img = [load_style(p) for p in args.interp_styles]
                 if args.morph:
                     weights = morph_weights(len(in_files), len(args.interp_styles))

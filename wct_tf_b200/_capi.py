@@ -61,6 +61,17 @@ SIGNATURES = {
     "wctb200_covariance_regions": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _vp]),
     "wctb200_style_swap_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i]),
     "wctb200_style_swap_level": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_wct_style_state_layout": (_sz, [_i, _i, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
+    "wctb200_adain_style_state_bytes": (_sz, [_i, _i]),
+    "wctb200_adain_style_state_layout": (_sz, [_i, _i, C.POINTER(_sz), C.POINTER(_sz)]),
+    "wctb200_adain_style_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    "wctb200_adain_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _f, _f, _vp, _vp, _sz, _vp]),
+    "wctb200_adain_apply_blend": (_i, [_vp, _i, _i, _i, _i, C.POINTER(_vp), _i, _vp, _i, _f, _f, _vp, _vp, _sz, _vp]),
+    "wctb200_style_swap_state_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "wctb200_style_swap_prepare_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "wctb200_style_swap_prepare": (_i, [_vp, _i, _i, _i, _i, _i, _f, _f, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_style_swap_apply_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i, _i]),
+    "wctb200_style_swap_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _vp, _sz, _vp]),
 }
 
 # tuning / probe hooks (wct_tf_b200/csrc/wctb200_debug.h): NOT part of the ABI, bound for tools/ and tests/ only

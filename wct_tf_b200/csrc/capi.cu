@@ -97,6 +97,22 @@ size_t style_swap_workspace_bytes(int C, int Hc, int Wc, int Hs, int Ws, int P, 
 int launch_style_swap_level(const __half* content, int Hc, int Wc, const __half* style, int Hs, int Ws, int C, int patch, int stride,
                             float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
                             cudaStream_t st);
+size_t style_swap_state_bytes(int C, int Hs, int Ws, int P, int S);
+size_t style_swap_prepare_workspace_bytes(int C);
+size_t style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S);
+int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int patch, int stride, float eps_cov, float thresh,
+                              void* state, int32_t* k_out, void* ws, size_t ws_bytes, cudaStream_t st);
+int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
+                            int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
+                            cudaStream_t st);
+size_t wct_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_cs, size_t* off_k);
+size_t adain_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_var);
+int launch_adain_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, void* state, cudaStream_t st);
+int launch_adain_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha, float eps,
+                       __half* out, void* ws, size_t ws_bytes, cudaStream_t st);
+int launch_adain_apply_blend(const __half* content, int Nc, int Hc, int Wc, int C, const void* const* states, int K,
+                             const float* weights, int Nw, float alpha, float eps, __half* out, void* ws, size_t ws_bytes,
+                             cudaStream_t st);
 int launch_conv3x3_ref(const __half*, ActGeom, const float*, const float*, int, int, __half*, cudaStream_t);
 int launch_conv_head(const float*, int, int, int, const float*, const float*, __half*, cudaStream_t);
 int launch_conv_tail(const __half*, ActGeom, const float*, const float*, int, float*, cudaStream_t);
@@ -419,6 +435,68 @@ int wctb200_style_swap_level(const void* content, int Hc, int Wc, const void* st
     WCTB_REQUIRE(geom_ok(1, Hc, Wc, C) && geom_ok(1, Hs, Ws, C), "style_swap_level: bad geometry");
     return launch_style_swap_level(HCP(content), Hc, Wc, HCP(style), Hs, Ws, C, patch, stride, alpha, eps_cov, thresh, HP(out), k_out, ws,
                                    ws_bytes, ST(stream));
+}
+static bool swap_style_ok(int C, int Hs, int Ws, int patch, int stride) {
+    return geom_ok(1, Hs, Ws, C) && patch >= 1 && patch <= 16 && stride >= 1 && stride <= 16 && Hs >= patch && Ws >= patch;
+}
+size_t wctb200_style_swap_state_bytes(int C, int Hs, int Ws, int patch, int stride) {
+    if (!swap_style_ok(C, Hs, Ws, patch, stride)) return 0;
+    return style_swap_state_bytes(C, Hs, Ws, patch, stride);
+}
+size_t wctb200_style_swap_prepare_workspace_bytes(int C, int Hs, int Ws, int patch, int stride) {
+    if (!swap_style_ok(C, Hs, Ws, patch, stride)) return 0;
+    return style_swap_prepare_workspace_bytes(C);
+}
+int wctb200_style_swap_prepare(const void* style, int Hs, int Ws, int C, int patch, int stride, float eps_cov, float thresh, void* state,
+                               int32_t* k_out, void* ws, size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(style && state && ws, "style_swap_prepare: null pointer");
+    WCTB_REQUIRE(geom_ok(1, Hs, Ws, C), "style_swap_prepare: bad geometry");
+    return launch_style_swap_prepare(HCP(style), Hs, Ws, C, patch, stride, eps_cov, thresh, state, k_out, ws, ws_bytes, ST(stream));
+}
+size_t wctb200_style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride) {
+    if (!swap_style_ok(C, Hs, Ws, patch, stride) || !geom_ok(Nc, Hc, Wc, C) || Hc < patch || Wc < patch) return 0;
+    return style_swap_apply_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride);
+}
+int wctb200_style_swap_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch, int stride,
+                             float alpha, float eps_cov, float thresh, void* out, int32_t* k_out, void* ws, size_t ws_bytes,
+                             void* stream) {
+    WCTB_REQUIRE(content && state && out && ws, "style_swap_apply: null pointer");
+    WCTB_REQUIRE(Nc >= 1, "style_swap_apply: Nc=%d < 1", Nc);
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C) && geom_ok(1, Hs, Ws, C), "style_swap_apply: bad geometry");
+    return launch_style_swap_apply(HCP(content), Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, HP(out), k_out,
+                                   ws, ws_bytes, ST(stream));
+}
+size_t wctb200_wct_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_cs, size_t* off_k) {
+    if (C < 8 || Ns < 1) return 0;
+    return wct_style_state_layout(C, Ns, off_mean, off_cs, off_k);
+}
+size_t wctb200_adain_style_state_bytes(int C, int Ns) {
+    if (C < 8 || C % 8 != 0 || Ns < 1) return 0;
+    return adain_style_state_layout(C, Ns, nullptr, nullptr);
+}
+size_t wctb200_adain_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_var) {
+    if (C < 8 || C % 8 != 0 || Ns < 1) return 0;
+    return adain_style_state_layout(C, Ns, off_mean, off_var);
+}
+int wctb200_adain_style_prepare(const void* style, int Ns, int Hs, int Ws, int C, void* state, void* stream) {
+    WCTB_REQUIRE(style && state, "adain_style_prepare: null pointer");
+    WCTB_REQUIRE(geom_ok(Ns, Hs, Ws, C), "adain_style_prepare: bad geometry");
+    return launch_adain_style_prepare(HCP(style), Ns, Hs, Ws, C, state, ST(stream));
+}
+int wctb200_adain_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha, float eps,
+                        void* out, void* ws, size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(content && state && out && ws, "adain_apply: null pointer");
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "adain_apply: bad geometry");
+    return launch_adain_apply(HCP(content), Nc, Hc, Wc, C, state, Ns, alpha, eps, HP(out), ws, ws_bytes, ST(stream));
+}
+int wctb200_adain_apply_blend(const void* content, int Nc, int Hc, int Wc, int C, const void* const* states, int K,
+                              const float* weights, int Nw, float alpha, float eps, void* out, void* ws, size_t ws_bytes,
+                              void* stream) {
+    WCTB_REQUIRE(content && states && weights && out && ws, "adain_apply_blend: null pointer");
+    WCTB_REQUIRE(K >= 1 && K <= 8, "adain_apply_blend: K=%d not in 1..8", K);
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "adain_apply_blend: bad geometry");
+    return launch_adain_apply_blend(HCP(content), Nc, Hc, Wc, C, states, K, weights, Nw, alpha, eps, HP(out), ws, ws_bytes,
+                                    ST(stream));
 }
 // tuning hooks (wctb200_debug.h; not part of the stable ABI)
 int wctb200_debug_set_conv_bn(int bn) {

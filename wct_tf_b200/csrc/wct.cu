@@ -807,6 +807,14 @@ size_t wct_style_state_bytes(int C, int Ns) {
     size_t a, b;
     return style_state_offsets(C, Ns, &a, &b);
 }
+size_t wct_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_cs, size_t* off_k) {
+    size_t a, b;
+    const size_t total = style_state_offsets(C, Ns, &a, &b);
+    if (off_mean) *off_mean = 0;
+    if (off_cs) *off_cs = a;
+    if (off_k) *off_k = b;
+    return total;
+}
 
 int launch_wct_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, float eps_cov, float eps_eig, float thresh,
                              void* state, void* ws, size_t ws_bytes, cudaStream_t st) {
@@ -1046,77 +1054,164 @@ int launch_covariance(const __half* act, int N, int H, int W, int C, float eps_c
     return launch_mean_cov(act, ActGeom(N, H, W, C), eps_cov, mean_out, cov_out, nullptr, dsum, st);
 }
 
-int launch_adain_level(const __half* content, int Nc, int Hc, int Wc, const __half* style, int Ns, int Hs, int Ws, int C,
-                       float alpha, float eps, __half* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_level: C=%d must be a multiple of 8 (<= 2048)", C);
-    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "adain_level: Ns must be 1 or Nc");
-    const WctWs L = wct_layout(C, Nc, Ns);
-    if (ws_bytes < L.total) {
-        set_error("adain_level: workspace %zu < %zu bytes", ws_bytes, L.total);
-        return WCTB200_EWS;
-    }
-    uint8_t* w = static_cast<uint8_t*>(ws);
-    float* shift = reinterpret_cast<float*>(w + L.shift);
-    float* mean = reinterpret_cast<float*>(w + L.mean);
-    float* var = reinterpret_cast<float*>(w + L.var);
-    float* inv = reinterpret_cast<float*>(w + L.inv);
-    float* ms = reinterpret_cast<float*>(w + L.ms);
-    // slot partials of both sides in the per-stream scratch (their count depends on H x W, the workspace size does not)
+// ---------------------------------------------------------------------------
+// AdaIN in split form: the style side is the per-channel moments of the style, which depend on the style features only.
+//   state layout: [Ns][C] mean | [Ns][C] var (fp32, biased; what k_moments_finalize writes), 256-byte aligned blocks
+// The apply computes the content moments, the coefficients and the affine map in the workspace of
+// wct_layout(C, Nc, 0) (fields shift, mean, var, inv, ms).  adain_level and adain_blend are prepare followed by apply.
+// ---------------------------------------------------------------------------
+static size_t adain_state_offsets(int C, int Ns, size_t* off_var) {
+    *off_var = align_up((size_t)Ns * C * 4, 256);
+    return align_up(*off_var + (size_t)Ns * C * 4, 256);
+}
+size_t adain_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_var) {
+    size_t ov;
+    const size_t total = adain_state_offsets(C, Ns, &ov);
+    if (off_mean) *off_mean = 0;
+    if (off_var) *off_var = ov;
+    return total;
+}
+
+int launch_adain_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, void* state, cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_style_prepare: C=%d must be a multiple of 8 (<= 2048)", C);
+    size_t off_var;
+    adain_state_offsets(C, Ns, &off_var);
+    // centring shift and slot partials in the per-stream scratch
+    const size_t nshift = align_up((size_t)Ns * C, 64);
+    const size_t part = (size_t)Ns * cdiv((long long)Hs * Ws, moments_slice(C)) * 2 * C;
+    float* scratch = nullptr;
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&scratch), (nshift + part) * sizeof(float), st, 5); if (rc0) return rc0; }
+    uint8_t* sp = static_cast<uint8_t*>(state);
+    return launch_moments(style, ActGeom(Ns, Hs, Ws, C), scratch, scratch + nshift, reinterpret_cast<float*>(sp),
+                          reinterpret_cast<float*>(sp + off_var), st);
+}
+
+// content moments of the apply calls into the workspace of wct_layout(C, Nc, 0)
+static int adain_content_moments(const __half* content, int Nc, int Hc, int Wc, int C, uint8_t* w, const WctWs& L, cudaStream_t st) {
     const size_t part_c = (size_t)Nc * cdiv((long long)Hc * Wc, moments_slice(C)) * 2 * C;
-    const size_t part_s = (size_t)Ns * cdiv((long long)Hs * Ws, moments_slice(C)) * 2 * C;
     float* part = nullptr;
-    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&part), (part_c + part_s) * sizeof(float), st, 5); if (rc0) return rc0; }
-    ActGeom gc(Nc, Hc, Wc, C), gs(Ns, Hs, Ws, C);
-    int rc = launch_moments(content, gc, shift, part, mean, var, st);
-    if (rc) return rc;
-    const long long oc = (long long)Nc * C;
-    rc = launch_moments(style, gs, shift + oc, part + part_c, mean + oc, var + oc, st);
-    if (rc) return rc;
-    k_adain_coeffs<<<cdiv(oc, 256), 256, 0, st>>>(var, mean + oc, var + oc, C, Nc, Ns, eps, inv, ms);
-    WCTB_CHECK_LAUNCH("k_adain_coeffs");
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&part), part_c * sizeof(float), st, 5); if (rc0) return rc0; }
+    return launch_moments(content, ActGeom(Nc, Hc, Wc, C), reinterpret_cast<float*>(w + L.shift), part, reinterpret_cast<float*>(w + L.mean),
+                          reinterpret_cast<float*>(w + L.var), st);
+}
+static int adain_affine(const __half* content, int Nc, int Hc, int Wc, int C, float alpha, uint8_t* w, const WctWs& L, __half* out,
+                        cudaStream_t st) {
     const long long total = (long long)Nc * Hc * Wc * (C / 8);
     long long blocks = (total + 255) / 256;
     if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
-    k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(content, gc, mean, inv, ms, alpha, out);
+    k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(content, ActGeom(Nc, Hc, Wc, C), reinterpret_cast<const float*>(w + L.mean),
+                                                     reinterpret_cast<const float*>(w + L.inv), reinterpret_cast<const float*>(w + L.ms),
+                                                     alpha, out);
     WCTB_CHECK_LAUNCH("k_affine_apply");
     return 0;
 }
 
+int launch_adain_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha, float eps,
+                       __half* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_apply: C=%d must be a multiple of 8 (<= 2048)", C);
+    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "adain_apply: Ns must be 1 or Nc");
+    const WctWs L = wct_layout(C, Nc, 0);
+    if (ws_bytes < L.total) {
+        set_error("adain_apply: workspace %zu < %zu bytes", ws_bytes, L.total);
+        return WCTB200_EWS;
+    }
+    uint8_t* w = static_cast<uint8_t*>(ws);
+    size_t off_var;
+    adain_state_offsets(C, Ns, &off_var);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    int rc = adain_content_moments(content, Nc, Hc, Wc, C, w, L, st);
+    if (rc) return rc;
+    k_adain_coeffs<<<cdiv((long long)Nc * C, 256), 256, 0, st>>>(reinterpret_cast<const float*>(w + L.var), reinterpret_cast<const float*>(sp),
+                                                              reinterpret_cast<const float*>(sp + off_var), C, Nc, Ns, eps,
+                                                              reinterpret_cast<float*>(w + L.inv), reinterpret_cast<float*>(w + L.ms));
+    WCTB_CHECK_LAUNCH("k_adain_coeffs");
+    return adain_affine(content, Nc, Hc, Wc, C, alpha, w, L, out, st);
+}
+
+int launch_adain_level(const __half* content, int Nc, int Hc, int Wc, const __half* style, int Ns, int Hs, int Ws, int C,
+                       float alpha, float eps, __half* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_level: C=%d must be a multiple of 8 (<= 2048)", C);
+    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "adain_level: Ns must be 1 or Nc");
+    const size_t need = wct_layout(C, Nc, Ns).total;
+    if (ws_bytes < need) {
+        set_error("adain_level: workspace %zu < %zu bytes", ws_bytes, need);
+        return WCTB200_EWS;
+    }
+    // the apply's workspace, then the style state (wct_layout(C, Nc, Ns) holds both)
+    const size_t base = wct_layout(C, Nc, 0).total;
+    size_t off_var;
+    const size_t sbytes = adain_state_offsets(C, Ns, &off_var);
+    WCTB_REQUIRE(base + sbytes <= need, "adain_level: workspace layout");
+    uint8_t* state = static_cast<uint8_t*>(ws) + base;
+    int rc = launch_adain_style_prepare(style, Ns, Hs, Ws, C, state, st);
+    if (rc) return rc;
+    return launch_adain_apply(content, Nc, Hc, Wc, C, state, Ns, alpha, eps, out, ws, base, st);
+}
+
 // AdaIN of a style blend: inv = rsqrt(vc + eps) * sum_k w_k sqrt(v_sk) and ms = sum_k w_k m_sk per (frame, channel), in k
 // order from the product w_0 S_0 (K = 1 with weight 1 gives k_adain_coeffs' values bit for bit).  Weight row z, or 0 if Nw == 1.
-__global__ void k_adain_blend_coeffs(const float* __restrict__ var_c, const float* __restrict__ mean_s, const float* __restrict__ var_s,
-                                     int C, int Nc, int K, const float* __restrict__ weights, int Nw, float eps,
-                                     float* __restrict__ inv, float* __restrict__ ms) {
+struct AdainSrc {
+    const float* mean[8];
+    const float* var[8];
+};
+__global__ void k_adain_blend_coeffs(const float* __restrict__ var_c, AdainSrc src, int C, int Nc, int K,
+                                     const float* __restrict__ weights, int Nw, float eps, float* __restrict__ inv,
+                                     float* __restrict__ ms) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= Nc * C) return;
     const int z = i / C, c = i % C;
     const float* wr = weights + (long long)(Nw == 1 ? 0 : z) * K;
-    float s = __fmul_rn(wr[0], sqrtf(var_s[c])), m = __fmul_rn(wr[0], mean_s[c]);
-    for (int k = 1; k < K; ++k) {
-        s = fmaf(wr[k], sqrtf(var_s[(long long)k * C + c]), s);
-        m = fmaf(wr[k], mean_s[(long long)k * C + c], m);
+    float s = __fmul_rn(wr[0], sqrtf(src.var[0][c])), m = __fmul_rn(wr[0], src.mean[0][c]);
+#pragma unroll
+    for (int k = 1; k < 8; ++k) {              // unrolled: the state pointers stay in the parameter space
+        if (k < K) {
+            s = fmaf(wr[k], sqrtf(src.var[k][c]), s);
+            m = fmaf(wr[k], src.mean[k][c], m);
+        }
     }
     inv[i] = rsqrtf(var_c[i] + eps) * s;
     ms[i] = m;
 }
 
-struct AdainBlendWs {
-    size_t shift, mean, var, inv, ms, total;
-};
-static AdainBlendWs adain_blend_layout(int C, int Nc, int K) {
-    AdainBlendWs L;
-    const size_t np = (size_t)Nc + K;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
-    L.shift = take(np * C * 4);        // content frames then the K styles
-    L.mean = take(np * C * 4);
-    L.var = take(np * C * 4);
-    L.inv = take((size_t)Nc * C * 4);
-    L.ms = take((size_t)Nc * C * 4);
-    L.total = o;
-    return L;
+int launch_adain_apply_blend(const __half* content, int Nc, int Hc, int Wc, int C, const void* const* states, int K,
+                             const float* weights, int Nw, float alpha, float eps, __half* out, void* ws, size_t ws_bytes,
+                             cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_apply_blend: C=%d must be a multiple of 8 (<= 2048)", C);
+    WCTB_REQUIRE(K >= 1 && K <= 8, "adain_apply_blend: K=%d not in 1..8", K);
+    WCTB_REQUIRE(Nw == 1 || Nw == Nc, "adain_apply_blend: Nw=%d must be 1 or Nc=%d", Nw, Nc);
+    const WctWs L = wct_layout(C, Nc, 0);
+    if (ws_bytes < L.total) {
+        set_error("adain_apply_blend: workspace %zu < %zu bytes", ws_bytes, L.total);
+        return WCTB200_EWS;
+    }
+    // each state from adain_style_prepare with Ns = 1: [C] mean | [C] var
+    size_t off_var;
+    adain_state_offsets(C, 1, &off_var);
+    AdainSrc src = {};
+    for (int k = 0; k < K; ++k) {
+        WCTB_REQUIRE(states[k], "adain_apply_blend: style state %d is null", k);
+        src.mean[k] = static_cast<const float*>(states[k]);
+        src.var[k] = reinterpret_cast<const float*>(static_cast<const uint8_t*>(states[k]) + off_var);
+    }
+    uint8_t* w = static_cast<uint8_t*>(ws);
+    int rc = adain_content_moments(content, Nc, Hc, Wc, C, w, L, st);
+    if (rc) return rc;
+    k_adain_blend_coeffs<<<cdiv((long long)Nc * C, 256), 256, 0, st>>>(reinterpret_cast<const float*>(w + L.var), src, C, Nc, K, weights,
+                                                                    Nw, eps, reinterpret_cast<float*>(w + L.inv),
+                                                                    reinterpret_cast<float*>(w + L.ms));
+    WCTB_CHECK_LAUNCH("k_adain_blend_coeffs");
+    return adain_affine(content, Nc, Hc, Wc, C, alpha, w, L, out, st);
 }
-size_t adain_blend_workspace_bytes(int C, int Nc, int K) { return adain_blend_layout(C, Nc, K).total; }
+
+// adain_blend: the K style states after the apply's workspace
+static size_t adain_blend_layout(int C, int Nc, int K, size_t* state_bytes) {
+    *state_bytes = adain_style_state_layout(C, 1, nullptr, nullptr);
+    return wct_layout(C, Nc, 0).total + (size_t)K * *state_bytes;
+}
+size_t adain_blend_workspace_bytes(int C, int Nc, int K) {
+    size_t sb;
+    return adain_blend_layout(C, Nc, K, &sb);
+}
 
 int launch_adain_blend(const __half* content, int Nc, int Hc, int Wc, int C, const void* const* styles, const int* Hs, const int* Ws,
                        int K, const float* weights, int Nw, float alpha, float eps, __half* out, void* ws, size_t ws_bytes,
@@ -1124,45 +1219,23 @@ int launch_adain_blend(const __half* content, int Nc, int Hc, int Wc, int C, con
     WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_blend: C=%d must be a multiple of 8 (<= 2048)", C);
     WCTB_REQUIRE(K >= 1 && K <= 8, "adain_blend: K=%d not in 1..8", K);
     WCTB_REQUIRE(Nw == 1 || Nw == Nc, "adain_blend: Nw=%d must be 1 or Nc=%d", Nw, Nc);
-    const AdainBlendWs L = adain_blend_layout(C, Nc, K);
-    if (ws_bytes < L.total) {
-        set_error("adain_blend: workspace %zu < %zu bytes", ws_bytes, L.total);
+    size_t sbytes;
+    const size_t need = adain_blend_layout(C, Nc, K, &sbytes);
+    if (ws_bytes < need) {
+        set_error("adain_blend: workspace %zu < %zu bytes", ws_bytes, need);
         return WCTB200_EWS;
     }
-    uint8_t* w = static_cast<uint8_t*>(ws);
-    float* shift = reinterpret_cast<float*>(w + L.shift);
-    float* mean = reinterpret_cast<float*>(w + L.mean);
-    float* var = reinterpret_cast<float*>(w + L.var);
-    float* inv = reinterpret_cast<float*>(w + L.inv);
-    float* ms = reinterpret_cast<float*>(w + L.ms);
-    // slot partials of the content and of every style in the per-stream scratch, as adain_level's
-    size_t part_off[9];
-    part_off[0] = (size_t)Nc * cdiv((long long)Hc * Wc, moments_slice(C)) * 2 * C;
+    const size_t base = wct_layout(C, Nc, 0).total;
+    const void* states[8];
     for (int k = 0; k < K; ++k) {
         WCTB_REQUIRE(styles[k], "adain_blend: style %d is null", k);
         WCTB_REQUIRE(Hs[k] >= 2 && Ws[k] >= 2, "adain_blend: style %d is %dx%d", k, Hs[k], Ws[k]);
-        part_off[k + 1] = part_off[k] + (size_t)cdiv((long long)Hs[k] * Ws[k], moments_slice(C)) * 2 * C;
-    }
-    float* part = nullptr;
-    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&part), part_off[K] * sizeof(float), st, 5); if (rc0) return rc0; }
-    ActGeom gc(Nc, Hc, Wc, C);
-    int rc = launch_moments(content, gc, shift, part, mean, var, st);
-    if (rc) return rc;
-    const long long oc = (long long)Nc * C;
-    for (int k = 0; k < K; ++k) {
-        const long long o = oc + (long long)k * C;
-        rc = launch_moments(static_cast<const __half*>(styles[k]), ActGeom(1, Hs[k], Ws[k], C), shift + o, part + part_off[k], mean + o,
-                            var + o, st);
+        void* state = static_cast<uint8_t*>(ws) + base + (size_t)k * sbytes;
+        int rc = launch_adain_style_prepare(static_cast<const __half*>(styles[k]), 1, Hs[k], Ws[k], C, state, st);
         if (rc) return rc;
+        states[k] = state;
     }
-    k_adain_blend_coeffs<<<cdiv(oc, 256), 256, 0, st>>>(var, mean + oc, var + oc, C, Nc, K, weights, Nw, eps, inv, ms);
-    WCTB_CHECK_LAUNCH("k_adain_blend_coeffs");
-    const long long total = (long long)Nc * Hc * Wc * (C / 8);
-    long long blocks = (total + 255) / 256;
-    if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
-    k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(content, gc, mean, inv, ms, alpha, out);
-    WCTB_CHECK_LAUNCH("k_affine_apply");
-    return 0;
+    return launch_adain_apply_blend(content, Nc, Hc, Wc, C, states, K, weights, Nw, alpha, eps, out, ws, base, st);
 }
 
 // ---------------------------------------------------------------------------
@@ -1403,40 +1476,85 @@ static inline int swap_grid(long long total, int block) {
     return (int)(b < 1 ? 1 : (b > device_sm_count() * 32ll ? device_sm_count() * 32ll : b));
 }
 
-struct SwapWs {
-    size_t base, zeros, dvec2, sigma2, mats, msplit, bias3, norms, idx, wc_feat, ws_feat, ss_feat, tmp, scores, wsplit, total;
-    int cout_pad, n_patches, prow, pcol, ho, wo;   // style patch grid prow x pcol, content score grid ho x wo
+// The style swap in split form.  The style side -- whitening of the style, its patch filters and the colouring operand --
+// depends only on the style features, so it is prepared once into a state and applied to any number of content frames.
+//   state layout (256-byte aligned blocks): [C] mean_s | int32 [2] (k_s, sweeps_s) | whitened style SPF16 [1,Hs,Ws,C]
+//   (gathered from) | [P*P][C] 1/||tap|| | split-fp16 patch filters [2][cout_pad][P*P*C] | colouring operand [2][C][C] (C_s
+//   split) | [C] its bias (m_s)
+struct SwapState {
+    size_t mean, k, feat, norms, wsplit, cmsplit, cbias, total;
+    int cout_pad, n_patches, prow, pcol;           // style patch grid prow x pcol
 };
-static SwapWs swap_layout(int C, int Hc, int Wc, int Hs, int Ws, int P, int S) {
-    SwapWs L;
+static SwapState swap_state_layout(int C, int Hs, int Ws, int P, int S) {
+    SwapState L;
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
     L.prow = (Hs - P) / S + 1;                                    // tf.extract_image_patches, VALID (ops.py:226)
     L.pcol = (Ws - P) / S + 1;
-    L.ho = (Hc - P) / S + 1;                                      // tf.nn.conv2d VALID with the same stride (ops.py:236-239)
-    L.wo = (Wc - P) / S + 1;
     L.n_patches = L.prow * L.pcol;
     L.cout_pad = (L.n_patches + 63) / 64 * 64;
-    L.base = take(wct_layout(C, 1, 1).total);
-    L.zeros = take((size_t)C * 4);
-    L.dvec2 = take((size_t)C * 4);
-    L.sigma2 = take((size_t)C * 4);
-    L.mats = take((size_t)3 * C * C * 4);                         // W_c, W_s (whitening), C_s (colouring)
-    L.msplit = take((size_t)3 * 2 * C * C * 2);
-    L.bias3 = take((size_t)3 * C * 4);
+    L.mean = take((size_t)C * 4);
+    L.k = take(2 * 4);
+    L.feat = take((size_t)ActGeom(1, Hs, Ws, C).plane * 2 * sizeof(__half));
     L.norms = take((size_t)P * P * C * 4);
-    L.idx = take((size_t)L.ho * L.wo * 4);
-    const size_t fc = (size_t)ActGeom(1, Hc, Wc, C).plane * 2 * sizeof(__half), fs = (size_t)ActGeom(1, Hs, Ws, C).plane * 2 * sizeof(__half);
-    L.wc_feat = take(fc);
-    L.ws_feat = take(fs);
-    L.ss_feat = take(fc);
-    L.tmp = take(fc);
-    L.scores = take((size_t)ActGeom(1, Hc, Wc, L.cout_pad).plane * 2 * sizeof(__half));
     L.wsplit = take((size_t)2 * P * P * C * L.cout_pad * sizeof(__half));
+    L.cmsplit = take((size_t)2 * C * C * 2);
+    L.cbias = take((size_t)C * 4);
     L.total = o;
     return L;
 }
-size_t style_swap_workspace_bytes(int C, int Hc, int Wc, int Hs, int Ws, int P, int S) { return swap_layout(C, Hc, Wc, Hs, Ws, P, S).total; }
+// workspace of the prepare: the eigensolver's (wct_layout(C, 0, 1)) and the style's whitening / colouring matrices
+struct SwapPrepWs {
+    size_t base, zeros, dvec2, sigma2, Wm, Cm, msplit, bias, total;
+};
+static SwapPrepWs swap_prep_layout(int C) {
+    SwapPrepWs L;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.base = take(wct_layout(C, 0, 1).total);
+    L.zeros = take((size_t)C * 4);
+    L.dvec2 = take((size_t)C * 4);
+    L.sigma2 = take((size_t)C * 4);
+    L.Wm = take((size_t)C * C * 4);                               // W_s (whitening)
+    L.Cm = take((size_t)C * C * 4);                               // C_s (colouring)
+    L.msplit = take((size_t)2 * C * C * 2);
+    L.bias = take((size_t)C * 4);
+    L.total = o;
+    return L;
+}
+// workspace of the apply over Nc frames: the content side (wct_layout(C, Nc, 0): per-frame whitening operands), the
+// whitened, swapped and coloured features, the correlation scores and the arg-max per VALID position
+struct SwapApplyWs {
+    size_t base, zeros, idx, wc_feat, ss_feat, tmp, scores, total;
+    int ho, wo;                                     // content score grid ho x wo
+};
+static SwapApplyWs swap_apply_layout(int C, int Nc, int Hc, int Wc, int P, int S, int cout_pad) {
+    SwapApplyWs L;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.ho = (Hc - P) / S + 1;                                      // tf.nn.conv2d VALID with the same stride (ops.py:236-239)
+    L.wo = (Wc - P) / S + 1;
+    L.base = take(wct_layout(C, Nc, 0).total);
+    L.zeros = take((size_t)C * 4);
+    L.idx = take((size_t)Nc * L.ho * L.wo * 4);
+    const size_t fc = (size_t)ActGeom(Nc, Hc, Wc, C).plane * 2 * sizeof(__half);
+    L.wc_feat = take(fc);
+    L.ss_feat = take(fc);
+    L.tmp = take(fc);
+    L.scores = take((size_t)ActGeom(Nc, Hc, Wc, cout_pad).plane * 2 * sizeof(__half));
+    L.total = o;
+    return L;
+}
+size_t style_swap_state_bytes(int C, int Hs, int Ws, int P, int S) { return swap_state_layout(C, Hs, Ws, P, S).total; }
+size_t style_swap_prepare_workspace_bytes(int C) { return swap_prep_layout(C).total; }
+size_t style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    return swap_apply_layout(C, Nc, Hc, Wc, P, S, swap_state_layout(C, Hs, Ws, P, S).cout_pad).total;
+}
+// style_swap_level: the state, then the prepare's or the apply's workspace
+size_t style_swap_workspace_bytes(int C, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    const size_t a = style_swap_prepare_workspace_bytes(C), b = style_swap_apply_workspace_bytes(C, 1, Hc, Wc, Hs, Ws, P, S);
+    return style_swap_state_bytes(C, Hs, Ws, P, S) + (a > b ? a : b);
+}
 
 // patch geometry of the swap: P x P patches taken every S pixels (ops.py:219-278: --ss-patch-size, --ss-stride)
 struct SwapGeom { int P, S, prow, pcol, ho, wo; };
@@ -1475,13 +1593,15 @@ __global__ void k_swap_patch_weights(const __half* __restrict__ feat, ActGeom g,
         wsplit[total + i] = lo;
     }
 }
-// first arg-max over the patch axis for every VALID strided position (y,x): the top-left-anchored P x P correlation
-// at interior pixel (y*S, x*S), which the conv kernel stored at that pixel's own padded cell
+// first arg-max over the patch axis for every VALID strided position (y,x) of frame blockIdx.y: the top-left-anchored P x P
+// correlation at interior pixel (y*S, x*S), which the conv kernel stored at that pixel's own padded cell.  A VALID anchor
+// reads padded rows y*S+1 .. y*S+P <= H of its own frame only, so a batch of frames in one correlation keeps them apart.
 __global__ void k_swap_argmax(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n_patches, int* __restrict__ idx) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= q.ho * q.wo) return;
+    const int n = blockIdx.y;
     const int y = warp / q.wo, x = warp - y * q.wo;
-    const long long pos = ((long long)(y * q.S + 1)) * g.Wp + (x * q.S + 1);
+    const long long pos = ((long long)n * g.Hp + y * q.S + 1) * g.Wp + (x * q.S + 1);
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (int n = lane; n < n_patches; n += 32) {
@@ -1494,19 +1614,24 @@ __global__ void k_swap_argmax(const __half* __restrict__ scores, ActGeom g, Swap
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
         if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
     }
-    if (lane == 0) idx[warp] = bi;
+    if (lane == 0) idx[(long long)n * q.ho * q.wo + warp] = bi;
 }
 // conv2d_transpose of the one-hot map with the raw patches, divided by the overlap count (ops.py:255-276): output pixel
 // (Y,X) averages, over the <= P*P patch positions (py,px) with py*S + dy = Y, px*S + dx = X that cover it, the style
 // pixel (sy*S + dy, sx*S + dx) of the matched patch.  The caller guarantees (ho-1)*S + P == H (wct.py:84-90 refits).
+// gc.N frames, each with its own arg-max map [ho*wo], all against the one style feature.
 __global__ void k_swap_gather(const __half* __restrict__ sfeat, ActGeom gs, SwapGeom q, const int* __restrict__ idx, ActGeom gc,
                               __half* __restrict__ out) {
     const int cg = gc.C / 8;
-    const long long total = (long long)gc.H * gc.W * cg;
+    const long long hw = (long long)gc.H * gc.W;
+    const long long total = (long long)gc.N * hw * cg;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int c0 = (int)(i % cg) * 8;
-        const int pix = (int)(i / cg);
+        const long long fp = i / cg;
+        const int n = (int)(fp / hw);
+        const int pix = (int)(fp - n * hw);
         const int Y = pix / gc.W, X = pix - Y * gc.W;
+        const int* fidx = idx + (long long)n * q.ho * q.wo;
         float acc[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[j] = 0.f;
@@ -1517,8 +1642,8 @@ __global__ void k_swap_gather(const __half* __restrict__ sfeat, ActGeom gs, Swap
             for (int dx = 0; dx < q.P; ++dx) {
                 const int tx = X - dx;
                 if (tx < 0 || tx % q.S != 0 || tx / q.S >= q.wo) continue;
-                const int n = idx[(ty / q.S) * q.wo + tx / q.S];
-                const int sy = n / q.pcol, sx = n - sy * q.pcol;
+                const int m = fidx[(ty / q.S) * q.wo + tx / q.S];
+                const int sy = m / q.pcol, sx = m - sy * q.pcol;
                 float v[8];
                 load8(sfeat, gs, ((long long)(sy * q.S + dy + 1)) * gs.Wp + (sx * q.S + dx + 1), c0, v);
 #pragma unroll
@@ -1531,7 +1656,7 @@ __global__ void k_swap_gather(const __half* __restrict__ sfeat, ActGeom gs, Swap
         for (int j = 0; j < 8; ++j) acc[j] *= inv;
         Half8 hi, lo;
         split8(acc, hi, lo);
-        store8_with_halo(out, gc, 0, Y, X, c0, hi, lo);
+        store8_with_halo(out, gc, n, Y, X, c0, hi, lo);
     }
 }
 // out = a*x + b*y on SPF16 interiors (+ halos)
@@ -1557,100 +1682,193 @@ __global__ void k_blend2(const __half* __restrict__ x, const __half* __restrict_
     }
 }
 
-int launch_style_swap_level(const __half* content, int Hc, int Wc, const __half* style, int Hs, int Ws, int C, int patch, int stride,
-                            float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
-                            cudaStream_t st) {
+static int swap_check_style(int C, int Hs, int Ws, int patch, int stride) {
     WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "style_swap: C=%d not in {64,128,256,512}", C);
     WCTB_REQUIRE(patch >= 1 && patch <= 16 && stride >= 1 && stride <= 16, "style_swap: patch %d / stride %d out of range", patch, stride);
-    WCTB_REQUIRE(Hc >= patch && Wc >= patch && Hs >= patch && Ws >= patch && Hc >= 2 && Wc >= 2 && Hs >= 2 && Ws >= 2,
-                 "style_swap: maps must be at least %dx%d (content %dx%d, style %dx%d)", patch, patch, Hc, Wc, Hs, Ws);
-    const SwapWs S = swap_layout(C, Hc, Wc, Hs, Ws, patch, stride);
-    // the swapped encoding must have the content's size (ops.py:199 reshapes it to [Hc*Wc, C]); wct.py:84-90 crops the content
-    // image beforehand when the stride makes the filter not fit (utils.swap_filter_fit)
-    WCTB_REQUIRE((S.ho - 1) * stride + patch == Hc && (S.wo - 1) * stride + patch == Wc,
-                 "style_swap: patch %d / stride %d does not tile a %dx%d encoding (refit the content: swap_filter_fit, wct.py:84-90)",
-                 patch, stride, Hc, Wc);
-    const SwapGeom q = {patch, stride, S.prow, S.pcol, S.ho, S.wo};
-    if (ws_bytes < S.total) {
-        set_error("style_swap: workspace %zu < %zu bytes", ws_bytes, S.total);
+    WCTB_REQUIRE(Hs >= patch && Ws >= patch && Hs >= 2 && Ws >= 2, "style_swap: the style map must be at least %dx%d (style %dx%d)",
+                 patch, patch, Hs, Ws);
+    return 0;
+}
+
+// Style side: whiten the style (S^-1/2, ops.py:193), colour operand S^+1/2 and m_s (ops.py:203-206), the whitened style
+// feature, its per-tap norms and the patch filters of the correlation (ops.py:226-233).
+int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int patch, int stride, float eps_cov, float thresh,
+                              void* state, int32_t* k_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    int rc = swap_check_style(C, Hs, Ws, patch, stride);
+    if (rc) return rc;
+    const SwapPrepWs PL = swap_prep_layout(C);
+    if (ws_bytes < PL.total) {
+        set_error("style_swap_prepare: workspace %zu < %zu bytes", ws_bytes, PL.total);
         return WCTB200_EWS;
     }
+    const SwapState SL = swap_state_layout(C, Hs, Ws, patch, stride);
+    const SwapGeom q = {patch, stride, SL.prow, SL.pcol, 0, 0};
     uint8_t* sw = static_cast<uint8_t*>(ws);
-    const WctWs L = wct_layout(C, 1, 1);
-    uint8_t* w = sw + S.base;
+    uint8_t* sp = static_cast<uint8_t*>(state);
+    const WctWs L = wct_layout(C, 0, 1);
+    uint8_t* w = sw + PL.base;
     double* dsum = reinterpret_cast<double*>(w + L.dsum);
-    float* mean = reinterpret_cast<float*>(w + L.mean);          // [mc, ms]
     float* G = reinterpret_cast<float*>(w + L.G);
     float* A0 = reinterpret_cast<float*>(w + L.A0);
     float* lam = reinterpret_cast<float*>(w + L.lam);
     float* sigma = reinterpret_cast<float*>(w + L.sigma);
-    float* dvec = reinterpret_cast<float*>(w + L.dvec);          // whitening scalings of content and style
+    float* dvec = reinterpret_cast<float*>(w + L.dvec);          // whitening scaling of the style
     float* conv = reinterpret_cast<float*>(w + L.conv);
-    int* kc = reinterpret_cast<int*>(w + L.kcount);
-    float* zeros = reinterpret_cast<float*>(sw + S.zeros);
-    float* dvec2 = reinterpret_cast<float*>(sw + S.dvec2);       // colouring scaling of the style
-    float* sigma2 = reinterpret_cast<float*>(sw + S.sigma2);
-    float* mats = reinterpret_cast<float*>(sw + S.mats);
-    __half* msplit = reinterpret_cast<__half*>(sw + S.msplit);
-    float* bias3 = reinterpret_cast<float*>(sw + S.bias3);
-    float* norms = reinterpret_cast<float*>(sw + S.norms);
-    int* idx = reinterpret_cast<int*>(sw + S.idx);
-    __half* wc_feat = reinterpret_cast<__half*>(sw + S.wc_feat);
-    __half* ws_feat = reinterpret_cast<__half*>(sw + S.ws_feat);
-    __half* ss_feat = reinterpret_cast<__half*>(sw + S.ss_feat);
-    __half* tmp = reinterpret_cast<__half*>(sw + S.tmp);
-    __half* scores = reinterpret_cast<__half*>(sw + S.scores);
-    __half* wsplit = reinterpret_cast<__half*>(sw + S.wsplit);
+    float* zeros = reinterpret_cast<float*>(sw + PL.zeros);
+    float* dvec2 = reinterpret_cast<float*>(sw + PL.dvec2);      // colouring scaling of the style
+    float* sigma2 = reinterpret_cast<float*>(sw + PL.sigma2);
+    float* Wm = reinterpret_cast<float*>(sw + PL.Wm);
+    float* Cm = reinterpret_cast<float*>(sw + PL.Cm);
+    __half* msplit = reinterpret_cast<__half*>(sw + PL.msplit);
+    float* bias = reinterpret_cast<float*>(sw + PL.bias);
+    float* mean_s = reinterpret_cast<float*>(sp + SL.mean);
+    int* ks = reinterpret_cast<int*>(sp + SL.k);
+    __half* feat = reinterpret_cast<__half*>(sp + SL.feat);
+    float* norms = reinterpret_cast<float*>(sp + SL.norms);
+    __half* wsplit = reinterpret_cast<__half*>(sp + SL.wsplit);
     const long long CC = (long long)C * C;
 
-    WCTB_CUDA(cudaMemsetAsync(kc, 0, 4 * 4, st));
+    WCTB_CUDA(cudaMemsetAsync(ks, 0, 2 * 4, st));
     WCTB_CUDA(cudaMemsetAsync(zeros, 0, (size_t)C * 4, st));
-    ActGeom gc(1, Hc, Wc, C), gs(1, Hs, Ws, C);
-    int rc = launch_mean_cov(content, gc, eps_cov, mean, G, A0, dsum, st);
+    ActGeom gs(1, Hs, Ws, C);
+    rc = launch_mean_cov(style, gs, eps_cov, mean_s, G, A0, dsum, st);
     if (rc) return rc;
-    rc = launch_mean_cov(style, gs, eps_cov, mean + C, G + CC, A0 + CC, dsum + C, st);
+    rc = launch_jacobi(G, C, 1, conv, ks + 1, st, nullptr);
     if (rc) return rc;
-    rc = launch_jacobi(G, C, 2, conv, kc + 2, st, nullptr);
+    rc = launch_eig_post(G, A0, lam, C, 1, thresh, 0.f, 1, sigma, dvec, ks, st);                // S^-1/2 (ops.py:193)
     if (rc) return rc;
-    rc = launch_eig_post(G, A0, lam, C, 2, thresh, 0.f, 2, sigma, dvec, kc, st);          // S^-1/2 for BOTH (ops.py:187,193)
-    if (rc) return rc;
-    k_eig_post<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(G + CC, lam + C, C, thresh, 0.f, 0, sigma2, dvec2, nullptr, nullptr);   // S^+1/2 (ops.py:203)
+    k_eig_post<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(G, lam, C, thresh, 0.f, 0, sigma2, dvec2, nullptr, nullptr);   // S^+1/2 (ops.py:203)
     WCTB_CHECK_LAUNCH("k_eig_post(colour)");
-    dim3 g2((unsigned)(C / 64), (unsigned)(C / 64), 2), g1((unsigned)(C / 64), (unsigned)(C / 64), 1);
-    k_outer_gemm<<<g2, 256, 0, st>>>(G, CC, G, CC, dvec, C, mats, CC, C);                   // W_c, W_s
+    dim3 g1((unsigned)(C / 64), (unsigned)(C / 64), 1);
+    k_outer_gemm<<<g1, 256, 0, st>>>(G, CC, G, CC, dvec, C, Wm, CC, C);                        // W_s
     WCTB_CHECK_LAUNCH("k_outer_gemm(whiten)");
-    k_outer_gemm<<<g1, 256, 0, st>>>(G + CC, CC, G + CC, CC, dvec2, C, mats + 2 * CC, CC, C);   // C_s
+    k_outer_gemm<<<g1, 256, 0, st>>>(G, CC, G, CC, dvec2, C, Cm, CC, C);                       // C_s
     WCTB_CHECK_LAUNCH("k_outer_gemm(colour)");
-    // operand 0/1: x -> W (x - m)   (alpha = 1, "style mean" = 0);  operand 2: x -> C_s x + m_s  ("content mean" = 0)
-    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), 2), 256, 0, st>>>(mats, C, 2, 1, 1.f, 0, mean, zeros, msplit, bias3);
+    // whitening operand: x -> W_s (x - m_s) (alpha = 1, "style mean" = 0); colouring operand: x -> C_s x + m_s ("content mean" = 0)
+    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(Wm, C, 1, 1, 1.f, 0, mean_s, zeros, msplit, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform(whiten)");
-    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(mats + 2 * CC, C, 1, 1, 1.f, 0, zeros, mean + C, msplit + 4 * CC,
-                                                                         bias3 + 2 * C);
+    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(Cm, C, 1, 1, 1.f, 0, zeros, mean_s,
+                                                                         reinterpret_cast<__half*>(sp + SL.cmsplit),
+                                                                         reinterpret_cast<float*>(sp + SL.cbias));
     WCTB_CHECK_LAUNCH("k_finalize_transform(colour)");
-    rc = launch_conv_tc(CONV_APPLY, content, 1, Hc, Wc, C, msplit, 1, nullptr, bias3, C, 0, wc_feat, st);
+    rc = launch_conv_tc(CONV_APPLY, style, 1, Hs, Ws, C, msplit, 1, nullptr, bias, C, 0, feat, st);
     if (rc) return rc;
-    rc = launch_conv_tc(CONV_APPLY, style, 1, Hs, Ws, C, msplit + 2 * CC, 1, nullptr, bias3 + C, C, 0, ws_feat, st);
-    if (rc) return rc;
-    k_swap_tap_norms<<<dim3((unsigned)cdiv(C, 256), (unsigned)(patch * patch)), 256, 0, st>>>(ws_feat, gs, q, norms);
+    k_swap_tap_norms<<<dim3((unsigned)cdiv(C, 256), (unsigned)(patch * patch)), 256, 0, st>>>(feat, gs, q, norms);
     WCTB_CHECK_LAUNCH("k_swap_tap_norms");
-    k_swap_patch_weights<<<swap_grid((long long)patch * patch * C * S.cout_pad, 256), 256, 0, st>>>(ws_feat, gs, q, norms, S.n_patches,
-                                                                                                  S.cout_pad, wsplit);
+    k_swap_patch_weights<<<swap_grid((long long)patch * patch * C * SL.cout_pad, 256), 256, 0, st>>>(feat, gs, q, norms, SL.n_patches,
+                                                                                                   SL.cout_pad, wsplit);
     WCTB_CHECK_LAUNCH("k_swap_patch_weights");
-    // every style patch is a filter: the P x P correlation (top-left anchored, all positions; the strided VALID subset is
-    // read by the arg-max) runs on the tensor-core conv kernel
-    rc = launch_conv_tc(CONV_TAPS, wc_feat, 1, Hc, Wc, C, wsplit, 1, nullptr, nullptr, S.cout_pad, 0, scores, st, patch);
-    if (rc) return rc;
-    const int npos = S.ho * S.wo;
-    k_swap_argmax<<<(unsigned)cdiv((long long)npos * 32, 256), 256, 0, st>>>(scores, ActGeom(1, Hc, Wc, S.cout_pad), q, S.n_patches, idx);
-    WCTB_CHECK_LAUNCH("k_swap_argmax");
-    k_swap_gather<<<swap_grid((long long)Hc * Wc * (C / 8), 256), 256, 0, st>>>(ws_feat, gs, q, idx, gc, ss_feat);
-    WCTB_CHECK_LAUNCH("k_swap_gather");
-    rc = launch_conv_tc(CONV_APPLY, ss_feat, 1, Hc, Wc, C, msplit + 4 * CC, 1, nullptr, bias3 + 2 * C, C, 0, tmp, st);
-    if (rc) return rc;
-    k_blend2<<<swap_grid((long long)Hc * Wc * (C / 8), 256), 256, 0, st>>>(tmp, content, gc, alpha, 1.f - alpha, out);   // ops.py:210
-    WCTB_CHECK_LAUNCH("k_blend2");
-    if (k_out) WCTB_CUDA(cudaMemcpyAsync(k_out, kc, 2 * 4, cudaMemcpyDeviceToDevice, st));
+    if (k_out) WCTB_CUDA(cudaMemcpyAsync(k_out, ks, 4, cudaMemcpyDeviceToDevice, st));
     return 0;
+}
+
+// Content side over Nc frames against one prepared style: whiten every frame with its own W_c (ops.py:187), correlate all
+// frames with the shared patch filters in one launch, arg-max and gather per frame, colour with the style, blend.
+int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
+                            int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
+                            cudaStream_t st) {
+    int rc = swap_check_style(C, Hs, Ws, patch, stride);
+    if (rc) return rc;
+    WCTB_REQUIRE(Nc >= 1 && Hc >= patch && Wc >= patch && Hc >= 2 && Wc >= 2,
+                 "style_swap_apply: %d content maps of %dx%d (patch %d)", Nc, Hc, Wc, patch);
+    const SwapState SL = swap_state_layout(C, Hs, Ws, patch, stride);
+    const SwapApplyWs AL = swap_apply_layout(C, Nc, Hc, Wc, patch, stride, SL.cout_pad);
+    // the swapped encoding must have the content's size (ops.py:199 reshapes it to [Hc*Wc, C]); wct.py:84-90 crops the content
+    // image beforehand when the stride makes the filter not fit (utils.swap_filter_fit)
+    WCTB_REQUIRE((AL.ho - 1) * stride + patch == Hc && (AL.wo - 1) * stride + patch == Wc,
+                 "style_swap: patch %d / stride %d does not tile a %dx%d encoding (refit the content: swap_filter_fit, wct.py:84-90)",
+                 patch, stride, Hc, Wc);
+    if (ws_bytes < AL.total) {
+        set_error("style_swap_apply: workspace %zu < %zu bytes", ws_bytes, AL.total);
+        return WCTB200_EWS;
+    }
+    const SwapGeom q = {patch, stride, SL.prow, SL.pcol, AL.ho, AL.wo};
+    uint8_t* sw = static_cast<uint8_t*>(ws);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    const WctWs L = wct_layout(C, Nc, 0);
+    uint8_t* w = sw + AL.base;
+    double* dsum = reinterpret_cast<double*>(w + L.dsum);
+    float* mean = reinterpret_cast<float*>(w + L.mean);
+    float* G = reinterpret_cast<float*>(w + L.G);
+    float* A0 = reinterpret_cast<float*>(w + L.A0);
+    float* lam = reinterpret_cast<float*>(w + L.lam);
+    float* sigma = reinterpret_cast<float*>(w + L.sigma);
+    float* dvec = reinterpret_cast<float*>(w + L.dvec);
+    float* Wcm = reinterpret_cast<float*>(w + L.Wc);
+    __half* msplit = reinterpret_cast<__half*>(w + L.Msplit);
+    float* bias = reinterpret_cast<float*>(w + L.bias);
+    float* conv = reinterpret_cast<float*>(w + L.conv);
+    int* kc = reinterpret_cast<int*>(w + L.kcount);
+    float* zeros = reinterpret_cast<float*>(sw + AL.zeros);
+    int* idx = reinterpret_cast<int*>(sw + AL.idx);
+    __half* wc_feat = reinterpret_cast<__half*>(sw + AL.wc_feat);
+    __half* ss_feat = reinterpret_cast<__half*>(sw + AL.ss_feat);
+    __half* tmp = reinterpret_cast<__half*>(sw + AL.tmp);
+    __half* scores = reinterpret_cast<__half*>(sw + AL.scores);
+    const long long CC = (long long)C * C;
+
+    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)Nc * 2 * 4, st));
+    WCTB_CUDA(cudaMemsetAsync(zeros, 0, (size_t)C * 4, st));
+    ActGeom gc(Nc, Hc, Wc, C), gs(1, Hs, Ws, C);
+    rc = launch_mean_cov(content, gc, eps_cov, mean, G, A0, dsum, st);
+    if (rc) return rc;
+    rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, nullptr);
+    if (rc) return rc;
+    rc = launch_eig_post(G, A0, lam, C, Nc, thresh, 0.f, Nc, sigma, dvec, kc, st);             // S^-1/2 per frame (ops.py:187)
+    if (rc) return rc;
+    k_outer_gemm<<<dim3((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc), 256, 0, st>>>(G, CC, G, CC, dvec, C, Wcm, CC, C);   // W_c
+    WCTB_CHECK_LAUNCH("k_outer_gemm(whiten)");
+    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), (unsigned)Nc), 256, 0, st>>>(Wcm, C, Nc, 1, 1.f, 0, mean, zeros, msplit, bias);
+    WCTB_CHECK_LAUNCH("k_finalize_transform(whiten)");
+    rc = launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, msplit, Nc, nullptr, bias, C, 0, wc_feat, st);
+    if (rc) return rc;
+    // every style patch is a filter: the P x P correlation of all frames (top-left anchored, all positions; the strided VALID
+    // subset is read by the arg-max) runs on the tensor-core conv kernel
+    rc = launch_conv_tc(CONV_TAPS, wc_feat, Nc, Hc, Wc, C, reinterpret_cast<const __half*>(sp + SL.wsplit), 1, nullptr, nullptr,
+                        SL.cout_pad, 0, scores, st, patch);
+    if (rc) return rc;
+    const int npos = AL.ho * AL.wo;
+    k_swap_argmax<<<dim3((unsigned)cdiv((long long)npos * 32, 256), (unsigned)Nc), 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, SL.cout_pad),
+                                                                                                q, SL.n_patches, idx);
+    WCTB_CHECK_LAUNCH("k_swap_argmax");
+    k_swap_gather<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(reinterpret_cast<const __half*>(sp + SL.feat), gs, q,
+                                                                                     idx, gc, ss_feat);
+    WCTB_CHECK_LAUNCH("k_swap_gather");
+    rc = launch_conv_tc(CONV_APPLY, ss_feat, Nc, Hc, Wc, C, reinterpret_cast<const __half*>(sp + SL.cmsplit), 1, nullptr,
+                        reinterpret_cast<const float*>(sp + SL.cbias), C, 0, tmp, st);
+    if (rc) return rc;
+    k_blend2<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(tmp, content, gc, alpha, 1.f - alpha, out);   // ops.py:210
+    WCTB_CHECK_LAUNCH("k_blend2");
+    if (k_out) {
+        // k_out: [k_c x Nc | k_s]
+        WCTB_CUDA(cudaMemcpyAsync(k_out, kc, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(k_out + Nc, sp + SL.k, 4, cudaMemcpyDeviceToDevice, st));
+    }
+    return 0;
+}
+
+int launch_style_swap_level(const __half* content, int Hc, int Wc, const __half* style, int Hs, int Ws, int C, int patch, int stride,
+                            float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
+                            cudaStream_t st) {
+    int rc = swap_check_style(C, Hs, Ws, patch, stride);
+    if (rc) return rc;
+    WCTB_REQUIRE(Hc >= patch && Wc >= patch && Hc >= 2 && Wc >= 2,
+                 "style_swap: maps must be at least %dx%d (content %dx%d, style %dx%d)", patch, patch, Hc, Wc, Hs, Ws);
+    WCTB_REQUIRE(((Hc - patch) / stride) * stride + patch == Hc && ((Wc - patch) / stride) * stride + patch == Wc,
+                 "style_swap: patch %d / stride %d does not tile a %dx%d encoding (refit the content: swap_filter_fit, wct.py:84-90)",
+                 patch, stride, Hc, Wc);
+    const size_t need = style_swap_workspace_bytes(C, Hc, Wc, Hs, Ws, patch, stride);
+    if (ws_bytes < need) {
+        set_error("style_swap: workspace %zu < %zu bytes", ws_bytes, need);
+        return WCTB200_EWS;
+    }
+    const size_t sbytes = style_swap_state_bytes(C, Hs, Ws, patch, stride);
+    uint8_t* state = static_cast<uint8_t*>(ws);
+    rc = launch_style_swap_prepare(style, Hs, Ws, C, patch, stride, eps_cov, thresh, state, nullptr, state + sbytes, ws_bytes - sbytes,
+                                   st);
+    if (rc) return rc;
+    return launch_style_swap_apply(content, 1, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, out, k_out,
+                                   state + sbytes, ws_bytes - sbytes, st);
 }
 
 }  // namespace wctb

@@ -11,6 +11,8 @@ import torch
 
 from . import _capi
 from .model import WCTModel, RELU_CHANNELS
+from .prepared import (PreparedStyle, SEMANTIC_KEYS, encoder_fingerprints, slice_act_planes, slice_adain_state,
+                       slice_wct_state)
 
 # wct_tf (ops.py:24-90, what the graph executes) vs wct_np (ops.py:92-140, the named oracle)
 SEMANTICS = {
@@ -54,6 +56,8 @@ class Engine(object):
         self.launches = 0          # kernels launched through the C-ABI (bench.py "gpu_launches")
         self.profile = None        # optional dict: key -> [torch.cuda.Event pairs, flops, bytes]
         self._tag = None           # profiling only: "style" / relu target of the level being enqueued
+        self._vgg_layers = weights["vgg"]          # encoder fingerprints of prepared styles (computed on first use)
+        self._fingerprints = None
         with torch.cuda.device(self.device):
             self._upload(weights)
 
@@ -271,6 +275,68 @@ class Engine(object):
                    bytes_=4.0 * C * (2 * content.N * hwc + style.N * hws))
         return out, kbuf
 
+    def adain_prepare(self, style):
+        """Style side of AdaIN on one level: the per-channel moments of the style, a state read by ``adain_apply``."""
+        state = torch.empty(self.lib.wctb200_adain_style_state_bytes(style.C, style.N), dtype=torch.uint8, device=self.device)
+        self._call("adain_style[C%d]" % style.C, 3, self.lib.wctb200_adain_style_prepare, style.ptr, style.N, style.H, style.W, style.C,
+                   state.data_ptr(), self._stream(), bytes_=4.0 * style.C * style.N * style.H * style.W)
+        return state
+
+    def adain_apply(self, content, state, n_style, alpha):
+        st = self._stream()
+        out = self._act(content.N, content.H, content.W, content.C)
+        ws = self._workspace(content.C, content.N, 0)
+        self._call("adain_level[C%d]" % content.C, 5, self.lib.wctb200_adain_apply, content.ptr, content.N, content.H, content.W,
+                   content.C, state.data_ptr(), n_style, float(alpha), 1e-5, out.ptr, ws.data_ptr(), ws.numel(), st,
+                   bytes_=4.0 * content.C * 2 * content.N * content.H * content.W)
+        return out, None
+
+    def adain_apply_blend(self, content, states, weights, alpha):
+        """AdaIN against the blend of K prepared styles (``adain_prepare`` states, one style each) with the weights of
+        ``weights`` (cuda fp32 [1|N, K])."""
+        st = self._stream()
+        C, N, K, Nw = content.C, content.N, len(states), weights.shape[0]
+        out = self._act(N, content.H, content.W, C)
+        ws = self._workspace(C, N, 0)
+        self._call("adain_blend[C%d]" % C, 5, self.lib.wctb200_adain_apply_blend, content.ptr, N, content.H, content.W, C,
+                   _capi.pointer_array([s.data_ptr() for s in states]), K, weights.data_ptr(), Nw, float(alpha), 1e-5, out.ptr,
+                   ws.data_ptr(), ws.numel(), st, bytes_=4.0 * C * 2 * N * content.H * content.W)
+        return out, None
+
+    def swap_prepare(self, style, patch, stride):
+        """Style side of the style swap (whitened style, patch filters, colouring operand) for one style feature."""
+        st = self._stream()
+        C = style.C
+        nbytes = self.lib.wctb200_style_swap_state_bytes(C, style.H, style.W, int(patch), int(stride))
+        if nbytes == 0:
+            raise ValueError("style swap needs a style encoding of at least %dx%d (style %dx%d)" % (patch, patch, style.H, style.W))
+        state = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = torch.empty(self.lib.wctb200_style_swap_prepare_workspace_bytes(C, style.H, style.W, int(patch), int(stride)),
+                         dtype=torch.uint8, device=self.device)
+        sem = SEMANTICS["tf"]                  # the reference only has the TF graph version of this op
+        self._call("swap_style[C%d]" % C, 12, self.lib.wctb200_style_swap_prepare, style.ptr, style.H, style.W, C, int(patch),
+                   int(stride), sem["eps_cov"], sem["thresh"], state.data_ptr(), None, ws.data_ptr(), ws.numel(), st)
+        return state
+
+    def swap_apply(self, content, state, style_hw, ss_alpha, want_info=False, patch=3, stride=1):
+        """wct_style_swap (ops.py:145-217) of the N content frames against one prepared style (``swap_prepare``)."""
+        st = self._stream()
+        C, N = content.C, content.N
+        Hs, Ws = style_hw
+        out = self._act(N, content.H, content.W, C)
+        nbytes = self.lib.wctb200_style_swap_apply_workspace_bytes(C, N, content.H, content.W, Hs, Ws, int(patch), int(stride))
+        if nbytes == 0:
+            raise ValueError("style swap needs encodings of at least %dx%d (content %dx%d, style %dx%d)"
+                             % (patch, patch, content.H, content.W, Hs, Ws))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        kbuf = torch.empty(N + 1, dtype=torch.int32, device=self.device) if want_info else None
+        sem = SEMANTICS["tf"]
+        self._call("style_swap[C%d]" % C, 11, self.lib.wctb200_style_swap_apply, content.ptr, N, content.H, content.W, C,
+                   state.data_ptr(), Hs, Ws, int(patch), int(stride), float(ss_alpha), sem["eps_cov"], sem["thresh"], out.ptr,
+                   kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel(), st)
+        ws.record_stream(torch.cuda.current_stream(self.device))   # freed by the caching allocator only after this stream is done
+        return out, kbuf
+
     def style_swap(self, content, style, ss_alpha, want_info=False, patch=3, stride=1):
         """wct_style_swap (ops.py:145-217) on one content/style pair with ``patch`` x ``patch`` windows every ``stride``."""
         assert content.N == 1 and style.N == 1, "style swap works on one content/style pair (ops.py:146)"
@@ -384,9 +450,13 @@ class Engine(object):
     # ------------------------------------------------------------------ pipeline
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None):
-        """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3], Ns in {1, N}.
-        Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
+        """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
+        {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
+
+        Every call runs the style side once -- the encode of the style and its per-level states (``_style_side``) -- and
+        then applies it; a ``PreparedStyle`` skips the first step.  A shared style swap (``swap5``) swaps the N frames in
+        one batched call per sub-batch; with one style per frame the frames run one by one.
 
         With ``self.groups`` = G > 1 the batch is cut into G sub-batches whose level chains are
         enqueued on G independent stream pairs: frames are independent (wct.py:97-103), and the
@@ -394,15 +464,15 @@ class Engine(object):
         other groups' convolutions (same arithmetic per frame; only the schedule changes).
 
         Spatial control: ``labels`` is a cuda uint8 label map [N|1,Hm,Wm] of any resolution and ``region_styles`` a list of
-        R (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes; ``style_u8`` is ignored.  At every level the map is resampled
-        to the feature grid and region r of a frame is transformed against style r (WCT only); labels >= R keep the
-        content feature.  The R styles are encoded and prepared once per call.
+        R (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes, or prepared styles of one style each; ``style_u8`` is ignored.
+        At every level the map is resampled to the feature grid and region r of a frame is transformed against style r
+        (WCT only); labels >= R keep the content feature.  The R styles are encoded and prepared once per call.
 
-        Style interpolation: ``interp_styles`` is a list of K (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes and
-        ``interp_weights`` a cuda float32 [1|N, K] tensor; ``style_u8`` is ignored.  Frame n is stylised with the blend of
-        the K styles under weight row n (one row: every frame), which for a row that sums to 1 is the same blend of the K
-        single-style outputs at every level (WCT and AdaIN are affine in the style statistics).  The weights are used as
-        given.  The K styles are encoded (and, for WCT, prepared) once per call."""
+        Style interpolation: ``interp_styles`` is a list of K (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes, or prepared
+        styles of one style each, and ``interp_weights`` a cuda float32 [1|N, K] tensor; ``style_u8`` is ignored.  Frame n is
+        stylised with the blend of the K styles under weight row n (one row: every frame), which for a row that sums to 1 is
+        the same blend of the K single-style outputs at every level (WCT and AdaIN are affine in the style statistics).  The
+        weights are used as given.  The K styles are encoded and prepared once per call."""
         N = content_u8.shape[0]
         if interp_styles is not None:
             if labels is not None or swap5:
@@ -431,32 +501,50 @@ class Engine(object):
             return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
                                        lambda lo, hi: ("regions", labels[lo:hi]))
         swap5 = bool(swap5) and "relu5_1" in [l.relu_target for l in self.model.levels]    # model.py:148: only relu5_1 swaps
-        if swap5:
-            if N != 1 or style_u8.shape[0] != 1:
-                raise ValueError("swap5 works on one content/style pair per call (ops.py:146)")
-            return self._stylize_one(content_u8, style_u8, alpha, adain, want_info, capture, True, ss_alpha,
-                                     ss_patch=ss_patch_size, ss_stride=ss_stride)
+        prepared = isinstance(style_u8, PreparedStyle)
+        n_style = style_u8.n if prepared else style_u8.shape[0]
+        if n_style not in (1, N):
+            raise ValueError("%d styles for %d frames: give one style, or one per frame" % (n_style, N))
+        if prepared:
+            self.check_prepared(style_u8, adain, swap5)
+        main = torch.cuda.current_stream(self.device)
+        if swap5 and n_style > 1:
+            # one style per frame: frame by frame (each frame's swap has its own style side)
+            outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
+                                 alpha=alpha, adain=adain, want_info=want_info, swap5=True, ss_alpha=ss_alpha,
+                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride) for i in range(N)]
+            return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
+        swap = (int(ss_patch_size), int(ss_stride)) if swap5 else None
+        shared = style_u8 if (prepared and n_style == 1) else None
+        owned = None
+        if n_style == 1 and not prepared and (G > 1 or swap5):
+            # ONE style for the whole batch (video, configs[2]): its encoder pass and per-level states are made once, every
+            # sub-batch group waits for the per-level events
+            self._group = 1 if G > 1 else 0
+            try:
+                owned = shared = self._style_side(style_u8, main, wct=not adain, adain=adain, keep5=swap5,
+                                                  skip=("relu5_1",) if swap5 else ())
+            finally:
+                self._group = 0
+        if swap is not None:
+            self.swap_state(shared, *swap)
         if G > 1:
-            main = torch.cuda.current_stream(self.device)
-            shared = None
-            if style_u8.shape[0] == 1 and not adain:
-                # ONE style for the whole batch (video, configs[2]): its encoder pass and eigendecompositions run once,
-                # every sub-batch group waits for the per-level events
-                self._group = 1
-                try:
-                    shared = self._style_side(style_u8, True, main)
-                finally:
-                    self._group = 0
-
             def run(lo, hi):
-                sg = style_u8 if style_u8.shape[0] == 1 else style_u8[lo:hi]
-                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, shared_style=shared)
+                if shared is not None:
+                    sg = shared
+                else:
+                    sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
+                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha)
             out = self._in_groups(N, G, main, run)
-            if shared is not None and shared["side"] is not main:
-                shared["side"].wait_stream(main)    # the shared style states are recycled only after every group used them
-            return out
-        return self._stylize_one(content_u8, style_u8, alpha, adain, want_info, capture)
+        else:
+            out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
+                                    swap=swap, ss_alpha=ss_alpha)
+        if owned is not None and owned.side is not main:
+            owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
+            if G == 1:
+                main.wait_stream(owned.side)
+        return out
 
     def _in_groups(self, N, G, main, run):
         """Cut a batch of N frames into G sub-batches and enqueue ``run(lo, hi)`` for each on its own stream (group g + 1
@@ -486,16 +574,25 @@ class Engine(object):
         return out
 
     def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame):
-        """``stylize`` with several style images (spatial control, style interpolation): their style sides run once per
-        call and are shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the label
-        maps or weight rows)."""
+        """``stylize`` with several styles (spatial control, style interpolation): images are prepared once per call, and
+        every style side is shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the
+        label maps or weight rows)."""
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
-        split = not adain                      # AdaIN keeps its style features inline
         self._group = 1 if G > 1 else 0
+        owned = []
         try:
-            sides = [self._style_side(s, split, main) for s in styles]
+            sides = []
+            for s in styles:
+                if isinstance(s, PreparedStyle):
+                    if s.n != 1:
+                        raise ValueError("each region / interpolated style must be one style, got a prepared style of %d" % s.n)
+                    self.check_prepared(s, adain, False)
+                    sides.append(s)
+                else:
+                    owned.append(self._style_side(s, main, wct=not adain, adain=adain))
+                    sides.append(owned[-1])
         finally:
             self._group = 0
         if G == 1:
@@ -503,85 +600,182 @@ class Engine(object):
         else:
             out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, adain, False, None,
                                                                                multi=per_frame(lo, hi) + (sides,)))
-        for side in {id(sd["side"]): sd["side"] for sd in sides}.values():
+        for side in {id(sd.side): sd.side for sd in owned}.values():
             if side is not main:
                 side.wait_stream(main)         # the style states are recycled only after every level used them
                 main.wait_stream(side)
         return out
 
-    def _style_side(self, style_u8, split, main):
-        """Style side of one call (model.py:70-72: ONE encoder pass emitting every target; ops.py:48-55,76 per level when
-        ``split``): enqueued on this group's style stream when overlap is on.  Returns the states / events / features."""
+    def _style_stream(self):
+        """This group's style stream (the style side overlaps the content work), or None without overlap."""
+        if not self.overlap_style:
+            return None
+        if self._group not in self._style_streams:
+            prio = -1 if (self.group_priorities and self._group <= 1) else 0
+            self._style_streams[self._group] = torch.cuda.Stream(device=self.device, priority=prio)
+        return self._style_streams[self._group]
+
+    def _style_side(self, style_u8, main, wct=True, adain=False, keep5=False, skip=()):
+        """The prepare step: style side of one call (model.py:70-72: ONE encoder pass emitting every target; per level the
+        WCT state of ops.py:48-55,76 when ``wct``, the AdaIN moments when ``adain``; levels in ``skip`` get neither), enqueued
+        on this group's style stream when overlap is on.  ``keep5`` keeps the relu5_1 feature (the style swap).  Returns a
+        ``PreparedStyle`` with one event per level."""
         lib = self.lib
-        side = main
-        if split and self.overlap_style:
-            if self._group not in self._style_streams:
-                prio = -1 if (self.group_priorities and self._group <= 1) else 0
-                self._style_streams[self._group] = torch.cuda.Stream(device=self.device, priority=prio)
-            side = self._style_streams[self._group]
+        side = self._style_stream() or main
+        if side is not main:
             side.wait_stream(main)             # style_u8 (and last step's buffers) are ready
-        states, events, feats = {}, {}, None
+        sem = SEMANTICS[self.semantics]
+        taps = list(dict.fromkeys(self.model.style_taps))
+        ps = PreparedStyle(style_u8.shape[0], {k: sem[k] for k in SEMANTIC_KEYS}, taps)
+        ps.side = side
         with torch.cuda.stream(side):
             tag, self._tag = self._tag, "style"
             style = torch.empty(style_u8.shape, dtype=torch.float32, device=self.device)
             self._call("u8_to_f32", 1, lib.wctb200_image_u8_to_f32, style_u8.data_ptr(), style_u8.numel(), style.data_ptr(),
                        self._stream())
             _, feats = self.encode(style, self.model.deepest_target, taps=self.model.style_taps)
-            if split:
-                for relu in self.model.style_taps:
-                    if relu not in states:
-                        states[relu] = self.style_prepare(feats[relu])
-                        ev = torch.cuda.Event()
-                        ev.record(side)
-                        events[relu] = ev
+            for relu in taps:
+                if relu not in skip:
+                    if wct:
+                        ps.wct[relu] = self.style_prepare(feats[relu])
+                    if adain:
+                        ps.adain[relu] = self.adain_prepare(feats[relu])
+                ev = torch.cuda.Event()
+                ev.record(side)
+                ps.events[relu] = ev
+            if keep5 and "relu5_1" in feats:
+                ps.feat5 = feats["relu5_1"]
             self._tag = tag
-        return dict(states=states, events=events, feats=feats, side=side)
+        return ps
 
-    def _stylize_one(self, content_u8, style_u8, alpha, adain, want_info, capture, swap5=False, ss_alpha=0.6, shared_style=None,
-                     ss_patch=3, ss_stride=1, multi=None):
+    def prepare(self, style_u8):
+        """Every part of the style side of ``style_u8`` (cuda uint8 [n,Hs,Ws,3]): WCT states and AdaIN moments of every
+        target, and the relu5_1 feature when relu5_1 is a target."""
+        main = torch.cuda.current_stream(self.device)
+        ps = self._style_side(style_u8, main, wct=True, adain=True, keep5=True)
+        style_u8.record_stream(ps.side)        # read on the style stream after the caller may have dropped it
+        ps.record_stream(main)
+        return ps
+
+    def prepare_call(self, style_u8, adain=False, swap5=False):
+        """The style side one call needs (WCT states, or the AdaIN moments; the relu5_1 feature for ``swap5``), made once
+        for a call that applies it several times (passes)."""
+        main = torch.cuda.current_stream(self.device)
+        ps = self._style_side(style_u8, main, wct=not adain, adain=adain, keep5=swap5)
+        style_u8.record_stream(ps.side)
+        return ps
+
+    def check_prepared(self, ps, adain, swap5):
+        """ValueError unless ``ps`` was prepared for this engine's encoder and semantics and covers its targets."""
+        sem = SEMANTICS[self.semantics]
+        for k in SEMANTIC_KEYS:
+            if float(ps.semantics[k]) != float(sem[k]):
+                raise ValueError("the prepared style was made with %s = %s, this model uses %s" % (k, ps.semantics[k], sem[k]))
+        need = dict.fromkeys(self.model.style_taps)
+        have = ps.adain if adain else ps.wct
+        for relu in need:
+            if relu not in have and not (swap5 and relu == "relu5_1"):
+                raise ValueError("the prepared style has no %s state for %s" % ("AdaIN" if adain else "WCT", relu))
+        if swap5 and ps.feat5 is None:
+            raise ValueError("the prepared style has no relu5_1 feature for the style swap")
+        if ps.fingerprints:
+            mine = self.fingerprints()
+            for relu in need:
+                if ps.fingerprints.get(relu) != mine[relu]:
+                    raise ValueError("the prepared style was made with other encoder weights up to %s" % relu)
+
+    def fingerprints(self):
+        """Encoder fingerprint per target (prepared.encoder_fingerprints), computed once."""
+        if self._fingerprints is None:
+            self._fingerprints = encoder_fingerprints(self._vgg_layers, self.model.style_taps)
+        return self._fingerprints
+
+    def slice_prepared(self, ps, lo, hi):
+        """Styles lo..hi-1 of a prepared style as a prepared style of their own (exact device copies on the current
+        stream, which first waits for the prepare)."""
+        cur = torch.cuda.current_stream(self.device)
+        if ps.side is not cur:
+            ps.wait(cur)
+        out = PreparedStyle(hi - lo, ps.semantics, ps.targets)
+        out.side = cur
+        out.fingerprints = ps.fingerprints
+        for relu, st in ps.wct.items():
+            out.wct[relu] = slice_wct_state(self.lib, st, RELU_CHANNELS[relu], ps.n, lo, hi)
+        for relu, st in ps.adain.items():
+            out.adain[relu] = slice_adain_state(self.lib, st, RELU_CHANNELS[relu], ps.n, lo, hi)
+        if ps.feat5 is not None:
+            f = ps.feat5
+            out.feat5 = self._act(hi - lo, f.H, f.W, f.C)
+            slice_act_planes(f.buf, f.N, f.H, f.W, f.C, lo, hi, out.feat5.buf)
+        ps.record_stream(cur)
+        return out
+
+    def swap_state(self, ps, patch, stride):
+        """The style-swap state of a prepared style of one style for (patch, stride): made on first use from its relu5_1
+        feature (on its style stream when it has one) and cached in it.  Returns (state, event)."""
+        key = (int(patch), int(stride))
+        if key not in ps.swap:
+            main = torch.cuda.current_stream(self.device)
+            st = ps.side if ps.side is not None else main
+            if st is not main:
+                st.wait_stream(main)
+            with torch.cuda.stream(st):
+                ps.wait(st, "relu5_1")
+                tag, self._tag = self._tag, "style"
+                state = self.swap_prepare(ps.feat5, *key)
+                self._tag = tag
+                ps.feat5.buf.record_stream(st)
+                ev = torch.cuda.Event()
+                ev.record(st)
+            ps.swap[key] = (state, ev)
+        return ps.swap[key]
+
+    def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None):
+        """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
+        ``swap``: (patch, stride) of the style swap at relu5_1 (its state is made by ``swap_state`` beforehand)."""
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
+        owned = None
         if multi is None:
-            assert content_u8.dtype == torch.uint8 and style_u8.dtype == torch.uint8
-            assert style_u8.shape[0] in (1, N)
+            assert content_u8.dtype == torch.uint8
+            if not isinstance(style, PreparedStyle):
+                assert style.dtype == torch.uint8 and style.shape[0] in (1, N)
+                owned = style = self._style_side(style, main, wct=not adain, adain=adain)
+            n_style = style.n
+            sides = [style]
         content = torch.empty(content_u8.shape, dtype=torch.float32, device=self.device)
         self._call("u8_to_f32", 1, lib.wctb200_image_u8_to_f32, content_u8.data_ptr(), content_u8.numel(), content.data_ptr(), st)
-        split = not adain and not swap5        # WCT: style side on its own stream; AdaIN / style swap: keep it inline
         if multi is not None:
             # ("regions", labels [N,Hm,Wm], R style sides) or ("interp", weight rows [1|N,K], K style sides): _stylize_multi
             mode, per_frame, sides = multi
-            ss = sides[0]
-            n_style = 1
-        else:
-            ss = shared_style if (shared_style is not None and split) else self._style_side(style_u8, split, main)
-            n_style = style_u8.shape[0]
-        side, style_states, style_events, style_feats = ss["side"], ss["states"], ss["events"], ss["feats"]
         infos = []
         x = content
         nlev = len(self.model.levels)
         for lvl in self.model.levels:
-            self._tag = lvl.relu_target
-            cf, _ = self.encode(x, lvl.relu_target)
-            if multi is not None:
-                for sd in sides:
-                    if split and sd["side"] is not main:     # AdaIN: the style features were encoded inline, before the groups
-                        main.wait_event(sd["events"][lvl.relu_target])
-                if mode == "regions":
-                    lab = self.labels_resize(per_frame, cf.H, cf.W)
-                    f, kbuf = self.wct_apply_regions(cf, lab, [sd["states"][lvl.relu_target] for sd in sides], alpha, want_info)
-                elif adain:
-                    f, kbuf = self.adain_blend(cf, [sd["feats"][lvl.relu_target] for sd in sides], per_frame, alpha)
-                else:
-                    f, kbuf = self.wct_apply_blend(cf, [sd["states"][lvl.relu_target] for sd in sides], per_frame, alpha, want_info)
-            elif swap5 and lvl.relu_target == "relu5_1":     # model.py:148-152: style swap wins over AdaIN / WCT at relu5_1
-                f, kbuf = self.style_swap(cf, style_feats[lvl.relu_target], ss_alpha, want_info, ss_patch, ss_stride)
-            elif split:
-                if side is not main:
-                    main.wait_event(style_events[lvl.relu_target])
-                f, kbuf = self.wct_apply(cf, style_states[lvl.relu_target], n_style, alpha, want_info)
+            relu = lvl.relu_target
+            self._tag = relu
+            cf, _ = self.encode(x, relu)
+            if swap is not None and relu == "relu5_1":      # model.py:148-152: style swap wins over AdaIN / WCT at relu5_1
+                state, ev = style.swap[swap]
+                main.wait_event(ev)
+                f, kbuf = self.swap_apply(cf, state, (style.feat5.H, style.feat5.W), ss_alpha, want_info, *swap)
             else:
-                f, kbuf = self.transform(cf, style_feats[lvl.relu_target], alpha, adain, want_info)
+                for sd in sides:
+                    if sd.side is not main:
+                        sd.wait(main, relu)
+                if multi is None:
+                    if adain:
+                        f, kbuf = self.adain_apply(cf, style.adain[relu], n_style, alpha)
+                    else:
+                        f, kbuf = self.wct_apply(cf, style.wct[relu], n_style, alpha, want_info)
+                elif mode == "regions":
+                    lab = self.labels_resize(per_frame, cf.H, cf.W)
+                    f, kbuf = self.wct_apply_regions(cf, lab, [sd.wct[relu] for sd in sides], alpha, want_info)
+                elif adain:
+                    f, kbuf = self.adain_apply_blend(cf, [sd.adain[relu] for sd in sides], per_frame, alpha)
+                else:
+                    f, kbuf = self.wct_apply_blend(cf, [sd.wct[relu] for sd in sides], per_frame, alpha, want_info)
             infos.append(kbuf)
             if capture is not None:
                 capture.setdefault("level_input", []).append(x)
@@ -592,9 +786,12 @@ class Engine(object):
             if capture is not None:
                 capture.setdefault("level_output", []).append(x)
         self._tag = None
-        if side is not main and shared_style is None and multi is None:
-            side.wait_stream(main)             # buffers handed across streams may be recycled only after both are done
-            main.wait_stream(side)
+        for sd in sides:
+            if sd is not owned:
+                sd.record_stream(main)         # a prepared style held by the caller may be dropped while this work is queued
+        if owned is not None and owned.side is not main:
+            owned.side.wait_stream(main)       # buffers handed across streams may be recycled only after both are done
+            main.wait_stream(owned.side)
         if want_info:
             self.last_info = infos
         return x

@@ -12,7 +12,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``content_mask`` is new: spatial control (WCT paper, section 4), a label map whose region r takes style r;
   * ``style_weights`` is new: style interpolation (WCT paper, section 4), a weighted blend of 1..8 styles, shared by
     every frame or one row per frame;
-  * ``synthesize`` is new: texture synthesis (WCT paper, section 4), the pipeline run on seeded noise made on the device.
+  * ``synthesize`` is new: texture synthesis (WCT paper, section 4), the pipeline run on seeded noise made on the device;
+  * ``prepare_style`` / ``load_style`` are new: the style side computed once (or read from a ``.wctstyle`` file) and
+    accepted wherever a style image is (wct_tf_b200/prepared.py).
 """
 from __future__ import annotations
 
@@ -22,7 +24,26 @@ import time
 import numpy as np
 import torch
 
-from .engine import Engine
+from .engine import Engine, SEMANTICS
+from .prepared import PreparedStyle
+
+
+def _to_dev(a, dev):
+    """uint8 image(s) [H,W,3] or [n,H,W,3], numpy or torch, host or device -> contiguous cuda uint8 [n,H,W,3]."""
+    if isinstance(a, np.ndarray):
+        a = torch.from_numpy(np.array(a, copy=True, order="C"))    # own, writable, contiguous
+    if a.dim() == 3:
+        a = a.unsqueeze(0)
+    if a.dtype != torch.uint8:
+        a = a.clamp(0, 255).to(torch.uint8)   # the reference feeds arrays "in [0,255]" (wct.py:74)
+    return a.to(dev, non_blocking=True).contiguous()
+
+
+def _style_list(styles):
+    """The styles of a mask / interpolation call as a list (one image or one prepared style stands for a list of one)."""
+    if isinstance(styles, PreparedStyle) or (isinstance(styles, (np.ndarray, torch.Tensor)) and styles.ndim == 3):
+        return [styles]
+    return list(styles)
 
 
 def _torch_device(device):
@@ -81,12 +102,14 @@ class WCT(object):
             m = m.unsqueeze(0)
         if m.dim() != 3 or m.shape[0] not in (1, n_frames) or m.shape[1] < 1 or m.shape[2] < 1:
             raise ValueError("content_mask must be [Hm,Wm] or [N,Hm,Wm] with N = %d frames, got %s" % (n_frames, tuple(m.shape)))
-        if isinstance(styles, (np.ndarray, torch.Tensor)) and styles.ndim == 3:
-            styles = [styles]
-        styles = list(styles)
+        styles = _style_list(styles)
         if not 1 <= len(styles) <= 8:
             raise ValueError("a content mask needs 1..8 region styles, got %d" % len(styles))
         for s in styles:
+            if isinstance(s, PreparedStyle):
+                if s.n != 1:
+                    raise ValueError("each region style must be one style, got a prepared style of %d" % s.n)
+                continue
             if s.dtype not in (np.uint8, torch.uint8) or s.ndim not in (3, 4) or s.shape[-1] != 3 or (s.ndim == 4 and s.shape[0] != 1):
                 raise ValueError("each region style must be one uint8 [Hs,Ws,3] image")
         return m.contiguous(), styles
@@ -116,12 +139,14 @@ class WCT(object):
     def check_interp(style_weights, n_frames, styles):
         """Host-side validation of an interpolation call: a list of 1..8 uint8 [Hs,Ws,3] style images (any sizes) and their
         weights (``normalize_weights``).  Returns (float32 weights [1|N, K], styles)."""
-        if isinstance(styles, (np.ndarray, torch.Tensor)) and styles.ndim == 3:
-            styles = [styles]
-        styles = list(styles)
+        styles = _style_list(styles)
         if not 1 <= len(styles) <= 8:
             raise ValueError("style interpolation needs 1..8 styles, got %d" % len(styles))
         for s in styles:
+            if isinstance(s, PreparedStyle):
+                if s.n != 1:
+                    raise ValueError("each interpolated style must be one style, got a prepared style of %d" % s.n)
+                continue
             if s.dtype not in (np.uint8, torch.uint8) or s.ndim not in (3, 4) or s.shape[-1] != 3 or (s.ndim == 4 and s.shape[0] != 1):
                 raise ValueError("each interpolated style must be one uint8 [Hs,Ws,3] image")
         return WCT.normalize_weights(style_weights, n_frames, len(styles)), styles
@@ -159,13 +184,15 @@ class WCT(object):
             mask, region_styles = self.check_mask(content_mask, n, styles)
 
         def to_dev(a):
-            if isinstance(a, np.ndarray):
-                a = torch.from_numpy(np.array(a, copy=True, order="C"))    # own, writable, contiguous
-            if a.dim() == 3:
-                a = a.unsqueeze(0)
-            if a.dtype != torch.uint8:
-                a = a.clamp(0, 255).to(torch.uint8)   # the reference feeds arrays "in [0,255]" (wct.py:74)
-            return a.to(dev, non_blocking=True).contiguous()
+            return _to_dev(a, dev)
+
+        def style_dev(a):
+            """A style image on the device, or a prepared style as it is.  With several passes an image is prepared once
+            here, and every pass applies it."""
+            if isinstance(a, PreparedStyle):
+                return a
+            a = to_dev(a)
+            return eng.prepare_call(a, adain=adain, swap5=swap5) if int(passes) > 1 else a
 
         if swap5 and self.ss_stride != 1:
             # wct.py:84-90: with a stride the filter may not fit; centre-crop the content (on the device) to a size it tiles
@@ -180,32 +207,28 @@ class WCT(object):
             c = to_dev(contents)
             if style_weights is not None:
                 w_dev = torch.from_numpy(weights).to(dev, non_blocking=True)
-                ist = [to_dev(x) for x in interp_styles]
+                ist = [style_dev(x) for x in interp_styles]
 
-                def one_pass(x):
+                def one_pass(x, first):
                     return eng.stylize(x, None, alpha=alpha, adain=adain, interp_styles=ist, interp_weights=w_dev)
             elif content_mask is not None:
                 lab = mask.to(dev, non_blocking=True)
-                rs = [to_dev(x) for x in region_styles]
+                rs = [style_dev(x) for x in region_styles]
 
-                def one_pass(x):
+                def one_pass(x, first):
                     return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs)
             else:
-                s = to_dev(styles)
+                s = style_dev(styles)
 
-                def one_pass(x):
-                    return eng.stylize(x, s, alpha=alpha, adain=adain)
-            if swap5:
-                # one pair per call like the reference graph (ops.py:146); frames of a batch are swapped one by one
-                outs = [eng.stylize(c[i:i + 1], s[i:i + 1] if s.shape[0] > 1 else s, alpha=alpha, adain=adain, swap5=True,
-                                    ss_alpha=ss_alpha, ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride)
-                        for i in range(c.shape[0])]
-                out_f = outs[0] if len(outs) == 1 else torch.cat(outs, dim=0)
-            else:
-                out_f = one_pass(c)
+                def one_pass(x, first):
+                    # the style swap acts in the first pass only (stylize_video.py:117-121).  A shared style swaps the
+                    # whole batch in one call; with one style per frame the engine swaps frame by frame.
+                    return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
+                                       ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride)
+            out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
-                out_f = one_pass(out_dev)
+                out_f = one_pass(out_dev, False)
                 out_dev = eng.to_u8(out_f)
             if return_device:
                 eng.check_device()            # synchronises; raises WctB200Error if a kernel recorded a pipeline time-out
@@ -224,6 +247,62 @@ class WCT(object):
         if return_float:
             return out_u8, out_f.cpu().numpy()
         return out_u8
+
+    def prepare_style(self, style):
+        """Prepare ``style`` (uint8 [H,W,3] or [n,H,W,3]; numpy or torch, host or device) once, for any number of calls.
+
+        Returns a ``PreparedStyle`` of n styles holding, per relu target, the WCT state for this model's semantics and the
+        AdaIN moments; the relu5_1 style feature when relu5_1 is a target (the style swap is prepared from it on first use);
+        and the style image on the host (``--concat``).  It is accepted wherever a style image is: ``predict_batch`` /
+        ``predict`` / ``synthesize`` with n in {1, N}, and as an entry (n = 1) of the style lists of ``style_weights`` and
+        ``content_mask``, with ``adain``, ``passes`` and ``swap5``.  The results are byte-identical to the image's."""
+        if isinstance(style, PreparedStyle):
+            return style
+        if style.dtype not in (np.uint8, torch.uint8) or style.ndim not in (3, 4) or style.shape[-1] != 3:
+            raise ValueError("a style must be uint8 [H,W,3] or [n,H,W,3]")
+        eng = self.engine
+        with torch.cuda.device(eng.device):
+            s = _to_dev(style, eng.device)
+            ps = eng.prepare(s)
+            ps.image = s.cpu().numpy()
+            ps.fingerprints = dict(eng.fingerprints())
+        return ps
+
+    def load_style(self, path):
+        """Read a ``.wctstyle`` file written by ``PreparedStyle.save``.  The file serves this model when its semantics
+        are this model's and it holds every relu target of this model with the same encoder weights up to that relu;
+        decoders do not matter.  Otherwise ValueError, naming the field: ``version``, ``eps_cov`` / ``eps_eig`` /
+        ``thresh``, ``targets`` or ``<relu>/fingerprint``."""
+        from . import prepared as P
+        eng = self.engine
+        data = P.read_file(path)
+        sem = SEMANTICS[eng.semantics]
+        taps = list(dict.fromkeys(self.model.style_taps))
+        P.check_file(data, path, sem, taps, eng.fingerprints())
+        image = data["image"]
+        ps = PreparedStyle(image.shape[0], {k: sem[k] for k in P.SEMANTIC_KEYS}, taps)
+        ps.image = image
+        ps.fingerprints = {relu: str(data["%s/fingerprint" % relu]) for relu in taps}
+        dev = eng.device
+        with torch.cuda.device(dev):
+            for relu in taps:
+                ps.wct[relu] = P.pack_wct_state(eng.lib, data["%s/wct_mean" % relu], data["%s/wct_cs" % relu], data["%s/wct_k" % relu], dev)
+                ps.adain[relu] = P.pack_adain_state(eng.lib, data["%s/adain_mean" % relu], data["%s/adain_var" % relu], dev)
+            if "relu5_1" in taps:
+                raw = data["relu5_1/feat"]                                      # float16 [2, n, Hs+2, Ws+2, 512]
+                if raw.dtype != np.float16 or raw.ndim != 5 or raw.shape[:2] != (2, ps.n) or raw.shape[4] != 512:
+                    raise ValueError("%s: relu5_1/feat: bad shape %s" % (path, raw.shape))
+                act = eng._act(ps.n, raw.shape[2] - 2, raw.shape[3] - 2, 512)
+                flat = torch.from_numpy(np.ascontiguousarray(raw).view(np.uint8).reshape(-1)).to(dev)
+                act.buf[:flat.numel()] = flat
+                ps.feat5 = act
+            main = torch.cuda.current_stream(dev)
+            ps.side = main
+            for relu in taps:
+                ev = torch.cuda.Event()
+                ev.record(main)
+                ps.events[relu] = ev
+        return ps
 
     def synthesize(self, styles, size, count=1, seed=0, first_index=0, **kw):
         """Texture synthesis (WCT paper, section 4; the reference's ``--noise``, webcam.py:191-192): stylise ``count`` frames
@@ -248,14 +327,16 @@ class WCT(object):
         is a list of R region styles and region r of the content takes style r.  With ``style_weights`` ([K]), ``style`` is a
         list of K styles and the content takes their weighted blend.'''
         s = time.time()
+        def host(x):
+            return x if isinstance(x, PreparedStyle) else np.asarray(x)
         if style_weights is not None:
-            out = self.predict_batch(np.asarray(content), [np.asarray(x) for x in style], alpha=alpha, adain=adain, swap5=swap5,
-                                     style_weights=style_weights, content_mask=content_mask)
+            out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
+                                     swap5=swap5, style_weights=style_weights, content_mask=content_mask)
         elif content_mask is not None:
-            out = self.predict_batch(np.asarray(content), [np.asarray(x) for x in style], alpha=alpha, adain=adain, swap5=swap5,
-                                     content_mask=content_mask)
+            out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
+                                     swap5=swap5, content_mask=content_mask)
         else:
-            out = self.predict_batch(np.asarray(content), np.asarray(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha)
+            out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
