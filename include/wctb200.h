@@ -193,11 +193,26 @@ WCTB200_API size_t wctb200_wct_style_state_layout(int C, int Ns, size_t* off_mea
  * R in 1..8, else WCTB200_EINVAL.  ws: device scratch of wctb200_wct_regions_workspace_bytes(C, Nc, R, Hc, Wc).
  * k_out (device int32 [2*(Nc*R + R)], may be NULL): [k_c x Nc*R | k_s x R | sweeps_c x Nc*R | sweeps_s x R], entry
  * n*R + r for frame n / region r; k_c = -1 (and 0 sweeps) for a skipped (frame, region).
+ * A state with k_s = -1 (an empty style region of wctb200_wct_style_prepare_regions) makes region r keep its content
+ * feature in every frame, as a region of fewer than 2 pixels does; k_out reports k_c = -1 for it.
  * With R = 1 and every label 0 the output is byte-identical to wctb200_wct_apply's. */
 WCTB200_API size_t wctb200_wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc);
 WCTB200_API int wctb200_wct_apply_regions(const void* content, int Nc, int Hc, int Wc, int C, const uint8_t* labels, int R,
                               const void* const* states, float alpha, float eps_cov, float eps_eig, float thresh,
                               int readd_content_mean, void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
+/* Style masks for spatial control: the style side of R regions from ONE style and its label map.  Writes one state of
+ * wctb200_wct_style_state_bytes(C, R) bytes (layout wctb200_wct_style_state_layout(C, R)) whose entry r is
+ * wctb200_wct_style_prepare's (same semantics flags) over the style pixels labelled r only.  When every pixel is labelled r,
+ * entry r is byte-identical to wctb200_wct_style_prepare of the style.  An entry whose region has fewer than 2 pixels is
+ * the sentinel k_s = -1 with 0 sweeps, mean 0 and C_s 0: wctb200_wct_apply_regions keeps that region's content.
+ * style SPF16 [1,Hs,Ws,C]; labels device uint8 [Hs][Ws] at the level's style feature resolution
+ * (wctb200_labels_resize_nearest; labels >= R belong to no entry).  C in {64,128,256,512}, R in 1..8, else
+ * WCTB200_EINVAL (also for a null pointer).  ws: device scratch of wctb200_wct_style_prepare_regions_workspace_bytes(C, R, Hs,
+ * Ws).  k_out (device int32 [2*R], may be NULL): [k_s x R | sweeps x R]. */
+WCTB200_API size_t wctb200_wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws);
+WCTB200_API int wctb200_wct_style_prepare_regions(const void* style, int Hs, int Ws, int C, const uint8_t* labels, int R,
+                                      float eps_cov, float eps_eig, float thresh, void* state, int32_t* k_out,
+                                      void* ws, size_t ws_bytes, void* stream);
 /* Style interpolation (WCT paper, section 4): the transform of wctb200_wct_apply (same semantics flags) against a weighted
  * blend of K styles.  The transform is affine in the style statistics, so the blend runs on the states: frame n is coloured
  * with C_w = sum_k w_k C_sk and shifted by m_w = sum_k w_k m_sk (an fp32 fmaf chain in k order), so that

@@ -8,7 +8,10 @@ content x style loop at stylize.py:70-119, output naming ``<content>_<style><ext
 
 Spatial control: ``--content-mask MASK --mask-styles S0 S1 ...`` splits the content by an 8-bit grayscale mask (gray value
 v -> region v*R // 256 for R styles: a black/white mask with two styles gives background / foreground) and region r takes
-style r; the output is ``<content>_<s0>+<s1>...<ext>``.
+style r; the output is ``<content>_<s0>+<s1>...<ext>``.  ``--style-masks M0 M1 ...`` (one per style, quantised the same
+way) gives each style a label map too: region r then takes only the pixels of style r in region r, so painting both
+masks with the same grey levels links the regions ("the sky of the photo takes the sky of the painting").  A path given
+twice is loaded once; one painting with one mask for every region is encoded once.
 
 Style interpolation: ``--interp-styles S0 S1 ... --interp-weights w0 w1 ...`` stylises with the weighted blend of 1..8
 styles (weights >= 0, normalised to sum 1; WCT or ``--adain``); the output is ``<content>_<s0>-<w0>+<s1>-<w1>...<ext>``
@@ -62,6 +65,8 @@ _FLAGS = [
     (("--semantics",), dict(type=str, default="tf", choices=["tf", "np"], help="wct_tf (the reference graph) or wct_np eps/blend rules")),
     (("--content-mask",), dict(type=str, default=None, help="8-bit grayscale region mask: gray v -> region v*R//256 (R = #--mask-styles)")),
     (("--mask-styles",), dict(nargs="+", type=str, default=None, help="one style image per mask region (with --content-mask)")),
+    (("--style-masks",), dict(nargs="+", type=str, default=None,
+                              help="one 8-bit grayscale mask per --mask-styles entry: region r takes the pixels of style r in region r")),
     (("--interp-styles",), dict(nargs="+", type=str, default=None, help="1..8 style images to blend (with --interp-weights)")),
     (("--interp-weights",), dict(nargs="+", type=float, default=None, help="one weight >= 0 per --interp-styles entry (normalised)")),
     # webcam.py:38; the three --noise-* flags are not in the reference.  Their defaults are filled in by parse_args, so that
@@ -102,9 +107,26 @@ def parse_args(argv=None):
                 parser.error("--content-mask does not combine with %s" % flag)
     elif args.mask_styles:
         parser.error("--mask-styles needs --content-mask")
+    check_style_mask_flags(parser, args)
     check_noise_flags(parser, args)
     check_prepared_flags(parser, args)
     return args
+
+
+def check_style_mask_flags(parser, args):
+    """--style-masks: one mask per --mask-styles entry, with --content-mask; not with --crop-size (a crop moves the style
+    off its mask) or prepared styles (they keep no feature maps to mask).  --style-size scales style and mask alike."""
+    if args.style_masks is None:
+        return
+    if args.content_mask is None:
+        parser.error("--style-masks needs --content-mask")
+    if len(args.style_masks) != len(args.mask_styles):
+        parser.error("--style-masks needs one mask per --mask-styles entry (%d masks, %d styles)"
+                     % (len(args.style_masks), len(args.mask_styles)))
+    if args.crop_size:
+        parser.error("--style-masks does not combine with --crop-size")
+    if any(is_prepared(p) for p in args.mask_styles):
+        parser.error("--style-masks does not combine with prepared styles (.wctstyle)")
 
 
 PREPARED_EXT = ".wctstyle"
@@ -282,24 +304,39 @@ def make_model(args):
                ss_patch_size=args.ss_patch_size, ss_stride=args.ss_stride, weights=weights, semantics=args.semantics, verbose=True)
 
 
-def _stylize_masked(model, content_dev, styles_dev, labels, args):
+def _stylize_masked(model, content_dev, styles_dev, labels, args, style_masks=None):
     kw = dict(alpha=args.alpha, return_device=True, content_mask=labels)
+    if style_masks is not None:
+        kw["style_masks"] = style_masks
     result = model.predict_batch(content_dev, styles_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, styles_dev, **kw)
     return result
 
 
+def _once_per_path(paths, load):
+    """``load(path)`` once per distinct path; a repeated path gives the same object again."""
+    cache = {}
+    for p in paths:
+        if p not in cache:
+            cache[p] = load(p)
+    return [cache[p] for p in paths]
+
+
 def main_masked(args, model, io, dimg, t_start):
-    """--content-mask: every content image, split by the mask, with region r in style r."""
-    labels = read_mask(args.content_mask, len(args.mask_styles))
+    """--content-mask: every content image, split by the mask, with region r in style r (with --style-masks, in the
+    pixels of style r labelled r).  A path given twice is loaded once and passed as the same object, so that one style
+    with one mask for several regions is encoded once."""
+    R = len(args.mask_styles)
+    labels = read_mask(args.content_mask, R)
+    style_masks = _once_per_path(args.style_masks, lambda p: read_mask(p, R)) if args.style_masks else None
     os.makedirs(args.out_path, exist_ok=True)
     device = model.engine.device
     written = 0
     prepared = PreparedStyles(model)
     for names, content_dev in _contents(args, io, dimg, device):
-        styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device, prepared) for p in args.mask_styles]
-        results = _stylize_masked(model, content_dev, styles_dev, labels, args)
+        styles_dev = _once_per_path(args.mask_styles, lambda p: _prepare_style(p, args, io, dimg, content_dev, device, prepared))
+        results = _stylize_masked(model, content_dev, styles_dev, labels, args, style_masks)
         for name, result in zip(names, results):
             target = os.path.join(args.out_path, mask_output_name(name, args.mask_styles))
             io.save_img(target, dimg.to_host(result))

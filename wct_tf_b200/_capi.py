@@ -52,6 +52,8 @@ SIGNATURES = {
     "wctb200_jacobi_eigh": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
     "wctb200_wct_regions_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "wctb200_wct_apply_regions": (_i, [_vp, _i, _i, _i, _i, _vp, _i, C.POINTER(_vp), _f, _f, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_wct_style_prepare_regions_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "wctb200_wct_style_prepare_regions": (_i, [_vp, _i, _i, _i, _vp, _i, _f, _f, _f, _vp, _vp, _vp, _sz, _vp]),
     "wctb200_wct_blend_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "wctb200_wct_apply_blend": (_i, [_vp, _i, _i, _i, _i, C.POINTER(_vp), _i, _vp, _i, _f, _f, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
     "wctb200_adain_blend_workspace_bytes": (_sz, [_i, _i, _i]),

@@ -138,6 +138,9 @@ size_t wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc);
 int launch_wct_apply_regions(const __half*, int, int, int, int, const uint8_t*, int, const void* const*, float, float, float, float,
                              int, __half*, int32_t*, void*, size_t, cudaStream_t);
 int launch_labels_resize(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, cudaStream_t st);
+size_t wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws);
+int launch_wct_style_prepare_regions(const __half*, int, int, int, const uint8_t*, int, float, float, float, void*, int32_t*, void*,
+                                     size_t, cudaStream_t);
 int launch_covariance_regions(const __half*, int, int, int, int, const uint8_t*, int, float, float*, float*, int*, cudaStream_t);
 int launch_jacobi(float*, int, int, float*, int*, cudaStream_t, const int* skip);
 int launch_eig_post(const float*, const float*, float*, int, int, float, float, int, float*, float*, int*, cudaStream_t, const int* skip);
@@ -347,6 +350,19 @@ int wctb200_wct_apply_regions(const void* content, int Nc, int Hc, int Wc, int C
     WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "wct_apply_regions: bad geometry");
     return launch_wct_apply_regions(HCP(content), Nc, Hc, Wc, C, labels, R, states, alpha, eps_cov, eps_eig, thresh,
                                     readd_content_mean, HP(out), k_out, ws, ws_bytes, ST(stream));
+}
+size_t wctb200_wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws) {
+    if (C < 8 || R < 1 || R > 8 || Hs < 2 || Ws < 2) return 0;
+    return wct_style_prepare_regions_workspace_bytes(C, R, Hs, Ws);
+}
+int wctb200_wct_style_prepare_regions(const void* style, int Hs, int Ws, int C, const uint8_t* labels, int R, float eps_cov,
+                                      float eps_eig, float thresh, void* state, int32_t* k_out, void* ws, size_t ws_bytes,
+                                      void* stream) {
+    WCTB_REQUIRE(style && labels && state && ws, "wct_style_prepare_regions: null pointer");
+    WCTB_REQUIRE(R >= 1 && R <= 8, "wct_style_prepare_regions: R=%d not in 1..8", R);
+    WCTB_REQUIRE(geom_ok(1, Hs, Ws, C), "wct_style_prepare_regions: bad geometry");
+    return launch_wct_style_prepare_regions(HCP(style), Hs, Ws, C, labels, R, eps_cov, eps_eig, thresh, state, k_out, ws, ws_bytes,
+                                            ST(stream));
 }
 size_t wctb200_wct_blend_workspace_bytes(int C, int Nc, int K, int Nw) {
     if (C < 8 || Nc < 1 || K < 1 || K > 8 || (Nw != 1 && Nw != Nc)) return 0;

@@ -1366,6 +1366,13 @@ static int region_scan(const uint8_t* labels, int N, int H, int W, int R, int* c
     return 0;
 }
 
+// a style state entry with k_s = -1 (a style mask region of < 2 pixels, wct_style_prepare_regions) keeps region r of every
+// frame: its pixel counts drop to 0, and every consumer skips a (frame, region) with counts < 2
+__global__ void k_regions_drop_empty_styles(const int* __restrict__ ks, int np, int R, int* __restrict__ counts) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < np && ks[2 * (i % R)] == -1) counts[i] = 0;
+}
+
 int launch_wct_apply_regions(const __half* content, int Nc, int Hc, int Wc, int C, const uint8_t* labels, int R,
                              const void* const* states, float alpha, float eps_cov, float eps_eig, float thresh, int readd,
                              __half* out, int32_t* k_out, void* ws, size_t ws_bytes, cudaStream_t st) {
@@ -1414,6 +1421,8 @@ int launch_wct_apply_regions(const __half* content, int Nc, int Hc, int Wc, int 
     WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)np * 2 * 4, st));
     int rc = region_scan(labels, Nc, Hc, Wc, R, counts, tmask, st);
     if (rc) return rc;
+    k_regions_drop_empty_styles<<<(unsigned)cdiv(np, 256), 256, 0, st>>>(ks, np, R, counts);
+    WCTB_CHECK_LAUNCH("k_regions_drop_empty_styles");
     // per (frame, region): masked covariance; then the content side of wct_apply over Nc*R matrices, style z % R
     rc = launch_mean_cov_regions(content, ActGeom(Nc, Hc, Wc, C), labels, R, counts, tmask, eps_cov, mean, G, A0, dsum, st);
     if (rc) return rc;
@@ -1459,6 +1468,94 @@ int launch_covariance_regions(const __half* act, int N, int H, int W, int C, con
     int rc = region_scan(labels, N, H, W, R, counts, tmask, st);
     if (rc) return rc;
     return launch_mean_cov_regions(act, ActGeom(N, H, W, C), labels, R, counts, tmask, eps_cov, mean_out, cov_out, nullptr, dsum, st);
+}
+
+// ---------------------------------------------------------------------------
+// Style masks: the style side of spatial control over the labelled parts of ONE style.  Entry r of the state of R styles
+// is wct_style_prepare restricted to the style pixels labelled r (the masked covariance of the content side, N = 1 and R
+// problems).  With every label equal to r the covariance kernel adds in the unmasked order, so entry r is then
+// byte-identical to wct_style_prepare.  An entry of < 2 pixels is the sentinel k_s = -1, 0 sweeps, mean 0, C_s 0, and
+// wct_apply_regions keeps the content of that region.
+// ---------------------------------------------------------------------------
+struct StyleRegionWs {
+    size_t base, counts, tmask, total;
+};
+static StyleRegionWs style_regions_layout(int C, int R, int Hs, int Ws) {
+    StyleRegionWs L;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.base = take(wct_layout(C, 0, R).total);        // the eigensolver's, as wct_style_prepare's for R styles
+    L.counts = take((size_t)R * 4);
+    L.tmask = take((size_t)((Ws + 31) / 32) * ((Hs + 1) / 2) * 2);
+    L.total = o;
+    return L;
+}
+size_t wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws) { return style_regions_layout(C, R, Hs, Ws).total; }
+
+// entries whose region has < 2 pixels -> the sentinel.  grid (blocks, R)
+__global__ void k_style_regions_empty(const int* __restrict__ counts, int C, int R, float* __restrict__ mean, float* __restrict__ Cs,
+                                      int* __restrict__ ks) {
+    const int r = blockIdx.y;
+    if (counts[r] >= 2) return;
+    const long long CC = (long long)C * C;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < CC; i += (long long)gridDim.x * blockDim.x) {
+        Cs[r * CC + i] = 0.f;
+        if (i < C) mean[(long long)r * C + i] = 0.f;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        ks[r] = -1;
+        ks[R + r] = 0;
+    }
+}
+
+int launch_wct_style_prepare_regions(const __half* style, int Hs, int Ws, int C, const uint8_t* labels, int R, float eps_cov,
+                                     float eps_eig, float thresh, void* state, int32_t* k_out, void* ws, size_t ws_bytes,
+                                     cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_style_prepare_regions: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(R >= 1 && R <= 8, "wct_style_prepare_regions: R=%d not in 1..8", R);
+    const StyleRegionWs SL = style_regions_layout(C, R, Hs, Ws);
+    if (ws_bytes < SL.total) {
+        set_error("wct_style_prepare_regions: workspace %zu < %zu bytes", ws_bytes, SL.total);
+        return WCTB200_EWS;
+    }
+    const WctWs L = wct_layout(C, 0, R);
+    uint8_t* w = static_cast<uint8_t*>(ws) + SL.base;
+    int* counts = reinterpret_cast<int*>(static_cast<uint8_t*>(ws) + SL.counts);
+    uint16_t* tmask = reinterpret_cast<uint16_t*>(static_cast<uint8_t*>(ws) + SL.tmask);
+    size_t off_cs, off_k;
+    style_state_offsets(C, R, &off_cs, &off_k);
+    uint8_t* sp = static_cast<uint8_t*>(state);
+    float* mean_s = reinterpret_cast<float*>(sp);
+    float* Cs = reinterpret_cast<float*>(sp + off_cs);
+    int* kc = reinterpret_cast<int*>(sp + off_k);
+    double* dsum = reinterpret_cast<double*>(w + L.dsum);
+    float* G = reinterpret_cast<float*>(w + L.G);
+    float* A0 = reinterpret_cast<float*>(w + L.A0);
+    float* lam = reinterpret_cast<float*>(w + L.lam);
+    float* sigma = reinterpret_cast<float*>(w + L.sigma);
+    float* dvec = reinterpret_cast<float*>(w + L.dvec);
+    float* conv = reinterpret_cast<float*>(w + L.conv);
+    int* ok = reinterpret_cast<int*>(w + L.ok);
+    const long long CC = (long long)C * C;
+    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)R * 2 * 4, st));
+    int rc = region_scan(labels, 1, Hs, Ws, R, counts, tmask, st);
+    if (rc) return rc;
+    rc = launch_mean_cov_regions(style, ActGeom(1, Hs, Ws, C), labels, R, counts, tmask, eps_cov, mean_s, G, A0, dsum, st);
+    if (rc) return rc;
+    // from here on wct_style_prepare's steps over the R matrices (an empty region's placeholder G = I is harmless)
+    rc = launch_matfun_ns(A0, C, R, /*n_first=*/0, thresh, eps_eig, Cs, ok, kc, st);
+    if (rc < 0) return rc;
+    rc = launch_jacobi(G, C, R, conv, kc + R, st, ok);
+    if (rc) return rc;
+    rc = launch_eig_post(G, A0, lam, C, R, thresh, eps_eig, /*n_content=*/0, sigma, dvec, kc, st, ok);
+    if (rc) return rc;
+    dim3 gg((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)R);
+    k_outer_gemm<<<gg, 256, 0, st>>>(G, CC, G, CC, dvec, C, Cs, CC, C, ok);
+    WCTB_CHECK_LAUNCH("k_outer_gemm(Cs)");
+    k_style_regions_empty<<<dim3((unsigned)cdiv(CC, 256 * 8), (unsigned)R), 256, 0, st>>>(counts, C, R, mean_s, Cs, kc);
+    WCTB_CHECK_LAUNCH("k_style_regions_empty");
+    if (k_out) WCTB_CUDA(cudaMemcpyAsync(k_out, kc, (size_t)R * 2 * 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
 }
 
 // ---------------------------------------------------------------------------

@@ -370,6 +370,22 @@ class Engine(object):
                    flops=2.0 * C * C * style.N * hws, bytes_=4.0 * C * style.N * hws)
         return state
 
+    def style_prepare_regions(self, style, labels, R):
+        """Style side of one level under a style mask: entry r of the returned state of R styles is ``style_prepare`` over
+        the pixels of ``style`` (one style) labelled r in ``labels`` (device uint8 [1,Hs,Ws] at the feature resolution).  An
+        entry of fewer than 2 pixels has k_s = -1, and ``wct_apply_regions`` keeps the content of that region."""
+        st = self._stream()
+        sem = SEMANTICS[self.semantics]
+        C = style.C
+        state = torch.empty(self.lib.wctb200_wct_style_state_bytes(C, R), dtype=torch.uint8, device=self.device)
+        ws = self._grow_workspace(("style_regions", C, R),
+                                  self.lib.wctb200_wct_style_prepare_regions_workspace_bytes(C, R, style.H, style.W))
+        hws = style.H * style.W
+        self._call("wct_style_regions[C%d]" % C, 10 + self._matfun_launches(C), self.lib.wctb200_wct_style_prepare_regions, style.ptr,
+                   style.H, style.W, C, labels.data_ptr(), R, sem["eps_cov"], sem["eps_eig"], sem["thresh"], state.data_ptr(), None,
+                   ws.data_ptr(), ws.numel(), st, flops=2.0 * C * C * hws, bytes_=4.0 * C * hws)
+        return state
+
     def wct_apply(self, content, state, n_style, alpha, want_info=False):
         st = self._stream()
         sem = SEMANTICS[self.semantics]
@@ -401,7 +417,7 @@ class Engine(object):
         ws = self._grow_workspace(("regions", C, N, R), self.lib.wctb200_wct_regions_workspace_bytes(C, N, R, content.H, content.W))
         kbuf = torch.empty(2 * (N * R + R), dtype=torch.int32, device=self.device) if want_info else None
         hwc = content.H * content.W
-        self._call("wct_regions[C%d]" % C, 12 + self._matfun_launches(C), self.lib.wctb200_wct_apply_regions, content.ptr, N,
+        self._call("wct_regions[C%d]" % C, 13 + self._matfun_launches(C), self.lib.wctb200_wct_apply_regions, content.ptr, N,
                    content.H, content.W, C, labels.data_ptr(), R, _capi.pointer_array([s.data_ptr() for s in states]),
                    float(alpha), sem["eps_cov"], sem["eps_eig"], sem["thresh"], sem["readd"], out.ptr,
                    kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel(), st,
@@ -449,7 +465,8 @@ class Engine(object):
 
     # ------------------------------------------------------------------ pipeline
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
-                ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None):
+                ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
+                region_masks=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -468,12 +485,20 @@ class Engine(object):
         At every level the map is resampled to the feature grid and region r of a frame is transformed against style r
         (WCT only); labels >= R keep the content feature.  The R styles are encoded and prepared once per call.
 
+        Style masks: ``region_masks`` (with ``labels``) is a list of R entries, each None (the whole style r) or a cuda
+        uint8 label map [Hm',Wm'] of style r, of any resolution.  Region r then takes the statistics of the pixels of style
+        r labelled r, the map sampled to each level's style feature grid by the rule of ``labels``; where that region has
+        fewer than 2 pixels at a level, region r of every frame keeps its content feature.  Entries that are the same
+        (style, mask) pair of objects share one encode and one masked prepare (``_region_sides``).
+
         Style interpolation: ``interp_styles`` is a list of K (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes, or prepared
         styles of one style each, and ``interp_weights`` a cuda float32 [1|N, K] tensor; ``style_u8`` is ignored.  Frame n is
         stylised with the blend of the K styles under weight row n (one row: every frame), which for a row that sums to 1 is
         the same blend of the K single-style outputs at every level (WCT and AdaIN are affine in the style statistics).  The
         weights are used as given.  The K styles are encoded and prepared once per call."""
         N = content_u8.shape[0]
+        if region_masks is not None and labels is None:
+            raise ValueError("style masks (region_masks) need a content label map (labels)")
         if interp_styles is not None:
             if labels is not None or swap5:
                 raise ValueError("style interpolation does not combine with spatial control (labels) or swap5")
@@ -498,8 +523,10 @@ class Engine(object):
             if labels.dtype != torch.uint8 or labels.dim() != 3 or labels.shape[0] not in (1, N):
                 raise ValueError("labels must be uint8 [Hm,Wm] or [N,Hm,Wm]")
             labels = labels.expand(N, -1, -1).contiguous()
+            if region_masks is not None:
+                region_masks = self.check_region_masks(region_masks, region_styles)
             return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
-                                       lambda lo, hi: ("regions", labels[lo:hi]))
+                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks)
         swap5 = bool(swap5) and "relu5_1" in [l.relu_target for l in self.model.levels]    # model.py:148: only relu5_1 swaps
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
@@ -573,26 +600,76 @@ class Engine(object):
             self._group_streams[g].wait_stream(main)
         return out
 
-    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame):
+    def check_region_masks(self, masks, styles):
+        """ValueError unless ``masks`` holds one entry per region style, each None or a uint8 label map [Hm',Wm'] (or
+        [1,Hm',Wm']) on this device, and no prepared style has a mask.  Returns the list with every map as [1,Hm',Wm'];
+        entries that were the same object stay the same object."""
+        masks = list(masks)
+        if len(masks) != len(styles):
+            raise ValueError("%d style masks for %d region styles: give one entry (None or a mask) per style" % (len(masks), len(styles)))
+        out, seen = [], {}
+        for s, m in zip(styles, masks):
+            if m is None:
+                out.append(None)
+                continue
+            if isinstance(s, PreparedStyle):
+                raise ValueError("a prepared style has no feature maps to mask: give the style image with its mask")
+            if id(m) not in seen:
+                if (not isinstance(m, torch.Tensor) or m.dtype != torch.uint8 or m.device != self.device or m.dim() not in (2, 3)
+                        or (m.dim() == 3 and m.shape[0] != 1) or m.shape[-2] < 1 or m.shape[-1] < 1):
+                    raise ValueError("each style mask must be a uint8 label map [Hm,Wm] on %s" % self.device)
+                seen[id(m)] = (m, m.reshape(1, m.shape[-2], m.shape[-1]).contiguous())
+            out.append(seen[id(m)][1])
+        return out
+
+    def _region_sides(self, styles, masks, main, adain=False):
+        """The style sides of a multi-style call: (one side per style, the sides made here).  Without ``masks`` every image
+        is prepared on its own.  With ``masks`` (``check_region_masks``) the entries that are the same (style, mask) pair of
+        objects share one side: an unmasked entry takes it whole, and a masked entry r takes its entry r, the style prepared
+        over its pixels labelled r (``_style_side`` with a mask)."""
+        sides, owned, shared = [], [], {}
+        R = len(styles)
+        for r, s in enumerate(styles):
+            m = masks[r] if masks is not None else None
+            if isinstance(s, PreparedStyle):
+                if s.n != 1:
+                    raise ValueError("each region / interpolated style must be one style, got a prepared style of %d" % s.n)
+                self.check_prepared(s, adain, False)
+                sides.append(s)
+            elif masks is None:
+                owned.append(self._style_side(s, main, wct=not adain, adain=adain))
+                sides.append(owned[-1])
+            else:
+                key = (id(s), id(m))
+                if key not in shared:
+                    shared[key] = self._style_side(s, main, labels=m, R=R) if m is not None else self._style_side(s, main)
+                    owned.append(shared[key])
+                sides.append(shared[key].entries[r] if m is not None else shared[key])
+        return sides, owned
+
+    def prepare_regions_call(self, styles, masks):
+        """The style sides of a spatial-control call with style masks (``check_region_masks``), made once for a call that
+        applies them several times (passes): one prepared style of one style per region."""
+        main = torch.cuda.current_stream(self.device)
+        sides, owned = self._region_sides(styles, masks, main)
+        for s, m in zip(styles, masks):
+            if not isinstance(s, PreparedStyle):
+                side = self._style_stream() or main
+                s.record_stream(side)
+                if m is not None:
+                    m.record_stream(side)
+        return sides
+
+    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None):
         """``stylize`` with several styles (spatial control, style interpolation): images are prepared once per call, and
         every style side is shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the
-        label maps or weight rows)."""
+        label maps or weight rows); ``masks``: the style masks of spatial control (``_region_sides``)."""
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
         self._group = 1 if G > 1 else 0
-        owned = []
         try:
-            sides = []
-            for s in styles:
-                if isinstance(s, PreparedStyle):
-                    if s.n != 1:
-                        raise ValueError("each region / interpolated style must be one style, got a prepared style of %d" % s.n)
-                    self.check_prepared(s, adain, False)
-                    sides.append(s)
-                else:
-                    owned.append(self._style_side(s, main, wct=not adain, adain=adain))
-                    sides.append(owned[-1])
+            sides, owned = self._region_sides(styles, masks, main, adain)
         finally:
             self._group = 0
         if G == 1:
@@ -615,19 +692,27 @@ class Engine(object):
             self._style_streams[self._group] = torch.cuda.Stream(device=self.device, priority=prio)
         return self._style_streams[self._group]
 
-    def _style_side(self, style_u8, main, wct=True, adain=False, keep5=False, skip=()):
+    def _style_side(self, style_u8, main, wct=True, adain=False, keep5=False, skip=(), labels=None, R=0):
         """The prepare step: style side of one call (model.py:70-72: ONE encoder pass emitting every target; per level the
         WCT state of ops.py:48-55,76 when ``wct``, the AdaIN moments when ``adain``; levels in ``skip`` get neither), enqueued
         on this group's style stream when overlap is on.  ``keep5`` keeps the relu5_1 feature (the style swap).  Returns a
-        ``PreparedStyle`` with one event per level."""
+        ``PreparedStyle`` with one event per level.
+
+        With ``labels`` (a style mask, cuda uint8 [1,Hm,Wm] of one style) the WCT state of each level is the masked prepare
+        of R regions, so the result is a prepared style of n = R; ``entries[r]`` is its slice r (``slice_prepared``) as a
+        prepared style of one style, cut per level as soon as that level is prepared and sharing its events."""
         lib = self.lib
         side = self._style_stream() or main
         if side is not main:
             side.wait_stream(main)             # style_u8 (and last step's buffers) are ready
         sem = SEMANTICS[self.semantics]
         taps = list(dict.fromkeys(self.model.style_taps))
-        ps = PreparedStyle(style_u8.shape[0], {k: sem[k] for k in SEMANTIC_KEYS}, taps)
+        ps = PreparedStyle(style_u8.shape[0] if labels is None else R, {k: sem[k] for k in SEMANTIC_KEYS}, taps)
         ps.side = side
+        if labels is not None:
+            ps.entries = [PreparedStyle(1, ps.semantics, taps) for _ in range(R)]
+            for e in ps.entries:
+                e.side, e.events = side, ps.events
         with torch.cuda.stream(side):
             tag, self._tag = self._tag, "style"
             style = torch.empty(style_u8.shape, dtype=torch.float32, device=self.device)
@@ -636,7 +721,12 @@ class Engine(object):
             _, feats = self.encode(style, self.model.deepest_target, taps=self.model.style_taps)
             for relu in taps:
                 if relu not in skip:
-                    if wct:
+                    if labels is not None:
+                        f = feats[relu]
+                        ps.wct[relu] = self.style_prepare_regions(f, self.labels_resize(labels, f.H, f.W), R)
+                        for r, e in enumerate(ps.entries):
+                            e.wct[relu] = slice_wct_state(lib, ps.wct[relu], f.C, R, r, r + 1)
+                    elif wct:
                         ps.wct[relu] = self.style_prepare(feats[relu])
                     if adain:
                         ps.adain[relu] = self.adain_prepare(feats[relu])

@@ -70,6 +70,7 @@ class PreparedStyle(object):
         self.image = None                         # host uint8 [n,H,W,3] (prepare_style / load_style)
         self.fingerprints = {}                    # relu -> encoder fingerprint (prepare_style / load_style)
         self.swap = {}                            # (patch, stride[, frame]) -> (device swap state, event)
+        self.entries = None                       # style-masked side (Engine._style_side): its n styles, one by one
 
     def __repr__(self):
         return "PreparedStyle(n=%d, targets=%s)" % (self.n, self.targets)

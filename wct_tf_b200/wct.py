@@ -10,6 +10,7 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
     content is centre-cropped so that the patches tile its relu5_1 encoding, as wct.py:84-90 does;
   * ``predict_batch`` is new: a batch of frames per call (frames are independent);
   * ``content_mask`` is new: spatial control (WCT paper, section 4), a label map whose region r takes style r;
+    ``style_masks`` restricts style r to its pixels labelled r;
   * ``style_weights`` is new: style interpolation (WCT paper, section 4), a weighted blend of 1..8 styles, shared by
     every frame or one row per frame;
   * ``synthesize`` is new: texture synthesis (WCT paper, section 4), the pipeline run on seeded noise made on the device;
@@ -115,6 +116,32 @@ class WCT(object):
         return m.contiguous(), styles
 
     @staticmethod
+    def check_style_masks(style_masks, styles):
+        """Host-side validation of the style masks of a spatial-control call: a list of one entry per region style (the
+        ``styles`` of ``check_mask``), each None (the whole style) or a uint8 label map [Hm',Wm'] of any resolution, and no
+        mask on a prepared style.  Returns the list with every map as a uint8 tensor; entries that were the same object
+        stay the same object, so that they share one encode and one masked prepare."""
+        if not isinstance(style_masks, (list, tuple)):
+            raise ValueError("style_masks must be a list with one entry (None or a mask) per region style")
+        if len(style_masks) != len(styles):
+            raise ValueError("%d style masks for %d region styles: give one entry (None or a mask) per style"
+                             % (len(style_masks), len(styles)))
+        out, seen = [], {}
+        for s, m in zip(styles, style_masks):
+            if m is None:
+                out.append(None)
+                continue
+            if isinstance(s, PreparedStyle):
+                raise ValueError("a prepared style has no feature maps to mask: give the style image with its mask")
+            if id(m) not in seen:
+                t = m if isinstance(m, torch.Tensor) else torch.from_numpy(np.asarray(m))
+                if t.dtype != torch.uint8 or t.dim() != 2 or t.shape[0] < 1 or t.shape[1] < 1:
+                    raise ValueError("each style mask must be a uint8 label map [Hm,Wm], got %s %s" % (t.dtype, tuple(t.shape)))
+                seen[id(m)] = (m, t.contiguous())
+            out.append(seen[id(m)][1])
+        return out
+
+    @staticmethod
     def normalize_weights(style_weights, n_frames, K, dtype=np.float32):
         """Host-side validation of interpolation weights: [K] (shared by every frame) or [N,K], finite, >= 0, every row with a
         positive sum.  Each row is divided by its sum in float64 (a one-hot row stays exact), then cast to ``dtype``.
@@ -152,7 +179,7 @@ class WCT(object):
         return WCT.normalize_weights(style_weights, n_frames, len(styles)), styles
 
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
-                      passes=1, return_device=False, content_mask=None, style_weights=None):
+                      passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -167,6 +194,13 @@ class WCT(object):
         a list of R (1..8) uint8 [Hs,Ws,3] images of any sizes, and region r of each frame takes style r.  The mask may have
         any resolution: every level samples it to its feature grid.  Labels >= R leave that region unstyled.  WCT only.
 
+        ``style_masks`` (with ``content_mask``): a list of R entries, each None or a uint8 label map [Hm',Wm'] of style r,
+        of any resolution.  Region r of every frame then takes the statistics of the pixels of style r labelled r ("the sky
+        of the photo takes the sky of the painting"); None takes the whole style.  Where the style region has fewer than 2
+        pixels at a level, region r keeps its content feature there.  Entries that are the same (style, mask) pair of
+        objects share one encode and one masked prepare, so one painting with one segmentation is encoded once.  Not with
+        prepared styles as masked entries.
+
         ``style_weights`` (style interpolation): ``styles`` is then a list of K (1..8) uint8 [Hs,Ws,3] images of any sizes
         and ``style_weights`` their weights, [K] for every frame or [N,K] (row n for frame n); finite, >= 0, each row with a
         positive sum, normalised to sum 1.  Frame n is stylised with the blend of the K styles, which equals the blend of
@@ -174,6 +208,8 @@ class WCT(object):
         eng = self.engine
         dev = eng.device
         n = 1 if np.ndim(contents) == 3 else contents.shape[0]
+        if style_masks is not None and content_mask is None:
+            raise ValueError("style_masks needs content_mask")
         if style_weights is not None:
             if content_mask is not None or swap5:
                 raise ValueError("style_weights does not combine with content_mask or swap5")
@@ -182,6 +218,8 @@ class WCT(object):
             if adain or swap5:
                 raise ValueError("content_mask works with WCT only: not with adain or swap5")
             mask, region_styles = self.check_mask(content_mask, n, styles)
+            if style_masks is not None:
+                style_masks = self.check_style_masks(style_masks, region_styles)
 
         def to_dev(a):
             return _to_dev(a, dev)
@@ -211,6 +249,23 @@ class WCT(object):
 
                 def one_pass(x, first):
                     return eng.stylize(x, None, alpha=alpha, adain=adain, interp_styles=ist, interp_weights=w_dev)
+            elif content_mask is not None and style_masks is not None:
+                lab = mask.to(dev, non_blocking=True)
+                # the same object stays the same object on the device: the engine shares its side
+                on_dev = {}
+                for x in region_styles:
+                    if id(x) not in on_dev:
+                        on_dev[id(x)] = x if isinstance(x, PreparedStyle) else to_dev(x)
+                for m in style_masks:
+                    if m is not None and id(m) not in on_dev:
+                        on_dev[id(m)] = m.to(dev, non_blocking=True).contiguous()
+                rs = [on_dev[id(x)] for x in region_styles]
+                sm = [None if m is None else on_dev[id(m)] for m in style_masks]
+                if int(passes) > 1:
+                    rs, sm = eng.prepare_regions_call(rs, eng.check_region_masks(sm, rs)), None
+
+                def one_pass(x, first):
+                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs, region_masks=sm)
             elif content_mask is not None:
                 lab = mask.to(dev, non_blocking=True)
                 rs = [style_dev(x) for x in region_styles]
@@ -322,19 +377,29 @@ class WCT(object):
         noise = noise_u8(count, H, W, seed=seed, first_index=first_index, device=self.engine.device)
         return self.predict_batch(noise, styles, **kw)
 
-    def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None):
+    def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
+                style_masks=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
-        is a list of R region styles and region r of the content takes style r.  With ``style_weights`` ([K]), ``style`` is a
-        list of K styles and the content takes their weighted blend.'''
+        is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
+        labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
+        blend.'''
         s = time.time()
+        seen = {}
+
         def host(x):
-            return x if isinstance(x, PreparedStyle) else np.asarray(x)
+            # one host array per object: a style given twice stays one object (style_masks share its side)
+            if id(x) not in seen:
+                seen[id(x)] = x if isinstance(x, PreparedStyle) else np.asarray(x)
+            return seen[id(x)]
+        if style_masks is not None and content_mask is None:
+            raise ValueError("style_masks needs content_mask")
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, style_weights=style_weights, content_mask=content_mask)
         elif content_mask is not None:
+            kw = {} if style_masks is None else dict(style_masks=style_masks)
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
-                                     swap5=swap5, content_mask=content_mask)
+                                     swap5=swap5, content_mask=content_mask, **kw)
         else:
             out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha)
         if self.verbose:
