@@ -114,12 +114,15 @@ def adain(content_features, style_features, alpha, epsilon=1e-5):
     return dt.type(alpha) * norm + dt.type(1 - alpha) * c
 
 
-def style_swap(content, style, patch_size=3, stride=1, return_info=False):
+def style_swap(content, style, patch_size=3, stride=1, return_info=False, idx=None):
     """ops.py:219-278 on 1xHxWxC arrays.  Every patch_size x patch_size patch of ``style`` (VALID, ``stride``) becomes
     a conv filter; the filters are l2-normalised along the PATCH axis (``tf.nn.l2_normalize(style_patches, dim=3)`` on a
     [p,p,C,n_patches] tensor, ops.py:233 -- i.e. per filter tap, across patches, not per patch); the content is
     cross-correlated with them (VALID), each position takes the arg-max patch (first maximum, like tf.argmax), the
-    UN-normalised patch is pasted back by the transposed conv and overlaps are averaged (ops.py:255-276)."""
+    UN-normalised patch is pasted back by the transposed conv and overlaps are averaged (ops.py:255-276).
+
+    ``idx`` (int [ho, wo]): paste these patches instead of the arg-max (the rest of the op evaluated at another
+    implementation's choice); the correlation is then not computed and ``return_info`` holds only ``idx``."""
     c = np.asarray(content)
     st = np.asarray(style)
     c = c[0] if c.ndim == 4 else c
@@ -134,12 +137,17 @@ def style_swap(content, style, patch_size=3, stride=1, return_info=False):
     norm = np.sqrt(np.maximum((patches ** 2).sum(axis=0, keepdims=True), dt.type(1e-12)))      # l2_normalize epsilon 1e-12
     pn = patches / norm
     ho, wo = (hc - p) // stride + 1, (wc - p) // stride + 1
-    flat = pn.reshape(len(patches), -1)
-    scores = np.empty((ho, wo, len(patches)), dtype=dt)
-    for y in range(ho):
-        for x in range(wo):
-            scores[y, x] = flat @ c[y * stride:y * stride + p, x * stride:x * stride + p, :].reshape(-1)
-    idx = scores.argmax(axis=2)
+    given = idx is not None
+    if given:
+        idx = np.asarray(idx)
+        assert idx.shape == (ho, wo) and idx.min() >= 0 and idx.max() < len(patches), "idx must name a patch per position"
+    else:
+        flat = pn.reshape(len(patches), -1)
+        scores = np.empty((ho, wo, len(patches)), dtype=dt)
+        for y in range(ho):
+            for x in range(wo):
+                scores[y, x] = flat @ c[y * stride:y * stride + p, x * stride:x * stride + p, :].reshape(-1)
+        idx = scores.argmax(axis=2)
     out = np.zeros((1, (ho - 1) * stride + p, (wo - 1) * stride + p, nc), dtype=dt)
     cnt = np.zeros(out.shape[1:3], dtype=dt)
     for y in range(ho):
@@ -147,15 +155,19 @@ def style_swap(content, style, patch_size=3, stride=1, return_info=False):
             out[0, y * stride:y * stride + p, x * stride:x * stride + p, :] += patches[idx[y, x]]
             cnt[y * stride:y * stride + p, x * stride:x * stride + p] += 1
     out = out / cnt[None, :, :, None]
+    if return_info and given:
+        return out, dict(idx=idx)
     if return_info:
         srt = np.sort(scores, axis=2)
         return out, dict(idx=idx, margin=srt[:, :, -1] - srt[:, :, -2], scores=scores)
     return out
 
 
-def wct_style_swap(content, style, alpha, patch_size=3, stride=1, eps=1e-8, thresh=THRESH, return_info=False):
+def wct_style_swap(content, style, alpha, patch_size=3, stride=1, eps=1e-8, thresh=THRESH, return_info=False, idx=None):
     """ops.py:145-217: whiten content AND style (S^-1/2 on the kept eigenvalues of cov + eps*I), style-swap the
-    whitened encodings, colour the result with the style (S^+1/2), add the style mean, blend with fc + mc."""
+    whitened encodings, colour the result with the style (S^+1/2), add the style mean, blend with fc + mc.
+    ``idx``: the patch per position to paste instead of the arg-max (``style_swap``).  ``return_info`` adds the whitened
+    content and style as 1xHxWxC arrays (``wc_feat``, ``ws_feat``)."""
     fcx, shape = _flat(content)
     fsx, sshape = _flat(style)
     dt = fcx.dtype
@@ -170,13 +182,14 @@ def wct_style_swap(content, style, alpha, patch_size=3, stride=1, eps=1e-8, thre
     k_c, k_s = int((wc > thresh).sum()), int((ws > thresh).sum())
     fc_hat = (Ec[:, :k_c] * wc[:k_c] ** dt.type(-0.5)) @ Ec[:, :k_c].T @ fc
     fs_hat = (Es[:, :k_s] * ws[:k_s] ** dt.type(-0.5)) @ Es[:, :k_s].T @ fs
-    swapped, inf = style_swap(_unflat(fc_hat, shape), _unflat(fs_hat, sshape), patch_size, stride, return_info=True)
+    wc_feat, ws_feat = _unflat(fc_hat, shape), _unflat(fs_hat, sshape)
+    swapped, inf = style_swap(wc_feat, ws_feat, patch_size, stride, return_info=True, idx=idx)
     assert swapped.shape[1:3] == shape[:2], "style swap changed the encoding size (wct.py:84-90 refits the content for stride > 1)"
     ss, _ = _flat(swapped)
     fcs_hat = (Es[:, :k_s] * np.sqrt(ws[:k_s])) @ Es[:, :k_s].T @ ss + ms
     out = _unflat(dt.type(alpha) * fcs_hat + dt.type(1 - alpha) * (fc + mc), shape)
     if return_info:
-        inf.update(k_c=k_c, k_s=k_s, wc=wc, ws=ws)
+        inf.update(k_c=k_c, k_s=k_s, wc=wc, ws=ws, wc_feat=wc_feat, ws_feat=ws_feat)
         return out, inf
     return out
 

@@ -54,6 +54,24 @@ def test_adain_matches_definition():
     assert np.allclose(y2, 0.25 * y1 + 0.75 * c)
 
 
+@pytest.mark.parametrize("patch,stride,hw", [(3, 1, (9, 11)), (3, 2, (9, 11)), (5, 2, (11, 9))])
+def test_style_swap_given_idx_equals_own_argmax(patch, stride, hw):
+    """``idx`` set to the oracle's own arg-max reproduces the default output bit for bit; another map changes it."""
+    rng = np.random.default_rng(patch + stride)
+    c = np.maximum(rng.standard_normal((1, hw[0], hw[1], 64)) + 0.3, 0)
+    s = np.maximum(rng.standard_normal((1, 10, 12, 64)) + 0.4, 0)
+    ref, info = ref_ops.wct_style_swap(c, s, 0.6, patch, stride, return_info=True)
+    got, ginfo = ref_ops.wct_style_swap(c, s, 0.6, patch, stride, return_info=True, idx=info["idx"])
+    assert np.array_equal(got, ref) and np.array_equal(ginfo["idx"], info["idx"]) and "scores" not in ginfo
+    for key in ("wc_feat", "ws_feat"):
+        assert np.array_equal(ginfo[key], info[key])
+    assert info["wc_feat"].shape == c.shape and info["ws_feat"].shape == s.shape
+    other = (info["idx"] + 1) % info["scores"].shape[2]
+    assert not np.array_equal(ref_ops.wct_style_swap(c, s, 0.6, patch, stride, idx=other), ref)
+    assert np.array_equal(ref_ops.style_swap(info["wc_feat"], info["ws_feat"], patch, stride, idx=info["idx"]),
+                          ref_ops.style_swap(info["wc_feat"], info["ws_feat"], patch, stride))
+
+
 def test_decoder_layer_names_match_reference_table():
     # model.py:283-298: relu5_1 -> layers 0..15 + output 16 (convs and upsamples both counted)
     l5 = nets.decoder_layers("relu5_1")

@@ -89,6 +89,7 @@ DEBUG_SIGNATURES = {
     "wctb200_debug_set_matfun": (_i, [_i, _i]),
     "wctb200_debug_matfun": (_i, [_vp, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp]),
     "wctb200_debug_set_cov_stages": (_i, [_i]),
+    "wctb200_debug_style_swap_layout": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, C.POINTER(C.c_longlong)]),
 }
 
 _lib = None

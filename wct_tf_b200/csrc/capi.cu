@@ -105,6 +105,7 @@ int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int pa
 int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
                             int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
                             cudaStream_t st);
+void style_swap_debug_layout(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, long long* out);
 size_t wct_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_cs, size_t* off_k);
 size_t adain_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_var);
 int launch_adain_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, void* state, cudaStream_t st);
@@ -542,6 +543,13 @@ int wctb200_debug_set_matfun(int mode, int max_it) {
     if (mode == 0 || mode == 1) g_matfun = mode;
     if (max_it >= 1 && max_it <= 64) g_matfun_max_it = max_it;
     return g_matfun;
+}
+int wctb200_debug_style_swap_layout(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride, long long* out) {
+    WCTB_REQUIRE(out, "debug_style_swap_layout: null pointer");
+    WCTB_REQUIRE(swap_style_ok(C, Hs, Ws, patch, stride) && geom_ok(Nc, Hc, Wc, C) && Hc >= patch && Wc >= patch,
+                 "debug_style_swap_layout: bad geometry");
+    style_swap_debug_layout(C, Nc, Hc, Wc, Hs, Ws, patch, stride, out);
+    return 0;
 }
 int wctb200_debug_set_conv_head_tc(int on) {
     if (on == 0 || on == 1) g_conv_head_tc = on;

@@ -1642,6 +1642,15 @@ static SwapApplyWs swap_apply_layout(int C, int Nc, int Hc, int Wc, int P, int S
     L.total = o;
     return L;
 }
+// where the stages of one prepare + apply leave their results (wctb200_debug_style_swap_layout: tests read them back)
+void style_swap_debug_layout(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, long long* out) {
+    const SwapState SL = swap_state_layout(C, Hs, Ws, P, S);
+    const SwapApplyWs AL = swap_apply_layout(C, Nc, Hc, Wc, P, S, SL.cout_pad);
+    const long long v[11] = {SL.n_patches, SL.cout_pad, AL.ho, AL.wo, (long long)SL.feat, (long long)SL.norms,
+                             (long long)SL.wsplit, (long long)AL.wc_feat, (long long)AL.scores, (long long)AL.idx,
+                             (long long)AL.ss_feat};
+    for (int i = 0; i < 11; ++i) out[i] = v[i];
+}
 size_t style_swap_state_bytes(int C, int Hs, int Ws, int P, int S) { return swap_state_layout(C, Hs, Ws, P, S).total; }
 size_t style_swap_prepare_workspace_bytes(int C) { return swap_prep_layout(C).total; }
 size_t style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {

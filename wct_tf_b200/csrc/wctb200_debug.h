@@ -35,6 +35,13 @@ WCTB200_API int wctb200_debug_matfun(const float* A, int C, int count, int n_fir
                                      float* info, void* stream);
 /* encoder head (3 -> 64): 1 = tensor cores with an operand built in shared memory (conv_head_tc.cu, default), 0 = SIMT */
 WCTB200_API int wctb200_debug_set_conv_head_tc(int on);
+/* where wctb200_style_swap_prepare / _apply leave each stage's result, for reading back after the apply (no stage
+ * overwrites another's).  out[11] = n_patches, cout_pad, ho, wo (the VALID score grid), then byte offsets
+ *   into the state:           whitened style SPF16 [1,Hs,Ws,C] | fp32 1/||tap|| [P*P][C] | split-fp16 filters [2][cout_pad][P*P*C]
+ *   into the apply workspace: whitened content SPF16 [Nc,Hc,Wc,C] | scores SPF16 [Nc,Hc,Wc,cout_pad] (the top-left anchored
+ *                             correlation at every pixel) | int32 arg-max [Nc][ho][wo] | gathered feature SPF16 [Nc,Hc,Wc,C] */
+WCTB200_API int wctb200_debug_style_swap_layout(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride,
+                                                long long* out);
 #ifdef __cplusplus
 }
 #endif
