@@ -313,6 +313,15 @@ WCTB200_API size_t wctb200_style_swap_apply_workspace_bytes(int C, int Nc, int H
 WCTB200_API int wctb200_style_swap_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state,
                              int Hs, int Ws, int patch, int stride, float alpha, float eps_cov, float thresh,
                              void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* stream);
+/*
+ * The apply also runs in less workspace, down to wctb200_style_swap_apply_min_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch,
+ * stride) (0 for a bad geometry): it then correlates the patches in chunks, each the largest multiple of the correlation's N
+ * tile that fits, and keeps a running first arg-max across them.  The output and k_out are byte-identical for every workspace
+ * size from that minimum up; from wctb200_style_swap_apply_workspace_bytes up the apply runs in one chunk.  Less than the
+ * minimum is WCTB200_EWS.  This is what makes the swap affordable at the finer levels (relu3_1 of a 512^2 image has 15 876
+ * patches: about 1.1 GB of scores per frame in one chunk).
+ */
+WCTB200_API size_t wctb200_style_swap_apply_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride);
 
 /* Stand-alone pieces of the transform, exposed for parity tests and profiling:
  * per-channel mean [N][C] and covariance [N][C][C] = fc fc^T/(HW-1) + eps_cov*I of a feature batch

@@ -6,7 +6,7 @@ per style to ``--out-path``.  ``stylize.py`` and ``stylize_video.py`` take these
       --style-path STYLES --out-path PREPARED [--style-size S] [--crop-size C] [--semantics tf|np]
 
 A file holds the (resized, cropped) style image, the WCT and AdaIN statistics of every target and the relu5_1 feature (for
-``--swap5``).  It serves any model with the same encoder weights and semantics, whatever its decoders, and any subset of
+``--swap5``), and with ``--swap-targets reluX_1 ...`` the feature of those levels too (for ``--swap-targets``).  It serves any model with the same encoder weights and semantics, whatever its decoders, and any subset of
 its targets; the model refuses it otherwise.
 """
 from __future__ import print_function
@@ -29,6 +29,8 @@ def build_parser():
     parser.add_argument("--style-size", type=int, default=0, help="short side of the style before cropping (0: keep)")
     parser.add_argument("--crop-size", type=int, default=0, help="centre-crop the style to a square of this size (0: off)")
     parser.add_argument("--out-path", type=str, required=True, help="folder that receives <stem>.wctstyle")
+    parser.add_argument("--swap-targets", nargs="+", type=str, default=None, metavar="RELU",
+                        help="also keep the style feature of these --relu-targets levels, for the style swap there")
     return parser
 
 
@@ -38,7 +40,11 @@ def output_name(style_path):
 
 def main(argv=None, model_factory=None, image_ops=None):
     import stylize
-    args = build_parser().parse_args(argv)
+    parser = build_parser()
+    args = parser.parse_args(argv)
+    for relu in args.swap_targets or []:
+        if relu not in args.relu_targets:
+            parser.error("--swap-targets: %s is not one of --relu-targets (%s)" % (relu, " ".join(args.relu_targets)))
     from wct_tf_b200 import imageio as io
     if image_ops is None:
         from wct_tf_b200 import device_image as image_ops
@@ -55,7 +61,8 @@ def main(argv=None, model_factory=None, image_ops=None):
         if args.crop_size > 0:
             img = image_ops.center_crop(img, args.crop_size)
         target = os.path.join(args.out_path, output_name(path))
-        model.prepare_style(img).save(target)
+        kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
+        model.prepare_style(img, **kw).save(target)
         print("Prepared {} -> {}".format(path, target))
     print("Prepared {} styles in {:.2f}s".format(len(styles), time.time() - t0))
     return len(styles)

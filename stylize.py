@@ -57,6 +57,8 @@ _FLAGS = [
     (("--concat",), dict(action="store_true", default=False, help="write [style | result] side by side")),
     (("--adain",), dict(action="store_true", default=False, help="AdaIN statistics matching instead of WCT")),
     (("--swap5",), dict(action="store_true", default=False, help="style swap at relu5_1 (patch 3, stride 1)")),
+    (("--swap-targets",), dict(nargs="+", type=str, default=None, metavar="RELU",
+                               help="style swap at these --relu-targets levels (e.g. relu3_1 for brush strokes); not with --swap5")),
     (("--ss-alpha",), dict(type=float, default=0.6, help="blend of the style-swapped feature")),
     (("--ss-patch-size",), dict(type=int, default=3)),
     (("--ss-stride",), dict(type=int, default=1)),
@@ -80,10 +82,10 @@ _NOISE_DEFAULTS = [("noise_size", [512, 512]), ("noise_count", 1), ("noise_seed"
 
 # flags that do not combine with --content-mask
 _MASK_EXCLUDES = [("style_path", "--style-path"), ("adain", "--adain"), ("swap5", "--swap5"), ("concat", "--concat"),
-                  ("random", "-r/--random")]
+                  ("random", "-r/--random"), ("swap_targets", "--swap-targets")]
 # flags that do not combine with --interp-styles
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("random", "-r/--random"), ("swap5", "--swap5"), ("concat", "--concat"),
-                    ("content_mask", "--content-mask")]
+                    ("content_mask", "--content-mask"), ("swap_targets", "--swap-targets")]
 
 
 def build_parser():
@@ -96,6 +98,7 @@ def build_parser():
 def parse_args(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
+    check_swap_flags(parser, args)
     check_interp_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
@@ -111,6 +114,17 @@ def parse_args(argv=None):
     check_noise_flags(parser, args)
     check_prepared_flags(parser, args)
     return args
+
+
+def check_swap_flags(parser, args):
+    """--swap-targets: levels of --relu-targets, not with --swap5 (which is --swap-targets relu5_1)."""
+    if args.swap_targets is None:
+        return
+    if args.swap5:
+        parser.error("--swap-targets does not combine with --swap5 (--swap5 is --swap-targets relu5_1)")
+    for relu in args.swap_targets:
+        if relu not in (args.relu_targets or []):
+            parser.error("--swap-targets: %s is not one of --relu-targets (%s)" % (relu, " ".join(args.relu_targets or [])))
 
 
 def check_style_mask_flags(parser, args):
@@ -286,6 +300,8 @@ def _prepare_style(path, args, io, dimg, content_dev, device, prepared=None):
 def _stylize_pair(model, content_dev, style_dev, args):
     """stylize.py:100-104; every pass takes and returns uint8 frames on the device (no host round trip between passes)."""
     kw = dict(alpha=args.alpha, swap5=args.swap5, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True)
+    if args.swap_targets:
+        kw["swap_targets"] = list(args.swap_targets)
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, style_dev, **kw)

@@ -41,9 +41,10 @@ _VIDEO_FLAGS = [
 ]
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
-           "--synthetic-weights", "--interp-styles", "--interp-weights")
+           "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets")
 # flags that do not combine with --interp-styles
-_INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat")]
+_INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat"),
+                    ("swap_targets", "--swap-targets")]
 
 
 def build_parser():
@@ -62,6 +63,7 @@ def parse_args(argv=None):
     import stylize
     parser = build_parser()
     args = parser.parse_args(argv)
+    stylize.check_swap_flags(parser, args)
     if args.morph:
         if args.interp_styles is None:
             parser.error("--morph needs --interp-styles")
@@ -146,6 +148,8 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
             # --passes (stylize_video.py:119-121) run back to back on the device; a style swap acts in the first pass and
             # swaps the whole batch against the one style in one call
             swap_kw = dict(swap5=True, ss_alpha=args.ss_alpha) if args.swap5 else {}
+            if args.swap_targets:
+                swap_kw = dict(swap_targets=list(args.swap_targets), ss_alpha=args.ss_alpha)
             one = weights is not None or not hasattr(style_img, "shape")   # a list of styles, or a prepared style
             out = wct_model.predict_batch(x, style_img if one else style_img[None], alpha=args.alpha,
                                           adain=args.adain, passes=args.passes, return_device=True,
@@ -158,7 +162,8 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 style_rgb = coral(style_img, fr) if args.keep_colors else style_img
                 kw = dict(alpha=args.alpha, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True,
                           **interp_kw(first + j, first + j + 1))
-                o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, **kw)
+                swap_kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
+                o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, **dict(kw, **swap_kw))
                 for _ in range(args.passes - 1):
                     o = wct_model.predict_batch(o, style_rgb, swap5=False, **kw)
                 results.append((o[0], style_rgb))

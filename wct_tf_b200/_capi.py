@@ -73,6 +73,7 @@ SIGNATURES = {
     "wctb200_style_swap_prepare_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "wctb200_style_swap_prepare": (_i, [_vp, _i, _i, _i, _i, _i, _f, _f, _vp, _vp, _vp, _sz, _vp]),
     "wctb200_style_swap_apply_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i, _i]),
+    "wctb200_style_swap_apply_min_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i, _i]),
     "wctb200_style_swap_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _vp, _sz, _vp]),
 }
 

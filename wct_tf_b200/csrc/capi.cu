@@ -100,6 +100,7 @@ int launch_style_swap_level(const __half* content, int Hc, int Wc, const __half*
 size_t style_swap_state_bytes(int C, int Hs, int Ws, int P, int S);
 size_t style_swap_prepare_workspace_bytes(int C);
 size_t style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S);
+size_t style_swap_apply_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S);
 int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int patch, int stride, float eps_cov, float thresh,
                               void* state, int32_t* k_out, void* ws, size_t ws_bytes, cudaStream_t st);
 int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
@@ -473,6 +474,10 @@ int wctb200_style_swap_prepare(const void* style, int Hs, int Ws, int C, int pat
 size_t wctb200_style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride) {
     if (!swap_style_ok(C, Hs, Ws, patch, stride) || !geom_ok(Nc, Hc, Wc, C) || Hc < patch || Wc < patch) return 0;
     return style_swap_apply_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride);
+}
+size_t wctb200_style_swap_apply_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride) {
+    if (!swap_style_ok(C, Hs, Ws, patch, stride) || !geom_ok(Nc, Hc, Wc, C) || Hc < patch || Wc < patch) return 0;
+    return style_swap_apply_min_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride);
 }
 int wctb200_style_swap_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch, int stride,
                              float alpha, float eps_cov, float thresh, void* out, int32_t* k_out, void* ws, size_t ws_bytes,

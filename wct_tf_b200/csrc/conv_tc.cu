@@ -652,9 +652,17 @@ int g_conv_bn_override = 0;  // test/tuning hook: force the N tile (64/128; 256 
 // mode CONV_TAPS : in [N,H,W,Cin], w_split [2][Cout][kw*kw*Cin],      out [N,H,W,Cout]: top-left anchored kw x kw correlation
 // regions (spatial control, CONV_APPLY with C = Cin = Cout): w_split [N*R][2][C][C], bias [N*R][C]; labels / counts / amask
 // as in ConvParams
+// N tile of a conv with Cout output channels: 128 when it divides Cout (or the test hook's forced tile)
+int conv_tc_bn(int Cout) {
+    int BN = Cout % 128 == 0 ? 128 : 64;
+    if (g_conv_bn_override && Cout % g_conv_bn_override == 0) BN = g_conv_bn_override > 128 ? 128 : g_conv_bn_override;
+    return BN;
+}
+
 static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
                         const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw,
-                        const uint8_t* labels, const int* counts, const uint16_t* amask, int R) {
+                        const uint8_t* labels, const int* counts, const uint16_t* amask, int R, int bn_req = 0,
+                        long long wplane = 0) {
     const bool reg = labels != nullptr;
     WCTB_REQUIRE(!reg || (mode == CONV_APPLY && Cin == Cout && nsets == N * R && flags == 0), "conv: bad regions apply");
     if (reg) nsets = N;                                   // per-image tiling; the region picks the set inside an image
@@ -672,8 +680,8 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
     const bool pool = (flags & WCTB200_POOL2) != 0;
     WCTB_REQUIRE(!pool || (mode == CONV_3X3 && (H + 1) / 2 >= 2 && (W + 1) / 2 >= 2), "conv: POOL2 needs the 3x3 mode and a pooled output >= 2x2");
     // N tile: at most 128 (a 64 x 256 fp32 chunk plus the running sum would not fit a warpgroup's registers)
-    int BN = Cout % 128 == 0 ? 128 : 64;
-    if (g_conv_bn_override && Cout % g_conv_bn_override == 0) BN = g_conv_bn_override > 128 ? 128 : g_conv_bn_override;
+    int BN = bn_req ? bn_req : conv_tc_bn(Cout);
+    WCTB_REQUIRE((BN == 64 || BN == 128) && Cout % BN == 0, "conv: N tile %d does not divide Cout=%d", BN, Cout);
 
     // one strip box per (filter row, channel slice) holds the rows of all its column taps
     const int ncol = mode == CONV_3X3 ? 3 : (mode == CONV_UP2 ? 2 : (mode == CONV_TAPS ? kw : 1));
@@ -683,7 +691,10 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
                                 (uint32_t)strip_rows);
     if (rc) return rc;
     const uint64_t K = (uint64_t)taps * Cin;
-    rc = make_tensor_map_3d(&mB, w_split, K, (uint64_t)Cout, (uint64_t)2 * wsets, K * 2, K * Cout * 2, (uint32_t)BN);
+    // weight planes [2 * wsets][Cout][K]; a slice of the rows of a larger filter bank keeps that bank's plane stride
+    const uint64_t wstride = wplane ? (uint64_t)wplane : K * Cout;
+    WCTB_REQUIRE(wstride >= K * Cout, "conv: weight plane stride %llu < %llu", (unsigned long long)wstride, (unsigned long long)(K * Cout));
+    rc = make_tensor_map_3d(&mB, w_split, K, (uint64_t)Cout, (uint64_t)2 * wsets, K * 2, wstride * 2, (uint32_t)BN);
     if (rc) return rc;
 
     ConvParams p;
@@ -735,6 +746,14 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
 int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
                    const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw) {
     return conv_tc_impl(mode, in, N, H, W, Cin, w_split, nsets, wscale, bias, Cout, flags, out, st, kw, nullptr, nullptr, nullptr, 1);
+}
+// CONV_TAPS over output channels [n0, n0 + Cout) of a bank of `wplane / (kw*kw*Cin)` filters: w_split points at row n0 of the
+// hi plane, the lo plane sits `wplane` elements further, and the N tile is `bn` (the bank's own, so that every output element
+// runs the same kernel variant and k order as in one launch over the whole bank)
+int launch_conv_taps_rows(const __half* in, int N, int H, int W, int Cin, const __half* w_split, long long wplane, int Cout, int bn,
+                          __half* out, cudaStream_t st, int kw) {
+    return conv_tc_impl(CONV_TAPS, in, N, H, W, Cin, w_split, 1, nullptr, nullptr, Cout, 0, out, st, kw, nullptr, nullptr, nullptr, 1,
+                        bn, wplane);
 }
 // out = M_{n,r} x + bias_{n,r} for the pixels of region r of image n, out = x for the rest (wct.cu: launch_wct_apply_regions)
 int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const uint8_t* labels,

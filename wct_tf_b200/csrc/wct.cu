@@ -1620,12 +1620,14 @@ static SwapPrepWs swap_prep_layout(int C) {
     return L;
 }
 // workspace of the apply over Nc frames: the content side (wct_layout(C, Nc, 0): per-frame whitening operands), the
-// whitened, swapped and coloured features, the correlation scores and the arg-max per VALID position
+// whitened, swapped and coloured features, the correlation scores of `cols` patches (all cout_pad of them in one chunk, or
+// one chunk of them) and the arg-max per VALID position.  The running best score of a chunked arg-max lives in `tmp`,
+// which only the colouring after the gather writes.
 struct SwapApplyWs {
     size_t base, zeros, idx, wc_feat, ss_feat, tmp, scores, total;
     int ho, wo;                                     // content score grid ho x wo
 };
-static SwapApplyWs swap_apply_layout(int C, int Nc, int Hc, int Wc, int P, int S, int cout_pad) {
+static SwapApplyWs swap_apply_layout(int C, int Nc, int Hc, int Wc, int P, int S, int cols) {
     SwapApplyWs L;
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
@@ -1638,7 +1640,7 @@ static SwapApplyWs swap_apply_layout(int C, int Nc, int Hc, int Wc, int P, int S
     L.wc_feat = take(fc);
     L.ss_feat = take(fc);
     L.tmp = take(fc);
-    L.scores = take((size_t)ActGeom(Nc, Hc, Wc, cout_pad).plane * 2 * sizeof(__half));
+    L.scores = take((size_t)ActGeom(Nc, Hc, Wc, cols).plane * 2 * sizeof(__half));
     L.total = o;
     return L;
 }
@@ -1655,6 +1657,10 @@ size_t style_swap_state_bytes(int C, int Hs, int Ws, int P, int S) { return swap
 size_t style_swap_prepare_workspace_bytes(int C) { return swap_prep_layout(C).total; }
 size_t style_swap_apply_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {
     return swap_apply_layout(C, Nc, Hc, Wc, P, S, swap_state_layout(C, Hs, Ws, P, S).cout_pad).total;
+}
+// the chunked apply's least workspace: a score buffer one N tile of the whole correlation wide
+size_t style_swap_apply_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    return swap_apply_layout(C, Nc, Hc, Wc, P, S, conv_tc_bn(swap_state_layout(C, Hs, Ws, P, S).cout_pad)).total;
 }
 // style_swap_level: the state, then the prepare's or the apply's workspace
 size_t style_swap_workspace_bytes(int C, int Hc, int Wc, int Hs, int Ws, int P, int S) {
@@ -1702,17 +1708,22 @@ __global__ void k_swap_patch_weights(const __half* __restrict__ feat, ActGeom g,
 // first arg-max over the patch axis for every VALID strided position (y,x) of frame blockIdx.y: the top-left-anchored P x P
 // correlation at interior pixel (y*S, x*S), which the conv kernel stored at that pixel's own padded cell.  A VALID anchor
 // reads padded rows y*S+1 .. y*S+P <= H of its own frame only, so a batch of frames in one correlation keeps them apart.
-__global__ void k_swap_argmax(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n_patches, int* __restrict__ idx) {
+// The scores hold the chunk of patches [n0, n0 + g.C) (g.C = the chunk's width); patches >= n_patches are padding.  The
+// first chunk (n0 = 0) sets (best, idx); a later one replaces them only where its own first maximum is strictly greater,
+// so after the last chunk idx is the first maximum over all patches, whatever the chunking.
+__global__ void k_swap_argmax(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n0, int n_patches,
+                              float* __restrict__ best_run, int* __restrict__ idx) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= q.ho * q.wo) return;
     const int n = blockIdx.y;
     const int y = warp / q.wo, x = warp - y * q.wo;
     const long long pos = ((long long)n * g.Hp + y * q.S + 1) * g.Wp + (x * q.S + 1);
+    const int cols = min(g.C, n_patches - n0);
     float best = -INFINITY;
     int bi = 0x7fffffff;
-    for (int n = lane; n < n_patches; n += 32) {
-        const float v = merge_f32(scores[pos * g.C + n], scores[g.plane + pos * g.C + n]);
-        if (v > best) { best = v; bi = n; }                       // strictly greater: keeps the first maximum of this lane
+    for (int j = lane; j < cols; j += 32) {
+        const float v = merge_f32(scores[pos * g.C + j], scores[g.plane + pos * g.C + j]);
+        if (v > best) { best = v; bi = n0 + j; }                  // strictly greater: keeps the first maximum of this lane
     }
 #pragma unroll
     for (int o = 16; o >= 1; o >>= 1) {
@@ -1720,7 +1731,13 @@ __global__ void k_swap_argmax(const __half* __restrict__ scores, ActGeom g, Swap
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
         if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
     }
-    if (lane == 0) idx[(long long)n * q.ho * q.wo + warp] = bi;
+    if (lane == 0) {
+        const long long o = (long long)n * q.ho * q.wo + warp;
+        if (n0 == 0 || best > best_run[o]) {
+            best_run[o] = best;
+            idx[o] = bi;
+        }
+    }
 }
 // conv2d_transpose of the one-hot map with the raw patches, divided by the overlap count (ops.py:255-276): output pixel
 // (Y,X) averages, over the <= P*P patch positions (py,px) with py*S + dy = Y, px*S + dx = X that cover it, the style
@@ -1884,9 +1901,21 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
     WCTB_REQUIRE((AL.ho - 1) * stride + patch == Hc && (AL.wo - 1) * stride + patch == Wc,
                  "style_swap: patch %d / stride %d does not tile a %dx%d encoding (refit the content: swap_filter_fit, wct.py:84-90)",
                  patch, stride, Hc, Wc);
+    // chunk width: all cout_pad patches when the workspace holds their scores, else the largest multiple of the whole
+    // correlation's N tile that fits (the same tile, hence the same kernel variant and k order, for every chunk)
+    const int BN = conv_tc_bn(SL.cout_pad);
+    int cols = SL.cout_pad;
     if (ws_bytes < AL.total) {
-        set_error("style_swap_apply: workspace %zu < %zu bytes", ws_bytes, AL.total);
-        return WCTB200_EWS;
+        const size_t col_bytes = (size_t)ActGeom(Nc, Hc, Wc, 1).plane * 2 * sizeof(__half);
+        const size_t avail = ws_bytes > AL.scores ? ws_bytes - AL.scores : 0;
+        const size_t fit = avail / col_bytes / BN * BN;
+        cols = (int)(fit < (size_t)SL.cout_pad ? fit : (size_t)SL.cout_pad);
+        while (cols >= BN && swap_apply_layout(C, Nc, Hc, Wc, patch, stride, cols).total > ws_bytes) cols -= BN;
+        if (cols < BN) {
+            set_error("style_swap_apply: workspace %zu < %zu bytes", ws_bytes,
+                      swap_apply_layout(C, Nc, Hc, Wc, patch, stride, BN).total);
+            return WCTB200_EWS;
+        }
     }
     const SwapGeom q = {patch, stride, SL.prow, SL.pcol, AL.ho, AL.wo};
     uint8_t* sw = static_cast<uint8_t*>(ws);
@@ -1929,14 +1958,21 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
     rc = launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, msplit, Nc, nullptr, bias, C, 0, wc_feat, st);
     if (rc) return rc;
     // every style patch is a filter: the P x P correlation of all frames (top-left anchored, all positions; the strided VALID
-    // subset is read by the arg-max) runs on the tensor-core conv kernel
-    rc = launch_conv_tc(CONV_TAPS, wc_feat, Nc, Hc, Wc, C, reinterpret_cast<const __half*>(sp + SL.wsplit), 1, nullptr, nullptr,
-                        SL.cout_pad, 0, scores, st, patch);
-    if (rc) return rc;
+    // subset is read by the arg-max) runs on the tensor-core conv kernel, `cols` filters (rows n0.. of the state's filter
+    // planes, read in place) per chunk
+    const long long K = (long long)patch * patch * C;
+    const __half* wsplit = reinterpret_cast<const __half*>(sp + SL.wsplit);
+    float* best_run = reinterpret_cast<float*>(tmp);
     const int npos = AL.ho * AL.wo;
-    k_swap_argmax<<<dim3((unsigned)cdiv((long long)npos * 32, 256), (unsigned)Nc), 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, SL.cout_pad),
-                                                                                                q, SL.n_patches, idx);
-    WCTB_CHECK_LAUNCH("k_swap_argmax");
+    for (int n0 = 0; n0 < SL.cout_pad; n0 += cols) {
+        const int m = SL.cout_pad - n0 < cols ? SL.cout_pad - n0 : cols;
+        rc = launch_conv_taps_rows(wc_feat, Nc, Hc, Wc, C, wsplit + (long long)n0 * K, (long long)SL.cout_pad * K, m, BN, scores, st,
+                                   patch);
+        if (rc) return rc;
+        k_swap_argmax<<<dim3((unsigned)cdiv((long long)npos * 32, 256), (unsigned)Nc), 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m),
+                                                                                                    q, n0, SL.n_patches, best_run, idx);
+        WCTB_CHECK_LAUNCH("k_swap_argmax");
+    }
     k_swap_gather<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(reinterpret_cast<const __half*>(sp + SL.feat), gs, q,
                                                                                      idx, gc, ss_feat);
     WCTB_CHECK_LAUNCH("k_swap_gather");

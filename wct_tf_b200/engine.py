@@ -20,6 +20,11 @@ SEMANTICS = {
     "np": dict(eps_cov=0.0, eps_eig=1e-5, thresh=1e-5, readd=0),
 }
 
+# Workspace of one style-swap apply: all of its scores when they fit this size, else at least one N tile of them.  The
+# apply then correlates the patches in chunks; the output is the same byte for byte (wctb200_style_swap_apply_min_workspace_
+# bytes).  At 512^2 a relu5_1 swap (4.4 MB of scores per frame) runs in one chunk, a relu3_1 swap (1.08 GB) in two.
+SWAP_WORKSPACE_BYTES = 1 << 30
+
 
 class Act(object):
     """SPF16 activation: device buffer + logical NHWC shape."""
@@ -328,6 +333,10 @@ class Engine(object):
         if nbytes == 0:
             raise ValueError("style swap needs encodings of at least %dx%d (content %dx%d, style %dx%d)"
                              % (patch, patch, content.H, content.W, Hs, Ws))
+        # the scores of the patch correlation are produced in chunks when they would not fit SWAP_WORKSPACE_BYTES; every
+        # chunking gives the same bytes (include/wctb200.h: wctb200_style_swap_apply_min_workspace_bytes)
+        least = self.lib.wctb200_style_swap_apply_min_workspace_bytes(C, N, content.H, content.W, Hs, Ws, int(patch), int(stride))
+        nbytes = min(nbytes, max(least, SWAP_WORKSPACE_BYTES))
         ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         kbuf = torch.empty(N + 1, dtype=torch.int32, device=self.device) if want_info else None
         sem = SEMANTICS["tf"]
@@ -464,9 +473,23 @@ class Engine(object):
         return out, None
 
     # ------------------------------------------------------------------ pipeline
+    def swap_levels(self, swap5=False, swap_targets=None):
+        """The relu levels a call swaps at: ``swap_targets`` (checked against this model's targets), or relu5_1 for
+        ``swap5`` when it is a target (model.py:148).  ValueError for both at once or a level that is not a target."""
+        have = [l.relu_target for l in self.model.levels]
+        if swap_targets is None:
+            return ("relu5_1",) if swap5 and "relu5_1" in have else ()
+        if swap5:
+            raise ValueError("give swap5 or swap_targets, not both (swap5 is swap_targets=['relu5_1'])")
+        levels = tuple(dict.fromkeys(str(r) for r in swap_targets))
+        for relu in levels:
+            if relu not in have:
+                raise ValueError("swap_targets: %s is not a relu target of this model (%s)" % (relu, ", ".join(have)))
+        return levels
+
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
-                region_masks=None):
+                region_masks=None, swap_targets=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -495,13 +518,19 @@ class Engine(object):
         styles of one style each, and ``interp_weights`` a cuda float32 [1|N, K] tensor; ``style_u8`` is ignored.  Frame n is
         stylised with the blend of the K styles under weight row n (one row: every frame), which for a row that sums to 1 is
         the same blend of the K single-style outputs at every level (WCT and AdaIN are affine in the style statistics).  The
-        weights are used as given.  The K styles are encoded and prepared once per call."""
+        weights are used as given.  The K styles are encoded and prepared once per call.
+
+        Style swap at any level: ``swap_targets`` is a list of relu targets at which the style swap replaces WCT / AdaIN,
+        with ``ss_alpha``, ``ss_patch_size`` and ``ss_stride``; ``swap5`` is ``swap_targets=["relu5_1"]``.  Not with spatial
+        control or interpolation."""
         N = content_u8.shape[0]
+        swap_lv = self.swap_levels(swap5, swap_targets)
+        swap5 = swap5 or swap_targets is not None         # the rejections below name both
         if region_masks is not None and labels is None:
             raise ValueError("style masks (region_masks) need a content label map (labels)")
         if interp_styles is not None:
             if labels is not None or swap5:
-                raise ValueError("style interpolation does not combine with spatial control (labels) or swap5")
+                raise ValueError("style interpolation does not combine with spatial control (labels) or swap5 / swap_targets")
             K = len(interp_styles)
             if not 1 <= K <= 8:
                 raise ValueError("style interpolation needs 1..8 styles, got %d" % K)
@@ -514,7 +543,7 @@ class Engine(object):
                                        lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]))
         if labels is not None:
             if adain or swap5:
-                raise ValueError("spatial control (labels) works with WCT only: not with adain or swap5")
+                raise ValueError("spatial control (labels) works with WCT only: not with adain or swap5 / swap_targets")
             R = len(region_styles) if region_styles is not None else 0
             if not 1 <= R <= 8:
                 raise ValueError("spatial control needs 1..8 region styles, got %d" % R)
@@ -527,35 +556,33 @@ class Engine(object):
                 region_masks = self.check_region_masks(region_masks, region_styles)
             return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
                                        lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks)
-        swap5 = bool(swap5) and "relu5_1" in [l.relu_target for l in self.model.levels]    # model.py:148: only relu5_1 swaps
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
         if n_style not in (1, N):
             raise ValueError("%d styles for %d frames: give one style, or one per frame" % (n_style, N))
         if prepared:
-            self.check_prepared(style_u8, adain, swap5)
+            self.check_prepared(style_u8, adain, swap_lv)
         main = torch.cuda.current_stream(self.device)
-        if swap5 and n_style > 1:
+        if swap_lv and n_style > 1:
             # one style per frame: frame by frame (each frame's swap has its own style side)
             outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
-                                 alpha=alpha, adain=adain, want_info=want_info, swap5=True, ss_alpha=ss_alpha,
+                                 alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
                                  ss_patch_size=ss_patch_size, ss_stride=ss_stride) for i in range(N)]
             return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
-        swap = (int(ss_patch_size), int(ss_stride)) if swap5 else None
+        swap = (int(ss_patch_size), int(ss_stride), swap_lv) if swap_lv else None
         shared = style_u8 if (prepared and n_style == 1) else None
         owned = None
-        if n_style == 1 and not prepared and (G > 1 or swap5):
+        if n_style == 1 and not prepared and (G > 1 or swap_lv):
             # ONE style for the whole batch (video, configs[2]): its encoder pass and per-level states are made once, every
             # sub-batch group waits for the per-level events
             self._group = 1 if G > 1 else 0
             try:
-                owned = shared = self._style_side(style_u8, main, wct=not adain, adain=adain, keep5=swap5,
-                                                  skip=("relu5_1",) if swap5 else ())
+                owned = shared = self._style_side(style_u8, main, wct=not adain, adain=adain, keep=swap_lv, skip=swap_lv)
             finally:
                 self._group = 0
-        if swap is not None:
-            self.swap_state(shared, *swap)
+        for relu in swap_lv:
+            self.swap_state(shared, relu, *swap[:2])
         if G > 1:
             def run(lo, hi):
                 if shared is not None:
@@ -634,7 +661,7 @@ class Engine(object):
             if isinstance(s, PreparedStyle):
                 if s.n != 1:
                     raise ValueError("each region / interpolated style must be one style, got a prepared style of %d" % s.n)
-                self.check_prepared(s, adain, False)
+                self.check_prepared(s, adain)
                 sides.append(s)
             elif masks is None:
                 owned.append(self._style_side(s, main, wct=not adain, adain=adain))
@@ -692,10 +719,11 @@ class Engine(object):
             self._style_streams[self._group] = torch.cuda.Stream(device=self.device, priority=prio)
         return self._style_streams[self._group]
 
-    def _style_side(self, style_u8, main, wct=True, adain=False, keep5=False, skip=(), labels=None, R=0):
+    def _style_side(self, style_u8, main, wct=True, adain=False, keep=(), skip=(), labels=None, R=0):
         """The prepare step: style side of one call (model.py:70-72: ONE encoder pass emitting every target; per level the
         WCT state of ops.py:48-55,76 when ``wct``, the AdaIN moments when ``adain``; levels in ``skip`` get neither), enqueued
-        on this group's style stream when overlap is on.  ``keep5`` keeps the relu5_1 feature (the style swap).  Returns a
+        on this group's style stream when overlap is on.  ``keep`` lists the levels whose feature it keeps (the style
+        swap is prepared from them).  Returns a
         ``PreparedStyle`` with one event per level.
 
         With ``labels`` (a style mask, cuda uint8 [1,Hm,Wm] of one style) the WCT state of each level is the masked prepare
@@ -733,30 +761,33 @@ class Engine(object):
                 ev = torch.cuda.Event()
                 ev.record(side)
                 ps.events[relu] = ev
-            if keep5 and "relu5_1" in feats:
-                ps.feat5 = feats["relu5_1"]
+            for relu in keep:
+                if relu in feats:
+                    ps.feats[relu] = feats[relu]
             self._tag = tag
         return ps
 
-    def prepare(self, style_u8):
+    def prepare(self, style_u8, swap_targets=()):
         """Every part of the style side of ``style_u8`` (cuda uint8 [n,Hs,Ws,3]): WCT states and AdaIN moments of every
-        target, and the relu5_1 feature when relu5_1 is a target."""
+        target, and the feature of relu5_1 (when it is a target) and of every level of ``swap_targets``."""
         main = torch.cuda.current_stream(self.device)
-        ps = self._style_side(style_u8, main, wct=True, adain=True, keep5=True)
+        keep = ("relu5_1",) + tuple(r for r in self.swap_levels(False, list(swap_targets)) if r != "relu5_1")
+        ps = self._style_side(style_u8, main, wct=True, adain=True, keep=keep)
         style_u8.record_stream(ps.side)        # read on the style stream after the caller may have dropped it
         ps.record_stream(main)
         return ps
 
-    def prepare_call(self, style_u8, adain=False, swap5=False):
-        """The style side one call needs (WCT states, or the AdaIN moments; the relu5_1 feature for ``swap5``), made once
-        for a call that applies it several times (passes)."""
+    def prepare_call(self, style_u8, adain=False, swap5=False, swap_targets=None):
+        """The style side one call needs (WCT states, or the AdaIN moments; the features of the swap levels of ``swap5`` /
+        ``swap_targets``), made once for a call that applies it several times (passes)."""
         main = torch.cuda.current_stream(self.device)
-        ps = self._style_side(style_u8, main, wct=not adain, adain=adain, keep5=swap5)
+        ps = self._style_side(style_u8, main, wct=not adain, adain=adain, keep=self.swap_levels(swap5, swap_targets))
         style_u8.record_stream(ps.side)
         return ps
 
-    def check_prepared(self, ps, adain, swap5):
-        """ValueError unless ``ps`` was prepared for this engine's encoder and semantics and covers its targets."""
+    def check_prepared(self, ps, adain, swap=()):
+        """ValueError unless ``ps`` was prepared for this engine's encoder and semantics and covers its targets, with the
+        feature of every level in ``swap`` (the swap levels of the call)."""
         sem = SEMANTICS[self.semantics]
         for k in SEMANTIC_KEYS:
             if float(ps.semantics[k]) != float(sem[k]):
@@ -764,10 +795,11 @@ class Engine(object):
         need = dict.fromkeys(self.model.style_taps)
         have = ps.adain if adain else ps.wct
         for relu in need:
-            if relu not in have and not (swap5 and relu == "relu5_1"):
+            if relu not in have and relu not in swap:
                 raise ValueError("the prepared style has no %s state for %s" % ("AdaIN" if adain else "WCT", relu))
-        if swap5 and ps.feat5 is None:
-            raise ValueError("the prepared style has no relu5_1 feature for the style swap")
+        for relu in swap:
+            if relu not in ps.feats:
+                raise ValueError("the prepared style has no %s feature for the style swap" % relu)
         if ps.fingerprints:
             mine = self.fingerprints()
             for relu in need:
@@ -793,28 +825,27 @@ class Engine(object):
             out.wct[relu] = slice_wct_state(self.lib, st, RELU_CHANNELS[relu], ps.n, lo, hi)
         for relu, st in ps.adain.items():
             out.adain[relu] = slice_adain_state(self.lib, st, RELU_CHANNELS[relu], ps.n, lo, hi)
-        if ps.feat5 is not None:
-            f = ps.feat5
-            out.feat5 = self._act(hi - lo, f.H, f.W, f.C)
-            slice_act_planes(f.buf, f.N, f.H, f.W, f.C, lo, hi, out.feat5.buf)
+        for relu, f in ps.feats.items():
+            out.feats[relu] = self._act(hi - lo, f.H, f.W, f.C)
+            slice_act_planes(f.buf, f.N, f.H, f.W, f.C, lo, hi, out.feats[relu].buf)
         ps.record_stream(cur)
         return out
 
-    def swap_state(self, ps, patch, stride):
-        """The style-swap state of a prepared style of one style for (patch, stride): made on first use from its relu5_1
-        feature (on its style stream when it has one) and cached in it.  Returns (state, event)."""
-        key = (int(patch), int(stride))
+    def swap_state(self, ps, relu, patch, stride):
+        """The style-swap state of a prepared style of one style at level ``relu`` for (patch, stride): made on first use
+        from its feature at that level (on its style stream when it has one) and cached in it.  Returns (state, event)."""
+        key = (relu, int(patch), int(stride))
         if key not in ps.swap:
             main = torch.cuda.current_stream(self.device)
             st = ps.side if ps.side is not None else main
             if st is not main:
                 st.wait_stream(main)
             with torch.cuda.stream(st):
-                ps.wait(st, "relu5_1")
+                ps.wait(st, relu)
                 tag, self._tag = self._tag, "style"
-                state = self.swap_prepare(ps.feat5, *key)
+                state = self.swap_prepare(ps.feats[relu], *key[1:])
                 self._tag = tag
-                ps.feat5.buf.record_stream(st)
+                ps.feats[relu].buf.record_stream(st)
                 ev = torch.cuda.Event()
                 ev.record(st)
             ps.swap[key] = (state, ev)
@@ -822,7 +853,7 @@ class Engine(object):
 
     def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
-        ``swap``: (patch, stride) of the style swap at relu5_1 (its state is made by ``swap_state`` beforehand)."""
+        ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand)."""
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
@@ -846,10 +877,11 @@ class Engine(object):
             relu = lvl.relu_target
             self._tag = relu
             cf, _ = self.encode(x, relu)
-            if swap is not None and relu == "relu5_1":      # model.py:148-152: style swap wins over AdaIN / WCT at relu5_1
-                state, ev = style.swap[swap]
+            if swap is not None and relu in swap[2]:      # model.py:148-152: style swap wins over AdaIN / WCT at its levels
+                state, ev = style.swap[(relu,) + swap[:2]]
                 main.wait_event(ev)
-                f, kbuf = self.swap_apply(cf, state, (style.feat5.H, style.feat5.W), ss_alpha, want_info, *swap)
+                sf = style.feats[relu]
+                f, kbuf = self.swap_apply(cf, state, (sf.H, sf.W), ss_alpha, want_info, *swap[:2])
             else:
                 for sd in sides:
                     if sd.side is not main:

@@ -3,8 +3,8 @@
 The style side -- the VGG encode of the style image and, per relu level, the WCT state (mean ``m_s``, colouring matrix
 ``C_s`` and ``k_s``) and the AdaIN moments -- depends only on the style image, the encoder weights and the semantics.
 A ``PreparedStyle`` holds it on the device for ``n`` styles (one shared style, or one per frame), together with the
-relu5_1 style feature when relu5_1 is a target (the style swap is prepared from it on first use, per patch and stride)
-and the uint8 style image on the host.
+style feature of relu5_1 when it is a target and of every level it was prepared to swap at (the style swap is prepared
+from them on first use, per level, patch and stride) and the uint8 style image on the host.
 
 ``PreparedStyle.save`` / ``load_file`` write and read a ``.wctstyle`` file: an ``np.savez`` container, read with
 ``allow_pickle=False``.  Per level it stores a fingerprint of the encoder weights up to that relu, so a file serves any
@@ -64,13 +64,25 @@ class PreparedStyle(object):
         self.targets = list(targets)              # relu targets the states cover
         self.wct = {}                             # relu -> device uint8 WCT state (wctb200_wct_style_prepare, Ns = n)
         self.adain = {}                           # relu -> device uint8 AdaIN state (wctb200_adain_style_prepare, Ns = n)
-        self.feat5 = None                         # engine.Act: SPF16 relu5_1 style feature [n,Hs,Ws,512] (relu5_1 a target)
+        self.feats = {}                           # relu -> engine.Act: SPF16 style feature [n,Hs,Ws,C] of a swap level
         self.events = {}                          # relu -> torch.cuda.Event recorded when that level's side is complete
         self.side = None                          # stream the side was enqueued on
         self.image = None                         # host uint8 [n,H,W,3] (prepare_style / load_style)
         self.fingerprints = {}                    # relu -> encoder fingerprint (prepare_style / load_style)
-        self.swap = {}                            # (patch, stride[, frame]) -> (device swap state, event)
+        self.swap = {}                            # (relu, patch, stride) -> (device swap state, event)
         self.entries = None                       # style-masked side (Engine._style_side): its n styles, one by one
+
+    @property
+    def feat5(self):
+        """The relu5_1 style feature (``feats["relu5_1"]``), or None."""
+        return self.feats.get("relu5_1")
+
+    @feat5.setter
+    def feat5(self, act):
+        if act is None:
+            self.feats.pop("relu5_1", None)
+        else:
+            self.feats["relu5_1"] = act
 
     def __repr__(self):
         return "PreparedStyle(n=%d, targets=%s)" % (self.n, self.targets)
@@ -84,8 +96,7 @@ class PreparedStyle(object):
 
     def tensors(self):
         ts = list(self.wct.values()) + list(self.adain.values()) + [st for st, _ in self.swap.values()]
-        if self.feat5 is not None:
-            ts.append(self.feat5.buf)
+        ts += [f.buf for f in self.feats.values()]
         return ts
 
     def record_stream(self, stream):
@@ -111,10 +122,9 @@ class PreparedStyle(object):
             am, av = unpack_adain_state(lib, self.adain[relu], C, self.n)
             arrays.update({"%s/fingerprint" % relu: np.array(self.fingerprints[relu]), "%s/wct_mean" % relu: mean,
                            "%s/wct_cs" % relu: cs, "%s/wct_k" % relu: k, "%s/adain_mean" % relu: am, "%s/adain_var" % relu: av})
-        if self.feat5 is not None:
-            f = self.feat5
+        for relu, f in self.feats.items():
             raw = f.buf[: 2 * f.N * (f.H + 2) * (f.W + 2) * f.C * 2].cpu().numpy()
-            arrays["relu5_1/feat"] = raw.view(np.float16).reshape(2, f.N, f.H + 2, f.W + 2, f.C)
+            arrays["%s/feat" % relu] = raw.view(np.float16).reshape(2, f.N, f.H + 2, f.W + 2, f.C)
         if not str(path).endswith(EXT):
             raise ValueError("a prepared style file must end in %s: %r" % (EXT, path))
         tmp = str(path) + ".tmp.npz"

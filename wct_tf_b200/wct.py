@@ -8,6 +8,7 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``device`` accepts the reference's TF strings ('/gpu:0') and torch strings;
   * ``swap5=True`` (style-swap at relu5_1, ops.py:145-278) honours ``ss_patch_size`` / ``ss_stride``; with a stride the
     content is centre-cropped so that the patches tile its relu5_1 encoding, as wct.py:84-90 does;
+  * ``swap_targets`` is new: the style swap at any relu levels (relu3_1 carries brush strokes, relu5_1 semantic parts);
   * ``predict_batch`` is new: a batch of frames per call (frames are independent);
   * ``content_mask`` is new: spatial control (WCT paper, section 4), a label map whose region r takes style r;
     ``style_masks`` restricts style r to its pixels labelled r;
@@ -26,6 +27,7 @@ import numpy as np
 import torch
 
 from .engine import Engine, SEMANTICS
+from .model import RELU_CHANNELS
 from .prepared import PreparedStyle
 
 
@@ -178,8 +180,50 @@ class WCT(object):
                 raise ValueError("each interpolated style must be one uint8 [Hs,Ws,3] image")
         return WCT.normalize_weights(style_weights, n_frames, len(styles)), styles
 
+    def swap_fit(self, contents, swap5, swap_targets, to_dev):
+        """wct.py:84-90 for the swap levels: with ``ss_stride`` > 1 the patches may not tile the encoding of the swap level;
+        centre-crop the content (on the device) so that they do.  One swap level at most with a stride (the crops of two
+        levels generally differ).  Returns the content frames.
+
+        ``swap5`` keeps the reference's rule (utils.swap_filter_fit on the relu5_1 encoding of the content).  For
+        ``swap_targets`` the encoding is the one the swap level actually sees: each earlier level of n pools decodes to
+        ceil(size / 2^n) 2^n, and the swap level reluK_1 pools K - 1 times.  The crop is the largest size <= the content's
+        whose encoding the patches tile; ValueError naming the level and the sizes when there is none."""
+        if self.ss_stride == 1 or not (swap5 or swap_targets is not None):
+            return contents
+        from .device_image import center_crop_to
+        from .imageio import swap_filter_fit
+        levels = ("relu5_1",) if swap_targets is None else self.engine.swap_levels(False, swap_targets)
+        if len(levels) > 1:
+            raise ValueError("ss_stride %d with %d swap levels (%s): a strided swap works at one level, whose encoding the "
+                             "content is cropped to" % (self.ss_stride, len(levels), ", ".join(levels)))
+        contents = to_dev(contents)
+        H, W = contents.shape[1], contents.shape[2]
+        if swap_targets is None:
+            refit, Ht, Wt = swap_filter_fit(H, W, self.ss_patch_size, self.ss_stride)
+            return center_crop_to(contents, Ht, Wt) if refit else contents
+        P, S = self.ss_patch_size, self.ss_stride
+        order = [l.relu_target for l in self.model.levels]
+        pools = [int(r[4]) - 1 for r in order[:order.index(levels[0]) + 1]]      # reluK_1 sits after K - 1 poolings
+
+        def encoding(x):
+            for n in pools[:-1]:
+                x = -(-x // 2 ** n) * 2 ** n
+            return -(-x // 2 ** pools[-1])
+
+        def fit(x):
+            while x >= 1 and (encoding(x) < P or (encoding(x) - P) % S):
+                x -= 1
+            return x
+        Ht, Wt = fit(H), fit(W)
+        if Ht < 1 or Wt < 1:
+            raise ValueError("the style swap at %s: patch %d / stride %d tiles the %s encoding of no crop of a %dx%d content"
+                             % (levels[0], P, S, levels[0], H, W))
+        return center_crop_to(contents, Ht, Wt) if (Ht, Wt) != (H, W) else contents
+
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
-                      passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None):
+                      passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
+                      swap_targets=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -204,19 +248,26 @@ class WCT(object):
         ``style_weights`` (style interpolation): ``styles`` is then a list of K (1..8) uint8 [Hs,Ws,3] images of any sizes
         and ``style_weights`` their weights, [K] for every frame or [N,K] (row n for frame n); finite, >= 0, each row with a
         positive sum, normalised to sum 1.  Frame n is stylised with the blend of the K styles, which equals the blend of
-        the K single-style results at every level.  WCT or AdaIN; not with ``content_mask`` or ``swap5``."""
+        the K single-style results at every level.  WCT or AdaIN; not with ``content_mask`` or ``swap5``.
+
+        ``swap_targets`` (style swap at any level): a list of relu targets at which the style swap replaces WCT / AdaIN in
+        the first pass, with ``ss_alpha`` and the model's ``ss_patch_size`` / ``ss_stride``.  ``swap5=True`` is
+        ``swap_targets=["relu5_1"]``; giving both is a ValueError, as is a level that is not a target.  With a stride
+        there is one swap level, and the content is cropped so that the patches tile its encoding.  Not with
+        ``content_mask`` or ``style_weights``."""
         eng = self.engine
         dev = eng.device
         n = 1 if np.ndim(contents) == 3 else contents.shape[0]
+        eng.swap_levels(swap5, swap_targets)                 # ValueError for both, or a level that is not a target
         if style_masks is not None and content_mask is None:
             raise ValueError("style_masks needs content_mask")
         if style_weights is not None:
-            if content_mask is not None or swap5:
-                raise ValueError("style_weights does not combine with content_mask or swap5")
+            if content_mask is not None or swap5 or swap_targets is not None:
+                raise ValueError("style_weights does not combine with content_mask or swap5 / swap_targets")
             weights, interp_styles = self.check_interp(style_weights, n, styles)
         if content_mask is not None:
-            if adain or swap5:
-                raise ValueError("content_mask works with WCT only: not with adain or swap5")
+            if adain or swap5 or swap_targets is not None:
+                raise ValueError("content_mask works with WCT only: not with adain or swap5 / swap_targets")
             mask, region_styles = self.check_mask(content_mask, n, styles)
             if style_masks is not None:
                 style_masks = self.check_style_masks(style_masks, region_styles)
@@ -230,17 +281,11 @@ class WCT(object):
             if isinstance(a, PreparedStyle):
                 return a
             a = to_dev(a)
-            return eng.prepare_call(a, adain=adain, swap5=swap5) if int(passes) > 1 else a
+            return eng.prepare_call(a, adain=adain, swap5=swap5, swap_targets=swap_targets) if int(passes) > 1 else a
 
-        if swap5 and self.ss_stride != 1:
-            # wct.py:84-90: with a stride the filter may not fit; centre-crop the content (on the device) to a size it tiles
-            from .device_image import center_crop_to
-            from .imageio import swap_filter_fit
-            with torch.cuda.device(dev):
-                contents = to_dev(contents)
-                refit, H, W = swap_filter_fit(contents.shape[1], contents.shape[2], self.ss_patch_size, self.ss_stride)
-                if refit:
-                    contents = center_crop_to(contents, H, W)
+        # wct.py:84-90: with a stride the filter may not fit; centre-crop the content (on the device) to a size it tiles
+        with torch.cuda.device(dev):
+            contents = self.swap_fit(contents, swap5, swap_targets, to_dev)
         with torch.cuda.device(dev):
             c = to_dev(contents)
             if style_weights is not None:
@@ -279,7 +324,8 @@ class WCT(object):
                     # the style swap acts in the first pass only (stylize_video.py:117-121).  A shared style swaps the
                     # whole batch in one call; with one style per frame the engine swaps frame by frame.
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
-                                       ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride)
+                                       ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
+                                       swap_targets=swap_targets if first else None)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -303,14 +349,16 @@ class WCT(object):
             return out_u8, out_f.cpu().numpy()
         return out_u8
 
-    def prepare_style(self, style):
+    def prepare_style(self, style, swap_targets=None):
         """Prepare ``style`` (uint8 [H,W,3] or [n,H,W,3]; numpy or torch, host or device) once, for any number of calls.
 
         Returns a ``PreparedStyle`` of n styles holding, per relu target, the WCT state for this model's semantics and the
         AdaIN moments; the relu5_1 style feature when relu5_1 is a target (the style swap is prepared from it on first use);
         and the style image on the host (``--concat``).  It is accepted wherever a style image is: ``predict_batch`` /
         ``predict`` / ``synthesize`` with n in {1, N}, and as an entry (n = 1) of the style lists of ``style_weights`` and
-        ``content_mask``, with ``adain``, ``passes`` and ``swap5``.  The results are byte-identical to the image's."""
+        ``content_mask``, with ``adain``, ``passes`` and ``swap5``.  The results are byte-identical to the image's.
+        ``swap_targets`` (relu targets) keeps the style feature of those levels too, for ``predict_batch(swap_targets=)``;
+        ``save`` stores them."""
         if isinstance(style, PreparedStyle):
             return style
         if style.dtype not in (np.uint8, torch.uint8) or style.ndim not in (3, 4) or style.shape[-1] != 3:
@@ -318,7 +366,7 @@ class WCT(object):
         eng = self.engine
         with torch.cuda.device(eng.device):
             s = _to_dev(style, eng.device)
-            ps = eng.prepare(s)
+            ps = eng.prepare(s, swap_targets or ())
             ps.image = s.cpu().numpy()
             ps.fingerprints = dict(eng.fingerprints())
         return ps
@@ -343,14 +391,18 @@ class WCT(object):
             for relu in taps:
                 ps.wct[relu] = P.pack_wct_state(eng.lib, data["%s/wct_mean" % relu], data["%s/wct_cs" % relu], data["%s/wct_k" % relu], dev)
                 ps.adain[relu] = P.pack_adain_state(eng.lib, data["%s/adain_mean" % relu], data["%s/adain_var" % relu], dev)
-            if "relu5_1" in taps:
-                raw = data["relu5_1/feat"]                                      # float16 [2, n, Hs+2, Ws+2, 512]
-                if raw.dtype != np.float16 or raw.ndim != 5 or raw.shape[:2] != (2, ps.n) or raw.shape[4] != 512:
-                    raise ValueError("%s: relu5_1/feat: bad shape %s" % (path, raw.shape))
-                act = eng._act(ps.n, raw.shape[2] - 2, raw.shape[3] - 2, 512)
+            for relu in taps:
+                # relu5_1 is always stored; another level only when the style was prepared to swap there
+                if relu != "relu5_1" and "%s/feat" % relu not in data:
+                    continue
+                C = RELU_CHANNELS[relu]
+                raw = data["%s/feat" % relu]                                    # float16 [2, n, Hs+2, Ws+2, C]
+                if raw.dtype != np.float16 or raw.ndim != 5 or raw.shape[:2] != (2, ps.n) or raw.shape[4] != C:
+                    raise ValueError("%s: %s/feat: bad shape %s" % (path, relu, raw.shape))
+                act = eng._act(ps.n, raw.shape[2] - 2, raw.shape[3] - 2, C)
                 flat = torch.from_numpy(np.ascontiguousarray(raw).view(np.uint8).reshape(-1)).to(dev)
                 act.buf[:flat.numel()] = flat
-                ps.feat5 = act
+                ps.feats[relu] = act
             main = torch.cuda.current_stream(dev)
             ps.side = main
             for relu in taps:
@@ -378,7 +430,7 @@ class WCT(object):
         return self.predict_batch(noise, styles, **kw)
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
-                style_masks=None):
+                style_masks=None, swap_targets=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
@@ -393,6 +445,8 @@ class WCT(object):
             return seen[id(x)]
         if style_masks is not None and content_mask is None:
             raise ValueError("style_masks needs content_mask")
+        if (style_weights is not None or content_mask is not None) and swap_targets is not None:
+            raise ValueError("swap_targets does not combine with content_mask or style_weights")
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, style_weights=style_weights, content_mask=content_mask)
@@ -401,7 +455,8 @@ class WCT(object):
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, content_mask=content_mask, **kw)
         else:
-            out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha)
+            kw = {} if swap_targets is None else dict(swap_targets=swap_targets)
+            out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
