@@ -106,6 +106,24 @@ WCTB200_API int wctb200_coral_apply_u8(const uint8_t* src, long long npix, const
 WCTB200_API int wctb200_noise_u8(uint8_t* out, int N, int H, int W, int C, unsigned long long seed, long long first_index,
                                  void* stream);
 
+/* ---- temporal stabilisation of video (DESIGN.md §3.3.6; flow.cu) ------------
+ * Luminance Y = (0.299 R + 0.587 G + 0.114 B) / 255 of npix RGB uint8 pixels, float32 out [npix]. */
+WCTB200_API int wctb200_luminance_u8(const uint8_t* rgb, long long npix, float* Y, void* stream);
+/* Optical flow (coarse-to-fine Horn-Schunck with warping) of the M - 1 consecutive pairs of Y float32 [M][H][W], M >= 2:
+ * flows float32 [2 (M - 1)][2][H][W] (u, v planes); problem 2t is the backward flow from frame t+1 to frame t, problem
+ * 2t+1 the forward flow from frame t to frame t+1.  Returns 0 from the query on bad geometry. */
+WCTB200_API size_t wctb200_flow_pairs_workspace_bytes(int M, int H, int W);
+WCTB200_API int wctb200_flow_pairs(const float* Y, int M, int H, int W, float* flows, void* ws, size_t ws_bytes, void* stream);
+/* Confidence of frame t+1 against frame t for t < M - 1: mask uint8 [M - 1][H][W] (0/1), counts int32 [M - 1] = the
+ * confident pixels before the cut rule (a pair with fewer than half its pixels confident gets mask 0 everywhere). */
+WCTB200_API int wctb200_flow_confidence(const float* Y, int M, int H, int W, const float* flows, uint8_t* mask, int32_t* counts,
+                                        void* stream);
+/* The recurrent blend, in place on frames uint8 [N][H][W][3]: O = round(P + beta c (O_prev(x + w_b) - P)), 0 <= beta < 1.
+ * With prev (uint8 [H][W][3], the stabilised frame before frame 0), frame i uses pair i (flows 2i, mask i); with prev NULL
+ * frame 0 is left as it is and frame i >= 1 uses pair i - 1.  One launch per frame, in order. */
+WCTB200_API int wctb200_temporal_blend_u8(uint8_t* frames, int N, int H, int W, const uint8_t* prev, const float* flows,
+                                          const uint8_t* masks, float beta, void* stream);
+
 /* ---- encoder / decoder layers ---------------------------------------------- */
 /* Weight preparation (one-time, device side):
  * w_hwio fp32 [3][3][Cin][Cout] (Keras kernel layout, vgg_normalised.py:33 /

@@ -12,6 +12,11 @@ Style interpolation: ``--interp-styles S0 S1 ...`` with ``--interp-weights w0 w1
 blend (output ``<clip>_<s0>-<w0>+<s1>-<w1>...``), and with ``--morph`` sweeps piecewise-linearly from S0 to the last style
 across the clip (``morph_weights``; output ``<clip>_morph_<s0>+<s1>...``).  A frame's weights depend on its index in the
 clip only, so ``--batch`` does not change a frame.
+
+Temporal stabilisation: ``--temporal STRENGTH`` (in [0, 1); default 0 = off) blends each stylised frame with its stabilised
+predecessor, warped by the optical flow of the content frames, where that flow is confident (``WCT.temporal_state``,
+DESIGN.md §3.3.6).  This reduces the flicker of frame-by-frame WCT.  Each (clip, style) run has one state, carried across
+batches and through the frame-by-frame path, so ``--batch`` does not change a frame; ``--concat`` comes after it.
 """
 from __future__ import division, print_function
 
@@ -38,6 +43,9 @@ _VIDEO_FLAGS = [
     (("--keep-tmp",), dict(action="store_true", default=False, help="keep the unpacked frames")),
     (("--batch",), dict(type=int, default=15, help="frames per predict_batch call (not in the reference)")),
     (("--fps",), dict(type=int, default=30, help="frame rate of the encoded video (not in the reference: fixed 30 there)")),
+    (("--temporal",), dict(type=float, default=0.0, metavar="STRENGTH",
+                           help="temporal stabilisation strength in [0, 1): blend each frame with its flow-warped stabilised "
+                                "predecessor (default 0: off)")),
 ]
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
@@ -81,6 +89,8 @@ def parse_args(argv=None):
     if args.interp_styles is None and args.style_path is None:
         parser.error("--style-path (or --interp-styles) is required")
     stylize.check_prepared_flags(parser, args)
+    if not 0.0 <= args.temporal < 1.0:
+        parser.error("--temporal must be in [0, 1), got %g" % args.temporal)
     return args
 
 
@@ -110,14 +120,16 @@ def batches(seq, n):
         yield seq[i:i + n]
 
 
-def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device, weights=None):
+def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device, weights=None, temporal=None):
     """All frames of one clip with one style (a uint8 CUDA tensor, already resized / cropped).  Frames of equal size are
     batched; the decode of batch i+1 and the PNG writes of batch i-1 overlap the GPU work of batch i.  Resize
     (``--content-size``), CORAL (``--keep-colors``), every pass and the ``--concat`` thumbnail run on the device
     (wct_tf_b200.device_image); a frame crosses PCIe once in each direction.
 
     Style interpolation: ``style_img`` is a list of K styles and ``weights`` a float64 [K] blend for every frame or [T, K],
-    row t for frame t of the clip, so a frame's weights do not depend on the batching."""
+    row t for frame t of the clip, so a frame's weights do not depend on the batching.
+
+    ``temporal``: the clip's temporal state (--temporal), passed to every predict_batch call in frame order."""
     def finish(out_f, frame_u8):
         io.save_img(out_f, frame_u8)
 
@@ -128,6 +140,8 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         if weights is None:
             return {}
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
+
+    temporal_kw = {} if temporal is None else dict(temporal=temporal)
 
     def coral(style, fr):
         if isinstance(style, list):
@@ -153,7 +167,7 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
             one = weights is not None or not hasattr(style_img, "shape")   # a list of styles, or a prepared style
             out = wct_model.predict_batch(x, style_img if one else style_img[None], alpha=args.alpha,
                                           adain=args.adain, passes=args.passes, return_device=True,
-                                          **dict(interp_kw(first, first + len(frames)), **swap_kw))
+                                          **dict(interp_kw(first, first + len(frames)), **swap_kw, **temporal_kw))
             results = [(out[i], style_img) for i in range(len(frames))]
         else:                                                  # per-frame styles (CORAL) or ragged sizes
             results = []
@@ -163,9 +177,13 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 kw = dict(alpha=args.alpha, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True,
                           **interp_kw(first + j, first + j + 1))
                 swap_kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
-                o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, **dict(kw, **swap_kw))
-                for _ in range(args.passes - 1):
-                    o = wct_model.predict_batch(o, style_rgb, swap5=False, **kw)
+                if temporal is not None:           # stabilised after the last pass: all passes in one call
+                    o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, passes=args.passes,
+                                                **dict(kw, **swap_kw, **temporal_kw))
+                else:
+                    o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, **dict(kw, **swap_kw))
+                    for _ in range(args.passes - 1):
+                        o = wct_model.predict_batch(o, style_rgb, swap5=False, **kw)
                 results.append((o[0], style_rgb))
         for (_, out_f), (o, srgb) in zip(group, results):
             if args.concat:                                    # stylize_video.py:125-128
@@ -259,7 +277,8 @@ def main(argv=None, wct_factory=None, image_ops=None):
                 continue
             os.makedirs(frames_dir, exist_ok=True)
             out_files = [os.path.join(frames_dir, os.path.splitext(os.path.basename(f))[0] + '.png') for f in in_files]
-            n = stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device, weights)
+            temporal = wct_model.temporal_state(args.temporal) if args.temporal > 0 else None    # one per (clip, style) run
+            n = stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, dimg, device, weights, temporal)
             total += n
             print("Stylized {} frames with {} -> {}".format(n, style_prefix, frames_dir))
             # stylize_video.py:137-149 re-encodes "frame_%d.png".  Frames extracted by ffmpeg carry that name; a user-supplied

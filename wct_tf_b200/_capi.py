@@ -32,6 +32,11 @@ SIGNATURES = {
     "wctb200_rgb_moments_u8": (_i, [_vp, C.c_longlong, _vp, _vp]),
     "wctb200_coral_apply_u8": (_i, [_vp, C.c_longlong, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "wctb200_noise_u8": (_i, [_vp, _i, _i, _i, _i, C.c_ulonglong, C.c_longlong, _vp]),
+    "wctb200_luminance_u8": (_i, [_vp, C.c_longlong, _vp, _vp]),
+    "wctb200_flow_pairs_workspace_bytes": (_sz, [_i, _i, _i]),
+    "wctb200_flow_pairs": (_i, [_vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "wctb200_flow_confidence": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "wctb200_temporal_blend_u8": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _vp]),
     "wctb200_conv_weight_bytes": (_sz, [_i, _i, _i]),
     "wctb200_prep_conv_weights": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "wctb200_prep_conv_weights_up2": (_i, [_vp, _i, _i, _vp, _vp]),

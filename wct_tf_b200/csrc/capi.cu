@@ -89,6 +89,12 @@ int launch_rgb_moments(const uint8_t* img, long long npix, unsigned long long* s
 int launch_coral_apply(const uint8_t* src, long long npix, const double* A, const double* sm, const double* ss, const double* tm,
                        const double* ts, uint8_t* dst, cudaStream_t st);
 int launch_noise_u8(uint8_t* out, int N, long long frame_bytes, unsigned long long seed, long long first_index, cudaStream_t st);
+int launch_luminance(const uint8_t* rgb, long long npix, float* Y, cudaStream_t st);
+size_t flow_pairs_workspace_bytes(int M, int H, int W);
+int launch_flow_pairs(const float* Y, int M, int H, int W, float* flows, void* ws, size_t ws_bytes, cudaStream_t st);
+int launch_flow_confidence(const float* Y, int M, int H, int W, const float* flows, uint8_t* mask, int* counts, cudaStream_t st);
+int launch_temporal_blend(uint8_t* frames, int N, int H, int W, const uint8_t* prev, const float* flows, const uint8_t* masks,
+                          float beta, cudaStream_t st);
 int launch_act_from_f32(const float*, ActGeom, __half*, cudaStream_t);
 int launch_act_to_f32(const __half*, ActGeom, float*, cudaStream_t);
 int launch_prep_weights(const float*, int, int, int, __half*, cudaStream_t);
@@ -256,6 +262,39 @@ int wctb200_noise_u8(uint8_t* out, int N, int H, int W, int C, unsigned long lon
     WCTB_REQUIRE(first_index >= 0 && first_index <= LLONG_MAX - N, "noise_u8: first_index=%lld with N=%d is out of range",
                  first_index, N);
     return launch_noise_u8(out, N, (long long)H * W * C, seed, first_index, ST(stream));
+}
+
+// the flow kernels index a plane with 32-bit pixel coordinates and a stack with 64-bit offsets
+static bool flow_geom_ok(int M, int H, int W) {
+    return M >= 2 && M <= 65536 && H >= 1 && W >= 1 && H <= (1 << 15) && W <= (1 << 15);
+}
+int wctb200_luminance_u8(const uint8_t* rgb, long long npix, float* Y, void* stream) {
+    WCTB_REQUIRE(rgb && Y && npix >= 1 && npix < (1ll << 40), "luminance_u8: bad arguments");
+    return launch_luminance(rgb, npix, Y, ST(stream));
+}
+size_t wctb200_flow_pairs_workspace_bytes(int M, int H, int W) {
+    if (!flow_geom_ok(M, H, W)) return 0;
+    return flow_pairs_workspace_bytes(M, H, W);
+}
+int wctb200_flow_pairs(const float* Y, int M, int H, int W, float* flows, void* ws, size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(Y && flows && ws, "flow_pairs: null pointer");
+    WCTB_REQUIRE(flow_geom_ok(M, H, W), "flow_pairs: bad geometry M=%d %dx%d (M >= 2 frames)", M, H, W);
+    return launch_flow_pairs(Y, M, H, W, flows, ws, ws_bytes, ST(stream));
+}
+int wctb200_flow_confidence(const float* Y, int M, int H, int W, const float* flows, uint8_t* mask, int32_t* counts,
+                            void* stream) {
+    WCTB_REQUIRE(Y && flows && mask && counts, "flow_confidence: null pointer");
+    WCTB_REQUIRE(flow_geom_ok(M, H, W), "flow_confidence: bad geometry M=%d %dx%d (M >= 2 frames)", M, H, W);
+    return launch_flow_confidence(Y, M, H, W, flows, mask, counts, ST(stream));
+}
+int wctb200_temporal_blend_u8(uint8_t* frames, int N, int H, int W, const uint8_t* prev, const float* flows, const uint8_t* masks,
+                              float beta, void* stream) {
+    WCTB_REQUIRE(frames && flows && masks, "temporal_blend_u8: null pointer");
+    WCTB_REQUIRE(N >= 1 && H >= 1 && W >= 1 && H <= (1 << 15) && W <= (1 << 15), "temporal_blend_u8: bad geometry N=%d %dx%d", N,
+                 H, W);
+    WCTB_REQUIRE(prev || N >= 2, "temporal_blend_u8: one frame without a predecessor has nothing to blend");
+    WCTB_REQUIRE(beta >= 0.f && beta < 1.f, "temporal_blend_u8: beta=%g outside [0, 1)", (double)beta);
+    return launch_temporal_blend(frames, N, H, W, prev, flows, masks, beta, ST(stream));
 }
 
 size_t wctb200_conv_weight_bytes(int taps, int Cin, int Cout) {

@@ -16,7 +16,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
     every frame or one row per frame;
   * ``synthesize`` is new: texture synthesis (WCT paper, section 4), the pipeline run on seeded noise made on the device;
   * ``prepare_style`` / ``load_style`` are new: the style side computed once (or read from a ``.wctstyle`` file) and
-    accepted wherever a style image is (wct_tf_b200/prepared.py).
+    accepted wherever a style image is (wct_tf_b200/prepared.py);
+  * ``temporal_state`` / ``predict_batch(temporal=)`` are new: temporal stabilisation of a clip's frames with the optical
+    flow of the content (wct_tf_b200/temporal.py).
 """
 from __future__ import annotations
 
@@ -223,7 +225,7 @@ class WCT(object):
 
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
-                      swap_targets=None):
+                      swap_targets=None, temporal=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -254,7 +256,14 @@ class WCT(object):
         the first pass, with ``ss_alpha`` and the model's ``ss_patch_size`` / ``ss_stride``.  ``swap5=True`` is
         ``swap_targets=["relu5_1"]``; giving both is a ValueError, as is a level that is not a target.  With a stride
         there is one swap level, and the content is cropped so that the patches tile its encoding.  Not with
-        ``content_mask`` or ``style_weights``."""
+        ``content_mask`` or ``style_weights``.
+
+        ``temporal`` (a ``temporal_state``): the N frames are the next N frames of that clip.  They are stylised exactly as
+        without it; after the last pass each frame is blended with its stabilised predecessor, warped by the optical flow of
+        the content frames, where that flow is confident (DESIGN.md §3.3.6), and the state moves on.  The first frame of a
+        clip, and a frame whose size differs from its predecessor's, come back unchanged.  Not with ``return_float``."""
+        if temporal is not None and return_float:
+            raise ValueError("temporal stabilisation works on the uint8 frames: not with return_float=True")
         eng = self.engine
         dev = eng.device
         n = 1 if np.ndim(contents) == 3 else contents.shape[0]
@@ -331,6 +340,9 @@ class WCT(object):
             for _ in range(int(passes) - 1):
                 out_f = one_pass(out_dev, False)
                 out_dev = eng.to_u8(out_f)
+            if temporal is not None:
+                from .temporal import stabilize_
+                stabilize_(temporal, c, out_dev)
             if return_device:
                 eng.check_device()            # synchronises; raises WctB200Error if a kernel recorded a pipeline time-out
                 return (out_dev, out_f) if return_float else out_dev
@@ -348,6 +360,14 @@ class WCT(object):
         if return_float:
             return out_u8, out_f.cpu().numpy()
         return out_u8
+
+    @staticmethod
+    def temporal_state(strength):
+        """The temporal state of one clip for ``predict_batch(temporal=)``: ``strength`` in [0, 1) is the weight beta of the
+        warped previous output (0 leaves every frame as it is); ValueError outside that range.  ``reset()`` starts the clip
+        again."""
+        from .temporal import TemporalState
+        return TemporalState(strength)
 
     def prepare_style(self, style, swap_targets=None):
         """Prepare ``style`` (uint8 [H,W,3] or [n,H,W,3]; numpy or torch, host or device) once, for any number of calls.
