@@ -291,6 +291,48 @@ WCTB200_API int wctb200_adain_apply_blend(const void* content, int Nc, int Hc, i
                               const void* const* states, int K, const float* weights, int Nw,
                               float alpha, float eps, void* out, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- tiled stylisation (DESIGN.md §3.3.7) -------------------------------------
+ * A level's content statistics are sums, so a frame too large for one pass is encoded tile by tile: the statistics of
+ * each tile's interior go into a record, the records are folded into one per frame in a fixed tile order, the record
+ * becomes the level's transform once, and a second pass applies that transform to every tile.
+ *
+ * Statistics record of N frames: fp64 n [N] (pixels), t [N][C] (the centring shift), s [N][C] = sum (x - t) and
+ * S = sum (x - t)(x - t)^T: [N][C][C] for WCT (diag = 0), its diagonal [N][C] for AdaIN (diag = 1).  Offsets from
+ * wctb200_stats_record_layout (returns the total, 0 for C not a multiple of 8 or > 2048, N < 1 or diag not 0/1).
+ *
+ * stats_rect: the record of the rectangle [y0, y0+h) x [x0, x0+w) of every frame of an SPF16 map [N,H,W,C] (h, w >= 1,
+ * inside the map).  The split into CTA slots and the sampled shift are those of an h x w map, so the whole-map rectangle
+ * gives the sums of wctb200_wct_apply / wctb200_adain_apply bit for bit.  WCT: C in {64,128,256,512}.
+ * stats_accumulate: folds record B into record A (same C, N, diag): B's sums are re-centred on A's shift in fp64 and
+ * added; a frame of A with n = 0 takes B's as they are.  Folding in a fixed order gives a deterministic result.
+ *
+ * Transforms from a record (frames with n >= 2): the content side of wctb200_wct_apply / wctb200_adain_apply from the
+ * record against a style state of Ns in {1, Nc} styles, written to a transform buffer instead of applied:
+ *   WCT: split-fp16 M [Nc][2][C][C] at *off_m, bias fp32 [Nc][C] at *off_bias, int32 [k_c x Nc | sweeps_c x Nc] at *off_k
+ *        (wctb200_wct_transform_layout; 0 for C not in {64,128,256,512} or N < 1); ws of wctb200_wct_workspace_bytes(C, Nc, 0).
+ *   AdaIN: fp32 mean_c, var_c, inv = rsqrt(var_c + eps) sqrt(var_s), ms, each [Nc][C] (wctb200_adain_transform_layout).
+ * transform_apply: out = the transform of frame i applied to frame i of any SPF16 map [N,H,W,C] of those frames (a tile
+ * with its halo); AdaIN takes alpha here.  A record of whole frames, then its transform, then the apply, gives the bytes
+ * of wctb200_wct_apply / wctb200_adain_apply. */
+WCTB200_API size_t wctb200_stats_record_layout(int C, int N, int diag, size_t* off_n, size_t* off_t, size_t* off_s, size_t* off_S);
+WCTB200_API int wctb200_wct_stats_rect(const void* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record,
+                                       void* stream);
+WCTB200_API int wctb200_adain_stats_rect(const void* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record,
+                                         void* stream);
+WCTB200_API int wctb200_stats_accumulate(void* record_a, const void* record_b, int C, int N, int diag, void* stream);
+WCTB200_API size_t wctb200_wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k);
+WCTB200_API int wctb200_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha,
+                                                 float eps_cov, float eps_eig, float thresh, int readd_content_mean,
+                                                 void* transform, void* ws, size_t ws_bytes, void* stream);
+WCTB200_API int wctb200_wct_transform_apply(const void* act, int N, int H, int W, int C, const void* transform, void* out,
+                                            void* stream);
+WCTB200_API size_t wctb200_adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, size_t* off_inv,
+                                                  size_t* off_ms);
+WCTB200_API int wctb200_adain_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float eps,
+                                                   void* transform, void* stream);
+WCTB200_API int wctb200_adain_transform_apply(const void* act, int N, int H, int W, int C, const void* transform, float alpha,
+                                              void* out, void* stream);
+
 /*
  * wct_style_swap (ops.py:145-217) + style_swap (ops.py:219-278) for ONE content/style pair: whiten both encodings, take every
  * patch x patch window of the whitened style at `stride` (--ss-patch-size / --ss-stride, stylize.py:33-34), replace every

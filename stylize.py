@@ -26,6 +26,11 @@ Prepared styles: ``--style-path``, ``--interp-styles`` and ``--mask-styles`` als
 content, pass and noise batch.  A run's styles are all prepared or all images, and prepared styles take no ``--style-size``,
 ``--crop-size`` or ``--keep-colors`` (their size and crop were fixed when they were prepared).
 
+Tiled stylisation: ``--tile-size T`` (a multiple of 16; 0: off) runs every level on T x T tiles widened by a halo, so device
+memory follows the tile and not the image, with each level's statistics taken over the whole image (DESIGN.md §3.3.7).  Not
+with ``--content-mask``, ``--interp-styles``, ``--swap5`` or ``--swap-targets``; ``--keep-colors``, ``--concat``,
+``--content-size``, ``--passes`` and ``--noise`` work on the whole image as without it.
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -71,6 +76,9 @@ _FLAGS = [
                               help="one 8-bit grayscale mask per --mask-styles entry: region r takes the pixels of style r in region r")),
     (("--interp-styles",), dict(nargs="+", type=str, default=None, help="1..8 style images to blend (with --interp-weights)")),
     (("--interp-weights",), dict(nargs="+", type=float, default=None, help="one weight >= 0 per --interp-styles entry (normalised)")),
+    (("--tile-size",), dict(type=int, default=0, metavar="T",
+                            help="stylise in T x T tiles (a multiple of 16) in bounded device memory, with every level's "
+                                 "statistics over the whole image (0: off)")),
     # webcam.py:38; the three --noise-* flags are not in the reference.  Their defaults are filled in by parse_args, so that
     # giving one without --noise can be told from leaving it out.
     (("--noise",), dict(action="store_true", default=False, help="Synthesize textures from noise images")),
@@ -100,6 +108,7 @@ def parse_args(argv=None):
     args = parser.parse_args(argv)
     check_swap_flags(parser, args)
     check_interp_flags(parser, args)
+    check_tile_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
@@ -125,6 +134,19 @@ def check_swap_flags(parser, args):
     for relu in args.swap_targets:
         if relu not in (args.relu_targets or []):
             parser.error("--swap-targets: %s is not one of --relu-targets (%s)" % (relu, " ".join(args.relu_targets or [])))
+
+
+def check_tile_flags(parser, args):
+    """--tile-size: a multiple of 16 (0: off); not with the region, interpolation and swap modes, which take statistics
+    the tiled path does not accumulate."""
+    if args.tile_size == 0:
+        return
+    if args.tile_size < 0 or args.tile_size % 16:
+        parser.error("--tile-size must be a positive multiple of 16 (0: off), got %d" % args.tile_size)
+    for attr, flag in [("content_mask", "--content-mask"), ("interp_styles", "--interp-styles"), ("swap5", "--swap5"),
+                       ("swap_targets", "--swap-targets")]:
+        if getattr(args, attr):
+            parser.error("--tile-size does not combine with %s" % flag)
 
 
 def check_style_mask_flags(parser, args):
@@ -302,6 +324,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
     kw = dict(alpha=args.alpha, swap5=args.swap5, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True)
     if args.swap_targets:
         kw["swap_targets"] = list(args.swap_targets)
+    if args.tile_size:
+        kw["tile_size"] = args.tile_size
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, style_dev, **kw)

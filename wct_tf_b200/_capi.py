@@ -80,6 +80,16 @@ SIGNATURES = {
     "wctb200_style_swap_apply_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i, _i]),
     "wctb200_style_swap_apply_min_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i, _i]),
     "wctb200_style_swap_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_stats_record_layout": (_sz, [_i, _i, _i, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
+    "wctb200_wct_stats_rect": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "wctb200_adain_stats_rect": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "wctb200_stats_accumulate": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "wctb200_wct_transform_layout": (_sz, [_i, _i, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
+    "wctb200_wct_transform_from_stats": (_i, [_vp, _i, _i, _vp, _i, _f, _f, _f, _f, _i, _vp, _vp, _sz, _vp]),
+    "wctb200_wct_transform_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "wctb200_adain_transform_layout": (_sz, [_i, _i, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
+    "wctb200_adain_transform_from_stats": (_i, [_vp, _i, _i, _vp, _i, _f, _vp, _vp]),
+    "wctb200_adain_transform_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _f, _vp, _vp]),
 }
 
 # tuning / probe hooks (wct_tf_b200/csrc/wctb200_debug.h): NOT part of the ABI, bound for tools/ and tests/ only

@@ -121,6 +121,19 @@ int launch_adain_apply(const __half* content, int Nc, int Hc, int Wc, int C, con
 int launch_adain_apply_blend(const __half* content, int Nc, int Hc, int Wc, int C, const void* const* states, int K,
                              const float* weights, int Nw, float alpha, float eps, __half* out, void* ws, size_t ws_bytes,
                              cudaStream_t st);
+size_t stats_record_layout(int C, int N, int diag, size_t* off_n, size_t* off_t, size_t* off_s, size_t* off_S);
+int launch_wct_stats_rect(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, cudaStream_t st);
+int launch_adain_stats_rect(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, cudaStream_t st);
+int launch_stats_accumulate(void* rec_a, const void* rec_b, int C, int N, int diag, cudaStream_t st);
+size_t wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k);
+size_t adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, size_t* off_inv, size_t* off_ms);
+int launch_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                                    float eps_eig, float thresh, int readd, void* transform, void* ws, size_t ws_bytes, cudaStream_t st);
+int launch_wct_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, __half* out, cudaStream_t st);
+int launch_adain_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float eps, void* transform,
+                                      cudaStream_t st);
+int launch_adain_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, float alpha, __half* out,
+                                 cudaStream_t st);
 int launch_conv3x3_ref(const __half*, ActGeom, const float*, const float*, int, int, __half*, cudaStream_t);
 int launch_conv_head(const float*, int, int, int, const float*, const float*, __half*, cudaStream_t);
 int launch_conv_tail(const __half*, ActGeom, const float*, const float*, int, float*, cudaStream_t);
@@ -558,6 +571,65 @@ int wctb200_adain_apply_blend(const void* content, int Nc, int Hc, int Wc, int C
     WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "adain_apply_blend: bad geometry");
     return launch_adain_apply_blend(HCP(content), Nc, Hc, Wc, C, states, K, weights, Nw, alpha, eps, HP(out), ws, ws_bytes,
                                     ST(stream));
+}
+// ---- tiled stylisation: statistics records and transforms (DESIGN.md §3.3.7) ----
+static bool wct_channels_ok(int C) { return C == 64 || C == 128 || C == 256 || C == 512; }
+static bool rect_ok(int H, int W, int y0, int x0, int h, int w) {
+    return y0 >= 0 && x0 >= 0 && h >= 1 && w >= 1 && (long long)y0 + h <= H && (long long)x0 + w <= W;
+}
+size_t wctb200_stats_record_layout(int C, int N, int diag, size_t* off_n, size_t* off_t, size_t* off_s, size_t* off_S) {
+    if (C < 8 || C % 8 != 0 || C > 2048 || N < 1 || (diag != 0 && diag != 1)) return 0;
+    return stats_record_layout(C, N, diag, off_n, off_t, off_s, off_S);
+}
+int wctb200_wct_stats_rect(const void* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, void* stream) {
+    WCTB_REQUIRE(act && record, "wct_stats_rect: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && wct_channels_ok(C), "wct_stats_rect: bad geometry");
+    WCTB_REQUIRE(rect_ok(H, W, y0, x0, h, w), "wct_stats_rect: rectangle (%d,%d)+%dx%d outside %dx%d", y0, x0, h, w, H, W);
+    return launch_wct_stats_rect(HCP(act), N, H, W, C, y0, x0, h, w, record, ST(stream));
+}
+int wctb200_adain_stats_rect(const void* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, void* stream) {
+    WCTB_REQUIRE(act && record, "adain_stats_rect: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && C <= 2048, "adain_stats_rect: bad geometry");
+    WCTB_REQUIRE(rect_ok(H, W, y0, x0, h, w), "adain_stats_rect: rectangle (%d,%d)+%dx%d outside %dx%d", y0, x0, h, w, H, W);
+    return launch_adain_stats_rect(HCP(act), N, H, W, C, y0, x0, h, w, record, ST(stream));
+}
+int wctb200_stats_accumulate(void* record_a, const void* record_b, int C, int N, int diag, void* stream) {
+    WCTB_REQUIRE(record_a && record_b, "stats_accumulate: null pointer");
+    WCTB_REQUIRE(wctb200_stats_record_layout(C, N, diag, nullptr, nullptr, nullptr, nullptr) > 0, "stats_accumulate: bad arguments");
+    return launch_stats_accumulate(record_a, record_b, C, N, diag, ST(stream));
+}
+size_t wctb200_wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k) {
+    if (!wct_channels_ok(C) || N < 1) return 0;
+    return wct_transform_layout(C, N, off_m, off_bias, off_k);
+}
+int wctb200_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                                     float eps_eig, float thresh, int readd_content_mean, void* transform, void* ws, size_t ws_bytes,
+                                     void* stream) {
+    WCTB_REQUIRE(record && state && transform && ws, "wct_transform_from_stats: null pointer");
+    WCTB_REQUIRE(wct_channels_ok(C) && Nc >= 1, "wct_transform_from_stats: bad arguments");
+    return launch_wct_transform_from_stats(record, Nc, C, state, Ns, alpha, eps_cov, eps_eig, thresh, readd_content_mean, transform,
+                                           ws, ws_bytes, ST(stream));
+}
+int wctb200_wct_transform_apply(const void* act, int N, int H, int W, int C, const void* transform, void* out, void* stream) {
+    WCTB_REQUIRE(act && transform && out, "wct_transform_apply: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && wct_channels_ok(C), "wct_transform_apply: bad geometry");
+    return launch_wct_transform_apply(HCP(act), N, H, W, C, transform, HP(out), ST(stream));
+}
+size_t wctb200_adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, size_t* off_inv, size_t* off_ms) {
+    if (C < 8 || C % 8 != 0 || C > 2048 || N < 1) return 0;
+    return adain_transform_layout(C, N, off_mean, off_var, off_inv, off_ms);
+}
+int wctb200_adain_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float eps, void* transform,
+                                       void* stream) {
+    WCTB_REQUIRE(record && state && transform, "adain_transform_from_stats: null pointer");
+    WCTB_REQUIRE(C >= 8 && C % 8 == 0 && C <= 2048 && Nc >= 1, "adain_transform_from_stats: bad arguments");
+    return launch_adain_transform_from_stats(record, Nc, C, state, Ns, eps, transform, ST(stream));
+}
+int wctb200_adain_transform_apply(const void* act, int N, int H, int W, int C, const void* transform, float alpha, void* out,
+                                  void* stream) {
+    WCTB_REQUIRE(act && transform && out, "adain_transform_apply: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && C <= 2048, "adain_transform_apply: bad geometry");
+    return launch_adain_transform_apply(HCP(act), N, H, W, C, transform, alpha, HP(out), ST(stream));
 }
 // tuning hooks (wctb200_debug.h; not part of the stable ABI)
 int wctb200_debug_set_conv_bn(int bn) {

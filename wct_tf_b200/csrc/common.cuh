@@ -434,6 +434,9 @@ int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, con
 int conv_tc_bn(int Cout);
 int launch_conv_taps_rows(const __half* in, int N, int H, int W, int Cin, const __half* w_split, long long wplane, int Cout, int bn,
                           __half* out, cudaStream_t st, int kw);
+// statistics record of N frames (tiled stylisation; wctb200_stats_record_layout): fp64 n [N], t [N][C], s [N][C],
+// S [N][C][C] (covariance) or [N][C] (AdaIN's moments: the diagonal)
+struct StatsRecord { double *n, *t, *s, *S; };
 // trailer of a prepared weight buffer: [0] = 1/scale (float), see wctb200_prep_conv_weights
 static inline const float* weight_scale_ptr(const __half* w_split, int taps_total, int Cin, int Cout) {
     return reinterpret_cast<const float*>(w_split + (size_t)2 * taps_total * Cin * Cout);

@@ -399,6 +399,39 @@ k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __r
     }
 }
 
+// The fixed-order fp64 reductions of the slots and the finalize expressions, shared by the whole-frame path (k_cov_sums,
+// k_cov_finalize) and the statistics record of a rectangle (k_cov_record, k_record_cov_finalize): a record of the whole
+// frame gives the same bits.
+__device__ __forceinline__ double psum_total(const float* __restrict__ psum, int ksplit, int C, int n, int c) {
+    double a = 0.0;
+    for (int s = 0; s < ksplit; ++s) a += (double)psum[((long long)n * ksplit + s) * C + c];
+    return a;
+}
+// four interleaved partial sums (a fixed order all the same): the serial fp64 chain over up to 256 slots took 73-85 us
+__device__ __forceinline__ double part_total(const float* __restrict__ pp, int nslots, long long cc) {
+    double v0 = 0.0, v1 = 0.0, v2 = 0.0, v3 = 0.0;
+    int s = 0;
+    for (; s + 4 <= nslots; s += 4) {
+        v0 += (double)pp[(long long)s * cc];
+        v1 += (double)pp[(long long)(s + 1) * cc];
+        v2 += (double)pp[(long long)(s + 2) * cc];
+        v3 += (double)pp[(long long)(s + 3) * cc];
+    }
+    for (; s < nslots; ++s) v0 += (double)pp[(long long)s * cc];
+    return (v0 + v1) + (v2 + v3);
+}
+__device__ __forceinline__ float mean_from_sums(float shift, double s, long long cnt) {
+    return cnt > 0 ? (float)((double)shift + s / (double)cnt) : shift;
+}
+// (S - si sj / cnt) / (cnt - 1) (+ eps_cov on the diagonal)
+__device__ __forceinline__ float cov_from_sums(double S, double si, double sj, long long cnt, bool diag, float eps_cov) {
+    double v = S;
+    v -= si * sj / (double)cnt;
+    float r = (float)(v / (double)(cnt - 1));
+    if (diag) r += eps_cov;
+    return r;
+}
+
 // dsum[n][c] = sum over splits of psum (fp64, fixed order); mean = shift + dsum / HW
 // (spatial control: `counts` [problems] replaces HW; a problem without pixels keeps its shift as the mean)
 __global__ void k_cov_sums(const float* __restrict__ psum, const float* __restrict__ shift, int C, int ksplit, long long HW,
@@ -407,10 +440,9 @@ __global__ void k_cov_sums(const float* __restrict__ psum, const float* __restri
     if (i >= total) return;
     const int n = i / C, c = i - n * C;
     const long long cnt = counts ? (long long)counts[n] : HW;
-    double a = 0.0;
-    for (int s = 0; s < ksplit; ++s) a += (double)psum[((long long)n * ksplit + s) * C + c];
+    const double a = psum_total(psum, ksplit, C, n, c);
     dsum[i] = a;
-    mean[i] = cnt > 0 ? (float)((double)shift[i] + a / (double)cnt) : shift[i];
+    mean[i] = mean_from_sums(shift[i], a, cnt);
 }
 
 // G = (sum_slots part - s s^T / HW) / (HW - 1) + eps_cov * I   (ops.py:45,50,108,121), exactly symmetric
@@ -433,23 +465,52 @@ __global__ void k_cov_finalize(const float* __restrict__ part, const double* __r
         // every (min,max) entry lies in a stored upper block: reading it for both (i,j) and (j,i) makes G exactly symmetric
         const long long e = (i <= j) ? (long long)i * C + j : (long long)j * C + i;
         const float* pp = part + n * nslots * (long long)C * C + e;
-        // four interleaved partial sums (a fixed order all the same): the serial fp64 chain over up to 256 slots took 73-85 us
-        double v0 = 0.0, v1 = 0.0, v2 = 0.0, v3 = 0.0;
-        const long long cc = (long long)C * C;
-        int s = 0;
-        for (; s + 4 <= nslots; s += 4) {
-            v0 += (double)pp[(long long)s * cc];
-            v1 += (double)pp[(long long)(s + 1) * cc];
-            v2 += (double)pp[(long long)(s + 2) * cc];
-            v3 += (double)pp[(long long)(s + 3) * cc];
-        }
-        for (; s < nslots; ++s) v0 += (double)pp[(long long)s * cc];
-        double v = (v0 + v1) + (v2 + v3);
-        v -= dsum[n * C + i] * dsum[n * C + j] / (double)cnt;
-        float r = (float)(v / (double)(cnt - 1));
-        if (i == j) r += eps_cov;
+        const double v = part_total(pp, nslots, (long long)C * C);
+        const float r = cov_from_sums(v, dsum[n * C + i], dsum[n * C + j], cnt, i == j, eps_cov);
         G[t] = r;
         if (A0) A0[t] = r;          // pristine copy: the Jacobi kernel overwrites G, the Rayleigh quotients need A
+    }
+}
+
+// ---------------------------------------------------------------------------
+// Statistics records (tiled stylisation, DESIGN.md §3.3.7).  A record of N frames holds, per frame, the pixel count n,
+// the centring shift t, s = sum (x - t) and S = sum (x - t)(x - t)^T (the diagonal only for AdaIN's moments), all fp64
+// (layout: stats_record_layout, wct.cu).  k_cov_record turns the slots of cov_tc_kernel into a record with the reductions
+// of k_cov_sums / k_cov_finalize; S is written in full, symmetric.
+// ---------------------------------------------------------------------------
+__global__ void k_cov_record(const float* __restrict__ part, const float* __restrict__ psum, const float* __restrict__ shift, int C,
+                             int nslots, int ksplit, long long HW, int count, double* __restrict__ rn, double* __restrict__ rt,
+                             double* __restrict__ rs, double* __restrict__ rS) {
+    const long long total = (long long)count * C * C;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const int j = (int)(t % C);
+        const int i = (int)((t / C) % C);
+        const long long n = t / ((long long)C * C);
+        const long long e = (i <= j) ? (long long)i * C + j : (long long)j * C + i;
+        rS[t] = part_total(part + n * nslots * (long long)C * C + e, nslots, (long long)C * C);
+        if (j == 0) {
+            rs[n * C + i] = psum_total(psum, ksplit, C, (int)n, i);
+            rt[n * C + i] = (double)shift[n * C + i];
+            if (i == 0) rn[n] = (double)HW;
+        }
+    }
+}
+
+// record -> mean [N][C], G (+ eps_cov I) and its copy A0, [N][C][C]: the expressions of k_cov_sums / k_cov_finalize
+__global__ void k_record_cov_finalize(const double* __restrict__ rn, const double* __restrict__ rt, const double* __restrict__ rs,
+                                      const double* __restrict__ rS, int C, int count, float eps_cov, float* __restrict__ mean,
+                                      float* __restrict__ G, float* __restrict__ A0) {
+    const long long total = (long long)count * C * C;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const int j = (int)(t % C);
+        const int i = (int)((t / C) % C);
+        const long long n = t / ((long long)C * C);
+        const long long cnt = (long long)rn[n];
+        const long long e = (i <= j) ? (long long)i * C + j : (long long)j * C + i;
+        const float r = cov_from_sums(rS[n * C * C + e], rs[n * C + i], rs[n * C + j], cnt, i == j, eps_cov);
+        G[t] = r;
+        A0[t] = r;
+        if (j == 0) mean[n * C + i] = mean_from_sums((float)rt[n * C + i], rs[n * C + i], cnt);
     }
 }
 
@@ -476,8 +537,10 @@ int launch_sample_shift(const __half* act, ActGeom g, float* shift, cudaStream_t
 // Spatial control (labels != nullptr): one problem per (image, region), z = n * R + r, over the pixels labelled r:
 // outputs [N*R][...]; counts [N*R] = pixels per problem and tmask [N][tiles] = regions present per 32 x 2 tile
 // (k_region_scan, wct.cu).
+// With `rec` the sums go to a statistics record instead (mean, G, A0, dsum unused).
 static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mean, float* G, float* A0, double* dsum,
-                         const uint8_t* labels, int R, const int* counts, const uint16_t* tmask, cudaStream_t st) {
+                         const uint8_t* labels, int R, const int* counts, const uint16_t* tmask, cudaStream_t st,
+                         const StatsRecord* rec = nullptr) {
     static PFN_encodeTiledC enc = nullptr;
     if (!enc) {
         void* ptr = nullptr;
@@ -556,6 +619,13 @@ static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mea
         cov_tc_kernel<false><<<grid, CovCfg::THREADS, CovCfg::SMEM_BYTES, st>>>(mX, p);
     }
     WCTB_CHECK_LAUNCH("cov_tc_kernel");
+    if (rec) {
+        const long long tot = (long long)nprob * g.C * g.C;
+        k_cov_record<<<(unsigned)(cdiv(tot, 256) > 4096 ? 4096 : cdiv(tot, 256)), 256, 0, st>>>(
+            part, psum, shift, g.C, p.nslots, p.ksplit, HW, nprob, rec->n, rec->t, rec->s, rec->S);
+        WCTB_CHECK_LAUNCH("k_cov_record");
+        return 0;
+    }
     k_cov_sums<<<cdiv((long long)nprob * g.C, 256), 256, 0, st>>>(psum, shift, g.C, p.ksplit, HW, nprob * g.C, dsum, mean, counts);
     WCTB_CHECK_LAUNCH("k_cov_sums");
     const long long tot = (long long)nprob * g.C * g.C;
@@ -571,6 +641,25 @@ int launch_mean_cov(const __half* act, ActGeom g, float eps_cov, float* mean, fl
 int launch_mean_cov_regions(const __half* act, ActGeom g, const uint8_t* labels, int R, const int* counts, const uint16_t* tmask,
                             float eps_cov, float* mean, float* G, float* A0, double* dsum, cudaStream_t st) {
     return mean_cov_impl(act, g, eps_cov, mean, G, A0, dsum, labels, R, counts, tmask, st);
+}
+// The record of the rectangle [y0, y0+h) x [x0, x0+w) of a feature batch [N][H][W][C]: the rectangle is a view of the
+// padded planes (base at its first pixel, the planes' strides, dims h x w), so the TMA boxes that stick out of it are
+// zero-filled and every kernel sees a frame of h x w pixels.  The split into CTAs and the sampled shift are those of an
+// h x w frame: the whole-frame rectangle takes today's split, samples and sums.
+int launch_cov_record(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, const StatsRecord& rec,
+                      cudaStream_t st) {
+    ActGeom v(N, H, W, C);
+    v.H = h;
+    v.W = w;
+    const __half* base = act + ((long long)y0 * v.Wp + x0) * C;
+    return mean_cov_impl(base, v, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, 1, nullptr, nullptr, st, &rec);
+}
+int launch_record_cov_finalize(const StatsRecord& rec, int C, int N, float eps_cov, float* mean, float* G, float* A0, cudaStream_t st) {
+    const long long tot = (long long)N * C * C;
+    k_record_cov_finalize<<<(unsigned)(cdiv(tot, 256) > 4096 ? 4096 : cdiv(tot, 256)), 256, 0, st>>>(rec.n, rec.t, rec.s, rec.S, C, N,
+                                                                                                      eps_cov, mean, G, A0);
+    WCTB_CHECK_LAUNCH("k_record_cov_finalize");
+    return 0;
 }
 
 }  // namespace wctb

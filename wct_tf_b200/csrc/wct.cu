@@ -79,21 +79,83 @@ k_chan_moments(const __half* __restrict__ act, ActGeom g, const float* __restric
 
 // mean = t + s / HW, var = S / HW - (s / HW)^2 (biased, tf.nn.moments) with s, S the slot sums of k_chan_moments added in
 // slot order in fp64
-__global__ void k_moments_finalize(const float* __restrict__ part, const float* __restrict__ shift, int C, int nslices, long long HW,
-                                   int total, float* __restrict__ mean, float* __restrict__ var) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    const int n = i / C, c = i - n * C;
-    const float* p = part + (long long)n * nslices * 2 * C + c;
-    double s = 0.0, S = 0.0;
+// (shared with the statistics record of a rectangle, k_moments_record / k_record_moments_finalize)
+__device__ __forceinline__ void moments_slot_sums(const float* __restrict__ p, int C, int nslices, double& s, double& S) {
+    s = 0.0;
+    S = 0.0;
 #pragma unroll 8
     for (int b = 0; b < nslices; ++b) {
         s += (double)p[(long long)b * 2 * C];
         S += (double)p[(long long)b * 2 * C + C];
     }
+}
+__device__ __forceinline__ void moments_from_sums(float shift, double s, double S, long long HW, float& mean, float& var) {
     const double m = s / (double)HW;
-    mean[i] = (float)((double)shift[i] + m);
-    var[i] = (float)fmax(S / (double)HW - m * m, 0.0);
+    mean = (float)((double)shift + m);
+    var = (float)fmax(S / (double)HW - m * m, 0.0);
+}
+__global__ void k_moments_finalize(const float* __restrict__ part, const float* __restrict__ shift, int C, int nslices, long long HW,
+                                   int total, float* __restrict__ mean, float* __restrict__ var) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int n = i / C, c = i - n * C;
+    double s, S;
+    moments_slot_sums(part + (long long)n * nslices * 2 * C + c, C, nslices, s, S);
+    moments_from_sums(shift[i], s, S, HW, mean[i], var[i]);
+}
+// the slots of k_chan_moments -> a statistics record with the diagonal S (layout: stats_record_layout)
+__global__ void k_moments_record(const float* __restrict__ part, const float* __restrict__ shift, int C, int nslices, long long HW,
+                                 int total, StatsRecord rec) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int n = i / C, c = i - n * C;
+    moments_slot_sums(part + (long long)n * nslices * 2 * C + c, C, nslices, rec.s[i], rec.S[i]);
+    rec.t[i] = (double)shift[i];
+    if (c == 0) rec.n[n] = (double)HW;
+}
+__global__ void k_record_moments_finalize(StatsRecord rec, int C, int total, float* __restrict__ mean, float* __restrict__ var) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    moments_from_sums((float)rec.t[i], rec.s[i], rec.S[i], (long long)rec.n[i / C], mean[i], var[i]);
+}
+
+// Accumulate record B into record A (tiled stylisation): B's sums are re-centred on A's shift in fp64,
+//   s_B' = s_B + n_B D,  S_B' = S_B + (D s_B^T + s_B D^T) + n_B D D^T,  D = t_B - t_A,
+// and added to A's.  A record with n = 0 takes B as it is (one accumulate into an empty record is the identity).  Two
+// launches: the S entries read n_A, t_A and s_B before k_record_fold_vec changes A's n, t and s (one block per frame).
+// Explicitly rounded products: no contraction, so entry (i, j) and (j, i) are the same bits.
+__global__ void k_record_fold_S(StatsRecord a, StatsRecord b, int C, int N, int diag) {
+    const long long per = diag ? (long long)C : (long long)C * C;
+    const long long total = (long long)N * per;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const long long n = t / per;
+        const int i = diag ? (int)(t - n * per) : (int)((t - n * per) / C);
+        const int j = diag ? i : (int)((t - n * per) % C);
+        if (a.n[n] == 0.0) {
+            a.S[t] = b.S[t];
+            continue;
+        }
+        const double di = __dsub_rn(b.t[n * C + i], a.t[n * C + i]), dj = __dsub_rn(b.t[n * C + j], a.t[n * C + j]);
+        const double cross = __dadd_rn(__dmul_rn(di, b.s[n * C + j]), __dmul_rn(b.s[n * C + i], dj));
+        const double sb = __dadd_rn(__dadd_rn(b.S[t], cross), __dmul_rn(b.n[n], __dmul_rn(di, dj)));
+        a.S[t] = __dadd_rn(a.S[t], sb);
+    }
+}
+__global__ void __launch_bounds__(256) k_record_fold_vec(StatsRecord a, StatsRecord b, int C) {
+    const int n = blockIdx.x;
+    const bool empty = a.n[n] == 0.0;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        const long long i = (long long)n * C + c;
+        if (empty) {
+            a.s[i] = b.s[i];
+            a.t[i] = b.t[i];
+        } else {
+            const double d = __dsub_rn(b.t[i], a.t[i]);
+            a.s[i] = __dadd_rn(a.s[i], __dadd_rn(b.s[i], __dmul_rn(b.n[n], d)));
+        }
+    }
+    __syncthreads();                            // every thread has read a.n[n]
+    if (threadIdx.x == 0) a.n[n] = __dadd_rn(a.n[n], b.n[n]);
 }
 
 // ---------------------------------------------------------------------------
@@ -663,6 +725,71 @@ static int launch_moments(const __half* act, ActGeom g, float* shift, float* par
     return 0;
 }
 
+// ---------------------------------------------------------------------------
+// Statistics records (tiled stylisation, DESIGN.md §3.3.7): fp64 n [N] | t [N][C] | s [N][C] | S [N][C][C] (diag: [N][C])
+// ---------------------------------------------------------------------------
+size_t stats_record_layout(int C, int N, int diag, size_t* off_n, size_t* off_t, size_t* off_s, size_t* off_S) {
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    const size_t a = take((size_t)N * 8), b = take((size_t)N * C * 8), c = take((size_t)N * C * 8);
+    const size_t d = take((size_t)N * (diag ? (size_t)C : (size_t)C * C) * 8);
+    if (off_n) *off_n = a;
+    if (off_t) *off_t = b;
+    if (off_s) *off_s = c;
+    if (off_S) *off_S = d;
+    return o;
+}
+static StatsRecord stats_record_at(const void* rec, int C, int N, int diag) {
+    size_t a, b, c, d;
+    stats_record_layout(C, N, diag, &a, &b, &c, &d);
+    uint8_t* p = static_cast<uint8_t*>(const_cast<void*>(rec));
+    return StatsRecord{reinterpret_cast<double*>(p + a), reinterpret_cast<double*>(p + b), reinterpret_cast<double*>(p + c),
+                       reinterpret_cast<double*>(p + d)};
+}
+
+int launch_cov_record(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, const StatsRecord& rec,
+                      cudaStream_t st);   // cov_tc.cu
+int launch_record_cov_finalize(const StatsRecord& rec, int C, int N, float eps_cov, float* mean, float* G, float* A0, cudaStream_t st);
+
+int launch_wct_stats_rect(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_stats_rect: C=%d not in {64,128,256,512}", C);
+    return launch_cov_record(act, N, H, W, C, y0, x0, h, w, stats_record_at(record, C, N, 0), st);
+}
+
+// AdaIN's moments of a rectangle: k_sample_shift and k_chan_moments over a view of the padded planes (see launch_cov_record)
+int launch_adain_stats_rect(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_stats_rect: C=%d must be a multiple of 8 (<= 2048)", C);
+    ActGeom v(N, H, W, C);
+    v.H = h;
+    v.W = w;
+    const __half* base = act + ((long long)y0 * v.Wp + x0) * C;
+    const long long HW = (long long)h * w;
+    const int slice = moments_slice(C);
+    const int nslices = cdiv(HW, slice);
+    const size_t nshift = align_up((size_t)N * C, 64);
+    float* scratch = nullptr;
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&scratch), (nshift + (size_t)N * nslices * 2 * C) * sizeof(float), st, 5); if (rc0) return rc0; }
+    float* shift = scratch;
+    float* part = scratch + nshift;
+    int rc = launch_sample_shift(base, v, shift, st);
+    if (rc) return rc;
+    k_chan_moments<<<dim3((unsigned)nslices, (unsigned)N), 256, 0, st>>>(base, v, shift, slice, part);
+    WCTB_CHECK_LAUNCH("k_chan_moments");
+    k_moments_record<<<cdiv((long long)N * C, 256), 256, 0, st>>>(part, shift, C, nslices, HW, N * C, stats_record_at(record, C, N, 1));
+    WCTB_CHECK_LAUNCH("k_moments_record");
+    return 0;
+}
+
+int launch_stats_accumulate(void* rec_a, const void* rec_b, int C, int N, int diag, cudaStream_t st) {
+    const StatsRecord a = stats_record_at(rec_a, C, N, diag), b = stats_record_at(rec_b, C, N, diag);
+    const long long tot = (long long)N * (diag ? (long long)C : (long long)C * C);
+    k_record_fold_S<<<(unsigned)(cdiv(tot, 256) > 4096 ? 4096 : cdiv(tot, 256)), 256, 0, st>>>(a, b, C, N, diag);
+    WCTB_CHECK_LAUNCH("k_record_fold_S");
+    k_record_fold_vec<<<(unsigned)N, 256, 0, st>>>(a, b, C);
+    WCTB_CHECK_LAUNCH("k_record_fold_vec");
+    return 0;
+}
+
 // cross-phase schedule of k_jacobi: 2^lg warp groups, started `stagger` cycles apart (wctb200_debug_set_jacobi)
 // -1 = auto: chosen by measurement (tools/jacobi_bench.py): C=512 -> 4 groups 300 cycles apart (6.76 ms vs 7.80 ms for
 // one group), smaller matrices -> 2 groups 600 cycles apart.
@@ -858,10 +985,21 @@ int launch_wct_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C,
 // Content side of the split transform (wct_apply, wct_apply_blend) in the workspace `w` of wct_layout(C, Nc, 0): means and
 // covariances of the Nc frames, then W_c = A^-1/2 by the matrix-function fast path or the eigensolver.  The kcount slot
 // receives [k_c x Nc | sweeps_c x Nc].
+static int wct_whiten(int Nc, int C, float eps_eig, float thresh, uint8_t* w, const WctWs& L, cudaStream_t st);
 static int wct_content_side(const __half* content, int Nc, int Hc, int Wc, int C, float eps_cov, float eps_eig, float thresh,
                             uint8_t* w, const WctWs& L, cudaStream_t st) {
     double* dsum = reinterpret_cast<double*>(w + L.dsum);
     float* mean = reinterpret_cast<float*>(w + L.mean);
+    float* G = reinterpret_cast<float*>(w + L.G);
+    int* kc = reinterpret_cast<int*>(w + L.kcount);
+    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)Nc * 2 * 4, st));
+    float* A0 = reinterpret_cast<float*>(w + L.A0);
+    int rc = launch_mean_cov(content, ActGeom(Nc, Hc, Wc, C), eps_cov, mean, G, A0, dsum, st);
+    if (rc) return rc;
+    return wct_whiten(Nc, C, eps_eig, thresh, w, L, st);
+}
+// W_c from the covariances G / A0 of wct_content_side (or of a statistics record)
+static int wct_whiten(int Nc, int C, float eps_eig, float thresh, uint8_t* w, const WctWs& L, cudaStream_t st) {
     float* G = reinterpret_cast<float*>(w + L.G);
     float* sigma = reinterpret_cast<float*>(w + L.sigma);
     float* dvec = reinterpret_cast<float*>(w + L.dvec);
@@ -869,13 +1007,10 @@ static int wct_content_side(const __half* content, int Nc, int Hc, int Wc, int C
     float* conv = reinterpret_cast<float*>(w + L.conv);
     int* kc = reinterpret_cast<int*>(w + L.kcount);
     const long long CC = (long long)C * C;
-    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)Nc * 2 * 4, st));
     float* A0 = reinterpret_cast<float*>(w + L.A0);
     float* lam = reinterpret_cast<float*>(w + L.lam);
-    int rc = launch_mean_cov(content, ActGeom(Nc, Hc, Wc, C), eps_cov, mean, G, A0, dsum, st);
-    if (rc) return rc;
     int* ok = reinterpret_cast<int*>(w + L.ok);
-    rc = launch_matfun_ns(A0, C, Nc, /*n_first=*/Nc, thresh, eps_eig, Wcm, ok, kc, st);   // W_c = A^-1/2 where every eigenvalue is kept
+    int rc = launch_matfun_ns(A0, C, Nc, /*n_first=*/Nc, thresh, eps_eig, Wcm, ok, kc, st);   // W_c = A^-1/2 where every eigenvalue is kept
     if (rc < 0) return rc;
     rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, ok);
     if (rc) return rc;
@@ -889,13 +1024,11 @@ static int wct_content_side(const __half* content, int Nc, int Hc, int Wc, int C
 
 // Style side of the split transform after wct_content_side: T = C_s W_c, the split-fp16 operand M and the bias, then
 // out = M x + bias on the tensor cores.  C_s [Ns][C][C] and mean_s [Ns][C] with Ns == 1 (shared) or Ns == Nc (per frame).
-static int wct_colour_apply(const __half* content, int Nc, int Hc, int Wc, int C, const float* Cs, const float* mean_s, int Ns,
-                            float alpha, int readd, uint8_t* w, const WctWs& L, __half* out, cudaStream_t st) {
+static int wct_colour_transform(int Nc, int C, const float* Cs, const float* mean_s, int Ns, float alpha, int readd, uint8_t* w,
+                                const WctWs& L, __half* Msplit, float* bias, cudaStream_t st) {
     const float* mean = reinterpret_cast<const float*>(w + L.mean);
     const float* Wcm = reinterpret_cast<const float*>(w + L.Wc);
     float* T = reinterpret_cast<float*>(w + L.T);
-    __half* Msplit = reinterpret_cast<__half*>(w + L.Msplit);
-    float* bias = reinterpret_cast<float*>(w + L.bias);
     const long long CC = (long long)C * C;
     dim3 gg((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc);
     k_outer_gemm<<<gg, 256, 0, st>>>(Cs, Ns == 1 ? 0 : CC, Wcm, CC, nullptr, 0, T, CC, C);   // T = C_s W_c
@@ -903,6 +1036,14 @@ static int wct_colour_apply(const __half* content, int Nc, int Hc, int Wc, int C
     dim3 gf((unsigned)cdiv(C, 8), (unsigned)Nc);
     k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean_s, Msplit, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform");
+    return 0;
+}
+static int wct_colour_apply(const __half* content, int Nc, int Hc, int Wc, int C, const float* Cs, const float* mean_s, int Ns,
+                            float alpha, int readd, uint8_t* w, const WctWs& L, __half* out, cudaStream_t st) {
+    __half* Msplit = reinterpret_cast<__half*>(w + L.Msplit);
+    float* bias = reinterpret_cast<float*>(w + L.bias);
+    int rc = wct_colour_transform(Nc, C, Cs, mean_s, Ns, alpha, readd, w, L, Msplit, bias, st);
+    if (rc) return rc;
     return launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, Msplit, Nc, nullptr, bias, C, 0, out, st);
 }
 
@@ -935,6 +1076,107 @@ int launch_wct_apply(const __half* content, int Nc, int Hc, int Wc, int C, const
         WCTB_CUDA(cudaMemcpyAsync(k_out + Nc + Ns, kc + Nc, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
         WCTB_CUDA(cudaMemcpyAsync(k_out + 2 * Nc + Ns, ks + Ns, (size_t)Ns * 4, cudaMemcpyDeviceToDevice, st));
     }
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// Transforms from statistics records (tiled stylisation): wct_apply / adain_apply with the content statistics read from a
+// record instead of summed over the content, cut after the transform.  The transform buffer is applied to any feature
+// map of the frame (a tile and its halo).  The steps after the statistics are the ones wct_apply / adain_apply run.
+//   WCT transform:   split-fp16 M [N][2][C][C] | bias fp32 [N][C] | int32 [k_c x N | sweeps_c x N]
+//   AdaIN transform: fp32 mean_c [N][C] | var_c [N][C] | inv [N][C] | ms [N][C]
+// ---------------------------------------------------------------------------
+size_t wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k) {
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    const size_t a = take((size_t)N * 2 * C * C * 2), b = take((size_t)N * C * 4), c = take((size_t)N * 2 * 4);
+    if (off_m) *off_m = a;
+    if (off_bias) *off_bias = b;
+    if (off_k) *off_k = c;
+    return o;
+}
+size_t adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, size_t* off_inv, size_t* off_ms) {
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    const size_t a = take((size_t)N * C * 4), b = take((size_t)N * C * 4), c = take((size_t)N * C * 4), d = take((size_t)N * C * 4);
+    if (off_mean) *off_mean = a;
+    if (off_var) *off_var = b;
+    if (off_inv) *off_inv = c;
+    if (off_ms) *off_ms = d;
+    return o;
+}
+
+int launch_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                                    float eps_eig, float thresh, int readd, void* transform, void* ws, size_t ws_bytes,
+                                    cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_transform_from_stats: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "wct_transform_from_stats: Ns must be 1 or Nc");
+    const WctWs L = wct_layout(C, Nc, 0);
+    if (ws_bytes < L.total) {
+        set_error("wct_transform_from_stats: workspace %zu < %zu bytes", ws_bytes, L.total);
+        return WCTB200_EWS;
+    }
+    uint8_t* w = static_cast<uint8_t*>(ws);
+    size_t off_cs, off_k;
+    style_state_offsets(C, Ns, &off_cs, &off_k);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    int* kc = reinterpret_cast<int*>(w + L.kcount);
+    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)Nc * 2 * 4, st));
+    int rc = launch_record_cov_finalize(stats_record_at(record, C, Nc, 0), C, Nc, eps_cov, reinterpret_cast<float*>(w + L.mean),
+                                        reinterpret_cast<float*>(w + L.G), reinterpret_cast<float*>(w + L.A0), st);
+    if (rc) return rc;
+    rc = wct_whiten(Nc, C, eps_eig, thresh, w, L, st);
+    if (rc) return rc;
+    size_t om, ob, ok;
+    wct_transform_layout(C, Nc, &om, &ob, &ok);
+    uint8_t* tp = static_cast<uint8_t*>(transform);
+    rc = wct_colour_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
+                              w, L, reinterpret_cast<__half*>(tp + om), reinterpret_cast<float*>(tp + ob), st);
+    if (rc) return rc;
+    WCTB_CUDA(cudaMemcpyAsync(tp + ok, kc, (size_t)Nc * 2 * 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+int launch_wct_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, __half* out, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_transform_apply: C=%d not in {64,128,256,512}", C);
+    size_t om, ob;
+    wct_transform_layout(C, N, &om, &ob, nullptr);
+    const uint8_t* tp = static_cast<const uint8_t*>(transform);
+    return launch_conv_tc(CONV_APPLY, act, N, H, W, C, reinterpret_cast<const __half*>(tp + om), N, nullptr,
+                          reinterpret_cast<const float*>(tp + ob), C, 0, out, st);
+}
+
+static size_t adain_state_offsets(int C, int Ns, size_t* off_var);
+int launch_adain_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float eps, void* transform,
+                                      cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_transform_from_stats: C=%d must be a multiple of 8 (<= 2048)", C);
+    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "adain_transform_from_stats: Ns must be 1 or Nc");
+    size_t off_var, a, b, c, d;
+    adain_state_offsets(C, Ns, &off_var);
+    adain_transform_layout(C, Nc, &a, &b, &c, &d);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    uint8_t* tp = static_cast<uint8_t*>(transform);
+    float* mean = reinterpret_cast<float*>(tp + a);
+    float* var = reinterpret_cast<float*>(tp + b);
+    k_record_moments_finalize<<<cdiv((long long)Nc * C, 256), 256, 0, st>>>(stats_record_at(record, C, Nc, 1), C, Nc * C, mean, var);
+    WCTB_CHECK_LAUNCH("k_record_moments_finalize");
+    k_adain_coeffs<<<cdiv((long long)Nc * C, 256), 256, 0, st>>>(var, reinterpret_cast<const float*>(sp), reinterpret_cast<const float*>(sp + off_var),
+                                                              C, Nc, Ns, eps, reinterpret_cast<float*>(tp + c), reinterpret_cast<float*>(tp + d));
+    WCTB_CHECK_LAUNCH("k_adain_coeffs");
+    return 0;
+}
+int launch_adain_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, float alpha, __half* out,
+                                 cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_transform_apply: C=%d must be a multiple of 8 (<= 2048)", C);
+    size_t a, c, d;
+    adain_transform_layout(C, N, &a, nullptr, &c, &d);
+    const uint8_t* tp = static_cast<const uint8_t*>(transform);
+    const long long total = (long long)N * H * W * (C / 8);
+    long long blocks = (total + 255) / 256;
+    if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
+    k_affine_apply<<<(unsigned)blocks, 256, 0, st>>>(act, ActGeom(N, H, W, C), reinterpret_cast<const float*>(tp + a),
+                                                     reinterpret_cast<const float*>(tp + c), reinterpret_cast<const float*>(tp + d),
+                                                     alpha, out);
+    WCTB_CHECK_LAUNCH("k_affine_apply");
     return 0;
 }
 

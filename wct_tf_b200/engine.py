@@ -918,6 +918,135 @@ class Engine(object):
             self.last_info = infos
         return x
 
+    # ------------------------------------------------------------------ tiled stylisation (DESIGN.md §3.3.7)
+    @staticmethod
+    def check_tile_size(tile_size):
+        """The tile edge of a tiled call: a positive multiple of 16 (tile boundaries on the pooling grid of every level);
+        ValueError otherwise."""
+        if isinstance(tile_size, bool) or not isinstance(tile_size, (int, np.integer)) or tile_size <= 0 or tile_size % 16:
+            raise ValueError("tile_size must be a positive multiple of 16, got %r" % (tile_size,))
+        return int(tile_size)
+
+    def stats_record(self, C, adain):
+        """A zeroed statistics record of one frame (n = 0: the empty record that the first accumulate fills)."""
+        nbytes = self.lib.wctb200_stats_record_layout(C, 1, int(adain), None, None, None, None)
+        return torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+
+    def stats_rect(self, feat, y0, x0, h, w, record, adain):
+        """Statistics of the rectangle [y0, y0+h) x [x0, x0+w) of ``feat`` into ``record`` (the covariance sums for WCT, the
+        per-channel moments for AdaIN)."""
+        fn = self.lib.wctb200_adain_stats_rect if adain else self.lib.wctb200_wct_stats_rect
+        self._call("%s_stats_rect[C%d]" % ("adain" if adain else "wct", feat.C), 3, fn, feat.ptr, feat.N, feat.H, feat.W, feat.C,
+                   int(y0), int(x0), int(h), int(w), record.data_ptr(), self._stream(), bytes_=4.0 * feat.C * feat.N * h * w)
+
+    def stats_accumulate(self, rec_a, rec_b, C, adain):
+        self._call("stats_accumulate[C%d]" % C, 2, self.lib.wctb200_stats_accumulate, rec_a.data_ptr(), rec_b.data_ptr(), C, 1,
+                   int(adain), self._stream())
+
+    def transform_from_stats(self, record, C, state, alpha, adain):
+        """The level transform of one frame from its statistics record against the style ``state`` of one style (a WCT
+        state, or AdaIN moments)."""
+        st = self._stream()
+        if adain:
+            tr = torch.empty(self.lib.wctb200_adain_transform_layout(C, 1, None, None, None, None), dtype=torch.uint8, device=self.device)
+            self._call("adain_transform[C%d]" % C, 2, self.lib.wctb200_adain_transform_from_stats, record.data_ptr(), 1, C,
+                       state.data_ptr(), 1, 1e-5, tr.data_ptr(), st)
+            return tr
+        sem = SEMANTICS[self.semantics]
+        tr = torch.empty(self.lib.wctb200_wct_transform_layout(C, 1, None, None, None), dtype=torch.uint8, device=self.device)
+        ws = self._workspace(C, 1, 0)           # keyed by C alone: the tile shapes of a call never add an entry
+        self._call("wct_transform[C%d]" % C, 7 + self._matfun_launches(C), self.lib.wctb200_wct_transform_from_stats,
+                   record.data_ptr(), 1, C, state.data_ptr(), 1, float(alpha), sem["eps_cov"], sem["eps_eig"], sem["thresh"],
+                   sem["readd"], tr.data_ptr(), ws.data_ptr(), ws.numel(), st)
+        return tr
+
+    def transform_apply(self, feat, transform, alpha, adain):
+        out = self._act(feat.N, feat.H, feat.W, feat.C)
+        hw = feat.N * feat.H * feat.W
+        if adain:
+            self._call("adain_transform_apply[C%d]" % feat.C, 1, self.lib.wctb200_adain_transform_apply, feat.ptr, feat.N, feat.H,
+                       feat.W, feat.C, transform.data_ptr(), float(alpha), out.ptr, self._stream(), bytes_=8.0 * feat.C * hw)
+        else:
+            self._call("wct_transform_apply[C%d]" % feat.C, 1, self.lib.wctb200_wct_transform_apply, feat.ptr, feat.N, feat.H,
+                       feat.W, feat.C, transform.data_ptr(), out.ptr, self._stream(), flops=2.0 * feat.C * feat.C * hw,
+                       bytes_=8.0 * feat.C * hw)
+        return out
+
+    def tiled_level(self, x, level_index, state, alpha, adain, tile_size, clip):
+        """One level of tiled stylisation on the float32 image ``x`` [1,H,W,3] against the style ``state`` of one style
+        (DESIGN.md §3.3.7).  Pass A encodes every tile's crop (its interior widened by h_A, clipped to the image) and folds
+        the statistics of the tile's interior feature into one record in tile order; the record becomes the level's
+        transform once.  Pass B encodes every crop widened by h_B, applies the transform to the whole tile feature,
+        decodes, and writes the decoded interior into the output image [1, g ceil(H/g), g ceil(W/g), 3]."""
+        from .model import RELU_LEVEL, tile_grid, tile_halos
+        lvl = self.model.levels[level_index]
+        relu, C = lvl.relu_target, lvl.channels
+        g = 2 ** (RELU_LEVEL[relu] - 1)
+        h_a, h_b = tile_halos(relu)
+        H, W = x.shape[1], x.shape[2]
+        tiles = tile_grid(H, W, tile_size)
+
+        def crop(y0, y1, x0, x1, h):
+            cy0, cx0 = max(0, y0 - h), max(0, x0 - h)
+            return cy0, cx0, x[:, cy0:min(H, y1 + h), cx0:min(W, x1 + h)].contiguous()
+
+        record, part = self.stats_record(C, adain), self.stats_record(C, adain)
+        for y0, y1, x0, x1 in tiles:
+            cy0, cx0, img = crop(y0, y1, x0, x1, h_a)
+            f, _ = self.encode(img, relu)
+            # the interior feature rectangle: [y0/g, ceil(y1/g)) of the whole map, in the crop's coordinates
+            fy0, fx0 = (y0 - cy0) // g, (x0 - cx0) // g
+            self.stats_rect(f, fy0, fx0, -(-y1 // g) - cy0 // g - fy0, -(-x1 // g) - cx0 // g - fx0, part, adain)
+            self.stats_accumulate(record, part, C, adain)
+        transform = self.transform_from_stats(record, C, state, alpha, adain)
+        out = torch.empty((1, g * -(-H // g), g * -(-W // g), 3), dtype=torch.float32, device=self.device)
+        for y0, y1, x0, x1 in tiles:
+            cy0, cx0, img = crop(y0, y1, x0, x1, h_b)
+            f, _ = self.encode(img, relu)
+            dec = self.decode(self.transform_apply(f, transform, alpha, adain), level_index, clip)
+            oy1, ox1 = g * -(-y1 // g), g * -(-x1 // g)
+            out[:, y0:oy1, x0:ox1] = dec[:, y0 - cy0:oy1 - cy0, x0 - cx0:ox1 - cx0]
+        return out
+
+    def stylize_tiled(self, content_u8, style_u8, alpha=1.0, adain=False, tile_size=1024):
+        """``stylize`` in tiles of ``tile_size`` (a positive multiple of 16) at every level, in bounded device memory: the
+        working set follows the largest crop, (tile_size + 2 h_B)^2, not the image.  Each level's statistics are those of
+        the whole image, so the result is the untiled one up to the order in which the statistics are summed, and byte
+        for byte the same when one tile covers the image.  ``style_u8``: a cuda uint8 image batch or a ``PreparedStyle``
+        of 1 or N styles.  The frames run one after another, each with its own statistics; the style side is untiled."""
+        T = self.check_tile_size(tile_size)
+        N = content_u8.shape[0]
+        prepared = isinstance(style_u8, PreparedStyle)
+        n_style = style_u8.n if prepared else style_u8.shape[0]
+        if n_style not in (1, N):
+            raise ValueError("%d styles for %d frames: give one style, or one per frame" % (n_style, N))
+        if prepared:
+            self.check_prepared(style_u8, adain)
+        main = torch.cuda.current_stream(self.device)
+        side = style_u8 if prepared else self._style_side(style_u8, main, wct=not adain, adain=adain)
+        nlev = len(self.model.levels)
+        outs = []
+        for i in range(N):
+            sd = side if n_style == 1 else self.slice_prepared(side, i, i + 1)
+            x = torch.empty((1,) + tuple(content_u8.shape[1:]), dtype=torch.float32, device=self.device)
+            self._call("u8_to_f32", 1, self.lib.wctb200_image_u8_to_f32, content_u8[i].data_ptr(), x.numel(), x.data_ptr(),
+                       self._stream())
+            for lvl in self.model.levels:
+                self._tag = lvl.relu_target
+                if sd.side is not main:
+                    sd.wait(main, lvl.relu_target)
+                state = sd.adain[lvl.relu_target] if adain else sd.wct[lvl.relu_target]
+                # model.py:86: clip between levels; model.py:94: last output unclipped
+                x = self.tiled_level(x, lvl.index, state, alpha, adain, T, clip=lvl.index < nlev - 1)
+            self._tag = None
+            outs.append(x)
+        if prepared:
+            style_u8.record_stream(main)       # a prepared style held by the caller may be dropped while this work is queued
+        elif side.side is not main:
+            side.side.wait_stream(main)        # buffers handed across streams may be recycled only after both are done
+            main.wait_stream(side.side)
+        return outs[0] if N == 1 else torch.cat(outs, dim=0)
+
     def to_u8(self, img_f32):
         """WCT.postprocess (wct.py:66-68)."""
         out = torch.empty(img_f32.shape, dtype=torch.uint8, device=self.device)

@@ -82,6 +82,37 @@ def decoder_plan(relu_target):
     return ops
 
 
+def _spread(ops, d):
+    """Depth (in the pixels after ``ops``) to which a wrong border of depth ``d`` spreads through ``ops``: a 3x3 conv adds 1,
+    an aligned 2x2 pool halves it (rounding up), an upsample doubles it."""
+    for op in ops:
+        if op.kind == "conv":
+            d += 1
+        elif op.kind == "pool":
+            d = -(-d // 2)
+        else:
+            d *= 2
+    return d
+
+
+def tile_halos(relu_target):
+    """Halos of tiled stylisation at level ``relu_target`` (DESIGN.md §3.3.7), in pixels of the level's input image, each a
+    multiple of g = 2^(pools to the relu): (h_A, h_B).  A tile's crop widened by h_A encodes to the same relu feature on the
+    tile's interior as the whole image does; widened by h_B it also decodes to the same image on the interior.  The cut
+    edge of a crop is the wrong border: its depth is walked through ``encoder_plan`` (h_A) and on through
+    ``decoder_plan`` (h_B)."""
+    g = 2 ** (RELU_LEVEL[relu_target] - 1)
+    d_feat = _spread(encoder_plan(relu_target), 0)
+    d_img = _spread(decoder_plan(relu_target), d_feat)
+    return d_feat * g, -(-d_img // g) * g
+
+
+def tile_grid(H, W, T):
+    """Interiors (y0, y1, x0, x1) of the T x T tiles of an H x W image in row-major order; the last row and column end at
+    the image border, so the interiors partition the image."""
+    return [(y0, min(y0 + T, H), x0, min(x0 + T, W)) for y0 in range(0, H, T) for x0 in range(0, W, T)]
+
+
 Level = namedtuple("Level", "index relu_target channels clip_input transform_rule")
 
 

@@ -225,7 +225,7 @@ class WCT(object):
 
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
-                      swap_targets=None, temporal=None):
+                      swap_targets=None, temporal=None, tile_size=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -261,7 +261,23 @@ class WCT(object):
         ``temporal`` (a ``temporal_state``): the N frames are the next N frames of that clip.  They are stylised exactly as
         without it; after the last pass each frame is blended with its stabilised predecessor, warped by the optical flow of
         the content frames, where that flow is confident (DESIGN.md §3.3.6), and the state moves on.  The first frame of a
-        clip, and a frame whose size differs from its predecessor's, come back unchanged.  Not with ``return_float``."""
+        clip, and a frame whose size differs from its predecessor's, come back unchanged.  Not with ``return_float``.
+
+        ``tile_size`` (tiled stylisation, DESIGN.md §3.3.7): a positive multiple of 16; None or 0 is off.  Every level runs
+        in tiles of that edge with crops widened by a halo, so device memory follows the tile, not the image, and images
+        too large for one pass (above about 11 600^2 pixels) can be stylised.  Each level's statistics are still those of
+        the whole image: the result equals the untiled one up to the order of their summation, and byte for byte when one
+        tile covers the image.  The frames of the batch run one after another.  Works with WCT and AdaIN, ``alpha``,
+        ``passes``, prepared styles, ``return_float`` / ``return_device`` / ``out`` and ``synthesize``; not with
+        ``content_mask``, ``style_masks``, ``style_weights``, ``swap5`` / ``swap_targets`` or ``temporal``."""
+        if tile_size is not None and tile_size != 0:
+            Engine.check_tile_size(tile_size)
+            if (content_mask is not None or style_masks is not None or style_weights is not None or swap5
+                    or swap_targets is not None or temporal is not None):
+                raise ValueError("tile_size does not combine with content_mask, style_masks, style_weights, swap5 / "
+                                 "swap_targets or temporal")
+        else:
+            tile_size = None
         if temporal is not None and return_float:
             raise ValueError("temporal stabilisation works on the uint8 frames: not with return_float=True")
         eng = self.engine
@@ -326,6 +342,11 @@ class WCT(object):
 
                 def one_pass(x, first):
                     return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs)
+            elif tile_size is not None:
+                s = style_dev(styles)
+
+                def one_pass(x, first):
+                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size)
             else:
                 s = style_dev(styles)
 
@@ -450,11 +471,11 @@ class WCT(object):
         return self.predict_batch(noise, styles, **kw)
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
-                style_masks=None, swap_targets=None):
+                style_masks=None, swap_targets=None, tile_size=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
-        blend.'''
+        blend.  ``tile_size`` stylises in tiles (``predict_batch``).'''
         s = time.time()
         seen = {}
 
@@ -469,13 +490,16 @@ class WCT(object):
             raise ValueError("swap_targets does not combine with content_mask or style_weights")
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
-                                     swap5=swap5, style_weights=style_weights, content_mask=content_mask)
+                                     swap5=swap5, style_weights=style_weights, content_mask=content_mask,
+                                     tile_size=tile_size)
         elif content_mask is not None:
             kw = {} if style_masks is None else dict(style_masks=style_masks)
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
-                                     swap5=swap5, content_mask=content_mask, **kw)
+                                     swap5=swap5, content_mask=content_mask, tile_size=tile_size, **kw)
         else:
             kw = {} if swap_targets is None else dict(swap_targets=swap_targets)
+            if tile_size is not None:
+                kw["tile_size"] = tile_size
             out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
