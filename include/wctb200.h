@@ -333,6 +333,29 @@ WCTB200_API int wctb200_adain_transform_from_stats(const void* record, int Nc, i
 WCTB200_API int wctb200_adain_transform_apply(const void* act, int N, int H, int W, int C, const void* transform, float alpha,
                                               void* out, void* stream);
 
+/* ---- optimal-transport transform (OST, DESIGN.md §3.3.8) ----------------------
+ * The closed-form Monge map between the content Gaussian N(m_c, A_c) and the style's, in place of WCT's T = C_s W_c:
+ *   M = W_c B^1/2 W_c,  B = S_c C_s C_s S_c,  S_c = E_k diag((lambda + eps_eig)^+1/2) E_k^T,
+ *   out = alpha (M (x - m_c) + m_s) + (1 - alpha) base   (base and the semantics flags as for wctb200_wct_apply).
+ * W_c, the kept set and C_s are wctb200_wct_apply's, so the style state is a wctb200_wct_style_prepare state unchanged.
+ * B^1/2 = V diag(sqrt(max(mu, 0))) V^T has no threshold: the matrix-function fast path where it converges, elsewhere the
+ * singular values of P = S_c C_s (B = P P^T) by the one-sided Jacobi solver, a column below its null level counting as 0.
+ * ost_apply: content SPF16 [Nc,Hc,Wc,C], state of Ns in {1, Nc} styles, out SPF16 [Nc,Hc,Wc,C].  C in {64,128,256,512} and
+ * Ns in {1, Nc}, else WCTB200_EINVAL; ws of wctb200_ost_workspace_bytes(C, Nc) bytes, else WCTB200_EWS.
+ * k_out (device int32 [5*Nc], may be NULL): [k_c x Nc | sweeps_c x Nc | ns_c x Nc | ns_b x Nc | sweeps_b x Nc]: the kept
+ * count and eigensolver sweeps of the content, then 1 where W_c (ns_c) and B^1/2 (ns_b) took the Newton-Schulz fast path
+ * (0: the eigensolver), then the eigensolver sweeps of B (0 on the fast path).
+ * ost_transform_from_stats: ost_apply's transform from a statistics record, in the layout of wctb200_wct_transform_layout
+ * (its int32 slot: [k_c x Nc | sweeps_c x Nc]), applied by wctb200_wct_transform_apply.  A record of whole frames gives
+ * the bytes of wctb200_ost_apply. */
+WCTB200_API size_t wctb200_ost_workspace_bytes(int C, int Nc);
+WCTB200_API int wctb200_ost_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha,
+                                  float eps_cov, float eps_eig, float thresh, int readd_content_mean, void* out, int32_t* k_out,
+                                  void* ws, size_t ws_bytes, void* stream);
+WCTB200_API int wctb200_ost_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha,
+                                                 float eps_cov, float eps_eig, float thresh, int readd_content_mean,
+                                                 void* transform, void* ws, size_t ws_bytes, void* stream);
+
 /*
  * wct_style_swap (ops.py:145-217) + style_swap (ops.py:219-278) for ONE content/style pair: whiten both encodings, take every
  * patch x patch window of the whitened style at `stride` (--ss-patch-size / --ss-stride, stylize.py:33-34), replace every

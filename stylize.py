@@ -31,6 +31,11 @@ memory follows the tile and not the image, with each level's statistics taken ov
 with ``--content-mask``, ``--interp-styles``, ``--swap5`` or ``--swap-targets``; ``--keep-colors``, ``--concat``,
 ``--content-size``, ``--passes`` and ``--noise`` work on the whole image as without it.
 
+Optimal-transport transform: ``--ost`` maps each level's content feature Gaussian onto the style's by the Monge map, the
+covariance-matching map that moves the features least, instead of WCT (DESIGN.md §3.3.8); it keeps more of the content's
+structure at the same ``--alpha``.  Output names are unchanged.  Not with ``--adain``, ``--content-mask`` or
+``--interp-styles``.
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -76,6 +81,8 @@ _FLAGS = [
                               help="one 8-bit grayscale mask per --mask-styles entry: region r takes the pixels of style r in region r")),
     (("--interp-styles",), dict(nargs="+", type=str, default=None, help="1..8 style images to blend (with --interp-weights)")),
     (("--interp-weights",), dict(nargs="+", type=float, default=None, help="one weight >= 0 per --interp-styles entry (normalised)")),
+    (("--ost",), dict(action="store_true", default=False,
+                      help="optimal-transport (Monge) map between the feature Gaussians instead of WCT")),
     (("--tile-size",), dict(type=int, default=0, metavar="T",
                             help="stylise in T x T tiles (a multiple of 16) in bounded device memory, with every level's "
                                  "statistics over the whole image (0: off)")),
@@ -109,6 +116,7 @@ def parse_args(argv=None):
     check_swap_flags(parser, args)
     check_interp_flags(parser, args)
     check_tile_flags(parser, args)
+    check_ost_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
@@ -134,6 +142,15 @@ def check_swap_flags(parser, args):
     for relu in args.swap_targets:
         if relu not in (args.relu_targets or []):
             parser.error("--swap-targets: %s is not one of --relu-targets (%s)" % (relu, " ".join(args.relu_targets or [])))
+
+
+def check_ost_flags(parser, args):
+    """--ost: a transform of the WCT style states; not with --adain, --content-mask or --interp-styles."""
+    if not getattr(args, "ost", False):
+        return
+    for attr, flag in [("adain", "--adain"), ("content_mask", "--content-mask"), ("interp_styles", "--interp-styles")]:
+        if getattr(args, attr, None):
+            parser.error("--ost does not combine with %s" % flag)
 
 
 def check_tile_flags(parser, args):
@@ -326,6 +343,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw["swap_targets"] = list(args.swap_targets)
     if args.tile_size:
         kw["tile_size"] = args.tile_size
+    if args.ost:
+        kw["ost"] = True
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, style_dev, **kw)

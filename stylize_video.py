@@ -17,6 +17,9 @@ Temporal stabilisation: ``--temporal STRENGTH`` (in [0, 1); default 0 = off) ble
 predecessor, warped by the optical flow of the content frames, where that flow is confident (``WCT.temporal_state``,
 DESIGN.md §3.3.6).  This reduces the flicker of frame-by-frame WCT.  Each (clip, style) run has one state, carried across
 batches and through the frame-by-frame path, so ``--batch`` does not change a frame; ``--concat`` comes after it.
+
+Optimal-transport transform: ``--ost`` uses the Monge map between the feature Gaussians instead of WCT at every level
+(DESIGN.md §3.3.8), on the batched and the frame-by-frame path alike.  Not with ``--adain`` or ``--interp-styles``.
 """
 from __future__ import division, print_function
 
@@ -49,7 +52,7 @@ _VIDEO_FLAGS = [
 ]
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
-           "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets")
+           "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost")
 # flags that do not combine with --interp-styles
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat"),
                     ("swap_targets", "--swap-targets")]
@@ -72,6 +75,7 @@ def parse_args(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
     stylize.check_swap_flags(parser, args)
+    stylize.check_ost_flags(parser, args)
     if args.morph:
         if args.interp_styles is None:
             parser.error("--morph needs --interp-styles")
@@ -142,6 +146,7 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
 
     temporal_kw = {} if temporal is None else dict(temporal=temporal)
+    ost_kw = dict(ost=True) if getattr(args, "ost", False) else {}
 
     def coral(style, fr):
         if isinstance(style, list):
@@ -167,7 +172,7 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
             one = weights is not None or not hasattr(style_img, "shape")   # a list of styles, or a prepared style
             out = wct_model.predict_batch(x, style_img if one else style_img[None], alpha=args.alpha,
                                           adain=args.adain, passes=args.passes, return_device=True,
-                                          **dict(interp_kw(first, first + len(frames)), **swap_kw, **temporal_kw))
+                                          **dict(interp_kw(first, first + len(frames)), **swap_kw, **temporal_kw, **ost_kw))
             results = [(out[i], style_img) for i in range(len(frames))]
         else:                                                  # per-frame styles (CORAL) or ragged sizes
             results = []
@@ -175,7 +180,7 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 fr = prep(dimg.to_device(fr, device))
                 style_rgb = coral(style_img, fr) if args.keep_colors else style_img
                 kw = dict(alpha=args.alpha, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True,
-                          **interp_kw(first + j, first + j + 1))
+                          **interp_kw(first + j, first + j + 1), **ost_kw)
                 swap_kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
                 if temporal is not None:           # stabilised after the last pass: all passes in one call
                     o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, passes=args.passes,

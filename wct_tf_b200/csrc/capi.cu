@@ -130,6 +130,11 @@ size_t adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, s
 int launch_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
                                     float eps_eig, float thresh, int readd, void* transform, void* ws, size_t ws_bytes, cudaStream_t st);
 int launch_wct_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, __half* out, cudaStream_t st);
+size_t ost_workspace_bytes(int C, int Nc);
+int launch_ost_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                     float eps_eig, float thresh, int readd, __half* out, int32_t* k_out, void* ws, size_t ws_bytes, cudaStream_t st);
+int launch_ost_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                                    float eps_eig, float thresh, int readd, void* transform, void* ws, size_t ws_bytes, cudaStream_t st);
 int launch_adain_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float eps, void* transform,
                                       cudaStream_t st);
 int launch_adain_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, float alpha, __half* out,
@@ -614,6 +619,26 @@ int wctb200_wct_transform_apply(const void* act, int N, int H, int W, int C, con
     WCTB_REQUIRE(act && transform && out, "wct_transform_apply: null pointer");
     WCTB_REQUIRE(geom_ok(N, H, W, C) && wct_channels_ok(C), "wct_transform_apply: bad geometry");
     return launch_wct_transform_apply(HCP(act), N, H, W, C, transform, HP(out), ST(stream));
+}
+size_t wctb200_ost_workspace_bytes(int C, int Nc) {
+    if (!wct_channels_ok(C) || Nc < 1) return 0;
+    return ost_workspace_bytes(C, Nc);
+}
+int wctb200_ost_apply(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                      float eps_eig, float thresh, int readd_content_mean, void* out, int32_t* k_out, void* ws, size_t ws_bytes,
+                      void* stream) {
+    WCTB_REQUIRE(content && state && out && ws, "ost_apply: null pointer");
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C), "ost_apply: bad geometry");
+    return launch_ost_apply(HCP(content), Nc, Hc, Wc, C, state, Ns, alpha, eps_cov, eps_eig, thresh, readd_content_mean, HP(out),
+                            k_out, ws, ws_bytes, ST(stream));
+}
+int wctb200_ost_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                                     float eps_eig, float thresh, int readd_content_mean, void* transform, void* ws, size_t ws_bytes,
+                                     void* stream) {
+    WCTB_REQUIRE(record && state && transform && ws, "ost_transform_from_stats: null pointer");
+    WCTB_REQUIRE(wct_channels_ok(C) && Nc >= 1, "ost_transform_from_stats: bad arguments");
+    return launch_ost_transform_from_stats(record, Nc, C, state, Ns, alpha, eps_cov, eps_eig, thresh, readd_content_mean, transform,
+                                           ws, ws_bytes, ST(stream));
 }
 size_t wctb200_adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, size_t* off_inv, size_t* off_ms) {
     if (C < 8 || C % 8 != 0 || C > 2048 || N < 1) return 0;

@@ -1145,6 +1145,188 @@ int launch_wct_transform_apply(const __half* act, int N, int H, int W, int C, co
                           reinterpret_cast<const float*>(tp + ob), C, 0, out, st);
 }
 
+// ---------------------------------------------------------------------------
+// Optimal-transport transform (OST, DESIGN.md §3.3.8): the Monge map between the content and style Gaussians,
+//   M = W_c B^1/2 W_c,   B = S_c C_s C_s S_c,   S_c = W_c (A_c + eps_eig I) = E_k (lambda + eps_eig)^+1/2 E_k^T,
+// in place of T = C_s W_c.  The content side (W_c) is wct_apply's and the style state is the WCT state unchanged; B^1/2
+// takes the matrix-function fast path where it converges (thresh = eps = 0: the guard reduces to convergence) and the
+// one-sided Jacobi solver on P = S_c C_s elsewhere (k_root_post: B^1/2 = sum sigma_i u_i u_i^T).  The products are
+// k_outer_gemm's A^T B; every operand is symmetric.
+//   workspace: wct_layout(C, Nc, 0) | S [Nc][C][C] (S_c, then B^1/2) | Q [Nc][C][C] (C_s S_c, then B^1/2 W_c)
+//              | B [Nc][C][C] | Gb [Nc][C][C] (Q, rotated in place by the eigensolver) | ok_b [Nc] | sweeps_b [Nc]
+// ---------------------------------------------------------------------------
+// B^1/2 from the one-sided Jacobi solver run on the columns of P = S_c C_s (B = P P^T) instead of on B: the solver rotates
+// them into g_i = sigma_i u_i with P P^T = sum sigma_i^2 u_i u_i^T, so  B^1/2 = sum sigma_i u_i u_i^T = G diag(1 / |g_i|) G^T.
+// The singular values come out with an absolute error of ~the solver's tolerance times sigma_max; B's eigenvalues would carry
+// that error squared relative to mu_max, and their roots ~1e-4 sqrt(mu_max) on every null direction, which W_c then
+// amplifies by up to 1 / (lambda_min + eps_eig).  A column whose squared norm is below 1e-11 of the largest is one the solver
+// treats as null (k_jacobi's null2: below what fp32 resolves) and gets d = 0: sigma_i = 0, sqrt(max(mu, 0)) of the oracle.
+__global__ void __launch_bounds__(256)
+k_root_post(const float* __restrict__ Gall, int C, float* __restrict__ dvec, const int* __restrict__ skip) {
+    const int prob = blockIdx.x;
+    if (skip && skip[prob]) return;
+    __shared__ float ss_col[512];
+    __shared__ float red[8];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float m = 0.f;
+    for (int col = warp; col < C; col += 8) {
+        const float* g = Gall + ((long long)prob * C + col) * C;
+        float ss = 0.f;
+        for (int i = lane; i < C; i += 32) ss = fmaf(g[i], g[i], ss);
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+        if (lane == 0) ss_col[col] = ss;
+        m = fmaxf(m, ss);
+    }
+    if (lane == 0) red[warp] = m;
+    __syncthreads();
+    float smax = 0.f;
+    for (int i = 0; i < 8; ++i) smax = fmaxf(smax, red[i]);
+    const float floor_ss = 1e-11f * smax;
+    for (int col = threadIdx.x; col < C; col += blockDim.x) {
+        const float ss = ss_col[col];
+        dvec[(long long)prob * C + col] = (ss > floor_ss && ss > 0.f) ? rsqrtf(ss) : 0.f;
+    }
+}
+
+__global__ void k_add_scaled(float* __restrict__ dst, const float* __restrict__ src, float a, long long n) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        dst[i] = fmaf(a, src[i], dst[i]);
+}
+
+struct OstWs {
+    WctWs L;
+    size_t S, Q, B, Gb, okb, swb, total;
+};
+static OstWs ost_layout(int C, int Nc) {
+    OstWs o;
+    o.L = wct_layout(C, Nc, 0);
+    size_t p = o.L.total;
+    auto take = [&](size_t bytes) { size_t r = p; p = align_up(p + bytes, 256); return r; };
+    const size_t mat = (size_t)Nc * C * C * 4;
+    o.S = take(mat);
+    o.Q = take(mat);
+    o.B = take(mat);
+    o.Gb = take(mat);
+    o.okb = take((size_t)Nc * 4);
+    o.swb = take((size_t)Nc * 4);
+    o.total = p;
+    return o;
+}
+size_t ost_workspace_bytes(int C, int Nc) { return ost_layout(C, Nc).total; }
+
+// after wct_content_side / wct_whiten: M into L.T, then the split operand and bias of k_finalize_transform
+static int ost_transform(int Nc, int C, const float* Cs, const float* mean_s, int Ns, float alpha, int readd, float eps_eig,
+                         uint8_t* w, const OstWs& O, __half* Msplit, float* bias, cudaStream_t st) {
+    const WctWs& L = O.L;
+    const long long CC = (long long)C * C;
+    const float* mean = reinterpret_cast<const float*>(w + L.mean);
+    const float* A0 = reinterpret_cast<const float*>(w + L.A0);
+    const float* Wcm = reinterpret_cast<const float*>(w + L.Wc);
+    float* T = reinterpret_cast<float*>(w + L.T);
+    float* S = reinterpret_cast<float*>(w + O.S);
+    float* Q = reinterpret_cast<float*>(w + O.Q);
+    float* B = reinterpret_cast<float*>(w + O.B);
+    float* Gb = reinterpret_cast<float*>(w + O.Gb);
+    int* okb = reinterpret_cast<int*>(w + O.okb);
+    int* swb = reinterpret_cast<int*>(w + O.swb);
+    const dim3 gg((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc);
+    k_outer_gemm<<<gg, 256, 0, st>>>(Wcm, CC, A0, CC, nullptr, 0, S, CC, C);                  // S_c = W_c A_c
+    WCTB_CHECK_LAUNCH("k_outer_gemm(Sc)");
+    if (eps_eig != 0.f) {                                                                     // + eps_eig W_c
+        k_add_scaled<<<cdiv((long long)Nc * CC, 256) > 1024 ? 1024 : cdiv((long long)Nc * CC, 256), 256, 0, st>>>(S, Wcm, eps_eig,
+                                                                                                              (long long)Nc * CC);
+        WCTB_CHECK_LAUNCH("k_add_scaled(Sc)");
+    }
+    k_outer_gemm<<<gg, 256, 0, st>>>(Cs, Ns == 1 ? 0 : CC, S, CC, nullptr, 0, Q, CC, C);      // Q = C_s S_c
+    WCTB_CHECK_LAUNCH("k_outer_gemm(Q)");
+    k_outer_gemm<<<gg, 256, 0, st>>>(Q, CC, Q, CC, nullptr, 0, B, CC, C);                     // B = Q^T Q (bit-symmetric)
+    WCTB_CHECK_LAUNCH("k_outer_gemm(B)");
+    // the rows of Q are the columns of P = S_c C_s: the eigensolver's input where the fast path does not take B
+    WCTB_CUDA(cudaMemcpyAsync(Gb, Q, (size_t)Nc * CC * 4, cudaMemcpyDeviceToDevice, st));
+    // B^1/2 into S: Newton-Schulz where it converges, else the singular values of P by the one-sided Jacobi solver
+    int rc = launch_matfun_ns(B, C, Nc, /*n_first=*/0, /*thresh=*/0.f, /*eps_eig=*/0.f, S, okb, nullptr, st);
+    if (rc < 0) return rc;
+    rc = launch_jacobi(Gb, C, Nc, reinterpret_cast<float*>(w + L.conv), swb, st, okb);
+    if (rc) return rc;
+    k_root_post<<<(unsigned)Nc, 256, 0, st>>>(Gb, C, reinterpret_cast<float*>(w + L.dvec), okb);
+    WCTB_CHECK_LAUNCH("k_root_post");
+    k_outer_gemm<<<gg, 256, 0, st>>>(Gb, CC, Gb, CC, reinterpret_cast<const float*>(w + L.dvec), C, S, CC, C, okb);
+    WCTB_CHECK_LAUNCH("k_outer_gemm(B^1/2)");
+    k_outer_gemm<<<gg, 256, 0, st>>>(S, CC, Wcm, CC, nullptr, 0, Q, CC, C);                   // B^1/2 W_c
+    WCTB_CHECK_LAUNCH("k_outer_gemm(B^1/2 Wc)");
+    k_outer_gemm<<<gg, 256, 0, st>>>(Wcm, CC, Q, CC, nullptr, 0, T, CC, C);                   // M = W_c B^1/2 W_c
+    WCTB_CHECK_LAUNCH("k_outer_gemm(M)");
+    const dim3 gf((unsigned)cdiv(C, 8), (unsigned)Nc);
+    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean_s, Msplit, bias);
+    WCTB_CHECK_LAUNCH("k_finalize_transform");
+    return 0;
+}
+
+int launch_ost_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha,
+                     float eps_cov, float eps_eig, float thresh, int readd, __half* out, int32_t* k_out, void* ws,
+                     size_t ws_bytes, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "ost_apply: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "ost_apply: Ns must be 1 or Nc");
+    const OstWs O = ost_layout(C, Nc);
+    if (ws_bytes < O.total) {
+        set_error("ost_apply: workspace %zu < %zu bytes", ws_bytes, O.total);
+        return WCTB200_EWS;
+    }
+    uint8_t* w = static_cast<uint8_t*>(ws);
+    size_t off_cs, off_k;
+    style_state_offsets(C, Ns, &off_cs, &off_k);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    int rc = wct_content_side(content, Nc, Hc, Wc, C, eps_cov, eps_eig, thresh, w, O.L, st);
+    if (rc) return rc;
+    __half* Msplit = reinterpret_cast<__half*>(w + O.L.Msplit);
+    float* bias = reinterpret_cast<float*>(w + O.L.bias);
+    rc = ost_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
+                       eps_eig, w, O, Msplit, bias, st);
+    if (rc) return rc;
+    rc = launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, Msplit, Nc, nullptr, bias, C, 0, out, st);
+    if (rc) return rc;
+    if (k_out) {
+        // k_out: [k_c x Nc | sweeps_c x Nc | ok_c x Nc | ok_b x Nc | sweeps_b x Nc]
+        WCTB_CUDA(cudaMemcpyAsync(k_out, w + O.L.kcount, (size_t)Nc * 2 * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(k_out + 2 * Nc, w + O.L.ok, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(k_out + 3 * Nc, w + O.okb, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(k_out + 4 * Nc, w + O.swb, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    return 0;
+}
+
+int launch_ost_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
+                                    float eps_eig, float thresh, int readd, void* transform, void* ws, size_t ws_bytes,
+                                    cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "ost_transform_from_stats: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(Ns == 1 || Ns == Nc, "ost_transform_from_stats: Ns must be 1 or Nc");
+    const OstWs O = ost_layout(C, Nc);
+    if (ws_bytes < O.total) {
+        set_error("ost_transform_from_stats: workspace %zu < %zu bytes", ws_bytes, O.total);
+        return WCTB200_EWS;
+    }
+    uint8_t* w = static_cast<uint8_t*>(ws);
+    size_t off_cs, off_k;
+    style_state_offsets(C, Ns, &off_cs, &off_k);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    int* kc = reinterpret_cast<int*>(w + O.L.kcount);
+    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)Nc * 2 * 4, st));
+    int rc = launch_record_cov_finalize(stats_record_at(record, C, Nc, 0), C, Nc, eps_cov, reinterpret_cast<float*>(w + O.L.mean),
+                                        reinterpret_cast<float*>(w + O.L.G), reinterpret_cast<float*>(w + O.L.A0), st);
+    if (rc) return rc;
+    rc = wct_whiten(Nc, C, eps_eig, thresh, w, O.L, st);
+    if (rc) return rc;
+    size_t om, ob, ok;
+    wct_transform_layout(C, Nc, &om, &ob, &ok);
+    uint8_t* tp = static_cast<uint8_t*>(transform);
+    rc = ost_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
+                       eps_eig, w, O, reinterpret_cast<__half*>(tp + om), reinterpret_cast<float*>(tp + ob), st);
+    if (rc) return rc;
+    WCTB_CUDA(cudaMemcpyAsync(tp + ok, kc, (size_t)Nc * 2 * 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
 static size_t adain_state_offsets(int C, int Ns, size_t* off_var);
 int launch_adain_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float eps, void* transform,
                                       cudaStream_t st) {

@@ -409,6 +409,35 @@ class Engine(object):
                    flops=2.0 * C * C * 2 * content.N * hwc, bytes_=4.0 * C * 2 * content.N * hwc)
         return out, kbuf
 
+    def _ost_launches(self, C):
+        """kernels OST adds to the WCT content side: the products of S_c, B and M, B^1/2 by the matrix-function fast path
+        and the eigensolver (Jacobi on P = S_c C_s, k_root_post, outer product), and the eps_eig term"""
+        return 8 + int(SEMANTICS[self.semantics]["eps_eig"] != 0.0) + self._matfun_launches(C)
+
+    def _ost_workspace(self, C, Nc):
+        key = ("ost", self._group, C, Nc)
+        ws = self._ws.get(key)
+        if ws is None:
+            ws = torch.empty(self.lib.wctb200_ost_workspace_bytes(C, Nc), dtype=torch.uint8, device=self.device)
+            self._ws[key] = ws
+        return ws
+
+    def ost_apply(self, content, state, n_style, alpha, want_info=False):
+        """The optimal-transport transform (DESIGN.md §3.3.8) of one level against a WCT style state of ``n_style`` styles.
+        ``want_info``: the int32 k_out [k_c | sweeps_c | ns_c | ns_b | sweeps_b] x N of ``wctb200_ost_apply``."""
+        st = self._stream()
+        sem = SEMANTICS[self.semantics]
+        C = content.C
+        out = self._act(content.N, content.H, content.W, C)
+        ws = self._ost_workspace(C, content.N)
+        kbuf = torch.empty(5 * content.N, dtype=torch.int32, device=self.device) if want_info else None
+        hwc = content.H * content.W
+        self._call("ost_level[C%d]" % C, 9 + self._matfun_launches(C) + self._ost_launches(C), self.lib.wctb200_ost_apply,
+                   content.ptr, content.N, content.H, content.W, C, state.data_ptr(), n_style, float(alpha), sem["eps_cov"],
+                   sem["eps_eig"], sem["thresh"], sem["readd"], out.ptr, kbuf.data_ptr() if want_info else None, ws.data_ptr(),
+                   ws.numel(), st, flops=2.0 * C * C * 2 * content.N * hwc, bytes_=4.0 * C * 2 * content.N * hwc)
+        return out, kbuf
+
     def labels_resize(self, labels, H, W):
         """Device uint8 label maps [N,Hm,Wm] -> [N,H,W] by proportional nearest sampling (spatial control)."""
         out = torch.empty((labels.shape[0], H, W), dtype=torch.uint8, device=self.device)
@@ -489,7 +518,7 @@ class Engine(object):
 
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
-                region_masks=None, swap_targets=None):
+                region_masks=None, swap_targets=None, ost=False):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -522,8 +551,15 @@ class Engine(object):
 
         Style swap at any level: ``swap_targets`` is a list of relu targets at which the style swap replaces WCT / AdaIN,
         with ``ss_alpha``, ``ss_patch_size`` and ``ss_stride``; ``swap5`` is ``swap_targets=["relu5_1"]``.  Not with spatial
-        control or interpolation."""
+        control or interpolation.
+
+        Optimal-transport transform: ``ost=True`` matches each level's content Gaussian to the style's by the Monge map
+        (DESIGN.md §3.3.8) instead of WCT, against the same WCT style states; swap levels still swap.  Not with ``adain``,
+        spatial control (``labels``) or interpolation (``interp_styles``): the blend of states is exact for WCT and AdaIN
+        only because they are affine in the style statistics, and M is not."""
         N = content_u8.shape[0]
+        if ost and (adain or labels is not None or interp_styles is not None):
+            raise ValueError("ost works with WCT style states only: not with adain, labels (spatial control) or interp_styles")
         swap_lv = self.swap_levels(swap5, swap_targets)
         swap5 = swap5 or swap_targets is not None         # the rejections below name both
         if region_masks is not None and labels is None:
@@ -567,7 +603,7 @@ class Engine(object):
             # one style per frame: frame by frame (each frame's swap has its own style side)
             outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
                                  alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
-                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride) for i in range(N)]
+                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost) for i in range(N)]
             return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
         swap = (int(ss_patch_size), int(ss_stride), swap_lv) if swap_lv else None
@@ -589,11 +625,11 @@ class Engine(object):
                     sg = shared
                 else:
                     sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
-                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha)
+                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost)
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
-                                    swap=swap, ss_alpha=ss_alpha)
+                                    swap=swap, ss_alpha=ss_alpha, ost=ost)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -851,9 +887,10 @@ class Engine(object):
             ps.swap[key] = (state, ev)
         return ps.swap[key]
 
-    def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None):
+    def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
-        ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand)."""
+        ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
+        optimal-transport transform instead of WCT at the other levels."""
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
@@ -889,6 +926,8 @@ class Engine(object):
                 if multi is None:
                     if adain:
                         f, kbuf = self.adain_apply(cf, style.adain[relu], n_style, alpha)
+                    elif ost:
+                        f, kbuf = self.ost_apply(cf, style.wct[relu], n_style, alpha, want_info)
                     else:
                         f, kbuf = self.wct_apply(cf, style.wct[relu], n_style, alpha, want_info)
                 elif mode == "regions":
@@ -943,9 +982,9 @@ class Engine(object):
         self._call("stats_accumulate[C%d]" % C, 2, self.lib.wctb200_stats_accumulate, rec_a.data_ptr(), rec_b.data_ptr(), C, 1,
                    int(adain), self._stream())
 
-    def transform_from_stats(self, record, C, state, alpha, adain):
+    def transform_from_stats(self, record, C, state, alpha, adain, ost=False):
         """The level transform of one frame from its statistics record against the style ``state`` of one style (a WCT
-        state, or AdaIN moments)."""
+        state, or AdaIN moments); ``ost``: the optimal-transport transform of a WCT state, in the WCT transform layout."""
         st = self._stream()
         if adain:
             tr = torch.empty(self.lib.wctb200_adain_transform_layout(C, 1, None, None, None, None), dtype=torch.uint8, device=self.device)
@@ -954,6 +993,12 @@ class Engine(object):
             return tr
         sem = SEMANTICS[self.semantics]
         tr = torch.empty(self.lib.wctb200_wct_transform_layout(C, 1, None, None, None), dtype=torch.uint8, device=self.device)
+        if ost:
+            ws = self._ost_workspace(C, 1)
+            self._call("ost_transform[C%d]" % C, 7 + self._matfun_launches(C) + self._ost_launches(C),
+                       self.lib.wctb200_ost_transform_from_stats, record.data_ptr(), 1, C, state.data_ptr(), 1, float(alpha),
+                       sem["eps_cov"], sem["eps_eig"], sem["thresh"], sem["readd"], tr.data_ptr(), ws.data_ptr(), ws.numel(), st)
+            return tr
         ws = self._workspace(C, 1, 0)           # keyed by C alone: the tile shapes of a call never add an entry
         self._call("wct_transform[C%d]" % C, 7 + self._matfun_launches(C), self.lib.wctb200_wct_transform_from_stats,
                    record.data_ptr(), 1, C, state.data_ptr(), 1, float(alpha), sem["eps_cov"], sem["eps_eig"], sem["thresh"],
@@ -972,7 +1017,7 @@ class Engine(object):
                        bytes_=8.0 * feat.C * hw)
         return out
 
-    def tiled_level(self, x, level_index, state, alpha, adain, tile_size, clip):
+    def tiled_level(self, x, level_index, state, alpha, adain, tile_size, clip, ost=False):
         """One level of tiled stylisation on the float32 image ``x`` [1,H,W,3] against the style ``state`` of one style
         (DESIGN.md §3.3.7).  Pass A encodes every tile's crop (its interior widened by h_A, clipped to the image) and folds
         the statistics of the tile's interior feature into one record in tile order; the record becomes the level's
@@ -998,7 +1043,7 @@ class Engine(object):
             fy0, fx0 = (y0 - cy0) // g, (x0 - cx0) // g
             self.stats_rect(f, fy0, fx0, -(-y1 // g) - cy0 // g - fy0, -(-x1 // g) - cx0 // g - fx0, part, adain)
             self.stats_accumulate(record, part, C, adain)
-        transform = self.transform_from_stats(record, C, state, alpha, adain)
+        transform = self.transform_from_stats(record, C, state, alpha, adain, ost)
         out = torch.empty((1, g * -(-H // g), g * -(-W // g), 3), dtype=torch.float32, device=self.device)
         for y0, y1, x0, x1 in tiles:
             cy0, cx0, img = crop(y0, y1, x0, x1, h_b)
@@ -1008,13 +1053,16 @@ class Engine(object):
             out[:, y0:oy1, x0:ox1] = dec[:, y0 - cy0:oy1 - cy0, x0 - cx0:ox1 - cx0]
         return out
 
-    def stylize_tiled(self, content_u8, style_u8, alpha=1.0, adain=False, tile_size=1024):
+    def stylize_tiled(self, content_u8, style_u8, alpha=1.0, adain=False, tile_size=1024, ost=False):
         """``stylize`` in tiles of ``tile_size`` (a positive multiple of 16) at every level, in bounded device memory: the
         working set follows the largest crop, (tile_size + 2 h_B)^2, not the image.  Each level's statistics are those of
         the whole image, so the result is the untiled one up to the order in which the statistics are summed, and byte
         for byte the same when one tile covers the image.  ``style_u8``: a cuda uint8 image batch or a ``PreparedStyle``
-        of 1 or N styles.  The frames run one after another, each with its own statistics; the style side is untiled."""
+        of 1 or N styles.  The frames run one after another, each with its own statistics; the style side is untiled.
+        ``ost``: the optimal-transport transform (DESIGN.md §3.3.8) instead of WCT; not with ``adain``."""
         T = self.check_tile_size(tile_size)
+        if ost and adain:
+            raise ValueError("ost works with WCT style states only: not with adain")
         N = content_u8.shape[0]
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
@@ -1037,7 +1085,7 @@ class Engine(object):
                     sd.wait(main, lvl.relu_target)
                 state = sd.adain[lvl.relu_target] if adain else sd.wct[lvl.relu_target]
                 # model.py:86: clip between levels; model.py:94: last output unclipped
-                x = self.tiled_level(x, lvl.index, state, alpha, adain, T, clip=lvl.index < nlev - 1)
+                x = self.tiled_level(x, lvl.index, state, alpha, adain, T, clip=lvl.index < nlev - 1, ost=ost)
             self._tag = None
             outs.append(x)
         if prepared:

@@ -18,7 +18,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``prepare_style`` / ``load_style`` are new: the style side computed once (or read from a ``.wctstyle`` file) and
     accepted wherever a style image is (wct_tf_b200/prepared.py);
   * ``temporal_state`` / ``predict_batch(temporal=)`` are new: temporal stabilisation of a clip's frames with the optical
-    flow of the content (wct_tf_b200/temporal.py).
+    flow of the content (wct_tf_b200/temporal.py);
+  * ``ost`` is new: the optimal-transport transform (Lu et al., ICCV 2019), the Monge map between the content and style
+    feature Gaussians, in place of WCT at every level.
 """
 from __future__ import annotations
 
@@ -225,7 +227,7 @@ class WCT(object):
 
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
-                      swap_targets=None, temporal=None, tile_size=None):
+                      swap_targets=None, temporal=None, tile_size=None, ost=False):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -269,7 +271,17 @@ class WCT(object):
         the whole image: the result equals the untiled one up to the order of their summation, and byte for byte when one
         tile covers the image.  The frames of the batch run one after another.  Works with WCT and AdaIN, ``alpha``,
         ``passes``, prepared styles, ``return_float`` / ``return_device`` / ``out`` and ``synthesize``; not with
-        ``content_mask``, ``style_masks``, ``style_weights``, ``swap5`` / ``swap_targets`` or ``temporal``."""
+        ``content_mask``, ``style_masks``, ``style_weights``, ``swap5`` / ``swap_targets`` or ``temporal``.
+
+        ``ost`` (optimal-transport transform, DESIGN.md §3.3.8): each level maps the content's feature Gaussian onto the
+        style's by the Monge map, the covariance-matching map that moves the features least, instead of WCT's whitening
+        and colouring; it keeps more of the content's structure at the same ``alpha``.  The style side is WCT's, so image
+        and prepared styles work unchanged.  Works with ``passes``, ``alpha``, ``return_float`` / ``return_device`` /
+        ``out``, ``temporal``, ``tile_size`` and ``swap5`` / ``swap_targets`` (the swap levels swap, the others use OST);
+        not with ``adain``, ``content_mask`` / ``style_masks`` or ``style_weights`` (M is not affine in the style
+        statistics, so the blend of styles does not carry over)."""
+        if ost and (adain or content_mask is not None or style_masks is not None or style_weights is not None):
+            raise ValueError("ost does not combine with adain, content_mask, style_masks or style_weights")
         if tile_size is not None and tile_size != 0:
             Engine.check_tile_size(tile_size)
             if (content_mask is not None or style_masks is not None or style_weights is not None or swap5
@@ -346,7 +358,7 @@ class WCT(object):
                 s = style_dev(styles)
 
                 def one_pass(x, first):
-                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size)
+                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size, ost=ost)
             else:
                 s = style_dev(styles)
 
@@ -355,7 +367,7 @@ class WCT(object):
                     # whole batch in one call; with one style per frame the engine swaps frame by frame.
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
-                                       swap_targets=swap_targets if first else None)
+                                       swap_targets=swap_targets if first else None, ost=ost)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -471,11 +483,11 @@ class WCT(object):
         return self.predict_batch(noise, styles, **kw)
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
-                style_masks=None, swap_targets=None, tile_size=None):
+                style_masks=None, swap_targets=None, tile_size=None, ost=False):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
-        blend.  ``tile_size`` stylises in tiles (``predict_batch``).'''
+        blend.  ``tile_size`` stylises in tiles and ``ost`` uses the optimal-transport transform (``predict_batch``).'''
         s = time.time()
         seen = {}
 
@@ -488,6 +500,8 @@ class WCT(object):
             raise ValueError("style_masks needs content_mask")
         if (style_weights is not None or content_mask is not None) and swap_targets is not None:
             raise ValueError("swap_targets does not combine with content_mask or style_weights")
+        if ost and (adain or content_mask is not None or style_weights is not None):
+            raise ValueError("ost does not combine with adain, content_mask, style_masks or style_weights")
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, style_weights=style_weights, content_mask=content_mask,
@@ -500,6 +514,8 @@ class WCT(object):
             kw = {} if swap_targets is None else dict(swap_targets=swap_targets)
             if tile_size is not None:
                 kw["tile_size"] = tile_size
+            if ost:
+                kw["ost"] = True
             out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
