@@ -104,6 +104,28 @@ def test_capi_exports_every_declared_symbol():
     assert lib.wctb200_wct_workspace_bytes(512, 1, 1) > 6 * 512 * 512 * 4
 
 
+def test_act_bytes_at_the_edges_of_the_accepted_geometries():
+    """An activation is accepted while N (2H+2)(2W+2) C/8 -- the 8-channel groups of its 2x upsampled output -- stays below 2^32
+    (which keeps H W below 2^30); one row, column or frame more is refused (0).  The sizes past 2^32 bytes are exact."""
+    from wct_tf_b200 import _capi
+    lib = _capi.load()
+
+    def act_bytes(n, h, w, c):
+        return 2 * n * (h + 2) * (w + 2) * c * 2
+
+    # square 64-channel frames: (2 * 11584 + 2)^2 * 8 < 2^32 <= (2 * 11585 + 2)(2 * 11584 + 2) * 8
+    assert lib.wctb200_act_bytes(1, 11584, 11584, 64) == act_bytes(1, 11584, 11584, 64)
+    assert lib.wctb200_act_bytes(1, 11585, 11584, 64) == 0
+    assert lib.wctb200_act_bytes(1, 11584, 11585, 64) == 0
+    # batches of 2048^2 at 64 channels: 31 frames (a 66.6 GB buffer) and not 32
+    assert lib.wctb200_act_bytes(31, 2048, 2048, 64) == act_bytes(31, 2048, 2048, 64)
+    assert lib.wctb200_act_bytes(32, 2048, 2048, 64) == 0
+    # a long thin 8-channel map: 6 (2W + 2) < 2^32 <= 6 (2W + 4)
+    w = (1 << 32) // 12 - 1
+    assert lib.wctb200_act_bytes(1, 2, w, 8) == act_bytes(1, 2, w, 8)
+    assert lib.wctb200_act_bytes(1, 2, w + 1, 8) == 0
+
+
 def test_device_string_mapping_and_no_cpu_fallback():
     from wct_tf_b200.wct import _torch_device
     assert _torch_device("/gpu:0") == "cuda:0" and _torch_device("/GPU:3") == "cuda:3"
