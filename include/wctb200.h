@@ -24,6 +24,12 @@
  *   REFLECT padding of ops.py:12-15 (mirror without edge repeat), written by the
  *   producer, so a 3x3 'valid' conv over the padded plane equals Conv2DReflect
  *   (ops.py:17-19).  C must be a multiple of 8; H,W >= 2.
+ *   Halo modes.  Each axis of the halo has one of three modes, named by the interior row (column) that feeds padded row 0
+ *   and the one that feeds row H+1: REFLECT (the default) 1 and H-2; EDGE (WCTB200_HALO_EDGE, the input of
+ *   wctb200_conv3x3_up2) 0 and H-1; WRAP (WCTB200_HALO_WRAP_X / _Y, seamless stylisation) H-1 and 0, so that a conv over
+ *   the padded plane pads that axis circularly.  Corner cells follow from the two axes.  The producers that take flags
+ *   (conv3x3, conv3x3_up2, conv_head_flags) write the mode they are given; every other producer writes REFLECT, and
+ *   wctb200_act_halo rewrites the halo of any activation in any mode.
  */
 #ifndef WCTB200_H
 #define WCTB200_H
@@ -58,6 +64,10 @@ extern "C" {
 #define WCTB200_POOL2    8   /* conv3x3: MaxPooling2D 2x2/2 'same' (vgg_normalised.py:41-42) folded into the epilogue: the
                                 output is [N, ceil(H/2), ceil(W/2), Cout] (>= 2x2) and the full-resolution tensor is never
                                 written -- for conv1_2 / 2_2 / 3_4 / 4_4, whose only consumer is the pool */
+#define WCTB200_HALO_WRAP_X 16  /* conv3x3, conv3x3_up2, conv_head_flags, act_halo: write a WRAPPED halo along x (padded column
+                                   0 holds interior column W-1, column W+1 holds column 0), so the next conv pads x circularly
+                                   (seamless stylisation).  With WCTB200_HALO_EDGE the other axis keeps the edge halo. */
+#define WCTB200_HALO_WRAP_Y 32  /* the same along y (padded row 0 holds interior row H-1, row H+1 holds row 0) */
 
 WCTB200_API int         wctb200_abi_version(void);
 WCTB200_API const char* wctb200_last_error(void);
@@ -71,6 +81,11 @@ WCTB200_API size_t wctb200_act_bytes(int N, int H, int W, int C);
 WCTB200_API int wctb200_act_from_f32(const float* nhwc, int N, int H, int W, int C, void* act, void* stream);
 /* SPF16 -> fp32 NHWC (interior only). */
 WCTB200_API int wctb200_act_to_f32(const void* act, int N, int H, int W, int C, float* nhwc, void* stream);
+/* Rewrites, in place, every halo cell of an SPF16 activation [N,H,W,C] from its interior in the mode of `flags`: 0 =
+ * REFLECT, WCTB200_HALO_EDGE, and the wrap bits WCTB200_HALO_WRAP_X / _Y (see "Halo modes" above).  The interior is not
+ * touched.  Other flag bits are WCTB200_EINVAL.  Seamless stylisation runs it after every transform, whose outputs carry
+ * the reflect halo. */
+WCTB200_API int wctb200_act_halo(void* act, int N, int H, int W, int C, int flags, void* stream);
 
 /* ---- image pre/post: WCT.preprocess / WCT.postprocess (wct.py:60-68) -------- */
 /* out[i] = img[i] / 255 */
@@ -141,13 +156,17 @@ WCTB200_API int wctb200_prep_conv_weights_up2(const float* w_hwio, int Cin, int 
 /* Conv2DReflect 3x3 (+bias, optional ReLU) on tensor cores (wgmma, split-fp16 x3):
  * replaces `Lambda(pad_reflect) -> Conv2D(valid)` of vgg_normalised.py:28-40 and
  * model.py:291.  Cin, Cout multiples of 64.  in/out: SPF16 [N,H,W,Cin] -> [N,H,W,Cout]
- * ([N,ceil(H/2),ceil(W/2),Cout] with WCTB200_POOL2). */
+ * ([N,ceil(H/2),ceil(W/2),Cout] with WCTB200_POOL2).  flags: WCTB200_RELU, WCTB200_HALO_EDGE, WCTB200_POOL2 and the wrap
+ * bits WCTB200_HALO_WRAP_X / _Y, which set the halo mode of the output (the conv reads its input's halo as it is). */
 WCTB200_API int wctb200_conv3x3(const void* act_in, int N, int H, int W, int Cin,
                     const void* w_split, const float* bias, int Cout, int flags,
                     void* act_out, void* stream);
 /* UpSampling2D (nearest x2, model.py:293) followed by Conv2DReflect 3x3 (+bias, optional ReLU), fused: act_in is the
  * LOW-resolution SPF16 [N,H,W,Cin] whose halo is EDGE-replicated (its producer ran with WCTB200_HALO_EDGE), act_out is
- * SPF16 [N,2H,2W,Cout] with the usual reflect halo.  4/9 of the MACs of the unfused pair and no upsampled tensor. */
+ * SPF16 [N,2H,2W,Cout] with the usual reflect halo.  4/9 of the MACs of the unfused pair and no upsampled tensor.
+ * flags: WCTB200_RELU and the wrap bits.  Circular padding of the upsampled map lands on the wrapped low-resolution halo
+ * (u[-1] = u[2W-1] = L[W-1]), so a wrapped axis needs act_in's halo wrapped on that axis (its producer ran with
+ * WCTB200_HALO_EDGE and the wrap bit) and wraps act_out's halo there. */
 WCTB200_API int wctb200_conv3x3_up2(const void* act_in, int N, int H, int W, int Cin,
                         const void* w_up2, const float* bias, int Cout, int flags,
                         void* act_out, void* stream);
@@ -160,6 +179,11 @@ WCTB200_API int wctb200_conv3x3_ref(const void* act_in, int N, int H, int W, int
  * b fp32 [64]; out SPF16 [N,H,W,64]. */
 WCTB200_API int wctb200_conv_head(const float* img, int N, int H, int W, const float* w, const float* b,
                       void* act_out, void* stream);
+/* wctb200_conv_head with halo flags: the wrap bits WCTB200_HALO_WRAP_X / _Y pad the image circularly along those axes
+ * (the head reads it with wrapped indices) and write a wrapped halo along them; the other axes reflect.  flags = 0 is
+ * wctb200_conv_head.  Other bits are WCTB200_EINVAL. */
+WCTB200_API int wctb200_conv_head_flags(const float* img, int N, int H, int W, const float* w, const float* b, int flags,
+                                        void* act_out, void* stream);
 /* Decoder tail: Conv2DReflect Cin->3, no activation (model.py:297-298), optional
  * clip to [0,1] (model.py:86).  w fp32 [9*Cin][3], b fp32 [3]; out fp32 NHWC [N,H,W,3]. */
 WCTB200_API int wctb200_conv_tail(const void* act_in, int N, int H, int W, int Cin, const float* w, const float* b,

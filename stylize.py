@@ -36,6 +36,11 @@ covariance-matching map that moves the features least, instead of WCT (DESIGN.md
 structure at the same ``--alpha``.  Output names are unchanged.  Not with ``--adain``, ``--content-mask`` or
 ``--interp-styles``.
 
+Seamless stylisation: ``--seamless {x,y,xy}`` pads every conv of the content path circularly along those axes (DESIGN.md
+§3.3.9), so the result's opposite edges meet: ``x`` for 360° equirectangular panoramas, ``xy`` for tileable textures
+(``--noise --seamless xy``).  Each wrapped side must be a multiple of 2^P, P the pools up to the deepest relu target (16
+for relu5_1).  Output names are unchanged.  Not with ``--swap5`` or ``--swap-targets``.
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -86,6 +91,8 @@ _FLAGS = [
     (("--tile-size",), dict(type=int, default=0, metavar="T",
                             help="stylise in T x T tiles (a multiple of 16) in bounded device memory, with every level's "
                                  "statistics over the whole image (0: off)")),
+    (("--seamless",), dict(type=str, default=None, choices=["x", "y", "xy"],
+                           help="wrap-around padding along x, y or both: panoramas (x) and tileable textures (xy)")),
     # webcam.py:38; the three --noise-* flags are not in the reference.  Their defaults are filled in by parse_args, so that
     # giving one without --noise can be told from leaving it out.
     (("--noise",), dict(action="store_true", default=False, help="Synthesize textures from noise images")),
@@ -117,6 +124,7 @@ def parse_args(argv=None):
     check_interp_flags(parser, args)
     check_tile_flags(parser, args)
     check_ost_flags(parser, args)
+    check_seamless_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
@@ -151,6 +159,16 @@ def check_ost_flags(parser, args):
     for attr, flag in [("adain", "--adain"), ("content_mask", "--content-mask"), ("interp_styles", "--interp-styles")]:
         if getattr(args, attr, None):
             parser.error("--ost does not combine with %s" % flag)
+
+
+def check_seamless_flags(parser, args):
+    """--seamless: not with the style swap (--swap5, --swap-targets), whose VALID patches are not periodic, or with
+    temporal stabilisation (stylize_video.py --temporal), whose optical flow does not see across the seam."""
+    if getattr(args, "seamless", None) is None:
+        return
+    for attr, flag in [("swap5", "--swap5"), ("swap_targets", "--swap-targets"), ("temporal", "--temporal")]:
+        if getattr(args, attr, None):
+            parser.error("--seamless does not combine with %s" % flag)
 
 
 def check_tile_flags(parser, args):
@@ -345,6 +363,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw["tile_size"] = args.tile_size
     if args.ost:
         kw["ost"] = True
+    if args.seamless:
+        kw["seamless"] = args.seamless
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, style_dev, **kw)
@@ -365,6 +385,8 @@ def make_model(args):
 
 def _stylize_masked(model, content_dev, styles_dev, labels, args, style_masks=None):
     kw = dict(alpha=args.alpha, return_device=True, content_mask=labels)
+    if args.seamless:
+        kw["seamless"] = args.seamless
     if style_masks is not None:
         kw["style_masks"] = style_masks
     result = model.predict_batch(content_dev, styles_dev, **kw)
@@ -410,6 +432,8 @@ def main_interp(args, model, io, dimg, t_start):
     os.makedirs(args.out_path, exist_ok=True)
     device = model.engine.device
     kw = dict(alpha=args.alpha, adain=args.adain, return_device=True, style_weights=np.asarray(args.interp_weights, np.float64))
+    if args.seamless:
+        kw["seamless"] = args.seamless
     written = 0
     prepared = PreparedStyles(model)
     for names, content_dev in _contents(args, io, dimg, device):

@@ -20,6 +20,10 @@ batches and through the frame-by-frame path, so ``--batch`` does not change a fr
 
 Optimal-transport transform: ``--ost`` uses the Monge map between the feature Gaussians instead of WCT at every level
 (DESIGN.md §3.3.8), on the batched and the frame-by-frame path alike.  Not with ``--adain`` or ``--interp-styles``.
+
+Seamless stylisation: ``--seamless {x,y,xy}`` pads the content path circularly (DESIGN.md §3.3.9), e.g. ``x`` for 360°
+clips, on both paths.  Not with ``--temporal`` (the optical flow does not see across the seam), ``--swap5`` or
+``--swap-targets``.
 """
 from __future__ import division, print_function
 
@@ -52,7 +56,7 @@ _VIDEO_FLAGS = [
 ]
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
-           "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost")
+           "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless")
 # flags that do not combine with --interp-styles
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat"),
                     ("swap_targets", "--swap-targets")]
@@ -95,6 +99,7 @@ def parse_args(argv=None):
     stylize.check_prepared_flags(parser, args)
     if not 0.0 <= args.temporal < 1.0:
         parser.error("--temporal must be in [0, 1), got %g" % args.temporal)
+    stylize.check_seamless_flags(parser, args)
     return args
 
 
@@ -146,7 +151,10 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
 
     temporal_kw = {} if temporal is None else dict(temporal=temporal)
-    ost_kw = dict(ost=True) if getattr(args, "ost", False) else {}
+    # --ost and --seamless, on both paths
+    opt_kw = dict(ost=True) if getattr(args, "ost", False) else {}
+    if getattr(args, "seamless", None):
+        opt_kw["seamless"] = args.seamless
 
     def coral(style, fr):
         if isinstance(style, list):
@@ -172,7 +180,7 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
             one = weights is not None or not hasattr(style_img, "shape")   # a list of styles, or a prepared style
             out = wct_model.predict_batch(x, style_img if one else style_img[None], alpha=args.alpha,
                                           adain=args.adain, passes=args.passes, return_device=True,
-                                          **dict(interp_kw(first, first + len(frames)), **swap_kw, **temporal_kw, **ost_kw))
+                                          **dict(interp_kw(first, first + len(frames)), **swap_kw, **temporal_kw, **opt_kw))
             results = [(out[i], style_img) for i in range(len(frames))]
         else:                                                  # per-frame styles (CORAL) or ragged sizes
             results = []
@@ -180,7 +188,7 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 fr = prep(dimg.to_device(fr, device))
                 style_rgb = coral(style_img, fr) if args.keep_colors else style_img
                 kw = dict(alpha=args.alpha, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True,
-                          **interp_kw(first + j, first + j + 1), **ost_kw)
+                          **interp_kw(first + j, first + j + 1), **opt_kw)
                 swap_kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
                 if temporal is not None:           # stabilised after the last pass: all passes in one call
                     o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, passes=args.passes,

@@ -13,6 +13,8 @@ RELU = 1
 CLIP01 = 2
 HALO_EDGE = 4
 POOL2 = 8
+HALO_WRAP_X = 16
+HALO_WRAP_Y = 32
 EINVAL, ECUDA, EWS, EDEVICE = -1, -2, -3, -4       # include/wctb200.h
 
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
@@ -25,6 +27,7 @@ SIGNATURES = {
     "wctb200_act_bytes": (_sz, [_i, _i, _i, _i]),
     "wctb200_act_from_f32": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "wctb200_act_to_f32": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    "wctb200_act_halo": (_i, [_vp, _i, _i, _i, _i, _i, _vp]),
     "wctb200_image_u8_to_f32": (_i, [_vp, _sz, _vp, _vp]),
     "wctb200_image_f32_to_u8": (_i, [_vp, _sz, _vp, _vp]),
     "wctb200_resize_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i]),
@@ -44,6 +47,7 @@ SIGNATURES = {
     "wctb200_conv3x3_up2": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
     "wctb200_conv3x3_ref": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
     "wctb200_conv_head": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "wctb200_conv_head_flags": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "wctb200_conv_tail": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "wctb200_maxpool2": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "wctb200_upsample2": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),

@@ -97,6 +97,7 @@ int launch_temporal_blend(uint8_t* frames, int N, int H, int W, const uint8_t* p
                           float beta, cudaStream_t st);
 int launch_act_from_f32(const float*, ActGeom, __half*, cudaStream_t);
 int launch_act_to_f32(const __half*, ActGeom, float*, cudaStream_t);
+int launch_act_halo(__half*, ActGeom, cudaStream_t);
 int launch_prep_weights(const float*, int, int, int, __half*, cudaStream_t);
 int launch_prep_weights_up2(const float*, int, int, __half*, cudaStream_t);
 size_t style_swap_workspace_bytes(int C, int Hc, int Wc, int Hs, int Ws, int P, int S);
@@ -140,7 +141,7 @@ int launch_adain_transform_from_stats(const void* record, int Nc, int C, const v
 int launch_adain_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, float alpha, __half* out,
                                  cudaStream_t st);
 int launch_conv3x3_ref(const __half*, ActGeom, const float*, const float*, int, int, __half*, cudaStream_t);
-int launch_conv_head(const float*, int, int, int, const float*, const float*, __half*, cudaStream_t);
+int launch_conv_head(const float*, int, int, int, const float*, const float*, int, __half*, cudaStream_t);
 int launch_conv_tail(const __half*, ActGeom, const float*, const float*, int, float*, cudaStream_t);
 int launch_maxpool2(const __half*, ActGeom, __half*, cudaStream_t);
 int launch_upsample2(const __half*, ActGeom, __half*, cudaStream_t);
@@ -235,6 +236,14 @@ int wctb200_act_from_f32(const float* nhwc, int N, int H, int W, int C, void* ac
 int wctb200_act_to_f32(const void* act, int N, int H, int W, int C, float* nhwc, void* stream) {
     WCTB_REQUIRE(geom_ok(N, H, W, C) && nhwc && act, "act_to_f32: bad arguments");
     return launch_act_to_f32(HCP(act), ActGeom(N, H, W, C), nhwc, ST(stream));
+}
+int wctb200_act_halo(void* act, int N, int H, int W, int C, int flags, void* stream) {
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && act, "act_halo: bad arguments");
+    WCTB_REQUIRE((flags & ~(WCTB200_HALO_EDGE | WCTB200_HALO_WRAP_X | WCTB200_HALO_WRAP_Y)) == 0, "act_halo: unknown flag bits 0x%x",
+                 flags);
+    ActGeom g(N, H, W, C);
+    g.set_halo(flags);
+    return launch_act_halo(HP(act), g, ST(stream));
 }
 
 int wctb200_image_u8_to_f32(const uint8_t* img, size_t count, float* out, void* stream) {
@@ -332,14 +341,16 @@ int wctb200_prep_conv_weights_up2(const float* w_hwio, int Cin, int Cout, void* 
 int wctb200_conv3x3(const void* act_in, int N, int H, int W, int Cin, const void* w_split, const float* bias, int Cout,
                     int flags, void* act_out, void* stream) {
     WCTB_REQUIRE(act_in && w_split && act_out, "conv3x3: null pointer");
-    WCTB_REQUIRE((flags & ~(WCTB200_RELU | WCTB200_HALO_EDGE | WCTB200_POOL2)) == 0, "conv3x3: unknown flag bits 0x%x", flags);
+    WCTB_REQUIRE((flags & ~(WCTB200_RELU | WCTB200_HALO_EDGE | WCTB200_POOL2 | WCTB200_HALO_WRAP_X | WCTB200_HALO_WRAP_Y)) == 0,
+                 "conv3x3: unknown flag bits 0x%x", flags);
     return launch_conv_tc(CONV_3X3, HCP(act_in), N, H, W, Cin, HCP(w_split), 1, weight_scale_ptr(HCP(w_split), 9, Cin, Cout),
                           bias, Cout, flags, HP(act_out), ST(stream));
 }
 int wctb200_conv3x3_up2(const void* act_in, int N, int H, int W, int Cin, const void* w_up2, const float* bias, int Cout,
                         int flags, void* act_out, void* stream) {
     WCTB_REQUIRE(act_in && w_up2 && act_out, "conv3x3_up2: null pointer");
-    WCTB_REQUIRE((flags & ~WCTB200_RELU) == 0, "conv3x3_up2: unknown flag bits 0x%x", flags);
+    WCTB_REQUIRE((flags & ~(WCTB200_RELU | WCTB200_HALO_WRAP_X | WCTB200_HALO_WRAP_Y)) == 0, "conv3x3_up2: unknown flag bits 0x%x",
+                 flags);
     WCTB_REQUIRE(geom_ok(N, 2 * H, 2 * W, Cout), "conv3x3_up2: output geometry too large");
     return launch_conv_tc(CONV_UP2, HCP(act_in), N, H, W, Cin, HCP(w_up2), 1, weight_scale_ptr(HCP(w_up2), 16, Cin, Cout),
                           bias, Cout, flags, HP(act_out), ST(stream));
@@ -351,7 +362,13 @@ int wctb200_conv3x3_ref(const void* act_in, int N, int H, int W, int Cin, const 
 }
 int wctb200_conv_head(const float* img, int N, int H, int W, const float* w, const float* b, void* act_out, void* stream) {
     WCTB_REQUIRE(img && w && b && act_out && geom_ok(N, H, W, 64), "conv_head: bad arguments");
-    return launch_conv_head(img, N, H, W, w, b, HP(act_out), ST(stream));
+    return launch_conv_head(img, N, H, W, w, b, 0, HP(act_out), ST(stream));
+}
+int wctb200_conv_head_flags(const float* img, int N, int H, int W, const float* w, const float* b, int flags, void* act_out,
+                            void* stream) {
+    WCTB_REQUIRE(img && w && b && act_out && geom_ok(N, H, W, 64), "conv_head_flags: bad arguments");
+    WCTB_REQUIRE((flags & ~(WCTB200_HALO_WRAP_X | WCTB200_HALO_WRAP_Y)) == 0, "conv_head_flags: unknown flag bits 0x%x", flags);
+    return launch_conv_head(img, N, H, W, w, b, flags, HP(act_out), ST(stream));
 }
 int wctb200_conv_tail(const void* act_in, int N, int H, int W, int Cin, const float* w, const float* b, int flags,
                       float* img_out, void* stream) {

@@ -63,17 +63,31 @@ int device_sm_count();
 // ---------------------------------------------------------------------------
 // SPF16 geometry
 // ---------------------------------------------------------------------------
+// Halo written by a producer, per axis: the interior row that feeds padded row 0 (ht) and the one that feeds padded row
+// H+1 (hb), and the interior columns that feed padded columns 0 (wl) and W+1 (wr).
+//   REFLECT (ops.py:12-15, the default): 1 and H-2;  EDGE (input of an UP2 conv, WCTB200_HALO_EDGE): 0 and H-1;
+//   WRAP (seamless stylisation, WCTB200_HALO_WRAP_X / _Y): H-1 and 0 -- a wrapped axis wraps whatever else is set.
+// Corner cells follow from the two axes.  In every mode the cell a pixel feeds sits as many rows above it (row 0) as below
+// it (row H+1): ht+1 = H-hb (reflect 2, edge 1, wrap H).
 struct ActGeom {
     int N, H, W, C;
     int Hp, Wp;          // H+2, W+2
-    int edge;            // halo written by a producer: 0 = REFLECT (ops.py:12-15), 1 = EDGE-replicated (input of an UP2 conv)
+    int ht, hb, wl, wr;  // interior sources of the halo rows / columns (above)
     long long P;         // N*Hp*Wp padded positions
     long long plane;     // P*C elements per plane
     __host__ __device__ ActGeom() {}
     __host__ __device__ ActGeom(int n, int h, int w, int c)
-        : N(n), H(h), W(w), C(c), Hp(h + 2), Wp(w + 2), edge(0) {
+        : N(n), H(h), W(w), C(c), Hp(h + 2), Wp(w + 2), ht(1), hb(h - 2), wl(1), wr(w - 2) {
         P = (long long)N * Hp * Wp;
         plane = P * C;
+    }
+    // halo mode from conv flags: WCTB200_HALO_EDGE and the wrap bits (other bits are ignored)
+    __host__ __device__ void set_halo(int flags) {
+        const bool edge = (flags & WCTB200_HALO_EDGE) != 0;
+        if (flags & WCTB200_HALO_WRAP_Y) { ht = H - 1; hb = 0; }
+        else if (edge) { ht = 0; hb = H - 1; }
+        if (flags & WCTB200_HALO_WRAP_X) { wl = W - 1; wr = 0; }
+        else if (edge) { wl = 0; wr = W - 1; }
     }
 };
 
@@ -134,12 +148,11 @@ __device__ __forceinline__ int halo_rows(int y, int H, int* rows) {
 // identical for 9 and for 4 k-iterations per tile.)
 __device__ __forceinline__ void store8_with_halo(__half* __restrict__ act, const ActGeom& g, int n, int y, int x,
                                                  int c0, const Half8& hi, const Half8& lo) {
-    // reflect: padded row 0 mirrors interior row 1, row H+1 mirrors row H-2; edge: they replicate rows 0 and H-1
-    const int m = g.edge ? 0 : 1;
+    // padded row 0 holds interior row g.ht, row H+1 holds row g.hb (ActGeom: reflect, edge or wrap); columns likewise
     __half* p0 = act + (((long long)n * g.Hp + y + 1) * g.Wp + x + 1) * g.C + c0;
     *reinterpret_cast<Half8*>(p0) = hi;
     *reinterpret_cast<Half8*>(p0 + g.plane) = lo;
-    const bool yt = (y == m), yb = (y == g.H - 1 - m), xl = (x == m), xr = (x == g.W - 1 - m);
+    const bool yt = (y == g.ht), yb = (y == g.hb), xl = (x == g.wl), xr = (x == g.wr);
     if (!(yt | yb | xl | xr)) return;
     const long long pitch = (long long)g.Wp * g.C;
     // element offsets from the pixel's own cell to the halo row / column that mirrors it (0 = none)
@@ -159,11 +172,10 @@ __device__ __forceinline__ void store8_with_halo(__half* __restrict__ act, const
 }
 
 // Epilogue variant: the pixel's padded position `ppos` = (n*Hp + y+1)*Wp + x+1 (fits 31 bits) and its border flags
-// (bit0: the pixel mirrors into padded row 0, bit1: into row H+1, bit2: into column 0, bit3: into column W+1) were computed
-// ONCE by the thread that owns the pixel; the 8 lanes that store its channels only add the channel offset.
+// (bit0: the pixel feeds padded row 0, bit1: row H+1, bit2: column 0, bit3: column W+1) were computed ONCE by the thread
+// that owns the pixel; the 8 lanes that store its channels only add the channel offset.
 __device__ __forceinline__ int halo_flags(const ActGeom& g, int y, int x) {
-    const int m = g.edge ? 0 : 1;
-    return (y == m ? 1 : 0) | (y == g.H - 1 - m ? 2 : 0) | (x == m ? 4 : 0) | (x == g.W - 1 - m ? 8 : 0);
+    return (y == g.ht ? 1 : 0) | (y == g.hb ? 2 : 0) | (x == g.wl ? 4 : 0) | (x == g.wr ? 8 : 0);
 }
 __device__ __forceinline__ void store8_at(__half* __restrict__ act, const ActGeom& g, unsigned int ppos, int flags, int c0,
                                           const Half8& hi, const Half8& lo) {
@@ -171,11 +183,11 @@ __device__ __forceinline__ void store8_at(__half* __restrict__ act, const ActGeo
     *reinterpret_cast<Half8*>(p0) = hi;
     *reinterpret_cast<Half8*>(p0 + g.plane) = lo;
     if (flags == 0) return;
-    // a mirrored cell sits (m+1) rows / columns beyond the pixel: reflect m = 1 -> 2 away, edge m = 0 -> 1 away
-    const int d = g.edge ? 1 : 2;
+    // the cell sits ht+1 rows above the pixel (row 0) or as many below it (row H+1; ActGeom); columns likewise
     const long long pitch = (long long)g.Wp * g.C;
-    const long long dy[3] = {0, (flags & 1) ? -d * pitch : 0, (flags & 2) ? d * pitch : 0};
-    const long long dx[3] = {0, (flags & 4) ? -(long long)d * g.C : 0, (flags & 8) ? (long long)d * g.C : 0};
+    const long long ry = g.ht + 1, rx = g.wl + 1;
+    const long long dy[3] = {0, (flags & 1) ? -ry * pitch : 0, (flags & 2) ? ry * pitch : 0};
+    const long long dx[3] = {0, (flags & 4) ? -rx * g.C : 0, (flags & 8) ? rx * g.C : 0};
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
         if (a && dy[a] == 0) continue;
@@ -187,6 +199,11 @@ __device__ __forceinline__ void store8_at(__half* __restrict__ act, const ActGeo
             *reinterpret_cast<Half8*>(q + g.plane) = lo;
         }
     }
+}
+
+// index of padded image coordinate i (-1..n) on an axis of n pixels: reflect (ops.py:12-15) or, with wrap, circular
+__device__ __forceinline__ int pad_index(int i, int n, bool wrap) {
+    return i < 0 ? (wrap ? i + n : -i) : (i >= n ? (wrap ? i - n : 2 * n - 2 - i) : i);
 }
 
 __device__ __forceinline__ void load8(const __half* __restrict__ act, const ActGeom& g, long long pos, int c0,

@@ -2,7 +2,7 @@
 // fp32 image in, SPF16 activation (interior + reflect halo) out.
 //
 // K = 27 is too short for a TMA-fed implicit GEMM (the operand would be 9 boxes of 6 bytes), so the A operand is BUILT in
-// shared memory by four producer warps: thread = pixel, its 3x3x3 reflect-indexed neighbourhood (27 fp32, L1 hits) is scaled
+// shared memory by four producer warps: thread = pixel, its 3x3x3 reflect- (or wrap-) indexed neighbourhood (27 fp32, L1 hits) is scaled
 // by 256 (the [0,1] image would put the lo halves into the fp16 subnormals), split into fp16 hi/lo and written as ONE
 // 128-byte K-major row  [hi k=0..31 | lo k=0..31]  in the 128B-swizzled layout the MMA expects.  With
 //     B rows  0..63  = [w_hi | w_hi]        ->  D[:,  0:64 ) = x_hi w_hi + x_lo w_hi
@@ -37,11 +37,10 @@ struct HeadParams {
     const float* img;
     const float* w;        // [27][64], k = (ky*3 + kx)*3 + ci
     const float* bias;     // [64]
+    int flags;             // WCTB200_HALO_WRAP_X / _Y: circular padding of the image and a wrapped halo on those axes
     __half* out;
     unsigned int* err;
 };
-
-__device__ __forceinline__ int reflect1(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
 __global__ void __launch_bounds__(HeadCfg::THREADS, 2)
 conv_head_tc_kernel(const HeadParams p) {
@@ -120,6 +119,7 @@ conv_head_tc_kernel(const HeadParams p) {
     if (warp < 4) {
         // ---- producers: one pixel per thread ----
         const int i = warp * 32 + lane;                    // row of the A tile
+        const bool wrap_x = (p.flags & WCTB200_HALO_WRAP_X) != 0, wrap_y = (p.flags & WCTB200_HALO_WRAP_Y) != 0;
         uint32_t tg = 0;
         for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x, ++tg) {
             const int s = tg % Cfg::STAGES;
@@ -136,10 +136,10 @@ conv_head_tc_kernel(const HeadParams p) {
                 const float* base = p.img + (long long)n * HW * 3;
 #pragma unroll
                 for (int ky = 0; ky < 3; ++ky) {
-                    const float* row = base + (long long)reflect1(y + ky - 1, p.H) * p.W * 3;
+                    const float* row = base + (long long)pad_index(y + ky - 1, p.H, wrap_y) * p.W * 3;
 #pragma unroll
                     for (int kx = 0; kx < 3; ++kx) {
-                        const float* px = row + reflect1(x + kx - 1, p.W) * 3;
+                        const float* px = row + pad_index(x + kx - 1, p.W, wrap_x) * 3;
 #pragma unroll
                         for (int ci = 0; ci < 3; ++ci) v[(ky * 3 + kx) * 3 + ci] = __ldg(px + ci) * 256.f;
                     }
@@ -166,7 +166,8 @@ conv_head_tc_kernel(const HeadParams p) {
     // ---- consumer warpgroup (warps 4-7): wgmma per 64-row half, D[:, 0:64) + D[:, 64:128) -> fp32 tile -> epilogue ----
     const int t = threadIdx.x - 128;
     const int fr = 16 * (t >> 5) + ((t & 31) >> 2), fc = 2 * (t & 3);
-    const ActGeom go(p.N, p.H, p.W, 64);
+    ActGeom go(p.N, p.H, p.W, 64);
+    go.set_halo(p.flags);
     const float osc = *s_oscale;
     uint8_t* wstg = epi + (warp - 4) * 8192;
     const uint64_t b_desc = gmma_desc_sw128(smem_u32(bsm));
@@ -231,7 +232,8 @@ conv_head_tc_kernel(const HeadParams p) {
 int g_conv_head_tc = 1;          // 0: the SIMT kernel of layers.cu (wctb200_debug_set_conv_head_tc)
 
 // returns 1 when not handled here (caller falls through to the SIMT kernel), 0 on success, < 0 on error
-int launch_conv_head_tc(const float* img, int N, int H, int W, const float* w, const float* b, __half* out, cudaStream_t st) {
+int launch_conv_head_tc(const float* img, int N, int H, int W, const float* w, const float* b, int flags, __half* out,
+                        cudaStream_t st) {
     using Cfg = HeadCfg;
     const ActGeom go(N, H, W, 64);
     if (!g_conv_head_tc || H < 2 || W < 2 || go.P >= (1ll << 31)) return 1;
@@ -242,6 +244,7 @@ int launch_conv_head_tc(const float* img, int N, int H, int W, const float* w, c
     p.img = img;
     p.w = w;
     p.bias = b;
+    p.flags = flags;
     p.out = out;
     p.err = device_error_word();
     WCTB_ENSURE_SMEM(conv_head_tc_kernel, Cfg::SMEM_BYTES);

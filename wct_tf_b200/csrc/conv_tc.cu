@@ -29,7 +29,8 @@
 // weights (wctb200_prep_conv_weights_up2): 16 instead of 36 tap-products per low-resolution pixel (4/9 of the
 // MACs), and the 4x larger upsampled tensor is never written or read.  At the border the reflect padding of the
 // UPSAMPLED image mirrors onto the same low-resolution pixel (u[-1] = u[1] = L[0]), i.e. L needs an EDGE-replicated
-// halo: its producer is launched with WCTB200_HALO_EDGE.
+// halo: its producer is launched with WCTB200_HALO_EDGE.  Under circular padding (seamless stylisation) u[-1] = u[2W-1] =
+// L[W-1], the WRAPPED low-resolution halo: WCTB200_HALO_WRAP_X / _Y override the edge halo on their axis.
 //
 // Precision.  fp32-class accuracy from fp16 tensor-core inputs: x = x_hi + x_lo,
 //   x*w ~= x_hi*w_hi + x_hi*w_lo + x_lo*w_hi     (3 x wgmma f16 x f16, fp32 accumulate in registers)
@@ -65,6 +66,7 @@ struct ConvParams {
     int nsets;
     int tiles_per_image;
     int flags;
+    ActGeom go;           // OUTPUT geometry with its halo mode, made on the host: the epilogue reads it from the parameter bank
     const float* bias;    // [nsets][Cout] or nullptr
     const float* wscale;  // device scalar: 1 / (power-of-two scale the weights were stored with), or nullptr (= 1)
     __half* out;          // SPF16, Cout channels; UP2: [N, 2H, 2W, Cout]
@@ -479,9 +481,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 
         // ---- epilogue warps 9-11: the same tile list and passes as the consumers, one tile hand-off per pass ----
         const int ew = warp - Cfg::CONSUMERS / 32 - 1;
-        const bool up2 = p.mode == CONV_UP2;
-        ActGeom go(p.N, up2 ? 2 * p.H : (p.pool ? (p.H + 1) / 2 : p.H), up2 ? 2 * p.W : (p.pool ? (p.W + 1) / 2 : p.W), p.Cout);
-        go.edge = (p.flags & WCTB200_HALO_EDGE) ? 1 : 0;
+        const ActGeom& go = p.go;
         const bool relu = (p.flags & WCTB200_RELU) != 0;
         const float wsc = p.wscale ? __ldg(p.wscale) : 1.f;
         uint32_t pass = 0;
@@ -712,6 +712,8 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
     p.pool_tx = cdiv(W, 64);
     p.pool_ho = (H + 1) / 2;
     p.flags = flags;
+    p.go = ActGeom(N, mode == CONV_UP2 ? 2 * H : (pool ? (H + 1) / 2 : H), mode == CONV_UP2 ? 2 * W : (pool ? (W + 1) / 2 : W), Cout);
+    p.go.set_halo(flags);
     p.bias = bias;
     p.wscale = wscale;
     p.out = out;

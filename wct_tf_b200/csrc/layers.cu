@@ -63,6 +63,37 @@ __global__ void k_act_to_f32(const __half* __restrict__ act, ActGeom g, float* _
     }
 }
 
+// Rewrites every halo cell of an SPF16 activation from the interior, in the halo mode of g (ActGeom::set_halo): one thread
+// per (halo cell, 8-channel group).  A cell reads only interior cells, so the order of the stores does not matter.  The
+// 2 (W+2) + 2 H halo cells of a frame are numbered top row, bottom row, then the left and right cells of each interior row.
+__global__ void k_act_halo(__half* __restrict__ act, ActGeom g) {
+    const int cg = g.C / 8;
+    const unsigned cells = 2u * (unsigned)g.Wp + 2u * (unsigned)g.H;
+    const long long total = (long long)g.N * cells * cg;
+    // 32-bit index arithmetic (launcher guarantees total < 2^32)
+    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < (unsigned)total; i += gridDim.x * blockDim.x) {
+        const int c0 = (int)(i % (unsigned)cg) * 8;
+        const unsigned t = i / (unsigned)cg;
+        const unsigned k = t % cells;
+        const int n = (int)(t / cells);
+        int py, px;                                   // padded coordinates of the halo cell
+        if (k < 2u * (unsigned)g.Wp) {
+            py = k < (unsigned)g.Wp ? 0 : g.H + 1;
+            px = (int)(k % (unsigned)g.Wp);
+        } else {
+            const unsigned r = k - 2u * (unsigned)g.Wp;
+            py = (int)(r >> 1) + 1;
+            px = (r & 1u) ? g.W + 1 : 0;
+        }
+        const int sy = py == 0 ? g.ht : (py == g.H + 1 ? g.hb : py - 1);
+        const int sx = px == 0 ? g.wl : (px == g.W + 1 ? g.wr : px - 1);
+        const long long src = (((long long)n * g.Hp + sy + 1) * g.Wp + sx + 1) * g.C + c0;
+        const long long dst = (((long long)n * g.Hp + py) * g.Wp + px) * g.C + c0;
+        *reinterpret_cast<Half8*>(act + dst) = *reinterpret_cast<const Half8*>(act + src);
+        *reinterpret_cast<Half8*>(act + g.plane + dst) = *reinterpret_cast<const Half8*>(act + g.plane + src);
+    }
+}
+
 // ---------------------------------------------------------------------------
 // weights: fp32 [taps][Cin][Cout] -> split fp16 [2][Cout][taps*Cin], stored scaled by a power of two
 //   trailer (after the planes): float[0] = 1/scale (undone in the conv epilogue), uint[1] = max|w| bits (scratch).
@@ -175,14 +206,12 @@ __global__ void k_conv3x3_ref(const __half* __restrict__ in, ActGeom gi, const f
 // encoder head: (1x1 preprocess conv folded into) conv1_1 3->64 + ReLU
 //   vgg_normalised.py:25-40.  One thread = one pixel x 8 output channels.
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
-
 // one thread = 4 horizontally adjacent pixels x 8 output channels: each conflict-free LDS.128
 // pair of weights feeds 32 FMAs (the first version, 1 pixel per thread, was shared-memory bound:
 // ncu short_scoreboard + mio_throttle, 2-way bank conflicts on the 32-byte-strided weight reads)
 __global__ void __launch_bounds__(256)
 k_conv_head(const float* __restrict__ img, int N, int H, int W, const float* __restrict__ w,
-            const float* __restrict__ b, __half* __restrict__ out) {
+            const float* __restrict__ b, int flags, __half* __restrict__ out) {
     // weights re-laid out [k][half][group][4] (channel c = 8*group + 4*half + j): the 8 lanes of a
     // quarter-warp read 8 consecutive 16-byte words
     __shared__ __align__(16) float sw[27 * 64];
@@ -193,7 +222,9 @@ k_conv_head(const float* __restrict__ img, int N, int H, int W, const float* __r
     }
     if (threadIdx.x < 64) sb[threadIdx.x] = b[threadIdx.x];
     __syncthreads();
-    const ActGeom go(N, H, W, 64);
+    ActGeom go(N, H, W, 64);
+    go.set_halo(flags);
+    const bool wrap_x = (flags & WCTB200_HALO_WRAP_X) != 0, wrap_y = (flags & WCTB200_HALO_WRAP_Y) != 0;
     const unsigned segs = (unsigned)(W + 3) / 4u;
     const unsigned total = (unsigned)N * (unsigned)H * segs * 8u;
     for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
@@ -210,12 +241,12 @@ k_conv_head(const float* __restrict__ img, int N, int H, int W, const float* __r
             for (int j = 0; j < 4; ++j) acc[p][j] = pack2(sb[g * 8 + 2 * j], sb[g * 8 + 2 * j + 1]);
 #pragma unroll
         for (int ky = 0; ky < 3; ++ky) {
-            const int yy = reflect_idx(y + ky - 1, H);
+            const int yy = pad_index(y + ky - 1, H, wrap_y);
             const float* row = img + ((long long)n * H + yy) * W * 3;
             f32x2 in[6][3];
 #pragma unroll
             for (int j = 0; j < 6; ++j) {
-                int xx = reflect_idx(xs + j - 1, W);
+                int xx = pad_index(xs + j - 1, W, wrap_x);
                 xx = min(max(xx, 0), W - 1);                 // columns past the ragged right edge: any valid address
 #pragma unroll
                 for (int ci = 0; ci < 3; ++ci) {
@@ -539,6 +570,11 @@ int launch_act_from_f32(const float* in, ActGeom g, __half* act, cudaStream_t st
     WCTB_CHECK_LAUNCH("k_act_from_f32");
     return 0;
 }
+int launch_act_halo(__half* act, ActGeom g, cudaStream_t st) {
+    k_act_halo<<<grid_for((long long)g.N * (2ll * g.Wp + 2ll * g.H) * (g.C / 8), 256), 256, 0, st>>>(act, g);
+    WCTB_CHECK_LAUNCH("k_act_halo");
+    return 0;
+}
 int launch_act_to_f32(const __half* act, ActGeom g, float* out, cudaStream_t st) {
     k_act_to_f32<<<grid_for((long long)g.N * g.H * g.W * (g.C / 8), 256), 256, 0, st>>>(act, g, out);
     WCTB_CHECK_LAUNCH("k_act_to_f32");
@@ -570,13 +606,15 @@ int launch_conv3x3_ref(const __half* in, ActGeom gi, const float* w, const float
     WCTB_CHECK_LAUNCH("k_conv3x3_ref");
     return 0;
 }
-int launch_conv_head_tc(const float* img, int N, int H, int W, const float* w, const float* b, __half* out, cudaStream_t st);
-int launch_conv_head(const float* img, int N, int H, int W, const float* w, const float* b, __half* out, cudaStream_t st) {
+int launch_conv_head_tc(const float* img, int N, int H, int W, const float* w, const float* b, int flags, __half* out,
+                        cudaStream_t st);
+int launch_conv_head(const float* img, int N, int H, int W, const float* w, const float* b, int flags, __half* out,
+                     cudaStream_t st) {
     {
-        const int rc = launch_conv_head_tc(img, N, H, W, w, b, out, st);      // tensor-core head (conv_head_tc.cu)
+        const int rc = launch_conv_head_tc(img, N, H, W, w, b, flags, out, st);      // tensor-core head (conv_head_tc.cu)
         if (rc <= 0) return rc;
     }
-    k_conv_head<<<grid_for((long long)N * H * ((W + 3) / 4) * 8, 256), 256, 0, st>>>(img, N, H, W, w, b, out);
+    k_conv_head<<<grid_for((long long)N * H * ((W + 3) / 4) * 8, 256), 256, 0, st>>>(img, N, H, W, w, b, flags, out);
     WCTB_CHECK_LAUNCH("k_conv_head");
     return 0;
 }

@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import _capi
-from .model import WCTModel, RELU_CHANNELS
+from .model import WCTModel, RELU_CHANNELS, check_seamless, seamless_axes
 from .prepared import (PreparedStyle, SEMANTIC_KEYS, encoder_fingerprints, slice_act_planes, slice_adain_state,
                        slice_wct_state)
 
@@ -172,16 +172,29 @@ class Engine(object):
         return ws
 
     # ------------------------------------------------------------------ layers
-    def encode(self, img, target, taps=()):
+    @staticmethod
+    def wrap_flags(seamless):
+        """The halo flag bits of a seamless mode (None, "x", "y", "xy"; DESIGN.md §3.3.9)."""
+        wx, wy = seamless_axes(seamless)
+        return (_capi.HALO_WRAP_X if wx else 0) | (_capi.HALO_WRAP_Y if wy else 0)
+
+    def halo(self, act, flags):
+        """Rewrite the halo of ``act`` in place in the mode of ``flags`` (the wrap bits; wctb200_act_halo)."""
+        self._call("act_halo[C%d]" % act.C, 1, self.lib.wctb200_act_halo, act.ptr, act.N, act.H, act.W, act.C, flags,
+                   self._stream(), bytes_=8.0 * act.C * act.N * (2 * (act.W + 2) + 2 * act.H))
+
+    def encode(self, img, target, taps=(), seamless=None):
         """img: float32 cuda tensor [N,H,W,3] in [0,1].  Runs the shared encoder up to
-        ``target`` (vgg_normalised.py:22-50); returns (act_at_target, {tap: act})."""
+        ``target`` (vgg_normalised.py:22-50); returns (act_at_target, {tap: act}).  ``seamless`` ("x", "y", "xy"):
+        every conv pads the wrapped axes circularly (DESIGN.md §3.3.9)."""
         N, H, W, _ = img.shape
         st = self._stream()
         lib = self.lib
+        wrap = self.wrap_flags(seamless)
         x = self._act(N, H, W, 64)
-        self._call("conv_head", 1, lib.wctb200_conv_head, img.data_ptr(), N, H, W, self.head_w.data_ptr(),
-                   self.head_b.data_ptr(), x.ptr, st, flops=2.0 * 27 * 64 * N * H * W,
-                   bytes_=N * H * W * (12.0 + 64 * 4))
+        head = (lib.wctb200_conv_head_flags, img.data_ptr(), N, H, W, self.head_w.data_ptr(), self.head_b.data_ptr(), wrap) if wrap \
+            else (lib.wctb200_conv_head, img.data_ptr(), N, H, W, self.head_w.data_ptr(), self.head_b.data_ptr())
+        self._call("conv_head", 1, *head, x.ptr, st, flops=2.0 * 27 * 64 * N * H * W, bytes_=N * H * W * (12.0 + 64 * 4))
         kept = {}
         if "relu1_1" in taps:
             kept["relu1_1"] = x
@@ -197,7 +210,7 @@ class Engine(object):
                 y = self._act(N, (x.H + 1) // 2, (x.W + 1) // 2, op.cout) if pooled else self._act(N, x.H, x.W, op.cout)
                 self._call("conv3x3_%s[%dx%d@%d]" % ("pool" if pooled else "tc", op.cin, op.cout, x.H), 1, lib.wctb200_conv3x3, x.ptr,
                            N, x.H, x.W, op.cin, self.enc_w[op.name].data_ptr(), self.enc_b[op.name].data_ptr(), op.cout,
-                           _capi.RELU | (_capi.POOL2 if pooled else 0), y.ptr, st, flops=2.0 * 9 * op.cin * op.cout * N * x.H * x.W,
+                           _capi.RELU | (_capi.POOL2 if pooled else 0) | wrap, y.ptr, st, flops=2.0 * 9 * op.cin * op.cout * N * x.H * x.W,
                            bytes_=4.0 * N * (x.H * x.W * op.cin + y.H * y.W * op.cout))
                 x = y
                 skip_pool = pooled
@@ -209,14 +222,18 @@ class Engine(object):
                 y = self._act(N, (x.H + 1) // 2, (x.W + 1) // 2, x.C)
                 self._call("maxpool2", 1, lib.wctb200_maxpool2, x.ptr, N, x.H, x.W, x.C, y.ptr, st,
                            bytes_=4.0 * N * x.C * (x.H * x.W + y.H * y.W))
+                if wrap:
+                    self.halo(y, wrap)
                 x = y
         return x, kept
 
-    def decode(self, feat, level_index, clip):
+    def decode(self, feat, level_index, clip, seamless=None):
         """Run decoder ``level_index`` (model.py:279-300) -> float32 image [N,H',W',3];
-        ``clip`` applies model.py:86's clip_by_value(0,1)."""
+        ``clip`` applies model.py:86's clip_by_value(0,1).  ``seamless``: the wrapped axes of ``encode``; ``feat``'s halo
+        must already be wrapped on them."""
         st = self._stream()
         lib = self.lib
+        wrap = self.wrap_flags(seamless)
         relu = self.model.levels[level_index].relu_target
         x = feat
         N = x.N
@@ -230,11 +247,13 @@ class Engine(object):
                 y = self._act(N, x.H * 2, x.W * 2, x.C)
                 self._call("upsample2", 1, lib.wctb200_upsample2, x.ptr, N, x.H, x.W, x.C, y.ptr, st,
                            bytes_=4.0 * N * x.C * x.H * x.W * 5)
+                if wrap:
+                    self.halo(y, wrap)
                 x = y
             elif op.act:
                 # a conv whose output feeds a folded upsample writes an EDGE-replicated halo (conv_tc.cu, mode UP2)
                 edge = self.fuse_upsample and i + 1 < len(ops) and self._fused_up(ops, i + 1)
-                flags = _capi.RELU | (_capi.HALO_EDGE if edge else 0)
+                flags = _capi.RELU | (_capi.HALO_EDGE if edge else 0) | wrap
                 if pending_up:
                     y = self._act(N, 2 * x.H, 2 * x.W, op.cout)
                     self._call("conv3x3_up2[%dx%d@%d]" % (op.cin, op.cout, y.H), 1, lib.wctb200_conv3x3_up2, x.ptr, N, x.H, x.W,
@@ -518,7 +537,7 @@ class Engine(object):
 
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
-                region_masks=None, swap_targets=None, ost=False):
+                region_masks=None, swap_targets=None, ost=False, seamless=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -556,8 +575,17 @@ class Engine(object):
         Optimal-transport transform: ``ost=True`` matches each level's content Gaussian to the style's by the Monge map
         (DESIGN.md §3.3.8) instead of WCT, against the same WCT style states; swap levels still swap.  Not with ``adain``,
         spatial control (``labels``) or interpolation (``interp_styles``): the blend of states is exact for WCT and AdaIN
-        only because they are affine in the style statistics, and M is not."""
+        only because they are affine in the style statistics, and M is not.
+
+        Seamless stylisation: ``seamless`` = "x", "y" or "xy" pads every conv of the content path circularly along those
+        axes (DESIGN.md §3.3.9), so the output equals that of the infinitely tiled content and tiles without a seam.  Each
+        wrapped axis must be a multiple of 2^P (P pools up to the deepest target); not with the style swap, whose VALID
+        patches are not periodic.  The style side is unchanged."""
         N = content_u8.shape[0]
+        if seamless is not None:
+            if swap5 or swap_targets is not None:
+                raise ValueError("seamless does not combine with swap5 / swap_targets: the swap's VALID patches are not periodic")
+            check_seamless(seamless, content_u8.shape[1], content_u8.shape[2], self.model.relu_targets)
         if ost and (adain or labels is not None or interp_styles is not None):
             raise ValueError("ost works with WCT style states only: not with adain, labels (spatial control) or interp_styles")
         swap_lv = self.swap_levels(swap5, swap_targets)
@@ -576,7 +604,7 @@ class Engine(object):
                 raise ValueError("interp_weights must be a float32 tensor [1|N, K] on %s" % self.device)
             w = w.contiguous()
             return self._stylize_multi(content_u8, list(interp_styles), alpha, adain, want_info, capture,
-                                       lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]))
+                                       lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]), seamless=seamless)
         if labels is not None:
             if adain or swap5:
                 raise ValueError("spatial control (labels) works with WCT only: not with adain or swap5 / swap_targets")
@@ -591,7 +619,7 @@ class Engine(object):
             if region_masks is not None:
                 region_masks = self.check_region_masks(region_masks, region_styles)
             return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
-                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks)
+                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks, seamless=seamless)
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
         if n_style not in (1, N):
@@ -625,11 +653,12 @@ class Engine(object):
                     sg = shared
                 else:
                     sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
-                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost)
+                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
+                                         seamless=seamless)
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
-                                    swap=swap, ss_alpha=ss_alpha, ost=ost)
+                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -723,7 +752,7 @@ class Engine(object):
                     m.record_stream(side)
         return sides
 
-    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None):
+    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None, seamless=None):
         """``stylize`` with several styles (spatial control, style interpolation): images are prepared once per call, and
         every style side is shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the
         label maps or weight rows); ``masks``: the style masks of spatial control (``_region_sides``)."""
@@ -736,10 +765,12 @@ class Engine(object):
         finally:
             self._group = 0
         if G == 1:
-            out = self._stylize_one(content_u8, None, alpha, adain, want_info, capture, multi=per_frame(0, N) + (sides,))
+            out = self._stylize_one(content_u8, None, alpha, adain, want_info, capture, multi=per_frame(0, N) + (sides,),
+                                    seamless=seamless)
         else:
             out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, adain, False, None,
-                                                                               multi=per_frame(lo, hi) + (sides,)))
+                                                                               multi=per_frame(lo, hi) + (sides,),
+                                                                               seamless=seamless))
         for side in {id(sd.side): sd.side for sd in owned}.values():
             if side is not main:
                 side.wait_stream(main)         # the style states are recycled only after every level used them
@@ -887,10 +918,13 @@ class Engine(object):
             ps.swap[key] = (state, ev)
         return ps.swap[key]
 
-    def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False):
+    def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
+                     seamless=None):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
         ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
-        optimal-transport transform instead of WCT at the other levels."""
+        optimal-transport transform instead of WCT at the other levels; ``seamless``: the wrapped axes of the content path
+        (the transforms write a reflect halo, which is rewritten before the decoder reads it)."""
+        wrap = self.wrap_flags(seamless)
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
@@ -913,7 +947,7 @@ class Engine(object):
         for lvl in self.model.levels:
             relu = lvl.relu_target
             self._tag = relu
-            cf, _ = self.encode(x, relu)
+            cf, _ = self.encode(x, relu, seamless=seamless)
             if swap is not None and relu in swap[2]:      # model.py:148-152: style swap wins over AdaIN / WCT at its levels
                 state, ev = style.swap[(relu,) + swap[:2]]
                 main.wait_event(ev)
@@ -937,13 +971,15 @@ class Engine(object):
                     f, kbuf = self.adain_apply_blend(cf, [sd.adain[relu] for sd in sides], per_frame, alpha)
                 else:
                     f, kbuf = self.wct_apply_blend(cf, [sd.wct[relu] for sd in sides], per_frame, alpha, want_info)
+            if wrap:
+                self.halo(f, wrap)
             infos.append(kbuf)
             if capture is not None:
                 capture.setdefault("level_input", []).append(x)
                 capture.setdefault("content_feat", []).append(cf)
                 capture.setdefault("transformed", []).append(f)
             # model.py:86: clip between levels; model.py:94: last output unclipped
-            x = self.decode(f, lvl.index, clip=(lvl.index < nlev - 1))
+            x = self.decode(f, lvl.index, clip=(lvl.index < nlev - 1), seamless=seamless)
             if capture is not None:
                 capture.setdefault("level_output", []).append(x)
         self._tag = None
@@ -1017,12 +1053,16 @@ class Engine(object):
                        bytes_=8.0 * feat.C * hw)
         return out
 
-    def tiled_level(self, x, level_index, state, alpha, adain, tile_size, clip, ost=False):
+    def tiled_level(self, x, level_index, state, alpha, adain, tile_size, clip, ost=False, seamless=None):
         """One level of tiled stylisation on the float32 image ``x`` [1,H,W,3] against the style ``state`` of one style
         (DESIGN.md §3.3.7).  Pass A encodes every tile's crop (its interior widened by h_A, clipped to the image) and folds
         the statistics of the tile's interior feature into one record in tile order; the record becomes the level's
         transform once.  Pass B encodes every crop widened by h_B, applies the transform to the whole tile feature,
-        decodes, and writes the decoded interior into the output image [1, g ceil(H/g), g ceil(W/g), 3]."""
+        decodes, and writes the decoded interior into the output image [1, g ceil(H/g), g ceil(W/g), 3].
+
+        ``seamless`` (DESIGN.md §3.3.9), per wrapped axis: when one tile spans the axis the crop is the whole axis and is
+        encoded with the wrap flag; otherwise the crop is widened by the same halos modulo the image size (a window of the
+        periodic image) and encoded with the reflect halo, which the halos keep out of the interior."""
         from .model import RELU_LEVEL, tile_grid, tile_halos
         lvl = self.model.levels[level_index]
         relu, C = lvl.relu_target, lvl.channels
@@ -1030,15 +1070,28 @@ class Engine(object):
         h_a, h_b = tile_halos(relu)
         H, W = x.shape[1], x.shape[2]
         tiles = tile_grid(H, W, tile_size)
+        wx, wy = seamless_axes(seamless)
+        mod_y, mod_x = wy and tile_size < H, wx and tile_size < W        # wrapped axes cut into tiles
+        crop_mode = ("x" if wx and not mod_x else "") + ("y" if wy and not mod_y else "") or None
+        crop_wrap = self.wrap_flags(crop_mode)
+
+        def span(lo, hi, h, n, modular):
+            """The crop [lo - h, hi + h) of an axis of n pixels: clipped to [0, n), or taken modulo n."""
+            if modular:
+                return lo - h, torch.arange(lo - h, hi + h, device=self.device) % n
+            return max(0, lo - h), slice(max(0, lo - h), min(n, hi + h))
 
         def crop(y0, y1, x0, x1, h):
-            cy0, cx0 = max(0, y0 - h), max(0, x0 - h)
-            return cy0, cx0, x[:, cy0:min(H, y1 + h), cx0:min(W, x1 + h)].contiguous()
+            cy0, ys = span(y0, y1, h, H, mod_y)
+            cx0, xs = span(x0, x1, h, W, mod_x)
+            img = x[:, ys] if isinstance(ys, slice) else x.index_select(1, ys)
+            img = img[:, :, xs] if isinstance(xs, slice) else img.index_select(2, xs)
+            return cy0, cx0, img.contiguous()
 
         record, part = self.stats_record(C, adain), self.stats_record(C, adain)
         for y0, y1, x0, x1 in tiles:
             cy0, cx0, img = crop(y0, y1, x0, x1, h_a)
-            f, _ = self.encode(img, relu)
+            f, _ = self.encode(img, relu, seamless=crop_mode)
             # the interior feature rectangle: [y0/g, ceil(y1/g)) of the whole map, in the crop's coordinates
             fy0, fx0 = (y0 - cy0) // g, (x0 - cx0) // g
             self.stats_rect(f, fy0, fx0, -(-y1 // g) - cy0 // g - fy0, -(-x1 // g) - cx0 // g - fx0, part, adain)
@@ -1047,23 +1100,28 @@ class Engine(object):
         out = torch.empty((1, g * -(-H // g), g * -(-W // g), 3), dtype=torch.float32, device=self.device)
         for y0, y1, x0, x1 in tiles:
             cy0, cx0, img = crop(y0, y1, x0, x1, h_b)
-            f, _ = self.encode(img, relu)
-            dec = self.decode(self.transform_apply(f, transform, alpha, adain), level_index, clip)
+            f, _ = self.encode(img, relu, seamless=crop_mode)
+            t = self.transform_apply(f, transform, alpha, adain)
+            if crop_wrap:
+                self.halo(t, crop_wrap)
+            dec = self.decode(t, level_index, clip, seamless=crop_mode)
             oy1, ox1 = g * -(-y1 // g), g * -(-x1 // g)
             out[:, y0:oy1, x0:ox1] = dec[:, y0 - cy0:oy1 - cy0, x0 - cx0:ox1 - cx0]
         return out
 
-    def stylize_tiled(self, content_u8, style_u8, alpha=1.0, adain=False, tile_size=1024, ost=False):
+    def stylize_tiled(self, content_u8, style_u8, alpha=1.0, adain=False, tile_size=1024, ost=False, seamless=None):
         """``stylize`` in tiles of ``tile_size`` (a positive multiple of 16) at every level, in bounded device memory: the
         working set follows the largest crop, (tile_size + 2 h_B)^2, not the image.  Each level's statistics are those of
         the whole image, so the result is the untiled one up to the order in which the statistics are summed, and byte
         for byte the same when one tile covers the image.  ``style_u8``: a cuda uint8 image batch or a ``PreparedStyle``
         of 1 or N styles.  The frames run one after another, each with its own statistics; the style side is untiled.
-        ``ost``: the optimal-transport transform (DESIGN.md §3.3.8) instead of WCT; not with ``adain``."""
+        ``ost``: the optimal-transport transform (DESIGN.md §3.3.8) instead of WCT; not with ``adain``.  ``seamless``: as for
+        ``stylize`` (``tiled_level``)."""
         T = self.check_tile_size(tile_size)
         if ost and adain:
             raise ValueError("ost works with WCT style states only: not with adain")
         N = content_u8.shape[0]
+        check_seamless(seamless, content_u8.shape[1], content_u8.shape[2], self.model.relu_targets)
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
         if n_style not in (1, N):
@@ -1085,7 +1143,7 @@ class Engine(object):
                     sd.wait(main, lvl.relu_target)
                 state = sd.adain[lvl.relu_target] if adain else sd.wct[lvl.relu_target]
                 # model.py:86: clip between levels; model.py:94: last output unclipped
-                x = self.tiled_level(x, lvl.index, state, alpha, adain, T, clip=lvl.index < nlev - 1, ost=ost)
+                x = self.tiled_level(x, lvl.index, state, alpha, adain, T, clip=lvl.index < nlev - 1, ost=ost, seamless=seamless)
             self._tag = None
             outs.append(x)
         if prepared:

@@ -113,6 +113,30 @@ def tile_grid(H, W, T):
     return [(y0, min(y0 + T, H), x0, min(x0 + T, W)) for y0 in range(0, H, T) for x0 in range(0, W, T)]
 
 
+SEAMLESS_MODES = (None, "x", "y", "xy")
+
+
+def seamless_axes(seamless):
+    """(wrap x, wrap y) of a seamless mode (DESIGN.md §3.3.9): None, "x" (panoramas), "y" or "xy" (tileable textures);
+    ValueError for any other value."""
+    if seamless not in SEAMLESS_MODES:
+        raise ValueError("seamless must be None, 'x', 'y' or 'xy', got %r" % (seamless,))
+    return seamless is not None and "x" in seamless, seamless is not None and "y" in seamless
+
+
+def check_seamless(seamless, H, W, relu_targets):
+    """ValueError unless ``seamless`` is a mode and every wrapped axis of an H x W content is a multiple of 2^P, P the
+    pools up to the deepest of ``relu_targets`` (16 for relu5_1): otherwise a 'same' pool would pair pixels across the
+    seam and the output would not be periodic.  Returns (wrap x, wrap y)."""
+    wx, wy = seamless_axes(seamless)
+    m = 2 ** (max(RELU_LEVEL[r] for r in relu_targets) - 1)
+    for axis, wrapped, size in (("width", wx, W), ("height", wy, H)):
+        if wrapped and size % m:
+            raise ValueError("seamless=%r: the content %s %d is not a multiple of %d (2^pools up to the deepest target): "
+                             "a pool would pair pixels across the seam" % (seamless, axis, size, m))
+    return wx, wy
+
+
 Level = namedtuple("Level", "index relu_target channels clip_input transform_rule")
 
 

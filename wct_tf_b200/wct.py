@@ -20,7 +20,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``temporal_state`` / ``predict_batch(temporal=)`` are new: temporal stabilisation of a clip's frames with the optical
     flow of the content (wct_tf_b200/temporal.py);
   * ``ost`` is new: the optimal-transport transform (Lu et al., ICCV 2019), the Monge map between the content and style
-    feature Gaussians, in place of WCT at every level.
+    feature Gaussians, in place of WCT at every level;
+  * ``seamless`` is new: circular padding of every conv of the content path along x, y or both, for 360° panoramas and
+    tileable textures.
 """
 from __future__ import annotations
 
@@ -31,7 +33,7 @@ import numpy as np
 import torch
 
 from .engine import Engine, SEMANTICS
-from .model import RELU_CHANNELS
+from .model import RELU_CHANNELS, seamless_axes
 from .prepared import PreparedStyle
 
 
@@ -227,7 +229,7 @@ class WCT(object):
 
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
-                      swap_targets=None, temporal=None, tile_size=None, ost=False):
+                      swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -279,7 +281,19 @@ class WCT(object):
         and prepared styles work unchanged.  Works with ``passes``, ``alpha``, ``return_float`` / ``return_device`` /
         ``out``, ``temporal``, ``tile_size`` and ``swap5`` / ``swap_targets`` (the swap levels swap, the others use OST);
         not with ``adain``, ``content_mask`` / ``style_masks`` or ``style_weights`` (M is not affine in the style
-        statistics, so the blend of styles does not carry over)."""
+        statistics, so the blend of styles does not carry over).
+
+        ``seamless`` (seamless stylisation, DESIGN.md §3.3.9): "x" wraps the width (360° equirectangular panoramas), "y"
+        the height, "xy" both (tileable textures, e.g. with ``synthesize``).  Every conv of the content path -- encoder,
+        decoders, and the clip between levels -- pads the wrapped axes circularly, so the output equals, exactly, that of
+        the infinitely tiled content and its opposite edges meet without a seam.  Each wrapped axis must be a multiple of
+        2^P, P the pools up to the deepest target (16 for relu5_1).  The style side is unchanged.  Works with WCT, AdaIN,
+        OST, ``alpha``, ``passes``, prepared styles, ``style_weights``, ``content_mask`` / ``style_masks``,
+        ``return_float`` / ``return_device`` / ``out`` and ``tile_size``; not with ``swap5`` / ``swap_targets`` (the
+        swap's VALID patches are not periodic) or ``temporal`` (the optical flow does not see across the seam)."""
+        seamless_axes(seamless)                              # ValueError for a value other than None, "x", "y", "xy"
+        if seamless is not None and (swap5 or swap_targets is not None or temporal is not None):
+            raise ValueError("seamless does not combine with swap5 / swap_targets or temporal")
         if ost and (adain or content_mask is not None or style_masks is not None or style_weights is not None):
             raise ValueError("ost does not combine with adain, content_mask, style_masks or style_weights")
         if tile_size is not None and tile_size != 0:
@@ -330,7 +344,8 @@ class WCT(object):
                 ist = [style_dev(x) for x in interp_styles]
 
                 def one_pass(x, first):
-                    return eng.stylize(x, None, alpha=alpha, adain=adain, interp_styles=ist, interp_weights=w_dev)
+                    return eng.stylize(x, None, alpha=alpha, adain=adain, interp_styles=ist, interp_weights=w_dev,
+                                       seamless=seamless)
             elif content_mask is not None and style_masks is not None:
                 lab = mask.to(dev, non_blocking=True)
                 # the same object stays the same object on the device: the engine shares its side
@@ -347,18 +362,18 @@ class WCT(object):
                     rs, sm = eng.prepare_regions_call(rs, eng.check_region_masks(sm, rs)), None
 
                 def one_pass(x, first):
-                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs, region_masks=sm)
+                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs, region_masks=sm, seamless=seamless)
             elif content_mask is not None:
                 lab = mask.to(dev, non_blocking=True)
                 rs = [style_dev(x) for x in region_styles]
 
                 def one_pass(x, first):
-                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs)
+                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs, seamless=seamless)
             elif tile_size is not None:
                 s = style_dev(styles)
 
                 def one_pass(x, first):
-                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size, ost=ost)
+                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size, ost=ost, seamless=seamless)
             else:
                 s = style_dev(styles)
 
@@ -367,7 +382,7 @@ class WCT(object):
                     # whole batch in one call; with one style per frame the engine swaps frame by frame.
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
-                                       swap_targets=swap_targets if first else None, ost=ost)
+                                       swap_targets=swap_targets if first else None, ost=ost, seamless=seamless)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -483,11 +498,12 @@ class WCT(object):
         return self.predict_batch(noise, styles, **kw)
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
-                style_masks=None, swap_targets=None, tile_size=None, ost=False):
+                style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
-        blend.  ``tile_size`` stylises in tiles and ``ost`` uses the optimal-transport transform (``predict_batch``).'''
+        blend.  ``tile_size`` stylises in tiles, ``ost`` uses the optimal-transport transform and ``seamless`` pads the content
+        path circularly (``predict_batch``).'''
         s = time.time()
         seen = {}
 
@@ -505,17 +521,19 @@ class WCT(object):
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, style_weights=style_weights, content_mask=content_mask,
-                                     tile_size=tile_size)
+                                     tile_size=tile_size, seamless=seamless)
         elif content_mask is not None:
             kw = {} if style_masks is None else dict(style_masks=style_masks)
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
-                                     swap5=swap5, content_mask=content_mask, tile_size=tile_size, **kw)
+                                     swap5=swap5, content_mask=content_mask, tile_size=tile_size, seamless=seamless, **kw)
         else:
             kw = {} if swap_targets is None else dict(swap_targets=swap_targets)
             if tile_size is not None:
                 kw["tile_size"] = tile_size
             if ost:
                 kw["ost"] = True
+            if seamless is not None:
+                kw["seamless"] = seamless
             out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
