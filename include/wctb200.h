@@ -430,6 +430,28 @@ WCTB200_API int wctb200_style_swap_apply(const void* content, int Nc, int Hc, in
  */
 WCTB200_API size_t wctb200_style_swap_apply_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride);
 
+/* ---- multimodal style transfer (DESIGN.md §3.3.10; mst.cu) ----------------
+ * Spherical k-means of one style feature (SPF16 [1,Hs,Ws,C], C in {64,128,256,512}) into K in 1..8 clusters of the unit
+ * directions u_p = f_p / max(|f_p|, 1e-12): k-means++ seeding with Philox4x32-10 draws (counter (j, level, 0, 0)), then at
+ * most 16 Lloyd iterations (argmax_k u.c_k, ties to the lowest k; c_k = normalised sum of its u_p, fp64 in a fixed order;
+ * an empty cluster keeps its centre), stopping after the first iteration that changes no label -- decided on the device.
+ * labels_out uint8 [Hs*Ws], centres_out fp32 [K][C], info_out int32 [K init pixel indices | iterations | K pixel counts].
+ * The result depends only on the feature, K and level.  ws: wctb200_mst_style_clusters_workspace_bytes bytes (0: bad
+ * arguments).  2K + 31 launches. */
+WCTB200_API size_t wctb200_mst_style_clusters_workspace_bytes(int Hs, int Ws, int C, int K);
+WCTB200_API int wctb200_mst_style_clusters(const void* style, int Hs, int Ws, int C, int K, int level, uint8_t* labels_out,
+                                           float* centres_out, int32_t* info_out, void* ws, size_t ws_bytes, void* stream);
+/* Data term of the content side: D_out fp32 [N][H][W][K] = 1 - u_p . c_k for the centres fp32 [K][C]; +inf where counts[k]
+ * (device int32 [K], the style pixels of cluster k) is below 2.  Reads the content once; one launch. */
+WCTB200_API int wctb200_mst_data_term(const void* content, int N, int H, int W, int C, const float* centres, const int32_t* counts,
+                                      int K, float* D_out, void* stream);
+/* Red-black ICM on D fp32 [N][H][W][K] with a Potts term of weight lambda >= 0 per disagreeing 4-neighbour inside the image:
+ * labels_out uint8 [N][H][W] starts at argmin_k D (ties: lowest k); each of `sweeps` sweeps updates the pixels with (y + x)
+ * even, then those with (y + x) odd, to argmin_k D[p,k] + lambda n_k(p), keeping the current label when it is among the
+ * minima and taking the lowest k otherwise; cost = __fadd_rn(D, __fmul_rn(lambda, n_k)).  1 + 2 sweeps launches. */
+WCTB200_API int wctb200_mst_smooth(const float* D, int N, int H, int W, int K, float lambda, int sweeps, uint8_t* labels_out,
+                                   void* stream);
+
 /* Stand-alone pieces of the transform, exposed for parity tests and profiling:
  * per-channel mean [N][C] and covariance [N][C][C] = fc fc^T/(HW-1) + eps_cov*I of a feature batch
  * (ops.py:43-45,105-108), fp32 outputs. */

@@ -41,6 +41,12 @@ Seamless stylisation: ``--seamless {x,y,xy}`` pads every conv of the content pat
 (``--noise --seamless xy``).  Each wrapped side must be a multiple of 2^P, P the pools up to the deepest relu target (16
 for relu5_1).  Output names are unchanged.  Not with ``--swap5`` or ``--swap-targets``.
 
+Multimodal style transfer: ``--mst K [--mst-smooth LAMBDA]`` clusters each level's style features into K (1..8) modes and
+matches every content pixel to the mode it resembles, with a Potts smoothness of weight LAMBDA (default 0.05), so regions
+of the content pair up with modes of the painting without masks (DESIGN.md §3.3.10).  Output names are unchanged.  Not with
+``--adain``, ``--ost``, ``--content-mask``, ``--interp-styles``, ``--swap5``, ``--swap-targets``, ``--tile-size``,
+``--seamless`` or prepared styles (``.wctstyle``).
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -93,6 +99,10 @@ _FLAGS = [
                                  "statistics over the whole image (0: off)")),
     (("--seamless",), dict(type=str, default=None, choices=["x", "y", "xy"],
                            help="wrap-around padding along x, y or both: panoramas (x) and tileable textures (xy)")),
+    (("--mst",), dict(type=int, default=None, metavar="K",
+                      help="multimodal style transfer: cluster each level's style into K modes (1..8) and match the content to them")),
+    (("--mst-smooth",), dict(type=float, default=None, metavar="LAMBDA",
+                             help="with --mst: Potts smoothness of the content labelling, finite and >= 0 (default 0.05)")),
     # webcam.py:38; the three --noise-* flags are not in the reference.  Their defaults are filled in by parse_args, so that
     # giving one without --noise can be told from leaving it out.
     (("--noise",), dict(action="store_true", default=False, help="Synthesize textures from noise images")),
@@ -125,6 +135,7 @@ def parse_args(argv=None):
     check_tile_flags(parser, args)
     check_ost_flags(parser, args)
     check_seamless_flags(parser, args)
+    check_mst_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
@@ -169,6 +180,35 @@ def check_seamless_flags(parser, args):
     for attr, flag in [("swap5", "--swap5"), ("swap_targets", "--swap-targets"), ("temporal", "--temporal")]:
         if getattr(args, attr, None):
             parser.error("--seamless does not combine with %s" % flag)
+
+
+MST_SMOOTH_DEFAULT = 0.05
+# flags that do not combine with --mst (stylize.py and stylize_video.py)
+_MST_EXCLUDES = [("adain", "--adain"), ("ost", "--ost"), ("content_mask", "--content-mask"), ("style_masks", "--style-masks"),
+                 ("interp_styles", "--interp-styles"), ("swap5", "--swap5"), ("swap_targets", "--swap-targets"),
+                 ("tile_size", "--tile-size"), ("seamless", "--seamless")]
+
+
+def check_mst_flags(parser, args):
+    """--mst K: 1..8 clusters; --mst-smooth (finite, >= 0) needs it and defaults to 0.05 here.  Not with the other
+    transforms, masks, blends, the swap, tiles, seamless or prepared styles (which keep no per-level features to cluster)."""
+    if getattr(args, "mst", None) is None:
+        if getattr(args, "mst_smooth", None) is not None:
+            parser.error("--mst-smooth needs --mst")
+        return
+    if not 1 <= args.mst <= 8:
+        parser.error("--mst takes 1..8 clusters, got %d" % args.mst)
+    if args.mst_smooth is None:
+        args.mst_smooth = MST_SMOOTH_DEFAULT
+    if not np.isfinite(args.mst_smooth) or args.mst_smooth < 0:
+        parser.error("--mst-smooth must be finite and >= 0, got %g" % args.mst_smooth)
+    for attr, flag in _MST_EXCLUDES:
+        if getattr(args, attr, None):
+            parser.error("--mst does not combine with %s" % flag)
+    style_path = getattr(args, "style_path", None)
+    if style_path and (is_prepared(style_path) or (os.path.isdir(style_path)
+                                                   and any(is_prepared(f) for f in os.listdir(style_path)))):
+        parser.error("--mst does not combine with prepared styles (.wctstyle)")
 
 
 def check_tile_flags(parser, args):
@@ -365,6 +405,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw["ost"] = True
     if args.seamless:
         kw["seamless"] = args.seamless
+    if args.mst is not None:
+        kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, style_dev, **kw)

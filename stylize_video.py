@@ -24,6 +24,9 @@ Optimal-transport transform: ``--ost`` uses the Monge map between the feature Ga
 Seamless stylisation: ``--seamless {x,y,xy}`` pads the content path circularly (DESIGN.md §3.3.9), e.g. ``x`` for 360°
 clips, on both paths.  Not with ``--temporal`` (the optical flow does not see across the seam), ``--swap5`` or
 ``--swap-targets``.
+
+Multimodal style transfer: ``--mst K [--mst-smooth LAMBDA]`` matches the content to K modes of the style at every level
+(DESIGN.md §3.3.10), on both paths, with the same rejections as stylize.py; it combines with ``--temporal``.
 """
 from __future__ import division, print_function
 
@@ -56,7 +59,8 @@ _VIDEO_FLAGS = [
 ]
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
-           "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless")
+           "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
+           "--mst", "--mst-smooth")
 # flags that do not combine with --interp-styles
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat"),
                     ("swap_targets", "--swap-targets")]
@@ -100,6 +104,7 @@ def parse_args(argv=None):
     if not 0.0 <= args.temporal < 1.0:
         parser.error("--temporal must be in [0, 1), got %g" % args.temporal)
     stylize.check_seamless_flags(parser, args)
+    stylize.check_mst_flags(parser, args)
     return args
 
 
@@ -151,10 +156,12 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
 
     temporal_kw = {} if temporal is None else dict(temporal=temporal)
-    # --ost and --seamless, on both paths
+    # --ost, --seamless and --mst, on both paths
     opt_kw = dict(ost=True) if getattr(args, "ost", False) else {}
     if getattr(args, "seamless", None):
         opt_kw["seamless"] = args.seamless
+    if getattr(args, "mst", None) is not None:
+        opt_kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
 
     def coral(style, fr):
         if isinstance(style, list):

@@ -97,6 +97,10 @@ SIGNATURES = {
     "wctb200_adain_transform_layout": (_sz, [_i, _i, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "wctb200_adain_transform_from_stats": (_i, [_vp, _i, _i, _vp, _i, _f, _vp, _vp]),
     "wctb200_adain_transform_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _f, _vp, _vp]),
+    "wctb200_mst_style_clusters_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "wctb200_mst_style_clusters": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_mst_data_term": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
+    "wctb200_mst_smooth": (_i, [_vp, _i, _i, _i, _i, _f, _i, _vp, _vp]),
 }
 
 # tuning / probe hooks (wct_tf_b200/csrc/wctb200_debug.h): NOT part of the ABI, bound for tools/ and tests/ only

@@ -1,4 +1,5 @@
 // extern "C" surface of libwctb200 (declared in include/wctb200.h).
+#include <float.h>
 #include <limits.h>
 #include <stdarg.h>
 #include <string.h>
@@ -165,6 +166,12 @@ size_t wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc);
 int launch_wct_apply_regions(const __half*, int, int, int, int, const uint8_t*, int, const void* const*, float, float, float, float,
                              int, __half*, int32_t*, void*, size_t, cudaStream_t);
 int launch_labels_resize(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, cudaStream_t st);
+size_t mst_clusters_workspace_bytes(int Hs, int Ws, int C, int K);
+int launch_mst_style_clusters(const __half* style, int Hs, int Ws, int C, int K, int level, uint8_t* labels, float* centres,
+                              int32_t* info, void* ws, size_t ws_bytes, cudaStream_t st);
+int launch_mst_data_term(const __half* act, int N, int H, int W, int C, const float* centres, const int32_t* counts, int K, float* D,
+                         cudaStream_t st);
+int launch_mst_smooth(const float* D, int N, int H, int W, int K, float lambda, int sweeps, uint8_t* labels, cudaStream_t st);
 size_t wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws);
 int launch_wct_style_prepare_regions(const __half*, int, int, int, const uint8_t*, int, float, float, float, void*, int32_t*, void*,
                                      size_t, cudaStream_t);
@@ -467,6 +474,32 @@ int wctb200_adain_blend(const void* content, int Nc, int Hc, int Wc, int C, cons
         WCTB_REQUIRE(geom_ok(1, Hs[k], Ws[k], C), "adain_blend: bad geometry of style %d", k);
     return launch_adain_blend(HCP(content), Nc, Hc, Wc, C, styles, Hs, Ws, K, weights, Nw, alpha, eps, HP(out), ws, ws_bytes,
                               ST(stream));
+}
+// multimodal style transfer (mst.cu): one channel count of the encoder levels, K in 1..8
+static bool mst_args_ok(int C, int K) { return (C == 64 || C == 128 || C == 256 || C == 512) && K >= 1 && K <= 8; }
+size_t wctb200_mst_style_clusters_workspace_bytes(int Hs, int Ws, int C, int K) {
+    if (!mst_args_ok(C, K) || !geom_ok(1, Hs, Ws, C)) return 0;
+    return mst_clusters_workspace_bytes(Hs, Ws, C, K);
+}
+int wctb200_mst_style_clusters(const void* style, int Hs, int Ws, int C, int K, int level, uint8_t* labels_out, float* centres_out,
+                               int32_t* info_out, void* ws, size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(style && labels_out && centres_out && info_out && ws, "mst_style_clusters: null pointer");
+    WCTB_REQUIRE(mst_args_ok(C, K) && geom_ok(1, Hs, Ws, C) && level >= 0,
+                 "mst_style_clusters: bad arguments %dx%d C=%d K=%d level=%d (C in {64,128,256,512}, K in 1..8)", Hs, Ws, C, K, level);
+    return launch_mst_style_clusters(HCP(style), Hs, Ws, C, K, level, labels_out, centres_out, info_out, ws, ws_bytes, ST(stream));
+}
+int wctb200_mst_data_term(const void* content, int N, int H, int W, int C, const float* centres, const int32_t* counts, int K,
+                          float* D_out, void* stream) {
+    WCTB_REQUIRE(content && centres && counts && D_out, "mst_data_term: null pointer");
+    WCTB_REQUIRE(mst_args_ok(C, K) && geom_ok(N, H, W, C), "mst_data_term: bad arguments N=%d %dx%d C=%d K=%d", N, H, W, C, K);
+    return launch_mst_data_term(HCP(content), N, H, W, C, centres, counts, K, D_out, ST(stream));
+}
+int wctb200_mst_smooth(const float* D, int N, int H, int W, int K, float lambda, int sweeps, uint8_t* labels_out, void* stream) {
+    WCTB_REQUIRE(D && labels_out, "mst_smooth: null pointer");
+    WCTB_REQUIRE(N >= 1 && H >= 1 && W >= 1 && (long long)N * H * W < (1ll << 40) && K >= 1 && K <= 8 && sweeps >= 0 &&
+                     sweeps <= 1024 && lambda >= 0.f && lambda <= FLT_MAX,
+                 "mst_smooth: bad arguments N=%d %dx%d K=%d lambda=%g sweeps=%d", N, H, W, K, (double)lambda, sweeps);
+    return launch_mst_smooth(D, N, H, W, K, lambda, sweeps, labels_out, ST(stream));
 }
 int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, void* stream) {
     WCTB_REQUIRE(src && dst, "labels_resize_nearest: null pointer");

@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import _capi
-from .model import WCTModel, RELU_CHANNELS, check_seamless, seamless_axes
+from .model import WCTModel, RELU_CHANNELS, RELU_LEVEL, check_seamless, seamless_axes
 from .prepared import (PreparedStyle, SEMANTIC_KEYS, encoder_fingerprints, slice_act_planes, slice_adain_state,
                        slice_wct_state)
 
@@ -24,6 +24,9 @@ SEMANTICS = {
 # apply then correlates the patches in chunks; the output is the same byte for byte (wctb200_style_swap_apply_min_workspace_
 # bytes).  At 512^2 a relu5_1 swap (4.4 MB of scores per frame) runs in one chunk, a relu3_1 swap (1.08 GB) in two.
 SWAP_WORKSPACE_BYTES = 1 << 30
+
+# Multimodal style transfer (DESIGN.md §3.3.10): red-black ICM sweeps of the content labelling per level
+MST_SWEEPS = 8
 
 
 class Act(object):
@@ -481,6 +484,89 @@ class Engine(object):
                    flops=2.0 * C * C * 2 * N * hwc, bytes_=4.0 * C * 2 * N * hwc)
         return out, kbuf
 
+    # ------------------------------------------------------------------ multimodal style transfer (DESIGN.md §3.3.10)
+    @staticmethod
+    def check_mst(K, lam):
+        """(K, lambda) of an MST call: K an integer in 1..8, lambda finite and >= 0; ValueError otherwise."""
+        if isinstance(K, bool) or not isinstance(K, (int, np.integer)) or not 1 <= K <= 8:
+            raise ValueError("mst must be a number of clusters in 1..8, got %r" % (K,))
+        try:
+            lam_f = float(lam)
+        except (TypeError, ValueError):
+            raise ValueError("mst_smooth must be a number, got %r" % (lam,))
+        if not np.isfinite(lam_f) or lam_f < 0:
+            raise ValueError("mst_smooth must be finite and >= 0, got %r" % (lam,))
+        return int(K), lam_f
+
+    def mst_clusters(self, style, K, level):
+        """Spherical k-means of the style feature ``style`` (one style) into K clusters, seeded by the draws of ``level`` (0 for
+        relu1_1 .. 4 for relu5_1).  Returns device (labels uint8 [1,Hs,Ws], centres fp32 [K,C], info int32 [K init indices |
+        iterations | K counts])."""
+        C = style.C
+        labels = torch.empty((1, style.H, style.W), dtype=torch.uint8, device=self.device)
+        centres = torch.empty((K, C), dtype=torch.float32, device=self.device)
+        info = torch.empty(2 * K + 1, dtype=torch.int32, device=self.device)
+        ws = self._grow_workspace(("mst_clusters",), self.lib.wctb200_mst_style_clusters_workspace_bytes(style.H, style.W, C, K))
+        self._call("mst_clusters[C%d@%dx%d]" % (C, style.H, style.W), 2 * K + 31, self.lib.wctb200_mst_style_clusters, style.ptr,
+                   style.H, style.W, C, K, int(level), labels.data_ptr(), centres.data_ptr(), info.data_ptr(), ws.data_ptr(),
+                   ws.numel(), self._stream(), bytes_=4.0 * C * style.H * style.W * (K + 16))
+        return labels, centres, info
+
+    def mst_data_term(self, content, centres, info):
+        """D fp32 [N,H,W,K] = 1 - u_p . c_k of the content feature against the K cluster centres (``mst_clusters``); +inf for a
+        cluster of fewer than 2 style pixels."""
+        K, C = centres.shape[0], content.C
+        D = torch.empty((content.N, content.H, content.W, K), dtype=torch.float32, device=self.device)
+        hw = content.N * content.H * content.W
+        self._call("mst_data_term[C%d]" % C, 1, self.lib.wctb200_mst_data_term, content.ptr, content.N, content.H, content.W, C,
+                   centres.data_ptr(), info[K + 1:].data_ptr(), K, D.data_ptr(), self._stream(),
+                   flops=2.0 * (K + 1) * C * hw, bytes_=4.0 * hw * (C + K))
+        return D
+
+    def mst_smooth(self, D, lam, sweeps=MST_SWEEPS):
+        """Content labels uint8 [N,H,W]: red-black ICM on the data term ``D`` with Potts weight ``lam``."""
+        N, H, W, K = D.shape
+        labels = torch.empty((N, H, W), dtype=torch.uint8, device=self.device)
+        self._call("mst_smooth", 1 + 2 * sweeps, self.lib.wctb200_mst_smooth, D.data_ptr(), N, H, W, K, float(lam), int(sweeps),
+                   labels.data_ptr(), self._stream(), bytes_=(1 + 2 * sweeps) * N * H * W * (4.0 * K + 1))
+        return labels
+
+    def prepare_mst_call(self, style_u8, K):
+        """The MST style side of one style image (cuda uint8 [1,Hs,Ws,3]), made once for a call that applies it several times
+        (passes)."""
+        main = torch.cuda.current_stream(self.device)
+        ps = self._style_side(style_u8, main, mst=K)
+        style_u8.record_stream(ps.side)
+        return ps
+
+    def _stylize_mst(self, content_u8, style, K, lam, alpha, want_info, capture):
+        """``stylize`` with multimodal style transfer: the style side clusters each level's style feature (``_style_side``
+        with ``mst``) unless ``style`` is such a side already, and every sub-batch group labels and transforms its frames."""
+        N = content_u8.shape[0]
+        main = torch.cuda.current_stream(self.device)
+        G = min(self.groups, N) if (capture is None and not want_info) else 1
+        owned = None
+        if isinstance(style, PreparedStyle):
+            ps = style
+        else:
+            self._group = 1 if G > 1 else 0
+            try:
+                ps = owned = self._style_side(style, main, mst=K)
+            finally:
+                self._group = 0
+        multi = ("mst", (lam, ps), ps.entries)
+        if G == 1:
+            out = self._stylize_one(content_u8, None, alpha, False, want_info, capture, multi=multi)
+        else:
+            out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, False, False, None,
+                                                                               multi=multi))
+        if owned is not None and owned.side is not main:
+            owned.side.wait_stream(main)        # the style states are recycled only after every level used them
+            main.wait_stream(owned.side)
+        elif owned is None:
+            ps.record_stream(main)
+        return out
+
     def _grow_workspace(self, key, nbytes):
         """Grow-only scratch per (group, key): the levels of a call differ in size."""
         key = (self._group,) + key
@@ -537,7 +623,7 @@ class Engine(object):
 
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
-                region_masks=None, swap_targets=None, ost=False, seamless=None):
+                region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -580,8 +666,27 @@ class Engine(object):
         Seamless stylisation: ``seamless`` = "x", "y" or "xy" pads every conv of the content path circularly along those
         axes (DESIGN.md §3.3.9), so the output equals that of the infinitely tiled content and tiles without a seam.  Each
         wrapped axis must be a multiple of 2^P (P pools up to the deepest target); not with the style swap, whose VALID
-        patches are not periodic.  The style side is unchanged."""
+        patches are not periodic.  The style side is unchanged.
+
+        Multimodal style transfer: ``mst`` = K (1..8) clusters each level's style feature into K modes and labels every
+        content pixel with the mode it resembles, smoothed by a Potts term of weight ``mst_smooth`` (DESIGN.md §3.3.10);
+        region k of each frame then takes the statistics of style mode k.  ``style_u8`` is one style image.  WCT only; not
+        with ``ost``, spatial control, interpolation, the style swap or ``seamless``.  K = 1 is the plain WCT call, byte for
+        byte."""
         N = content_u8.shape[0]
+        if mst is not None:
+            K, lam = self.check_mst(mst, mst_smooth)
+            if (adain or ost or labels is not None or region_masks is not None or interp_styles is not None or swap5
+                    or swap_targets is not None or seamless is not None):
+                raise ValueError("mst works with WCT only: not with adain, ost, labels / region_masks, interp_styles, swap5 / "
+                                 "swap_targets or seamless")
+            if isinstance(style_u8, PreparedStyle):
+                if style_u8.mst_k != K or any(relu not in style_u8.mst for relu in self.model.style_taps):
+                    raise ValueError("mst clusters the style's features at every level, which a prepared style does not keep: "
+                                     "give the style image")
+            elif style_u8.shape[0] != 1:
+                raise ValueError("mst takes one style for the whole batch, got %d" % style_u8.shape[0])
+            return self._stylize_mst(content_u8, style_u8, K, lam, alpha, want_info, capture)
         if seamless is not None:
             if swap5 or swap_targets is not None:
                 raise ValueError("seamless does not combine with swap5 / swap_targets: the swap's VALID patches are not periodic")
@@ -786,7 +891,7 @@ class Engine(object):
             self._style_streams[self._group] = torch.cuda.Stream(device=self.device, priority=prio)
         return self._style_streams[self._group]
 
-    def _style_side(self, style_u8, main, wct=True, adain=False, keep=(), skip=(), labels=None, R=0):
+    def _style_side(self, style_u8, main, wct=True, adain=False, keep=(), skip=(), labels=None, R=0, mst=0):
         """The prepare step: style side of one call (model.py:70-72: ONE encoder pass emitting every target; per level the
         WCT state of ops.py:48-55,76 when ``wct``, the AdaIN moments when ``adain``; levels in ``skip`` get neither), enqueued
         on this group's style stream when overlap is on.  ``keep`` lists the levels whose feature it keeps (the style
@@ -795,16 +900,23 @@ class Engine(object):
 
         With ``labels`` (a style mask, cuda uint8 [1,Hm,Wm] of one style) the WCT state of each level is the masked prepare
         of R regions, so the result is a prepared style of n = R; ``entries[r]`` is its slice r (``slice_prepared``) as a
-        prepared style of one style, cut per level as soon as that level is prepared and sharing its events."""
+        prepared style of one style, cut per level as soon as that level is prepared and sharing its events.
+
+        With ``mst`` = K (one style image) each level's style feature is clustered (``mst_clusters``) and its WCT state is
+        the masked prepare of the K clusters under the style's own labels: a prepared style of n = K with ``entries`` as
+        above, and the labels, centres and info of every level in ``mst``."""
         lib = self.lib
         side = self._style_stream() or main
         if side is not main:
             side.wait_stream(main)             # style_u8 (and last step's buffers) are ready
         sem = SEMANTICS[self.semantics]
         taps = list(dict.fromkeys(self.model.style_taps))
-        ps = PreparedStyle(style_u8.shape[0] if labels is None else R, {k: sem[k] for k in SEMANTIC_KEYS}, taps)
+        if mst:
+            R = int(mst)
+        ps = PreparedStyle(style_u8.shape[0] if labels is None and not mst else R, {k: sem[k] for k in SEMANTIC_KEYS}, taps)
         ps.side = side
-        if labels is not None:
+        ps.mst_k = int(mst)
+        if labels is not None or mst:
             ps.entries = [PreparedStyle(1, ps.semantics, taps) for _ in range(R)]
             for e in ps.entries:
                 e.side, e.events = side, ps.events
@@ -816,7 +928,14 @@ class Engine(object):
             _, feats = self.encode(style, self.model.deepest_target, taps=self.model.style_taps)
             for relu in taps:
                 if relu not in skip:
-                    if labels is not None:
+                    if mst:
+                        f = feats[relu]
+                        lab, cen, info = self.mst_clusters(f, R, RELU_LEVEL[relu] - 1)
+                        ps.mst[relu] = dict(labels=lab, centres=cen, info=info)
+                        ps.wct[relu] = self.style_prepare_regions(f, lab, R)
+                        for r, e in enumerate(ps.entries):
+                            e.wct[relu] = slice_wct_state(lib, ps.wct[relu], f.C, R, r, r + 1)
+                    elif labels is not None:
                         f = feats[relu]
                         ps.wct[relu] = self.style_prepare_regions(f, self.labels_resize(labels, f.H, f.W), R)
                         for r, e in enumerate(ps.entries):
@@ -939,7 +1058,8 @@ class Engine(object):
         content = torch.empty(content_u8.shape, dtype=torch.float32, device=self.device)
         self._call("u8_to_f32", 1, lib.wctb200_image_u8_to_f32, content_u8.data_ptr(), content_u8.numel(), content.data_ptr(), st)
         if multi is not None:
-            # ("regions", labels [N,Hm,Wm], R style sides) or ("interp", weight rows [1|N,K], K style sides): _stylize_multi
+            # ("regions", labels [N,Hm,Wm], R style sides) or ("interp", weight rows [1|N,K], K style sides): _stylize_multi;
+            # ("mst", (lambda, the MST side), its K cluster sides): _stylize_mst
             mode, per_frame, sides = multi
         infos = []
         x = content
@@ -967,6 +1087,15 @@ class Engine(object):
                 elif mode == "regions":
                     lab = self.labels_resize(per_frame, cf.H, cf.W)
                     f, kbuf = self.wct_apply_regions(cf, lab, [sd.wct[relu] for sd in sides], alpha, want_info)
+                elif mode == "mst":
+                    lam, ms = per_frame
+                    m = ms.mst[relu]
+                    lab = self.mst_smooth(self.mst_data_term(cf, m["centres"], m["info"]), lam)
+                    f, kbuf = self.wct_apply_regions(cf, lab, [sd.wct[relu] for sd in sides], alpha, want_info)
+                    if capture is not None:
+                        for key, val in (("mst_style_labels", m["labels"]), ("mst_centres", m["centres"]), ("mst_info", m["info"]),
+                                         ("mst_content_labels", lab)):
+                            capture.setdefault(key, []).append(val)
                 elif adain:
                     f, kbuf = self.adain_apply_blend(cf, [sd.adain[relu] for sd in sides], per_frame, alpha)
                 else:

@@ -71,6 +71,8 @@ class PreparedStyle(object):
         self.fingerprints = {}                    # relu -> encoder fingerprint (prepare_style / load_style)
         self.swap = {}                            # (relu, patch, stride) -> (device swap state, event)
         self.entries = None                       # style-masked side (Engine._style_side): its n styles, one by one
+        self.mst = {}                             # relu -> dict(labels, centres, info): MST clusters (Engine._style_side)
+        self.mst_k = 0                            # K of an MST side (its n = K styles are the clusters), 0 otherwise
 
     @property
     def feat5(self):
@@ -97,6 +99,7 @@ class PreparedStyle(object):
     def tensors(self):
         ts = list(self.wct.values()) + list(self.adain.values()) + [st for st, _ in self.swap.values()]
         ts += [f.buf for f in self.feats.values()]
+        ts += [t for m in self.mst.values() for t in m.values()]
         return ts
 
     def record_stream(self, stream):

@@ -22,7 +22,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``ost`` is new: the optimal-transport transform (Lu et al., ICCV 2019), the Monge map between the content and style
     feature Gaussians, in place of WCT at every level;
   * ``seamless`` is new: circular padding of every conv of the content path along x, y or both, for 360° panoramas and
-    tileable textures.
+    tileable textures;
+  * ``mst`` is new: multimodal style transfer (Zhang, Zhu & Zhu, ICCV 2019), each level's style clustered into K modes
+    and every content pixel matched to one, so regions pair up without masks.
 """
 from __future__ import annotations
 
@@ -229,7 +231,7 @@ class WCT(object):
 
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
-                      swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None):
+                      swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -290,7 +292,28 @@ class WCT(object):
         2^P, P the pools up to the deepest target (16 for relu5_1).  The style side is unchanged.  Works with WCT, AdaIN,
         OST, ``alpha``, ``passes``, prepared styles, ``style_weights``, ``content_mask`` / ``style_masks``,
         ``return_float`` / ``return_device`` / ``out`` and ``tile_size``; not with ``swap5`` / ``swap_targets`` (the
-        swap's VALID patches are not periodic) or ``temporal`` (the optical flow does not see across the seam)."""
+        swap's VALID patches are not periodic) or ``temporal`` (the optical flow does not see across the seam).
+
+        ``mst`` (multimodal style transfer, DESIGN.md §3.3.10): K in 1..8.  At every level the style's features are
+        clustered into K modes (spherical k-means on their directions), every content pixel is labelled with the mode it
+        resembles, the labelling is smoothed by a Potts term of weight ``mst_smooth`` (finite, >= 0; default 0.05), and
+        content region k takes the WCT statistics of style mode k.  A painting with several distinct modes is then not
+        averaged into one.  K = 1 is the plain WCT call, byte for byte; ``mst=None`` changes nothing.  ``styles`` is one
+        style image.  Works with both semantics, ``alpha``, ``passes`` (the style side is made once per call), batches,
+        ``return_float`` / ``return_device`` / ``out``, ``synthesize`` and ``temporal``; not with prepared styles (they
+        keep no per-level features), one style per frame, ``adain``, ``ost``, ``content_mask`` / ``style_masks``,
+        ``style_weights``, ``swap5`` / ``swap_targets``, ``tile_size`` or ``seamless``."""
+        if mst is not None:
+            mst, mst_smooth = Engine.check_mst(mst, mst_smooth)
+            if (adain or ost or content_mask is not None or style_masks is not None or style_weights is not None or swap5
+                    or swap_targets is not None or (tile_size is not None and tile_size != 0) or seamless is not None):
+                raise ValueError("mst does not combine with adain, ost, content_mask, style_masks, style_weights, swap5 / "
+                                 "swap_targets, tile_size or seamless")
+            if isinstance(styles, PreparedStyle):
+                raise ValueError("mst clusters the style's features at every level, which a prepared style does not keep: "
+                                 "give the style image")
+            if isinstance(styles, (list, tuple)) or np.ndim(styles) not in (3, 4) or (np.ndim(styles) == 4 and styles.shape[0] != 1):
+                raise ValueError("mst takes one style image [Hs,Ws,3] for every frame, not one style per frame")
         seamless_axes(seamless)                              # ValueError for a value other than None, "x", "y", "xy"
         if seamless is not None and (swap5 or swap_targets is not None or temporal is not None):
             raise ValueError("seamless does not combine with swap5 / swap_targets or temporal")
@@ -369,6 +392,13 @@ class WCT(object):
 
                 def one_pass(x, first):
                     return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs, seamless=seamless)
+            elif mst is not None:
+                s = to_dev(styles)
+                if int(passes) > 1:
+                    s = eng.prepare_mst_call(s, mst)
+
+                def one_pass(x, first):
+                    return eng.stylize(x, s, alpha=alpha, mst=mst, mst_smooth=mst_smooth)
             elif tile_size is not None:
                 s = style_dev(styles)
 
@@ -498,12 +528,12 @@ class WCT(object):
         return self.predict_batch(noise, styles, **kw)
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
-                style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None):
+                style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
-        blend.  ``tile_size`` stylises in tiles, ``ost`` uses the optimal-transport transform and ``seamless`` pads the content
-        path circularly (``predict_batch``).'''
+        blend.  ``tile_size`` stylises in tiles, ``ost`` uses the optimal-transport transform, ``seamless`` pads the content
+        path circularly and ``mst`` = K matches the content to K modes of the style (``predict_batch``).'''
         s = time.time()
         seen = {}
 
@@ -518,6 +548,8 @@ class WCT(object):
             raise ValueError("swap_targets does not combine with content_mask or style_weights")
         if ost and (adain or content_mask is not None or style_weights is not None):
             raise ValueError("ost does not combine with adain, content_mask, style_masks or style_weights")
+        if mst is not None and (style_weights is not None or content_mask is not None):
+            raise ValueError("mst does not combine with content_mask, style_masks or style_weights")
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, style_weights=style_weights, content_mask=content_mask,
@@ -534,6 +566,8 @@ class WCT(object):
                 kw["ost"] = True
             if seamless is not None:
                 kw["seamless"] = seamless
+            if mst is not None:
+                kw.update(mst=mst, mst_smooth=mst_smooth)
             out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
