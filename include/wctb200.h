@@ -452,6 +452,31 @@ WCTB200_API int wctb200_mst_data_term(const void* content, int N, int H, int W, 
 WCTB200_API int wctb200_mst_smooth(const float* D, int N, int H, int W, int K, float lambda, int sweeps, uint8_t* labels_out,
                                    void* stream);
 
+/* ---- soft spatial control (DESIGN.md §3.3.11) -----------------------------------
+ * mask_feather: labels device uint8 [N][Hm][Wm], R in 1..8, sigma in (0, 1024] mask pixels -> out fp32 [N][R][Hm][Wm]: the
+ * one-hot plane of label r blurred by a separable Gaussian (taps exp(-d^2 / 2 sigma^2), |d| <= ceil(3 sigma), normalised in
+ * fp64, clamp-to-edge).  Labels >= R are the keep plane, which is what the R planes leave.
+ * weights_resize_area: fp32 [N][K][Hm][Wm] -> [N][K][Hf][Wf] by the exact area average (fractional box coverage, fp64 sum,
+ * rounded once): the identity at equal size, for up- and downsampling alike.
+ * wct_stats_weighted: the statistics records of N*K problems (problem n*K + k: frame n under weight plane k of weights
+ * fp32 [N][K][H][W], weights >= 0) in the layout of wctb200_stats_record_layout(C, N*K, 0): with W = sum w, Q = sum w^2,
+ * n = W^2 / Q (0 without weight) and s, S of the weighted sums scaled by n / W, so that wctb200_wct_transform_from_stats
+ * (or ost_transform_from_stats) over the N*K problems gives mean t + s / W and cov (S - s s^T / W) / (W - Q / W).  A
+ * record of n < 2, or a style entry with k_s = -1, gets k_c = -1 in the transform.  C in {64,128,256,512}, K in 1..8.
+ * wct_transform_apply_weighted: out(p) = sum_k v_k (M_{n,k} x + b_{n,k}) + (1 - sum_k v_k) x with v_k = s(p) w_k(p) over
+ * the transforms of N*K problems (a k_c = -1 transform has v = 0); weights [N][K][H][W] or NULL (K = 1, weight 1), strength
+ * fp32 [N][H][W] in [0,1] or NULL (1); sum_k w_k <= 1.  A pixel with every v_k = 0 keeps its input bytes.  One-hot
+ * weights give the bytes of wctb200_wct_apply_regions, and weights = strength = NULL those of wctb200_wct_transform_apply.
+ * adain_transform_apply_strength: wctb200_adain_transform_apply with alpha s(p) at pixel p, strength fp32 [N][H][W]. */
+WCTB200_API int wctb200_mask_feather(const uint8_t* labels, int N, int Hm, int Wm, int R, float sigma, float* out, void* stream);
+WCTB200_API int wctb200_weights_resize_area(const float* src, int N, int K, int Hm, int Wm, int Hf, int Wf, float* dst, void* stream);
+WCTB200_API int wctb200_wct_stats_weighted(const void* act, int N, int H, int W, int C, const float* weights, int K, void* record,
+                                           void* stream);
+WCTB200_API int wctb200_wct_transform_apply_weighted(const void* act, int N, int H, int W, int C, const void* transform, int K,
+                                                     const float* weights, const float* strength, void* out, void* stream);
+WCTB200_API int wctb200_adain_transform_apply_strength(const void* act, int N, int H, int W, int C, const void* transform, float alpha,
+                                                       const float* strength, void* out, void* stream);
+
 /* Stand-alone pieces of the transform, exposed for parity tests and profiling:
  * per-channel mean [N][C] and covariance [N][C][C] = fc fc^T/(HW-1) + eps_cov*I of a feature batch
  * (ops.py:43-45,105-108), fp32 outputs. */

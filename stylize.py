@@ -103,6 +103,12 @@ _FLAGS = [
                       help="multimodal style transfer: cluster each level's style into K modes (1..8) and match the content to them")),
     (("--mst-smooth",), dict(type=float, default=None, metavar="LAMBDA",
                              help="with --mst: Potts smoothness of the content labelling, finite and >= 0 (default 0.05)")),
+    (("--strength-map",), dict(type=str, default=None, metavar="PATH",
+                               help="8-bit grayscale map of the per-pixel stylisation strength (gray v -> v/255)")),
+    (("--mask-feather",), dict(type=float, default=None, metavar="SIGMA",
+                               help="with --content-mask: feather the region edges by a Gaussian of SIGMA mask pixels")),
+    (("--mask-weights",), dict(nargs="+", type=str, default=None, metavar="W",
+                               help="one 8-bit grayscale soft weight map per --mask-styles entry, in place of --content-mask")),
     # webcam.py:38; the three --noise-* flags are not in the reference.  Their defaults are filled in by parse_args, so that
     # giving one without --noise can be told from leaving it out.
     (("--noise",), dict(action="store_true", default=False, help="Synthesize textures from noise images")),
@@ -144,8 +150,9 @@ def parse_args(argv=None):
         for attr, flag in _MASK_EXCLUDES:
             if getattr(args, attr):
                 parser.error("--content-mask does not combine with %s" % flag)
-    elif args.mask_styles:
+    elif args.mask_styles and not args.mask_weights:
         parser.error("--mask-styles needs --content-mask")
+    check_soft_flags(parser, args)
     check_style_mask_flags(parser, args)
     check_noise_flags(parser, args)
     check_prepared_flags(parser, args)
@@ -161,6 +168,56 @@ def check_swap_flags(parser, args):
     for relu in args.swap_targets:
         if relu not in (args.relu_targets or []):
             parser.error("--swap-targets: %s is not one of --relu-targets (%s)" % (relu, " ".join(args.relu_targets or [])))
+
+
+# flags that do not combine with soft spatial control (--strength-map, --mask-feather, --mask-weights)
+_SOFT_EXCLUDES = [("interp_styles", "--interp-styles"), ("swap5", "--swap5"), ("swap_targets", "--swap-targets"),
+                  ("mst", "--mst"), ("tile_size", "--tile-size")]
+
+
+def check_soft_flags(parser, args):
+    """--strength-map, --mask-feather SIGMA (finite, > 0, with --content-mask) and --mask-weights (one map per
+    --mask-styles entry, in place of --content-mask; WCT only): not with blends, the swap, MST or tiles."""
+    soft = [f for a, f in (("strength_map", "--strength-map"), ("mask_feather", "--mask-feather"),
+                           ("mask_weights", "--mask-weights")) if getattr(args, a, None) is not None]
+    if not soft:
+        return
+    for attr, flag in _SOFT_EXCLUDES:
+        if getattr(args, attr, None):
+            parser.error("%s does not combine with %s" % (soft[0], flag))
+    if getattr(args, "mask_feather", None) is not None:
+        if args.content_mask is None:
+            parser.error("--mask-feather needs --content-mask")
+        if not np.isfinite(args.mask_feather) or not 0 < args.mask_feather <= 1024:
+            parser.error("--mask-feather must be a finite sigma in (0, 1024], got %g" % args.mask_feather)
+    if getattr(args, "mask_weights", None) is not None:
+        if args.content_mask is not None:
+            parser.error("--mask-weights replaces --content-mask: give one of them")
+        if not args.mask_styles or len(args.mask_weights) != len(args.mask_styles):
+            parser.error("--mask-weights needs one map per --mask-styles entry")
+        if len(args.mask_styles) > 8:
+            parser.error("--mask-styles takes at most 8 styles")
+        for attr, flag in _MASK_EXCLUDES + [("ost", "--ost")]:
+            if getattr(args, attr, None):
+                parser.error("--mask-weights does not combine with %s" % flag)
+
+
+def read_grey(path):
+    """8-bit grayscale map file -> uint8 [H, W] (read as v/255 by the soft spatial-control options)."""
+    from PIL import Image
+    return np.asarray(Image.open(path).convert("L"), dtype=np.uint8)
+
+
+def soft_kw(args):
+    """predict_batch options of soft spatial control from the parsed flags."""
+    kw = {}
+    if getattr(args, "strength_map", None):
+        kw["strength_map"] = read_grey(args.strength_map)
+    if getattr(args, "mask_feather", None) is not None:
+        kw["mask_feather"] = float(args.mask_feather)
+    if getattr(args, "mask_weights", None):
+        kw["content_weights"] = np.stack([read_grey(p) for p in args.mask_weights])
+    return kw
 
 
 def check_ost_flags(parser, args):
@@ -229,8 +286,8 @@ def check_style_mask_flags(parser, args):
     off its mask) or prepared styles (they keep no feature maps to mask).  --style-size scales style and mask alike."""
     if args.style_masks is None:
         return
-    if args.content_mask is None:
-        parser.error("--style-masks needs --content-mask")
+    if args.content_mask is None and getattr(args, "mask_weights", None) is None:
+        parser.error("--style-masks needs --content-mask (or --mask-weights)")
     if len(args.style_masks) != len(args.mask_styles):
         parser.error("--style-masks needs one mask per --mask-styles entry (%d masks, %d styles)"
                      % (len(args.style_masks), len(args.mask_styles)))
@@ -407,6 +464,7 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw["seamless"] = args.seamless
     if args.mst is not None:
         kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
+    kw.update(soft_kw(args))
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):
         result = model.predict_batch(result, style_dev, **kw)
@@ -426,7 +484,10 @@ def make_model(args):
 
 
 def _stylize_masked(model, content_dev, styles_dev, labels, args, style_masks=None):
-    kw = dict(alpha=args.alpha, return_device=True, content_mask=labels)
+    kw = dict(alpha=args.alpha, return_device=True)
+    if labels is not None:
+        kw["content_mask"] = labels
+    kw.update(soft_kw(args))
     if args.seamless:
         kw["seamless"] = args.seamless
     if style_masks is not None:
@@ -451,7 +512,7 @@ def main_masked(args, model, io, dimg, t_start):
     pixels of style r labelled r).  A path given twice is loaded once and passed as the same object, so that one style
     with one mask for several regions is encoded once."""
     R = len(args.mask_styles)
-    labels = read_mask(args.content_mask, R)
+    labels = read_mask(args.content_mask, R) if args.content_mask is not None else None
     style_masks = _once_per_path(args.style_masks, lambda p: read_mask(p, R)) if args.style_masks else None
     os.makedirs(args.out_path, exist_ok=True)
     device = model.engine.device
@@ -502,7 +563,7 @@ def main(argv=None, model_factory=make_model, image_ops=None):
     model = model_factory(args)
     if args.interp_styles is not None:
         return main_interp(args, model, io, dimg, t_start)
-    if args.content_mask is not None:
+    if args.content_mask is not None or args.mask_weights is not None:
         return main_masked(args, model, io, dimg, t_start)
     styles = style_listing(args.style_path, io)
     if os.path.isdir(args.style_path) and args.random > 0:

@@ -60,7 +60,7 @@ _VIDEO_FLAGS = [
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
            "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
-           "--mst", "--mst-smooth")
+           "--mst", "--mst-smooth", "--strength-map")
 # flags that do not combine with --interp-styles
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat"),
                     ("swap_targets", "--swap-targets")]
@@ -105,6 +105,11 @@ def parse_args(argv=None):
         parser.error("--temporal must be in [0, 1), got %g" % args.temporal)
     stylize.check_seamless_flags(parser, args)
     stylize.check_mst_flags(parser, args)
+    if args.strength_map is not None:
+        for attr, flag in [("interp_styles", "--interp-styles"), ("swap5", "--swap5"), ("swap_targets", "--swap-targets"),
+                           ("mst", "--mst")]:
+            if getattr(args, attr, None):
+                parser.error("--strength-map does not combine with %s" % flag)
     return args
 
 
@@ -162,6 +167,9 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         opt_kw["seamless"] = args.seamless
     if getattr(args, "mst", None) is not None:
         opt_kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
+    if getattr(args, "strength_map", None):
+        import stylize
+        opt_kw["strength_map"] = stylize.read_grey(args.strength_map)   # one map for every frame
 
     def coral(style, fr):
         if isinstance(style, list):

@@ -141,6 +141,13 @@ int launch_adain_transform_from_stats(const void* record, int Nc, int C, const v
                                       cudaStream_t st);
 int launch_adain_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, float alpha, __half* out,
                                  cudaStream_t st);
+int launch_mask_feather(const uint8_t* labels, int N, int Hm, int Wm, int R, float sigma, float* out, cudaStream_t st);
+int launch_weights_resize_area(const float* src, int N, int K, int Hm, int Wm, int Hf, int Wf, float* dst, cudaStream_t st);
+int launch_wct_stats_weighted(const __half* act, int N, int H, int W, int C, const float* wts, int K, void* record, cudaStream_t st);
+int launch_wct_transform_apply_weighted(const __half* act, int N, int H, int W, int C, const void* transform, int K, const float* wts,
+                                        const float* str, __half* out, cudaStream_t st);
+int launch_adain_transform_apply_strength(const __half* act, int N, int H, int W, int C, const void* transform, float alpha,
+                                          const float* strength, __half* out, cudaStream_t st);
 int launch_conv3x3_ref(const __half*, ActGeom, const float*, const float*, int, int, __half*, cudaStream_t);
 int launch_conv_head(const float*, int, int, int, const float*, const float*, int, __half*, cudaStream_t);
 int launch_conv_tail(const __half*, ActGeom, const float*, const float*, int, float*, cudaStream_t);
@@ -705,6 +712,36 @@ int wctb200_adain_transform_apply(const void* act, int N, int H, int W, int C, c
     WCTB_REQUIRE(act && transform && out, "adain_transform_apply: null pointer");
     WCTB_REQUIRE(geom_ok(N, H, W, C) && C <= 2048, "adain_transform_apply: bad geometry");
     return launch_adain_transform_apply(HCP(act), N, H, W, C, transform, alpha, HP(out), ST(stream));
+}
+// ---- soft spatial control (DESIGN.md §3.3.11) ----
+int wctb200_mask_feather(const uint8_t* labels, int N, int Hm, int Wm, int R, float sigma, float* out, void* stream) {
+    WCTB_REQUIRE(labels && out, "mask_feather: null pointer");
+    WCTB_REQUIRE(N >= 1 && Hm >= 1 && Wm >= 1 && (long long)N * R * Hm * Wm < (1ll << 40), "mask_feather: bad geometry");
+    return launch_mask_feather(labels, N, Hm, Wm, R, sigma, out, ST(stream));
+}
+int wctb200_weights_resize_area(const float* src, int N, int K, int Hm, int Wm, int Hf, int Wf, float* dst, void* stream) {
+    WCTB_REQUIRE(src && dst, "weights_resize_area: null pointer");
+    WCTB_REQUIRE(N >= 1 && K >= 1 && Hm >= 1 && Wm >= 1 && Hf >= 1 && Wf >= 1 && Hm <= 65536 && Wm <= 65536 && Hf <= 65536 && Wf <= 65536,
+                 "weights_resize_area: bad geometry N=%d K=%d %dx%d -> %dx%d", N, K, Hm, Wm, Hf, Wf);
+    return launch_weights_resize_area(src, N, K, Hm, Wm, Hf, Wf, dst, ST(stream));
+}
+int wctb200_wct_stats_weighted(const void* act, int N, int H, int W, int C, const float* weights, int K, void* record, void* stream) {
+    WCTB_REQUIRE(act && weights && record, "wct_stats_weighted: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && wct_channels_ok(C), "wct_stats_weighted: bad geometry");
+    WCTB_REQUIRE(K >= 1 && K <= 8, "wct_stats_weighted: K=%d not in 1..8", K);
+    return launch_wct_stats_weighted(HCP(act), N, H, W, C, weights, K, record, ST(stream));
+}
+int wctb200_wct_transform_apply_weighted(const void* act, int N, int H, int W, int C, const void* transform, int K, const float* weights,
+                                         const float* strength, void* out, void* stream) {
+    WCTB_REQUIRE(act && transform && out, "wct_transform_apply_weighted: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && wct_channels_ok(C), "wct_transform_apply_weighted: bad geometry");
+    return launch_wct_transform_apply_weighted(HCP(act), N, H, W, C, transform, K, weights, strength, HP(out), ST(stream));
+}
+int wctb200_adain_transform_apply_strength(const void* act, int N, int H, int W, int C, const void* transform, float alpha,
+                                           const float* strength, void* out, void* stream) {
+    WCTB_REQUIRE(act && transform && strength && out, "adain_transform_apply_strength: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && C <= 2048, "adain_transform_apply_strength: bad geometry");
+    return launch_adain_transform_apply_strength(HCP(act), N, H, W, C, transform, alpha, strength, HP(out), ST(stream));
 }
 // tuning hooks (wctb200_debug.h; not part of the stable ABI)
 int wctb200_debug_set_conv_bn(int bn) {

@@ -437,6 +437,16 @@ __device__ __forceinline__ void frag_to_tile(const float (&d)[R], float* tile, i
         *reinterpret_cast<float2*>(tile + (r + 8) * pitch + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
     }
 }
+// Weight of transform k at pixel pix of frame n in the weighted apply (soft spatial control, DESIGN.md §3.3.11):
+// v = s(p) w_k(p), with w = 1 without weight planes (K = 1) and s = 1 without a strength map; 0 for a skipped problem
+// (k_c = -1).  wts [N][K][H][W], str [N][H][W], kc [N*K].
+__device__ __forceinline__ float soft_weight(const float* __restrict__ wts, const float* __restrict__ str, const int* __restrict__ kc,
+                                             int K, int n, int k, long long HW, long long pix) {
+    if (kc[n * K + k] < 0) return 0.f;
+    float v = wts ? __ldg(wts + ((long long)n * K + k) * HW + pix) : 1.f;
+    if (str) v = __ldg(str + (long long)n * HW + pix) * v;
+    return v;
+}
 #endif  // __CUDACC__
 
 // per-(device, stream, slot) grow-only scratch buffer (capi.cu); valid until the next call with the same key

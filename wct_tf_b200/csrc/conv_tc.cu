@@ -77,7 +77,25 @@ struct ConvParams {
     const int* counts;    // [N*R] pixels per (image, region); a region with fewer than 2 pixels keeps its input
     const uint16_t* amask;// [m_tiles]: bit r set when the tile holds a pixel of region r, bit R when it holds a kept pixel
     int R;
+    // weighted apply (conv_tc2_kernel<.., REG, WGT = true>, soft spatial control): R = K transforms per image, pixel weights
+    // soft_weight(wts, str, kc, ...); amask bit k: a pixel of the tile has v_k > 0, bit K: one has every v_k = 0
+    const float* wts;     // [N][K][H][W] or nullptr (K = 1, weight 1)
+    const float* str;     // [N][H][W] strength or nullptr (1)
+    const int* kc;        // [N*K] k_c of each transform, -1 = skipped
 };
+
+// v_k at row `row` of an APPLY tile (0 on halo and junk rows)
+__device__ __forceinline__ float row_weight(const ConvParams& p, long long p0, long long p_end, int row, int k) {
+    const unsigned int pos = (unsigned int)p0 + (unsigned int)row;
+    if (pos >= (unsigned int)p_end) return 0.f;
+    const unsigned int hpwp = (unsigned int)(p.Hp * p.Wp);
+    const unsigned int n = pos / hpwp;
+    const unsigned int r = pos - n * hpwp;
+    const int yy = (int)(r / (unsigned int)p.Wp);
+    const int xx = (int)(r - (unsigned int)yy * (unsigned int)p.Wp);
+    if (yy < 1 || yy > p.H || xx < 1 || xx > p.W) return 0.f;
+    return soft_weight(p.wts, p.str, p.kc, p.R, (int)n, k, (long long)p.H * p.W, (long long)(yy - 1) * p.W + (xx - 1));
+}
 
 // region a pixel takes in the regions apply: its label, or R (keep the input) for labels >= R and regions of < 2 pixels
 __device__ __forceinline__ int region_of(const uint8_t* labels, const int* counts, int R, int n, int H, int W, int y, int x) {
@@ -247,10 +265,11 @@ __device__ __forceinline__ void finish8(const float (&a)[8], float wsc, const fl
 // Where row `row` of a 128-position tile goes: returns its halo flags and sets its padded output position, or returns -1
 // when nothing is stored (halo / junk row of the padded tiling, a pixel of another region, an aborted pipeline).
 // REG: the pass stores the pixels of region `want` (R: the pixels that keep their input).
+// WGT: the rows whose weight sum V (vsum[row]) is > 0, or (want == R) the rows with V = 0.
 // (32-bit position arithmetic: P < 2^31 is checked by the launcher; 64-bit divisions cost ~60 instructions each)
-template <bool REG>
+template <bool REG, bool WGT = false>
 __device__ __forceinline__ int row_target(const ConvParams& p, const ActGeom& go, const TileCoord& tc, int row, int want,
-                                          volatile int* abort_flag, unsigned int& ppos) {
+                                          volatile int* abort_flag, unsigned int& ppos, const float* vsum = nullptr) {
     ppos = 0;
     const unsigned int pos = (unsigned int)tc.p0 + (unsigned int)row;
     if (pos >= (unsigned int)tc.p_end) return -1;
@@ -262,7 +281,11 @@ __device__ __forceinline__ int row_target(const ConvParams& p, const ActGeom& go
     if (yy < 1 || yy > p.H || xx < 1 || xx > p.W || *abort_flag) return -1;
     int y = yy - 1, x = xx - 1;
     if (p.mode == CONV_UP2) { y = 2 * y + (tc.cls >> 1); x = 2 * x + (tc.cls & 1); }
-    if (REG && region_of(p.labels, p.counts, p.R, (int)n, p.H, p.W, y, x) != want) return -1;
+    if (WGT) {
+        if ((vsum[row] > 0.f) == (want == p.R)) return -1;
+    } else if (REG && region_of(p.labels, p.counts, p.R, (int)n, p.H, p.W, y, x) != want) {
+        return -1;
+    }
     ppos = ((unsigned int)n * (unsigned int)go.Hp + (unsigned int)(y + 1)) * (unsigned int)go.Wp + (unsigned int)(x + 1);
     return halo_flags(go, y, x);
 }
@@ -271,16 +294,18 @@ __device__ __forceinline__ int row_target(const ConvParams& p, const ActGeom& go
 // channels (8 lanes per position, 8 channels per lane); unit u = (32-row chunk * 8 + j) * NB + 64-channel block goes to
 // warp u % EPI_WARPS.  The lane of a chunk row computes that row's target once; the 8 lanes storing it take it by shuffle.
 // KEEP (REG only): copy the input pixels of the rows to keep (hi and lo bytes) instead of finishing the fp32 tile.
-template <class Cfg, bool REG, bool KEEP>
+// WGT (weighted apply): vst [K + 1][BM] holds v_k and V of every row, `todo` the transforms of the tile; a row finishes as
+// sum + v_0 b_0 + v_1 b_1 + ... (+ (1 - V) x where V < 1), in k order, the bias read from global memory.
+template <class Cfg, bool REG, bool KEEP, bool WGT = false>
 __device__ __forceinline__ void epi_rows(const ConvParams& p, const ActGeom& go, const TileCoord& tc, const float* ctile,
                                          const float* sb, float wsc, bool relu, int want, int ew, int lane,
-                                         volatile int* abort_flag) {
+                                         volatile int* abort_flag, const float* vst = nullptr, unsigned todo = 0u, int img = 0) {
     constexpr int U = 8 * Cfg::NB;                       // units per 32-row chunk
     const int c = lane & 7;
 #pragma unroll 1
     for (int chunk = 0; chunk < Cfg::BM / 32; ++chunk) {
         unsigned int pp;
-        const int fl = row_target<REG>(p, go, tc, chunk * 32 + lane, want, abort_flag, pp);
+        const int fl = row_target<REG, WGT>(p, go, tc, chunk * 32 + lane, want, abort_flag, pp, WGT ? vst + p.R * Cfg::BM : nullptr);
         for (int v = ((ew - chunk * U) % Cfg::EPI_WARPS + Cfg::EPI_WARPS) % Cfg::EPI_WARPS; v < U; v += Cfg::EPI_WARPS) {
             const int j = v / Cfg::NB, b = v - j * Cfg::NB;
             const int r = j * 4 + (lane >> 3);
@@ -293,6 +318,30 @@ __device__ __forceinline__ void epi_rows(const ConvParams& p, const ActGeom& go,
                 const __half* src = p.in + (long long)q * p.Cin + tc.n0 + ch;   // APPLY: input and output positions agree
                 hi = *reinterpret_cast<const Half8*>(src);
                 lo = *reinterpret_cast<const Half8*>(src + (long long)p.P * p.Cin);
+            } else if (WGT) {
+                const int row = chunk * 32 + r;
+                float a[8];
+                tile_load8(ctile + row * Cfg::PITCH + ch, c, a);
+#pragma unroll
+                for (int i = 0; i < 8; ++i) a[i] *= wsc;
+                for (unsigned m = todo; m; m &= m - 1u) {    // (v = 1: fmaf is the plain add of the unweighted epilogue)
+                    const int k = __ffs(m) - 1;
+                    const float vk = vst[k * Cfg::BM + row];
+                    if (vk == 0.f) continue;
+                    const float4* bk = reinterpret_cast<const float4*>(p.bias + (long long)(img * p.R + k) * p.Cout + tc.n0 + ch);
+                    const float4 b0 = __ldg(bk), b1 = __ldg(bk + 1);
+                    a[0] = fmaf(vk, b0.x, a[0]); a[1] = fmaf(vk, b0.y, a[1]); a[2] = fmaf(vk, b0.z, a[2]); a[3] = fmaf(vk, b0.w, a[3]);
+                    a[4] = fmaf(vk, b1.x, a[4]); a[5] = fmaf(vk, b1.y, a[5]); a[6] = fmaf(vk, b1.z, a[6]); a[7] = fmaf(vk, b1.w, a[7]);
+                }
+                const float keep = 1.f - vst[p.R * Cfg::BM + row];
+                if (keep != 0.f) {          // (skipped at V = 1: -0 + 0 would turn a sign bit)
+                    const __half* src = p.in + (long long)q * p.Cin + tc.n0 + ch;
+                    float x[8];
+                    merge8(*reinterpret_cast<const Half8*>(src), *reinterpret_cast<const Half8*>(src + (long long)p.P * p.Cin), x);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) a[i] = fmaf(keep, x[i], a[i]);
+                }
+                split8(a, hi, lo);
             } else {
                 float a[8], bb[8];
                 tile_load8(ctile + (chunk * 32 + r) * Cfg::PITCH + ch, c, a);
@@ -363,7 +412,11 @@ __device__ __forceinline__ void epi_pool(const ConvParams& p, const ActGeom& go,
 // REG (spatial control, CONV_APPLY only): every tile runs one mainloop + epilogue pass per region present in it (its own
 // weight set, stores only the rows of that region), then copies the rows to keep; a tile inside one region costs what the
 // plain apply costs.
-template <int BN, bool FUSE_, bool REG = false>
+// WGT (with REG: the weighted apply of soft spatial control, DESIGN.md §3.3.11): one mainloop pass per transform k present
+// in the tile, each chunk added as fmaf(v_k(row), ch + cx, sum) into ONE running sum across the passes; the epilogue
+// finishes the tile once (sum_k v_k b_k and the keep term) and copies the rows whose weights are all 0.  v = 1 gives the
+// plain add, so one-hot weights give REG's bits.
+template <int BN, bool FUSE_, bool REG = false, bool WGT = false>
 __global__ void __launch_bounds__(Conv2Cfg<BN, FUSE_>::THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const ConvParams p,
                 const int total_tiles, const int n_tiles) {
@@ -381,6 +434,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     volatile int* abort_flag = reinterpret_cast<volatile int*>(tile_empty + 1);
     float* sbias = reinterpret_cast<float*>(aux + 256);  // [2][BN]: bias of the pass (by pass parity)
     float* ctile = reinterpret_cast<float*>(aux + Cfg::AUX_BYTES);
+    float* vst = ctile + Cfg::BM * Cfg::PITCH;           // WGT: [K + 1][BM] v_k and V of the rows of the epilogue's tile
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -490,6 +544,32 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             const int mt = tile / n_tiles;
             unsigned todo = 1u;
             if constexpr (REG) todo = p.amask[mt] & ((1u << p.R) - 1u);
+            if constexpr (WGT) {
+                const int img = mt / p.tiles_per_image;
+                asm volatile("bar.sync 1, %0;" ::"r"(32 * Cfg::EPI_WARPS) : "memory");   // the previous tile's vst is read
+                for (int row = threadIdx.x - (Cfg::CONSUMERS + 32); row < Cfg::BM; row += 32 * Cfg::EPI_WARPS) {
+                    float V = 0.f;
+                    for (int k = 0; k < p.R; ++k) {
+                        const float v = ((todo >> k) & 1u) ? row_weight(p, tc.p0, tc.p_end, row, k) : 0.f;
+                        vst[k * Cfg::BM + row] = v;
+                        V += v;
+                    }
+                    vst[p.R * Cfg::BM + row] = V;
+                }
+                if (todo) {
+                    mbar_wait(tile_full, pass & 1, abort_flag, p.err, 0x301u);
+                    asm volatile("bar.sync 1, %0;" ::"r"(32 * Cfg::EPI_WARPS) : "memory");
+                    epi_rows<Cfg, REG, false, true>(p, go, tc, ctile, sbias, wsc, relu, 0, ew, lane, abort_flag, vst, todo, img);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(tile_empty);
+                    ++pass;
+                } else {
+                    asm volatile("bar.sync 1, %0;" ::"r"(32 * Cfg::EPI_WARPS) : "memory");
+                }
+                if ((p.amask[mt] >> p.R) & 1u)
+                    epi_rows<Cfg, REG, true, true>(p, go, tc, ctile, sbias, wsc, relu, p.R, ew, lane, abort_flag, vst, 0u, img);
+                continue;
+            }
             for (; todo; todo &= todo - 1u, ++pass) {
                 const int region = __ffs(todo) - 1;
                 const int set = REG ? mt / p.tiles_per_image * p.R + region : tc.set;
@@ -520,10 +600,24 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         unsigned todo = 1u;
         if constexpr (REG) todo = p.amask[tile / n_tiles] & ((1u << p.R) - 1u);
-        for (; todo; todo &= todo - 1u, ++pass) {
+        if (WGT && !todo) continue;                       // the epilogue only copies the kept rows
         float sum[Cfg::SUM_REGS];
+        if constexpr (WGT) {
 #pragma unroll
-        for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
+            for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
+        }
+        for (; todo; todo &= todo - 1u) {
+        float vrow[2] = {1.f, 1.f};                      // WGT: v_k of this thread's two fragment rows
+        if constexpr (WGT) {
+            const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
+            const int k = __ffs(todo) - 1;
+            const int r0 = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);
+            vrow[0] = row_weight(p, tc.p0, tc.p_end, r0, k);
+            vrow[1] = row_weight(p, tc.p0, tc.p_end, r0 + 8, k);
+        } else {
+#pragma unroll
+            for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
+        }
         int it = 0, kx = 0;
         for (int c = 0; c < nchunks; ++c) {
             float ch[Cfg::CHUNK_REGS], cx[Cfg::SUM_REGS];
@@ -562,7 +656,16 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                     if (lane == 0) mbar_arrive(&emptyA[sa]);
                 }
             }
-            if constexpr (Cfg::FUSE) {
+            if constexpr (WGT) {
+                // fragment register i belongs to row r0 + 8 ((i >> 1) & 1)
+                if constexpr (Cfg::FUSE) {
+#pragma unroll
+                    for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = fmaf(vrow[(i >> 1) & 1], ch[i] + (ch[Cfg::SUM_REGS + i] + cx[i]), sum[i]);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = fmaf(vrow[(i >> 1) & 1], ch[i] + cx[i], sum[i]);
+                }
+            } else if constexpr (Cfg::FUSE) {
 #pragma unroll
                 for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] += ch[i] + (ch[Cfg::SUM_REGS + i] + cx[i]);
             } else {
@@ -571,12 +674,22 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             }
         }
 
-        // ---- hand the fp32 tile to the epilogue warps (row-major in shared memory: a wgmma fragment spreads one row
-        // over 4 lanes); the previous tile must have been read, which it normally was during this mainloop ----
-        mbar_wait(tile_empty, (pass & 1) ^ 1u, abort_flag, p.err, 0x300u);
-        frag_to_tile(sum, ctile, Cfg::PITCH, 64 * wg, t);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tile_full);
+        if constexpr (!WGT) {
+            // ---- hand the fp32 tile to the epilogue warps (row-major in shared memory: a wgmma fragment spreads one row
+            // over 4 lanes); the previous tile must have been read, which it normally was during this mainloop ----
+            mbar_wait(tile_empty, (pass & 1) ^ 1u, abort_flag, p.err, 0x300u);
+            frag_to_tile(sum, ctile, Cfg::PITCH, 64 * wg, t);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(tile_full);
+            ++pass;
+        }
+        }
+        if constexpr (WGT) {                              // every pass is in the running sum: one hand-off per tile
+            mbar_wait(tile_empty, (pass & 1) ^ 1u, abort_flag, p.err, 0x300u);
+            frag_to_tile(sum, ctile, Cfg::PITCH, 64 * wg, t);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(tile_full);
+            ++pass;
         }
     }
 }
@@ -626,18 +739,21 @@ int make_tensor_map_3d(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d
 
 int g_conv_oversub = 4;
 
-template <int BN, bool FUSE_, bool REG = false>
+template <int BN, bool FUSE_, bool REG = false, bool WGT = false>
 static int launch2_bn(const CUtensorMap& mA, const CUtensorMap& mB, const ConvParams& p, int total_tiles, int n_tiles,
                       cudaStream_t st) {
     using Cfg = Conv2Cfg<BN, FUSE_>;
-    WCTB_ENSURE_SMEM((conv_tc2_kernel<BN, FUSE_, REG>), Cfg::SMEM_BYTES);
+    // WGT: the rows' v_k and V ([9][BM] fp32) after the fp32 tile
+    constexpr int SMEM = Cfg::SMEM_BYTES + (WGT ? 9 * Cfg::BM * 4 : 0);
+    static_assert(SMEM <= 227 * 1024, "conv: shared memory exceeds the 227 KB opt-in limit");
+    WCTB_ENSURE_SMEM((conv_tc2_kernel<BN, FUSE_, REG, WGT>), SMEM);
     // Over-subscribed persistent grid: with g_conv_oversub x #SMs CTAs (1 resident per SM) the
     // hardware block scheduler hands queued CTAs to whichever SMs are free, so a conv launched
     // while the Jacobi clusters of the other stream hold half the SMs still balances its tiles
     // (a grid of exactly #SMs would run as two unbalanced waves).
     int grid = device_sm_count() * (g_conv_oversub > 0 ? g_conv_oversub : 1);
     if (grid > total_tiles) grid = total_tiles;
-    conv_tc2_kernel<BN, FUSE_, REG><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(mA, mB, p, total_tiles, n_tiles);
+    conv_tc2_kernel<BN, FUSE_, REG, WGT><<<grid, Cfg::THREADS, SMEM, st>>>(mA, mB, p, total_tiles, n_tiles);
     WCTB_CHECK_LAUNCH("conv_tc2_kernel");
     return 0;
 }
@@ -662,8 +778,9 @@ int conv_tc_bn(int Cout) {
 static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
                         const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw,
                         const uint8_t* labels, const int* counts, const uint16_t* amask, int R, int bn_req = 0,
-                        long long wplane = 0) {
-    const bool reg = labels != nullptr;
+                        long long wplane = 0, const float* wts = nullptr, const float* str = nullptr, const int* kc = nullptr) {
+    const bool wgt = kc != nullptr;
+    const bool reg = labels != nullptr || wgt;
     WCTB_REQUIRE(!reg || (mode == CONV_APPLY && Cin == Cout && nsets == N * R && flags == 0), "conv: bad regions apply");
     if (reg) nsets = N;                                   // per-image tiling; the region picks the set inside an image
     WCTB_REQUIRE(N >= 1 && H >= 2 && W >= 2, "conv: bad geometry N=%d H=%d W=%d", N, H, W);
@@ -723,6 +840,9 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
     p.counts = counts;
     p.amask = amask;
     p.R = R;
+    p.wts = wts;
+    p.str = str;
+    p.kc = kc;
     if (reg) {
         p.per_image = 1;
         p.nsets = N;
@@ -730,6 +850,13 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
     const int m_tiles = pool ? N * p.pool_ho * p.pool_tx : (p.per_image ? N * p.tiles_per_image : cdiv(gi.P, 128));
     const int n_tiles = Cout / BN;
     const int total = m_tiles * n_tiles * (mode == CONV_UP2 ? 4 : 1);
+    if (wgt) {
+        switch (BN) {
+            case 64: return g_conv_fuse == 0 ? launch2_bn<64, false, true, true>(mA, mB, p, total, n_tiles, st)
+                                             : launch2_bn<64, true, true, true>(mA, mB, p, total, n_tiles, st);
+            default: return launch2_bn<128, false, true, true>(mA, mB, p, total, n_tiles, st);
+        }
+    }
     if (reg) {
         switch (BN) {
             case 64: return g_conv_fuse == 0 ? launch2_bn<64, false, true>(mA, mB, p, total, n_tiles, st)
@@ -761,6 +888,13 @@ int launch_conv_taps_rows(const __half* in, int N, int H, int W, int Cin, const 
 int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const uint8_t* labels,
                               const int* counts, const uint16_t* amask, int R, __half* out, cudaStream_t st) {
     return conv_tc_impl(CONV_APPLY, in, N, H, W, C, w_split, N * R, nullptr, bias, C, 0, out, st, 3, labels, counts, amask, R);
+}
+// out = sum_k v_k (M_{n,k} x + bias_{n,k}) + (1 - sum_k v_k) x, v_k = soft_weight(wts, str, kc, ...) (wct.cu:
+// launch_wct_transform_apply_weighted); amask as in ConvParams
+int launch_conv_apply_weighted(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const float* wts,
+                               const float* str, const int* kc, const uint16_t* amask, int K, __half* out, cudaStream_t st) {
+    return conv_tc_impl(CONV_APPLY, in, N, H, W, C, w_split, N * K, nullptr, bias, C, 0, out, st, 3, nullptr, nullptr, amask, K, 0, 0,
+                        wts, str, kc);
 }
 
 }  // namespace wctb

@@ -44,6 +44,8 @@ struct CovParams {
     const uint8_t* labels;       // [N][H][W] region label per pixel
     const uint16_t* tmask;       // [N][tiles_y * tiles_x]: bit r set when the 32 x 2 tile holds a pixel labelled r
     int R;
+    // soft spatial control (cov_tc_kernel<true, true>): problem z = image * R + k weighs pixel p by wts[z][p] >= 0
+    const float* wts;            // [N][R][H][W]; tmask bit k: the tile holds a pixel of nonzero weight k
 };
 
 struct CovCfg {
@@ -71,7 +73,10 @@ __device__ __forceinline__ void tma_load_5d_cov(void* smem_dst, const void* map,
 // MASK = false: one problem per image (blockIdx.y = image).  MASK = true (spatial control): blockIdx.y = image * R + region;
 // producer and consumers skip the tiles without a pixel of the region (each tile is read once per region present in it),
 // and the centring step writes zeros for the staged pixels of other regions, exactly as for out-of-range pixels.
-template <bool MASK>
+// WGT (with MASK, soft spatial control, DESIGN.md §3.3.11): region r is weight plane r; the centring step scales the staged
+// x - t by sqrt(w) (zeros where w = 0, as MASK writes them), so the product sums w (x - t)(x - t)^T, and s sums w (x - t).
+// With 0/1 weights every value, and so every sum, is that of MASK.
+template <bool MASK, bool WGT = false>
 __global__ void __launch_bounds__(CovCfg::THREADS, 1)
 cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
     using Cfg = CovCfg;
@@ -187,12 +192,18 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
         mbar_wait(&full[s], ph, abort_flag, p.err, 0x550u + s);
         uint8_t* st = smem + s * stage_bytes;
         bool keep[2] = {true, true};                 // MASK: the pixel carries this CTA's region label
+        float wv[2] = {1.f, 1.f};                    // WGT: the pixel's weight
         if (MASK) {
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
                 const int r = rg + 32 * k;
                 const int x = tx * 32 + (r & 31), y = ty * 2 + (r >> 5);
-                keep[k] = x < p.W && y < p.H && p.labels[((long long)img * p.H + y) * p.W + x] == reg;
+                if (WGT) {
+                    wv[k] = (x < p.W && y < p.H) ? __ldg(p.wts + ((long long)prob * p.H + y) * p.W + x) : 0.f;
+                    keep[k] = wv[k] > 0.f;
+                } else {
+                    keep[k] = x < p.W && y < p.H && p.labels[((long long)img * p.H + y) * p.W + x] == reg;
+                }
             }
         }
 #pragma unroll
@@ -223,7 +234,12 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
                         for (int j = 0; j < 8; ++j) v[j] -= sh[op][sl][j];
                         if (op == 0) {
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) sums[sl][j] += v[j];
+                            for (int j = 0; j < 8; ++j) sums[sl][j] += WGT ? wv[k] * v[j] : v[j];
+                        }
+                        if (WGT) {
+                            const float sq = sqrtf(wv[k]);
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) v[j] *= sq;
                         }
                         Half8 nh, nl;
                         split8(v, nh, nl);
@@ -345,13 +361,16 @@ cov_tc_kernel(const __grid_constant__ CUtensorMap mapX, const CovParams p) {
 // MASK (spatial control): grid (C/64, N*R); problem z = n*R + r takes the mean of the sampled pixels labelled r, or of the
 // whole sample when it holds none of them.  A frame-wide shift alone is not enough: a region mean far from t cancels in
 // S - s s^T / n.  With every label equal to r the additions are those of the unmasked kernel.
-template <bool MASK>
+// WGT (soft spatial control): the weighted mean of the sampled pixels under weight plane z (wts [N*R][H][W]), or the
+// frame's shift when they carry no weight; 0/1 weights give MASK's additions.
+template <bool MASK, bool WGT = false>
 __global__ void __launch_bounds__(256)
 k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __restrict__ shift, const uint8_t* __restrict__ labels,
-               int R) {
+               int R, const float* __restrict__ wts = nullptr) {
     __shared__ float red[32][64];
     __shared__ float red_all[MASK ? 32 : 1][64];
     __shared__ int red_n[MASK ? 32 : 1];
+    __shared__ float red_w[WGT ? 32 : 1];
     const int grp = threadIdx.x & 7, rl = threadIdx.x >> 3;
     const int c0 = blockIdx.x * 64 + grp * 8;
     const int n = MASK ? blockIdx.y / R : blockIdx.y;
@@ -361,6 +380,7 @@ k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __r
     const long long nk = c0 < g.C ? ns : 0;
     float s[8], sa[8];
     int cnt = 0;
+    float sw = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) { s[j] = 0.f; sa[j] = 0.f; }
 #pragma unroll 4
@@ -372,6 +392,14 @@ k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __r
         if (MASK) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) sa[j] += v[j];
+            if (WGT) {
+                const float w = wts[(long long)blockIdx.y * HW + q];
+                if (!(w > 0.f)) continue;
+                sw += w;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) s[j] = fmaf(w, v[j], s[j]);
+                continue;
+            }
             if (labels[(long long)n * HW + q] != reg) continue;
             ++cnt;
         }
@@ -384,17 +412,20 @@ k_sample_shift(const __half* __restrict__ act, ActGeom g, int stride, float* __r
         if (MASK) red_all[rl][grp * 8 + j] = sa[j];
     }
     if (MASK && grp == 0) red_n[rl] = cnt;
+    if (WGT && grp == 0) red_w[rl] = sw;
     __syncthreads();
     if (threadIdx.x < 64 && blockIdx.x * 64 + threadIdx.x < g.C) {
-        float a = 0.f, aa = 0.f;
+        float a = 0.f, aa = 0.f, ww = 0.f;
         int m = 0;
 #pragma unroll
         for (int r = 0; r < 32; ++r) {
             a += red[r][threadIdx.x];
             if (MASK) { aa += red_all[r][threadIdx.x]; m += red_n[r]; }
+            if (WGT) ww += red_w[r];
         }
         float t = a / (float)ns;
         if (MASK) t = m > 0 ? a / (float)m : aa / (float)ns;
+        if (WGT) t = ww > 0.f ? a / ww : aa / (float)ns;
         shift[(long long)blockIdx.y * g.C + blockIdx.x * 64 + threadIdx.x] = t;
     }
 }
@@ -423,11 +454,22 @@ __device__ __forceinline__ double part_total(const float* __restrict__ pp, int n
 __device__ __forceinline__ float mean_from_sums(float shift, double s, long long cnt) {
     return cnt > 0 ? (float)((double)shift + s / (double)cnt) : shift;
 }
+// (a record's n is a real number: Kish's effective count of a weighted record; an integer n gives the integer form's bits)
+__device__ __forceinline__ float mean_from_sums(float shift, double s, double cnt) {
+    return cnt > 0.0 ? (float)((double)shift + s / cnt) : shift;
+}
 // (S - si sj / cnt) / (cnt - 1) (+ eps_cov on the diagonal)
 __device__ __forceinline__ float cov_from_sums(double S, double si, double sj, long long cnt, bool diag, float eps_cov) {
     double v = S;
     v -= si * sj / (double)cnt;
     float r = (float)(v / (double)(cnt - 1));
+    if (diag) r += eps_cov;
+    return r;
+}
+__device__ __forceinline__ float cov_from_sums(double S, double si, double sj, double cnt, bool diag, float eps_cov) {
+    double v = S;
+    v -= si * sj / cnt;
+    float r = (float)(v / (cnt - 1.0));
     if (diag) r += eps_cov;
     return r;
 }
@@ -477,26 +519,41 @@ __global__ void k_cov_finalize(const float* __restrict__ part, const double* __r
 // the centring shift t, s = sum (x - t) and S = sum (x - t)(x - t)^T (the diagonal only for AdaIN's moments), all fp64
 // (layout: stats_record_layout, wct.cu).  k_cov_record turns the slots of cov_tc_kernel into a record with the reductions
 // of k_cov_sums / k_cov_finalize; S is written in full, symmetric.
+// Weighted (wq: W = sum w, Q = sum w^2 per problem): the record of Kish's effective count n_eff = W^2 / Q, with s and S
+// scaled by n_eff / W, so that the record's finalize gives mean t + s / W and cov (S - s s^T / W) / (W - Q / W); 0/1
+// weights give n_eff = W and the scale 1 exactly.  A problem without weight gets n = 0.
 // ---------------------------------------------------------------------------
 __global__ void k_cov_record(const float* __restrict__ part, const float* __restrict__ psum, const float* __restrict__ shift, int C,
                              int nslots, int ksplit, long long HW, int count, double* __restrict__ rn, double* __restrict__ rt,
-                             double* __restrict__ rs, double* __restrict__ rS) {
+                             double* __restrict__ rs, double* __restrict__ rS, const double* __restrict__ wq = nullptr) {
     const long long total = (long long)count * C * C;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
         const int j = (int)(t % C);
         const int i = (int)((t / C) % C);
         const long long n = t / ((long long)C * C);
         const long long e = (i <= j) ? (long long)i * C + j : (long long)j * C + i;
-        rS[t] = part_total(part + n * nslots * (long long)C * C + e, nslots, (long long)C * C);
+        double cnt = (double)HW, sc = 1.0;
+        if (wq) {
+            const double W = wq[2 * n], Q = wq[2 * n + 1];
+            cnt = W > 0.0 ? W * W / Q : 0.0;
+            sc = W > 0.0 ? cnt / W : 0.0;
+        }
+        double v = part_total(part + n * nslots * (long long)C * C + e, nslots, (long long)C * C);
+        if (wq) v *= sc;
+        rS[t] = v;
         if (j == 0) {
-            rs[n * C + i] = psum_total(psum, ksplit, C, (int)n, i);
+            double a = psum_total(psum, ksplit, C, (int)n, i);
+            if (wq) a *= sc;
+            rs[n * C + i] = a;
             rt[n * C + i] = (double)shift[n * C + i];
-            if (i == 0) rn[n] = (double)HW;
+            if (i == 0) rn[n] = cnt;
         }
     }
 }
 
-// record -> mean [N][C], G (+ eps_cov I) and its copy A0, [N][C][C]: the expressions of k_cov_sums / k_cov_finalize
+// record -> mean [N][C], G (+ eps_cov I) and its copy A0, [N][C][C]: the expressions of k_cov_sums / k_cov_finalize.
+// n is read as a real number (a weighted record's n_eff); a record of n < 2 gets G = I, k_cov_finalize's placeholder for a
+// problem that is skipped (its k_c is -1: k_transform_kout).
 __global__ void k_record_cov_finalize(const double* __restrict__ rn, const double* __restrict__ rt, const double* __restrict__ rs,
                                       const double* __restrict__ rS, int C, int count, float eps_cov, float* __restrict__ mean,
                                       float* __restrict__ G, float* __restrict__ A0) {
@@ -505,9 +562,10 @@ __global__ void k_record_cov_finalize(const double* __restrict__ rn, const doubl
         const int j = (int)(t % C);
         const int i = (int)((t / C) % C);
         const long long n = t / ((long long)C * C);
-        const long long cnt = (long long)rn[n];
+        const double cnt = rn[n];
         const long long e = (i <= j) ? (long long)i * C + j : (long long)j * C + i;
-        const float r = cov_from_sums(rS[n * C * C + e], rs[n * C + i], rs[n * C + j], cnt, i == j, eps_cov);
+        const float r = cnt < 2.0 ? (i == j ? 1.f : 0.f)
+                                  : cov_from_sums(rS[n * C * C + e], rs[n * C + i], rs[n * C + j], cnt, i == j, eps_cov);
         G[t] = r;
         A0[t] = r;
         if (j == 0) mean[n * C + i] = mean_from_sums((float)rt[n * C + i], rs[n * C + i], cnt);
@@ -538,9 +596,11 @@ int launch_sample_shift(const __half* act, ActGeom g, float* shift, cudaStream_t
 // outputs [N*R][...]; counts [N*R] = pixels per problem and tmask [N][tiles] = regions present per 32 x 2 tile
 // (k_region_scan, wct.cu).
 // With `rec` the sums go to a statistics record instead (mean, G, A0, dsum unused).
+// With `wts` (soft spatial control, [N][R][H][W] fp32 weights, tmask of nonzero weights, wq = W, Q per problem) the
+// problems are weighted and the sums go to the Kish-normalised record `rec` (k_cov_record).
 static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mean, float* G, float* A0, double* dsum,
                          const uint8_t* labels, int R, const int* counts, const uint16_t* tmask, cudaStream_t st,
-                         const StatsRecord* rec = nullptr) {
+                         const StatsRecord* rec = nullptr, const float* wts = nullptr, const double* wq = nullptr) {
     static PFN_encodeTiledC enc = nullptr;
     if (!enc) {
         void* ptr = nullptr;
@@ -554,7 +614,8 @@ static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mea
     }
     WCTB_REQUIRE(g.C == 64 || (g.C % 128 == 0 && g.C <= 2048), "covariance: C=%d must be 64 or a multiple of 128 (<= 2048)", g.C);
     const long long HW = (long long)g.H * g.W;
-    const bool masked = labels != nullptr;
+    const bool weighted = wts != nullptr;
+    const bool masked = labels != nullptr || weighted;
     const int nprob = masked ? g.N * R : g.N;
     CovParams p;
     p.C = g.C; p.W = g.W; p.H = g.H; p.N = g.N;
@@ -585,9 +646,14 @@ static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mea
     p.labels = labels;
     p.tmask = tmask;
     p.R = masked ? R : 1;
+    p.wts = wts;
     // (blocks below the diagonal are never written -- and never read: k_cov_finalize only touches (min,max) entries)
 
-    if (masked) {
+    if (weighted) {
+        k_sample_shift<true, true><<<dim3((unsigned)(g.C / 64), (unsigned)nprob), 256, 0, st>>>(act, g, shift_stride(HW), shift,
+                                                                                                 nullptr, R, wts);
+        WCTB_CHECK_LAUNCH("k_sample_shift");
+    } else if (masked) {
         k_sample_shift<true><<<dim3((unsigned)(g.C / 64), (unsigned)nprob), 256, 0, st>>>(act, g, shift_stride(HW), shift, labels, R);
         WCTB_CHECK_LAUNCH("k_sample_shift");
     } else {
@@ -611,7 +677,10 @@ static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mea
         return WCTB200_ECUDA;
     }
     dim3 grid((unsigned)(npairs * p.ksplit), (unsigned)nprob);
-    if (masked) {
+    if (weighted) {
+        WCTB_ENSURE_SMEM((cov_tc_kernel<true, true>), CovCfg::SMEM_BYTES);
+        cov_tc_kernel<true, true><<<grid, CovCfg::THREADS, CovCfg::SMEM_BYTES, st>>>(mX, p);
+    } else if (masked) {
         WCTB_ENSURE_SMEM(cov_tc_kernel<true>, CovCfg::SMEM_BYTES);
         cov_tc_kernel<true><<<grid, CovCfg::THREADS, CovCfg::SMEM_BYTES, st>>>(mX, p);
     } else {
@@ -622,7 +691,7 @@ static int mean_cov_impl(const __half* act, ActGeom g, float eps_cov, float* mea
     if (rec) {
         const long long tot = (long long)nprob * g.C * g.C;
         k_cov_record<<<(unsigned)(cdiv(tot, 256) > 4096 ? 4096 : cdiv(tot, 256)), 256, 0, st>>>(
-            part, psum, shift, g.C, p.nslots, p.ksplit, HW, nprob, rec->n, rec->t, rec->s, rec->S);
+            part, psum, shift, g.C, p.nslots, p.ksplit, HW, nprob, rec->n, rec->t, rec->s, rec->S, wq);
         WCTB_CHECK_LAUNCH("k_cov_record");
         return 0;
     }
@@ -653,6 +722,13 @@ int launch_cov_record(const __half* act, int N, int H, int W, int C, int y0, int
     v.W = w;
     const __half* base = act + ((long long)y0 * v.Wp + x0) * C;
     return mean_cov_impl(base, v, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, 1, nullptr, nullptr, st, &rec);
+}
+// The weighted record of N*K problems (soft spatial control): weights [N][K][H][W], tmask [N][tiles] of nonzero weights,
+// wq [N*K][2] = (W, Q) (wct.cu: launch_wct_stats_weighted)
+int launch_cov_record_weighted(const __half* act, int N, int H, int W, int C, const float* wts, int K, const uint16_t* tmask,
+                               const double* wq, const StatsRecord& rec, cudaStream_t st) {
+    return mean_cov_impl(act, ActGeom(N, H, W, C), 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, K, nullptr, tmask, st, &rec,
+                         wts, wq);
 }
 int launch_record_cov_finalize(const StatsRecord& rec, int C, int N, float eps_cov, float* mean, float* G, float* A0, cudaStream_t st) {
     const long long tot = (long long)N * C * C;

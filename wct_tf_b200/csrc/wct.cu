@@ -671,6 +671,32 @@ __global__ void k_affine_apply(const __half* __restrict__ in, ActGeom g, const f
         store8_with_halo(out, g, n, y, x, c0, hi, lo);
     }
 }
+// k_affine_apply with a strength map (soft spatial control): alpha s(p) in place of alpha, str [N][H][W]; s = 1 gives
+// k_affine_apply's bits
+__global__ void k_affine_apply_strength(const __half* __restrict__ in, ActGeom g, const float* __restrict__ mean_c,
+                                        const float* __restrict__ inv, const float* __restrict__ ms, float alpha,
+                                        const float* __restrict__ str, __half* __restrict__ out) {
+    const int cgs = g.C / 8;
+    const long long total = (long long)g.N * g.H * g.W * cgs;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int c0 = (int)(i % cgs) * 8;
+        const long long pix = i / cgs;
+        const int x = (int)(pix % g.W);
+        const int y = (int)((pix / g.W) % g.H);
+        const int n = (int)(pix / ((long long)g.W * g.H));
+        const float a = alpha * __ldg(str + pix);
+        float v[8];
+        load8(in, g, ((long long)n * g.Hp + y + 1) * g.Wp + x + 1, c0, v);
+        const float* mc = mean_c + (long long)n * g.C + c0;
+        const float* iv = inv + (long long)n * g.C + c0;
+        const float* m_s = ms + (long long)n * g.C + c0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = fmaf(a, fmaf(v[j] - mc[j], iv[j], m_s[j]), (1.f - a) * v[j]);
+        Half8 hi, lo;
+        split8(v, hi, lo);
+        store8_with_halo(out, g, n, y, x, c0, hi, lo);
+    }
+}
 
 // ---------------------------------------------------------------------------
 // host side
@@ -1106,6 +1132,16 @@ size_t adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, s
     return o;
 }
 
+// the k slot of a transform: k_c, or -1 for a problem that is skipped -- a record of n < 2 (a weighted problem of too
+// little weight) or a style entry with k_s = -1 (an empty style-mask region) -- then the sweeps
+__global__ void k_transform_kout(const int* __restrict__ kc, const double* __restrict__ rn, const int* __restrict__ ks, int Nc, int Ns,
+                                 int* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= Nc) return;
+    out[i] = (rn[i] < 2.0 || ks[Ns == 1 ? 0 : i] == -1) ? -1 : kc[i];
+    out[Nc + i] = kc[Nc + i];
+}
+
 int launch_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
                                     float eps_eig, float thresh, int readd, void* transform, void* ws, size_t ws_bytes,
                                     cudaStream_t st) {
@@ -1133,7 +1169,10 @@ int launch_wct_transform_from_stats(const void* record, int Nc, int C, const voi
     rc = wct_colour_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
                               w, L, reinterpret_cast<__half*>(tp + om), reinterpret_cast<float*>(tp + ob), st);
     if (rc) return rc;
-    WCTB_CUDA(cudaMemcpyAsync(tp + ok, kc, (size_t)Nc * 2 * 4, cudaMemcpyDeviceToDevice, st));
+    k_transform_kout<<<(unsigned)cdiv(Nc, 256), 256, 0, st>>>(kc, stats_record_at(record, C, Nc, 0).n,
+                                                            reinterpret_cast<const int*>(sp + off_k), Nc, Ns,
+                                                            reinterpret_cast<int*>(tp + ok));
+    WCTB_CHECK_LAUNCH("k_transform_kout");
     return 0;
 }
 int launch_wct_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, __half* out, cudaStream_t st) {
@@ -1323,7 +1362,10 @@ int launch_ost_transform_from_stats(const void* record, int Nc, int C, const voi
     rc = ost_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
                        eps_eig, w, O, reinterpret_cast<__half*>(tp + om), reinterpret_cast<float*>(tp + ob), st);
     if (rc) return rc;
-    WCTB_CUDA(cudaMemcpyAsync(tp + ok, kc, (size_t)Nc * 2 * 4, cudaMemcpyDeviceToDevice, st));
+    k_transform_kout<<<(unsigned)cdiv(Nc, 256), 256, 0, st>>>(kc, stats_record_at(record, C, Nc, 0).n,
+                                                            reinterpret_cast<const int*>(sp + off_k), Nc, Ns,
+                                                            reinterpret_cast<int*>(tp + ok));
+    WCTB_CHECK_LAUNCH("k_transform_kout");
     return 0;
 }
 
@@ -1359,6 +1401,21 @@ int launch_adain_transform_apply(const __half* act, int N, int H, int W, int C, 
                                                      reinterpret_cast<const float*>(tp + c), reinterpret_cast<const float*>(tp + d),
                                                      alpha, out);
     WCTB_CHECK_LAUNCH("k_affine_apply");
+    return 0;
+}
+int launch_adain_transform_apply_strength(const __half* act, int N, int H, int W, int C, const void* transform, float alpha,
+                                          const float* strength, __half* out, cudaStream_t st) {
+    WCTB_REQUIRE(C % 8 == 0 && C <= 2048, "adain_transform_apply_strength: C=%d must be a multiple of 8 (<= 2048)", C);
+    size_t a, c, d;
+    adain_transform_layout(C, N, &a, nullptr, &c, &d);
+    const uint8_t* tp = static_cast<const uint8_t*>(transform);
+    const long long total = (long long)N * H * W * (C / 8);
+    long long blocks = (total + 255) / 256;
+    if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
+    k_affine_apply_strength<<<(unsigned)blocks, 256, 0, st>>>(act, ActGeom(N, H, W, C), reinterpret_cast<const float*>(tp + a),
+                                                              reinterpret_cast<const float*>(tp + c), reinterpret_cast<const float*>(tp + d),
+                                                              alpha, strength, out);
+    WCTB_CHECK_LAUNCH("k_affine_apply_strength");
     return 0;
 }
 
@@ -1892,6 +1949,232 @@ int launch_covariance_regions(const __half* act, int N, int H, int W, int C, con
     int rc = region_scan(labels, N, H, W, R, counts, tmask, st);
     if (rc) return rc;
     return launch_mean_cov_regions(act, ActGeom(N, H, W, C), labels, R, counts, tmask, eps_cov, mean_out, cov_out, nullptr, dsum, st);
+}
+
+// ---------------------------------------------------------------------------
+// Soft spatial control (DESIGN.md §3.3.11): K weight planes per frame and a strength map.  Region k's statistics are
+// weighted by w_k (a Kish-normalised record, cov_tc.cu), and the apply blends the K transforms per pixel:
+//   out(p) = sum_k v_k(p) (M_{n,k} x_p + b_{n,k}) + (1 - sum_k v_k(p)) x_p,   v_k = s(p) w_k(p).
+// ---------------------------------------------------------------------------
+// feathering: one-hot plane r of a label map (r < R), blurred by a separable Gaussian of sigma mask pixels, truncated at
+// rad = ceil(3 sigma), taps exp(-d^2 / 2 sigma^2) normalised in fp64, clamp-to-edge borders.  Pass 1 (rows) writes fp64
+// [N][R][Hm][Wm] partial sums, pass 2 (columns) the fp32 planes.  Every block makes the taps in shared memory.
+__device__ __forceinline__ void feather_taps(double* taps, int rad, double sigma) {
+    for (int d = threadIdx.x; d <= rad; d += blockDim.x) taps[d] = exp(-(double)d * d / (2.0 * sigma * sigma));
+    __syncthreads();
+    __shared__ double norm;
+    if (threadIdx.x == 0) {
+        double a = taps[0];
+        for (int d = 1; d <= rad; ++d) a += 2.0 * taps[d];
+        norm = a;
+    }
+    __syncthreads();
+    for (int d = threadIdx.x; d <= rad; d += blockDim.x) taps[d] /= norm;
+    __syncthreads();
+}
+__global__ void __launch_bounds__(256)
+k_feather_rows(const uint8_t* __restrict__ labels, int N, int Hm, int Wm, int R, double sigma, int rad, double* __restrict__ tmp) {
+    extern __shared__ double taps[];
+    feather_taps(taps, rad, sigma);
+    const long long total = (long long)N * R * Hm * Wm;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % Wm);
+        const long long t = i / Wm;
+        const int y = (int)(t % Hm);
+        const long long nr = t / Hm;
+        const int r = (int)(nr % R), n = (int)(nr / R);
+        const uint8_t* row = labels + ((long long)n * Hm + y) * Wm;
+        double a = 0.0;
+        for (int d = -rad; d <= rad; ++d) {
+            const int xx = min(max(x + d, 0), Wm - 1);
+            if (row[xx] == r) a += taps[d < 0 ? -d : d];
+        }
+        tmp[i] = a;
+    }
+}
+__global__ void __launch_bounds__(256)
+k_feather_cols(const double* __restrict__ tmp, int N, int Hm, int Wm, int R, double sigma, int rad, float* __restrict__ out) {
+    extern __shared__ double taps[];
+    feather_taps(taps, rad, sigma);
+    const long long total = (long long)N * R * Hm * Wm;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % Wm);
+        const long long t = i / Wm;
+        const int y = (int)(t % Hm);
+        const double* plane = tmp + (t / Hm) * Hm * Wm;
+        double a = 0.0;
+        for (int d = -rad; d <= rad; ++d) {
+            const int yy = min(max(y + d, 0), Hm - 1);
+            a += taps[d < 0 ? -d : d] * plane[(long long)yy * Wm + x];
+        }
+        out[i] = (float)a;
+    }
+}
+int launch_mask_feather(const uint8_t* labels, int N, int Hm, int Wm, int R, float sigma, float* out, cudaStream_t st) {
+    WCTB_REQUIRE(R >= 1 && R <= 8, "mask_feather: R=%d not in 1..8", R);
+    WCTB_REQUIRE(sigma > 0.f && sigma <= 1024.f, "mask_feather: sigma=%g not in (0, 1024]", (double)sigma);
+    const int rad = (int)ceil(3.0 * (double)sigma);
+    const long long total = (long long)N * R * Hm * Wm;
+    double* tmp = nullptr;
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&tmp), (size_t)total * sizeof(double), st, 6); if (rc0) return rc0; }
+    long long blocks = (total + 255) / 256;
+    if (blocks > device_sm_count() * 16ll) blocks = device_sm_count() * 16ll;
+    const size_t smem = (size_t)(rad + 1) * sizeof(double);
+    if (smem > 48 * 1024) {
+        WCTB_CUDA(cudaFuncSetAttribute(k_feather_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        WCTB_CUDA(cudaFuncSetAttribute(k_feather_cols, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    k_feather_rows<<<(unsigned)blocks, 256, smem, st>>>(labels, N, Hm, Wm, R, (double)sigma, rad, tmp);
+    WCTB_CHECK_LAUNCH("k_feather_rows");
+    k_feather_cols<<<(unsigned)blocks, 256, smem, st>>>(tmp, N, Hm, Wm, R, (double)sigma, rad, out);
+    WCTB_CHECK_LAUNCH("k_feather_cols");
+    return 0;
+}
+
+// exact area average of P planes Hm x Wm onto Hf x Wf: in units of 1 / (Hf Hm), output row y covers [y Hm, (y+1) Hm) and
+// source row i covers [i Hf, (i+1) Hf); the integer overlaps weigh the sources, the fp64 sum is divided by Hm Wm and rounded
+// once.  The identity at equal size; preserves a constant.
+__global__ void k_weights_resize_area(const float* __restrict__ src, long long P, int Hm, int Wm, int Hf, int Wf, float* __restrict__ dst) {
+    const long long total = P * Hf * Wf;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int x = (int)(i % Wf);
+        const long long t = i / Wf;
+        const int y = (int)(t % Hf);
+        const float* plane = src + (t / Hf) * Hm * Wm;
+        const long long ya = (long long)y * Hm, yb = ya + Hm, xa = (long long)x * Wm, xb = xa + Wm;
+        double a = 0.0;
+        for (long long si = ya / Hf; si * Hf < yb; ++si) {
+            const long long oy = min(yb, (si + 1) * Hf) - max(ya, si * Hf);
+            double r = 0.0;
+            for (long long sj = xa / Wf; sj * Wf < xb; ++sj) {
+                const long long ox = min(xb, (sj + 1) * Wf) - max(xa, sj * Wf);
+                r += (double)ox * (double)plane[si * Wm + sj];
+            }
+            a += (double)oy * r;
+        }
+        dst[i] = (float)(a / ((double)Hm * (double)Wm));
+    }
+}
+int launch_weights_resize_area(const float* src, int N, int K, int Hm, int Wm, int Hf, int Wf, float* dst, cudaStream_t st) {
+    const long long total = (long long)N * K * Hf * Wf;
+    long long blocks = (total + 255) / 256;
+    if (blocks > device_sm_count() * 16ll) blocks = device_sm_count() * 16ll;
+    k_weights_resize_area<<<(unsigned)blocks, 256, 0, st>>>(src, (long long)N * K, Hm, Wm, Hf, Wf, dst);
+    WCTB_CHECK_LAUNCH("k_weights_resize_area");
+    return 0;
+}
+
+// one warp per 32 x 2 covariance tile: tmask[n][tile] bit k when a pixel of the tile has w_k > 0.  grid (cdiv(tiles, 8), N)
+__global__ void __launch_bounds__(256)
+k_weights_scan(const float* __restrict__ wts, int H, int W, int K, int tiles_x, int tiles, uint16_t* __restrict__ tmask) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int t = blockIdx.x * 8 + warp, n = blockIdx.y;
+    if (t >= tiles) return;
+    const int ty = t / tiles_x, tx = t - ty * tiles_x;
+    const int x = tx * 32 + lane;
+    const long long HW = (long long)H * W;
+    unsigned bits = 0;
+    for (int k = 0; k < K; ++k) {
+        bool any = false;
+        for (int j = 0; j < 2; ++j) {
+            const int y = ty * 2 + j;
+            if (x < W && y < H && wts[((long long)n * K + k) * HW + (long long)y * W + x] > 0.f) any = true;
+        }
+        if (__any_sync(0xffffffffu, any)) bits |= 1u << k;
+    }
+    if (lane == 0) tmask[(long long)n * tiles + t] = (uint16_t)bits;
+}
+// wq[z] = (W, Q) = (sum w, sum w^2) of weight plane z, fp64 in a fixed order (256 strided partial sums, then a fixed tree):
+// a function of the plane alone.  grid N*K.
+__global__ void __launch_bounds__(256) k_weights_wq(const float* __restrict__ wts, long long HW, double* __restrict__ wq) {
+    __shared__ double sw[256], sq[256];
+    const float* w = wts + (long long)blockIdx.x * HW;
+    double a = 0.0, b = 0.0;
+    for (long long i = threadIdx.x; i < HW; i += 256) {
+        const double v = (double)w[i];
+        a += v;
+        b += v * v;
+    }
+    sw[threadIdx.x] = a;
+    sq[threadIdx.x] = b;
+    __syncthreads();
+    for (int o = 128; o >= 1; o >>= 1) {
+        if (threadIdx.x < o) {
+            sw[threadIdx.x] += sw[threadIdx.x + o];
+            sq[threadIdx.x] += sq[threadIdx.x + o];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        wq[2 * blockIdx.x] = sw[0];
+        wq[2 * blockIdx.x + 1] = sq[0];
+    }
+}
+
+int launch_cov_record_weighted(const __half* act, int N, int H, int W, int C, const float* wts, int K, const uint16_t* tmask,
+                               const double* wq, const StatsRecord& rec, cudaStream_t st);   // cov_tc.cu
+
+int launch_wct_stats_weighted(const __half* act, int N, int H, int W, int C, const float* wts, int K, void* record, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_stats_weighted: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(K >= 1 && K <= 8, "wct_stats_weighted: K=%d not in 1..8", K);
+    const int tiles_x = (W + 31) / 32, tiles = tiles_x * ((H + 1) / 2);
+    const size_t wq_bytes = align_up((size_t)N * K * 2 * sizeof(double), 256);
+    uint8_t* scratch = nullptr;
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&scratch), wq_bytes + (size_t)N * tiles * 2, st, 6); if (rc0) return rc0; }
+    double* wq = reinterpret_cast<double*>(scratch);
+    uint16_t* tmask = reinterpret_cast<uint16_t*>(scratch + wq_bytes);
+    k_weights_scan<<<dim3((unsigned)cdiv(tiles, 8), (unsigned)N), 256, 0, st>>>(wts, H, W, K, tiles_x, tiles, tmask);
+    WCTB_CHECK_LAUNCH("k_weights_scan");
+    k_weights_wq<<<(unsigned)(N * K), 256, 0, st>>>(wts, (long long)H * W, wq);
+    WCTB_CHECK_LAUNCH("k_weights_wq");
+    return launch_cov_record_weighted(act, N, H, W, C, wts, K, tmask, wq, stats_record_at(record, C, N * K, 0), st);
+}
+
+// per 128-position tile of the weighted apply (per-image tiling over the padded plane): bit k when a pixel has v_k > 0,
+// bit K when a pixel has every v_k = 0 (it keeps its input).  One warp per tile.
+__global__ void __launch_bounds__(256)
+k_weighted_apply_tiles(const float* __restrict__ wts, const float* __restrict__ str, const int* __restrict__ kc, int N, int H, int W,
+                       int K, int tiles_per_image, uint16_t* __restrict__ amask) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long t = (long long)blockIdx.x * 8 + warp;
+    if (t >= (long long)N * tiles_per_image) return;
+    const int n = (int)(t / tiles_per_image), mt = (int)(t - (long long)n * tiles_per_image);
+    const int Wp = W + 2;
+    const long long HpWp = (long long)(H + 2) * Wp, HW = (long long)H * W;
+    unsigned bits = 0;
+    for (int j = lane; j < 128; j += 32) {
+        const long long r = (long long)mt * 128 + j;
+        if (r >= HpWp) break;
+        const int yy = (int)(r / Wp), xx = (int)(r - (long long)yy * Wp);
+        if (yy < 1 || yy > H || xx < 1 || xx > W) continue;
+        const long long pix = (long long)(yy - 1) * W + xx - 1;
+        unsigned b = 0;
+        for (int k = 0; k < K; ++k)
+            if (soft_weight(wts, str, kc, K, n, k, HW, pix) > 0.f) b |= 1u << k;
+        bits |= b ? b : 1u << K;
+    }
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    if (lane == 0) amask[t] = (uint16_t)bits;
+}
+
+int launch_conv_apply_weighted(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const float* wts,
+                               const float* str, const int* kc, const uint16_t* amask, int K, __half* out, cudaStream_t st);
+
+int launch_wct_transform_apply_weighted(const __half* act, int N, int H, int W, int C, const void* transform, int K, const float* wts,
+                                        const float* str, __half* out, cudaStream_t st) {
+    WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_transform_apply_weighted: C=%d not in {64,128,256,512}", C);
+    WCTB_REQUIRE(K >= 1 && K <= 8 && (wts || K == 1), "wct_transform_apply_weighted: K=%d not in 1..8 (1 without weights)", K);
+    size_t om, ob, ok;
+    wct_transform_layout(C, N * K, &om, &ob, &ok);
+    const uint8_t* tp = static_cast<const uint8_t*>(transform);
+    const int* kc = reinterpret_cast<const int*>(tp + ok);
+    const int tpi = cdiv((long long)(H + 2) * (W + 2), 128);
+    uint16_t* amask = nullptr;
+    { int rc0 = scratch_alloc(reinterpret_cast<void**>(&amask), (size_t)N * tpi * 2, st, 7); if (rc0) return rc0; }
+    k_weighted_apply_tiles<<<(unsigned)cdiv((long long)N * tpi, 8), 256, 0, st>>>(wts, str, kc, N, H, W, K, tpi, amask);
+    WCTB_CHECK_LAUNCH("k_weighted_apply_tiles");
+    return launch_conv_apply_weighted(act, N, H, W, C, reinterpret_cast<const __half*>(tp + om), reinterpret_cast<const float*>(tp + ob),
+                                      wts, str, kc, amask, K, out, st);
 }
 
 // ---------------------------------------------------------------------------

@@ -6,6 +6,8 @@ hand-written sm_90a kernel behind the C-ABI (include/wctb200.h).
 """
 from __future__ import annotations
 
+import ctypes
+
 import numpy as np
 import torch
 
@@ -39,6 +41,13 @@ class Act(object):
     @property
     def ptr(self):
         return self.buf.data_ptr()
+
+
+def _soft_slice(soft, lo, hi):
+    """The maps of a soft spatial-control call (strength, weights) for frames [lo, hi)."""
+    if soft is None:
+        return None
+    return tuple(None if m is None else m[lo:hi] for m in soft)
 
 
 class Engine(object):
@@ -484,6 +493,99 @@ class Engine(object):
                    flops=2.0 * C * C * 2 * N * hwc, bytes_=4.0 * C * 2 * N * hwc)
         return out, kbuf
 
+    # ------------------------------------------------------------------ soft spatial control (DESIGN.md §3.3.11)
+    def mask_feather(self, labels, R, sigma):
+        """Device uint8 label maps [N,Hm,Wm] -> fp32 weight planes [N,R,Hm,Wm]: the one-hot plane of each label r < R blurred
+        by a Gaussian of ``sigma`` mask pixels (labels >= R are the keep plane, which the R planes leave)."""
+        N, Hm, Wm = labels.shape
+        out = torch.empty((N, R, Hm, Wm), dtype=torch.float32, device=self.device)
+        self._call("mask_feather", 2, self.lib.wctb200_mask_feather, labels.data_ptr(), N, Hm, Wm, R, float(sigma), out.data_ptr(),
+                   self._stream())
+        return out
+
+    def weights_resize(self, maps, H, W):
+        """Device fp32 maps [N,K,Hm,Wm] -> [N,K,H,W] by the exact area average."""
+        N, K, Hm, Wm = maps.shape
+        out = torch.empty((N, K, H, W), dtype=torch.float32, device=self.device)
+        self._call("weights_resize", 1, self.lib.wctb200_weights_resize_area, maps.data_ptr(), N, K, Hm, Wm, H, W, out.data_ptr(),
+                   self._stream())
+        return out
+
+    def _gather_states(self, states, N, C):
+        """One WCT style state of N*K entries from K states of one style each: entry n*K + k is states[k]."""
+        K = len(states)
+        om, oc, ok, om2, oc2, ok2 = (ctypes.c_size_t() for _ in range(6))
+        self.lib.wctb200_wct_style_state_layout(C, 1, ctypes.byref(om), ctypes.byref(oc), ctypes.byref(ok))
+        total = self.lib.wctb200_wct_style_state_layout(C, N * K, ctypes.byref(om2), ctypes.byref(oc2), ctypes.byref(ok2))
+        out = torch.zeros(total, dtype=torch.uint8, device=self.device)
+        P = N * K
+        for name, o1, o2, nb in (("mean", om, om2, 4 * C), ("cs", oc, oc2, 4 * C * C)):
+            src = torch.stack([s[o1.value:o1.value + nb] for s in states])            # [K, nb]
+            out[o2.value:o2.value + P * nb].view(N, K, nb).copy_(src.unsqueeze(0).expand(N, K, nb))
+        ks = torch.stack([s[ok.value:ok.value + 8].view(torch.int32) for s in states])  # [K, 2]: k_s, sweeps
+        kv = out[ok2.value:ok2.value + 8 * P].view(torch.int32).view(2, N, K)
+        kv.copy_(ks.t().unsqueeze(1).expand(2, N, K))
+        return out
+
+    def soft_level(self, cf, soft, states, n_style, alpha, adain=False, ost=False, labels=None):
+        """One level of a call with soft spatial control (DESIGN.md §3.3.11).  ``soft`` = (strength [N,Hm,Wm] | None,
+        weights [N,K,Hm,Wm] | None) at map resolution; ``states``: the level's style state (one WCT or AdaIN state of
+        ``n_style`` styles), or with weights or ``labels`` a list of K states of one style each; ``labels``: the hard label
+        map [N,Hm,Wm] of a masked call, whose one-hot planes (nearest sampling) are the weights."""
+        st = self._stream()
+        sem = SEMANTICS[self.semantics]
+        strength, weights = soft
+        C, N = cf.C, cf.N
+        s_l = self.weights_resize(strength.unsqueeze(1), cf.H, cf.W) if strength is not None else None
+        out = self._act(N, cf.H, cf.W, C)
+        if weights is None and labels is None:
+            record = torch.empty(self.lib.wctb200_stats_record_layout(C, N, int(adain), None, None, None, None), dtype=torch.uint8,
+                                 device=self.device)
+            self._call("%s_stats_rect[C%d]" % ("adain" if adain else "wct", C), 3,
+                       self.lib.wctb200_adain_stats_rect if adain else self.lib.wctb200_wct_stats_rect, cf.ptr, N, cf.H, cf.W, C,
+                       0, 0, cf.H, cf.W, record.data_ptr(), st)
+            if adain:
+                tr = torch.empty(self.lib.wctb200_adain_transform_layout(C, N, None, None, None, None), dtype=torch.uint8,
+                                 device=self.device)
+                self._call("adain_transform[C%d]" % C, 2, self.lib.wctb200_adain_transform_from_stats, record.data_ptr(), N, C,
+                           states.data_ptr(), n_style, 1e-5, tr.data_ptr(), st)
+                self._call("adain_apply_strength[C%d]" % C, 1, self.lib.wctb200_adain_transform_apply_strength, cf.ptr, N, cf.H,
+                           cf.W, C, tr.data_ptr(), float(alpha), s_l.data_ptr(), out.ptr, st)
+                return out, None
+            P, K, w_l, state = N, 1, None, states
+        else:
+            K = len(states)
+            if weights is not None:
+                w_l = self.weights_resize(weights, cf.H, cf.W)
+            else:
+                lab = self.labels_resize(labels, cf.H, cf.W)
+                w_l = (lab.unsqueeze(1) == torch.arange(K, dtype=torch.uint8, device=self.device).view(1, K, 1, 1)).float()
+            P = N * K
+            state = self._gather_states(states, N, C)
+            n_style = P
+            record = torch.empty(self.lib.wctb200_stats_record_layout(C, P, 0, None, None, None, None), dtype=torch.uint8,
+                                 device=self.device)
+            self._call("wct_stats_weighted[C%d]" % C, 5, self.lib.wctb200_wct_stats_weighted, cf.ptr, N, cf.H, cf.W, C,
+                       w_l.data_ptr(), K, record.data_ptr(), st)
+        tr = torch.empty(self.lib.wctb200_wct_transform_layout(C, P, None, None, None), dtype=torch.uint8, device=self.device)
+        if ost:
+            ws = self._ost_workspace(C, P)
+            self._call("ost_transform[C%d]" % C, 8 + self._matfun_launches(C) + self._ost_launches(C),
+                       self.lib.wctb200_ost_transform_from_stats, record.data_ptr(), P, C, state.data_ptr(), n_style, float(alpha),
+                       sem["eps_cov"], sem["eps_eig"], sem["thresh"], sem["readd"], tr.data_ptr(), ws.data_ptr(), ws.numel(), st)
+        else:
+            ws = self._workspace(C, P, 0)
+            self._call("wct_transform[C%d]" % C, 8 + self._matfun_launches(C), self.lib.wctb200_wct_transform_from_stats,
+                       record.data_ptr(), P, C, state.data_ptr(), n_style, float(alpha), sem["eps_cov"], sem["eps_eig"],
+                       sem["thresh"], sem["readd"], tr.data_ptr(), ws.data_ptr(), ws.numel(), st)
+        hwc = cf.H * cf.W
+        self._call("wct_apply_weighted[C%d]" % C, 2, self.lib.wctb200_wct_transform_apply_weighted, cf.ptr, N, cf.H, cf.W, C,
+                   tr.data_ptr(), K, w_l.data_ptr() if w_l is not None else None, s_l.data_ptr() if s_l is not None else None,
+                   out.ptr, st, flops=2.0 * C * C * 2 * N * hwc * K, bytes_=4.0 * C * 2 * N * hwc)
+        if w_l is not None:
+            w_l.record_stream(torch.cuda.current_stream(self.device))
+        return out, None
+
     # ------------------------------------------------------------------ multimodal style transfer (DESIGN.md §3.3.10)
     @staticmethod
     def check_mst(K, lam):
@@ -623,7 +725,8 @@ class Engine(object):
 
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
-                region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05):
+                region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05, strength_map=None,
+                content_weights=None, mask_feather=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -672,8 +775,56 @@ class Engine(object):
         content pixel with the mode it resembles, smoothed by a Potts term of weight ``mst_smooth`` (DESIGN.md §3.3.10);
         region k of each frame then takes the statistics of style mode k.  ``style_u8`` is one style image.  WCT only; not
         with ``ost``, spatial control, interpolation, the style swap or ``seamless``.  K = 1 is the plain WCT call, byte for
-        byte."""
+        byte.
+
+        Soft spatial control (DESIGN.md §3.3.11): ``strength_map`` (cuda fp32 [1|N,Hm,Wm] in [0,1]) scales the stylisation
+        per pixel, out = s T(x) + (1 - s) x, with WCT, OST, AdaIN and hard masks; ``content_weights`` (cuda fp32
+        [1|N,K,Hm,Wm], weights >= 0 summing to <= 1 per pixel, with ``region_styles`` of K styles and no ``labels``) blends
+        the K region transforms per pixel, each region's statistics weighted by its plane; ``mask_feather`` = sigma (with
+        ``labels``) turns the label map into Gaussian-feathered weights.  Maps of any resolution are area-averaged to each
+        level.  WCT only for weights; not with interpolation, the style swap or ``mst``."""
         N = content_u8.shape[0]
+        soft = None
+        if strength_map is not None or content_weights is not None or mask_feather is not None:
+            if mst is not None or interp_styles is not None or swap5 or swap_targets is not None:
+                raise ValueError("strength_map / content_weights / mask_feather do not combine with mst, interp_styles or "
+                                 "swap5 / swap_targets")
+            if content_weights is not None and labels is not None:
+                raise ValueError("content_weights replaces labels: give one of them")
+            if mask_feather is not None and labels is None:
+                raise ValueError("mask_feather needs labels")
+            if (content_weights is not None or mask_feather is not None) and (adain or ost):
+                raise ValueError("content_weights / mask_feather work with WCT only: not with adain or ost")
+            sm = None
+            if strength_map is not None:
+                sm = strength_map if strength_map.dim() == 3 else strength_map.unsqueeze(0)
+                if sm.dtype != torch.float32 or sm.dim() != 3 or sm.shape[0] not in (1, N) or sm.device != self.device:
+                    raise ValueError("strength_map must be a float32 tensor [1|N,Hm,Wm] on %s" % self.device)
+                sm = sm.expand(N, -1, -1).contiguous()
+            cw = None
+            if content_weights is not None:
+                R = len(region_styles) if region_styles is not None else 0
+                cw = content_weights if content_weights.dim() == 4 else content_weights.unsqueeze(0)
+                if (cw.dtype != torch.float32 or cw.dim() != 4 or cw.shape[0] not in (1, N) or cw.shape[1] != R or not 1 <= R <= 8
+                        or cw.device != self.device):
+                    raise ValueError("content_weights must be a float32 tensor [1|N,K,Hm,Wm] on %s with K = 1..8 region styles"
+                                     % self.device)
+                cw = cw.expand(N, -1, -1, -1).contiguous()
+            elif mask_feather is not None:
+                sigma = float(mask_feather)
+                if not (np.isfinite(sigma) and 0.0 < sigma <= 1024.0):
+                    raise ValueError("mask_feather must be a finite sigma in (0, 1024] mask pixels, got %r" % (mask_feather,))
+                R = len(region_styles) if region_styles is not None else 0
+                if not 1 <= R <= 8:
+                    raise ValueError("spatial control needs 1..8 region styles, got %d" % R)
+                lab = labels if labels.dim() == 3 else labels.unsqueeze(0)
+                if lab.dtype != torch.uint8 or lab.dim() != 3 or lab.shape[0] not in (1, N):
+                    raise ValueError("labels must be uint8 [Hm,Wm] or [N,Hm,Wm]")
+                cw = self.mask_feather(lab.contiguous(), R, sigma).expand(N, -1, -1, -1).contiguous()
+            soft = (sm, cw)
+            if cw is not None and labels is None:
+                # soft weights take the place of the label map: a region call whose labels are never read
+                labels = torch.zeros((N, 1, 1), dtype=torch.uint8, device=self.device)
         if mst is not None:
             K, lam = self.check_mst(mst, mst_smooth)
             if (adain or ost or labels is not None or region_masks is not None or interp_styles is not None or swap5
@@ -724,7 +875,7 @@ class Engine(object):
             if region_masks is not None:
                 region_masks = self.check_region_masks(region_masks, region_styles)
             return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
-                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks, seamless=seamless)
+                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks, seamless=seamless, soft=soft)
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
         if n_style not in (1, N):
@@ -759,11 +910,11 @@ class Engine(object):
                 else:
                     sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
                 return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
-                                         seamless=seamless)
+                                         seamless=seamless, soft=_soft_slice(soft, lo, hi))
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
-                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless)
+                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -857,7 +1008,7 @@ class Engine(object):
                     m.record_stream(side)
         return sides
 
-    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None, seamless=None):
+    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None, seamless=None, soft=None):
         """``stylize`` with several styles (spatial control, style interpolation): images are prepared once per call, and
         every style side is shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the
         label maps or weight rows); ``masks``: the style masks of spatial control (``_region_sides``)."""
@@ -871,11 +1022,11 @@ class Engine(object):
             self._group = 0
         if G == 1:
             out = self._stylize_one(content_u8, None, alpha, adain, want_info, capture, multi=per_frame(0, N) + (sides,),
-                                    seamless=seamless)
+                                    seamless=seamless, soft=soft)
         else:
             out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, adain, False, None,
                                                                                multi=per_frame(lo, hi) + (sides,),
-                                                                               seamless=seamless))
+                                                                               seamless=seamless, soft=_soft_slice(soft, lo, hi)))
         for side in {id(sd.side): sd.side for sd in owned}.values():
             if side is not main:
                 side.wait_stream(main)         # the style states are recycled only after every level used them
@@ -1038,7 +1189,7 @@ class Engine(object):
         return ps.swap[key]
 
     def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
-                     seamless=None):
+                     seamless=None, soft=None):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
         ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
         optimal-transport transform instead of WCT at the other levels; ``seamless``: the wrapped axes of the content path
@@ -1077,7 +1228,12 @@ class Engine(object):
                 for sd in sides:
                     if sd.side is not main:
                         sd.wait(main, relu)
-                if multi is None:
+                if soft is not None and multi is None:
+                    f, kbuf = self.soft_level(cf, soft, style.adain[relu] if adain else style.wct[relu], n_style, alpha, adain, ost)
+                elif soft is not None:             # regions: soft weights, or the hard labels' one-hot planes
+                    f, kbuf = self.soft_level(cf, soft, [sd.wct[relu] for sd in sides], None, alpha,
+                                              labels=per_frame if soft[1] is None else None)
+                elif multi is None:
                     if adain:
                         f, kbuf = self.adain_apply(cf, style.adain[relu], n_style, alpha)
                     elif ost:
@@ -1160,12 +1316,12 @@ class Engine(object):
         tr = torch.empty(self.lib.wctb200_wct_transform_layout(C, 1, None, None, None), dtype=torch.uint8, device=self.device)
         if ost:
             ws = self._ost_workspace(C, 1)
-            self._call("ost_transform[C%d]" % C, 7 + self._matfun_launches(C) + self._ost_launches(C),
+            self._call("ost_transform[C%d]" % C, 8 + self._matfun_launches(C) + self._ost_launches(C),
                        self.lib.wctb200_ost_transform_from_stats, record.data_ptr(), 1, C, state.data_ptr(), 1, float(alpha),
                        sem["eps_cov"], sem["eps_eig"], sem["thresh"], sem["readd"], tr.data_ptr(), ws.data_ptr(), ws.numel(), st)
             return tr
         ws = self._workspace(C, 1, 0)           # keyed by C alone: the tile shapes of a call never add an entry
-        self._call("wct_transform[C%d]" % C, 7 + self._matfun_launches(C), self.lib.wctb200_wct_transform_from_stats,
+        self._call("wct_transform[C%d]" % C, 8 + self._matfun_launches(C), self.lib.wctb200_wct_transform_from_stats,
                    record.data_ptr(), 1, C, state.data_ptr(), 1, float(alpha), sem["eps_cov"], sem["eps_eig"], sem["thresh"],
                    sem["readd"], tr.data_ptr(), ws.data_ptr(), ws.numel(), st)
         return tr

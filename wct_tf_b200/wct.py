@@ -113,6 +113,11 @@ class WCT(object):
             m = m.unsqueeze(0)
         if m.dim() != 3 or m.shape[0] not in (1, n_frames) or m.shape[1] < 1 or m.shape[2] < 1:
             raise ValueError("content_mask must be [Hm,Wm] or [N,Hm,Wm] with N = %d frames, got %s" % (n_frames, tuple(m.shape)))
+        return m.contiguous(), WCT.check_region_styles(styles)
+
+    @staticmethod
+    def check_region_styles(styles):
+        """A list of 1..8 region styles: uint8 [Hs,Ws,3] images or prepared styles of one style each; ValueError else."""
         styles = _style_list(styles)
         if not 1 <= len(styles) <= 8:
             raise ValueError("a content mask needs 1..8 region styles, got %d" % len(styles))
@@ -123,7 +128,35 @@ class WCT(object):
                 continue
             if s.dtype not in (np.uint8, torch.uint8) or s.ndim not in (3, 4) or s.shape[-1] != 3 or (s.ndim == 4 and s.shape[0] != 1):
                 raise ValueError("each region style must be one uint8 [Hs,Ws,3] image")
-        return m.contiguous(), styles
+        return styles
+
+    @staticmethod
+    def check_soft_map(a, n_frames, name, planes=None):
+        """Host-side validation of a soft spatial-control map (DESIGN.md §3.3.11): [Hm,Wm] or [N,Hm,Wm] (``planes`` = K:
+        [K,Hm,Wm] or [N,K,Hm,Wm]), float in [0,1] or uint8 read as v/255.  Returns float32 [1|N,(K,)Hm,Wm]; soft weights
+        whose sum over K exceeds 1 at a pixel are divided by that sum."""
+        t = a.detach().cpu() if isinstance(a, torch.Tensor) else torch.from_numpy(np.asarray(a))
+        if t.dtype == torch.uint8:
+            t = t.to(torch.float64) / 255.0
+        elif t.dtype.is_floating_point:
+            t = t.to(torch.float64)
+        else:
+            raise ValueError("%s must be float in [0,1] or uint8, got %s" % (name, t.dtype))
+        rank = 2 if planes is None else 3
+        if t.dim() == rank:
+            t = t.unsqueeze(0)
+        ok = t.dim() == rank + 1 and t.shape[0] in (1, n_frames) and t.shape[-1] >= 1 and t.shape[-2] >= 1
+        if ok and planes is not None:
+            ok = t.shape[1] == planes
+        if not ok:
+            want = "[Hm,Wm] or [N,Hm,Wm]" if planes is None else "[K,Hm,Wm] or [N,K,Hm,Wm] with K = %d styles" % planes
+            raise ValueError("%s must be %s with N = %d frames, got %s" % (name, want, n_frames, tuple(t.shape)))
+        if not bool(torch.isfinite(t).all()) or bool((t < 0).any()) or bool((t > 1).any()):
+            raise ValueError("%s must hold finite values in [0, 1]" % name)
+        if planes is not None:
+            tot = t.sum(dim=1, keepdim=True)
+            t = torch.where(tot > 1, t / tot.clamp(min=1), t)
+        return t.to(torch.float32).contiguous()
 
     @staticmethod
     def check_style_masks(style_masks, styles):
@@ -231,7 +264,8 @@ class WCT(object):
 
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
-                      swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05):
+                      swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
+                      strength_map=None, content_weights=None, mask_feather=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -302,7 +336,33 @@ class WCT(object):
         style image.  Works with both semantics, ``alpha``, ``passes`` (the style side is made once per call), batches,
         ``return_float`` / ``return_device`` / ``out``, ``synthesize`` and ``temporal``; not with prepared styles (they
         keep no per-level features), one style per frame, ``adain``, ``ost``, ``content_mask`` / ``style_masks``,
-        ``style_weights``, ``swap5`` / ``swap_targets``, ``tile_size`` or ``seamless``."""
+        ``style_weights``, ``swap5`` / ``swap_targets``, ``tile_size`` or ``seamless``.
+
+        Soft spatial control (DESIGN.md §3.3.11).  ``strength_map``: [Hm,Wm] or [N,Hm,Wm], float in [0,1] or uint8 read as
+        v/255, the per-pixel strength s of the call, out = s T(x) + (1 - s) x (in ``np`` semantics towards the unmodified
+        feature x); with WCT, OST, AdaIN, masks, prepared styles, ``alpha``, ``passes``, ``seamless`` and ``temporal``.
+        ``content_weights``: [K,Hm,Wm] or [N,K,Hm,Wm] soft weights of the K region styles given in ``styles`` as for
+        ``content_mask`` (divided by their sum where it exceeds 1); region k's statistics are weighted by plane k and each
+        pixel blends the K transforms, the rest keeping the content.  ``mask_feather`` = sigma > 0 (with ``content_mask``):
+        the label map feathered by a Gaussian of sigma mask pixels into such weights.  Weights work with WCT only; none of
+        the three combines with ``style_weights``, ``swap5`` / ``swap_targets``, ``mst`` or ``tile_size``, and
+        ``content_weights`` not with ``content_mask``.  None for all three changes nothing."""
+        soft = strength_map is not None or content_weights is not None or mask_feather is not None
+        if soft:
+            if (style_weights is not None or swap5 or swap_targets is not None or mst is not None
+                    or (tile_size is not None and tile_size != 0)):
+                raise ValueError("strength_map / content_weights / mask_feather do not combine with style_weights, swap5 / "
+                                 "swap_targets, mst or tile_size")
+            if content_weights is not None and content_mask is not None:
+                raise ValueError("content_weights replaces content_mask: give one of them")
+            if mask_feather is not None:
+                if content_mask is None:
+                    raise ValueError("mask_feather needs content_mask")
+                if isinstance(mask_feather, bool) or not isinstance(mask_feather, (int, float, np.integer, np.floating)) \
+                        or not np.isfinite(mask_feather) or not 0 < mask_feather <= 1024:
+                    raise ValueError("mask_feather must be a finite sigma in (0, 1024] mask pixels, got %r" % (mask_feather,))
+            if (content_weights is not None or mask_feather is not None) and (adain or ost):
+                raise ValueError("content_weights / mask_feather work with WCT only: not with adain or ost")
         if mst is not None:
             mst, mst_smooth = Engine.check_mst(mst, mst_smooth)
             if (adain or ost or content_mask is not None or style_masks is not None or style_weights is not None or swap5
@@ -333,8 +393,8 @@ class WCT(object):
         dev = eng.device
         n = 1 if np.ndim(contents) == 3 else contents.shape[0]
         eng.swap_levels(swap5, swap_targets)                 # ValueError for both, or a level that is not a target
-        if style_masks is not None and content_mask is None:
-            raise ValueError("style_masks needs content_mask")
+        if style_masks is not None and content_mask is None and content_weights is None:
+            raise ValueError("style_masks needs content_mask (or content_weights)")
         if style_weights is not None:
             if content_mask is not None or swap5 or swap_targets is not None:
                 raise ValueError("style_weights does not combine with content_mask or swap5 / swap_targets")
@@ -345,6 +405,15 @@ class WCT(object):
             mask, region_styles = self.check_mask(content_mask, n, styles)
             if style_masks is not None:
                 style_masks = self.check_style_masks(style_masks, region_styles)
+        if content_weights is not None:
+            region_styles = self.check_region_styles(styles)
+            cweights = self.check_soft_map(content_weights, n, "content_weights", planes=len(region_styles))
+            mask = torch.zeros((1, 1, 1), dtype=torch.uint8)     # soft weights take the place of the label map
+            if style_masks is not None:
+                style_masks = self.check_style_masks(style_masks, region_styles)
+            content_mask = mask
+        smap = self.check_soft_map(strength_map, n, "strength_map") if strength_map is not None else None
+        soft_kw = {}
 
         def to_dev(a):
             return _to_dev(a, dev)
@@ -362,6 +431,12 @@ class WCT(object):
             contents = self.swap_fit(contents, swap5, swap_targets, to_dev)
         with torch.cuda.device(dev):
             c = to_dev(contents)
+            if smap is not None:
+                soft_kw["strength_map"] = smap.to(dev, non_blocking=True)
+            if content_weights is not None:
+                soft_kw["content_weights"] = cweights.to(dev, non_blocking=True)
+            elif mask_feather is not None:
+                soft_kw["mask_feather"] = float(mask_feather)
             if style_weights is not None:
                 w_dev = torch.from_numpy(weights).to(dev, non_blocking=True)
                 ist = [style_dev(x) for x in interp_styles]
@@ -385,13 +460,15 @@ class WCT(object):
                     rs, sm = eng.prepare_regions_call(rs, eng.check_region_masks(sm, rs)), None
 
                 def one_pass(x, first):
-                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs, region_masks=sm, seamless=seamless)
+                    return eng.stylize(x, None, alpha=alpha, labels=None if content_weights is not None else lab, region_styles=rs,
+                                       region_masks=sm, seamless=seamless, **soft_kw)
             elif content_mask is not None:
                 lab = mask.to(dev, non_blocking=True)
                 rs = [style_dev(x) for x in region_styles]
 
                 def one_pass(x, first):
-                    return eng.stylize(x, None, alpha=alpha, labels=lab, region_styles=rs, seamless=seamless)
+                    return eng.stylize(x, None, alpha=alpha, labels=None if content_weights is not None else lab, region_styles=rs,
+                                       seamless=seamless, **soft_kw)
             elif mst is not None:
                 s = to_dev(styles)
                 if int(passes) > 1:
@@ -412,7 +489,7 @@ class WCT(object):
                     # whole batch in one call; with one style per frame the engine swaps frame by frame.
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
-                                       swap_targets=swap_targets if first else None, ost=ost, seamless=seamless)
+                                       swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, **soft_kw)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -528,12 +605,17 @@ class WCT(object):
         return self.predict_batch(noise, styles, **kw)
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
-                style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05):
+                style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
+                strength_map=None, content_weights=None, mask_feather=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
         blend.  ``tile_size`` stylises in tiles, ``ost`` uses the optimal-transport transform, ``seamless`` pads the content
-        path circularly and ``mst`` = K matches the content to K modes of the style (``predict_batch``).'''
+        path circularly and ``mst`` = K matches the content to K modes of the style; ``strength_map``, ``content_weights``
+        ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
+        (``predict_batch``).'''
+        soft = {k: v for k, v in (("strength_map", strength_map), ("content_weights", content_weights),
+                                  ("mask_feather", mask_feather)) if v is not None}
         s = time.time()
         seen = {}
 
@@ -553,9 +635,10 @@ class WCT(object):
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, style_weights=style_weights, content_mask=content_mask,
-                                     tile_size=tile_size, seamless=seamless)
-        elif content_mask is not None:
+                                     tile_size=tile_size, seamless=seamless, **soft)
+        elif content_mask is not None or content_weights is not None:
             kw = {} if style_masks is None else dict(style_masks=style_masks)
+            kw.update(soft)
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, content_mask=content_mask, tile_size=tile_size, seamless=seamless, **kw)
         else:
@@ -568,6 +651,7 @@ class WCT(object):
                 kw["seamless"] = seamless
             if mst is not None:
                 kw.update(mst=mst, mst_smooth=mst_smooth)
+            kw.update(soft)
             out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
