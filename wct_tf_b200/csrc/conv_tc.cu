@@ -118,10 +118,12 @@ __device__ __forceinline__ int region_of(const uint8_t* labels, const int* count
 //     BN = 64: 3), the B ring one tap's [b_hi | b_lo] per k-iteration (BN = 128: 2, BN = 64: 4).  k-iterations run in
 //     the order (filter row, channel slice, column tap), so a strip is released after its last column tap.  With one
 //     channel slice (Cin = 64) this is the tap order of a ring without strips, and the sums are the same bit for bit;
-//   * chunked accumulation: CH k-iterations accumulate into register chunks that start from zero (one for a_hi b_hi, one
-//     for the two small cross products) and are then added into the running sum with round-to-nearest FADDs.  The tensor
-//     core adds into its fp32 accumulator with truncation; short chunks summed in registers keep the conv at fp32-class
-//     error for K up to 4608;
+//   * accumulation: the tensor core adds into its fp32 accumulator with truncation.  a_hi b_hi accumulates CH k-iterations
+//     at a time into a register chunk that starts from zero and is then added into the running sum with round-to-nearest
+//     FADDs; the two small cross products (|a_lo| <= 2^-11 |a|, |b_lo| <= 2^-11 |b|) accumulate in ONE accumulator over
+//     the whole K, added once at the end, whose truncation error stays below 2^-24 sum |a||b| for K up to 4608
+//     (DESIGN.md §3.1).  So a k-iteration is two wgmma groups, a_hi b_hi then the cross products, and at BN = 64 the
+//     cross products of one k-iteration still run while the next one is issued;
 //   * tile hand-off: one fp32 tile buffer in shared memory and two mbarriers.  Every consumer warp arrives on tile_full
 //     after writing its fragment rows; every epilogue warp arrives on tile_empty after its last read.  A consumer waits
 //     on tile_empty only before writing the NEXT tile, a whole mainloop later, so the epilogue runs in the shadow of the
@@ -153,6 +155,10 @@ struct Conv2Cfg {
     static constexpr int CHUNK_REGS = FUSE ? BN : BN / 2;       // per-thread fp32 registers of one accumulation chunk
     static constexpr int SUM_REGS = BN / 2;                     // per-thread fp32 registers of the m64 x BN running sum
     static constexpr int CH = 2;                                // k-iterations per accumulation chunk
+    // wgmma groups a consumer leaves in flight from one k-iteration into the next.  Measured on the H100 (DESIGN.md §6):
+    // BN = 64 is 1-7 % faster with its cross products running while it issues the next k-iteration than drained; BN = 128
+    // (two B slots) is 20-40 % slower that way, so it drains every k-iteration
+    static constexpr int IN_FLIGHT = BN == 64 ? 1 : 0;
     static constexpr int CONSUMERS = 256;
     static constexpr int THREADS = CONSUMERS + 128;
     static constexpr int EPI_WARPS = 3;                         // warps 9-11 of the producer warpgroup
@@ -212,31 +218,54 @@ __device__ __forceinline__ TileCoord tile_coord(const ConvParams& p, int tile, i
     return t;
 }
 
-// One pipeline stage (BK = 64: four 16-wide k-steps) of split-fp16 products into the chunk accumulators:
-// `ch` takes a_hi b_hi (FUSE: a_hi [b_hi | b_lo]), `cx` the small cross terms a_hi b_lo + a_lo b_hi (FUSE: a_lo b_hi), so
-// that the truncating adds of the cross terms never touch the large a_hi b_hi sum.
-// NP = 3: all three products (default), 2: without a_lo b_hi, 1: a_hi b_hi only (experiment knob).
-// NP is a template argument so that the wgmma sequence has no branches between its instructions.
-template <class Cfg, int NP>
-__device__ __forceinline__ void conv_stage_mma(float (&ch)[Cfg::CHUNK_REGS], float (&cx)[Cfg::SUM_REGS], uint64_t a_hi,
-                                               uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
+// One pipeline stage (BK = 64: four 16-wide k-steps) of split-fp16 products, issued as two commit groups.
+// conv_stage_ch: `ch`, the chunk accumulator of a_hi b_hi (FUSE: a_hi [b_hi | b_lo]), restarted from zero when `first`.
+template <class Cfg>
+__device__ __forceinline__ void conv_stage_ch(float (&ch)[Cfg::CHUNK_REGS], uint64_t a_hi, uint64_t b_hi, bool first) {
 #pragma unroll
     for (int k = 0; k < Cfg::BK / 16; ++k) {
         const uint64_t ko = (uint64_t)(k * 32 >> 4);
         const uint32_t acc_in = (first && k == 0) ? 0u : 1u;
+        // FUSE: [b_hi | b_lo] is one 2*BN-row K-major tile: columns [0,BN) += a_hi b_hi, [BN,2BN) += a_hi b_lo
+        if constexpr (Cfg::CHUNK_REGS == 64) wgmma_m64n128k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
+        else wgmma_m64n64k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
+    }
+    wgmma_commit();
+}
+
+// conv_stage_cx: `cx`, the accumulator of the small cross terms a_hi b_lo + a_lo b_hi (FUSE: a_lo b_hi) over the whole pass,
+// zeroed by the caller when the pass starts.  The truncating adds of the cross terms never touch the large a_hi b_hi sum.
+// NP = 3: all three products (default), 2: without a_lo b_hi, 1: a_hi b_hi only (experiment knob; the group is empty).
+// NP is a template argument so that the wgmma sequence has no branches between its instructions.
+template <class Cfg, int NP>
+__device__ __forceinline__ void conv_stage_cx(float (&cx)[Cfg::SUM_REGS], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi,
+                                              uint64_t b_lo) {
+#pragma unroll
+    for (int k = 0; k < Cfg::BK / 16; ++k) {
+        const uint64_t ko = (uint64_t)(k * 32 >> 4);
         if constexpr (Cfg::FUSE) {
-            // [b_hi | b_lo] is one 2*BN-row K-major tile: columns [0,BN) += a_hi b_hi, [BN,2BN) += a_hi b_lo
-            wgmma_m64n128k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
-            if (NP >= 3) wgmma_m64n64k16<0, 0>(cx, a_lo + ko, b_hi + ko, acc_in);
-        } else if constexpr (Cfg::CHUNK_REGS == 64) {
-            wgmma_m64n128k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
-            if (NP >= 2) wgmma_m64n128k16<0, 0>(cx, a_hi + ko, b_lo + ko, acc_in);
+            if (NP >= 3) wgmma_m64n64k16<0, 0>(cx, a_lo + ko, b_hi + ko, 1u);
+        } else if constexpr (Cfg::SUM_REGS == 64) {
+            if (NP >= 2) wgmma_m64n128k16<0, 0>(cx, a_hi + ko, b_lo + ko, 1u);
             if (NP >= 3) wgmma_m64n128k16<0, 0>(cx, a_lo + ko, b_hi + ko, 1u);
         } else {
-            wgmma_m64n64k16<0, 0>(ch, a_hi + ko, b_hi + ko, acc_in);
-            if (NP >= 2) wgmma_m64n64k16<0, 0>(cx, a_hi + ko, b_lo + ko, acc_in);
+            if (NP >= 2) wgmma_m64n64k16<0, 0>(cx, a_hi + ko, b_lo + ko, 1u);
             if (NP >= 3) wgmma_m64n64k16<0, 0>(cx, a_lo + ko, b_hi + ko, 1u);
         }
+    }
+    wgmma_commit();
+}
+
+// sum += acc (FUSE chunk: its two column halves a_hi b_hi + a_hi b_lo added first); WGT: sum = fmaf(v_row, acc, sum).
+// Round-to-nearest FADD / FFMA, in the same order in every instantiation, so that unit weights give the plain sum's bits.
+template <class Cfg, bool WGT, int R>
+__device__ __forceinline__ void add_into_sum(float (&sum)[Cfg::SUM_REGS], const float (&acc)[R], const float (&vrow)[2]) {
+#pragma unroll
+    for (int i = 0; i < Cfg::SUM_REGS; ++i) {
+        float a = acc[i];
+        if constexpr (R > Cfg::SUM_REGS) a += acc[Cfg::SUM_REGS + i];
+        // fragment register i belongs to row r0 + 8 ((i >> 1) & 1)
+        sum[i] = WGT ? fmaf(vrow[(i >> 1) & 1], a, sum[i]) : sum[i] + a;
     }
 }
 
@@ -413,9 +442,9 @@ __device__ __forceinline__ void epi_pool(const ConvParams& p, const ActGeom& go,
 // weight set, stores only the rows of that region), then copies the rows to keep; a tile inside one region costs what the
 // plain apply costs.
 // WGT (with REG: the weighted apply of soft spatial control, DESIGN.md §3.3.11): one mainloop pass per transform k present
-// in the tile, each chunk added as fmaf(v_k(row), ch + cx, sum) into ONE running sum across the passes; the epilogue
-// finishes the tile once (sum_k v_k b_k and the keep term) and copies the rows whose weights are all 0.  v = 1 gives the
-// plain add, so one-hot weights give REG's bits.
+// in the tile, each chunk added as fmaf(v_k(row), ch, sum) and the pass's cross products as fmaf(v_k(row), cx, sum) into
+// ONE running sum across the passes; the epilogue finishes the tile once (sum_k v_k b_k and the keep term) and copies the
+// rows whose weights are all 0.  v = 1 gives the plain add, so one-hot weights give REG's bits.
 template <int BN, bool FUSE_, bool REG = false, bool WGT = false>
 __global__ void __launch_bounds__(Conv2Cfg<BN, FUSE_>::THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const ConvParams p,
@@ -468,7 +497,6 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const int kiters = p.taps * ksl;
     const int ncol = REG ? 1 : p.ncol;                   // the regions apply is a 1x1 conv
     const bool pool = !REG && p.pool;
-    const int nchunks = (kiters + Cfg::CH - 1) / Cfg::CH;
 
     // register split, checked with ptxas -v to spill nothing: the consumers of BN = 128 need more than 200 and the epilogue
     // warps more than 56 (REG: 80).  setmaxnreg.inc only receives what the other warpgroups released, so the split must
@@ -618,61 +646,78 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 #pragma unroll
             for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
         }
-        int it = 0, kx = 0;
-        for (int c = 0; c < nchunks; ++c) {
-            float ch[Cfg::CHUNK_REGS], cx[Cfg::SUM_REGS];
+        // ch restarts every CH k-iterations and is added into sum at each chunk end; cx runs over the whole pass and is added
+        // once, after the last chunk (DESIGN.md §3.1)
+        float ch[Cfg::CHUNK_REGS], cx[Cfg::SUM_REGS];
 #pragma unroll
-            for (int i = 0; i < Cfg::CHUNK_REGS; ++i) ch[i] = 0.f;
+        for (int i = 0; i < Cfg::CHUNK_REGS; ++i) ch[i] = 0.f;
 #pragma unroll
-            for (int i = 0; i < Cfg::SUM_REGS; ++i) cx[i] = 0.f;
-            const int it_end = min(kiters, (c + 1) * Cfg::CH);
-            for (; it < it_end; ++it, ++itg) {
-                const int sa = stg % Cfg::A_STAGES;
-                if (kx == 0) mbar_wait(&fullA[sa], (stg / Cfg::A_STAGES) & 1, abort_flag, p.err, 0x210u + sa);
-                const int s = itg % Cfg::B_STAGES;
-                const uint32_t ph = (itg / Cfg::B_STAGES) & 1;
-                mbar_wait(&full[s], ph, abort_flag, p.err, 0x200u + s);
-                // this warpgroup's operand rows: tile rows 64 wg .. (POOL2: the second segment), column tap kx kx rows further
-                const uint32_t sta = smem_u32(smem + sa * Cfg::STRIP_BYTES) + (wg * (pool ? Cfg::POOL_SEG_ROWS : 64) + kx) * 128;
-                const uint64_t a_hi = gmma_desc_sw128(sta);
-                const uint64_t a_lo = gmma_desc_sw128(sta + Cfg::PLANE_BYTES);
-                const uint32_t stb = smem_u32(bring + s * Cfg::B_SLOT_BYTES);
-                const uint64_t b_hi = gmma_desc_sw128(stb);
-                const uint64_t b_lo = gmma_desc_sw128(stb + Cfg::B_BYTES);
-                const bool first = (it == c * Cfg::CH);
-                wgmma_fence();
-                if (p.products >= 3) conv_stage_mma<Cfg, 3>(ch, cx, a_hi, a_lo, b_hi, b_lo, first);
-                else if (p.products == 2) conv_stage_mma<Cfg, 2>(ch, cx, a_hi, a_lo, b_hi, b_lo, first);
-                else conv_stage_mma<Cfg, 1>(ch, cx, a_hi, a_lo, b_hi, b_lo, first);
-                wgmma_commit();
-                wgmma_wait<0>();
-                acc_fence(ch);
-                acc_fence(cx);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[s]);   // slot may be refilled
-                if (++kx == ncol) {                    // last column tap of the strip
-                    kx = 0;
-                    ++stg;
-                    if (lane == 0) mbar_arrive(&emptyA[sa]);
+        for (int i = 0; i < Cfg::SUM_REGS; ++i) cx[i] = 0.f;
+        int kx = 0;
+        for (int it = 0; it < kiters; ++it, ++itg) {
+            const int sa = stg % Cfg::A_STAGES;
+            if (kx == 0) mbar_wait(&fullA[sa], (stg / Cfg::A_STAGES) & 1, abort_flag, p.err, 0x210u + sa);
+            const int s = itg % Cfg::B_STAGES;
+            const uint32_t ph = (itg / Cfg::B_STAGES) & 1;
+            mbar_wait(&full[s], ph, abort_flag, p.err, 0x200u + s);
+            // this warpgroup's operand rows: tile rows 64 wg .. (POOL2: the second segment), column tap kx kx rows further
+            const uint32_t sta = smem_u32(smem + sa * Cfg::STRIP_BYTES) + (wg * (pool ? Cfg::POOL_SEG_ROWS : 64) + kx) * 128;
+            const uint64_t a_hi = gmma_desc_sw128(sta);
+            const uint64_t a_lo = gmma_desc_sw128(sta + Cfg::PLANE_BYTES);
+            const uint32_t stb = smem_u32(bring + s * Cfg::B_SLOT_BYTES);
+            const uint64_t b_hi = gmma_desc_sw128(stb);
+            const uint64_t b_lo = gmma_desc_sw128(stb + Cfg::B_BYTES);
+            // IN_FLIGHT: in flight at the top of every k-iteration but the pass's first is the cx group of k-iteration it - 1,
+            // nothing else.  Each wait below leaves exactly one group running, so the same group is in flight on every path
+            // into the loop's back edge: where the paths differ, ptxas serialises every wgmma of the kernel.
+            wgmma_fence();
+            conv_stage_ch<Cfg>(ch, a_hi, b_hi, it % Cfg::CH == 0);
+            wgmma_wait<1>();                             // IN_FLIGHT: cx of k-iteration it - 1 has retired
+            // (REG runs APPLY convs, which the products knob leaves at 3: one wgmma sequence keeps the regions apply at
+            // BN = 128 within its 208 registers)
+            if (REG || p.products >= 3) conv_stage_cx<Cfg, 3>(cx, a_hi, a_lo, b_hi, b_lo);
+            else if (p.products == 2) conv_stage_cx<Cfg, 2>(cx, a_hi, a_lo, b_hi, b_lo);
+            else conv_stage_cx<Cfg, 1>(cx, a_hi, a_lo, b_hi, b_lo);
+            if constexpr (Cfg::IN_FLIGHT) {
+                // free the B slot of k-iteration it - 1, and its strip after its last column tap (after the issue above, so
+                // that the cross products are queued first)
+                if (it > 0) {
+                    __syncwarp();
+                    if (lane == 0) {
+                        mbar_arrive(&empty[(itg - 1) % Cfg::B_STAGES]);
+                        if (kx == 0) mbar_arrive(&emptyA[(stg - 1) % Cfg::A_STAGES]);
+                    }
                 }
             }
-            if constexpr (WGT) {
-                // fragment register i belongs to row r0 + 8 ((i >> 1) & 1)
-                if constexpr (Cfg::FUSE) {
-#pragma unroll
-                    for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = fmaf(vrow[(i >> 1) & 1], ch[i] + (ch[Cfg::SUM_REGS + i] + cx[i]), sum[i]);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = fmaf(vrow[(i >> 1) & 1], ch[i] + cx[i], sum[i]);
+            wgmma_wait<Cfg::IN_FLIGHT>();                // ch of this k-iteration has retired (IN_FLIGHT: its cx runs on)
+            if constexpr (!Cfg::IN_FLIGHT) {             // free this k-iteration's slot, and its strip after the last tap
+                __syncwarp();
+                if (lane == 0) {
+                    mbar_arrive(&empty[s]);
+                    if (kx + 1 == ncol) mbar_arrive(&emptyA[sa]);
                 }
-            } else if constexpr (Cfg::FUSE) {
-#pragma unroll
-                for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] += ch[i] + (ch[Cfg::SUM_REGS + i] + cx[i]);
-            } else {
-#pragma unroll
-                for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] += ch[i] + cx[i];
+            }
+            if (++kx == ncol) {
+                kx = 0;
+                ++stg;
+            }
+            if ((it + 1) % Cfg::CH == 0) {              // chunk end
+                acc_fence(ch);
+                add_into_sum<Cfg, WGT>(sum, ch, vrow);
             }
         }
+        wgmma_wait<0>();
+        acc_fence(ch);
+        acc_fence(cx);
+        if constexpr (Cfg::IN_FLIGHT) {
+            __syncwarp();
+            if (lane == 0) {                             // the last k-iteration is the last column tap of its strip
+                mbar_arrive(&empty[(itg - 1) % Cfg::B_STAGES]);
+                mbar_arrive(&emptyA[(stg - 1) % Cfg::A_STAGES]);
+            }
+        }
+        if (kiters % Cfg::CH != 0) add_into_sum<Cfg, WGT>(sum, ch, vrow);   // the last chunk is a short one
+        add_into_sum<Cfg, WGT>(sum, cx, vrow);
 
         if constexpr (!WGT) {
             // ---- hand the fp32 tile to the epilogue warps (row-major in shared memory: a wgmma fragment spreads one row
