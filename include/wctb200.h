@@ -452,6 +452,29 @@ WCTB200_API int wctb200_mst_data_term(const void* content, int N, int H, int W, 
 WCTB200_API int wctb200_mst_smooth(const float* D, int N, int H, int W, int K, float lambda, int sweeps, uint8_t* labels_out,
                                    void* stream);
 
+/* ---- exact feature distribution matching (EFDM, DESIGN.md §3.3.12; efdm.cu) ------
+ * A segment is one (frame, channel) of a feature map.  Each content segment of Nc = H*W values x_p takes the distribution of
+ * the same channel of its style (Q_0 <= ... <= Q_{Ms-1}, Ms = Hs*Ws) by rank: with the content sorted,
+ *   q(r) = Q linearly interpolated at u(r) = clamp((2r+1) Ms / (2 Nc) - 1/2, 0, Ms-1)   (q(r) = Q_r when Ms = Nc),
+ * every run [r0, r1) of equal content values takes t = mean of q over the run (fp64 prefix sums in a fixed order), and
+ *   out_p = alpha t + (1 - alpha) x_p,   x_p = hi + lo of the SPF16 input, -0 counted as +0.
+ * out is SPF16 [N,H,W,C] with the reflect halo; alpha = 0 copies the content's bytes.  C a multiple of 8; the content is at
+ * least 2x2; a style may be 1x1.
+ * style_prepare: style SPF16 [Ns,Hs,Ws,C] -> state, the sorted values fp32 [Ns][C][Ms], of
+ * wctb200_efdm_style_state_bytes(C, Ns, Hs, Ws) bytes (0: bad geometry).  Workspace: wctb200_efdm_style_workspace_bytes(C, Ns,
+ * Hs, Ws, S) bytes sort S segments at a time (14 launches per chunk of S).
+ * apply: content SPF16 [N,H,W,C] against a state of Ns in {1, N} styles (frame n takes style n, or style 0), WCTB200_EINVAL
+ * otherwise.  ws: wctb200_efdm_workspace_bytes(C, N, H, W, S) bytes process S whole segments at a time (18 launches per chunk;
+ * 1 launch for alpha = 0, which reads no workspace); less than one segment's is WCTB200_EWS.  The output is byte-identical
+ * for every workspace size, and a frame's bytes do not depend on the other frames of the call. */
+WCTB200_API size_t wctb200_efdm_style_state_bytes(int C, int Ns, int Hs, int Ws);
+WCTB200_API size_t wctb200_efdm_style_workspace_bytes(int C, int Ns, int Hs, int Ws, int max_segments);
+WCTB200_API int wctb200_efdm_style_prepare(const void* style, int Ns, int Hs, int Ws, int C, void* state, void* ws, size_t ws_bytes,
+                                           void* stream);
+WCTB200_API size_t wctb200_efdm_workspace_bytes(int C, int N, int H, int W, int max_segments);
+WCTB200_API int wctb200_efdm_apply(const void* content, int N, int H, int W, int C, const void* state, int Ns, int Hs, int Ws,
+                                   float alpha, void* out, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- soft spatial control (DESIGN.md §3.3.11) -----------------------------------
  * mask_feather: labels device uint8 [N][Hm][Wm], R in 1..8, sigma in (0, 1024] mask pixels -> out fp32 [N][R][Hm][Wm]: the
  * one-hot plane of label r blurred by a separable Gaussian (taps exp(-d^2 / 2 sigma^2), |d| <= ceil(3 sigma), normalised in

@@ -47,6 +47,12 @@ of the content pair up with modes of the painting without masks (DESIGN.md §3.3
 ``--adain``, ``--ost``, ``--content-mask``, ``--interp-styles``, ``--swap5``, ``--swap-targets``, ``--tile-size``,
 ``--seamless`` or prepared styles (``.wctstyle``).
 
+Exact feature distribution matching: ``--efdm`` gives every channel of each level the whole value distribution of the same
+channel of the style, by rank, instead of matching only its covariance (DESIGN.md §3.3.12): sparse bright strokes and an
+even wash with the same statistics stylise differently.  It suits ``--noise`` texture synthesis.  Output names are
+unchanged.  Not with ``--adain``, ``--ost``, ``--mst``, ``--content-mask``, ``--mask-weights``, ``--mask-feather``,
+``--strength-map``, ``--interp-styles``, ``--tile-size`` or prepared styles (``.wctstyle``).
+
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
 models are not on disk (offline build).
@@ -103,6 +109,8 @@ _FLAGS = [
                       help="multimodal style transfer: cluster each level's style into K modes (1..8) and match the content to them")),
     (("--mst-smooth",), dict(type=float, default=None, metavar="LAMBDA",
                              help="with --mst: Potts smoothness of the content labelling, finite and >= 0 (default 0.05)")),
+    (("--efdm",), dict(action="store_true", default=False,
+                       help="exact feature distribution matching: give every channel the style's whole value distribution")),
     (("--strength-map",), dict(type=str, default=None, metavar="PATH",
                                help="8-bit grayscale map of the per-pixel stylisation strength (gray v -> v/255)")),
     (("--mask-feather",), dict(type=float, default=None, metavar="SIGMA",
@@ -142,6 +150,7 @@ def parse_args(argv=None):
     check_ost_flags(parser, args)
     check_seamless_flags(parser, args)
     check_mst_flags(parser, args)
+    check_efdm_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
@@ -266,6 +275,26 @@ def check_mst_flags(parser, args):
     if style_path and (is_prepared(style_path) or (os.path.isdir(style_path)
                                                    and any(is_prepared(f) for f in os.listdir(style_path)))):
         parser.error("--mst does not combine with prepared styles (.wctstyle)")
+
+
+# flags that do not combine with --efdm (stylize.py and stylize_video.py)
+_EFDM_EXCLUDES = [("adain", "--adain"), ("ost", "--ost"), ("mst", "--mst"), ("content_mask", "--content-mask"),
+                  ("style_masks", "--style-masks"), ("mask_weights", "--mask-weights"), ("mask_feather", "--mask-feather"),
+                  ("strength_map", "--strength-map"), ("interp_styles", "--interp-styles"), ("tile_size", "--tile-size")]
+
+
+def check_efdm_flags(parser, args):
+    """--efdm: a transform of its own, on whole images; not with the other transforms, masks, soft maps, blends, tiles
+    (ranks are taken over the whole image) or prepared styles (which keep no sorted features)."""
+    if not getattr(args, "efdm", False):
+        return
+    for attr, flag in _EFDM_EXCLUDES:
+        if getattr(args, attr, None):
+            parser.error("--efdm does not combine with %s" % flag)
+    style_path = getattr(args, "style_path", None)
+    if style_path and (is_prepared(style_path) or (os.path.isdir(style_path)
+                                                   and any(is_prepared(f) for f in os.listdir(style_path)))):
+        parser.error("--efdm does not combine with prepared styles (.wctstyle)")
 
 
 def check_tile_flags(parser, args):
@@ -464,6 +493,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw["seamless"] = args.seamless
     if args.mst is not None:
         kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
+    if args.efdm:
+        kw["efdm"] = True
     kw.update(soft_kw(args))
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):

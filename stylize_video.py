@@ -27,6 +27,9 @@ clips, on both paths.  Not with ``--temporal`` (the optical flow does not see ac
 
 Multimodal style transfer: ``--mst K [--mst-smooth LAMBDA]`` matches the content to K modes of the style at every level
 (DESIGN.md §3.3.10), on both paths, with the same rejections as stylize.py; it combines with ``--temporal``.
+
+Exact feature distribution matching: ``--efdm`` gives every channel of each level the style's whole value distribution
+(DESIGN.md §3.3.12), on both paths, with the same rejections as stylize.py; it combines with ``--temporal`` and the swap.
 """
 from __future__ import division, print_function
 
@@ -60,7 +63,7 @@ _VIDEO_FLAGS = [
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
            "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
-           "--mst", "--mst-smooth", "--strength-map")
+           "--mst", "--mst-smooth", "--strength-map", "--efdm")
 # flags that do not combine with --interp-styles
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat"),
                     ("swap_targets", "--swap-targets")]
@@ -105,6 +108,7 @@ def parse_args(argv=None):
         parser.error("--temporal must be in [0, 1), got %g" % args.temporal)
     stylize.check_seamless_flags(parser, args)
     stylize.check_mst_flags(parser, args)
+    stylize.check_efdm_flags(parser, args)
     if args.strength_map is not None:
         for attr, flag in [("interp_styles", "--interp-styles"), ("swap5", "--swap5"), ("swap_targets", "--swap-targets"),
                            ("mst", "--mst")]:
@@ -161,8 +165,10 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
 
     temporal_kw = {} if temporal is None else dict(temporal=temporal)
-    # --ost, --seamless and --mst, on both paths
+    # --ost, --seamless, --mst and --efdm, on both paths
     opt_kw = dict(ost=True) if getattr(args, "ost", False) else {}
+    if getattr(args, "efdm", False):
+        opt_kw["efdm"] = True
     if getattr(args, "seamless", None):
         opt_kw["seamless"] = args.seamless
     if getattr(args, "mst", None) is not None:

@@ -101,6 +101,11 @@ SIGNATURES = {
     "wctb200_mst_style_clusters": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "wctb200_mst_data_term": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "wctb200_mst_smooth": (_i, [_vp, _i, _i, _i, _i, _f, _i, _vp, _vp]),
+    "wctb200_efdm_style_state_bytes": (_sz, [_i, _i, _i, _i]),
+    "wctb200_efdm_style_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "wctb200_efdm_style_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "wctb200_efdm_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "wctb200_efdm_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _f, _vp, _vp, _sz, _vp]),
     "wctb200_mask_feather": (_i, [_vp, _i, _i, _i, _i, _f, _vp, _vp]),
     "wctb200_weights_resize_area": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "wctb200_wct_stats_weighted": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp]),

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libwctb200.so")
 SOURCES = ["capi.cu", "layers.cu", "conv_tc.cu", "cov_tc.cu", "wct.cu", "image_ops.cu", "conv_tail_tc.cu", "conv_head_tc.cu", "matfun_tc.cu",
-           "flow.cu", "mst.cu"]
+           "flow.cu", "mst.cu", "efdm.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 NVCC_FLAGS += os.environ.get("WCTB_NVCC_EXTRA", "").split()      # experiments, e.g. -DWCTB_MBAR_TEST_WAIT

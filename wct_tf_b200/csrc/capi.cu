@@ -179,6 +179,13 @@ int launch_mst_style_clusters(const __half* style, int Hs, int Ws, int C, int K,
 int launch_mst_data_term(const __half* act, int N, int H, int W, int C, const float* centres, const int32_t* counts, int K, float* D,
                          cudaStream_t st);
 int launch_mst_smooth(const float* D, int N, int H, int W, int K, float lambda, int sweeps, uint8_t* labels, cudaStream_t st);
+size_t efdm_style_state_bytes(int C, int Ns, int Hs, int Ws);
+size_t efdm_style_workspace_bytes(int C, int Ns, int Hs, int Ws, int max_segments);
+size_t efdm_workspace_bytes(int C, int N, int H, int W, int max_segments);
+int launch_efdm_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, float* state, void* ws, size_t ws_bytes,
+                              cudaStream_t st);
+int launch_efdm_apply(const __half* content, int N, int H, int W, int C, const float* state, int Ns, int Hs, int Ws, float alpha,
+                      __half* out, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws);
 int launch_wct_style_prepare_regions(const __half*, int, int, int, const uint8_t*, int, float, float, float, void*, int32_t*, void*,
                                      size_t, cudaStream_t);
@@ -507,6 +514,39 @@ int wctb200_mst_smooth(const float* D, int N, int H, int W, int K, float lambda,
                      sweeps <= 1024 && lambda >= 0.f && lambda <= FLT_MAX,
                  "mst_smooth: bad arguments N=%d %dx%d K=%d lambda=%g sweeps=%d", N, H, W, K, (double)lambda, sweeps);
     return launch_mst_smooth(D, N, H, W, K, lambda, sweeps, labels_out, ST(stream));
+}
+// exact feature distribution matching (efdm.cu).  A style map may be 1x1 (only its interior is read); the content is an
+// activation of at least 2x2, which its reflect halo needs.
+static bool efdm_style_ok(int Ns, int Hs, int Ws, int C) {
+    return Ns >= 1 && Hs >= 1 && Ws >= 1 && C >= 8 && C % 8 == 0 && (long long)Hs * Ws < (1ll << 31) &&
+           (long long)Ns * (Hs + 2) * (Ws + 2) * (C / 8) < (1ll << 32);
+}
+size_t wctb200_efdm_style_state_bytes(int C, int Ns, int Hs, int Ws) {
+    if (!efdm_style_ok(Ns, Hs, Ws, C)) return 0;
+    return efdm_style_state_bytes(C, Ns, Hs, Ws);
+}
+size_t wctb200_efdm_style_workspace_bytes(int C, int Ns, int Hs, int Ws, int max_segments) {
+    if (!efdm_style_ok(Ns, Hs, Ws, C) || max_segments < 1) return 0;
+    return efdm_style_workspace_bytes(C, Ns, Hs, Ws, max_segments);
+}
+int wctb200_efdm_style_prepare(const void* style, int Ns, int Hs, int Ws, int C, void* state, void* ws, size_t ws_bytes,
+                               void* stream) {
+    WCTB_REQUIRE(style && state && ws, "efdm_style_prepare: null pointer");
+    WCTB_REQUIRE(efdm_style_ok(Ns, Hs, Ws, C), "efdm_style_prepare: bad geometry Ns=%d %dx%d C=%d", Ns, Hs, Ws, C);
+    return launch_efdm_style_prepare(HCP(style), Ns, Hs, Ws, C, static_cast<float*>(state), ws, ws_bytes, ST(stream));
+}
+size_t wctb200_efdm_workspace_bytes(int C, int N, int H, int W, int max_segments) {
+    if (!geom_ok(N, H, W, C) || max_segments < 1) return 0;
+    return efdm_workspace_bytes(C, N, H, W, max_segments);
+}
+int wctb200_efdm_apply(const void* content, int N, int H, int W, int C, const void* state, int Ns, int Hs, int Ws, float alpha,
+                       void* out, void* ws, size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(content && state && out && (ws || alpha == 0.f), "efdm_apply: null pointer");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && efdm_style_ok(Ns, Hs, Ws, C) && (Ns == 1 || Ns == N),
+                 "efdm_apply: bad geometry N=%d %dx%d C=%d, Ns=%d %dx%d (Ns in {1, N})", N, H, W, C, Ns, Hs, Ws);
+    WCTB_REQUIRE(alpha >= -FLT_MAX && alpha <= FLT_MAX, "efdm_apply: alpha must be finite");
+    return launch_efdm_apply(HCP(content), N, H, W, C, static_cast<const float*>(state), Ns, Hs, Ws, alpha, HP(out), ws, ws_bytes,
+                             ST(stream));
 }
 int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, void* stream) {
     WCTB_REQUIRE(src && dst, "labels_resize_nearest: null pointer");

@@ -30,6 +30,11 @@ SWAP_WORKSPACE_BYTES = 1 << 30
 # Multimodal style transfer (DESIGN.md §3.3.10): red-black ICM sweeps of the content labelling per level
 MST_SWEEPS = 8
 
+# Exact feature distribution matching (DESIGN.md §3.3.12): device scratch of one level's sort, in bytes.  The apply sorts
+# as many whole (frame, channel) segments at a time as this holds (24 bytes a value, so 2 GB is 85 M values: the relu1_1
+# level of 5 frames at 512^2, or a quarter of one 4096^2 frame); the bytes do not depend on it.
+EFDM_WORKSPACE_BYTES = 2 << 30
+
 
 class Act(object):
     """SPF16 activation: device buffer + logical NHWC shape."""
@@ -669,6 +674,42 @@ class Engine(object):
             ps.record_stream(main)
         return out
 
+    # ------------------------------------------------------------------ exact feature distribution matching (§3.3.12)
+    def _efdm_chunk(self, total, per_seg_fn):
+        """(segments per chunk, chunks) of an EFDM sort of ``total`` segments within EFDM_WORKSPACE_BYTES."""
+        per_seg = per_seg_fn(2) - per_seg_fn(1)
+        S = max(1, min(total, (EFDM_WORKSPACE_BYTES - per_seg_fn(1) + per_seg) // max(per_seg, 1)))
+        return S, -(-total // S)
+
+    def efdm_prepare(self, style):
+        """Style side of EFDM on one level: every channel's values, sorted (fp32 [n][C][Hs*Ws]).  Returns dict(state, H, W)."""
+        lib, C, n = self.lib, style.C, style.N
+        state = torch.empty(lib.wctb200_efdm_style_state_bytes(C, n, style.H, style.W), dtype=torch.uint8, device=self.device)
+        S, chunks = self._efdm_chunk(n * C, lambda k: lib.wctb200_efdm_style_workspace_bytes(C, n, style.H, style.W, k))
+        nbytes = lib.wctb200_efdm_style_workspace_bytes(C, n, style.H, style.W, S)
+        ws = self._grow_workspace(("efdm_style",), nbytes)
+        m = n * C * style.H * style.W
+        # the exact size of S segments (a grown buffer may be larger): the chunking, and so the launch count, is the one above
+        self._call("efdm_style[C%d]" % C, 14 * chunks, lib.wctb200_efdm_style_prepare, style.ptr, n, style.H, style.W, C,
+                   state.data_ptr(), ws.data_ptr(), nbytes, self._stream(), bytes_=84.0 * m)
+        return dict(state=state, H=style.H, W=style.W)
+
+    def efdm_apply(self, content, st, n_style, alpha):
+        """EFDM of one level against an ``efdm_prepare`` state of ``n_style`` in {1, N} styles."""
+        lib, C, N = self.lib, content.C, content.N
+        out = self._act(N, content.H, content.W, C)
+        m = N * C * content.H * content.W
+        if float(alpha) == 0.0:
+            chunks, ws_ptr, ws_n = 0, None, 0
+        else:
+            S, chunks = self._efdm_chunk(N * C, lambda k: lib.wctb200_efdm_workspace_bytes(C, N, content.H, content.W, k))
+            ws_n = lib.wctb200_efdm_workspace_bytes(C, N, content.H, content.W, S)
+            ws_ptr = self._grow_workspace(("efdm",), ws_n).data_ptr()
+        self._call("efdm_level[C%d]" % C, 18 * chunks if chunks else 1, lib.wctb200_efdm_apply, content.ptr, N, content.H,
+                   content.W, C, st["state"].data_ptr(), n_style, st["H"], st["W"], float(alpha), out.ptr, ws_ptr, ws_n,
+                   self._stream(), bytes_=(130.0 if chunks else 8.0) * m)
+        return out, None
+
     def _grow_workspace(self, key, nbytes):
         """Grow-only scratch per (group, key): the levels of a call differ in size."""
         key = (self._group,) + key
@@ -726,7 +767,7 @@ class Engine(object):
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
                 region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05, strength_map=None,
-                content_weights=None, mask_feather=None):
+                content_weights=None, mask_feather=None, efdm=False):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -782,8 +823,23 @@ class Engine(object):
         [1|N,K,Hm,Wm], weights >= 0 summing to <= 1 per pixel, with ``region_styles`` of K styles and no ``labels``) blends
         the K region transforms per pixel, each region's statistics weighted by its plane; ``mask_feather`` = sigma (with
         ``labels``) turns the label map into Gaussian-feathered weights.  Maps of any resolution are area-averaged to each
-        level.  WCT only for weights; not with interpolation, the style swap or ``mst``."""
+        level.  WCT only for weights; not with interpolation, the style swap or ``mst``.
+
+        Exact feature distribution matching (DESIGN.md §3.3.12): ``efdm=True`` gives every channel of each level the value
+        distribution of the same channel of the style, by rank (ties take the mean of their ranks' style values), instead
+        of WCT; swap levels still swap.  ``style_u8`` is one style or one per frame.  Not with ``adain``, ``ost``, ``mst``,
+        spatial control, interpolation or the soft maps; a ``PreparedStyle`` only as made by ``prepare_call(efdm=True)``."""
         N = content_u8.shape[0]
+        if efdm:
+            if (adain or ost or mst is not None or labels is not None or region_masks is not None or interp_styles is not None
+                    or strength_map is not None or content_weights is not None or mask_feather is not None):
+                raise ValueError("efdm does not combine with adain, ost, mst, labels / region_masks, interp_styles or "
+                                 "strength_map / content_weights / mask_feather")
+            if isinstance(style_u8, PreparedStyle):
+                skip = self.swap_levels(swap5, swap_targets)
+                if any(relu not in style_u8.efdm and relu not in skip for relu in self.model.style_taps):
+                    raise ValueError("efdm sorts the style's features at every level, which a prepared style does not keep: "
+                                     "give the style image")
         soft = None
         if strength_map is not None or content_weights is not None or mask_feather is not None:
             if mst is not None or interp_styles is not None or swap5 or swap_targets is not None:
@@ -880,14 +936,14 @@ class Engine(object):
         n_style = style_u8.n if prepared else style_u8.shape[0]
         if n_style not in (1, N):
             raise ValueError("%d styles for %d frames: give one style, or one per frame" % (n_style, N))
-        if prepared:
+        if prepared and not efdm:
             self.check_prepared(style_u8, adain, swap_lv)
         main = torch.cuda.current_stream(self.device)
         if swap_lv and n_style > 1:
             # one style per frame: frame by frame (each frame's swap has its own style side)
             outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
                                  alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
-                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost) for i in range(N)]
+                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm) for i in range(N)]
             return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
         swap = (int(ss_patch_size), int(ss_stride), swap_lv) if swap_lv else None
@@ -898,7 +954,8 @@ class Engine(object):
             # sub-batch group waits for the per-level events
             self._group = 1 if G > 1 else 0
             try:
-                owned = shared = self._style_side(style_u8, main, wct=not adain, adain=adain, keep=swap_lv, skip=swap_lv)
+                owned = shared = self._style_side(style_u8, main, wct=not adain and not efdm, adain=adain, keep=swap_lv, skip=swap_lv,
+                                                  efdm=efdm)
             finally:
                 self._group = 0
         for relu in swap_lv:
@@ -910,11 +967,11 @@ class Engine(object):
                 else:
                     sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
                 return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
-                                         seamless=seamless, soft=_soft_slice(soft, lo, hi))
+                                         seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm)
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
-                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft)
+                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft, efdm=efdm)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -1042,7 +1099,7 @@ class Engine(object):
             self._style_streams[self._group] = torch.cuda.Stream(device=self.device, priority=prio)
         return self._style_streams[self._group]
 
-    def _style_side(self, style_u8, main, wct=True, adain=False, keep=(), skip=(), labels=None, R=0, mst=0):
+    def _style_side(self, style_u8, main, wct=True, adain=False, keep=(), skip=(), labels=None, R=0, mst=0, efdm=False):
         """The prepare step: style side of one call (model.py:70-72: ONE encoder pass emitting every target; per level the
         WCT state of ops.py:48-55,76 when ``wct``, the AdaIN moments when ``adain``; levels in ``skip`` get neither), enqueued
         on this group's style stream when overlap is on.  ``keep`` lists the levels whose feature it keeps (the style
@@ -1055,7 +1112,10 @@ class Engine(object):
 
         With ``mst`` = K (one style image) each level's style feature is clustered (``mst_clusters``) and its WCT state is
         the masked prepare of the K clusters under the style's own labels: a prepared style of n = K with ``entries`` as
-        above, and the labels, centres and info of every level in ``mst``."""
+        above, and the labels, centres and info of every level in ``mst``.
+
+        With ``efdm`` every level also gets its EFDM state (``efdm_prepare``: the style's values sorted per channel) in
+        ``efdm``."""
         lib = self.lib
         side = self._style_stream() or main
         if side is not main:
@@ -1095,6 +1155,8 @@ class Engine(object):
                         ps.wct[relu] = self.style_prepare(feats[relu])
                     if adain:
                         ps.adain[relu] = self.adain_prepare(feats[relu])
+                    if efdm:
+                        ps.efdm[relu] = self.efdm_prepare(feats[relu])
                 ev = torch.cuda.Event()
                 ev.record(side)
                 ps.events[relu] = ev
@@ -1114,11 +1176,12 @@ class Engine(object):
         ps.record_stream(main)
         return ps
 
-    def prepare_call(self, style_u8, adain=False, swap5=False, swap_targets=None):
-        """The style side one call needs (WCT states, or the AdaIN moments; the features of the swap levels of ``swap5`` /
-        ``swap_targets``), made once for a call that applies it several times (passes)."""
+    def prepare_call(self, style_u8, adain=False, swap5=False, swap_targets=None, efdm=False):
+        """The style side one call needs (WCT states, the AdaIN moments, or the EFDM states; the features of the swap levels
+        of ``swap5`` / ``swap_targets``), made once for a call that applies it several times (passes)."""
         main = torch.cuda.current_stream(self.device)
-        ps = self._style_side(style_u8, main, wct=not adain, adain=adain, keep=self.swap_levels(swap5, swap_targets))
+        ps = self._style_side(style_u8, main, wct=not adain and not efdm, adain=adain, keep=self.swap_levels(swap5, swap_targets),
+                              efdm=efdm)
         style_u8.record_stream(ps.side)
         return ps
 
@@ -1162,6 +1225,9 @@ class Engine(object):
             out.wct[relu] = slice_wct_state(self.lib, st, RELU_CHANNELS[relu], ps.n, lo, hi)
         for relu, st in ps.adain.items():
             out.adain[relu] = slice_adain_state(self.lib, st, RELU_CHANNELS[relu], ps.n, lo, hi)
+        for relu, st in ps.efdm.items():
+            per = RELU_CHANNELS[relu] * st["H"] * st["W"] * 4          # the sorted values of one style
+            out.efdm[relu] = dict(st, state=st["state"][lo * per:hi * per].clone())
         for relu, f in ps.feats.items():
             out.feats[relu] = self._act(hi - lo, f.H, f.W, f.C)
             slice_act_planes(f.buf, f.N, f.H, f.W, f.C, lo, hi, out.feats[relu].buf)
@@ -1189,10 +1255,11 @@ class Engine(object):
         return ps.swap[key]
 
     def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
-                     seamless=None, soft=None):
+                     seamless=None, soft=None, efdm=False):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
         ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
-        optimal-transport transform instead of WCT at the other levels; ``seamless``: the wrapped axes of the content path
+        optimal-transport transform instead of WCT at the other levels, ``efdm`` exact feature distribution matching;
+        ``seamless``: the wrapped axes of the content path
         (the transforms write a reflect halo, which is rewritten before the decoder reads it)."""
         wrap = self.wrap_flags(seamless)
         lib, st = self.lib, self._stream()
@@ -1203,7 +1270,7 @@ class Engine(object):
             assert content_u8.dtype == torch.uint8
             if not isinstance(style, PreparedStyle):
                 assert style.dtype == torch.uint8 and style.shape[0] in (1, N)
-                owned = style = self._style_side(style, main, wct=not adain, adain=adain)
+                owned = style = self._style_side(style, main, wct=not adain and not efdm, adain=adain, efdm=efdm)
             n_style = style.n
             sides = [style]
         content = torch.empty(content_u8.shape, dtype=torch.float32, device=self.device)
@@ -1236,6 +1303,8 @@ class Engine(object):
                 elif multi is None:
                     if adain:
                         f, kbuf = self.adain_apply(cf, style.adain[relu], n_style, alpha)
+                    elif efdm:
+                        f, kbuf = self.efdm_apply(cf, style.efdm[relu], n_style, alpha)
                     elif ost:
                         f, kbuf = self.ost_apply(cf, style.wct[relu], n_style, alpha, want_info)
                     else:

@@ -24,7 +24,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``seamless`` is new: circular padding of every conv of the content path along x, y or both, for 360° panoramas and
     tileable textures;
   * ``mst`` is new: multimodal style transfer (Zhang, Zhu & Zhu, ICCV 2019), each level's style clustered into K modes
-    and every content pixel matched to one, so regions pair up without masks.
+    and every content pixel matched to one, so regions pair up without masks;
+  * ``efdm`` is new: exact feature distribution matching (Zhang et al., CVPR 2022), every channel's values given the
+    style's by rank.
 """
 from __future__ import annotations
 
@@ -265,7 +267,7 @@ class WCT(object):
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
                       swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
-                      strength_map=None, content_weights=None, mask_feather=None):
+                      strength_map=None, content_weights=None, mask_feather=None, efdm=False):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -346,7 +348,30 @@ class WCT(object):
         pixel blends the K transforms, the rest keeping the content.  ``mask_feather`` = sigma > 0 (with ``content_mask``):
         the label map feathered by a Gaussian of sigma mask pixels into such weights.  Weights work with WCT only; none of
         the three combines with ``style_weights``, ``swap5`` / ``swap_targets``, ``mst`` or ``tile_size``, and
-        ``content_weights`` not with ``content_mask``.  None for all three changes nothing."""
+        ``content_weights`` not with ``content_mask``.  None for all three changes nothing.
+
+        ``efdm`` (exact feature distribution matching, DESIGN.md §3.3.12): at every level each channel of each frame takes
+        the whole value distribution of the same channel of its style, not only its mean and variance or covariance: the
+        content values are ranked, value rank r takes the style's quantile at r, and equal values take the mean of their
+        ranks' quantiles.  Sparse bright strokes and an even wash with the same statistics then stylise differently.
+        ``efdm=False`` changes nothing.  Works with ``alpha``, ``passes`` (the style is sorted once per call), one style or
+        one per frame, sub-batch groups, ``return_float`` / ``return_device`` / ``out``, ``synthesize``, ``seamless``,
+        ``temporal`` and ``swap5`` / ``swap_targets`` (the swap levels swap in the first pass, the others use EFDM); not
+        with ``adain``, ``ost``, ``mst``, ``content_mask`` / ``style_masks`` / ``content_weights`` / ``mask_feather``,
+        ``strength_map``, ``style_weights``, ``tile_size`` (the ranks are over the whole image) or prepared styles (they
+        keep no sorted features)."""
+        if efdm:
+            bad = [name for name, on in (("adain", adain), ("ost", ost), ("mst", mst is not None),
+                                         ("content_mask", content_mask is not None), ("style_masks", style_masks is not None),
+                                         ("content_weights", content_weights is not None),
+                                         ("mask_feather", mask_feather is not None), ("strength_map", strength_map is not None),
+                                         ("style_weights", style_weights is not None),
+                                         ("tile_size", tile_size is not None and tile_size != 0)) if on]
+            if bad:
+                raise ValueError("efdm does not combine with %s" % ", ".join(bad))
+            if isinstance(styles, PreparedStyle):
+                raise ValueError("efdm sorts the style's features at every level, which a prepared style does not keep: "
+                                 "give the style image")
         soft = strength_map is not None or content_weights is not None or mask_feather is not None
         if soft:
             if (style_weights is not None or swap5 or swap_targets is not None or mst is not None
@@ -424,7 +449,7 @@ class WCT(object):
             if isinstance(a, PreparedStyle):
                 return a
             a = to_dev(a)
-            return eng.prepare_call(a, adain=adain, swap5=swap5, swap_targets=swap_targets) if int(passes) > 1 else a
+            return eng.prepare_call(a, adain=adain, swap5=swap5, swap_targets=swap_targets, efdm=efdm) if int(passes) > 1 else a
 
         # wct.py:84-90: with a stride the filter may not fit; centre-crop the content (on the device) to a size it tiles
         with torch.cuda.device(dev):
@@ -489,7 +514,8 @@ class WCT(object):
                     # whole batch in one call; with one style per frame the engine swaps frame by frame.
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
-                                       swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, **soft_kw)
+                                       swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, efdm=efdm,
+                                       **soft_kw)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -606,12 +632,13 @@ class WCT(object):
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
                 style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
-                strength_map=None, content_weights=None, mask_feather=None):
+                strength_map=None, content_weights=None, mask_feather=None, efdm=False):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
         blend.  ``tile_size`` stylises in tiles, ``ost`` uses the optimal-transport transform, ``seamless`` pads the content
-        path circularly and ``mst`` = K matches the content to K modes of the style; ``strength_map``, ``content_weights``
+        path circularly, ``mst`` = K matches the content to K modes of the style and ``efdm`` matches every channel's whole
+        value distribution to the style's; ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
         (``predict_batch``).'''
         soft = {k: v for k, v in (("strength_map", strength_map), ("content_weights", content_weights),
@@ -632,6 +659,8 @@ class WCT(object):
             raise ValueError("ost does not combine with adain, content_mask, style_masks or style_weights")
         if mst is not None and (style_weights is not None or content_mask is not None):
             raise ValueError("mst does not combine with content_mask, style_masks or style_weights")
+        if efdm and (style_weights is not None or content_mask is not None or content_weights is not None):
+            raise ValueError("efdm does not combine with content_mask, style_masks, content_weights or style_weights")
         if style_weights is not None:
             out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
                                      swap5=swap5, style_weights=style_weights, content_mask=content_mask,
@@ -651,6 +680,8 @@ class WCT(object):
                 kw["seamless"] = seamless
             if mst is not None:
                 kw.update(mst=mst, mst_smooth=mst_smooth)
+            if efdm:
+                kw["efdm"] = True
             kw.update(soft)
             out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
         if self.verbose:
