@@ -27,31 +27,29 @@ content, pass and noise batch.  A run's styles are all prepared or all images, a
 ``--crop-size`` or ``--keep-colors`` (their size and crop were fixed when they were prepared).
 
 Tiled stylisation: ``--tile-size T`` (a multiple of 16; 0: off) runs every level on T x T tiles widened by a halo, so device
-memory follows the tile and not the image, with each level's statistics taken over the whole image (DESIGN.md §3.3.7).  Not
-with ``--content-mask``, ``--interp-styles``, ``--swap5`` or ``--swap-targets``; ``--keep-colors``, ``--concat``,
-``--content-size``, ``--passes`` and ``--noise`` work on the whole image as without it.
+memory follows the tile and not the image, with each level's statistics taken over the whole image (DESIGN.md §3.3.7).
+``--keep-colors``, ``--concat``, ``--content-size``, ``--passes`` and ``--noise`` work on the whole image as without it.
 
 Optimal-transport transform: ``--ost`` maps each level's content feature Gaussian onto the style's by the Monge map, the
 covariance-matching map that moves the features least, instead of WCT (DESIGN.md §3.3.8); it keeps more of the content's
-structure at the same ``--alpha``.  Output names are unchanged.  Not with ``--adain``, ``--content-mask`` or
-``--interp-styles``.
+structure at the same ``--alpha``.  Output names are unchanged.
 
 Seamless stylisation: ``--seamless {x,y,xy}`` pads every conv of the content path circularly along those axes (DESIGN.md
 §3.3.9), so the result's opposite edges meet: ``x`` for 360° equirectangular panoramas, ``xy`` for tileable textures
 (``--noise --seamless xy``).  Each wrapped side must be a multiple of 2^P, P the pools up to the deepest relu target (16
-for relu5_1).  Output names are unchanged.  Not with ``--swap5`` or ``--swap-targets``.
+for relu5_1).  Output names are unchanged.
 
 Multimodal style transfer: ``--mst K [--mst-smooth LAMBDA]`` clusters each level's style features into K (1..8) modes and
 matches every content pixel to the mode it resembles, with a Potts smoothness of weight LAMBDA (default 0.05), so regions
-of the content pair up with modes of the painting without masks (DESIGN.md §3.3.10).  Output names are unchanged.  Not with
-``--adain``, ``--ost``, ``--content-mask``, ``--interp-styles``, ``--swap5``, ``--swap-targets``, ``--tile-size``,
-``--seamless`` or prepared styles (``.wctstyle``).
+of the content pair up with modes of the painting without masks (DESIGN.md §3.3.10).  Output names are unchanged.
 
 Exact feature distribution matching: ``--efdm`` gives every channel of each level the whole value distribution of the same
 channel of the style, by rank, instead of matching only its covariance (DESIGN.md §3.3.12): sparse bright strokes and an
 even wash with the same statistics stylise differently.  It suits ``--noise`` texture synthesis.  Output names are
-unchanged.  Not with ``--adain``, ``--ost``, ``--mst``, ``--content-mask``, ``--mask-weights``, ``--mask-feather``,
-``--strength-map``, ``--interp-styles``, ``--tile-size`` or prepared styles (``.wctstyle``).
+unchanged.
+
+Which of these options combine is decided by one table, ``wct_tf_b200/options.py``; a rejected combination is a parser error
+naming both flags.
 
 ``--checkpoints`` are TF1 checkpoint directories or ``.npz`` bundles, ``--vgg-path`` a Torch7 ``.t7`` or ``.npz`` file
 (wct_tf_b200.weights.load_weights); ``--synthetic-weights SEED`` runs with seeded random weights when the published
@@ -126,12 +124,8 @@ _FLAGS = [
 ]
 _NOISE_DEFAULTS = [("noise_size", [512, 512]), ("noise_count", 1), ("noise_seed", 0)]
 
-# flags that do not combine with --content-mask
-_MASK_EXCLUDES = [("style_path", "--style-path"), ("adain", "--adain"), ("swap5", "--swap5"), ("concat", "--concat"),
-                  ("random", "-r/--random"), ("swap_targets", "--swap-targets")]
-# flags that do not combine with --interp-styles
-_INTERP_EXCLUDES = [("style_path", "--style-path"), ("random", "-r/--random"), ("swap5", "--swap5"), ("concat", "--concat"),
-                    ("content_mask", "--content-mask"), ("swap_targets", "--swap-targets")]
+# flags of the one-style mode that the multi-style modes (--content-mask / --mask-weights, --interp-styles) take no part of
+_MULTI_EXCLUDES = [("style_path", "--style-path"), ("random", "-r/--random"), ("concat", "--concat")]
 
 
 def build_parser():
@@ -146,22 +140,22 @@ def parse_args(argv=None):
     args = parser.parse_args(argv)
     check_swap_flags(parser, args)
     check_interp_flags(parser, args)
-    check_tile_flags(parser, args)
-    check_ost_flags(parser, args)
-    check_seamless_flags(parser, args)
-    check_mst_flags(parser, args)
-    check_efdm_flags(parser, args)
+    check_values(parser, args)
+    check_options(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
-        if len(args.mask_styles) > 8:
-            parser.error("--mask-styles takes at most 8 styles")
-        for attr, flag in _MASK_EXCLUDES:
-            if getattr(args, attr):
-                parser.error("--content-mask does not combine with %s" % flag)
-    elif args.mask_styles and not args.mask_weights:
+    elif args.mask_weights is not None:
+        if not args.mask_styles or len(args.mask_weights) != len(args.mask_styles):
+            parser.error("--mask-weights needs one map per --mask-styles entry")
+    elif args.mask_styles:
         parser.error("--mask-styles needs --content-mask")
-    check_soft_flags(parser, args)
+    if args.mask_styles and len(args.mask_styles) > 8:
+        parser.error("--mask-styles takes at most 8 styles")
+    mode = "--content-mask" if args.content_mask is not None else "--mask-weights" if args.mask_weights is not None else None
+    for attr, flag in _MULTI_EXCLUDES if mode else []:
+        if getattr(args, attr):
+            parser.error("%s takes no %s" % (mode, flag))
     check_style_mask_flags(parser, args)
     check_noise_flags(parser, args)
     check_prepared_flags(parser, args)
@@ -173,42 +167,53 @@ def check_swap_flags(parser, args):
     if args.swap_targets is None:
         return
     if args.swap5:
-        parser.error("--swap-targets does not combine with --swap5 (--swap5 is --swap-targets relu5_1)")
+        parser.error("give --swap5 or --swap-targets, not both (--swap5 is --swap-targets relu5_1)")
     for relu in args.swap_targets:
         if relu not in (args.relu_targets or []):
             parser.error("--swap-targets: %s is not one of --relu-targets (%s)" % (relu, " ".join(args.relu_targets or [])))
 
 
-# flags that do not combine with soft spatial control (--strength-map, --mask-feather, --mask-weights)
-_SOFT_EXCLUDES = [("interp_styles", "--interp-styles"), ("swap5", "--swap5"), ("swap_targets", "--swap-targets"),
-                  ("mst", "--mst"), ("tile_size", "--tile-size")]
+MST_SMOOTH_DEFAULT = 0.05
 
 
-def check_soft_flags(parser, args):
-    """--strength-map, --mask-feather SIGMA (finite, > 0, with --content-mask) and --mask-weights (one map per
-    --mask-styles entry, in place of --content-mask; WCT only): not with blends, the swap, MST or tiles."""
-    soft = [f for a, f in (("strength_map", "--strength-map"), ("mask_feather", "--mask-feather"),
-                           ("mask_weights", "--mask-weights")) if getattr(args, a, None) is not None]
-    if not soft:
-        return
-    for attr, flag in _SOFT_EXCLUDES:
-        if getattr(args, attr, None):
-            parser.error("%s does not combine with %s" % (soft[0], flag))
-    if getattr(args, "mask_feather", None) is not None:
-        if args.content_mask is None:
-            parser.error("--mask-feather needs --content-mask")
-        if not np.isfinite(args.mask_feather) or not 0 < args.mask_feather <= 1024:
-            parser.error("--mask-feather must be a finite sigma in (0, 1024], got %g" % args.mask_feather)
-    if getattr(args, "mask_weights", None) is not None:
-        if args.content_mask is not None:
-            parser.error("--mask-weights replaces --content-mask: give one of them")
-        if not args.mask_styles or len(args.mask_weights) != len(args.mask_styles):
-            parser.error("--mask-weights needs one map per --mask-styles entry")
-        if len(args.mask_styles) > 8:
-            parser.error("--mask-styles takes at most 8 styles")
-        for attr, flag in _MASK_EXCLUDES + [("ost", "--ost")]:
-            if getattr(args, attr, None):
-                parser.error("--mask-weights does not combine with %s" % flag)
+def check_values(parser, args):
+    """The values of --tile-size (0: off), --mst / --mst-smooth (which needs --mst and defaults to 0.05 here),
+    --mask-feather and --temporal (stylize_video.py), as wct_tf_b200/options.py checks them."""
+    from wct_tf_b200 import options
+    try:
+        if getattr(args, "tile_size", 0):
+            options.check_tile_size(args.tile_size, "--tile-size")
+        if args.mst is None and args.mst_smooth is not None:
+            raise ValueError("--mst-smooth needs --mst")
+        if args.mst is not None:
+            if args.mst_smooth is None:
+                args.mst_smooth = MST_SMOOTH_DEFAULT
+            options.check_mst(args.mst, args.mst_smooth, ("--mst", "--mst-smooth"))
+        if getattr(args, "mask_feather", None) is not None:
+            options.check_mask_feather(args.mask_feather, "--mask-feather")
+        if hasattr(args, "temporal"):
+            options.check_temporal_strength(args.temporal, "--temporal")
+    except ValueError as e:
+        parser.error(str(e))
+
+
+def check_options(parser, args):
+    """The combinations of the stylising flags that wct_tf_b200/options.py rejects, as parser errors naming both flags."""
+    from wct_tf_b200 import options
+    style_path = getattr(args, "style_path", None)
+    on = dict(adain=args.adain, ost=args.ost, efdm=args.efdm, mst=args.mst is not None,
+              swap=args.swap5 or args.swap_targets is not None, content_mask=getattr(args, "content_mask", None) is not None,
+              style_masks=getattr(args, "style_masks", None) is not None, style_weights=args.interp_styles is not None,
+              content_weights=getattr(args, "mask_weights", None) is not None,
+              mask_feather=getattr(args, "mask_feather", None) is not None, strength_map=args.strength_map is not None,
+              tile_size=bool(getattr(args, "tile_size", 0)), seamless=args.seamless is not None,
+              temporal=bool(getattr(args, "temporal", 0)),
+              prepared=bool(style_path) and (is_prepared(style_path) or (os.path.isdir(style_path)
+                                                                         and any(is_prepared(f) for f in os.listdir(style_path)))))
+    try:
+        options.check({name for name, v in on.items() if v}, options.CLI)
+    except ValueError as e:
+        parser.error(str(e))
 
 
 def read_grey(path):
@@ -229,87 +234,6 @@ def soft_kw(args):
     return kw
 
 
-def check_ost_flags(parser, args):
-    """--ost: a transform of the WCT style states; not with --adain, --content-mask or --interp-styles."""
-    if not getattr(args, "ost", False):
-        return
-    for attr, flag in [("adain", "--adain"), ("content_mask", "--content-mask"), ("interp_styles", "--interp-styles")]:
-        if getattr(args, attr, None):
-            parser.error("--ost does not combine with %s" % flag)
-
-
-def check_seamless_flags(parser, args):
-    """--seamless: not with the style swap (--swap5, --swap-targets), whose VALID patches are not periodic, or with
-    temporal stabilisation (stylize_video.py --temporal), whose optical flow does not see across the seam."""
-    if getattr(args, "seamless", None) is None:
-        return
-    for attr, flag in [("swap5", "--swap5"), ("swap_targets", "--swap-targets"), ("temporal", "--temporal")]:
-        if getattr(args, attr, None):
-            parser.error("--seamless does not combine with %s" % flag)
-
-
-MST_SMOOTH_DEFAULT = 0.05
-# flags that do not combine with --mst (stylize.py and stylize_video.py)
-_MST_EXCLUDES = [("adain", "--adain"), ("ost", "--ost"), ("content_mask", "--content-mask"), ("style_masks", "--style-masks"),
-                 ("interp_styles", "--interp-styles"), ("swap5", "--swap5"), ("swap_targets", "--swap-targets"),
-                 ("tile_size", "--tile-size"), ("seamless", "--seamless")]
-
-
-def check_mst_flags(parser, args):
-    """--mst K: 1..8 clusters; --mst-smooth (finite, >= 0) needs it and defaults to 0.05 here.  Not with the other
-    transforms, masks, blends, the swap, tiles, seamless or prepared styles (which keep no per-level features to cluster)."""
-    if getattr(args, "mst", None) is None:
-        if getattr(args, "mst_smooth", None) is not None:
-            parser.error("--mst-smooth needs --mst")
-        return
-    if not 1 <= args.mst <= 8:
-        parser.error("--mst takes 1..8 clusters, got %d" % args.mst)
-    if args.mst_smooth is None:
-        args.mst_smooth = MST_SMOOTH_DEFAULT
-    if not np.isfinite(args.mst_smooth) or args.mst_smooth < 0:
-        parser.error("--mst-smooth must be finite and >= 0, got %g" % args.mst_smooth)
-    for attr, flag in _MST_EXCLUDES:
-        if getattr(args, attr, None):
-            parser.error("--mst does not combine with %s" % flag)
-    style_path = getattr(args, "style_path", None)
-    if style_path and (is_prepared(style_path) or (os.path.isdir(style_path)
-                                                   and any(is_prepared(f) for f in os.listdir(style_path)))):
-        parser.error("--mst does not combine with prepared styles (.wctstyle)")
-
-
-# flags that do not combine with --efdm (stylize.py and stylize_video.py)
-_EFDM_EXCLUDES = [("adain", "--adain"), ("ost", "--ost"), ("mst", "--mst"), ("content_mask", "--content-mask"),
-                  ("style_masks", "--style-masks"), ("mask_weights", "--mask-weights"), ("mask_feather", "--mask-feather"),
-                  ("strength_map", "--strength-map"), ("interp_styles", "--interp-styles"), ("tile_size", "--tile-size")]
-
-
-def check_efdm_flags(parser, args):
-    """--efdm: a transform of its own, on whole images; not with the other transforms, masks, soft maps, blends, tiles
-    (ranks are taken over the whole image) or prepared styles (which keep no sorted features)."""
-    if not getattr(args, "efdm", False):
-        return
-    for attr, flag in _EFDM_EXCLUDES:
-        if getattr(args, attr, None):
-            parser.error("--efdm does not combine with %s" % flag)
-    style_path = getattr(args, "style_path", None)
-    if style_path and (is_prepared(style_path) or (os.path.isdir(style_path)
-                                                   and any(is_prepared(f) for f in os.listdir(style_path)))):
-        parser.error("--efdm does not combine with prepared styles (.wctstyle)")
-
-
-def check_tile_flags(parser, args):
-    """--tile-size: a multiple of 16 (0: off); not with the region, interpolation and swap modes, which take statistics
-    the tiled path does not accumulate."""
-    if args.tile_size == 0:
-        return
-    if args.tile_size < 0 or args.tile_size % 16:
-        parser.error("--tile-size must be a positive multiple of 16 (0: off), got %d" % args.tile_size)
-    for attr, flag in [("content_mask", "--content-mask"), ("interp_styles", "--interp-styles"), ("swap5", "--swap5"),
-                       ("swap_targets", "--swap-targets")]:
-        if getattr(args, attr):
-            parser.error("--tile-size does not combine with %s" % flag)
-
-
 def check_style_mask_flags(parser, args):
     """--style-masks: one mask per --mask-styles entry, with --content-mask; not with --crop-size (a crop moves the style
     off its mask) or prepared styles (they keep no feature maps to mask).  --style-size scales style and mask alike."""
@@ -321,9 +245,9 @@ def check_style_mask_flags(parser, args):
         parser.error("--style-masks needs one mask per --mask-styles entry (%d masks, %d styles)"
                      % (len(args.style_masks), len(args.mask_styles)))
     if args.crop_size:
-        parser.error("--style-masks does not combine with --crop-size")
+        parser.error("--style-masks takes no --crop-size")
     if any(is_prepared(p) for p in args.mask_styles):
-        parser.error("--style-masks does not combine with prepared styles (.wctstyle)")
+        parser.error("--style-masks takes no prepared styles (.wctstyle)")
 
 
 PREPARED_EXT = ".wctstyle"
@@ -356,7 +280,7 @@ def check_prepared_flags(parser, args, flags=("style_size", "crop_size", "keep_c
         parser.error("prepared styles (.wctstyle) and style images do not mix in one run")
     for attr in flags:
         if getattr(args, attr, None):
-            parser.error("prepared styles (.wctstyle) do not combine with --%s" % attr.replace("_", "-"))
+            parser.error("prepared styles (.wctstyle) take no --%s" % attr.replace("_", "-"))
 
 
 class PreparedStyles(object):
@@ -379,7 +303,7 @@ def check_noise_flags(parser, args):
                 parser.error("--%s needs --noise" % attr.replace("_", "-"))
         return
     if args.content_path is not None or args.content_size or args.keep_colors:
-        parser.error("--noise does not combine with --content-path, --content-size or --keep-colors")
+        parser.error("--noise takes no --content-path, --content-size or --keep-colors")
     for attr, default in _NOISE_DEFAULTS:
         if getattr(args, attr) is None:
             setattr(args, attr, default)
@@ -391,7 +315,7 @@ def check_noise_flags(parser, args):
         parser.error("--noise-seed must be in 0 .. 2^64-1")
 
 
-def check_interp_flags(parser, args, excludes=_INTERP_EXCLUDES):
+def check_interp_flags(parser, args, excludes=_MULTI_EXCLUDES):
     """--interp-styles / --interp-weights: each needs the other, one weight per style, 1..8 styles, valid weights."""
     if args.interp_styles is None and args.interp_weights is None:
         return
@@ -405,7 +329,7 @@ def check_interp_flags(parser, args, excludes=_INTERP_EXCLUDES):
         parser.error("--interp-styles takes at most 8 styles")
     for attr, flag in excludes:
         if getattr(args, attr, None):
-            parser.error("--interp-styles does not combine with %s" % flag)
+            parser.error("--interp-styles takes no %s" % flag)
     try:
         normalized_weights(args.interp_weights)
     except ValueError as e:

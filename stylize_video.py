@@ -19,17 +19,18 @@ DESIGN.md §3.3.6).  This reduces the flicker of frame-by-frame WCT.  Each (clip
 batches and through the frame-by-frame path, so ``--batch`` does not change a frame; ``--concat`` comes after it.
 
 Optimal-transport transform: ``--ost`` uses the Monge map between the feature Gaussians instead of WCT at every level
-(DESIGN.md §3.3.8), on the batched and the frame-by-frame path alike.  Not with ``--adain`` or ``--interp-styles``.
+(DESIGN.md §3.3.8), on the batched and the frame-by-frame path alike.
 
 Seamless stylisation: ``--seamless {x,y,xy}`` pads the content path circularly (DESIGN.md §3.3.9), e.g. ``x`` for 360°
-clips, on both paths.  Not with ``--temporal`` (the optical flow does not see across the seam), ``--swap5`` or
-``--swap-targets``.
+clips, on both paths.
 
 Multimodal style transfer: ``--mst K [--mst-smooth LAMBDA]`` matches the content to K modes of the style at every level
-(DESIGN.md §3.3.10), on both paths, with the same rejections as stylize.py; it combines with ``--temporal``.
+(DESIGN.md §3.3.10), on both paths.
 
 Exact feature distribution matching: ``--efdm`` gives every channel of each level the style's whole value distribution
-(DESIGN.md §3.3.12), on both paths, with the same rejections as stylize.py; it combines with ``--temporal`` and the swap.
+(DESIGN.md §3.3.12), on both paths.
+
+Which of these options combine is decided by one table, ``wct_tf_b200/options.py``, as for stylize.py.
 """
 from __future__ import division, print_function
 
@@ -64,9 +65,8 @@ _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
            "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
            "--mst", "--mst-smooth", "--strength-map", "--efdm")
-# flags that do not combine with --interp-styles
-_INTERP_EXCLUDES = [("style_path", "--style-path"), ("swap5", "--swap5"), ("concat", "--concat"),
-                    ("swap_targets", "--swap-targets")]
+# flags of the one-style mode that --interp-styles takes no part of
+_INTERP_EXCLUDES = [("style_path", "--style-path"), ("concat", "--concat")]
 
 
 def build_parser():
@@ -86,17 +86,16 @@ def parse_args(argv=None):
     parser = build_parser()
     args = parser.parse_args(argv)
     stylize.check_swap_flags(parser, args)
-    stylize.check_ost_flags(parser, args)
     if args.morph:
         if args.interp_styles is None:
             parser.error("--morph needs --interp-styles")
         if args.interp_weights is not None:
-            parser.error("--morph does not combine with --interp-weights")
+            parser.error("--morph takes no --interp-weights")
         if not 2 <= len(args.interp_styles) <= 8:
             parser.error("--morph needs 2..8 --interp-styles")
         for attr, flag in _INTERP_EXCLUDES:
             if getattr(args, attr):
-                parser.error("--interp-styles does not combine with %s" % flag)
+                parser.error("--interp-styles takes no %s" % flag)
     else:
         if args.interp_styles is not None and args.interp_weights is None:
             parser.error("--interp-styles needs --interp-weights or --morph")
@@ -104,16 +103,8 @@ def parse_args(argv=None):
     if args.interp_styles is None and args.style_path is None:
         parser.error("--style-path (or --interp-styles) is required")
     stylize.check_prepared_flags(parser, args)
-    if not 0.0 <= args.temporal < 1.0:
-        parser.error("--temporal must be in [0, 1), got %g" % args.temporal)
-    stylize.check_seamless_flags(parser, args)
-    stylize.check_mst_flags(parser, args)
-    stylize.check_efdm_flags(parser, args)
-    if args.strength_map is not None:
-        for attr, flag in [("interp_styles", "--interp-styles"), ("swap5", "--swap5"), ("swap_targets", "--swap-targets"),
-                           ("mst", "--mst")]:
-            if getattr(args, attr, None):
-                parser.error("--strength-map does not combine with %s" % flag)
+    stylize.check_values(parser, args)
+    stylize.check_options(parser, args)
     return args
 
 

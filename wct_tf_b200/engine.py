@@ -11,7 +11,7 @@ import ctypes
 import numpy as np
 import torch
 
-from . import _capi
+from . import _capi, options
 from .model import WCTModel, RELU_CHANNELS, RELU_LEVEL, check_seamless, seamless_axes
 from .prepared import (PreparedStyle, SEMANTIC_KEYS, encoder_fingerprints, slice_act_planes, slice_adain_state,
                        slice_wct_state)
@@ -592,18 +592,7 @@ class Engine(object):
         return out, None
 
     # ------------------------------------------------------------------ multimodal style transfer (DESIGN.md §3.3.10)
-    @staticmethod
-    def check_mst(K, lam):
-        """(K, lambda) of an MST call: K an integer in 1..8, lambda finite and >= 0; ValueError otherwise."""
-        if isinstance(K, bool) or not isinstance(K, (int, np.integer)) or not 1 <= K <= 8:
-            raise ValueError("mst must be a number of clusters in 1..8, got %r" % (K,))
-        try:
-            lam_f = float(lam)
-        except (TypeError, ValueError):
-            raise ValueError("mst_smooth must be a number, got %r" % (lam,))
-        if not np.isfinite(lam_f) or lam_f < 0:
-            raise ValueError("mst_smooth must be finite and >= 0, got %r" % (lam,))
-        return int(K), lam_f
+    check_mst = staticmethod(options.check_mst)                 # (K, lambda) of an MST call: options.check_mst
 
     def mst_clusters(self, style, K, level):
         """Spherical k-means of the style feature ``style`` (one style) into K clusters, seeded by the draws of ``level`` (0 for
@@ -781,10 +770,12 @@ class Engine(object):
         eigendecompositions are latency bound on a few SMs, so one group's Jacobi clusters overlap the
         other groups' convolutions (same arithmetic per frame; only the schedule changes).
 
+        Which of the options below combine is decided by one table, ``wct_tf_b200/options.py``.
+
         Spatial control: ``labels`` is a cuda uint8 label map [N|1,Hm,Wm] of any resolution and ``region_styles`` a list of
         R (1..8) cuda uint8 images [1,Hs,Ws,3] of any sizes, or prepared styles of one style each; ``style_u8`` is ignored.
-        At every level the map is resampled to the feature grid and region r of a frame is transformed against style r
-        (WCT only); labels >= R keep the content feature.  The R styles are encoded and prepared once per call.
+        At every level the map is resampled to the feature grid and region r of a frame is transformed against style r;
+        labels >= R keep the content feature.  The R styles are encoded and prepared once per call.
 
         Style masks: ``region_masks`` (with ``labels``) is a list of R entries, each None (the whole style r) or a cuda
         uint8 label map [Hm',Wm'] of style r, of any resolution.  Region r then takes the statistics of the pixels of style
@@ -799,58 +790,45 @@ class Engine(object):
         weights are used as given.  The K styles are encoded and prepared once per call.
 
         Style swap at any level: ``swap_targets`` is a list of relu targets at which the style swap replaces WCT / AdaIN,
-        with ``ss_alpha``, ``ss_patch_size`` and ``ss_stride``; ``swap5`` is ``swap_targets=["relu5_1"]``.  Not with spatial
-        control or interpolation.
+        with ``ss_alpha``, ``ss_patch_size`` and ``ss_stride``; ``swap5`` is ``swap_targets=["relu5_1"]``.
 
         Optimal-transport transform: ``ost=True`` matches each level's content Gaussian to the style's by the Monge map
-        (DESIGN.md §3.3.8) instead of WCT, against the same WCT style states; swap levels still swap.  Not with ``adain``,
-        spatial control (``labels``) or interpolation (``interp_styles``): the blend of states is exact for WCT and AdaIN
-        only because they are affine in the style statistics, and M is not.
+        (DESIGN.md §3.3.8) instead of WCT, against the same WCT style states; swap levels still swap.
 
         Seamless stylisation: ``seamless`` = "x", "y" or "xy" pads every conv of the content path circularly along those
         axes (DESIGN.md §3.3.9), so the output equals that of the infinitely tiled content and tiles without a seam.  Each
-        wrapped axis must be a multiple of 2^P (P pools up to the deepest target); not with the style swap, whose VALID
-        patches are not periodic.  The style side is unchanged.
+        wrapped axis must be a multiple of 2^P (P pools up to the deepest target).  The style side is unchanged.
 
         Multimodal style transfer: ``mst`` = K (1..8) clusters each level's style feature into K modes and labels every
         content pixel with the mode it resembles, smoothed by a Potts term of weight ``mst_smooth`` (DESIGN.md §3.3.10);
-        region k of each frame then takes the statistics of style mode k.  ``style_u8`` is one style image.  WCT only; not
-        with ``ost``, spatial control, interpolation, the style swap or ``seamless``.  K = 1 is the plain WCT call, byte for
-        byte.
+        region k of each frame then takes the statistics of style mode k.  ``style_u8`` is one style image.  K = 1 is the
+        plain WCT call, byte for byte.
 
         Soft spatial control (DESIGN.md §3.3.11): ``strength_map`` (cuda fp32 [1|N,Hm,Wm] in [0,1]) scales the stylisation
-        per pixel, out = s T(x) + (1 - s) x, with WCT, OST, AdaIN and hard masks; ``content_weights`` (cuda fp32
+        per pixel, out = s T(x) + (1 - s) x; ``content_weights`` (cuda fp32
         [1|N,K,Hm,Wm], weights >= 0 summing to <= 1 per pixel, with ``region_styles`` of K styles and no ``labels``) blends
         the K region transforms per pixel, each region's statistics weighted by its plane; ``mask_feather`` = sigma (with
         ``labels``) turns the label map into Gaussian-feathered weights.  Maps of any resolution are area-averaged to each
-        level.  WCT only for weights; not with interpolation, the style swap or ``mst``.
+        level.
 
         Exact feature distribution matching (DESIGN.md §3.3.12): ``efdm=True`` gives every channel of each level the value
         distribution of the same channel of the style, by rank (ties take the mean of their ranks' style values), instead
-        of WCT; swap levels still swap.  ``style_u8`` is one style or one per frame.  Not with ``adain``, ``ost``, ``mst``,
-        spatial control, interpolation or the soft maps; a ``PreparedStyle`` only as made by ``prepare_call(efdm=True)``."""
+        of WCT; swap levels still swap.  ``style_u8`` is one style or one per frame; a ``PreparedStyle`` only as made by
+        ``prepare_call(efdm=True)``."""
         N = content_u8.shape[0]
-        if efdm:
-            if (adain or ost or mst is not None or labels is not None or region_masks is not None or interp_styles is not None
-                    or strength_map is not None or content_weights is not None or mask_feather is not None):
-                raise ValueError("efdm does not combine with adain, ost, mst, labels / region_masks, interp_styles or "
-                                 "strength_map / content_weights / mask_feather")
-            if isinstance(style_u8, PreparedStyle):
-                skip = self.swap_levels(swap5, swap_targets)
-                if any(relu not in style_u8.efdm and relu not in skip for relu in self.model.style_taps):
-                    raise ValueError("efdm sorts the style's features at every level, which a prepared style does not keep: "
-                                     "give the style image")
+        options.check({name for name, on in (
+            ("adain", adain), ("ost", ost), ("efdm", efdm), ("mst", mst is not None), ("swap", swap5 or swap_targets is not None),
+            ("content_mask", labels is not None), ("style_masks", region_masks is not None),
+            ("style_weights", interp_styles is not None), ("content_weights", content_weights is not None),
+            ("mask_feather", mask_feather is not None), ("strength_map", strength_map is not None),
+            ("seamless", seamless is not None)) if on}, options.ENGINE)
+        if efdm and isinstance(style_u8, PreparedStyle):
+            skip = self.swap_levels(swap5, swap_targets)
+            if any(relu not in style_u8.efdm and relu not in skip for relu in self.model.style_taps):
+                raise ValueError("efdm sorts the style's features at every level, which a prepared style does not keep: "
+                                 "give the style image")
         soft = None
         if strength_map is not None or content_weights is not None or mask_feather is not None:
-            if mst is not None or interp_styles is not None or swap5 or swap_targets is not None:
-                raise ValueError("strength_map / content_weights / mask_feather do not combine with mst, interp_styles or "
-                                 "swap5 / swap_targets")
-            if content_weights is not None and labels is not None:
-                raise ValueError("content_weights replaces labels: give one of them")
-            if mask_feather is not None and labels is None:
-                raise ValueError("mask_feather needs labels")
-            if (content_weights is not None or mask_feather is not None) and (adain or ost):
-                raise ValueError("content_weights / mask_feather work with WCT only: not with adain or ost")
             sm = None
             if strength_map is not None:
                 sm = strength_map if strength_map.dim() == 3 else strength_map.unsqueeze(0)
@@ -867,9 +845,7 @@ class Engine(object):
                                      % self.device)
                 cw = cw.expand(N, -1, -1, -1).contiguous()
             elif mask_feather is not None:
-                sigma = float(mask_feather)
-                if not (np.isfinite(sigma) and 0.0 < sigma <= 1024.0):
-                    raise ValueError("mask_feather must be a finite sigma in (0, 1024] mask pixels, got %r" % (mask_feather,))
+                sigma = options.check_mask_feather(mask_feather)
                 R = len(region_styles) if region_styles is not None else 0
                 if not 1 <= R <= 8:
                     raise ValueError("spatial control needs 1..8 region styles, got %d" % R)
@@ -882,11 +858,7 @@ class Engine(object):
                 # soft weights take the place of the label map: a region call whose labels are never read
                 labels = torch.zeros((N, 1, 1), dtype=torch.uint8, device=self.device)
         if mst is not None:
-            K, lam = self.check_mst(mst, mst_smooth)
-            if (adain or ost or labels is not None or region_masks is not None or interp_styles is not None or swap5
-                    or swap_targets is not None or seamless is not None):
-                raise ValueError("mst works with WCT only: not with adain, ost, labels / region_masks, interp_styles, swap5 / "
-                                 "swap_targets or seamless")
+            K, lam = options.check_mst(mst, mst_smooth)
             if isinstance(style_u8, PreparedStyle):
                 if style_u8.mst_k != K or any(relu not in style_u8.mst for relu in self.model.style_taps):
                     raise ValueError("mst clusters the style's features at every level, which a prepared style does not keep: "
@@ -895,18 +867,9 @@ class Engine(object):
                 raise ValueError("mst takes one style for the whole batch, got %d" % style_u8.shape[0])
             return self._stylize_mst(content_u8, style_u8, K, lam, alpha, want_info, capture)
         if seamless is not None:
-            if swap5 or swap_targets is not None:
-                raise ValueError("seamless does not combine with swap5 / swap_targets: the swap's VALID patches are not periodic")
             check_seamless(seamless, content_u8.shape[1], content_u8.shape[2], self.model.relu_targets)
-        if ost and (adain or labels is not None or interp_styles is not None):
-            raise ValueError("ost works with WCT style states only: not with adain, labels (spatial control) or interp_styles")
         swap_lv = self.swap_levels(swap5, swap_targets)
-        swap5 = swap5 or swap_targets is not None         # the rejections below name both
-        if region_masks is not None and labels is None:
-            raise ValueError("style masks (region_masks) need a content label map (labels)")
         if interp_styles is not None:
-            if labels is not None or swap5:
-                raise ValueError("style interpolation does not combine with spatial control (labels) or swap5 / swap_targets")
             K = len(interp_styles)
             if not 1 <= K <= 8:
                 raise ValueError("style interpolation needs 1..8 styles, got %d" % K)
@@ -918,8 +881,6 @@ class Engine(object):
             return self._stylize_multi(content_u8, list(interp_styles), alpha, adain, want_info, capture,
                                        lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]), seamless=seamless)
         if labels is not None:
-            if adain or swap5:
-                raise ValueError("spatial control (labels) works with WCT only: not with adain or swap5 / swap_targets")
             R = len(region_styles) if region_styles is not None else 0
             if not 1 <= R <= 8:
                 raise ValueError("spatial control needs 1..8 region styles, got %d" % R)
@@ -1348,13 +1309,7 @@ class Engine(object):
         return x
 
     # ------------------------------------------------------------------ tiled stylisation (DESIGN.md §3.3.7)
-    @staticmethod
-    def check_tile_size(tile_size):
-        """The tile edge of a tiled call: a positive multiple of 16 (tile boundaries on the pooling grid of every level);
-        ValueError otherwise."""
-        if isinstance(tile_size, bool) or not isinstance(tile_size, (int, np.integer)) or tile_size <= 0 or tile_size % 16:
-            raise ValueError("tile_size must be a positive multiple of 16, got %r" % (tile_size,))
-        return int(tile_size)
+    check_tile_size = staticmethod(options.check_tile_size)     # the tile edge of a tiled call: options.check_tile_size
 
     def stats_record(self, C, adain):
         """A zeroed statistics record of one frame (n = 0: the empty record that the first accumulate fills)."""
@@ -1469,11 +1424,11 @@ class Engine(object):
         the whole image, so the result is the untiled one up to the order in which the statistics are summed, and byte
         for byte the same when one tile covers the image.  ``style_u8``: a cuda uint8 image batch or a ``PreparedStyle``
         of 1 or N styles.  The frames run one after another, each with its own statistics; the style side is untiled.
-        ``ost``: the optimal-transport transform (DESIGN.md §3.3.8) instead of WCT; not with ``adain``.  ``seamless``: as for
+        ``ost``: the optimal-transport transform (DESIGN.md §3.3.8) instead of WCT.  ``seamless``: as for
         ``stylize`` (``tiled_level``)."""
-        T = self.check_tile_size(tile_size)
-        if ost and adain:
-            raise ValueError("ost works with WCT style states only: not with adain")
+        T = options.check_tile_size(tile_size)
+        options.check({name for name, on in (("tile_size", True), ("adain", adain), ("ost", ost),
+                                             ("seamless", seamless is not None)) if on}, options.ENGINE)
         N = content_u8.shape[0]
         check_seamless(seamless, content_u8.shape[1], content_u8.shape[2], self.model.relu_targets)
         prepared = isinstance(style_u8, PreparedStyle)

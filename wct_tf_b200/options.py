@@ -1,0 +1,120 @@
+"""Which options of a stylising call combine, and the checks of their values.
+
+This is the one statement of that policy.  ``WCT.predict_batch``, ``Engine.stylize`` / ``stylize_tiled`` and the flags of
+``stylize.py`` / ``stylize_video.py`` each map their arguments to a set of the canonical option names below and call
+``check`` with their vocabulary, so that every caller accepts the same combinations and names them in its own words.
+"""
+import numpy as np
+
+# canonical option -> its spelling as a predict_batch keyword, an Engine.stylize keyword and a CLI flag (None: that caller
+# has no such option)
+SPELLINGS = {
+    "adain": ("adain", "adain", "--adain"),
+    "ost": ("ost", "ost", "--ost"),
+    "efdm": ("efdm", "efdm", "--efdm"),
+    "mst": ("mst", "mst", "--mst"),
+    "swap": ("swap5 / swap_targets", "swap5 / swap_targets", "--swap5 / --swap-targets"),
+    "content_mask": ("content_mask", "labels", "--content-mask"),
+    "style_masks": ("style_masks", "region_masks", "--style-masks"),
+    "style_weights": ("style_weights", "interp_styles", "--interp-styles"),
+    "content_weights": ("content_weights", "content_weights", "--mask-weights"),
+    "mask_feather": ("mask_feather", "mask_feather", "--mask-feather"),
+    "strength_map": ("strength_map", "strength_map", "--strength-map"),
+    "tile_size": ("tile_size", "tile_size", "--tile-size"),
+    "seamless": ("seamless", "seamless", "--seamless"),
+    "temporal": ("temporal", None, "--temporal"),
+    "return_float": ("return_float", None, None),
+    "prepared": ("a prepared style", None, "prepared styles (.wctstyle)"),
+    "per_frame_styles": ("one style per frame", None, None),
+}
+API, ENGINE, CLI = ({name: s[i] for name, s in SPELLINGS.items()} for i in range(3))
+
+_MASKS = ("content_mask", "style_masks", "content_weights", "mask_feather")
+
+# (option, the options it does not combine with, why); checked in this order
+EXCLUDES = [
+    ("efdm", ("adain", "ost", "mst"), "each level takes one transform"),
+    ("efdm", _MASKS + ("strength_map", "style_weights"), "the sorted-value map has no region, weighted or blended form"),
+    ("efdm", ("tile_size",), "the ranks are taken over the whole image"),
+    ("efdm", ("prepared",), "it sorts the style's features at every level, which a prepared style does not keep"),
+    ("content_weights", ("content_mask",), "the soft weights replace the label map; give one of them"),
+    ("strength_map", ("style_weights", "swap", "mst", "tile_size"),
+     "the per-pixel blend runs on untiled WCT, OST and AdaIN levels"),
+    ("content_weights", ("style_weights", "swap", "mst", "tile_size", "adain", "ost"),
+     "the weighted statistics and their blend are WCT's"),
+    ("mask_feather", ("style_weights", "swap", "mst", "tile_size", "adain", "ost"),
+     "feathering makes soft weights, whose statistics and blend are WCT's"),
+    ("mst", ("adain", "ost"), "AdaIN / OST per cluster is not defined"),
+    ("mst", ("content_mask", "style_masks", "style_weights"), "MST makes the regions itself"),
+    ("mst", ("swap",), "every level runs WCT per cluster"),
+    ("mst", ("tile_size",), "the clustering and the labelling need the whole level"),
+    ("mst", ("seamless",), "red-black smoothing on a wrapped ring of odd length is not an independent set"),
+    ("mst", ("prepared",), "it clusters the style's features at every level, which a prepared style does not keep"),
+    ("mst", ("per_frame_styles",), "the style is clustered once for every frame"),
+    ("seamless", ("swap",), "the swap's VALID patches are not periodic"),
+    ("seamless", ("temporal",), "the optical flow does not see across the seam"),
+    ("ost", ("adain",), "OST is a transform of the WCT style states"),
+    ("ost", ("content_mask", "style_masks", "style_weights"), "M is not affine in the style statistics"),
+    ("tile_size", ("content_mask", "style_masks", "style_weights"), "the tiled levels take the statistics of one whole style"),
+    ("tile_size", ("swap",), "the swap's gather needs a patch-sized extra halo"),
+    ("tile_size", ("temporal",), "the tiled path has no stabilisation pass"),
+    ("temporal", ("return_float",), "temporal stabilisation works on the uint8 frames"),
+    ("style_weights", ("content_mask", "swap"), "interpolation blends the transforms of whole styles"),
+    ("content_mask", ("adain", "swap"), "spatial control is WCT only"),
+]
+
+# (option, the options of which it needs one)
+NEEDS = [
+    ("mask_feather", ("content_mask",)),
+    ("style_masks", ("content_mask", "content_weights")),
+]
+
+
+def check(active, vocab):
+    """ValueError for the first rule of ``EXCLUDES`` / ``NEEDS`` that the set of canonical option names ``active`` breaks,
+    naming the options as ``vocab`` (``API``, ``ENGINE`` or ``CLI``) spells them."""
+    for a, others, why in EXCLUDES:
+        if a in active:
+            for b in others:
+                if b in active:
+                    raise ValueError("%s does not combine with %s: %s" % (vocab[a], vocab[b], why))
+    for a, wants in NEEDS:
+        if a in active and not active.intersection(wants):
+            raise ValueError("%s needs %s" % (vocab[a], " or ".join(vocab[w] for w in wants)))
+
+
+def check_mst(K, lam, names=("mst", "mst_smooth")):
+    """(K, lambda) of an MST call: K an integer in 1..8, lambda finite and >= 0; ValueError otherwise."""
+    if isinstance(K, bool) or not isinstance(K, (int, np.integer)) or not 1 <= K <= 8:
+        raise ValueError("%s must be a number of clusters in 1..8, got %r" % (names[0], K))
+    try:
+        lam_f = float(lam)
+    except (TypeError, ValueError):
+        raise ValueError("%s must be a number, got %r" % (names[1], lam))
+    if not np.isfinite(lam_f) or lam_f < 0:
+        raise ValueError("%s must be finite and >= 0, got %r" % (names[1], lam))
+    return int(K), lam_f
+
+
+def check_tile_size(tile_size, name="tile_size"):
+    """The tile edge of a tiled call: a positive multiple of 16 (tile boundaries on the pooling grid of every level);
+    ValueError otherwise."""
+    if isinstance(tile_size, bool) or not isinstance(tile_size, (int, np.integer)) or tile_size <= 0 or tile_size % 16:
+        raise ValueError("%s must be a positive multiple of 16, got %r" % (name, tile_size))
+    return int(tile_size)
+
+
+def check_mask_feather(sigma, name="mask_feather"):
+    """The feathering sigma in mask pixels: a finite number in (0, 1024]; ValueError otherwise."""
+    if isinstance(sigma, bool) or not isinstance(sigma, (int, float, np.integer, np.floating)) \
+            or not np.isfinite(sigma) or not 0 < sigma <= 1024:
+        raise ValueError("%s must be a finite sigma in (0, 1024] mask pixels, got %r" % (name, sigma))
+    return float(sigma)
+
+
+def check_temporal_strength(strength, name="temporal strength"):
+    """The weight beta of the warped previous output: in [0, 1); ValueError otherwise."""
+    strength = float(strength)
+    if not 0.0 <= strength < 1.0:
+        raise ValueError("%s must be in [0, 1), got %r" % (name, strength))
+    return strength

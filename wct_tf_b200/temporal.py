@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _capi
+from . import _capi, options
 
 
 def _stream():
@@ -23,10 +23,7 @@ class TemporalState(object):
     stylised size) and its stabilised uint8 output [H, W, 3], both on the device.  ``reset()`` starts the clip again."""
 
     def __init__(self, strength):
-        strength = float(strength)
-        if not 0.0 <= strength < 1.0:
-            raise ValueError("temporal strength must be in [0, 1), got %r" % (strength,))
-        self.strength = strength
+        self.strength = options.check_temporal_strength(strength)
         self.reset()
 
     def reset(self):

@@ -36,6 +36,7 @@ import time
 import numpy as np
 import torch
 
+from . import options
 from .engine import Engine, SEMANTICS
 from .model import RELU_CHANNELS, seamless_axes
 from .prepared import PreparedStyle
@@ -278,9 +279,12 @@ class WCT(object):
         /255 (wct.py:60-64), so the result is bit-identical to calling predict once per pass; style swap only acts in the
         first pass, as in stylize_video.py:117-121.  ``return_device=True`` returns the uint8 cuda tensor instead of a host copy.
 
+        Which of the options below combine is decided by one table, ``wct_tf_b200/options.py``; a call it rejects raises a
+        ValueError naming both options before any device work.
+
         ``content_mask`` (spatial control): uint8 label map [Hm,Wm] shared by every frame, or [N,Hm,Wm]; ``styles`` is then
         a list of R (1..8) uint8 [Hs,Ws,3] images of any sizes, and region r of each frame takes style r.  The mask may have
-        any resolution: every level samples it to its feature grid.  Labels >= R leave that region unstyled.  WCT only.
+        any resolution: every level samples it to its feature grid.  Labels >= R leave that region unstyled.
 
         ``style_masks`` (with ``content_mask``): a list of R entries, each None or a uint8 label map [Hm',Wm'] of style r,
         of any resolution.  Region r of every frame then takes the statistics of the pixels of style r labelled r ("the sky
@@ -292,141 +296,83 @@ class WCT(object):
         ``style_weights`` (style interpolation): ``styles`` is then a list of K (1..8) uint8 [Hs,Ws,3] images of any sizes
         and ``style_weights`` their weights, [K] for every frame or [N,K] (row n for frame n); finite, >= 0, each row with a
         positive sum, normalised to sum 1.  Frame n is stylised with the blend of the K styles, which equals the blend of
-        the K single-style results at every level.  WCT or AdaIN; not with ``content_mask`` or ``swap5``.
+        the K single-style results at every level.
 
         ``swap_targets`` (style swap at any level): a list of relu targets at which the style swap replaces WCT / AdaIN in
         the first pass, with ``ss_alpha`` and the model's ``ss_patch_size`` / ``ss_stride``.  ``swap5=True`` is
         ``swap_targets=["relu5_1"]``; giving both is a ValueError, as is a level that is not a target.  With a stride
-        there is one swap level, and the content is cropped so that the patches tile its encoding.  Not with
-        ``content_mask`` or ``style_weights``.
+        there is one swap level, and the content is cropped so that the patches tile its encoding.
 
         ``temporal`` (a ``temporal_state``): the N frames are the next N frames of that clip.  They are stylised exactly as
         without it; after the last pass each frame is blended with its stabilised predecessor, warped by the optical flow of
         the content frames, where that flow is confident (DESIGN.md §3.3.6), and the state moves on.  The first frame of a
-        clip, and a frame whose size differs from its predecessor's, come back unchanged.  Not with ``return_float``.
+        clip, and a frame whose size differs from its predecessor's, come back unchanged.
 
         ``tile_size`` (tiled stylisation, DESIGN.md §3.3.7): a positive multiple of 16; None or 0 is off.  Every level runs
         in tiles of that edge with crops widened by a halo, so device memory follows the tile, not the image, and images
         too large for one pass (above about 11 600^2 pixels) can be stylised.  Each level's statistics are still those of
         the whole image: the result equals the untiled one up to the order of their summation, and byte for byte when one
-        tile covers the image.  The frames of the batch run one after another.  Works with WCT and AdaIN, ``alpha``,
-        ``passes``, prepared styles, ``return_float`` / ``return_device`` / ``out`` and ``synthesize``; not with
-        ``content_mask``, ``style_masks``, ``style_weights``, ``swap5`` / ``swap_targets`` or ``temporal``.
+        tile covers the image.  The frames of the batch run one after another.
 
         ``ost`` (optimal-transport transform, DESIGN.md §3.3.8): each level maps the content's feature Gaussian onto the
         style's by the Monge map, the covariance-matching map that moves the features least, instead of WCT's whitening
         and colouring; it keeps more of the content's structure at the same ``alpha``.  The style side is WCT's, so image
-        and prepared styles work unchanged.  Works with ``passes``, ``alpha``, ``return_float`` / ``return_device`` /
-        ``out``, ``temporal``, ``tile_size`` and ``swap5`` / ``swap_targets`` (the swap levels swap, the others use OST);
-        not with ``adain``, ``content_mask`` / ``style_masks`` or ``style_weights`` (M is not affine in the style
-        statistics, so the blend of styles does not carry over).
+        and prepared styles work unchanged; with the style swap, the swap levels swap and the others use OST.
 
         ``seamless`` (seamless stylisation, DESIGN.md §3.3.9): "x" wraps the width (360° equirectangular panoramas), "y"
         the height, "xy" both (tileable textures, e.g. with ``synthesize``).  Every conv of the content path -- encoder,
         decoders, and the clip between levels -- pads the wrapped axes circularly, so the output equals, exactly, that of
         the infinitely tiled content and its opposite edges meet without a seam.  Each wrapped axis must be a multiple of
-        2^P, P the pools up to the deepest target (16 for relu5_1).  The style side is unchanged.  Works with WCT, AdaIN,
-        OST, ``alpha``, ``passes``, prepared styles, ``style_weights``, ``content_mask`` / ``style_masks``,
-        ``return_float`` / ``return_device`` / ``out`` and ``tile_size``; not with ``swap5`` / ``swap_targets`` (the
-        swap's VALID patches are not periodic) or ``temporal`` (the optical flow does not see across the seam).
+        2^P, P the pools up to the deepest target (16 for relu5_1).  The style side is unchanged.
 
         ``mst`` (multimodal style transfer, DESIGN.md §3.3.10): K in 1..8.  At every level the style's features are
         clustered into K modes (spherical k-means on their directions), every content pixel is labelled with the mode it
         resembles, the labelling is smoothed by a Potts term of weight ``mst_smooth`` (finite, >= 0; default 0.05), and
         content region k takes the WCT statistics of style mode k.  A painting with several distinct modes is then not
         averaged into one.  K = 1 is the plain WCT call, byte for byte; ``mst=None`` changes nothing.  ``styles`` is one
-        style image.  Works with both semantics, ``alpha``, ``passes`` (the style side is made once per call), batches,
-        ``return_float`` / ``return_device`` / ``out``, ``synthesize`` and ``temporal``; not with prepared styles (they
-        keep no per-level features), one style per frame, ``adain``, ``ost``, ``content_mask`` / ``style_masks``,
-        ``style_weights``, ``swap5`` / ``swap_targets``, ``tile_size`` or ``seamless``.
+        style image, clustered once per call however many ``passes``.
 
         Soft spatial control (DESIGN.md §3.3.11).  ``strength_map``: [Hm,Wm] or [N,Hm,Wm], float in [0,1] or uint8 read as
         v/255, the per-pixel strength s of the call, out = s T(x) + (1 - s) x (in ``np`` semantics towards the unmodified
-        feature x); with WCT, OST, AdaIN, masks, prepared styles, ``alpha``, ``passes``, ``seamless`` and ``temporal``.
+        feature x).
         ``content_weights``: [K,Hm,Wm] or [N,K,Hm,Wm] soft weights of the K region styles given in ``styles`` as for
         ``content_mask`` (divided by their sum where it exceeds 1); region k's statistics are weighted by plane k and each
         pixel blends the K transforms, the rest keeping the content.  ``mask_feather`` = sigma > 0 (with ``content_mask``):
-        the label map feathered by a Gaussian of sigma mask pixels into such weights.  Weights work with WCT only; none of
-        the three combines with ``style_weights``, ``swap5`` / ``swap_targets``, ``mst`` or ``tile_size``, and
-        ``content_weights`` not with ``content_mask``.  None for all three changes nothing.
+        the label map feathered by a Gaussian of sigma mask pixels into such weights.  None for all three changes nothing.
 
         ``efdm`` (exact feature distribution matching, DESIGN.md §3.3.12): at every level each channel of each frame takes
         the whole value distribution of the same channel of its style, not only its mean and variance or covariance: the
         content values are ranked, value rank r takes the style's quantile at r, and equal values take the mean of their
         ranks' quantiles.  Sparse bright strokes and an even wash with the same statistics then stylise differently.
-        ``efdm=False`` changes nothing.  Works with ``alpha``, ``passes`` (the style is sorted once per call), one style or
-        one per frame, sub-batch groups, ``return_float`` / ``return_device`` / ``out``, ``synthesize``, ``seamless``,
-        ``temporal`` and ``swap5`` / ``swap_targets`` (the swap levels swap in the first pass, the others use EFDM); not
-        with ``adain``, ``ost``, ``mst``, ``content_mask`` / ``style_masks`` / ``content_weights`` / ``mask_feather``,
-        ``strength_map``, ``style_weights``, ``tile_size`` (the ranks are over the whole image) or prepared styles (they
-        keep no sorted features)."""
-        if efdm:
-            bad = [name for name, on in (("adain", adain), ("ost", ost), ("mst", mst is not None),
-                                         ("content_mask", content_mask is not None), ("style_masks", style_masks is not None),
-                                         ("content_weights", content_weights is not None),
-                                         ("mask_feather", mask_feather is not None), ("strength_map", strength_map is not None),
-                                         ("style_weights", style_weights is not None),
-                                         ("tile_size", tile_size is not None and tile_size != 0)) if on]
-            if bad:
-                raise ValueError("efdm does not combine with %s" % ", ".join(bad))
-            if isinstance(styles, PreparedStyle):
-                raise ValueError("efdm sorts the style's features at every level, which a prepared style does not keep: "
-                                 "give the style image")
-        soft = strength_map is not None or content_weights is not None or mask_feather is not None
-        if soft:
-            if (style_weights is not None or swap5 or swap_targets is not None or mst is not None
-                    or (tile_size is not None and tile_size != 0)):
-                raise ValueError("strength_map / content_weights / mask_feather do not combine with style_weights, swap5 / "
-                                 "swap_targets, mst or tile_size")
-            if content_weights is not None and content_mask is not None:
-                raise ValueError("content_weights replaces content_mask: give one of them")
-            if mask_feather is not None:
-                if content_mask is None:
-                    raise ValueError("mask_feather needs content_mask")
-                if isinstance(mask_feather, bool) or not isinstance(mask_feather, (int, float, np.integer, np.floating)) \
-                        or not np.isfinite(mask_feather) or not 0 < mask_feather <= 1024:
-                    raise ValueError("mask_feather must be a finite sigma in (0, 1024] mask pixels, got %r" % (mask_feather,))
-            if (content_weights is not None or mask_feather is not None) and (adain or ost):
-                raise ValueError("content_weights / mask_feather work with WCT only: not with adain or ost")
+        ``efdm=False`` changes nothing.  The style is sorted once per call however many ``passes``; with the style swap,
+        the swap levels swap in the first pass and the others use EFDM."""
+        prepared = isinstance(styles, PreparedStyle)
+        per_frame = not prepared and (isinstance(styles, (list, tuple)) or np.ndim(styles) not in (3, 4)
+                                      or (np.ndim(styles) == 4 and styles.shape[0] != 1))
+        options.check({name for name, on in (
+            ("adain", adain), ("ost", ost), ("efdm", efdm), ("mst", mst is not None), ("swap", swap5 or swap_targets is not None),
+            ("content_mask", content_mask is not None), ("style_masks", style_masks is not None),
+            ("style_weights", style_weights is not None), ("content_weights", content_weights is not None),
+            ("mask_feather", mask_feather is not None), ("strength_map", strength_map is not None),
+            ("tile_size", tile_size is not None and tile_size != 0), ("seamless", seamless is not None),
+            ("temporal", temporal is not None), ("return_float", return_float), ("prepared", prepared),
+            ("per_frame_styles", per_frame)) if on}, options.API)
+        if mask_feather is not None:
+            options.check_mask_feather(mask_feather)
         if mst is not None:
-            mst, mst_smooth = Engine.check_mst(mst, mst_smooth)
-            if (adain or ost or content_mask is not None or style_masks is not None or style_weights is not None or swap5
-                    or swap_targets is not None or (tile_size is not None and tile_size != 0) or seamless is not None):
-                raise ValueError("mst does not combine with adain, ost, content_mask, style_masks, style_weights, swap5 / "
-                                 "swap_targets, tile_size or seamless")
-            if isinstance(styles, PreparedStyle):
-                raise ValueError("mst clusters the style's features at every level, which a prepared style does not keep: "
-                                 "give the style image")
-            if isinstance(styles, (list, tuple)) or np.ndim(styles) not in (3, 4) or (np.ndim(styles) == 4 and styles.shape[0] != 1):
-                raise ValueError("mst takes one style image [Hs,Ws,3] for every frame, not one style per frame")
+            mst, mst_smooth = options.check_mst(mst, mst_smooth)
         seamless_axes(seamless)                              # ValueError for a value other than None, "x", "y", "xy"
-        if seamless is not None and (swap5 or swap_targets is not None or temporal is not None):
-            raise ValueError("seamless does not combine with swap5 / swap_targets or temporal")
-        if ost and (adain or content_mask is not None or style_masks is not None or style_weights is not None):
-            raise ValueError("ost does not combine with adain, content_mask, style_masks or style_weights")
         if tile_size is not None and tile_size != 0:
-            Engine.check_tile_size(tile_size)
-            if (content_mask is not None or style_masks is not None or style_weights is not None or swap5
-                    or swap_targets is not None or temporal is not None):
-                raise ValueError("tile_size does not combine with content_mask, style_masks, style_weights, swap5 / "
-                                 "swap_targets or temporal")
+            options.check_tile_size(tile_size)
         else:
             tile_size = None
-        if temporal is not None and return_float:
-            raise ValueError("temporal stabilisation works on the uint8 frames: not with return_float=True")
         eng = self.engine
         dev = eng.device
         n = 1 if np.ndim(contents) == 3 else contents.shape[0]
         eng.swap_levels(swap5, swap_targets)                 # ValueError for both, or a level that is not a target
-        if style_masks is not None and content_mask is None and content_weights is None:
-            raise ValueError("style_masks needs content_mask (or content_weights)")
         if style_weights is not None:
-            if content_mask is not None or swap5 or swap_targets is not None:
-                raise ValueError("style_weights does not combine with content_mask or swap5 / swap_targets")
             weights, interp_styles = self.check_interp(style_weights, n, styles)
         if content_mask is not None:
-            if adain or swap5 or swap_targets is not None:
-                raise ValueError("content_mask works with WCT only: not with adain or swap5 / swap_targets")
             mask, region_styles = self.check_mask(content_mask, n, styles)
             if style_masks is not None:
                 style_masks = self.check_style_masks(style_masks, region_styles)
@@ -641,8 +587,6 @@ class WCT(object):
         value distribution to the style's; ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
         (``predict_batch``).'''
-        soft = {k: v for k, v in (("strength_map", strength_map), ("content_weights", content_weights),
-                                  ("mask_feather", mask_feather)) if v is not None}
         s = time.time()
         seen = {}
 
@@ -651,39 +595,15 @@ class WCT(object):
             if id(x) not in seen:
                 seen[id(x)] = x if isinstance(x, PreparedStyle) else np.asarray(x)
             return seen[id(x)]
-        if style_masks is not None and content_mask is None:
-            raise ValueError("style_masks needs content_mask")
-        if (style_weights is not None or content_mask is not None) and swap_targets is not None:
-            raise ValueError("swap_targets does not combine with content_mask or style_weights")
-        if ost and (adain or content_mask is not None or style_weights is not None):
-            raise ValueError("ost does not combine with adain, content_mask, style_masks or style_weights")
-        if mst is not None and (style_weights is not None or content_mask is not None):
-            raise ValueError("mst does not combine with content_mask, style_masks or style_weights")
-        if efdm and (style_weights is not None or content_mask is not None or content_weights is not None):
-            raise ValueError("efdm does not combine with content_mask, style_masks, content_weights or style_weights")
-        if style_weights is not None:
-            out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
-                                     swap5=swap5, style_weights=style_weights, content_mask=content_mask,
-                                     tile_size=tile_size, seamless=seamless, **soft)
-        elif content_mask is not None or content_weights is not None:
-            kw = {} if style_masks is None else dict(style_masks=style_masks)
-            kw.update(soft)
-            out = self.predict_batch(np.asarray(content), [host(x) for x in _style_list(style)], alpha=alpha, adain=adain,
-                                     swap5=swap5, content_mask=content_mask, tile_size=tile_size, seamless=seamless, **kw)
+        if style_weights is not None or content_mask is not None or content_weights is not None:
+            style = [host(x) for x in _style_list(style)]
         else:
-            kw = {} if swap_targets is None else dict(swap_targets=swap_targets)
-            if tile_size is not None:
-                kw["tile_size"] = tile_size
-            if ost:
-                kw["ost"] = True
-            if seamless is not None:
-                kw["seamless"] = seamless
-            if mst is not None:
-                kw.update(mst=mst, mst_smooth=mst_smooth)
-            if efdm:
-                kw["efdm"] = True
-            kw.update(soft)
-            out = self.predict_batch(np.asarray(content), host(style), alpha=alpha, adain=adain, swap5=swap5, ss_alpha=ss_alpha, **kw)
+            style = host(style)
+        out = self.predict_batch(np.asarray(content), style, alpha=alpha, swap5=swap5, ss_alpha=ss_alpha, adain=adain,
+                                 content_mask=content_mask, style_weights=style_weights, style_masks=style_masks,
+                                 swap_targets=swap_targets, tile_size=tile_size, ost=ost, seamless=seamless, mst=mst,
+                                 mst_smooth=mst_smooth, strength_map=strength_map, content_weights=content_weights,
+                                 mask_feather=mask_feather, efdm=efdm)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
