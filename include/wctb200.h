@@ -334,6 +334,9 @@ WCTB200_API int wctb200_adain_apply_blend(const void* content, int Nc, int Hc, i
  * record against a style state of Ns in {1, Nc} styles, written to a transform buffer instead of applied:
  *   WCT: split-fp16 M [Nc][2][C][C] at *off_m, bias fp32 [Nc][C] at *off_bias, int32 [k_c x Nc | sweeps_c x Nc] at *off_k
  *        (wctb200_wct_transform_layout; 0 for C not in {64,128,256,512} or N < 1); ws of wctb200_wct_workspace_bytes(C, Nc, 0).
+ *        Row exponents int32 e [Nc][C] at wctb200_wct_transform_row_exp_offset(C, Nc) (inside the total): row i of M is
+ *        stored times 2^e_i and the apply multiplies it back exactly.  The library picks e_i so that max_j |M_ij| 2^e_i is in
+ *        [512, 1024), keeping every lo half that matters a normal fp16 number; e = 0 (a zeroed slot) is a row stored as is.
  *   AdaIN: fp32 mean_c, var_c, inv = rsqrt(var_c + eps) sqrt(var_s), ms, each [Nc][C] (wctb200_adain_transform_layout).
  * transform_apply: out = the transform of frame i applied to frame i of any SPF16 map [N,H,W,C] of those frames (a tile
  * with its halo); AdaIN takes alpha here.  A record of whole frames, then its transform, then the apply, gives the bytes
@@ -345,6 +348,7 @@ WCTB200_API int wctb200_adain_stats_rect(const void* act, int N, int H, int W, i
                                          void* stream);
 WCTB200_API int wctb200_stats_accumulate(void* record_a, const void* record_b, int C, int N, int diag, void* stream);
 WCTB200_API size_t wctb200_wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k);
+WCTB200_API size_t wctb200_wct_transform_row_exp_offset(int C, int N);
 WCTB200_API int wctb200_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha,
                                                  float eps_cov, float eps_eig, float thresh, int readd_content_mean,
                                                  void* transform, void* ws, size_t ws_bytes, void* stream);

@@ -253,8 +253,9 @@ def test_weighted_apply_matches_fp64(C):
     tr, M, b = _transform(C, N * K, C + 2, dead=(1 * K + 2,))
     act = U.act_from_numpy(x)
     out = U.act_alloc(N, H, W, C)
-    _capi.check(U.lib().wctb200_wct_transform_apply_weighted(act.data_ptr(), N, H, W, C, tr.data_ptr(), K, U.dev(w).data_ptr(),
-                                                              U.dev(s).data_ptr(), out.data_ptr(), U.stream()))
+    d_w, d_s = U.dev(w), U.dev(s)                         # held until the kernel has read them
+    _capi.check(U.lib().wctb200_wct_transform_apply_weighted(act.data_ptr(), N, H, W, C, tr.data_ptr(), K, d_w.data_ptr(),
+                                                              d_s.data_ptr(), out.data_ptr(), U.stream()))
     U.check_device()
     xin = U.act_raw_padded(act, N, H, W, C)
     got = U.act_raw_padded(out, N, H, W, C)

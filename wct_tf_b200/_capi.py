@@ -89,6 +89,7 @@ SIGNATURES = {
     "wctb200_adain_stats_rect": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "wctb200_stats_accumulate": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "wctb200_wct_transform_layout": (_sz, [_i, _i, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
+    "wctb200_wct_transform_row_exp_offset": (_sz, [_i, _i]),
     "wctb200_wct_transform_from_stats": (_i, [_vp, _i, _i, _vp, _i, _f, _f, _f, _f, _i, _vp, _vp, _sz, _vp]),
     "wctb200_ost_workspace_bytes": (_sz, [_i, _i]),
     "wctb200_ost_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _f, _f, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),

@@ -127,7 +127,7 @@ size_t stats_record_layout(int C, int N, int diag, size_t* off_n, size_t* off_t,
 int launch_wct_stats_rect(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, cudaStream_t st);
 int launch_adain_stats_rect(const __half* act, int N, int H, int W, int C, int y0, int x0, int h, int w, void* record, cudaStream_t st);
 int launch_stats_accumulate(void* rec_a, const void* rec_b, int C, int N, int diag, cudaStream_t st);
-size_t wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k);
+size_t wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k, size_t* off_exp);
 size_t adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, size_t* off_inv, size_t* off_ms);
 int launch_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
                                     float eps_eig, float thresh, int readd, void* transform, void* ws, size_t ws_bytes, cudaStream_t st);
@@ -702,7 +702,13 @@ int wctb200_stats_accumulate(void* record_a, const void* record_b, int C, int N,
 }
 size_t wctb200_wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k) {
     if (!wct_channels_ok(C) || N < 1) return 0;
-    return wct_transform_layout(C, N, off_m, off_bias, off_k);
+    return wct_transform_layout(C, N, off_m, off_bias, off_k, nullptr);
+}
+size_t wctb200_wct_transform_row_exp_offset(int C, int N) {
+    if (!wct_channels_ok(C) || N < 1) return 0;
+    size_t off;
+    wct_transform_layout(C, N, nullptr, nullptr, nullptr, &off);
+    return off;
 }
 int wctb200_wct_transform_from_stats(const void* record, int Nc, int C, const void* state, int Ns, float alpha, float eps_cov,
                                      float eps_eig, float thresh, int readd_content_mean, void* transform, void* ws, size_t ws_bytes,

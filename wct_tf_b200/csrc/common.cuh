@@ -100,6 +100,20 @@ __device__ __forceinline__ void split_f32(float x, __half& hi, __half& lo) {
     hi = __float2half_rn(x);
     lo = __float2half_rn(x - __half2float(hi));
 }
+// exponent S of the power of two that puts a max |value| (as float bits) into [512, 1024), 0 for 0 / NaN: the split of the
+// scaled values keeps every lo that matters a normal fp16 number (DESIGN.md §3.1).  Conv weights (layers.cu, weight_scale)
+// and the rows of the apply operand (wct.cu: k_finalize_transform) are stored with it.
+__device__ __forceinline__ int weight_scale_exp(unsigned int absmax_bits) {
+    const float amax = __uint_as_float(absmax_bits);
+    if (!(amax > 0.f)) return 0;
+    int e;
+    frexpf(amax, &e);                               // amax = m * 2^e, m in [0.5, 1)
+    const int S = 10 - e;                           // amax * 2^S in [512, 1024)
+    return S < -14 ? -14 : (S > 40 ? 40 : S);
+}
+// 2^e exactly, for e in [-126, 127]
+__device__ __forceinline__ float pow2i(int e) { return __int_as_float((127 + e) << 23); }
+__device__ __forceinline__ float weight_scale(unsigned int absmax_bits) { return exp2f((float)weight_scale_exp(absmax_bits)); }
 __device__ __forceinline__ float merge_f32(__half hi, __half lo) { return __half2float(hi) + __half2float(lo); }
 
 // 8 channels = one 16-byte vector per plane
@@ -458,6 +472,9 @@ int scratch_alloc(void** ptr, size_t bytes, cudaStream_t st, int slot);
 enum ConvMode { CONV_3X3 = 0, CONV_APPLY = 1, CONV_UP2 = 2, CONV_TAPS = 3 };
 int launch_conv_tc(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
                    const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw = 3);
+// out = M_n x + bias_n with row i of M_n stored times 2^rexp[n][i] (k_finalize_transform; rexp nullptr: all 0)
+int launch_conv_apply(const __half* in, int N, int H, int W, int C, const __half* w_split, int nsets, const int* rexp,
+                      const float* bias, __half* out, cudaStream_t st);
 int conv_tc_bn(int Cout);
 int launch_conv_taps_rows(const __half* in, int N, int H, int W, int Cin, const __half* w_split, long long wplane, int Cout, int bn,
                           __half* out, cudaStream_t st, int kw);

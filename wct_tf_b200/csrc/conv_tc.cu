@@ -69,6 +69,7 @@ struct ConvParams {
     ActGeom go;           // OUTPUT geometry with its halo mode, made on the host: the epilogue reads it from the parameter bank
     const float* bias;    // [nsets][Cout] or nullptr
     const float* wscale;  // device scalar: 1 / (power-of-two scale the weights were stored with), or nullptr (= 1)
+    const int* rexp;      // CONV_APPLY: [nsets][Cout], row i of set n stored times 2^rexp (k_finalize_transform), or nullptr (0)
     __half* out;          // SPF16, Cout channels; UP2: [N, 2H, 2W, Cout]
     unsigned int* err;
     // regions apply (conv_tc2_kernel<.., REG = true>, spatial control): weight/bias set = image * R + region
@@ -167,7 +168,7 @@ struct Conv2Cfg {
     // 8 banks apart); the epilogue reads 256 contiguous bytes of one row per 8 lanes, which no pitch affects
     static constexpr int PITCH = BN + 8;
     static constexpr int TILE_BYTES = BM * PITCH * 4;
-    static constexpr int AUX_BYTES = 256 + 2 * BN * 4;          // mbarriers + abort flag, then the bias of two passes
+    static constexpr int AUX_BYTES = 256 + 4 * BN * 4;          // mbarriers + abort flag, then the bias and scale of two passes
     static constexpr int RING_BYTES = A_STAGES * STRIP_BYTES + B_STAGES * B_SLOT_BYTES;
     static constexpr int SMEM_BYTES = RING_BYTES + AUX_BYTES + TILE_BYTES + 1024;
     static_assert(SMEM_BYTES <= 227 * 1024, "conv: shared memory exceeds the 227 KB opt-in limit");
@@ -256,16 +257,24 @@ __device__ __forceinline__ void conv_stage_cx(float (&cx)[Cfg::SUM_REGS], uint64
     wgmma_commit();
 }
 
-// sum += acc (FUSE chunk: its two column halves a_hi b_hi + a_hi b_lo added first); WGT: sum = fmaf(v_row, acc, sum).
-// Round-to-nearest FADD / FFMA, in the same order in every instantiation, so that unit weights give the plain sum's bits.
+// sum += acc (FUSE chunk: its two column halves a_hi b_hi + a_hi b_lo added first); WGT: sum = fmaf(v_row s_col, acc, sum)
+// with s_col = 2^-rexp of the pass's weight set at that column (cexp: [BN] of the tile, or nullptr), which makes the
+// running sum s times the plain one exactly.  Round-to-nearest FADD / FFMA, in the same order in every instantiation, so
+// that unit weights give the plain sum's bits.
 template <class Cfg, bool WGT, int R>
-__device__ __forceinline__ void add_into_sum(float (&sum)[Cfg::SUM_REGS], const float (&acc)[R], const float (&vrow)[2]) {
+__device__ __forceinline__ void add_into_sum(float (&sum)[Cfg::SUM_REGS], const float (&acc)[R], const float (&vrow)[2],
+                                             const int* cexp = nullptr, int t = 0) {
 #pragma unroll
     for (int i = 0; i < Cfg::SUM_REGS; ++i) {
         float a = acc[i];
         if constexpr (R > Cfg::SUM_REGS) a += acc[Cfg::SUM_REGS + i];
-        // fragment register i belongs to row r0 + 8 ((i >> 1) & 1)
-        sum[i] = WGT ? fmaf(vrow[(i >> 1) & 1], a, sum[i]) : sum[i] + a;
+        // fragment register i belongs to row r0 + 8 ((i >> 1) & 1) and column 8 (i >> 2) + 2 (t & 3) + (i & 1)
+        if constexpr (WGT) {
+            const float v = cexp ? vrow[(i >> 1) & 1] * pow2i(-__ldg(cexp + 8 * (i >> 2) + 2 * (t & 3) + (i & 1))) : vrow[(i >> 1) & 1];
+            sum[i] = fmaf(v, a, sum[i]);
+        } else {
+            sum[i] = sum[i] + a;
+        }
     }
 }
 
@@ -280,12 +289,20 @@ __device__ __forceinline__ void tile_load8(const float* src, int c, float (&v)[8
     v[4] = h.x; v[5] = h.y; v[6] = h.z; v[7] = h.w;
 }
 
-// *scale + bias, ReLU, split: 8 channels of one output position
-__device__ __forceinline__ void finish8(const float (&a)[8], float wsc, const float* sb, bool relu, Half8& hi, Half8& lo) {
+// *scale + bias, ReLU, split: 8 channels of one output position, biases at s and their scales 2 BN further (the layer's
+// one scale, or in CONV_APPLY each row's own).  Every scale is a power of two, so a * scale is exact and the sum rounds
+// once, as fmaf(a, scale, bias) would.
+template <class Cfg>
+__device__ __forceinline__ void finish8(float (&a)[8], const float* s, int c, bool relu, Half8& hi, Half8& lo) {
+    float t8[8];
+    tile_load8(s + 2 * Cfg::NB * 64, c, t8);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a[j] *= t8[j];
+    tile_load8(s, c, t8);
     float v[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-        const float t = fmaf(a[j], wsc, sb[j]);
+        const float t = a[j] + t8[j];
         v[j] = relu ? fmaxf(t, 0.f) : t;
     }
     split8(v, hi, lo);
@@ -372,10 +389,9 @@ __device__ __forceinline__ void epi_rows(const ConvParams& p, const ActGeom& go,
                 }
                 split8(a, hi, lo);
             } else {
-                float a[8], bb[8];
+                float a[8];
                 tile_load8(ctile + (chunk * 32 + r) * Cfg::PITCH + ch, c, a);
-                tile_load8(sb + ch, c, bb);
-                finish8(a, wsc, bb, relu, hi, lo);
+                finish8<Cfg>(a, sb + ch, c, relu, hi, lo);
             }
             store8_at(p.out, go, q, f, tc.n0 + ch, hi, lo);
         }
@@ -430,10 +446,8 @@ __device__ __forceinline__ void epi_pool(const ConvParams& p, const ActGeom& go,
                 for (int i = 0; i < 8; ++i) m[i] = fmaxf(m[i], a[i]);
             }
         }
-        float bb[8];
-        tile_load8(sb + ch, c, bb);
         Half8 hi, lo;
-        finish8(m, wsc, bb, relu, hi, lo);
+        finish8<Cfg>(m, sb + ch, c, relu, hi, lo);
         store8_at(p.out, go, q, f, tc.n0 + ch, hi, lo);
     }
 }
@@ -461,7 +475,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     uint64_t* tile_full = empty + Cfg::B_STAGES;         // the fp32 tile is written (one arrival per consumer warp)
     uint64_t* tile_empty = tile_full + 1;                // the fp32 tile is read (one arrival per epilogue warp)
     volatile int* abort_flag = reinterpret_cast<volatile int*>(tile_empty + 1);
-    float* sbias = reinterpret_cast<float*>(aux + 256);  // [2][BN]: bias of the pass (by pass parity)
+    float* sbias = reinterpret_cast<float*>(aux + 256);  // [2][BN] bias, then [2][BN] scale of the pass (by pass parity)
     float* ctile = reinterpret_cast<float*>(aux + Cfg::AUX_BYTES);
     float* vst = ctile + Cfg::BM * Cfg::PITCH;           // WGT: [K + 1][BM] v_k and V of the rows of the epilogue's tile
 
@@ -498,7 +512,8 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const int ncol = REG ? 1 : p.ncol;                   // the regions apply is a 1x1 conv
     const bool pool = !REG && p.pool;
 
-    // register split, checked with ptxas -v to spill nothing: the consumers of BN = 128 need more than 200 and the epilogue
+    // register split, checked with ptxas -v to spill nothing (but 8 bytes in the weighted apply at BN = 128, whose consumers
+    // also read the row scales of each pass): the consumers of BN = 128 need more than 200 and the epilogue
     // warps more than 56 (REG: 80).  setmaxnreg.inc only receives what the other warpgroups released, so the split must
     // stay within the 3 x 128 x 168 registers the CTA was launched with, or the consumers wait for registers forever.
     constexpr int EPI_REGS = REG ? (BN == 128 ? 88 : 104) : 72;
@@ -604,8 +619,10 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 // bias of this pass into the buffer of its parity: that buffer was last read two passes ago, before every
                 // epilogue warp passed the previous pass's barrier
                 float* sb = sbias + (pass & 1) * BN;
-                for (int i = threadIdx.x - (Cfg::CONSUMERS + 32); i < BN; i += 32 * Cfg::EPI_WARPS)
+                for (int i = threadIdx.x - (Cfg::CONSUMERS + 32); i < BN; i += 32 * Cfg::EPI_WARPS) {
                     sb[i] = p.bias ? __ldg(p.bias + (long long)(p.mode == CONV_APPLY ? set : 0) * p.Cout + tc.n0 + i) : 0.f;   // UP2: set = weight parity class, ONE bias
+                    sb[2 * BN + i] = p.rexp ? pow2i(-__ldg(p.rexp + (long long)set * p.Cout + tc.n0 + i)) : wsc;
+                }
                 mbar_wait(tile_full, pass & 1, abort_flag, p.err, 0x301u);
                 asm volatile("bar.sync 1, %0;" ::"r"(32 * Cfg::EPI_WARPS) : "memory");
                 if (p.pool) epi_pool<Cfg>(p, go, tc, ctile, sb, wsc, relu, ew, lane, abort_flag);
@@ -636,12 +653,14 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         }
         for (; todo; todo &= todo - 1u) {
         float vrow[2] = {1.f, 1.f};                      // WGT: v_k of this thread's two fragment rows
+        const int* cexp = nullptr;                       // WGT: the row exponents of transform k at the tile's channels
         if constexpr (WGT) {
             const TileCoord tc = tile_coord(p, tile, n_tiles, BN);
             const int k = __ffs(todo) - 1;
             const int r0 = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);
             vrow[0] = row_weight(p, tc.p0, tc.p_end, r0, k);
             vrow[1] = row_weight(p, tc.p0, tc.p_end, r0 + 8, k);
+            if (p.rexp) cexp = p.rexp + (long long)((tile / n_tiles) / p.tiles_per_image * p.R + k) * p.Cout + tc.n0;
         } else {
 #pragma unroll
             for (int i = 0; i < Cfg::SUM_REGS; ++i) sum[i] = 0.f;
@@ -703,7 +722,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             }
             if ((it + 1) % Cfg::CH == 0) {              // chunk end
                 acc_fence(ch);
-                add_into_sum<Cfg, WGT>(sum, ch, vrow);
+                add_into_sum<Cfg, WGT>(sum, ch, vrow, cexp, t);
             }
         }
         wgmma_wait<0>();
@@ -716,8 +735,8 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 mbar_arrive(&emptyA[(stg - 1) % Cfg::A_STAGES]);
             }
         }
-        if (kiters % Cfg::CH != 0) add_into_sum<Cfg, WGT>(sum, ch, vrow);   // the last chunk is a short one
-        add_into_sum<Cfg, WGT>(sum, cx, vrow);
+        if (kiters % Cfg::CH != 0) add_into_sum<Cfg, WGT>(sum, ch, vrow, cexp, t);   // the last chunk is a short one
+        add_into_sum<Cfg, WGT>(sum, cx, vrow, cexp, t);
 
         if constexpr (!WGT) {
             // ---- hand the fp32 tile to the epilogue warps (row-major in shared memory: a wgmma fragment spreads one row
@@ -808,7 +827,8 @@ int g_conv_fuse = -1;        // -1 auto, 0 never, 1 whenever the tile allows (wc
 int g_conv_bn_override = 0;  // test/tuning hook: force the N tile (64/128; 256 runs as 128)
 
 // mode CONV_3X3  : in [N,H,W,Cin], w_split [2][Cout][9*Cin],          out [N,H,W,Cout]
-// mode CONV_APPLY: in [N,H,W,Cin], w_split [nsets][2][Cout][Cin],     out [N,H,W,Cout]   (per-image weight sets)
+// mode CONV_APPLY: in [N,H,W,Cin], w_split [nsets][2][Cout][Cin],     out [N,H,W,Cout]   (per-image weight sets; rexp
+//                  [nsets][Cout]: row i stored times 2^rexp, or nullptr)
 // mode CONV_UP2  : in [N,H,W,Cin] (edge halo), w_split [4][2][Cout][4*Cin], out [N,2H,2W,Cout]
 // mode CONV_TAPS : in [N,H,W,Cin], w_split [2][Cout][kw*kw*Cin],      out [N,H,W,Cout]: top-left anchored kw x kw correlation
 // regions (spatial control, CONV_APPLY with C = Cin = Cout): w_split [N*R][2][C][C], bias [N*R][C]; labels / counts / amask
@@ -823,7 +843,8 @@ int conv_tc_bn(int Cout) {
 static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin, const __half* w_split, int nsets,
                         const float* wscale, const float* bias, int Cout, int flags, __half* out, cudaStream_t st, int kw,
                         const uint8_t* labels, const int* counts, const uint16_t* amask, int R, int bn_req = 0,
-                        long long wplane = 0, const float* wts = nullptr, const float* str = nullptr, const int* kc = nullptr) {
+                        long long wplane = 0, const float* wts = nullptr, const float* str = nullptr, const int* kc = nullptr,
+                        const int* rexp = nullptr) {
     const bool wgt = kc != nullptr;
     const bool reg = labels != nullptr || wgt;
     WCTB_REQUIRE(!reg || (mode == CONV_APPLY && Cin == Cout && nsets == N * R && flags == 0), "conv: bad regions apply");
@@ -878,6 +899,7 @@ static int conv_tc_impl(int mode, const __half* in, int N, int H, int W, int Cin
     p.go.set_halo(flags);
     p.bias = bias;
     p.wscale = wscale;
+    p.rexp = mode == CONV_APPLY ? rexp : nullptr;
     p.out = out;
     p.err = device_error_word();
     p.in = in;
@@ -930,16 +952,23 @@ int launch_conv_taps_rows(const __half* in, int N, int H, int W, int Cin, const 
                         bn, wplane);
 }
 // out = M_{n,r} x + bias_{n,r} for the pixels of region r of image n, out = x for the rest (wct.cu: launch_wct_apply_regions)
-int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const uint8_t* labels,
-                              const int* counts, const uint16_t* amask, int R, __half* out, cudaStream_t st) {
-    return conv_tc_impl(CONV_APPLY, in, N, H, W, C, w_split, N * R, nullptr, bias, C, 0, out, st, 3, labels, counts, amask, R);
+int launch_conv_apply(const __half* in, int N, int H, int W, int C, const __half* w_split, int nsets, const int* rexp,
+                      const float* bias, __half* out, cudaStream_t st) {
+    return conv_tc_impl(CONV_APPLY, in, N, H, W, C, w_split, nsets, nullptr, bias, C, 0, out, st, 3, nullptr, nullptr, nullptr, 1, 0, 0,
+                        nullptr, nullptr, nullptr, rexp);
+}
+int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const int* rexp, const float* bias,
+                              const uint8_t* labels, const int* counts, const uint16_t* amask, int R, __half* out, cudaStream_t st) {
+    return conv_tc_impl(CONV_APPLY, in, N, H, W, C, w_split, N * R, nullptr, bias, C, 0, out, st, 3, labels, counts, amask, R, 0, 0,
+                        nullptr, nullptr, nullptr, rexp);
 }
 // out = sum_k v_k (M_{n,k} x + bias_{n,k}) + (1 - sum_k v_k) x, v_k = soft_weight(wts, str, kc, ...) (wct.cu:
 // launch_wct_transform_apply_weighted); amask as in ConvParams
-int launch_conv_apply_weighted(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const float* wts,
-                               const float* str, const int* kc, const uint16_t* amask, int K, __half* out, cudaStream_t st) {
+int launch_conv_apply_weighted(const __half* in, int N, int H, int W, int C, const __half* w_split, const int* rexp, const float* bias,
+                               const float* wts, const float* str, const int* kc, const uint16_t* amask, int K, __half* out,
+                               cudaStream_t st) {
     return conv_tc_impl(CONV_APPLY, in, N, H, W, C, w_split, N * K, nullptr, bias, C, 0, out, st, 3, nullptr, nullptr, amask, K, 0, 0,
-                        wts, str, kc);
+                        wts, str, kc, rexp);
 }
 
 }  // namespace wctb

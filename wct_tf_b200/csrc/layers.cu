@@ -111,15 +111,6 @@ __global__ void k_absmax(const float* __restrict__ w, long long n, unsigned int*
     for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) atomicMax(out_bits, __float_as_uint(m));    // non-negative floats order like their bits
 }
-__device__ __forceinline__ float weight_scale(unsigned int absmax_bits) {
-    const float amax = __uint_as_float(absmax_bits);
-    if (!(amax > 0.f)) return 1.f;
-    int e;
-    frexpf(amax, &e);                               // amax = m * 2^e, m in [0.5, 1)
-    int S = 10 - e;                                 // amax * 2^S in [512, 1024)
-    S = S < -14 ? -14 : (S > 40 ? 40 : S);
-    return exp2f((float)S);                         // exact power of two
-}
 __global__ void k_prep_weights(const float* __restrict__ w, int taps, int Cin, int Cout, __half* __restrict__ ws,
                                float* __restrict__ trailer) {
     const long long K = (long long)taps * Cin;

@@ -605,12 +605,14 @@ k_outer_gemm(const float* __restrict__ A, long long sa, const float* __restrict_
             make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
 }
 
-// M = alpha*T + (1-alpha)*I  -> split-fp16 GEMM operand [frame][2][C][C] (row = output channel)
-// bias = alpha*ms - M*mc + (1-alpha)*readd*mc                       (ops.py:80-83 / 131-133)
+// M = alpha*T + (1-alpha)*I  -> split-fp16 GEMM operand [frame][2][C][C] (row = output channel), row i stored times 2^e_i,
+// e_i in mexp [frame][C]: the power of two that puts the row's max |m| into [512, 1024) (weight_scale_exp), so that no lo
+// half that matters is an fp16 subnormal (DESIGN.md §3.1); the apply's epilogue multiplies by 2^-e_i exactly
+// bias = alpha*ms - M*mc + (1-alpha)*readd*mc  from the unscaled M     (ops.py:80-83 / 131-133)
 //   one warp per (frame, output channel); style mean z % Ns (Ns == 1: shared; regions: problem z = frame*R + r, Ns = R)
 __global__ void k_finalize_transform(const float* __restrict__ T, int C, int Nc, int Ns, float alpha, int readd,
                                      const float* __restrict__ mean_c, const float* __restrict__ mean_s,
-                                     __half* __restrict__ Msplit, float* __restrict__ bias) {
+                                     __half* __restrict__ Msplit, int* __restrict__ mexp, float* __restrict__ bias) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int row = blockIdx.x * (blockDim.x >> 5) + warp;
     const int z = blockIdx.y;
@@ -620,11 +622,18 @@ __global__ void k_finalize_transform(const float* __restrict__ T, int C, int Nc,
     const float* ms = mean_s + (long long)(Ns == 1 ? 0 : z % Ns) * C;
     __half* mh = Msplit + (((long long)z * 2 + 0) * C + row) * C;
     __half* ml = Msplit + (((long long)z * 2 + 1) * C + row) * C;
+    float amax = 0.f;
+    for (int j = lane; j < C; j += 32) amax = fmaxf(amax, fabsf(alpha * t[j] + (j == row ? 1.f - alpha : 0.f)));
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const int e = weight_scale_exp(__float_as_uint(amax));
+    const float sc = pow2i(e);
+    if (lane == 0) mexp[(long long)z * C + row] = e;
     float dot = 0.f;
     for (int j = lane; j < C; j += 32) {
         const float m = alpha * t[j] + (j == row ? 1.f - alpha : 0.f);
         __half hi, lo;
-        split_f32(m, hi, lo);
+        split_f32(m * sc, hi, lo);
         mh[j] = hi;
         ml[j] = lo;
         dot = fmaf(m, mc[j], dot);
@@ -704,7 +713,7 @@ __global__ void k_affine_apply_strength(const __half* __restrict__ in, ActGeom g
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 struct WctWs {
-    size_t shift, dsum, mean, var, G, A0, lam, sigma, dvec, Wc, Cs, T, Msplit, bias, conv, kcount, ok, inv, ms, total;
+    size_t shift, dsum, mean, var, G, A0, lam, sigma, dvec, Wc, Cs, T, Msplit, Mexp, bias, conv, kcount, ok, inv, ms, total;
 };
 static WctWs wct_layout(int C, int Nc, int Ns) {
     WctWs w;
@@ -724,6 +733,7 @@ static WctWs wct_layout(int C, int Nc, int Ns) {
     w.Cs = take((size_t)Ns * C * C * 4);
     w.T = take((size_t)Nc * C * C * 4);
     w.Msplit = take((size_t)Nc * 2 * C * C * 2);
+    w.Mexp = take((size_t)Nc * C * 4);
     w.bias = take((size_t)Nc * C * 4);
     w.conv = take(np * 16 * 4);
     w.kcount = take(np * 2 * 4);
@@ -933,10 +943,11 @@ int launch_wct_level(const __half* content, int Nc, int Hc, int Wc, const __half
     k_outer_gemm<<<gt, 256, 0, st>>>(Csm, Ns == 1 ? 0 : CC, Wcm, CC, nullptr, 0, T, CC, C);   // T = C_s W_c (C_s symmetric)
     WCTB_CHECK_LAUNCH("k_outer_gemm(T)");
     dim3 gf((unsigned)cdiv(C, 8), (unsigned)Nc);
-    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean + (long long)Nc * C, Msplit, bias);
+    int* Mexp = reinterpret_cast<int*>(w + L.Mexp);
+    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean + (long long)Nc * C, Msplit, Mexp, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform");
     // out = M x + bias on the tensor cores (1-tap conv, per-frame weight set)
-    rc = launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, Msplit, Nc, nullptr, bias, C, 0, out, st);
+    rc = launch_conv_apply(content, Nc, Hc, Wc, C, Msplit, Nc, Mexp, bias, out, st);
     if (rc) return rc;
     if (k_out) WCTB_CUDA(cudaMemcpyAsync(k_out, kc, (size_t)np * 2 * 4, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -1051,7 +1062,7 @@ static int wct_whiten(int Nc, int C, float eps_eig, float thresh, uint8_t* w, co
 // Style side of the split transform after wct_content_side: T = C_s W_c, the split-fp16 operand M and the bias, then
 // out = M x + bias on the tensor cores.  C_s [Ns][C][C] and mean_s [Ns][C] with Ns == 1 (shared) or Ns == Nc (per frame).
 static int wct_colour_transform(int Nc, int C, const float* Cs, const float* mean_s, int Ns, float alpha, int readd, uint8_t* w,
-                                const WctWs& L, __half* Msplit, float* bias, cudaStream_t st) {
+                                const WctWs& L, __half* Msplit, int* Mexp, float* bias, cudaStream_t st) {
     const float* mean = reinterpret_cast<const float*>(w + L.mean);
     const float* Wcm = reinterpret_cast<const float*>(w + L.Wc);
     float* T = reinterpret_cast<float*>(w + L.T);
@@ -1060,17 +1071,18 @@ static int wct_colour_transform(int Nc, int C, const float* Cs, const float* mea
     k_outer_gemm<<<gg, 256, 0, st>>>(Cs, Ns == 1 ? 0 : CC, Wcm, CC, nullptr, 0, T, CC, C);   // T = C_s W_c
     WCTB_CHECK_LAUNCH("k_outer_gemm(T)");
     dim3 gf((unsigned)cdiv(C, 8), (unsigned)Nc);
-    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean_s, Msplit, bias);
+    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean_s, Msplit, Mexp, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform");
     return 0;
 }
 static int wct_colour_apply(const __half* content, int Nc, int Hc, int Wc, int C, const float* Cs, const float* mean_s, int Ns,
                             float alpha, int readd, uint8_t* w, const WctWs& L, __half* out, cudaStream_t st) {
     __half* Msplit = reinterpret_cast<__half*>(w + L.Msplit);
+    int* Mexp = reinterpret_cast<int*>(w + L.Mexp);
     float* bias = reinterpret_cast<float*>(w + L.bias);
-    int rc = wct_colour_transform(Nc, C, Cs, mean_s, Ns, alpha, readd, w, L, Msplit, bias, st);
+    int rc = wct_colour_transform(Nc, C, Cs, mean_s, Ns, alpha, readd, w, L, Msplit, Mexp, bias, st);
     if (rc) return rc;
-    return launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, Msplit, Nc, nullptr, bias, C, 0, out, st);
+    return launch_conv_apply(content, Nc, Hc, Wc, C, Msplit, Nc, Mexp, bias, out, st);
 }
 
 int launch_wct_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Ns, float alpha,
@@ -1110,15 +1122,18 @@ int launch_wct_apply(const __half* content, int Nc, int Hc, int Wc, int C, const
 // record instead of summed over the content, cut after the transform.  The transform buffer is applied to any feature
 // map of the frame (a tile and its halo).  The steps after the statistics are the ones wct_apply / adain_apply run.
 //   WCT transform:   split-fp16 M [N][2][C][C] | bias fp32 [N][C] | int32 [k_c x N | sweeps_c x N]
+//                    | int32 [N][C] e: row i of M is stored times 2^e_i (k_finalize_transform; 0 = as is)
 //   AdaIN transform: fp32 mean_c [N][C] | var_c [N][C] | inv [N][C] | ms [N][C]
 // ---------------------------------------------------------------------------
-size_t wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k) {
+size_t wct_transform_layout(int C, int N, size_t* off_m, size_t* off_bias, size_t* off_k, size_t* off_exp) {
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
     const size_t a = take((size_t)N * 2 * C * C * 2), b = take((size_t)N * C * 4), c = take((size_t)N * 2 * 4);
+    const size_t d = take((size_t)N * C * 4);
     if (off_m) *off_m = a;
     if (off_bias) *off_bias = b;
     if (off_k) *off_k = c;
+    if (off_exp) *off_exp = d;
     return o;
 }
 size_t adain_transform_layout(int C, int N, size_t* off_mean, size_t* off_var, size_t* off_inv, size_t* off_ms) {
@@ -1163,11 +1178,12 @@ int launch_wct_transform_from_stats(const void* record, int Nc, int C, const voi
     if (rc) return rc;
     rc = wct_whiten(Nc, C, eps_eig, thresh, w, L, st);
     if (rc) return rc;
-    size_t om, ob, ok;
-    wct_transform_layout(C, Nc, &om, &ob, &ok);
+    size_t om, ob, ok, oexp;
+    wct_transform_layout(C, Nc, &om, &ob, &ok, &oexp);
     uint8_t* tp = static_cast<uint8_t*>(transform);
     rc = wct_colour_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
-                              w, L, reinterpret_cast<__half*>(tp + om), reinterpret_cast<float*>(tp + ob), st);
+                              w, L, reinterpret_cast<__half*>(tp + om), reinterpret_cast<int*>(tp + oexp),
+                              reinterpret_cast<float*>(tp + ob), st);
     if (rc) return rc;
     k_transform_kout<<<(unsigned)cdiv(Nc, 256), 256, 0, st>>>(kc, stats_record_at(record, C, Nc, 0).n,
                                                             reinterpret_cast<const int*>(sp + off_k), Nc, Ns,
@@ -1177,11 +1193,11 @@ int launch_wct_transform_from_stats(const void* record, int Nc, int C, const voi
 }
 int launch_wct_transform_apply(const __half* act, int N, int H, int W, int C, const void* transform, __half* out, cudaStream_t st) {
     WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_transform_apply: C=%d not in {64,128,256,512}", C);
-    size_t om, ob;
-    wct_transform_layout(C, N, &om, &ob, nullptr);
+    size_t om, ob, oexp;
+    wct_transform_layout(C, N, &om, &ob, nullptr, &oexp);
     const uint8_t* tp = static_cast<const uint8_t*>(transform);
-    return launch_conv_tc(CONV_APPLY, act, N, H, W, C, reinterpret_cast<const __half*>(tp + om), N, nullptr,
-                          reinterpret_cast<const float*>(tp + ob), C, 0, out, st);
+    return launch_conv_apply(act, N, H, W, C, reinterpret_cast<const __half*>(tp + om), N,
+                          reinterpret_cast<const int*>(tp + oexp), reinterpret_cast<const float*>(tp + ob), out, st);
 }
 
 // ---------------------------------------------------------------------------
@@ -1256,7 +1272,7 @@ size_t ost_workspace_bytes(int C, int Nc) { return ost_layout(C, Nc).total; }
 
 // after wct_content_side / wct_whiten: M into L.T, then the split operand and bias of k_finalize_transform
 static int ost_transform(int Nc, int C, const float* Cs, const float* mean_s, int Ns, float alpha, int readd, float eps_eig,
-                         uint8_t* w, const OstWs& O, __half* Msplit, float* bias, cudaStream_t st) {
+                         uint8_t* w, const OstWs& O, __half* Msplit, int* Mexp, float* bias, cudaStream_t st) {
     const WctWs& L = O.L;
     const long long CC = (long long)C * C;
     const float* mean = reinterpret_cast<const float*>(w + L.mean);
@@ -1297,7 +1313,7 @@ static int ost_transform(int Nc, int C, const float* Cs, const float* mean_s, in
     k_outer_gemm<<<gg, 256, 0, st>>>(Wcm, CC, Q, CC, nullptr, 0, T, CC, C);                   // M = W_c B^1/2 W_c
     WCTB_CHECK_LAUNCH("k_outer_gemm(M)");
     const dim3 gf((unsigned)cdiv(C, 8), (unsigned)Nc);
-    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean_s, Msplit, bias);
+    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, Nc, Ns, alpha, readd, mean, mean_s, Msplit, Mexp, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform");
     return 0;
 }
@@ -1319,11 +1335,12 @@ int launch_ost_apply(const __half* content, int Nc, int Hc, int Wc, int C, const
     int rc = wct_content_side(content, Nc, Hc, Wc, C, eps_cov, eps_eig, thresh, w, O.L, st);
     if (rc) return rc;
     __half* Msplit = reinterpret_cast<__half*>(w + O.L.Msplit);
+    int* Mexp = reinterpret_cast<int*>(w + O.L.Mexp);
     float* bias = reinterpret_cast<float*>(w + O.L.bias);
     rc = ost_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
-                       eps_eig, w, O, Msplit, bias, st);
+                       eps_eig, w, O, Msplit, Mexp, bias, st);
     if (rc) return rc;
-    rc = launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, Msplit, Nc, nullptr, bias, C, 0, out, st);
+    rc = launch_conv_apply(content, Nc, Hc, Wc, C, Msplit, Nc, Mexp, bias, out, st);
     if (rc) return rc;
     if (k_out) {
         // k_out: [k_c x Nc | sweeps_c x Nc | ok_c x Nc | ok_b x Nc | sweeps_b x Nc]
@@ -1356,11 +1373,12 @@ int launch_ost_transform_from_stats(const void* record, int Nc, int C, const voi
     if (rc) return rc;
     rc = wct_whiten(Nc, C, eps_eig, thresh, w, O.L, st);
     if (rc) return rc;
-    size_t om, ob, ok;
-    wct_transform_layout(C, Nc, &om, &ob, &ok);
+    size_t om, ob, ok, oexp;
+    wct_transform_layout(C, Nc, &om, &ob, &ok, &oexp);
     uint8_t* tp = static_cast<uint8_t*>(transform);
     rc = ost_transform(Nc, C, reinterpret_cast<const float*>(sp + off_cs), reinterpret_cast<const float*>(sp), Ns, alpha, readd,
-                       eps_eig, w, O, reinterpret_cast<__half*>(tp + om), reinterpret_cast<float*>(tp + ob), st);
+                       eps_eig, w, O, reinterpret_cast<__half*>(tp + om), reinterpret_cast<int*>(tp + oexp),
+                       reinterpret_cast<float*>(tp + ob), st);
     if (rc) return rc;
     k_transform_kout<<<(unsigned)cdiv(Nc, 256), 256, 0, st>>>(kc, stats_record_at(record, C, Nc, 0).n,
                                                             reinterpret_cast<const int*>(sp + off_k), Nc, Ns,
@@ -1836,7 +1854,7 @@ size_t wct_regions_workspace_bytes(int C, int Nc, int R, int Hc, int Wc) { retur
 
 int launch_mean_cov_regions(const __half* act, ActGeom g, const uint8_t* labels, int R, const int* counts, const uint16_t* tmask,
                             float eps_cov, float* mean, float* G, float* A0, double* dsum, cudaStream_t st);
-int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias,
+int launch_conv_apply_regions(const __half* in, int N, int H, int W, int C, const __half* w_split, const int* rexp, const float* bias,
                               const uint8_t* labels, const int* counts, const uint16_t* amask, int R, __half* out, cudaStream_t st);
 
 static int region_scan(const uint8_t* labels, int N, int H, int W, int R, int* counts, uint16_t* tmask, cudaStream_t st) {
@@ -1919,13 +1937,14 @@ int launch_wct_apply_regions(const __half* content, int Nc, int Hc, int Wc, int 
     k_outer_gemm<<<gg, 256, 0, st>>>(Cs, CC, Wcm, CC, nullptr, 0, T, CC, C, nullptr, R);   // T = C_s(z % R) W_c(z)
     WCTB_CHECK_LAUNCH("k_outer_gemm(T)");
     dim3 gf((unsigned)cdiv(C, 8), (unsigned)np);
-    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, np, R, alpha, readd, mean, mean_s, Msplit, bias);
+    int* Mexp = reinterpret_cast<int*>(w + L.Mexp);
+    k_finalize_transform<<<gf, 256, 0, st>>>(T, C, np, R, alpha, readd, mean, mean_s, Msplit, Mexp, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform");
     // out = M_{n,r} x + bias_{n,r} per pixel of region r; every other pixel keeps its input bytes
     const long long napply = (long long)Nc * RL.tiles_per_image;
     k_region_apply_tiles<<<(unsigned)cdiv(napply, 8), 256, 0, st>>>(labels, counts, Nc, Hc, Wc, R, RL.tiles_per_image, amask);
     WCTB_CHECK_LAUNCH("k_region_apply_tiles");
-    rc = launch_conv_apply_regions(content, Nc, Hc, Wc, C, Msplit, bias, labels, counts, amask, R, out, st);
+    rc = launch_conv_apply_regions(content, Nc, Hc, Wc, C, Msplit, Mexp, bias, labels, counts, amask, R, out, st);
     if (rc) return rc;
     if (k_out) {
         k_regions_kout<<<(unsigned)cdiv(np > R ? np : R, 256), 256, 0, st>>>(kc, counts, ks, np, R, k_out);
@@ -2157,15 +2176,16 @@ k_weighted_apply_tiles(const float* __restrict__ wts, const float* __restrict__ 
     if (lane == 0) amask[t] = (uint16_t)bits;
 }
 
-int launch_conv_apply_weighted(const __half* in, int N, int H, int W, int C, const __half* w_split, const float* bias, const float* wts,
-                               const float* str, const int* kc, const uint16_t* amask, int K, __half* out, cudaStream_t st);
+int launch_conv_apply_weighted(const __half* in, int N, int H, int W, int C, const __half* w_split, const int* rexp, const float* bias,
+                               const float* wts, const float* str, const int* kc, const uint16_t* amask, int K, __half* out,
+                               cudaStream_t st);
 
 int launch_wct_transform_apply_weighted(const __half* act, int N, int H, int W, int C, const void* transform, int K, const float* wts,
                                         const float* str, __half* out, cudaStream_t st) {
     WCTB_REQUIRE(C == 64 || C == 128 || C == 256 || C == 512, "wct_transform_apply_weighted: C=%d not in {64,128,256,512}", C);
     WCTB_REQUIRE(K >= 1 && K <= 8 && (wts || K == 1), "wct_transform_apply_weighted: K=%d not in 1..8 (1 without weights)", K);
-    size_t om, ob, ok;
-    wct_transform_layout(C, N * K, &om, &ob, &ok);
+    size_t om, ob, ok, oexp;
+    wct_transform_layout(C, N * K, &om, &ob, &ok, &oexp);
     const uint8_t* tp = static_cast<const uint8_t*>(transform);
     const int* kc = reinterpret_cast<const int*>(tp + ok);
     const int tpi = cdiv((long long)(H + 2) * (W + 2), 128);
@@ -2173,8 +2193,8 @@ int launch_wct_transform_apply_weighted(const __half* act, int N, int H, int W, 
     { int rc0 = scratch_alloc(reinterpret_cast<void**>(&amask), (size_t)N * tpi * 2, st, 7); if (rc0) return rc0; }
     k_weighted_apply_tiles<<<(unsigned)cdiv((long long)N * tpi, 8), 256, 0, st>>>(wts, str, kc, N, H, W, K, tpi, amask);
     WCTB_CHECK_LAUNCH("k_weighted_apply_tiles");
-    return launch_conv_apply_weighted(act, N, H, W, C, reinterpret_cast<const __half*>(tp + om), reinterpret_cast<const float*>(tp + ob),
-                                      wts, str, kc, amask, K, out, st);
+    return launch_conv_apply_weighted(act, N, H, W, C, reinterpret_cast<const __half*>(tp + om), reinterpret_cast<const int*>(tp + oexp),
+                                      reinterpret_cast<const float*>(tp + ob), wts, str, kc, amask, K, out, st);
 }
 
 // ---------------------------------------------------------------------------
@@ -2284,9 +2304,9 @@ static inline int swap_grid(long long total, int block) {
 // depends only on the style features, so it is prepared once into a state and applied to any number of content frames.
 //   state layout (256-byte aligned blocks): [C] mean_s | int32 [2] (k_s, sweeps_s) | whitened style SPF16 [1,Hs,Ws,C]
 //   (gathered from) | [P*P][C] 1/||tap|| | split-fp16 patch filters [2][cout_pad][P*P*C] | colouring operand [2][C][C] (C_s
-//   split) | [C] its bias (m_s)
+//   split, row i times 2^e_i) | int32 [C] e | [C] its bias (m_s)
 struct SwapState {
-    size_t mean, k, feat, norms, wsplit, cmsplit, cbias, total;
+    size_t mean, k, feat, norms, wsplit, cmsplit, cmexp, cbias, total;
     int cout_pad, n_patches, prow, pcol;           // style patch grid prow x pcol
 };
 static SwapState swap_state_layout(int C, int Hs, int Ws, int P, int S) {
@@ -2303,13 +2323,14 @@ static SwapState swap_state_layout(int C, int Hs, int Ws, int P, int S) {
     L.norms = take((size_t)P * P * C * 4);
     L.wsplit = take((size_t)2 * P * P * C * L.cout_pad * sizeof(__half));
     L.cmsplit = take((size_t)2 * C * C * 2);
+    L.cmexp = take((size_t)C * 4);
     L.cbias = take((size_t)C * 4);
     L.total = o;
     return L;
 }
 // workspace of the prepare: the eigensolver's (wct_layout(C, 0, 1)) and the style's whitening / colouring matrices
 struct SwapPrepWs {
-    size_t base, zeros, dvec2, sigma2, Wm, Cm, msplit, bias, total;
+    size_t base, zeros, dvec2, sigma2, Wm, Cm, msplit, mexp, bias, total;
 };
 static SwapPrepWs swap_prep_layout(int C) {
     SwapPrepWs L;
@@ -2322,6 +2343,7 @@ static SwapPrepWs swap_prep_layout(int C) {
     L.Wm = take((size_t)C * C * 4);                               // W_s (whitening)
     L.Cm = take((size_t)C * C * 4);                               // C_s (colouring)
     L.msplit = take((size_t)2 * C * C * 2);
+    L.mexp = take((size_t)C * 4);
     L.bias = take((size_t)C * 4);
     L.total = o;
     return L;
@@ -2550,6 +2572,7 @@ int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int pa
     float* Wm = reinterpret_cast<float*>(sw + PL.Wm);
     float* Cm = reinterpret_cast<float*>(sw + PL.Cm);
     __half* msplit = reinterpret_cast<__half*>(sw + PL.msplit);
+    int* mexp = reinterpret_cast<int*>(sw + PL.mexp);
     float* bias = reinterpret_cast<float*>(sw + PL.bias);
     float* mean_s = reinterpret_cast<float*>(sp + SL.mean);
     int* ks = reinterpret_cast<int*>(sp + SL.k);
@@ -2575,13 +2598,14 @@ int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int pa
     k_outer_gemm<<<g1, 256, 0, st>>>(G, CC, G, CC, dvec2, C, Cm, CC, C);                       // C_s
     WCTB_CHECK_LAUNCH("k_outer_gemm(colour)");
     // whitening operand: x -> W_s (x - m_s) (alpha = 1, "style mean" = 0); colouring operand: x -> C_s x + m_s ("content mean" = 0)
-    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(Wm, C, 1, 1, 1.f, 0, mean_s, zeros, msplit, bias);
+    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(Wm, C, 1, 1, 1.f, 0, mean_s, zeros, msplit, mexp, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform(whiten)");
     k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), 1), 256, 0, st>>>(Cm, C, 1, 1, 1.f, 0, zeros, mean_s,
                                                                          reinterpret_cast<__half*>(sp + SL.cmsplit),
+                                                                         reinterpret_cast<int*>(sp + SL.cmexp),
                                                                          reinterpret_cast<float*>(sp + SL.cbias));
     WCTB_CHECK_LAUNCH("k_finalize_transform(colour)");
-    rc = launch_conv_tc(CONV_APPLY, style, 1, Hs, Ws, C, msplit, 1, nullptr, bias, C, 0, feat, st);
+    rc = launch_conv_apply(style, 1, Hs, Ws, C, msplit, 1, mexp, bias, feat, st);
     if (rc) return rc;
     k_swap_tap_norms<<<dim3((unsigned)cdiv(C, 256), (unsigned)(patch * patch)), 256, 0, st>>>(feat, gs, q, norms);
     WCTB_CHECK_LAUNCH("k_swap_tap_norms");
@@ -2638,6 +2662,7 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
     float* dvec = reinterpret_cast<float*>(w + L.dvec);
     float* Wcm = reinterpret_cast<float*>(w + L.Wc);
     __half* msplit = reinterpret_cast<__half*>(w + L.Msplit);
+    int* mexp = reinterpret_cast<int*>(w + L.Mexp);
     float* bias = reinterpret_cast<float*>(w + L.bias);
     float* conv = reinterpret_cast<float*>(w + L.conv);
     int* kc = reinterpret_cast<int*>(w + L.kcount);
@@ -2660,9 +2685,9 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
     if (rc) return rc;
     k_outer_gemm<<<dim3((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc), 256, 0, st>>>(G, CC, G, CC, dvec, C, Wcm, CC, C);   // W_c
     WCTB_CHECK_LAUNCH("k_outer_gemm(whiten)");
-    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), (unsigned)Nc), 256, 0, st>>>(Wcm, C, Nc, 1, 1.f, 0, mean, zeros, msplit, bias);
+    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), (unsigned)Nc), 256, 0, st>>>(Wcm, C, Nc, 1, 1.f, 0, mean, zeros, msplit, mexp, bias);
     WCTB_CHECK_LAUNCH("k_finalize_transform(whiten)");
-    rc = launch_conv_tc(CONV_APPLY, content, Nc, Hc, Wc, C, msplit, Nc, nullptr, bias, C, 0, wc_feat, st);
+    rc = launch_conv_apply(content, Nc, Hc, Wc, C, msplit, Nc, mexp, bias, wc_feat, st);
     if (rc) return rc;
     // every style patch is a filter: the P x P correlation of all frames (top-left anchored, all positions; the strided VALID
     // subset is read by the arg-max) runs on the tensor-core conv kernel, `cols` filters (rows n0.. of the state's filter
@@ -2683,8 +2708,8 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
     k_swap_gather<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(reinterpret_cast<const __half*>(sp + SL.feat), gs, q,
                                                                                      idx, gc, ss_feat);
     WCTB_CHECK_LAUNCH("k_swap_gather");
-    rc = launch_conv_tc(CONV_APPLY, ss_feat, Nc, Hc, Wc, C, reinterpret_cast<const __half*>(sp + SL.cmsplit), 1, nullptr,
-                        reinterpret_cast<const float*>(sp + SL.cbias), C, 0, tmp, st);
+    rc = launch_conv_apply(ss_feat, Nc, Hc, Wc, C, reinterpret_cast<const __half*>(sp + SL.cmsplit), 1,
+                        reinterpret_cast<const int*>(sp + SL.cmexp), reinterpret_cast<const float*>(sp + SL.cbias), tmp, st);
     if (rc) return rc;
     k_blend2<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(tmp, content, gc, alpha, 1.f - alpha, out);   // ops.py:210
     WCTB_CHECK_LAUNCH("k_blend2");
