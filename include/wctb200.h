@@ -433,6 +433,28 @@ WCTB200_API int wctb200_style_swap_apply(const void* content, int Nc, int Hc, in
  * patches: about 1.1 GB of scores per frame in one chunk).
  */
 WCTB200_API size_t wctb200_style_swap_apply_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride);
+/*
+ * Labelled style swap (DESIGN.md §3.3.13; neural doodle): wctb200_style_swap_apply in which each content anchor draws only
+ * on the style patches that carry its own label.  content_labels: device uint8 [Ncl][Hm][Wm], Ncl in {1, Nc} (1: every
+ * frame shares the map); style_labels: device uint8 [Hms][Wms], the labels of the state's style.  Maps of any resolution
+ * (1..32768 per side) are sampled onto the content / style feature grids by the rule of wctb200_labels_resize_nearest.  With
+ * o = (patch-1)/2, patch n = py*pcol + px carries the style label at (py*stride + o, px*stride + o), and the anchor (y, x)
+ * of frame i the content label at (y*stride + o, x*stride + o).  The anchor takes the first maximum of its scores over the
+ * patches of its label, or over every patch when no patch carries that label.  Labels are compared for equality only.
+ *   label_buf: device scratch of wctb200_style_swap_labels_workspace_bytes(Ncl, Hc, Wc, Hs, Ws, patch, stride) bytes (0 for
+ *   a bad geometry) for the sampled maps and the patch labels, separate from ws, which is sized and chunked exactly as for
+ *   wctb200_style_swap_apply.  A smaller label_buf is WCTB200_EWS; the other errors are wctb200_style_swap_apply's.
+ * Identities: with one label everywhere (or any labelling in which every anchor may take every patch) the output and k_out
+ * are byte-identical to wctb200_style_swap_apply's; every workspace size from the minimum up gives the same bytes; frame i
+ * of an apply is bit-identical to the apply of that frame alone with its own map.
+ */
+WCTB200_API size_t wctb200_style_swap_labels_workspace_bytes(int Ncl, int Hc, int Wc, int Hs, int Ws, int patch, int stride);
+WCTB200_API int wctb200_style_swap_apply_labels(const void* content, int Nc, int Hc, int Wc, int C, const void* state,
+                                    int Hs, int Ws, int patch, int stride, float alpha, float eps_cov, float thresh,
+                                    const uint8_t* content_labels, int Ncl, int Hm, int Wm,
+                                    const uint8_t* style_labels, int Hms, int Wms,
+                                    void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* label_buf, size_t label_bytes,
+                                    void* stream);
 
 /* ---- multimodal style transfer (DESIGN.md §3.3.10; mst.cu) ----------------
  * Spherical k-means of one style feature (SPF16 [1,Hs,Ws,C], C in {64,128,256,512}) into K in 1..8 clusters of the unit

@@ -48,6 +48,12 @@ channel of the style, by rank, instead of matching only its covariance (DESIGN.m
 even wash with the same statistics stylise differently.  It suits ``--noise`` texture synthesis.  Output names are
 unchanged.
 
+Labelled style swap (neural doodle): ``--swap-labels CONTENT_MAP STYLE_MAP`` with ``--swap5`` / ``--swap-targets`` gives
+the content and the style each a flat-colour label map (RGB or grey PNG, any resolution); every content patch is then
+rebuilt only from style patches of the same colour, or from all of them where the style has none (DESIGN.md §3.3.13).  The
+distinct colours of both maps together, sorted by their packed 24-bit value, are the labels.  It takes one style file and
+one content file or ``--noise`` (every noise frame shares the map), and no ``--crop-size``.  Output names are unchanged.
+
 Which of these options combine is decided by one table, ``wct_tf_b200/options.py``; a rejected combination is a parser error
 naming both flags.
 
@@ -115,6 +121,9 @@ _FLAGS = [
                                help="with --content-mask: feather the region edges by a Gaussian of SIGMA mask pixels")),
     (("--mask-weights",), dict(nargs="+", type=str, default=None, metavar="W",
                                help="one 8-bit grayscale soft weight map per --mask-styles entry, in place of --content-mask")),
+    (("--swap-labels",), dict(nargs=2, type=str, default=None, metavar=("CONTENT_MAP", "STYLE_MAP"),
+                              help="with --swap5 / --swap-targets: flat-colour label maps of the content and the style; each "
+                                   "content patch takes only style patches of its own colour")),
     # webcam.py:38; the three --noise-* flags are not in the reference.  Their defaults are filled in by parse_args, so that
     # giving one without --noise can be told from leaving it out.
     (("--noise",), dict(action="store_true", default=False, help="Synthesize textures from noise images")),
@@ -159,6 +168,7 @@ def parse_args(argv=None):
     check_style_mask_flags(parser, args)
     check_noise_flags(parser, args)
     check_prepared_flags(parser, args)
+    check_swap_label_flags(parser, args)
     return args
 
 
@@ -174,6 +184,43 @@ def check_swap_flags(parser, args):
 
 
 MST_SMOOTH_DEFAULT = 0.05
+
+
+def read_label_maps(content_map, style_map):
+    """Two flat-colour label map files -> uint8 labels (content [H,W], style [H',W']): the distinct colours of both maps
+    together, sorted by their packed 24-bit RGB value, become labels 0..K-1.  ValueError for more than 256 colours."""
+    from PIL import Image
+    packed = []
+    for path in (content_map, style_map):
+        rgb = np.asarray(Image.open(path).convert("RGB"), dtype=np.uint32)
+        packed.append((rgb[..., 0] << 16) | (rgb[..., 1] << 8) | rgb[..., 2])
+    colours, inverse = np.unique(np.concatenate([p.ravel() for p in packed]), return_inverse=True)
+    if len(colours) > 256:
+        raise ValueError("%d colours in the two label maps, at most 256: label maps must be flat colours (PNG, not JPEG)"
+                         % len(colours))
+    labels = inverse.astype(np.uint8)
+    n = packed[0].size
+    return labels[:n].reshape(packed[0].shape), labels[n:].reshape(packed[1].shape)
+
+
+def check_swap_label_flags(parser, args):
+    """--swap-labels CONTENT_MAP STYLE_MAP: needs --swap5 / --swap-targets, one --style-path file (image or .wctstyle; no
+    folder, no -r), one --content-path file or --noise, and no --crop-size (a crop would cut the style but not its map).
+    The maps are read here (``read_label_maps``) into ``args.swap_label_maps``."""
+    if args.swap_labels is None:
+        return
+    if not (args.swap5 or args.swap_targets is not None):
+        parser.error("--swap-labels needs --swap5 or --swap-targets")
+    if not args.style_path or os.path.isdir(args.style_path) or args.random:
+        parser.error("--swap-labels needs one --style-path file (no folder, no -r/--random)")
+    if not args.noise and (not args.content_path or os.path.isdir(args.content_path)):
+        parser.error("--swap-labels needs one --content-path file or --noise")
+    if args.crop_size:
+        parser.error("--swap-labels takes no --crop-size")
+    try:
+        args.swap_label_maps = read_label_maps(*args.swap_labels)
+    except (OSError, ValueError) as e:
+        parser.error("--swap-labels: %s" % e)
 
 
 def check_values(parser, args):
@@ -419,6 +466,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
     if args.efdm:
         kw["efdm"] = True
+    if getattr(args, "swap_labels", None):
+        kw["swap_labels"] = args.swap_label_maps
     kw.update(soft_kw(args))
     result = model.predict_batch(content_dev, style_dev, **kw)
     for _ in range(args.passes - 1):

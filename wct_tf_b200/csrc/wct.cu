@@ -2434,14 +2434,38 @@ __global__ void k_swap_patch_weights(const __half* __restrict__ feat, ActGeom g,
         wsplit[total + i] = lo;
     }
 }
+// Labels of a labelled swap (DESIGN.md §3.3.13): the content and style label maps sampled onto their feature grids
+// (k_labels_resize), patch n's label l(n) = Ls'[py*S + o][px*S + o] with o = (P-1)/2, and the 256-bit set of labels some
+// patch carries.  An anchor whose label no patch carries may take any patch.
+struct SwapLabels {
+    const uint8_t* clab;        // sampled content labels [Ncl][Hc][Wc]
+    long long clab_frame;       // frame stride of clab: Hc*Wc, or 0 when every frame shares one map
+    const uint8_t* plab;        // l(n) for n < n_patches
+    const uint32_t* present;    // [8]: bit l of word l/32 set when some patch carries label l
+};
+// l(n) of every patch and the present set (order-independent atomicOr into zeroed words); one thread per patch
+__global__ void k_swap_patch_labels(const uint8_t* __restrict__ slab, int Ws, SwapGeom q, int n_patches, uint8_t* __restrict__ plab,
+                                    uint32_t* __restrict__ present) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_patches) return;
+    const int o = (q.P - 1) / 2;
+    const int py = i / q.pcol, px = i - py * q.pcol;
+    const uint8_t l = slab[(long long)(py * q.S + o) * Ws + px * q.S + o];
+    plab[i] = l;
+    atomicOr(&present[l >> 5], 1u << (l & 31));
+}
 // first arg-max over the patch axis for every VALID strided position (y,x) of frame blockIdx.y: the top-left-anchored P x P
 // correlation at interior pixel (y*S, x*S), which the conv kernel stored at that pixel's own padded cell.  A VALID anchor
 // reads padded rows y*S+1 .. y*S+P <= H of its own frame only, so a batch of frames in one correlation keeps them apart.
 // The scores hold the chunk of patches [n0, n0 + g.C) (g.C = the chunk's width); patches >= n_patches are padding.  The
 // first chunk (n0 = 0) sets (best, idx); a later one replaces them only where its own first maximum is strictly greater,
 // so after the last chunk idx is the first maximum over all patches, whatever the chunking.
+// LABELS: only the patches of the anchor's own label are candidates (all of them when no patch carries it); a skipped
+// patch's score is never loaded.  A chunk without a candidate leaves (-inf, sentinel), which the first chunk may store and
+// any later candidate replaces, so idx ends as a real patch: every anchor has at least one candidate overall.
+template <bool LABELS>
 __global__ void k_swap_argmax(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n0, int n_patches,
-                              float* __restrict__ best_run, int* __restrict__ idx) {
+                              float* __restrict__ best_run, int* __restrict__ idx, SwapLabels lab) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= q.ho * q.wo) return;
     const int n = blockIdx.y;
@@ -2450,9 +2474,20 @@ __global__ void k_swap_argmax(const __half* __restrict__ scores, ActGeom g, Swap
     const int cols = min(g.C, n_patches - n0);
     float best = -INFINITY;
     int bi = 0x7fffffff;
-    for (int j = lane; j < cols; j += 32) {
-        const float v = merge_f32(scores[pos * g.C + j], scores[g.plane + pos * g.C + j]);
-        if (v > best) { best = v; bi = n0 + j; }                  // strictly greater: keeps the first maximum of this lane
+    if constexpr (LABELS) {
+        const int o = (q.P - 1) / 2;
+        const int l = lab.clab[n * lab.clab_frame + (long long)(y * q.S + o) * g.W + x * q.S + o];
+        const bool any = ((lab.present[l >> 5] >> (l & 31)) & 1u) == 0u;
+        for (int j = lane; j < cols; j += 32) {
+            if (!any && lab.plab[n0 + j] != l) continue;
+            const float v = merge_f32(scores[pos * g.C + j], scores[g.plane + pos * g.C + j]);
+            if (v > best) { best = v; bi = n0 + j; }
+        }
+    } else {
+        for (int j = lane; j < cols; j += 32) {
+            const float v = merge_f32(scores[pos * g.C + j], scores[g.plane + pos * g.C + j]);
+            if (v > best) { best = v; bi = n0 + j; }              // strictly greater: keeps the first maximum of this lane
+        }
     }
 #pragma unroll
     for (int o = 16; o >= 1; o >>= 1) {
@@ -2616,11 +2651,42 @@ int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int pa
     return 0;
 }
 
+// the label buffer of a labelled apply (256-byte aligned blocks): sampled content labels [Ncl][Hc][Wc] | sampled style labels
+// [Hs][Ws] | l(n) [n_patches] | present set uint32 [8].  Separate from the apply's workspace, whose layout and chunk policy
+// it leaves as they are.
+struct SwapLabelWs {
+    size_t clab, slab, plab, present, total;
+};
+static SwapLabelWs swap_labels_layout(int Ncl, int Hc, int Wc, int Hs, int Ws, int n_patches) {
+    SwapLabelWs L;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    L.clab = take((size_t)Ncl * Hc * Wc);
+    L.slab = take((size_t)Hs * Ws);
+    L.plab = take((size_t)n_patches);
+    L.present = take(8 * sizeof(uint32_t));
+    L.total = o;
+    return L;
+}
+size_t style_swap_labels_workspace_bytes(int Ncl, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    return swap_labels_layout(Ncl, Hc, Wc, Hs, Ws, swap_state_layout(64, Hs, Ws, P, S).n_patches).total;
+}
+// the label maps of a labelled apply as given: content [Ncl][Hm][Wm] (Ncl in {1, Nc}), style [Hms][Wms]
+struct SwapLabelMaps {
+    const uint8_t* content;
+    int Ncl, Hm, Wm;
+    const uint8_t* style;
+    int Hms, Wms;
+    void* buf;
+    size_t buf_bytes;
+};
+
 // Content side over Nc frames against one prepared style: whiten every frame with its own W_c (ops.py:187), correlate all
-// frames with the shared patch filters in one launch, arg-max and gather per frame, colour with the style, blend.
-int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
-                            int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
-                            cudaStream_t st) {
+// frames with the shared patch filters in one launch, arg-max and gather per frame, colour with the style, blend.  With
+// `maps` the arg-max is the labelled one (DESIGN.md §3.3.13); everything else is the same launch for launch.
+static int style_swap_apply_impl(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
+                                 int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws,
+                                 size_t ws_bytes, const SwapLabelMaps* maps, cudaStream_t st) {
     int rc = swap_check_style(C, Hs, Ws, patch, stride);
     if (rc) return rc;
     WCTB_REQUIRE(Nc >= 1 && Hc >= patch && Wc >= patch && Hc >= 2 && Wc >= 2,
@@ -2632,6 +2698,19 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
     WCTB_REQUIRE((AL.ho - 1) * stride + patch == Hc && (AL.wo - 1) * stride + patch == Wc,
                  "style_swap: patch %d / stride %d does not tile a %dx%d encoding (refit the content: swap_filter_fit, wct.py:84-90)",
                  patch, stride, Hc, Wc);
+    SwapLabels lab = {nullptr, 0, nullptr, nullptr};
+    SwapLabelWs LL = {};
+    if (maps) {
+        WCTB_REQUIRE(maps->content && maps->style && maps->buf, "style_swap_apply_labels: null pointer");
+        WCTB_REQUIRE((maps->Ncl == 1 || maps->Ncl == Nc) && maps->Hm >= 1 && maps->Wm >= 1 && maps->Hms >= 1 && maps->Wms >= 1,
+                     "style_swap_apply_labels: %d content label maps of %dx%d for %d frames, style labels %dx%d", maps->Ncl,
+                     maps->Hm, maps->Wm, Nc, maps->Hms, maps->Wms);
+        LL = swap_labels_layout(maps->Ncl, Hc, Wc, Hs, Ws, SL.n_patches);
+        if (maps->buf_bytes < LL.total) {
+            set_error("style_swap_apply_labels: label buffer %zu < %zu bytes", maps->buf_bytes, LL.total);
+            return WCTB200_EWS;
+        }
+    }
     // chunk width: all cout_pad patches when the workspace holds their scores, else the largest multiple of the whole
     // correlation's N tile that fits (the same tile, hence the same kernel variant and k order, for every chunk)
     const int BN = conv_tc_bn(SL.cout_pad);
@@ -2696,13 +2775,29 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
     const __half* wsplit = reinterpret_cast<const __half*>(sp + SL.wsplit);
     float* best_run = reinterpret_cast<float*>(tmp);
     const int npos = AL.ho * AL.wo;
+    if (maps) {
+        uint8_t* lb = static_cast<uint8_t*>(maps->buf);
+        rc = launch_labels_resize(maps->content, maps->Ncl, maps->Hm, maps->Wm, Hc, Wc, lb + LL.clab, st);
+        if (rc) return rc;
+        rc = launch_labels_resize(maps->style, 1, maps->Hms, maps->Wms, Hs, Ws, lb + LL.slab, st);
+        if (rc) return rc;
+        uint32_t* present = reinterpret_cast<uint32_t*>(lb + LL.present);
+        WCTB_CUDA(cudaMemsetAsync(present, 0, 8 * sizeof(uint32_t), st));
+        k_swap_patch_labels<<<(unsigned)cdiv(SL.n_patches, 256), 256, 0, st>>>(lb + LL.slab, Ws, q, SL.n_patches, lb + LL.plab,
+                                                                                present);
+        WCTB_CHECK_LAUNCH("k_swap_patch_labels");
+        lab = {lb + LL.clab, maps->Ncl == 1 ? 0ll : (long long)Hc * Wc, lb + LL.plab, present};
+    }
     for (int n0 = 0; n0 < SL.cout_pad; n0 += cols) {
         const int m = SL.cout_pad - n0 < cols ? SL.cout_pad - n0 : cols;
         rc = launch_conv_taps_rows(wc_feat, Nc, Hc, Wc, C, wsplit + (long long)n0 * K, (long long)SL.cout_pad * K, m, BN, scores, st,
                                    patch);
         if (rc) return rc;
-        k_swap_argmax<<<dim3((unsigned)cdiv((long long)npos * 32, 256), (unsigned)Nc), 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m),
-                                                                                                    q, n0, SL.n_patches, best_run, idx);
+        const dim3 grid((unsigned)cdiv((long long)npos * 32, 256), (unsigned)Nc);
+        if (maps)
+            k_swap_argmax<true><<<grid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, SL.n_patches, best_run, idx, lab);
+        else
+            k_swap_argmax<false><<<grid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, SL.n_patches, best_run, idx, lab);
         WCTB_CHECK_LAUNCH("k_swap_argmax");
     }
     k_swap_gather<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(reinterpret_cast<const __half*>(sp + SL.feat), gs, q,
@@ -2719,6 +2814,20 @@ int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C
         WCTB_CUDA(cudaMemcpyAsync(k_out + Nc, sp + SL.k, 4, cudaMemcpyDeviceToDevice, st));
     }
     return 0;
+}
+int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
+                            int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
+                            cudaStream_t st) {
+    return style_swap_apply_impl(content, Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, out, k_out, ws,
+                                 ws_bytes, nullptr, st);
+}
+int launch_style_swap_apply_labels(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws,
+                                   int patch, int stride, float alpha, float eps_cov, float thresh, const uint8_t* content_labels,
+                                   int Ncl, int Hm, int Wm, const uint8_t* style_labels, int Hms, int Wms, __half* out,
+                                   int32_t* k_out, void* ws, size_t ws_bytes, void* label_buf, size_t label_bytes, cudaStream_t st) {
+    const SwapLabelMaps maps = {content_labels, Ncl, Hm, Wm, style_labels, Hms, Wms, label_buf, label_bytes};
+    return style_swap_apply_impl(content, Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, out, k_out, ws,
+                                 ws_bytes, &maps, st);
 }
 
 int launch_style_swap_level(const __half* content, int Hc, int Wc, const __half* style, int Hs, int Ws, int C, int patch, int stride,

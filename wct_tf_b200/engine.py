@@ -48,6 +48,12 @@ class Act(object):
         return self.buf.data_ptr()
 
 
+def _frame_labels(swap_labels, lo, hi):
+    """The (content, style) label maps of frames lo..hi of a labelled swap: a stack of one map per frame is sliced, a
+    shared map [1,...] is kept."""
+    return tuple(t if t.shape[0] == 1 else t[lo:hi] for t in swap_labels)
+
+
 def _soft_slice(soft, lo, hi):
     """The maps of a soft spatial-control call (strength, weights) for frames [lo, hi)."""
     if soft is None:
@@ -359,8 +365,10 @@ class Engine(object):
                    int(stride), sem["eps_cov"], sem["thresh"], state.data_ptr(), None, ws.data_ptr(), ws.numel(), st)
         return state
 
-    def swap_apply(self, content, state, style_hw, ss_alpha, want_info=False, patch=3, stride=1):
-        """wct_style_swap (ops.py:145-217) of the N content frames against one prepared style (``swap_prepare``)."""
+    def swap_apply(self, content, state, style_hw, ss_alpha, want_info=False, patch=3, stride=1, labels=None):
+        """wct_style_swap (ops.py:145-217) of the N content frames against one prepared style (``swap_prepare``).
+        ``labels``: (content labels cuda uint8 [1|N,Hm,Wm], style labels cuda uint8 [1,Hm',Wm']) of a labelled swap
+        (DESIGN.md §3.3.13), each anchor matched only to the style patches of its own label."""
         st = self._stream()
         C, N = content.C, content.N
         Hs, Ws = style_hw
@@ -376,10 +384,23 @@ class Engine(object):
         ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         kbuf = torch.empty(N + 1, dtype=torch.int32, device=self.device) if want_info else None
         sem = SEMANTICS["tf"]
-        self._call("style_swap[C%d]" % C, 11, self.lib.wctb200_style_swap_apply, content.ptr, N, content.H, content.W, C,
-                   state.data_ptr(), Hs, Ws, int(patch), int(stride), float(ss_alpha), sem["eps_cov"], sem["thresh"], out.ptr,
-                   kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel(), st)
-        ws.record_stream(torch.cuda.current_stream(self.device))   # freed by the caching allocator only after this stream is done
+        cur = torch.cuda.current_stream(self.device)
+        if labels is None:
+            self._call("style_swap[C%d]" % C, 11, self.lib.wctb200_style_swap_apply, content.ptr, N, content.H, content.W, C,
+                       state.data_ptr(), Hs, Ws, int(patch), int(stride), float(ss_alpha), sem["eps_cov"], sem["thresh"], out.ptr,
+                       kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel(), st)
+        else:
+            cl, sl = (t.contiguous() for t in labels)
+            lbuf = torch.empty(self.lib.wctb200_style_swap_labels_workspace_bytes(cl.shape[0], content.H, content.W, Hs, Ws,
+                                                                                  int(patch), int(stride)),
+                               dtype=torch.uint8, device=self.device)
+            self._call("style_swap_labels[C%d]" % C, 14, self.lib.wctb200_style_swap_apply_labels, content.ptr, N, content.H,
+                       content.W, C, state.data_ptr(), Hs, Ws, int(patch), int(stride), float(ss_alpha), sem["eps_cov"],
+                       sem["thresh"], cl.data_ptr(), cl.shape[0], cl.shape[1], cl.shape[2], sl.data_ptr(), sl.shape[-2],
+                       sl.shape[-1], out.ptr, kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel(),
+                       lbuf.data_ptr(), lbuf.numel(), st)
+            lbuf.record_stream(cur)
+        ws.record_stream(cur)   # freed by the caching allocator only after this stream is done
         return out, kbuf
 
     def style_swap(self, content, style, ss_alpha, want_info=False, patch=3, stride=1):
@@ -756,7 +777,7 @@ class Engine(object):
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
                 region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05, strength_map=None,
-                content_weights=None, mask_feather=None, efdm=False):
+                content_weights=None, mask_feather=None, efdm=False, swap_labels=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -791,6 +812,9 @@ class Engine(object):
 
         Style swap at any level: ``swap_targets`` is a list of relu targets at which the style swap replaces WCT / AdaIN,
         with ``ss_alpha``, ``ss_patch_size`` and ``ss_stride``; ``swap5`` is ``swap_targets=["relu5_1"]``.
+        ``swap_labels`` = (content labels, style labels), cuda uint8 [1|N,Hm,Wm] and [1|Ns,Hm',Wm'] of any resolution,
+        makes every swap level a labelled swap (DESIGN.md §3.3.13): each content patch draws only on the style patches of
+        its own label, or on all of them when the style has none of that label.  The other levels are unchanged.
 
         Optimal-transport transform: ``ost=True`` matches each level's content Gaussian to the style's by the Monge map
         (DESIGN.md §3.3.8) instead of WCT, against the same WCT style states; swap levels still swap.
@@ -869,6 +893,13 @@ class Engine(object):
         if seamless is not None:
             check_seamless(seamless, content_u8.shape[1], content_u8.shape[2], self.model.relu_targets)
         swap_lv = self.swap_levels(swap5, swap_targets)
+        if swap_labels is not None:
+            n_sty = style_u8.n if isinstance(style_u8, PreparedStyle) else style_u8.shape[0]
+            cl, sl = options.check_swap_labels(swap_labels, bool(swap_lv), N, n_sty)
+            for t in (cl, sl):
+                if not isinstance(t, torch.Tensor) or t.device != self.device:
+                    raise ValueError("swap_labels must be uint8 tensors on %s" % self.device)
+            swap_labels = (cl.contiguous(), sl.contiguous())
         if interp_styles is not None:
             K = len(interp_styles)
             if not 1 <= K <= 8:
@@ -904,7 +935,9 @@ class Engine(object):
             # one style per frame: frame by frame (each frame's swap has its own style side)
             outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
                                  alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
-                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm) for i in range(N)]
+                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm,
+                                 swap_labels=None if swap_labels is None else _frame_labels(swap_labels, i, i + 1))
+                    for i in range(N)]
             return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
         swap = (int(ss_patch_size), int(ss_stride), swap_lv) if swap_lv else None
@@ -928,11 +961,13 @@ class Engine(object):
                 else:
                     sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
                 return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
-                                         seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm)
+                                         seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm,
+                                         swap_labels=None if swap_labels is None else _frame_labels(swap_labels, lo, hi))
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
-                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft, efdm=efdm)
+                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft, efdm=efdm,
+                                    swap_labels=swap_labels)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -1216,12 +1251,13 @@ class Engine(object):
         return ps.swap[key]
 
     def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
-                     seamless=None, soft=None, efdm=False):
+                     seamless=None, soft=None, efdm=False, swap_labels=None):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
         ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
         optimal-transport transform instead of WCT at the other levels, ``efdm`` exact feature distribution matching;
         ``seamless``: the wrapped axes of the content path
-        (the transforms write a reflect halo, which is rewritten before the decoder reads it)."""
+        (the transforms write a reflect halo, which is rewritten before the decoder reads it); ``swap_labels``: the (content
+        [1|N], style [1]) label maps of a labelled swap at the swap levels."""
         wrap = self.wrap_flags(seamless)
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
@@ -1251,7 +1287,7 @@ class Engine(object):
                 state, ev = style.swap[(relu,) + swap[:2]]
                 main.wait_event(ev)
                 sf = style.feats[relu]
-                f, kbuf = self.swap_apply(cf, state, (sf.H, sf.W), ss_alpha, want_info, *swap[:2])
+                f, kbuf = self.swap_apply(cf, state, (sf.H, sf.W), ss_alpha, want_info, *swap[:2], labels=swap_labels)
             else:
                 for sd in sides:
                     if sd.side is not main:

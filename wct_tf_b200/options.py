@@ -3,6 +3,10 @@
 This is the one statement of that policy.  ``WCT.predict_batch``, ``Engine.stylize`` / ``stylize_tiled`` and the flags of
 ``stylize.py`` / ``stylize_video.py`` each map their arguments to a set of the canonical option names below and call
 ``check`` with their vocabulary, so that every caller accepts the same combinations and names them in its own words.
+
+``swap_labels`` (the labelled style swap, ``check_swap_labels``) has no entry in ``SPELLINGS``: it is a parameter of
+``swap``, as ``mst_smooth`` is of ``mst``.  It needs the swap, and through it takes the swap's exclusions; it adds none of
+its own.
 """
 import numpy as np
 
@@ -94,6 +98,36 @@ def check_mst(K, lam, names=("mst", "mst_smooth")):
     if not np.isfinite(lam_f) or lam_f < 0:
         raise ValueError("%s must be finite and >= 0, got %r" % (names[1], lam))
     return int(K), lam_f
+
+
+def _label_map(a, name, counts):
+    """One uint8 label map [Hm,Wm] or stack [n,Hm,Wm] with n in ``counts``, numpy or torch; returned as [n,Hm,Wm]."""
+    if not (hasattr(a, "dtype") and hasattr(a, "shape") and hasattr(a, "ndim")):
+        a = np.asarray(a)
+    if str(a.dtype) not in ("uint8", "torch.uint8"):
+        raise ValueError("%s must be uint8 labels, got %s" % (name, a.dtype))
+    if a.ndim == 2:
+        a = a[None]
+    if a.ndim != 3 or a.shape[0] not in counts:
+        raise ValueError("%s must be [Hm,Wm] or [N,Hm,Wm] with N = %s, got shape %s"
+                         % (name, " or ".join(str(c) for c in sorted(set(counts))), tuple(a.shape)))
+    if a.shape[1] < 1 or a.shape[2] < 1:
+        raise ValueError("%s must not be empty, got %s" % (name, tuple(a.shape)))
+    return a
+
+
+def check_swap_labels(swap_labels, swap, n_frames, n_styles=1, names=("swap_labels", "swap5 / swap_targets")):
+    """The label maps of a labelled style swap (DESIGN.md §3.3.13): a pair (content labels [Hm,Wm] or [N,Hm,Wm], style
+    labels [Hm',Wm'], or [N,Hm',Wm'] with one style per frame), uint8, numpy or torch.  ``swap``: whether the call swaps at
+    any level.  Returns (content [1|N,Hm,Wm], style [1|Ns,Hm',Wm']) as given, with the frame axis added; ValueError
+    otherwise, before any device work."""
+    if not swap:
+        raise ValueError("%s needs %s: the labels steer the style swap" % names)
+    if not isinstance(swap_labels, (tuple, list)) or len(swap_labels) != 2:
+        raise ValueError("%s must be a pair (content labels, style labels)" % names[0])
+    content = _label_map(swap_labels[0], names[0] + " content labels", (1, n_frames))
+    style = _label_map(swap_labels[1], names[0] + " style labels", (1, n_styles))
+    return content, style
 
 
 def check_tile_size(tile_size, name="tile_size"):

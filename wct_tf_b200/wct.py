@@ -26,7 +26,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``mst`` is new: multimodal style transfer (Zhang, Zhu & Zhu, ICCV 2019), each level's style clustered into K modes
     and every content pixel matched to one, so regions pair up without masks;
   * ``efdm`` is new: exact feature distribution matching (Zhang et al., CVPR 2022), every channel's values given the
-    style's by rank.
+    style's by rank;
+  * ``swap_labels`` is new: the labelled style swap (neural doodle, Champandard 2016), each content patch matched only to
+    style patches of its own label.
 """
 from __future__ import annotations
 
@@ -268,7 +270,7 @@ class WCT(object):
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
                       swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
-                      strength_map=None, content_weights=None, mask_feather=None, efdm=False):
+                      strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -345,7 +347,15 @@ class WCT(object):
         content values are ranked, value rank r takes the style's quantile at r, and equal values take the mean of their
         ranks' quantiles.  Sparse bright strokes and an even wash with the same statistics then stylise differently.
         ``efdm=False`` changes nothing.  The style is sorted once per call however many ``passes``; with the style swap,
-        the swap levels swap in the first pass and the others use EFDM."""
+        the swap levels swap in the first pass and the others use EFDM.
+
+        ``swap_labels`` (labelled style swap, DESIGN.md §3.3.13; with ``swap5`` / ``swap_targets``): a pair (content
+        labels, style labels) of uint8 label maps, numpy or torch, host or device: content [Hm,Wm] or [N,Hm,Wm]; style
+        [Hm',Wm'] for a shared style, or with one style per frame [Hm',Wm'] or [N,Hm',Wm'].  At every swap level each content
+        patch draws only on the style patches with its own label ("water here, trees there"); where the style has no patch
+        of that label it draws on all of them.  Maps of any resolution are sampled onto each level's feature grids.  With a
+        stride the content is cropped as for the swap, and a content map of exactly the content's size is cropped with it
+        (any other size is stretched over the image as stylised).  Labels act in the first pass only, like the swap."""
         prepared = isinstance(styles, PreparedStyle)
         per_frame = not prepared and (isinstance(styles, (list, tuple)) or np.ndim(styles) not in (3, 4)
                                       or (np.ndim(styles) == 4 and styles.shape[0] != 1))
@@ -370,6 +380,10 @@ class WCT(object):
         dev = eng.device
         n = 1 if np.ndim(contents) == 3 else contents.shape[0]
         eng.swap_levels(swap5, swap_targets)                 # ValueError for both, or a level that is not a target
+        if swap_labels is not None:
+            n_sty = styles.n if prepared else (len(styles) if isinstance(styles, (list, tuple))
+                                               else 1 if np.ndim(styles) == 3 else styles.shape[0])
+            swap_labels = options.check_swap_labels(swap_labels, swap5 or swap_targets is not None, n, n_sty)
         if style_weights is not None:
             weights, interp_styles = self.check_interp(style_weights, n, styles)
         if content_mask is not None:
@@ -398,10 +412,19 @@ class WCT(object):
             return eng.prepare_call(a, adain=adain, swap5=swap5, swap_targets=swap_targets, efdm=efdm) if int(passes) > 1 else a
 
         # wct.py:84-90: with a stride the filter may not fit; centre-crop the content (on the device) to a size it tiles
+        Hc0, Wc0 = contents.shape[-3], contents.shape[-2]
         with torch.cuda.device(dev):
             contents = self.swap_fit(contents, swap5, swap_targets, to_dev)
         with torch.cuda.device(dev):
             c = to_dev(contents)
+            lab_dev = None
+            if swap_labels is not None:
+                cl, sl = (t if isinstance(t, torch.Tensor) else torch.from_numpy(np.array(t, copy=True, order="C"))
+                          for t in swap_labels)
+                if tuple(cl.shape[1:]) == (Hc0, Wc0) and tuple(c.shape[1:3]) != (Hc0, Wc0):
+                    y0, x0 = (Hc0 - c.shape[1]) // 2, (Wc0 - c.shape[2]) // 2      # center_crop_to's window
+                    cl = cl[:, y0:y0 + c.shape[1], x0:x0 + c.shape[2]]
+                lab_dev = (cl.to(dev, non_blocking=True).contiguous(), sl.to(dev, non_blocking=True).contiguous())
             if smap is not None:
                 soft_kw["strength_map"] = smap.to(dev, non_blocking=True)
             if content_weights is not None:
@@ -461,7 +484,7 @@ class WCT(object):
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
                                        swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, efdm=efdm,
-                                       **soft_kw)
+                                       swap_labels=lab_dev if first else None, **soft_kw)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -578,7 +601,7 @@ class WCT(object):
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
                 style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
-                strength_map=None, content_weights=None, mask_feather=None, efdm=False):
+                strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
@@ -586,7 +609,7 @@ class WCT(object):
         path circularly, ``mst`` = K matches the content to K modes of the style and ``efdm`` matches every channel's whole
         value distribution to the style's; ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
-        (``predict_batch``).'''
+        (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap.'''
         s = time.time()
         seen = {}
 
@@ -603,7 +626,7 @@ class WCT(object):
                                  content_mask=content_mask, style_weights=style_weights, style_masks=style_masks,
                                  swap_targets=swap_targets, tile_size=tile_size, ost=ost, seamless=seamless, mst=mst,
                                  mst_smooth=mst_smooth, strength_map=strength_map, content_weights=content_weights,
-                                 mask_feather=mask_feather, efdm=efdm)
+                                 mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
