@@ -195,7 +195,7 @@ size_t wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws);
 int launch_wct_style_prepare_regions(const __half*, int, int, int, const uint8_t*, int, float, float, float, void*, int32_t*, void*,
                                      size_t, cudaStream_t);
 int launch_covariance_regions(const __half*, int, int, int, int, const uint8_t*, int, float, float*, float*, int*, cudaStream_t);
-int launch_jacobi(float*, int, int, float*, int*, cudaStream_t, const int* skip);
+int launch_jacobi(float*, int, int, float*, int*, cudaStream_t, const int* skip, float thresh);
 int launch_eig_post(const float*, const float*, float*, int, int, float, float, int, float*, float*, int*, cudaStream_t, const int* skip);
 extern int g_conv_bn_override;
 extern int g_conv_oversub;
@@ -594,7 +594,7 @@ int wctb200_jacobi_eigh(float* a, int C, int count, float* sigma, int32_t* sweep
     float* a0 = scratch + (size_t)count * 16;
     float* lam = a0 + nmat;
     cudaError_t ce = cudaMemcpyAsync(a0, a, nmat * sizeof(float), cudaMemcpyDeviceToDevice, ST(stream));
-    int rc = ce == cudaSuccess ? launch_jacobi(a, C, count, conv, sweeps, ST(stream), nullptr) : cuda_fail(ce, "cudaMemcpyAsync");
+    int rc = ce == cudaSuccess ? launch_jacobi(a, C, count, conv, sweeps, ST(stream), nullptr, 0.f) : cuda_fail(ce, "cudaMemcpyAsync");
     if (!rc) rc = launch_eig_post(a, a0, lam, C, count, 0.f, 0.f, count, sigma, nullptr, nullptr, ST(stream), nullptr);
     return rc;
 }

@@ -28,11 +28,14 @@ __device__ __forceinline__ float rcp_ap(float x) {
 //     is orthonormal, an inexact t only leaves a residual for the next sweep;
 //   * (c,s): r = h^-1/2 refined by one Newton step, s = t r, and c is applied as 1 + cm1 with
 //     cm1 = -s^2/(1+r), so that small angles neither shrink nor grow the columns (no eigenvalue bias).
-//   * a pair whose columns are BOTH at the rounding-noise floor (|col|^2 < null2 = 1e-11 max|col|^2 of the previous sweep)
-//     is left alone and not counted: such columns span the null space of a rank-deficient map, their mutual cosines
-//     are O(1) noise that never converges (26 sweeps instead of 13 on a rank-299 512x512 matrix), and their
-//     directions inside the null space do not matter.  Pairs of a noise column with a live column are still rotated:
-//     that is what keeps the noise columns' Rayleigh quotients second-order small.
+//   * a pair whose columns are BOTH at the rounding-noise floor (|col|^2 < null2 of the previous sweep, k_jacobi:
+//     |col| < min(3.16e-6 max|col|, max(thresh / 2, 16 * 2^-24 max|col|))) is left alone and not counted: such columns
+//     span the null space of a rank-deficient map, their mutual cosines are O(1) noise that never converges (26 sweeps
+//     instead of 13 on a rank-299 512x512 matrix), and their directions inside the null space do not matter.  What the
+//     floor guarantees: a kept column (|col| ~ lambda > thresh) is live whenever lambda > 16 * 2^-24 lambda_max, i.e.
+//     wherever fp32 determines its direction; the noise columns (~7 * 2^-24 lambda_max) are not.  Pairs of a noise
+//     column with a live column are still rotated: that is what keeps the noise columns' Rayleigh quotients
+//     second-order small.
 __device__ __forceinline__ void rot_scalars(float g, float a, float b, float tol2, float tolq2, float null2, float& flag,
                                             float& t, float& s, float& cm1) {
     const float ab = a * b, gg = g * g;

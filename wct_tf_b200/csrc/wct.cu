@@ -301,7 +301,7 @@ __device__ float g_jacobi_tolq = 1e-4f;   // predicted-convergence level (see k_
 template <int NN>
 __global__ void __launch_bounds__(512, 1)
 k_jacobi(float* __restrict__ Gall, float* __restrict__ conv_ws, int* __restrict__ sweeps_out, int max_sweeps, float tol,
-         int lg, int stagger, const int* __restrict__ skip) {
+         int lg, int stagger, const int* __restrict__ skip, float thresh) {
     if (skip && skip[blockIdx.y]) {          // matrix handled by the matrix-function fast path (matfun_tc.cu): whole cluster leaves
         if (blockIdx.x == 0 && threadIdx.x == 0 && sweeps_out) sweeps_out[blockIdx.y] = 0;
         return;
@@ -447,7 +447,12 @@ k_jacobi(float* __restrict__ Gall, float* __restrict__ conv_ws, int* __restrict_
             }
             cluster.sync();   // everyone has read before the next sweep overwrites
         }
-        null2 = 1e-11f * amx;                          // |column| < 3e-6 of the largest column: below what fp32 resolves in A
+        // Null floor (rot_scalars): |column| below max(thresh / 2, 16 * 2^-24 * max|column|), and never above the
+        // 3.16e-6 * max|column| of the original rule.  Kept columns (|g| ~ lambda > thresh) stay live as long as fp32
+        // resolves them against lambda_max; the rounding-noise columns of a rank-deficient map (~4e-7 lambda_max, i.e.
+        // ~7 x 2^-24 lambda_max) stay below it.  A floor of 3.16e-6 lambda_max alone froze a graded kept tail
+        // between thresh and that level after sweep 0 and whitened it wrong by O(1) (tests/test_gpu_whitening.py).
+        null2 = fminf(1e-11f * amx, fmaxf(0.25f * thresh * thresh, 9.1e-13f * amx));
         __syncthreads();
         if (gmax < 2.f) { ++sweep; break; }
     }
@@ -835,7 +840,7 @@ int set_jacobi_tolq(float v) {
     return cudaMemcpyToSymbol(g_jacobi_tolq, &v, sizeof(float)) == cudaSuccess ? 0 : -1;
 }
 
-int launch_jacobi(float* G, int C, int count, float* conv_ws, int* sweeps, cudaStream_t st, const int* skip) {
+int launch_jacobi(float* G, int C, int count, float* conv_ws, int* sweeps, cudaStream_t st, const int* skip, float thresh) {
     const float tol = 2.f * sqrtf((float)C) * 5.96e-8f;
     const int max_sweeps = 40;
     const int lg = g_jacobi_lg >= 0 ? g_jacobi_lg : (C >= 512 ? 2 : 1);
@@ -855,7 +860,7 @@ int launch_jacobi(float* G, int C, int count, float* conv_ws, int* sweeps, cudaS
     case NN: {                                                                                                       \
         WCTB_ENSURE_SMEM(k_jacobi<NN>, JacobiCfg<NN>::SMEM_BYTES);                                                   \
         cfg.dynamicSmemBytes = JacobiCfg<NN>::SMEM_BYTES;                                                            \
-        WCTB_CUDA(cudaLaunchKernelEx(&cfg, k_jacobi<NN>, G, conv_ws, sweeps, max_sweeps, tol, lg, stagger, skip));         \
+        WCTB_CUDA(cudaLaunchKernelEx(&cfg, k_jacobi<NN>, G, conv_ws, sweeps, max_sweeps, tol, lg, stagger, skip, thresh));         \
         break;                                                                                                       \
     }
     switch (C) {
@@ -931,7 +936,7 @@ int launch_wct_level(const __half* content, int Nc, int Hc, int Wc, const __half
     int* ok = reinterpret_cast<int*>(w + L.ok);
     rc = launch_matfun_ns(A0, C, np, Nc, thresh, eps_eig, Wcm, ok, kc, st);        // Wc and Cs are contiguous in ws (Wc then Cs)
     if (rc < 0) return rc;
-    rc = launch_jacobi(G, C, np, conv, kc + np, st, ok);
+    rc = launch_jacobi(G, C, np, conv, kc + np, st, ok, thresh);
     if (rc) return rc;
     rc = launch_eig_post(G, A0, lam, C, np, thresh, eps_eig, Nc, sigma, dvec, kc, st, ok);
     if (rc) return rc;
@@ -1009,7 +1014,7 @@ int launch_wct_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C,
     int* ok = reinterpret_cast<int*>(w + L.ok);
     rc = launch_matfun_ns(A0, C, Ns, /*n_first=*/0, thresh, eps_eig, Cs, ok, kc, st);     // C_s = A^+1/2 where every eigenvalue is kept
     if (rc < 0) return rc;
-    rc = launch_jacobi(G, C, Ns, conv, kc + Ns, st, ok);
+    rc = launch_jacobi(G, C, Ns, conv, kc + Ns, st, ok, thresh);
     if (rc) return rc;
     rc = launch_eig_post(G, A0, lam, C, Ns, thresh, eps_eig, /*n_content=*/0, sigma, dvec, kc, st, ok);
     if (rc) return rc;
@@ -1049,7 +1054,7 @@ static int wct_whiten(int Nc, int C, float eps_eig, float thresh, uint8_t* w, co
     int* ok = reinterpret_cast<int*>(w + L.ok);
     int rc = launch_matfun_ns(A0, C, Nc, /*n_first=*/Nc, thresh, eps_eig, Wcm, ok, kc, st);   // W_c = A^-1/2 where every eigenvalue is kept
     if (rc < 0) return rc;
-    rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, ok);
+    rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, ok, thresh);
     if (rc) return rc;
     rc = launch_eig_post(G, A0, lam, C, Nc, thresh, eps_eig, Nc, sigma, dvec, kc, st, ok);
     if (rc) return rc;
@@ -1302,7 +1307,7 @@ static int ost_transform(int Nc, int C, const float* Cs, const float* mean_s, in
     // B^1/2 into S: Newton-Schulz where it converges, else the singular values of P by the one-sided Jacobi solver
     int rc = launch_matfun_ns(B, C, Nc, /*n_first=*/0, /*thresh=*/0.f, /*eps_eig=*/0.f, S, okb, nullptr, st);
     if (rc < 0) return rc;
-    rc = launch_jacobi(Gb, C, Nc, reinterpret_cast<float*>(w + L.conv), swb, st, okb);
+    rc = launch_jacobi(Gb, C, Nc, reinterpret_cast<float*>(w + L.conv), swb, st, okb, /*thresh=*/0.f);
     if (rc) return rc;
     k_root_post<<<(unsigned)Nc, 256, 0, st>>>(Gb, C, reinterpret_cast<float*>(w + L.dvec), okb);
     WCTB_CHECK_LAUNCH("k_root_post");
@@ -1927,7 +1932,7 @@ int launch_wct_apply_regions(const __half* content, int Nc, int Hc, int Wc, int 
     if (rc) return rc;
     rc = launch_matfun_ns(A0, C, np, /*n_first=*/np, thresh, eps_eig, Wcm, ok, kc, st);
     if (rc < 0) return rc;
-    rc = launch_jacobi(G, C, np, conv, kc + np, st, ok);
+    rc = launch_jacobi(G, C, np, conv, kc + np, st, ok, thresh);
     if (rc) return rc;
     rc = launch_eig_post(G, A0, lam, C, np, thresh, eps_eig, np, sigma, dvec, kc, st, ok);
     if (rc) return rc;
@@ -2272,7 +2277,7 @@ int launch_wct_style_prepare_regions(const __half* style, int Hs, int Ws, int C,
     // from here on wct_style_prepare's steps over the R matrices (an empty region's placeholder G = I is harmless)
     rc = launch_matfun_ns(A0, C, R, /*n_first=*/0, thresh, eps_eig, Cs, ok, kc, st);
     if (rc < 0) return rc;
-    rc = launch_jacobi(G, C, R, conv, kc + R, st, ok);
+    rc = launch_jacobi(G, C, R, conv, kc + R, st, ok, thresh);
     if (rc) return rc;
     rc = launch_eig_post(G, A0, lam, C, R, thresh, eps_eig, /*n_content=*/0, sigma, dvec, kc, st, ok);
     if (rc) return rc;
@@ -2621,7 +2626,7 @@ int launch_style_swap_prepare(const __half* style, int Hs, int Ws, int C, int pa
     ActGeom gs(1, Hs, Ws, C);
     rc = launch_mean_cov(style, gs, eps_cov, mean_s, G, A0, dsum, st);
     if (rc) return rc;
-    rc = launch_jacobi(G, C, 1, conv, ks + 1, st, nullptr);
+    rc = launch_jacobi(G, C, 1, conv, ks + 1, st, nullptr, thresh);
     if (rc) return rc;
     rc = launch_eig_post(G, A0, lam, C, 1, thresh, 0.f, 1, sigma, dvec, ks, st);                // S^-1/2 (ops.py:193)
     if (rc) return rc;
@@ -2758,7 +2763,7 @@ static int style_swap_apply_impl(const __half* content, int Nc, int Hc, int Wc, 
     ActGeom gc(Nc, Hc, Wc, C), gs(1, Hs, Ws, C);
     rc = launch_mean_cov(content, gc, eps_cov, mean, G, A0, dsum, st);
     if (rc) return rc;
-    rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, nullptr);
+    rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, nullptr, thresh);
     if (rc) return rc;
     rc = launch_eig_post(G, A0, lam, C, Nc, thresh, 0.f, Nc, sigma, dvec, kc, st);             // S^-1/2 per frame (ops.py:187)
     if (rc) return rc;
