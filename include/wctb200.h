@@ -501,6 +501,25 @@ WCTB200_API size_t wctb200_efdm_workspace_bytes(int C, int N, int H, int W, int 
 WCTB200_API int wctb200_efdm_apply(const void* content, int N, int H, int W, int C, const void* state, int Ns, int Hs, int Ws,
                                    float alpha, void* out, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- sliced distribution matching (DESIGN.md §3.3.14; efdm.cu) ----------------------------------------------------
+ * EFDM in K random orthonormal bases of each level's channels, chained: y_1 = G_1 x_0, m_k = EFDM(y_k, S_k) at alpha = 1,
+ * y_{k+1} = G_{k+1} m_k for k = 1..K+1, out = alpha m_{K+1} + (1 - alpha) x_0 (G_k = R_k R_{k-1}^T folds the back- and
+ * forward-rotations; G_{K+1} = R_K^T; S_{K+1} the plain EFDM state).  C a multiple of 64.
+ * rotated_style_prepare: the state of one step, the sorted values of R y for the style SPF16 [Ns,Hs,Ws,C] and R fp32 C x C
+ * (row-major, y_c = sum_j R[c][j] v_j), in wctb200_efdm_style_state_bytes / _style_workspace_bytes as the plain prepare.
+ * sliced_step: m = EFDM(G v, state) at alpha = 1, with v the fp32 planes src [N][C][H*W] or, when src is NULL, the SPF16
+ * content [N,H,W,C]; written to the fp32 planes out_planes [N][C][H*W] (wctb200_efdm_planes_bytes, 0: bad geometry) or,
+ * when out_planes is NULL, as alpha m + (1 - alpha) content to SPF16 out with the reflect halo (alpha = 0 copies the
+ * content's bytes).  out_planes must not alias src.  ws: wctb200_efdm_workspace_bytes(C, N, H, W, S), as for the apply.
+ * G v is one fmaf chain per value over the input channels in index order, so a frame's bytes depend on nothing but its own
+ * values, its style's and G: the same for every workspace size, batch and chunking. */
+WCTB200_API size_t wctb200_efdm_planes_bytes(int C, int N, int H, int W);
+WCTB200_API int wctb200_efdm_rotated_style_prepare(const void* style, int Ns, int Hs, int Ws, int C, const float* R, void* state,
+                                                   void* ws, size_t ws_bytes, void* stream);
+WCTB200_API int wctb200_efdm_sliced_step(const void* content, const float* src, int N, int H, int W, int C, const float* G,
+                                         const void* state, int Ns, int Hs, int Ws, float alpha, float* out_planes, void* out,
+                                         void* ws, size_t ws_bytes, void* stream);
+
 /* ---- soft spatial control (DESIGN.md §3.3.11) -----------------------------------
  * mask_feather: labels device uint8 [N][Hm][Wm], R in 1..8, sigma in (0, 1024] mask pixels -> out fp32 [N][R][Hm][Wm]: the
  * one-hot plane of label r blurred by a separable Gaussian (taps exp(-d^2 / 2 sigma^2), |d| <= ceil(3 sigma), normalised in

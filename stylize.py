@@ -48,6 +48,10 @@ channel of the style, by rank, instead of matching only its covariance (DESIGN.m
 even wash with the same statistics stylise differently.  It suits ``--noise`` texture synthesis.  Output names are
 unchanged.
 
+Sliced distribution matching: ``--efdm-slices K`` (0..32, with ``--efdm``) first runs EFDM in K random rotations of each
+level's channels, each on the previous one's output, so that how the channels go together is matched too and not only
+each channel's own values (DESIGN.md §3.3.14).  0 is plain ``--efdm``.  Output names are unchanged.
+
 Labelled style swap (neural doodle): ``--swap-labels CONTENT_MAP STYLE_MAP`` with ``--swap5`` / ``--swap-targets`` gives
 the content and the style each a flat-colour label map (RGB or grey PNG, any resolution); every content patch is then
 rebuilt only from style patches of the same colour, or from all of them where the style has none (DESIGN.md §3.3.13).  The
@@ -115,6 +119,9 @@ _FLAGS = [
                              help="with --mst: Potts smoothness of the content labelling, finite and >= 0 (default 0.05)")),
     (("--efdm",), dict(action="store_true", default=False,
                        help="exact feature distribution matching: give every channel the style's whole value distribution")),
+    (("--efdm-slices",), dict(type=int, default=0, metavar="K",
+                              help="with --efdm: match in K random channel rotations first, then per channel (0..32, "
+                                   "default 0)")),
     (("--strength-map",), dict(type=str, default=None, metavar="PATH",
                                help="8-bit grayscale map of the per-pixel stylisation strength (gray v -> v/255)")),
     (("--mask-feather",), dict(type=float, default=None, metavar="SIGMA",
@@ -225,7 +232,7 @@ def check_swap_label_flags(parser, args):
 
 def check_values(parser, args):
     """The values of --tile-size (0: off), --mst / --mst-smooth (which needs --mst and defaults to 0.05 here),
-    --mask-feather and --temporal (stylize_video.py), as wct_tf_b200/options.py checks them."""
+    --mask-feather, --efdm-slices and --temporal (stylize_video.py), as wct_tf_b200/options.py checks them."""
     from wct_tf_b200 import options
     try:
         if getattr(args, "tile_size", 0):
@@ -238,6 +245,7 @@ def check_values(parser, args):
             options.check_mst(args.mst, args.mst_smooth, ("--mst", "--mst-smooth"))
         if getattr(args, "mask_feather", None) is not None:
             options.check_mask_feather(args.mask_feather, "--mask-feather")
+        options.check_efdm_slices(args.efdm_slices, args.efdm, options.CLI)
         if hasattr(args, "temporal"):
             options.check_temporal_strength(args.temporal, "--temporal")
     except ValueError as e:
@@ -466,6 +474,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
     if args.efdm:
         kw["efdm"] = True
+    if args.efdm_slices:
+        kw["efdm_slices"] = args.efdm_slices
     if getattr(args, "swap_labels", None):
         kw["swap_labels"] = args.swap_label_maps
     kw.update(soft_kw(args))

@@ -28,7 +28,7 @@ Multimodal style transfer: ``--mst K [--mst-smooth LAMBDA]`` matches the content
 (DESIGN.md §3.3.10), on both paths.
 
 Exact feature distribution matching: ``--efdm`` gives every channel of each level the style's whole value distribution
-(DESIGN.md §3.3.12), on both paths.
+(DESIGN.md §3.3.12), on both paths; ``--efdm-slices K`` first matches in K random channel rotations (§3.3.14).
 
 Which of these options combine is decided by one table, ``wct_tf_b200/options.py``, as for stylize.py.
 """
@@ -64,7 +64,7 @@ _VIDEO_FLAGS = [
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
            "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
-           "--mst", "--mst-smooth", "--strength-map", "--efdm")
+           "--mst", "--mst-smooth", "--strength-map", "--efdm", "--efdm-slices")
 # flags of the one-style mode that --interp-styles takes no part of
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("concat", "--concat")]
 
@@ -156,10 +156,12 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
 
     temporal_kw = {} if temporal is None else dict(temporal=temporal)
-    # --ost, --seamless, --mst and --efdm, on both paths
+    # --ost, --seamless, --mst, --efdm and --efdm-slices, on both paths
     opt_kw = dict(ost=True) if getattr(args, "ost", False) else {}
     if getattr(args, "efdm", False):
         opt_kw["efdm"] = True
+    if getattr(args, "efdm_slices", 0):
+        opt_kw["efdm_slices"] = args.efdm_slices
     if getattr(args, "seamless", None):
         opt_kw["seamless"] = args.seamless
     if getattr(args, "mst", None) is not None:

@@ -110,6 +110,9 @@ SIGNATURES = {
     "wctb200_efdm_style_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "wctb200_efdm_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "wctb200_efdm_apply": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _f, _vp, _vp, _sz, _vp]),
+    "wctb200_efdm_planes_bytes": (_sz, [_i, _i, _i, _i]),
+    "wctb200_efdm_rotated_style_prepare": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "wctb200_efdm_sliced_step": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _sz, _vp]),
     "wctb200_mask_feather": (_i, [_vp, _i, _i, _i, _i, _f, _vp, _vp]),
     "wctb200_weights_resize_area": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "wctb200_wct_stats_weighted": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp]),

@@ -187,8 +187,12 @@ int launch_mst_smooth(const float* D, int N, int H, int W, int K, float lambda, 
 size_t efdm_style_state_bytes(int C, int Ns, int Hs, int Ws);
 size_t efdm_style_workspace_bytes(int C, int Ns, int Hs, int Ws, int max_segments);
 size_t efdm_workspace_bytes(int C, int N, int H, int W, int max_segments);
-int launch_efdm_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, float* state, void* ws, size_t ws_bytes,
-                              cudaStream_t st);
+int launch_efdm_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, const float* R, float* state, void* ws,
+                              size_t ws_bytes, cudaStream_t st);
+size_t efdm_planes_bytes(int C, int N, int H, int W);
+int launch_efdm_sliced_step(const __half* content, const float* src, int N, int H, int W, int C, const float* G, const float* state,
+                            int Ns, int Hs, int Ws, float alpha, float* out_planes, __half* out, void* ws, size_t ws_bytes,
+                            cudaStream_t st);
 int launch_efdm_apply(const __half* content, int N, int H, int W, int C, const float* state, int Ns, int Hs, int Ws, float alpha,
                       __half* out, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t wct_style_prepare_regions_workspace_bytes(int C, int R, int Hs, int Ws);
@@ -538,7 +542,7 @@ int wctb200_efdm_style_prepare(const void* style, int Ns, int Hs, int Ws, int C,
                                void* stream) {
     WCTB_REQUIRE(style && state && ws, "efdm_style_prepare: null pointer");
     WCTB_REQUIRE(efdm_style_ok(Ns, Hs, Ws, C), "efdm_style_prepare: bad geometry Ns=%d %dx%d C=%d", Ns, Hs, Ws, C);
-    return launch_efdm_style_prepare(HCP(style), Ns, Hs, Ws, C, static_cast<float*>(state), ws, ws_bytes, ST(stream));
+    return launch_efdm_style_prepare(HCP(style), Ns, Hs, Ws, C, nullptr, static_cast<float*>(state), ws, ws_bytes, ST(stream));
 }
 size_t wctb200_efdm_workspace_bytes(int C, int N, int H, int W, int max_segments) {
     if (!geom_ok(N, H, W, C) || max_segments < 1) return 0;
@@ -552,6 +556,29 @@ int wctb200_efdm_apply(const void* content, int N, int H, int W, int C, const vo
     WCTB_REQUIRE(alpha >= -FLT_MAX && alpha <= FLT_MAX, "efdm_apply: alpha must be finite");
     return launch_efdm_apply(HCP(content), N, H, W, C, static_cast<const float*>(state), Ns, Hs, Ws, alpha, HP(out), ws, ws_bytes,
                              ST(stream));
+}
+// sliced distribution matching (efdm.cu, DESIGN.md §3.3.14): the rotation mixes whole 64-channel blocks of a frame
+size_t wctb200_efdm_planes_bytes(int C, int N, int H, int W) {
+    if (!geom_ok(N, H, W, C) || C % 64) return 0;
+    return efdm_planes_bytes(C, N, H, W);
+}
+int wctb200_efdm_rotated_style_prepare(const void* style, int Ns, int Hs, int Ws, int C, const float* R, void* state, void* ws,
+                                       size_t ws_bytes, void* stream) {
+    WCTB_REQUIRE(style && R && state && ws, "efdm_rotated_style_prepare: null pointer");
+    WCTB_REQUIRE(efdm_style_ok(Ns, Hs, Ws, C) && C % 64 == 0, "efdm_rotated_style_prepare: bad geometry Ns=%d %dx%d C=%d (C %% 64 == 0)",
+                 Ns, Hs, Ws, C);
+    return launch_efdm_style_prepare(HCP(style), Ns, Hs, Ws, C, R, static_cast<float*>(state), ws, ws_bytes, ST(stream));
+}
+int wctb200_efdm_sliced_step(const void* content, const float* src, int N, int H, int W, int C, const float* G, const void* state,
+                             int Ns, int Hs, int Ws, float alpha, float* out_planes, void* out, void* ws, size_t ws_bytes,
+                             void* stream) {
+    WCTB_REQUIRE(G && state && ws && (content || src) && (out_planes ? !out : (content && out)),
+                 "efdm_sliced_step: null pointer (content or src in; out_planes, or content and out)");
+    WCTB_REQUIRE(geom_ok(N, H, W, C) && C % 64 == 0 && efdm_style_ok(Ns, Hs, Ws, C) && (Ns == 1 || Ns == N),
+                 "efdm_sliced_step: bad geometry N=%d %dx%d C=%d, Ns=%d %dx%d (C %% 64 == 0, Ns in {1, N})", N, H, W, C, Ns, Hs, Ws);
+    WCTB_REQUIRE(alpha >= -FLT_MAX && alpha <= FLT_MAX, "efdm_sliced_step: alpha must be finite");
+    return launch_efdm_sliced_step(HCP(content), src, N, H, W, C, G, static_cast<const float*>(state), Ns, Hs, Ws, alpha, out_planes,
+                                   HP(out), ws, ws_bytes, ST(stream));
 }
 int wctb200_labels_resize_nearest(const uint8_t* src, int N, int Hm, int Wm, int Hf, int Wf, uint8_t* dst, void* stream) {
     WCTB_REQUIRE(src && dst, "labels_resize_nearest: null pointer");

@@ -12,6 +12,10 @@
 // Every segment is sorted by tiles of TILE keys whatever the batch, so a segment's bytes depend on nothing but its own values
 // and its style's: the apply runs as many whole segments at a time as the workspace holds, with byte-identical results for
 // every workspace size.  The sort's stability does not reach the output: all members of a run take the same value.
+//
+// Sliced distribution matching (DESIGN.md §3.3.14) chains steps of the same content pass with the keys built by
+// k_efdm_rotate_keys (y = G v) instead of k_efdm_keys: the runs go to fp32 channel-major planes, which the next step
+// rotates, and the last step stores alpha t + (1 - alpha) x0 with the original content x0 (k_efdm_store<true>).
 #include <algorithm>
 
 #include "common.cuh"
@@ -72,6 +76,82 @@ __global__ void __launch_bounds__(256) k_efdm_keys(const __half* __restrict__ ac
         for (int pj = tx; pj < TP; pj += 32) {
             const int p = p0 + pj;
             if (p < L) keys[(long long)(sl0 + si) * L + p] = tile[si][pj];
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// sliced key build (DESIGN.md §3.3.14): keys of y = G v for segments [s0, s0+S), channel-major [S][L], where v is frame n's
+// C values at a pixel, read from the SPF16 NHWC interior (planes == NULL) or from fp32 channel-major planes [N][C][L].  A CTA
+// computes RC output channels x RP pixels of one frame (C % RC == 0, so a channel block never straddles frames); every
+// output is one fmaf chain over the input channels in index order, so its rounding does not depend on the tile, the chunk
+// or the batch.  Blocks are aligned to RC segments from segment 0; only the chunk's segments are written.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int RC = 64, RP = 128, RJ = 32;   // output channels, pixels, input channels per smem stage
+__global__ void __launch_bounds__(256) k_efdm_rotate_keys(const __half* __restrict__ act, const float* __restrict__ planes, ActGeom g,
+                                                          const float* __restrict__ G, long long s0, int S,
+                                                          unsigned int* __restrict__ keys) {
+    __shared__ __align__(16) float Gs[RJ][RC + 4];
+    __shared__ float Vs[RJ][RP + 1];
+    const int C = g.C, L = g.H * g.W;
+    const int p0 = blockIdx.x * RP;
+    const long long sb = (s0 / RC + blockIdx.y) * RC;        // first segment of this block
+    const long long n = sb / C;
+    const int c0 = (int)(sb - n * C);
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // pixels tx + 32 i, channels ty * 8 + r
+    float acc[8][4];
+#pragma unroll
+    for (int r = 0; r < 8; ++r)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[r][i] = 0.f;
+    for (int j0 = 0; j0 < C; j0 += RJ) {
+        for (int e = threadIdx.x; e < RJ * RC; e += 256) {
+            const int c = e % RC, j = e / RC;
+            Gs[j][c] = G[(long long)(c0 + c) * C + j0 + j];
+        }
+        if (planes) {
+            for (int e = threadIdx.x; e < RJ * RP; e += 256) {
+                const int pi = e % RP, j = e / RP;
+                const int p = p0 + pi;
+                Vs[j][pi] = p < L ? planes[(n * C + j0 + j) * (long long)L + p] : 0.f;
+            }
+        } else {
+            for (int e = threadIdx.x; e < RJ * RP; e += 256) {
+                const int j = e % RJ, pi = e / RJ;
+                const int p = p0 + pi;
+                float v = 0.f;
+                if (p < L) {
+                    const int y = p / g.W, x = p - y * g.W;
+                    const long long off = ((n * g.Hp + y + 1) * g.Wp + x + 1) * C + j0 + j;
+                    v = merge_f32(act[off], act[g.plane + off]);
+                }
+                Vs[j][pi] = v;
+            }
+        }
+        __syncthreads();
+#pragma unroll 4
+        for (int j = 0; j < RJ; ++j) {
+            const float4 ga = *reinterpret_cast<const float4*>(&Gs[j][ty * 8]);
+            const float4 gb = *reinterpret_cast<const float4*>(&Gs[j][ty * 8 + 4]);
+            const float gr[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
+            float v[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) v[i] = Vs[j][tx + 32 * i];
+#pragma unroll
+            for (int r = 0; r < 8; ++r)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) acc[r][i] = fmaf(gr[r], v[i], acc[r][i]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+        const long long s = sb + ty * 8 + r;
+        if (s < s0 || s >= s0 + S) continue;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int p = p0 + tx + 32 * i;
+            if (p < L) keys[(s - s0) * L + p] = efdm_key(acc[r][i]);
         }
     }
 }
@@ -442,9 +522,11 @@ __device__ __forceinline__ void efdm_store(__half* __restrict__ act, const ActGe
     }
 }
 
-// out [S][L] fp32 of segments [s0, s0+S) -> SPF16 NHWC with the reflect halo (the transpose of k_efdm_keys)
+// out [S][L] fp32 of segments [s0, s0+S) -> SPF16 NHWC with the reflect halo (the transpose of k_efdm_keys).  BLEND (the
+// last sliced step): the value stored is alpha t + (1 - alpha) x0, x0 the SPF16 content at the same cell.
+template <bool BLEND>
 __global__ void __launch_bounds__(256) k_efdm_store(const float* __restrict__ vals, ActGeom g, long long s0, int S,
-                                                    __half* __restrict__ act) {
+                                                    __half* __restrict__ act, const __half* __restrict__ x0, float alpha) {
     __shared__ float tile[TS][TP + 1];
     const int L = g.H * g.W;
     const int p0 = blockIdx.x * TP;
@@ -466,15 +548,19 @@ __global__ void __launch_bounds__(256) k_efdm_store(const float* __restrict__ va
     for (int pi = ty; pi < TP; pi += 8) {
         const int p = p0 + pi;
         if (p < L) {
-            __half hi, lo;
-            split_f32(tile[tx][pi], hi, lo);
             const int y = p / g.W, x = p - y * g.W;
+            float v = tile[tx][pi];
+            if (BLEND) {
+                const long long off = ((n * g.Hp + y + 1) * g.Wp + x + 1) * g.C + c;
+                v = fmaf(alpha, v, (1.0f - alpha) * merge_f32(x0[off], x0[g.plane + off]));
+            }
+            __half hi, lo;
+            split_f32(v, hi, lo);
             efdm_store(act, g, n, y, x, c, hi, lo);
         }
     }
 }
 
-// alpha = 0: the content's own bytes, with the reflect halo
 __global__ void k_efdm_copy(const __half* __restrict__ in, ActGeom g, __half* __restrict__ out) {
     const long long total = (long long)g.N * g.H * g.W * (g.C / 8);
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -538,8 +624,9 @@ static long long efdm_chunk(long long total_segs, long long L, bool idx, size_t 
     return lo;
 }
 
-int launch_efdm_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, float* state, void* ws, size_t ws_bytes,
-                              cudaStream_t st) {
+// R NULL: the plain state.  R (fp32 C x C, C % RC == 0): the sorted values of R y, the state of a sliced step.
+int launch_efdm_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, const float* R, float* state, void* ws,
+                              size_t ws_bytes, cudaStream_t st) {
     const long long total = (long long)Ns * C, L = (long long)Hs * Ws;
     const long long S = efdm_chunk(total, L, false, ws_bytes);
     if (S < 1) {
@@ -552,8 +639,14 @@ int launch_efdm_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C
         const int n = (int)std::min(S, total - s0);
         const EfdmWs w = efdm_layout(n, L, false);
         unsigned int* kA = reinterpret_cast<unsigned int*>(b + w.kA);
-        k_efdm_keys<<<dim3(cdiv(L, TP), cdiv(n, TS)), 256, 0, st>>>(style, g, s0, n, kA);
-        WCTB_CHECK_LAUNCH("k_efdm_keys");
+        if (R) {
+            k_efdm_rotate_keys<<<dim3(cdiv(L, RP), (unsigned)((s0 + n - 1) / RC - s0 / RC + 1)), 256, 0, st>>>(style, nullptr, g, R,
+                                                                                                           s0, n, kA);
+            WCTB_CHECK_LAUNCH("k_efdm_rotate_keys");
+        } else {
+            k_efdm_keys<<<dim3(cdiv(L, TP), cdiv(n, TS)), 256, 0, st>>>(style, g, s0, n, kA);
+            WCTB_CHECK_LAUNCH("k_efdm_keys");
+        }
         int rc = efdm_sort(kA, reinterpret_cast<unsigned int*>(b + w.kB), nullptr, nullptr, n, (int)L,
                            reinterpret_cast<unsigned int*>(b + w.hist), st);
         if (rc) return rc;
@@ -565,16 +658,23 @@ int launch_efdm_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C
     return 0;
 }
 
-int launch_efdm_apply(const __half* content, int N, int H, int W, int C, const float* state, int Ns, int Hs, int Ws, float alpha,
-                      __half* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    const ActGeom g(N, H, W, C);
-    if (alpha == 0.f) {
-        const long long total = (long long)N * H * W * (C / 8);
-        k_efdm_copy<<<(unsigned)std::min<long long>(cdiv(total, 256), (long long)device_sm_count() * 16), 256, 0, st>>>(content, g, out);
-        WCTB_CHECK_LAUNCH("k_efdm_copy");
-        return 0;
-    }
-    const long long total = (long long)N * C, L = (long long)H * W;
+// alpha = 0: the content's own bytes, with the reflect halo
+static int efdm_copy(const __half* content, const ActGeom& g, __half* out, cudaStream_t st) {
+    const long long total = (long long)g.N * g.H * g.W * (g.C / 8);
+    k_efdm_copy<<<(unsigned)std::min<long long>(cdiv(total, 256), (long long)device_sm_count() * 16), 256, 0, st>>>(content, g, out);
+    WCTB_CHECK_LAUNCH("k_efdm_copy");
+    return 0;
+}
+
+// The content side of one EFDM pass over the N*C segments, as many whole segments at a time as ws holds.  The keys are the
+// content's own values (G NULL) or those of G v (v from the SPF16 `content`, or from fp32 planes `src` when not NULL).  The
+// run values go to fp32 planes `out_planes` at alpha = 1, or to SPF16 `out` blended with the keys' values (plain EFDM) or,
+// for a sliced step, with `content`.
+static int efdm_content_pass(const __half* content, const float* src, const float* G, const ActGeom& g, const float* state,
+                             int Ns, int Ms, float alpha, float* out_planes, __half* out, void* ws, size_t ws_bytes,
+                             cudaStream_t st) {
+    const int C = g.C;
+    const long long total = (long long)g.N * C, L = (long long)g.H * g.W;
     const long long S = efdm_chunk(total, L, true, ws_bytes);
     if (S < 1) {
         set_error("efdm_apply: workspace %zu < %zu bytes (one segment)", ws_bytes, efdm_layout(1, L, true).total);
@@ -590,25 +690,56 @@ int launch_efdm_apply(const __half* content, int N, int H, int W, int C, const f
         unsigned int* iA = reinterpret_cast<unsigned int*>(b + w.iA);
         double* tsum = reinterpret_cast<double*>(b + w.tsum);
         double* P = reinterpret_cast<double*>(b + w.P);
-        k_efdm_keys<<<dim3(cdiv(L, TP), cdiv(n, TS)), 256, 0, st>>>(content, g, s0, n, kA);
-        WCTB_CHECK_LAUNCH("k_efdm_keys");
+        if (G) {
+            k_efdm_rotate_keys<<<dim3(cdiv(L, RP), (unsigned)((s0 + n - 1) / RC - s0 / RC + 1)), 256, 0, st>>>(content, src, g, G, s0,
+                                                                                                           n, kA);
+            WCTB_CHECK_LAUNCH("k_efdm_rotate_keys");
+        } else {
+            k_efdm_keys<<<dim3(cdiv(L, TP), cdiv(n, TS)), 256, 0, st>>>(content, g, s0, n, kA);
+            WCTB_CHECK_LAUNCH("k_efdm_keys");
+        }
         int rc = efdm_sort(kA, kB, iA, reinterpret_cast<unsigned int*>(b + w.iB), n, (int)L,
                            reinterpret_cast<unsigned int*>(b + w.hist), st);
         if (rc) return rc;
-        EfdmQ E{state, C, Ns, Hs * Ws, (int)L, s0};
+        EfdmQ E{state, C, Ns, Ms, (int)L, s0};
         k_efdm_qsum<<<dim3(T, n), THREADS, 0, st>>>(E, T, tsum);
         WCTB_CHECK_LAUNCH("k_efdm_qsum");
         k_efdm_qscan<<<cdiv(n, 128), 128, 0, st>>>(tsum, T, n);
         WCTB_CHECK_LAUNCH("k_efdm_qscan");
         k_efdm_prefix<<<dim3(T, n), THREADS, 0, st>>>(E, T, tsum, P);
         WCTB_CHECK_LAUNCH("k_efdm_prefix");
-        float* vals = reinterpret_cast<float*>(kB);     // free after the sort (an even number of passes ends in kA)
-        k_efdm_runs<<<dim3(T, n), THREADS, 0, st>>>(kA, iA, P, (int)L, T, alpha, vals);
+        // the run values: into the planes, or into kB, free after the sort (an even number of passes ends in kA)
+        float* vals = out_planes ? out_planes + s0 * L : reinterpret_cast<float*>(kB);
+        k_efdm_runs<<<dim3(T, n), THREADS, 0, st>>>(kA, iA, P, (int)L, T, G ? 1.0f : alpha, vals);
         WCTB_CHECK_LAUNCH("k_efdm_runs");
-        k_efdm_store<<<dim3(cdiv(L, TP), cdiv(n, TS)), 256, 0, st>>>(vals, g, s0, n, out);
+        if (out_planes) continue;
+        if (G) {
+            k_efdm_store<true><<<dim3(cdiv(L, TP), cdiv(n, TS)), 256, 0, st>>>(vals, g, s0, n, out, content, alpha);
+        } else {
+            k_efdm_store<false><<<dim3(cdiv(L, TP), cdiv(n, TS)), 256, 0, st>>>(vals, g, s0, n, out, nullptr, 0.f);
+        }
         WCTB_CHECK_LAUNCH("k_efdm_store");
     }
     return 0;
+}
+
+int launch_efdm_apply(const __half* content, int N, int H, int W, int C, const float* state, int Ns, int Hs, int Ws, float alpha,
+                      __half* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    const ActGeom g(N, H, W, C);
+    if (alpha == 0.f) return efdm_copy(content, g, out, st);
+    return efdm_content_pass(content, nullptr, nullptr, g, state, Ns, Hs * Ws, alpha, nullptr, out, ws, ws_bytes, st);
+}
+
+size_t efdm_planes_bytes(int C, int N, int H, int W) { return efdm_align((size_t)N * C * H * W * sizeof(float)); }
+
+// one step of the sliced chain: m = EFDM(G v, state) at alpha = 1, v = the SPF16 `content` (src NULL) or the planes `src`;
+// m goes to `out_planes`, or (out_planes NULL) alpha m + (1 - alpha) content goes to SPF16 `out`
+int launch_efdm_sliced_step(const __half* content, const float* src, int N, int H, int W, int C, const float* G, const float* state,
+                            int Ns, int Hs, int Ws, float alpha, float* out_planes, __half* out, void* ws, size_t ws_bytes,
+                            cudaStream_t st) {
+    const ActGeom g(N, H, W, C);
+    if (!out_planes && alpha == 0.f) return efdm_copy(content, g, out, st);
+    return efdm_content_pass(content, src, G, g, state, Ns, Hs * Ws, alpha, out_planes, out, ws, ws_bytes, st);
 }
 
 }  // namespace wctb

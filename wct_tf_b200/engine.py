@@ -11,7 +11,7 @@ import ctypes
 import numpy as np
 import torch
 
-from . import _capi, options
+from . import _capi, options, sliced
 from .model import WCTModel, RELU_CHANNELS, RELU_LEVEL, check_seamless, seamless_axes
 from .prepared import (PreparedStyle, SEMANTIC_KEYS, encoder_fingerprints, slice_act_planes, slice_adain_state,
                        slice_wct_state)
@@ -86,6 +86,7 @@ class Engine(object):
         self._tag = None           # profiling only: "style" / relu target of the level being enqueued
         self._vgg_layers = weights["vgg"]          # encoder fingerprints of prepared styles (computed on first use)
         self._fingerprints = None
+        self._sliced = {}                 # (C, K) -> device bases and step matrices of sliced EFDM
         with torch.cuda.device(self.device):
             self._upload(weights)
 
@@ -691,18 +692,62 @@ class Engine(object):
         S = max(1, min(total, (EFDM_WORKSPACE_BYTES - per_seg_fn(1) + per_seg) // max(per_seg, 1)))
         return S, -(-total // S)
 
-    def efdm_prepare(self, style):
-        """Style side of EFDM on one level: every channel's values, sorted (fp32 [n][C][Hs*Ws]).  Returns dict(state, H, W)."""
+    def efdm_prepare(self, style, R=None):
+        """Style side of EFDM on one level: every channel's values, sorted (fp32 [n][C][Hs*Ws]).  Returns dict(state, H, W).
+        With ``R`` (cuda fp32 C x C) the values are those of R y, the state of one sliced step (§3.3.14)."""
         lib, C, n = self.lib, style.C, style.N
         state = torch.empty(lib.wctb200_efdm_style_state_bytes(C, n, style.H, style.W), dtype=torch.uint8, device=self.device)
         S, chunks = self._efdm_chunk(n * C, lambda k: lib.wctb200_efdm_style_workspace_bytes(C, n, style.H, style.W, k))
         nbytes = lib.wctb200_efdm_style_workspace_bytes(C, n, style.H, style.W, S)
-        ws = self._grow_workspace(("efdm_style",), nbytes)
+        # the rotated states of a per-frame style are made on the content stream, while the style stream may still be
+        # preparing later levels: each has its own scratch
+        ws = self._grow_workspace(("efdm_style",) if R is None else ("efdm_style_rot",), nbytes)
         m = n * C * style.H * style.W
         # the exact size of S segments (a grown buffer may be larger): the chunking, and so the launch count, is the one above
-        self._call("efdm_style[C%d]" % C, 14 * chunks, lib.wctb200_efdm_style_prepare, style.ptr, n, style.H, style.W, C,
-                   state.data_ptr(), ws.data_ptr(), nbytes, self._stream(), bytes_=84.0 * m)
+        if R is None:
+            self._call("efdm_style[C%d]" % C, 14 * chunks, lib.wctb200_efdm_style_prepare, style.ptr, n, style.H, style.W, C,
+                       state.data_ptr(), ws.data_ptr(), nbytes, self._stream(), bytes_=84.0 * m)
+        else:
+            self._call("efdm_style_rot[C%d]" % C, 14 * chunks, lib.wctb200_efdm_rotated_style_prepare, style.ptr, n, style.H,
+                       style.W, C, R.data_ptr(), state.data_ptr(), ws.data_ptr(), nbytes, self._stream(),
+                       flops=2.0 * C * m, bytes_=84.0 * m)
         return dict(state=state, H=style.H, W=style.W)
+
+    def sliced_matrices(self, C, K):
+        """(R_1..R_K, G_1..G_{K+1}) of ``sliced`` as cuda fp32 C x C tensors, made once per (C, K)."""
+        key = (int(C), int(K))
+        if key not in self._sliced:
+            to = lambda a: torch.from_numpy(np.array(a, dtype=np.float32)).to(self.device)
+            self._sliced[key] = ([to(R) for R in sliced.rotations(C, K)], [to(G) for G in sliced.step_matrices(C, K)])
+        return self._sliced[key]
+
+    def efdm_sliced_apply(self, content, st, n_style, alpha, feat=None):
+        """Sliced distribution matching of one level (§3.3.14): the chain of ``st["slices"]`` = K rotated EFDM steps and
+        the plain one.  The state of step k is ``st["rot"][k]`` when the side made them (a shared style), otherwise it is
+        made from the style feature ``feat`` just before the step and dropped after it."""
+        lib, C, N, K = self.lib, content.C, content.N, st["slices"]
+        if float(alpha) == 0.0:
+            return self.efdm_apply(content, st, n_style, alpha)
+        Rs, Gs = self.sliced_matrices(C, K)
+        H, W = content.H, content.W
+        m = N * C * H * W
+        S, chunks = self._efdm_chunk(N * C, lambda k: lib.wctb200_efdm_workspace_bytes(C, N, H, W, k))
+        ws_n = lib.wctb200_efdm_workspace_bytes(C, N, H, W, S)
+        ws_ptr = self._grow_workspace(("efdm",), ws_n).data_ptr()
+        pn = lib.wctb200_efdm_planes_bytes(C, N, H, W)
+        # m_k stays in fp32 planes; step k + 1 reads all channels of m_k while writing m_{k+1}, so two buffers take turns
+        planes = [self._grow_workspace(("efdm_planes", i), pn).data_ptr() for i in range(min(K, 2))]
+        out = self._act(N, H, W, C)
+        src = None
+        for k in range(K + 1):
+            last = k == K
+            state = st["state"] if last else (st["rot"][k] if st.get("rot") else self.efdm_prepare(feat, Rs[k])["state"])
+            dst = None if last else planes[k % 2]
+            self._call("efdm_sliced[C%d]" % C, (18 if last else 17) * chunks, lib.wctb200_efdm_sliced_step, content.ptr, src,
+                       N, H, W, C, Gs[k].data_ptr(), state.data_ptr(), n_style, st["H"], st["W"], float(alpha), dst,
+                       out.ptr if last else None, ws_ptr, ws_n, self._stream(), flops=2.0 * C * m, bytes_=130.0 * m)
+            src = dst
+        return out, None
 
     def efdm_apply(self, content, st, n_style, alpha):
         """EFDM of one level against an ``efdm_prepare`` state of ``n_style`` in {1, N} styles."""
@@ -777,7 +822,7 @@ class Engine(object):
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
                 region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05, strength_map=None,
-                content_weights=None, mask_feather=None, efdm=False, swap_labels=None):
+                content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -838,7 +883,13 @@ class Engine(object):
         Exact feature distribution matching (DESIGN.md §3.3.12): ``efdm=True`` gives every channel of each level the value
         distribution of the same channel of the style, by rank (ties take the mean of their ranks' style values), instead
         of WCT; swap levels still swap.  ``style_u8`` is one style or one per frame; a ``PreparedStyle`` only as made by
-        ``prepare_call(efdm=True)``."""
+        ``prepare_call(efdm=True)``.
+
+        Sliced distribution matching (DESIGN.md §3.3.14): ``efdm_slices`` = K in 0..32 (with ``efdm``) first runs EFDM in
+        K random orthonormal bases of each level's channels, each step rotating the previous one's output, so that the
+        joint distribution of the channels approaches the style's; the last step is plain EFDM, and the blend at ``alpha``
+        is with the content feature.  K = 0 is plain EFDM.  A ``PreparedStyle`` must come from
+        ``prepare_call(efdm=True, efdm_slices=K)`` with the same K."""
         N = content_u8.shape[0]
         options.check({name for name, on in (
             ("adain", adain), ("ost", ost), ("efdm", efdm), ("mst", mst is not None), ("swap", swap5 or swap_targets is not None),
@@ -846,11 +897,15 @@ class Engine(object):
             ("style_weights", interp_styles is not None), ("content_weights", content_weights is not None),
             ("mask_feather", mask_feather is not None), ("strength_map", strength_map is not None),
             ("seamless", seamless is not None)) if on}, options.ENGINE)
+        efdm_slices = options.check_efdm_slices(efdm_slices, efdm, options.ENGINE)
         if efdm and isinstance(style_u8, PreparedStyle):
             skip = self.swap_levels(swap5, swap_targets)
             if any(relu not in style_u8.efdm and relu not in skip for relu in self.model.style_taps):
                 raise ValueError("efdm sorts the style's features at every level, which a prepared style does not keep: "
                                  "give the style image")
+            if any(st["slices"] != efdm_slices for st in style_u8.efdm.values()):
+                raise ValueError("the prepared style was made for efdm_slices = %d, the call asks for %d"
+                                 % (next(iter(style_u8.efdm.values()))["slices"], efdm_slices))
         soft = None
         if strength_map is not None or content_weights is not None or mask_feather is not None:
             sm = None
@@ -935,7 +990,7 @@ class Engine(object):
             # one style per frame: frame by frame (each frame's swap has its own style side)
             outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
                                  alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
-                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm,
+                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm, efdm_slices=efdm_slices,
                                  swap_labels=None if swap_labels is None else _frame_labels(swap_labels, i, i + 1))
                     for i in range(N)]
             return torch.cat(outs, dim=0)
@@ -949,7 +1004,7 @@ class Engine(object):
             self._group = 1 if G > 1 else 0
             try:
                 owned = shared = self._style_side(style_u8, main, wct=not adain and not efdm, adain=adain, keep=swap_lv, skip=swap_lv,
-                                                  efdm=efdm)
+                                                  efdm=efdm, efdm_slices=efdm_slices)
             finally:
                 self._group = 0
         for relu in swap_lv:
@@ -961,13 +1016,13 @@ class Engine(object):
                 else:
                     sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
                 return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
-                                         seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm,
+                                         seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm, efdm_slices=efdm_slices,
                                          swap_labels=None if swap_labels is None else _frame_labels(swap_labels, lo, hi))
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
                                     swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft, efdm=efdm,
-                                    swap_labels=swap_labels)
+                                    swap_labels=swap_labels, efdm_slices=efdm_slices)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -1095,7 +1150,8 @@ class Engine(object):
             self._style_streams[self._group] = torch.cuda.Stream(device=self.device, priority=prio)
         return self._style_streams[self._group]
 
-    def _style_side(self, style_u8, main, wct=True, adain=False, keep=(), skip=(), labels=None, R=0, mst=0, efdm=False):
+    def _style_side(self, style_u8, main, wct=True, adain=False, keep=(), skip=(), labels=None, R=0, mst=0, efdm=False,
+                    efdm_slices=0):
         """The prepare step: style side of one call (model.py:70-72: ONE encoder pass emitting every target; per level the
         WCT state of ops.py:48-55,76 when ``wct``, the AdaIN moments when ``adain``; levels in ``skip`` get neither), enqueued
         on this group's style stream when overlap is on.  ``keep`` lists the levels whose feature it keeps (the style
@@ -1111,7 +1167,9 @@ class Engine(object):
         above, and the labels, centres and info of every level in ``mst``.
 
         With ``efdm`` every level also gets its EFDM state (``efdm_prepare``: the style's values sorted per channel) in
-        ``efdm``."""
+        ``efdm``.  With ``efdm_slices`` = K > 0 as well (sliced EFDM, §3.3.14), a side of one style also makes the K
+        rotated states of each level (``rot``); a side of one style per frame keeps each level's feature instead, from which
+        ``efdm_sliced_apply`` makes each state just before its step."""
         lib = self.lib
         side = self._style_stream() or main
         if side is not main:
@@ -1152,7 +1210,12 @@ class Engine(object):
                     if adain:
                         ps.adain[relu] = self.adain_prepare(feats[relu])
                     if efdm:
-                        ps.efdm[relu] = self.efdm_prepare(feats[relu])
+                        ps.efdm[relu] = dict(self.efdm_prepare(feats[relu]), slices=int(efdm_slices), rot=None)
+                        if efdm_slices and ps.n == 1:
+                            ps.efdm[relu]["rot"] = [self.efdm_prepare(feats[relu], R)["state"]
+                                                    for R in self.sliced_matrices(feats[relu].C, efdm_slices)[0]]
+                        elif efdm_slices:
+                            ps.feats[relu] = feats[relu]
                 ev = torch.cuda.Event()
                 ev.record(side)
                 ps.events[relu] = ev
@@ -1172,12 +1235,13 @@ class Engine(object):
         ps.record_stream(main)
         return ps
 
-    def prepare_call(self, style_u8, adain=False, swap5=False, swap_targets=None, efdm=False):
-        """The style side one call needs (WCT states, the AdaIN moments, or the EFDM states; the features of the swap levels
-        of ``swap5`` / ``swap_targets``), made once for a call that applies it several times (passes)."""
+    def prepare_call(self, style_u8, adain=False, swap5=False, swap_targets=None, efdm=False, efdm_slices=0):
+        """The style side one call needs (WCT states, the AdaIN moments, or the EFDM states, with ``efdm_slices`` those of
+        every slice; the features of the swap levels of ``swap5`` / ``swap_targets``), made once for a call that applies it
+        several times (passes)."""
         main = torch.cuda.current_stream(self.device)
         ps = self._style_side(style_u8, main, wct=not adain and not efdm, adain=adain, keep=self.swap_levels(swap5, swap_targets),
-                              efdm=efdm)
+                              efdm=efdm, efdm_slices=efdm_slices)
         style_u8.record_stream(ps.side)
         return ps
 
@@ -1223,7 +1287,8 @@ class Engine(object):
             out.adain[relu] = slice_adain_state(self.lib, st, RELU_CHANNELS[relu], ps.n, lo, hi)
         for relu, st in ps.efdm.items():
             per = RELU_CHANNELS[relu] * st["H"] * st["W"] * 4          # the sorted values of one style
-            out.efdm[relu] = dict(st, state=st["state"][lo * per:hi * per].clone())
+            out.efdm[relu] = dict(st, state=st["state"][lo * per:hi * per].clone(),
+                                  rot=[r[lo * per:hi * per].clone() for r in st["rot"]] if st.get("rot") else None)
         for relu, f in ps.feats.items():
             out.feats[relu] = self._act(hi - lo, f.H, f.W, f.C)
             slice_act_planes(f.buf, f.N, f.H, f.W, f.C, lo, hi, out.feats[relu].buf)
@@ -1251,10 +1316,11 @@ class Engine(object):
         return ps.swap[key]
 
     def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
-                     seamless=None, soft=None, efdm=False, swap_labels=None):
+                     seamless=None, soft=None, efdm=False, swap_labels=None, efdm_slices=0):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
         ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
-        optimal-transport transform instead of WCT at the other levels, ``efdm`` exact feature distribution matching;
+        optimal-transport transform instead of WCT at the other levels, ``efdm`` exact feature distribution matching (in
+        ``efdm_slices`` rotated bases first when > 0);
         ``seamless``: the wrapped axes of the content path
         (the transforms write a reflect halo, which is rewritten before the decoder reads it); ``swap_labels``: the (content
         [1|N], style [1]) label maps of a labelled swap at the swap levels."""
@@ -1267,7 +1333,8 @@ class Engine(object):
             assert content_u8.dtype == torch.uint8
             if not isinstance(style, PreparedStyle):
                 assert style.dtype == torch.uint8 and style.shape[0] in (1, N)
-                owned = style = self._style_side(style, main, wct=not adain and not efdm, adain=adain, efdm=efdm)
+                owned = style = self._style_side(style, main, wct=not adain and not efdm, adain=adain, efdm=efdm,
+                                                 efdm_slices=efdm_slices)
             n_style = style.n
             sides = [style]
         content = torch.empty(content_u8.shape, dtype=torch.float32, device=self.device)
@@ -1300,6 +1367,8 @@ class Engine(object):
                 elif multi is None:
                     if adain:
                         f, kbuf = self.adain_apply(cf, style.adain[relu], n_style, alpha)
+                    elif efdm and efdm_slices:
+                        f, kbuf = self.efdm_sliced_apply(cf, style.efdm[relu], n_style, alpha, style.feats.get(relu))
                     elif efdm:
                         f, kbuf = self.efdm_apply(cf, style.efdm[relu], n_style, alpha)
                     elif ost:

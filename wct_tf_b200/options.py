@@ -6,7 +6,7 @@ This is the one statement of that policy.  ``WCT.predict_batch``, ``Engine.styli
 
 ``swap_labels`` (the labelled style swap, ``check_swap_labels``) has no entry in ``SPELLINGS``: it is a parameter of
 ``swap``, as ``mst_smooth`` is of ``mst``.  It needs the swap, and through it takes the swap's exclusions; it adds none of
-its own.
+its own.  ``efdm_slices`` (sliced distribution matching, ``check_efdm_slices``) is in the same way a parameter of ``efdm``.
 """
 import numpy as np
 
@@ -128,6 +128,18 @@ def check_swap_labels(swap_labels, swap, n_frames, n_styles=1, names=("swap_labe
     content = _label_map(swap_labels[0], names[0] + " content labels", (1, n_frames))
     style = _label_map(swap_labels[1], names[0] + " style labels", (1, n_styles))
     return content, style
+
+
+def check_efdm_slices(K, efdm, vocab=API):
+    """The number of rotated bases of sliced distribution matching (DESIGN.md §3.3.14): an integer in 0..32, and above 0
+    only with ``efdm``.  Returns it as an int; ValueError otherwise, naming the options as ``vocab`` spells them (``--efdm``
+    becomes ``--efdm-slices`` in the CLI's)."""
+    name = "--efdm-slices" if vocab is CLI else "efdm_slices"
+    if isinstance(K, bool) or not isinstance(K, (int, np.integer)) or not 0 <= K <= 32:
+        raise ValueError("%s must be an integer in 0..32, got %r" % (name, K))
+    if K and not efdm:
+        raise ValueError("%s needs %s: the slices are steps of EFDM" % (name, vocab["efdm"]))
+    return int(K)
 
 
 def check_tile_size(tile_size, name="tile_size"):

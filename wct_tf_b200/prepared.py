@@ -73,7 +73,8 @@ class PreparedStyle(object):
         self.entries = None                       # style-masked side (Engine._style_side): its n styles, one by one
         self.mst = {}                             # relu -> dict(labels, centres, info): MST clusters (Engine._style_side)
         self.mst_k = 0                            # K of an MST side (its n = K styles are the clusters), 0 otherwise
-        self.efdm = {}                            # relu -> dict(state, H, W): sorted style values (Engine._style_side)
+        self.efdm = {}                            # relu -> dict(state, H, W, slices, rot): sorted style values, and those of
+                                                  # the K rotated bases of a shared sliced side (Engine._style_side)
 
     @property
     def feat5(self):
@@ -102,6 +103,7 @@ class PreparedStyle(object):
         ts += [f.buf for f in self.feats.values()]
         ts += [t for m in self.mst.values() for t in m.values()]
         ts += [e["state"] for e in self.efdm.values()]
+        ts += [t for e in self.efdm.values() for t in e.get("rot") or ()]
         return ts
 
     def record_stream(self, stream):

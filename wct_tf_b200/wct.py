@@ -270,7 +270,8 @@ class WCT(object):
     def predict_batch(self, contents, styles, alpha=1, adain=False, return_float=False, out=None, swap5=False, ss_alpha=1,
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
                       swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
-                      strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None):
+                      strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None,
+                      efdm_slices=0):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -349,6 +350,11 @@ class WCT(object):
         ``efdm=False`` changes nothing.  The style is sorted once per call however many ``passes``; with the style swap,
         the swap levels swap in the first pass and the others use EFDM.
 
+        ``efdm_slices`` = K in 0..32 (sliced distribution matching, DESIGN.md §3.3.14; with ``efdm``): before the plain EFDM
+        step, each level runs EFDM in K random orthonormal bases of its channels, each on the previous step's output, so the
+        joint distribution of the channels (their correlations, and the shape of their mixtures) moves towards the style's
+        and not only each channel's own.  Every channel still ends with EFDM's marginal.  K = 0 changes nothing.
+
         ``swap_labels`` (labelled style swap, DESIGN.md §3.3.13; with ``swap5`` / ``swap_targets``): a pair (content
         labels, style labels) of uint8 label maps, numpy or torch, host or device: content [Hm,Wm] or [N,Hm,Wm]; style
         [Hm',Wm'] for a shared style, or with one style per frame [Hm',Wm'] or [N,Hm',Wm'].  At every swap level each content
@@ -367,6 +373,7 @@ class WCT(object):
             ("tile_size", tile_size is not None and tile_size != 0), ("seamless", seamless is not None),
             ("temporal", temporal is not None), ("return_float", return_float), ("prepared", prepared),
             ("per_frame_styles", per_frame)) if on}, options.API)
+        efdm_slices = options.check_efdm_slices(efdm_slices, efdm)
         if mask_feather is not None:
             options.check_mask_feather(mask_feather)
         if mst is not None:
@@ -409,7 +416,8 @@ class WCT(object):
             if isinstance(a, PreparedStyle):
                 return a
             a = to_dev(a)
-            return eng.prepare_call(a, adain=adain, swap5=swap5, swap_targets=swap_targets, efdm=efdm) if int(passes) > 1 else a
+            return (eng.prepare_call(a, adain=adain, swap5=swap5, swap_targets=swap_targets, efdm=efdm, efdm_slices=efdm_slices)
+                    if int(passes) > 1 else a)
 
         # wct.py:84-90: with a stride the filter may not fit; centre-crop the content (on the device) to a size it tiles
         Hc0, Wc0 = contents.shape[-3], contents.shape[-2]
@@ -484,7 +492,7 @@ class WCT(object):
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
                                        swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, efdm=efdm,
-                                       swap_labels=lab_dev if first else None, **soft_kw)
+                                       efdm_slices=efdm_slices, swap_labels=lab_dev if first else None, **soft_kw)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -601,13 +609,13 @@ class WCT(object):
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
                 style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
-                strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None):
+                strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
         blend.  ``tile_size`` stylises in tiles, ``ost`` uses the optimal-transport transform, ``seamless`` pads the content
         path circularly, ``mst`` = K matches the content to K modes of the style and ``efdm`` matches every channel's whole
-        value distribution to the style's; ``strength_map``, ``content_weights``
+        value distribution to the style's (first in ``efdm_slices`` rotated bases); ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
         (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap.'''
         s = time.time()
@@ -626,7 +634,7 @@ class WCT(object):
                                  content_mask=content_mask, style_weights=style_weights, style_masks=style_masks,
                                  swap_targets=swap_targets, tile_size=tile_size, ost=ost, seamless=seamless, mst=mst,
                                  mst_smooth=mst_smooth, strength_map=strength_map, content_weights=content_weights,
-                                 mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels)
+                                 mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels, efdm_slices=efdm_slices)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
