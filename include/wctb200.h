@@ -112,6 +112,21 @@ WCTB200_API int wctb200_rgb_moments_u8(const uint8_t* img, long long npix, unsig
 WCTB200_API int wctb200_coral_apply_u8(const uint8_t* src, long long npix, const double* A, const double* src_mean,
                                        const double* src_std, const double* tgt_mean, const double* tgt_std, uint8_t* dst,
                                        void* stream);
+/* rgb_moments of each of N frames img [N][npix_per_frame][3]: sums [N][9] on the DEVICE, frame n's words as rgb_moments_u8
+ * gives them for that frame alone (rgb_moments_u8 is the N = 1 case).  N >= 1, npix_per_frame >= 1, N * npix_per_frame
+ * < 2^40, else WCTB200_EINVAL. */
+WCTB200_API int wctb200_rgb_moments_batch_u8(const uint8_t* img, int N, long long npix_per_frame, unsigned long long* sums,
+                                             void* stream);
+/* Luminance-only transfer (DESIGN.md §3.3.15).  Y = (299 R + 587 G + 114 B) / 1000 per pixel, in fp32 (one correctly
+ * rounded division of the exact integer).  kb: DEVICE float32 [N][2], 8-byte aligned, one (k, b) per frame.
+ * match: dst[n] = clip(rint(k_n Y + b_n), 0, 255) replicated to R = G = B; k = 1, b = 0 makes the grey of an image.
+ * merge: dst[n]_c = clip(rint(content_c + ((k_n Y(stylised) + b_n) - Y(content))), 0, 255) for c in R, G, B.
+ * Every operation is a rounded fp32 fma / add / division in that order (rint: half to even), so frame n's bytes do not
+ * depend on N.  Images are uint8 [N][npix_per_frame][3]; geometry as for rgb_moments_batch_u8. */
+WCTB200_API int wctb200_luminance_match_u8(const uint8_t* src, int N, long long npix_per_frame, const float* kb, uint8_t* dst,
+                                           void* stream);
+WCTB200_API int wctb200_luminance_merge_u8(const uint8_t* content, const uint8_t* stylised, int N, long long npix_per_frame,
+                                           const float* kb, uint8_t* dst, void* stream);
 /* Texture synthesis input (--noise, webcam.py:191-192 np.random.randint(0, 256, shape, np.uint8)): N frames of uniform random
  * bytes, out device uint8 [N][H][W][C].  Frame n has the absolute index f = first_index + n; byte j of its H*W*C bytes
  * (row-major HWC) is byte j % 16 of Philox4x32-10 (Random123) with counter (b_lo, b_hi, f_lo, f_hi), b = j / 16 (64-bit), and

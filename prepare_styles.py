@@ -7,7 +7,8 @@ per style to ``--out-path``.  ``stylize.py`` and ``stylize_video.py`` take these
 
 A file holds the (resized, cropped) style image, the WCT and AdaIN statistics of every target and the relu5_1 feature (for
 ``--swap5``), and with ``--swap-targets reluX_1 ...`` the feature of those levels too (for ``--swap-targets``).  It serves any model with the same encoder weights and semantics, whatever its decoders, and any subset of
-its targets; the model refuses it otherwise.
+its targets; the model refuses it otherwise.  ``--luminance-only`` prepares the grey of each style (same file name), which
+is the form ``--luminance-only`` stylisation takes.
 """
 from __future__ import print_function
 
@@ -31,6 +32,8 @@ def build_parser():
     parser.add_argument("--out-path", type=str, required=True, help="folder that receives <stem>.wctstyle")
     parser.add_argument("--swap-targets", nargs="+", type=str, default=None, metavar="RELU",
                         help="also keep the style feature of these --relu-targets levels, for the style swap there")
+    parser.add_argument("--luminance-only", action="store_true", default=False,
+                        help="prepare the grey of each style, for stylize.py / stylize_video.py --luminance-only")
     return parser
 
 
@@ -62,6 +65,8 @@ def main(argv=None, model_factory=None, image_ops=None):
             img = image_ops.center_crop(img, args.crop_size)
         target = os.path.join(args.out_path, output_name(path))
         kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
+        if args.luminance_only:
+            kw["luminance_only"] = True
         model.prepare_style(img, **kw).save(target)
         print("Prepared {} -> {}".format(path, target))
     print("Prepared {} styles in {:.2f}s".format(len(styles), time.time() - t0))

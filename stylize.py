@@ -58,6 +58,12 @@ rebuilt only from style patches of the same colour, or from all of them where th
 distinct colours of both maps together, sorted by their packed 24-bit value, are the labels.  It takes one style file and
 one content file or ``--noise`` (every noise frame shares the map), and no ``--crop-size``.  Output names are unchanged.
 
+Colour preservation: ``--luminance-only`` stylises the luminance only and puts the content's own colours back on the
+result, so the output keeps the content's palette and takes brightness and texture from the style (DESIGN.md §3.3.15).
+It combines with the options above; not with ``--keep-colors`` or ``--noise``, and a ``.wctstyle`` style must have been
+prepared with ``prepare_styles.py --luminance-only``.  ``--passes`` then run in one call and the colours are merged once,
+after the last.  Output names are unchanged.
+
 Which of these options combine is decided by one table, ``wct_tf_b200/options.py``; a rejected combination is a parser error
 naming both flags.
 
@@ -128,6 +134,8 @@ _FLAGS = [
                                help="with --content-mask: feather the region edges by a Gaussian of SIGMA mask pixels")),
     (("--mask-weights",), dict(nargs="+", type=str, default=None, metavar="W",
                                help="one 8-bit grayscale soft weight map per --mask-styles entry, in place of --content-mask")),
+    (("--luminance-only",), dict(action="store_true", default=False,
+                                 help="stylise the luminance only and keep the content's colours (not with --keep-colors)")),
     (("--swap-labels",), dict(nargs=2, type=str, default=None, metavar=("CONTENT_MAP", "STYLE_MAP"),
                               help="with --swap5 / --swap-targets: flat-colour label maps of the content and the style; each "
                                    "content patch takes only style patches of its own colour")),
@@ -158,6 +166,7 @@ def parse_args(argv=None):
     check_interp_flags(parser, args)
     check_values(parser, args)
     check_options(parser, args)
+    check_luminance_flags(parser, args)
     if args.content_mask is not None:
         if not args.mask_styles:
             parser.error("--content-mask needs --mask-styles")
@@ -262,13 +271,36 @@ def check_options(parser, args):
               content_weights=getattr(args, "mask_weights", None) is not None,
               mask_feather=getattr(args, "mask_feather", None) is not None, strength_map=args.strength_map is not None,
               tile_size=bool(getattr(args, "tile_size", 0)), seamless=args.seamless is not None,
-              temporal=bool(getattr(args, "temporal", 0)),
+              temporal=bool(getattr(args, "temporal", 0)), luminance_only=getattr(args, "luminance_only", False),
               prepared=bool(style_path) and (is_prepared(style_path) or (os.path.isdir(style_path)
                                                                          and any(is_prepared(f) for f in os.listdir(style_path)))))
     try:
         options.check({name for name, v in on.items() if v}, options.CLI)
     except ValueError as e:
         parser.error(str(e))
+
+
+def check_luminance_flags(parser, args):
+    """--luminance-only: not with --keep-colors (both decide the output's colours) or --noise (noise has no colours to
+    keep).  A .wctstyle style must have been prepared with prepare_styles.py --luminance-only; the model checks that when
+    it reads the file."""
+    if not getattr(args, "luminance_only", False):
+        return
+    if args.keep_colors:
+        parser.error("--luminance-only does not combine with --keep-colors: both decide the colours")
+    if getattr(args, "noise", False):
+        parser.error("--luminance-only takes no --noise: noise frames have no colours to keep")
+
+
+def run_passes(model, content_dev, styles, args, kw):
+    """stylize.py:100-104: --passes calls, each on the previous result.  With --luminance-only the passes run in one call
+    on the grey frames and the colours are merged once, after the last (the style swap then acts in the first pass)."""
+    if getattr(args, "luminance_only", False):
+        return model.predict_batch(content_dev, styles, luminance_only=True, passes=args.passes, **kw)
+    result = model.predict_batch(content_dev, styles, **kw)
+    for _ in range(args.passes - 1):
+        result = model.predict_batch(result, styles, **kw)
+    return result
 
 
 def read_grey(path):
@@ -479,10 +511,7 @@ def _stylize_pair(model, content_dev, style_dev, args):
     if getattr(args, "swap_labels", None):
         kw["swap_labels"] = args.swap_label_maps
     kw.update(soft_kw(args))
-    result = model.predict_batch(content_dev, style_dev, **kw)
-    for _ in range(args.passes - 1):
-        result = model.predict_batch(result, style_dev, **kw)
-    return result
+    return run_passes(model, content_dev, style_dev, args, kw)
 
 
 def make_model(args):
@@ -506,10 +535,7 @@ def _stylize_masked(model, content_dev, styles_dev, labels, args, style_masks=No
         kw["seamless"] = args.seamless
     if style_masks is not None:
         kw["style_masks"] = style_masks
-    result = model.predict_batch(content_dev, styles_dev, **kw)
-    for _ in range(args.passes - 1):
-        result = model.predict_batch(result, styles_dev, **kw)
-    return result
+    return run_passes(model, content_dev, styles_dev, args, kw)
 
 
 def _once_per_path(paths, load):
@@ -555,9 +581,7 @@ def main_interp(args, model, io, dimg, t_start):
     prepared = PreparedStyles(model)
     for names, content_dev in _contents(args, io, dimg, device):
         styles_dev = [_prepare_style(p, args, io, dimg, content_dev, device, prepared) for p in args.interp_styles]
-        results = model.predict_batch(content_dev, styles_dev, **kw)
-        for _ in range(args.passes - 1):
-            results = model.predict_batch(results, styles_dev, **kw)
+        results = run_passes(model, content_dev, styles_dev, args, kw)
         for name, result in zip(names, results):
             target = os.path.join(args.out_path, interp_output_name(name, args.interp_styles, args.interp_weights))
             io.save_img(target, dimg.to_host(result))

@@ -30,6 +30,10 @@ Multimodal style transfer: ``--mst K [--mst-smooth LAMBDA]`` matches the content
 Exact feature distribution matching: ``--efdm`` gives every channel of each level the style's whole value distribution
 (DESIGN.md §3.3.12), on both paths; ``--efdm-slices K`` first matches in K random channel rotations (§3.3.14).
 
+Colour preservation: ``--luminance-only`` stylises the luminance and keeps each frame's own colours (DESIGN.md §3.3.15).
+Unlike ``--keep-colors``, which makes every frame its own style, frames of one size stay in batches, and each frame is a
+function of its own content only.  All passes run in one call; the colours are merged after the last.
+
 Which of these options combine is decided by one table, ``wct_tf_b200/options.py``, as for stylize.py.
 """
 from __future__ import division, print_function
@@ -64,7 +68,7 @@ _VIDEO_FLAGS = [
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
            "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
-           "--mst", "--mst-smooth", "--strength-map", "--efdm", "--efdm-slices")
+           "--mst", "--mst-smooth", "--strength-map", "--efdm", "--efdm-slices", "--luminance-only")
 # flags of the one-style mode that --interp-styles takes no part of
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("concat", "--concat")]
 
@@ -105,6 +109,7 @@ def parse_args(argv=None):
     stylize.check_prepared_flags(parser, args)
     stylize.check_values(parser, args)
     stylize.check_options(parser, args)
+    stylize.check_luminance_flags(parser, args)
     return args
 
 
@@ -156,8 +161,10 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
 
     temporal_kw = {} if temporal is None else dict(temporal=temporal)
-    # --ost, --seamless, --mst, --efdm and --efdm-slices, on both paths
+    # --ost, --seamless, --mst, --efdm, --efdm-slices and --luminance-only, on both paths
     opt_kw = dict(ost=True) if getattr(args, "ost", False) else {}
+    if getattr(args, "luminance_only", False):
+        opt_kw["luminance_only"] = True
     if getattr(args, "efdm", False):
         opt_kw["efdm"] = True
     if getattr(args, "efdm_slices", 0):
@@ -204,7 +211,7 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 kw = dict(alpha=args.alpha, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True,
                           **interp_kw(first + j, first + j + 1), **opt_kw)
                 swap_kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
-                if temporal is not None:           # stabilised after the last pass: all passes in one call
+                if temporal is not None or "luminance_only" in opt_kw:   # stabilised / merged after the last pass
                     o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, passes=args.passes,
                                                 **dict(kw, **swap_kw, **temporal_kw))
                 else:

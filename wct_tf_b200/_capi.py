@@ -34,6 +34,9 @@ SIGNATURES = {
     "wctb200_resize_bilinear_u8": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "wctb200_rgb_moments_u8": (_i, [_vp, C.c_longlong, _vp, _vp]),
     "wctb200_coral_apply_u8": (_i, [_vp, C.c_longlong, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "wctb200_rgb_moments_batch_u8": (_i, [_vp, _i, C.c_longlong, _vp, _vp]),
+    "wctb200_luminance_match_u8": (_i, [_vp, _i, C.c_longlong, _vp, _vp, _vp]),
+    "wctb200_luminance_merge_u8": (_i, [_vp, _vp, _i, C.c_longlong, _vp, _vp, _vp]),
     "wctb200_noise_u8": (_i, [_vp, _i, _i, _i, _i, C.c_ulonglong, C.c_longlong, _vp]),
     "wctb200_luminance_u8": (_i, [_vp, C.c_longlong, _vp, _vp]),
     "wctb200_flow_pairs_workspace_bytes": (_sz, [_i, _i, _i]),

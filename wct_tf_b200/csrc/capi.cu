@@ -87,6 +87,10 @@ size_t resize_workspace_bytes(int N, int Hs, int Ws, int C, int Hd, int Wd, int 
 int launch_resize_u8(const uint8_t* src, int N, int Hs, int Ws, int C, int Hd, int Wd, int y0, int x0, int Hout, int Wout,
                      uint8_t* dst, void* ws, size_t ws_bytes, cudaStream_t st);
 int launch_rgb_moments(const uint8_t* img, long long npix, unsigned long long* sums, cudaStream_t st);
+int launch_rgb_moments_batch(const uint8_t* img, int N, long long npf, unsigned long long* sums, cudaStream_t st);
+int launch_luma_match(const uint8_t* src, int N, long long npf, const float* kb, uint8_t* dst, cudaStream_t st);
+int launch_luma_merge(const uint8_t* content, const uint8_t* styl, int N, long long npf, const float* kb, uint8_t* dst,
+                      cudaStream_t st);
 int launch_coral_apply(const uint8_t* src, long long npix, const double* A, const double* sm, const double* ss, const double* tm,
                        const double* ts, uint8_t* dst, cudaStream_t st);
 int launch_noise_u8(uint8_t* out, int N, long long frame_bytes, unsigned long long seed, long long first_index, cudaStream_t st);
@@ -306,6 +310,26 @@ int wctb200_resize_bilinear_u8(const uint8_t* src, int N, int Hs, int Ws, int C,
 int wctb200_rgb_moments_u8(const uint8_t* img, long long npix, unsigned long long* sums, void* stream) {
     WCTB_REQUIRE(img && sums && npix >= 1 && npix < (1ll << 40), "rgb_moments_u8: bad arguments");
     return launch_rgb_moments(img, npix, sums, ST(stream));
+}
+// N frames of npf pixels: every byte offset is 64-bit inside the kernels, and N * npf < 2^40 keeps the integer sums exact
+static bool frames_ok(int N, long long npf) { return N >= 1 && npf >= 1 && npf < (1ll << 40) && (long long)N * npf < (1ll << 40); }
+int wctb200_rgb_moments_batch_u8(const uint8_t* img, int N, long long npix_per_frame, unsigned long long* sums, void* stream) {
+    WCTB_REQUIRE(img && sums, "rgb_moments_batch_u8: null pointer");
+    WCTB_REQUIRE(frames_ok(N, npix_per_frame), "rgb_moments_batch_u8: bad geometry N=%d npix=%lld", N, npix_per_frame);
+    return launch_rgb_moments_batch(img, N, npix_per_frame, sums, ST(stream));
+}
+int wctb200_luminance_match_u8(const uint8_t* src, int N, long long npix_per_frame, const float* kb, uint8_t* dst, void* stream) {
+    WCTB_REQUIRE(src && kb && dst, "luminance_match_u8: null pointer");
+    WCTB_REQUIRE(((uintptr_t)kb & 7) == 0, "luminance_match_u8: kb must be 8-byte aligned");
+    WCTB_REQUIRE(frames_ok(N, npix_per_frame), "luminance_match_u8: bad geometry N=%d npix=%lld", N, npix_per_frame);
+    return launch_luma_match(src, N, npix_per_frame, kb, dst, ST(stream));
+}
+int wctb200_luminance_merge_u8(const uint8_t* content, const uint8_t* stylised, int N, long long npix_per_frame, const float* kb,
+                               uint8_t* dst, void* stream) {
+    WCTB_REQUIRE(content && stylised && kb && dst, "luminance_merge_u8: null pointer");
+    WCTB_REQUIRE(((uintptr_t)kb & 7) == 0, "luminance_merge_u8: kb must be 8-byte aligned");
+    WCTB_REQUIRE(frames_ok(N, npix_per_frame), "luminance_merge_u8: bad geometry N=%d npix=%lld", N, npix_per_frame);
+    return launch_luma_merge(content, stylised, N, npix_per_frame, kb, dst, ST(stream));
 }
 int wctb200_coral_apply_u8(const uint8_t* src, long long npix, const double* A, const double* src_mean, const double* src_std,
                            const double* tgt_mean, const double* tgt_std, uint8_t* dst, void* stream) {

@@ -12,6 +12,10 @@
 // not).  This is byte/integer work bound by HBM: one thread per output pixel, the (<= ksize) taps of a pixel are contiguous
 // in the input row (horizontal) or a strided column walk that neighbouring threads coalesce (vertical).
 //
+// Luminance-only transfer.  The same nine sums per frame give each frame's exact luminance moments on the host; two
+// per-pixel maps (match: RGB -> a grey of given mean and scale; merge: add a luminance difference to all three channels)
+// run before and after the stylisation.
+//
 // CORAL.  The pixel-sized work is (i) nine integer sums per image (sum x_c, sum x_c x_d -- exact in uint64) and (ii) the
 // per-pixel affine map out = (A ((x/255 - m_s) / s_s)) * s_t + m_t in double precision followed by the reference's
 // clip / *255 / truncation.  The 3x3 algebra in between (matSqrt through numpy's SVD, whose sign conventions the
@@ -213,25 +217,29 @@ int launch_resize_u8(const uint8_t* src, int N, int Hs, int Ws, int C, int Hd, i
 // ---------------------------------------------------------------------------
 // CORAL
 // ---------------------------------------------------------------------------
-// sums[0..2] = sum x_c, sums[3..8] = sum x_0x_0, x_0x_1, x_0x_2, x_1x_1, x_1x_2, x_2x_2   (exact integers)
-__global__ void k_rgb_moments(const uint8_t* __restrict__ img, long long npix, unsigned long long* __restrict__ sums) {
-    unsigned long long s[9];
+// Frame n (blockIdx.y, striding by gridDim.y) of N: sums[n][0..2] = sum x_c, sums[n][3..8] = sum x_0x_0, x_0x_1, x_0x_2,
+// x_1x_1, x_1x_2, x_2x_2 over its npf pixels (exact integers)
+__global__ void k_rgb_moments(const uint8_t* __restrict__ img, int N, long long npf, unsigned long long* __restrict__ sums) {
+    for (int n = blockIdx.y; n < N; n += gridDim.y) {
+        const uint8_t* f = img + (long long)n * npf * 3;
+        unsigned long long s[9];
 #pragma unroll
-    for (int i = 0; i < 9; ++i) s[i] = 0ull;
-    for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += (long long)gridDim.x * blockDim.x) {
-        const unsigned int a = img[3 * p], b = img[3 * p + 1], c = img[3 * p + 2];
-        s[0] += a; s[1] += b; s[2] += c;
-        s[3] += a * a; s[4] += a * b; s[5] += a * c;
-        s[6] += b * b; s[7] += b * c; s[8] += c * c;
-    }
+        for (int i = 0; i < 9; ++i) s[i] = 0ull;
+        for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < npf; p += (long long)gridDim.x * blockDim.x) {
+            const unsigned int a = f[3 * p], b = f[3 * p + 1], c = f[3 * p + 2];
+            s[0] += a; s[1] += b; s[2] += c;
+            s[3] += a * a; s[4] += a * b; s[5] += a * c;
+            s[6] += b * b; s[7] += b * c; s[8] += c * c;
+        }
 #pragma unroll
-    for (int i = 0; i < 9; ++i) {
+        for (int i = 0; i < 9; ++i) {
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s[i] += __shfl_xor_sync(0xffffffffu, s[i], o);
-    }
-    if ((threadIdx.x & 31) == 0) {
+            for (int o = 16; o > 0; o >>= 1) s[i] += __shfl_xor_sync(0xffffffffu, s[i], o);
+        }
+        if ((threadIdx.x & 31) == 0) {
 #pragma unroll
-        for (int i = 0; i < 9; ++i) atomicAdd(sums + i, s[i]);     // integer: order-independent, deterministic
+            for (int i = 0; i < 9; ++i) atomicAdd(sums + 9ll * n + i, s[i]);     // integer: order-independent, deterministic
+        }
     }
 }
 
@@ -258,11 +266,25 @@ __global__ void k_coral_apply(const uint8_t* __restrict__ src, long long npix, c
     }
 }
 
-int launch_rgb_moments(const uint8_t* img, long long npix, unsigned long long* sums, cudaStream_t st) {
-    WCTB_CUDA(cudaMemsetAsync(sums, 0, 9 * sizeof(unsigned long long), st));
-    k_rgb_moments<<<grid_for(npix, 256), 256, 0, st>>>(img, npix, sums);
+// Per-frame launches of the frame-axis kernels: frames on y, and the pixels of a frame on x with the grid_for budget shared
+// between the frames of a batch (a 30-frame batch of 512^2 frames gets ~70 blocks per frame, not 1024).
+static dim3 frames_grid(int N, long long npf, int block) {
+    const int ny = N < 65535 ? N : 65535;
+    long long gx = (npf + block - 1) / block;
+    const long long cap = (long long)device_sm_count() * 16 / ny;
+    if (gx > cap) gx = cap;
+    return dim3((unsigned)(gx < 1 ? 1 : gx), (unsigned)ny);
+}
+
+int launch_rgb_moments_batch(const uint8_t* img, int N, long long npf, unsigned long long* sums, cudaStream_t st) {
+    WCTB_CUDA(cudaMemsetAsync(sums, 0, 9ull * N * sizeof(unsigned long long), st));
+    k_rgb_moments<<<frames_grid(N, npf, 256), 256, 0, st>>>(img, N, npf, sums);
     WCTB_CHECK_LAUNCH("k_rgb_moments");
     return 0;
+}
+
+int launch_rgb_moments(const uint8_t* img, long long npix, unsigned long long* sums, cudaStream_t st) {
+    return launch_rgb_moments_batch(img, 1, npix, sums, st);
 }
 
 int launch_coral_apply(const uint8_t* src, long long npix, const double* A, const double* sm, const double* ss, const double* tm,
@@ -277,6 +299,63 @@ int launch_coral_apply(const uint8_t* src, long long npix, const double* A, cons
     }
     k_coral_apply<<<grid_for(npix, 256), 256, 0, st>>>(src, npix, P, dst);
     WCTB_CHECK_LAUNCH("k_coral_apply");
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// Luminance-only transfer (DESIGN.md §3.3.15)
+// ---------------------------------------------------------------------------
+// Y = (299 R + 587 G + 114 B) / 1000: the integer numerator is exact and below 2^24, so Y is one correctly rounded fp32
+// division.  Every step below is an explicitly rounded fp32 operation in a fixed order, so a frame's bytes depend on its
+// pixels and its (k, b) only, never on N or the launch shape.
+__device__ __forceinline__ float luma_bt601(const uint8_t* p) {
+    return __fdiv_rn((float)(299 * (int)p[0] + 587 * (int)p[1] + 114 * (int)p[2]), 1000.0f);
+}
+
+__device__ __forceinline__ uint8_t round_clip8(float v) {
+    v = rintf(v);                                            // half to even, as numpy's rint
+    return (uint8_t)(v < 0.0f ? 0.0f : (v > 255.0f ? 255.0f : v));
+}
+
+// dst[n][p] = replicated clip(rint(k_n Y + b_n)), kb[n] = (k_n, b_n)
+__global__ void k_luma_match_u8(const uint8_t* __restrict__ src, int N, long long npf, const float2* __restrict__ kb,
+                                uint8_t* __restrict__ dst) {
+    for (int n = blockIdx.y; n < N; n += gridDim.y) {
+        const float2 q = kb[n];
+        const long long base = (long long)n * npf * 3;
+        for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < npf; p += (long long)gridDim.x * blockDim.x) {
+            const long long o = base + 3 * p;
+            const uint8_t g = round_clip8(__fmaf_rn(q.x, luma_bt601(src + o), q.y));
+            dst[o] = g; dst[o + 1] = g; dst[o + 2] = g;
+        }
+    }
+}
+
+// dst[n][p][c] = clip(rint(content_c + ((kinv_n Y_S + b_n) - Y_content))), kb[n] = (kinv_n, b_n)
+__global__ void k_luma_merge_u8(const uint8_t* __restrict__ content, const uint8_t* __restrict__ styl, int N, long long npf,
+                                const float2* __restrict__ kb, uint8_t* __restrict__ dst) {
+    for (int n = blockIdx.y; n < N; n += gridDim.y) {
+        const float2 q = kb[n];
+        const long long base = (long long)n * npf * 3;
+        for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < npf; p += (long long)gridDim.x * blockDim.x) {
+            const long long o = base + 3 * p;
+            const float d = __fsub_rn(__fmaf_rn(q.x, luma_bt601(styl + o), q.y), luma_bt601(content + o));
+#pragma unroll
+            for (int c = 0; c < 3; ++c) dst[o + c] = round_clip8(__fadd_rn((float)content[o + c], d));
+        }
+    }
+}
+
+int launch_luma_match(const uint8_t* src, int N, long long npf, const float* kb, uint8_t* dst, cudaStream_t st) {
+    k_luma_match_u8<<<frames_grid(N, npf, 256), 256, 0, st>>>(src, N, npf, reinterpret_cast<const float2*>(kb), dst);
+    WCTB_CHECK_LAUNCH("k_luma_match_u8");
+    return 0;
+}
+
+int launch_luma_merge(const uint8_t* content, const uint8_t* styl, int N, long long npf, const float* kb, uint8_t* dst,
+                      cudaStream_t st) {
+    k_luma_merge_u8<<<frames_grid(N, npf, 256), 256, 0, st>>>(content, styl, N, npf, reinterpret_cast<const float2*>(kb), dst);
+    WCTB_CHECK_LAUNCH("k_luma_merge_u8");
     return 0;
 }
 

@@ -3,7 +3,9 @@
 the ``--concat`` thumbnail stylize.py:107-111), operating on ``torch.uint8`` CUDA tensors HxWx3 (or NxHxWx3) through the C ABI
 (``wctb200_resize_bilinear_u8``, ``wctb200_rgb_moments_u8``, ``wctb200_coral_apply_u8``).  A decoded image goes to the GPU once
 and stays there through resize, crop, CORAL, every ``--passes`` round and the concat; only the finished frame comes back.
-``noise_u8`` makes the noise frames of texture synthesis (``--noise``) on the device (``wctb200_noise_u8``).
+``noise_u8`` makes the noise frames of texture synthesis (``--noise``) on the device (``wctb200_noise_u8``).  The
+``luminance_*`` functions are the pixel steps of luminance-only transfer (``--luminance-only``, DESIGN.md §3.3.15): exact
+per-frame luminance moments, the matched grey and the merge of a stylised luminance into the content's colours.
 
 There is no CPU fallback: the functions raise ``WctB200Error`` when the library or a CUDA device is missing.  The only host
 arithmetic is the 3x3 algebra of CORAL (the reference's ``matSqrt`` goes through ``np.linalg.svd`` and, as written, depends on
@@ -151,6 +153,101 @@ def preserve_colors_np(style_rgb, content_rgb):
         _capi.check(lib.wctb200_coral_apply_u8(src.data_ptr(), src.numel() // 3, keep[0][1], keep[1][1], keep[2][1], keep[3][1],
                                                keep[4][1], out.data_ptr(), _stream()))
     return out
+
+
+# BT.601 luma weights in thousandths: L = 299 R + 587 G + 114 B is an exact integer, Y = L / 1000 (flow.cu's k_luminance)
+LUMA_WEIGHTS = (299, 587, 114)
+
+
+def _frames(img):
+    x, _ = _as_batch(img)
+    if not x.is_cuda:
+        raise _capi.WctB200Error("device_image works on CUDA tensors (use to_device)")
+    if x.shape[-1] != 3:
+        raise ValueError("expected RGB frames, got shape %s" % (tuple(x.shape),))
+    return x.contiguous()
+
+
+def luminance_moments(img):
+    """(npix per frame, [sum L], [sum L^2]) of uint8 RGB frames [H,W,3] or [N,H,W,3], L = 299 R + 587 G + 114 B: exact Python
+    integers per frame, from the device's nine integer sums per frame (``wctb200_rgb_moments_batch_u8``) as w.s1 and
+    w^T S2 w."""
+    lib = _capi.load()
+    x = _frames(img)
+    N, npf = x.shape[0], x.shape[1] * x.shape[2]
+    with torch.cuda.device(x.device):
+        sums = torch.empty((N, 9), dtype=torch.int64, device=x.device)
+        _capi.check(lib.wctb200_rgb_moments_batch_u8(x.data_ptr(), N, npf, sums.data_ptr(), _stream()))
+        rows = sums.cpu().tolist()
+    w0, w1, w2 = LUMA_WEIGHTS
+    s1 = [w0 * r[0] + w1 * r[1] + w2 * r[2] for r in rows]
+    s2 = [w0 * w0 * r[3] + 2 * w0 * w1 * r[4] + 2 * w0 * w2 * r[5] + w1 * w1 * r[6] + 2 * w1 * w2 * r[7] + w2 * w2 * r[8]
+          for r in rows]
+    return npf, s1, s2
+
+
+def luminance_stats_from_moments(npix, s1, s2):
+    """(mean, population std) of Y = L / 1000 in float64 from exact moments of L (scalars or per-frame lists): the
+    variance's numerator n S2 - S1^2 is an exact integer."""
+    one = not isinstance(s1, (list, tuple))
+    s1, s2 = ([s1], [s2]) if one else (s1, s2)
+    mean = np.array([a / (1000.0 * npix) for a in s1])
+    sd = np.sqrt(np.array([float(npix * b - a * a) for a, b in zip(s1, s2)]) / (float(npix) ** 2 * 1e6))
+    return (mean[0], sd[0]) if one else (mean, sd)
+
+
+def luminance_stats(img):
+    """Per-frame (mean, population std) of the luminance Y = (299 R + 587 G + 114 B) / 1000 of uint8 RGB frames on the
+    device: two float64 arrays [N] from exact integer moments."""
+    return luminance_stats_from_moments(*luminance_moments(img))
+
+
+def _kb(k, b, n, device):
+    """Per-frame (k, b) as a device float32 [n, 2] (k and b: scalars or length-n sequences, float64 on the host)."""
+    kb = np.empty((n, 2), np.float32)
+    kb[:, 0], kb[:, 1] = np.broadcast_to(np.asarray(k, np.float64), n), np.broadcast_to(np.asarray(b, np.float64), n)
+    return torch.from_numpy(kb).to(device, non_blocking=True)
+
+
+def luminance_match(img, k, b):
+    """Replicated grey clip(rint(k Y + b)) of uint8 RGB frames on the device (``wctb200_luminance_match_u8``); ``k`` and
+    ``b`` per frame (or one for all)."""
+    lib = _capi.load()
+    x = _frames(img)
+    N, npf = x.shape[0], x.shape[1] * x.shape[2]
+    with torch.cuda.device(x.device):
+        kb = _kb(k, b, N, x.device)
+        out = torch.empty_like(x)
+        _capi.check(lib.wctb200_luminance_match_u8(x.data_ptr(), N, npf, kb.data_ptr(), out.data_ptr(), _stream()))
+    return out if img.dim() == 4 else out[0]
+
+
+def luminance_grey(img):
+    """The grey of uint8 RGB frames: clip(rint(Y)) in R = G = B."""
+    return luminance_match(img, 1.0, 0.0)
+
+
+def luminance_merge(content, stylised, k_inv, b):
+    """Content frames with their luminance replaced by k_inv Y(stylised) + b (per frame), the same difference added to R, G
+    and B so that the content's chrominance stays (``wctb200_luminance_merge_u8``).  Both uint8 RGB, of one shape."""
+    lib = _capi.load()
+    c, s = _frames(content), _frames(stylised)
+    if c.shape != s.shape:
+        raise ValueError("luminance_merge: content %s and stylised %s frames differ in shape" % (tuple(c.shape), tuple(s.shape)))
+    N, npf = c.shape[0], c.shape[1] * c.shape[2]
+    with torch.cuda.device(c.device):
+        kb = _kb(k_inv, b, N, c.device)
+        out = torch.empty_like(c)
+        _capi.check(lib.wctb200_luminance_merge_u8(c.data_ptr(), s.data_ptr(), N, npf, kb.data_ptr(), out.data_ptr(), _stream()))
+    return out if content.dim() == 4 else out[0]
+
+
+def luminance_params(mean_c, sd_c, mean_s, sd_s):
+    """Per-frame parameters of luminance-only transfer from the content's and the style's luminance statistics (float64):
+    k = sd_s / sd_c (1 when either is 0), the match (k, mean_s - k mean_c) and the merge (1/k, mean_c - mean_s / k)."""
+    mean_c, sd_c, mean_s, sd_s = np.broadcast_arrays(*(np.asarray(v, np.float64) for v in (mean_c, sd_c, mean_s, sd_s)))
+    k = np.where((sd_c > 0) & (sd_s > 0), sd_s / np.where(sd_c > 0, sd_c, 1.0), 1.0)
+    return (k, mean_s - k * mean_c), (1.0 / k, mean_c - mean_s / k)
 
 
 def noise_u8(count, height, width, seed=0, first_index=0, device="cuda:0"):

@@ -7,6 +7,9 @@ This is the one statement of that policy.  ``WCT.predict_batch``, ``Engine.styli
 ``swap_labels`` (the labelled style swap, ``check_swap_labels``) has no entry in ``SPELLINGS``: it is a parameter of
 ``swap``, as ``mst_smooth`` is of ``mst``.  It needs the swap, and through it takes the swap's exclusions; it adds none of
 its own.  ``efdm_slices`` (sliced distribution matching, ``check_efdm_slices``) is in the same way a parameter of ``efdm``.
+
+``luminance_only`` (colour preservation) is in ``AROUND``: it runs the whole call on grey frames and merges the colours
+into its uint8 result, so it combines with every option of ``SPELLINGS`` but ``return_float``.
 """
 import numpy as np
 
@@ -31,7 +34,12 @@ SPELLINGS = {
     "prepared": ("a prepared style", None, "prepared styles (.wctstyle)"),
     "per_frame_styles": ("one style per frame", None, None),
 }
-API, ENGINE, CLI = ({name: s[i] for name, s in SPELLINGS.items()} for i in range(3))
+# options that act around the stylising call, on its uint8 frames before and after it, and never reach the engine's levels;
+# spelled as SPELLINGS
+AROUND = {
+    "luminance_only": ("luminance_only", None, "--luminance-only"),
+}
+API, ENGINE, CLI = ({name: s[i] for name, s in list(SPELLINGS.items()) + list(AROUND.items())} for i in range(3))
 
 _MASKS = ("content_mask", "style_masks", "content_weights", "mask_feather")
 
@@ -65,6 +73,7 @@ EXCLUDES = [
     ("temporal", ("return_float",), "temporal stabilisation works on the uint8 frames"),
     ("style_weights", ("content_mask", "swap"), "interpolation blends the transforms of whole styles"),
     ("content_mask", ("adain", "swap"), "spatial control is WCT only"),
+    ("luminance_only", ("return_float",), "the colours are merged into the uint8 frames"),
 ]
 
 # (option, the options of which it needs one)

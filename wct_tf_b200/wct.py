@@ -28,7 +28,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``efdm`` is new: exact feature distribution matching (Zhang et al., CVPR 2022), every channel's values given the
     style's by rank;
   * ``swap_labels`` is new: the labelled style swap (neural doodle, Champandard 2016), each content patch matched only to
-    style patches of its own label.
+    style patches of its own label;
+  * ``luminance_only`` is new: colour preservation (Gatys et al., CVPR 2017, §5), the luminance stylised and the content's
+    colours kept.
 """
 from __future__ import annotations
 
@@ -271,7 +273,7 @@ class WCT(object):
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
                       swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
                       strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None,
-                      efdm_slices=0):
+                      efdm_slices=0, luminance_only=False):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -361,7 +363,18 @@ class WCT(object):
         patch draws only on the style patches with its own label ("water here, trees there"); where the style has no patch
         of that label it draws on all of them.  Maps of any resolution are sampled onto each level's feature grids.  With a
         stride the content is cropped as for the swap, and a content map of exactly the content's size is cropped with it
-        (any other size is stretched over the image as stylised).  Labels act in the first pass only, like the swap."""
+        (any other size is stretched over the image as stylised).  Labels act in the first pass only, like the swap.
+
+        ``luminance_only`` (colour preservation, DESIGN.md §3.3.15): stylise the luminance only and keep the content's
+        colours.  The content frames (after a stride swap's crop) are made grey with the style's luminance mean and spread
+        (``device_image.luminance_match``), the call runs with every other option on them against the grey of each style
+        (``luminance_grey``; a prepared style must have been prepared grey, ``prepare_style(luminance_only=True)``), and
+        after the last pass the stylised luminance, mapped back to the content's mean and spread, replaces the content's
+        luminance in all three channels (``luminance_merge``): the output has the content's YIQ chrominance up to uint8
+        rounding.  With several styles the style statistics are those of their mixture: per frame under ``style_weights``,
+        pooled over the distinct region styles with a content mask or weights.  ``temporal`` stabilises the merged frames.
+        False changes nothing."""
+        call = dict(locals()) if luminance_only else None     # every keyword, re-issued on the grey frames
         prepared = isinstance(styles, PreparedStyle)
         per_frame = not prepared and (isinstance(styles, (list, tuple)) or np.ndim(styles) not in (3, 4)
                                       or (np.ndim(styles) == 4 and styles.shape[0] != 1))
@@ -372,7 +385,7 @@ class WCT(object):
             ("mask_feather", mask_feather is not None), ("strength_map", strength_map is not None),
             ("tile_size", tile_size is not None and tile_size != 0), ("seamless", seamless is not None),
             ("temporal", temporal is not None), ("return_float", return_float), ("prepared", prepared),
-            ("per_frame_styles", per_frame)) if on}, options.API)
+            ("per_frame_styles", per_frame), ("luminance_only", luminance_only)) if on}, options.API)
         efdm_slices = options.check_efdm_slices(efdm_slices, efdm)
         if mask_feather is not None:
             options.check_mask_feather(mask_feather)
@@ -405,6 +418,9 @@ class WCT(object):
                 style_masks = self.check_style_masks(style_masks, region_styles)
             content_mask = mask
         smap = self.check_soft_map(strength_map, n, "strength_map") if strength_map is not None else None
+        if luminance_only:
+            call["swap_labels"] = swap_labels
+            return self._predict_luminance(contents, styles, call, n)
         soft_kw = {}
 
         def to_dev(a):
@@ -429,9 +445,7 @@ class WCT(object):
             if swap_labels is not None:
                 cl, sl = (t if isinstance(t, torch.Tensor) else torch.from_numpy(np.array(t, copy=True, order="C"))
                           for t in swap_labels)
-                if tuple(cl.shape[1:]) == (Hc0, Wc0) and tuple(c.shape[1:3]) != (Hc0, Wc0):
-                    y0, x0 = (Hc0 - c.shape[1]) // 2, (Wc0 - c.shape[2]) // 2      # center_crop_to's window
-                    cl = cl[:, y0:y0 + c.shape[1], x0:x0 + c.shape[2]]
+                cl = self._crop_labels(cl, (Hc0, Wc0), c.shape[1:3])
                 lab_dev = (cl.to(dev, non_blocking=True).contiguous(), sl.to(dev, non_blocking=True).contiguous())
             if smap is not None:
                 soft_kw["strength_map"] = smap.to(dev, non_blocking=True)
@@ -504,20 +518,96 @@ class WCT(object):
             if return_device:
                 eng.check_device()            # synchronises; raises WctB200Error if a kernel recorded a pipeline time-out
                 return (out_dev, out_f) if return_float else out_dev
-            if out is not None:
-                out.copy_(out_dev, non_blocking=True)
-                out_u8 = out
-            else:
-                out_u8 = torch.empty(out_dev.shape, dtype=torch.uint8, pin_memory=True)
-                out_u8.copy_(out_dev, non_blocking=True)
-            # the call is synchronous like sess.run (wct.py:97); a device-side time-out would otherwise leave every
-            # later frame silently wrong (kernels skip their stores once the error word is set)
-            eng.check_device()
-            if out is None:
-                out_u8 = out_u8.numpy().copy()
+            out_u8 = self._to_host(out_dev, out)
         if return_float:
             return out_u8, out_f.cpu().numpy()
         return out_u8
+
+    @staticmethod
+    def _crop_labels(cl, hw0, hw):
+        """A content label map [n,Hm,Wm] of exactly the content's size ``hw0`` cropped with the content to ``hw``
+        (center_crop_to's window); any other map as it is."""
+        if tuple(cl.shape[1:]) == tuple(hw0) and tuple(hw) != tuple(hw0):
+            y0, x0 = (hw0[0] - hw[0]) // 2, (hw0[1] - hw[1]) // 2
+            cl = cl[:, y0:y0 + hw[0], x0:x0 + hw[1]]
+        return cl
+
+    def _to_host(self, out_dev, out):
+        """The uint8 frames ``out_dev`` copied into ``out`` (a pinned uint8 tensor) or into a new numpy array."""
+        if out is not None:
+            out.copy_(out_dev, non_blocking=True)
+            out_u8 = out
+        else:
+            out_u8 = torch.empty(out_dev.shape, dtype=torch.uint8, pin_memory=True)
+            out_u8.copy_(out_dev, non_blocking=True)
+        # the call is synchronous like sess.run (wct.py:97); a device-side time-out would otherwise leave every
+        # later frame silently wrong (kernels skip their stores once the error word is set)
+        self.engine.check_device()
+        if out is None:
+            out_u8 = out_u8.numpy().copy()
+        return out_u8
+
+    @staticmethod
+    def check_grey_prepared(ps):
+        """ValueError unless the prepared style ``ps`` was prepared from a grey image (R = G = B everywhere), which is
+        what luminance-only transfer takes: its statistics come from that image."""
+        img = ps.image
+        if img is None or not ((img[..., 0] == img[..., 1]).all() and (img[..., 1] == img[..., 2]).all()):
+            raise ValueError("luminance_only takes a prepared style only when it was prepared grey: prepare it with "
+                             "prepare_style(style, luminance_only=True) (prepare_styles.py --luminance-only)")
+
+    def _predict_luminance(self, contents, styles, call, n):
+        """predict_batch(luminance_only=True) for a call that has passed predict_batch's checks (DESIGN.md §3.3.15)."""
+        from . import device_image as D
+        from .temporal import stabilize_
+        listed = any(call[k] is not None for k in ("style_weights", "content_mask", "content_weights"))
+        entries = _style_list(styles) if listed else [styles]
+        for x in entries:
+            if isinstance(x, PreparedStyle):
+                self.check_grey_prepared(x)
+        dev = self.engine.device
+        with torch.cuda.device(dev):
+            full = _to_dev(contents, dev)
+            c = self.swap_fit(full, call["swap5"], call["swap_targets"], lambda a: _to_dev(a, dev))
+            if call["swap_labels"] is not None:
+                cl, sl = call["swap_labels"]
+                call["swap_labels"] = (self._crop_labels(cl, full.shape[1:3], c.shape[1:3]), sl)
+            mean_c, sd_c = D.luminance_stats(c)
+            # one grey, and the exact luminance moments of that grey, per distinct style object (the same object stays
+            # the same object, so that style masks keep sharing its side)
+            grey, moments = {}, {}
+            for x in entries:
+                if id(x) not in grey:
+                    img = _to_dev(x.image, dev) if isinstance(x, PreparedStyle) else D.luminance_grey(_to_dev(x, dev))
+                    grey[id(x)] = x if isinstance(x, PreparedStyle) else img
+                    moments[id(x)] = D.luminance_moments(img)
+            if call["style_weights"] is not None:
+                w = self.normalize_weights(call["style_weights"], n, len(entries), dtype=np.float64)      # [1|N, K]
+                st = np.array([D.luminance_stats_from_moments(m[0], m[1][0], m[2][0])
+                               for m in (moments[id(x)] for x in entries)])                               # [K, 2]
+                mean_s = w @ st[:, 0]
+                sd_s = np.sqrt(np.maximum(w @ (st[:, 1] ** 2 + st[:, 0] ** 2) - mean_s ** 2, 0.0))
+            elif listed:
+                npix = sum(m[0] for m in moments.values())
+                mean_s, sd_s = D.luminance_stats_from_moments(npix, sum(m[1][0] for m in moments.values()),
+                                                              sum(m[2][0] for m in moments.values()))
+            else:
+                mean_s, sd_s = D.luminance_stats_from_moments(*moments[id(styles)])
+            (k, b), (k_inv, b_merge) = D.luminance_params(mean_c, sd_c, mean_s, sd_s)
+            # the grey has the cropped content's size, which the call below does not crop again
+            g = D.luminance_match(c, k, b)
+            inner = dict(call, luminance_only=False, temporal=None, out=None, return_device=True)
+            del inner["self"], inner["contents"], inner["styles"]
+            s = self.predict_batch(g, [grey[id(x)] for x in entries] if listed else grey[id(styles)], **inner)
+            if tuple(s.shape[1:3]) != tuple(c.shape[1:3]):        # odd sizes: the decoders round the size up
+                c = D.imresize(c, s.shape[1:3])
+            out_dev = D.luminance_merge(c, s, k_inv, b_merge)
+            if call["temporal"] is not None:
+                stabilize_(call["temporal"], c, out_dev)
+            if call["return_device"]:
+                self.engine.check_device()
+                return out_dev
+            return self._to_host(out_dev, call["out"])
 
     @staticmethod
     def temporal_state(strength):
@@ -527,7 +617,7 @@ class WCT(object):
         from .temporal import TemporalState
         return TemporalState(strength)
 
-    def prepare_style(self, style, swap_targets=None):
+    def prepare_style(self, style, swap_targets=None, luminance_only=False):
         """Prepare ``style`` (uint8 [H,W,3] or [n,H,W,3]; numpy or torch, host or device) once, for any number of calls.
 
         Returns a ``PreparedStyle`` of n styles holding, per relu target, the WCT state for this model's semantics and the
@@ -536,7 +626,8 @@ class WCT(object):
         ``predict`` / ``synthesize`` with n in {1, N}, and as an entry (n = 1) of the style lists of ``style_weights`` and
         ``content_mask``, with ``adain``, ``passes`` and ``swap5``.  The results are byte-identical to the image's.
         ``swap_targets`` (relu targets) keeps the style feature of those levels too, for ``predict_batch(swap_targets=)``;
-        ``save`` stores them."""
+        ``save`` stores them.  ``luminance_only=True`` prepares the grey of the style (``device_image.luminance_grey``), the
+        form ``predict_batch(luminance_only=True)`` takes; used without that option it is simply a grey style."""
         if isinstance(style, PreparedStyle):
             return style
         if style.dtype not in (np.uint8, torch.uint8) or style.ndim not in (3, 4) or style.shape[-1] != 3:
@@ -544,6 +635,9 @@ class WCT(object):
         eng = self.engine
         with torch.cuda.device(eng.device):
             s = _to_dev(style, eng.device)
+            if luminance_only:
+                from .device_image import luminance_grey
+                s = luminance_grey(s)
             ps = eng.prepare(s, swap_targets or ())
             ps.image = s.cpu().numpy()
             ps.fingerprints = dict(eng.fingerprints())
@@ -601,7 +695,9 @@ class WCT(object):
         Texture i depends only on the seed, ``first_index + i`` and the size, the styles and options, and the weights: not
         on ``count``, on how a run is cut into calls, or on the engine's sub-batch groups (the pipeline is batch-invariant,
         tests/test_gpu_invariance.py).  ``synthesize(count=5)`` equals ``synthesize(count=2)`` followed by
-        ``synthesize(count=3, first_index=2)``."""
+        ``synthesize(count=3, first_index=2)``.  ``luminance_only`` is rejected: noise has no colours to keep."""
+        if kw.get("luminance_only"):
+            raise ValueError("synthesize takes no luminance_only: noise frames have no colours to keep")
         from .device_image import noise_u8
         H, W = (size, size) if isinstance(size, (int, np.integer)) else size
         noise = noise_u8(count, H, W, seed=seed, first_index=first_index, device=self.engine.device)
@@ -609,7 +705,8 @@ class WCT(object):
 
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
                 style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
-                strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0):
+                strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0,
+                luminance_only=False):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
@@ -617,7 +714,8 @@ class WCT(object):
         path circularly, ``mst`` = K matches the content to K modes of the style and ``efdm`` matches every channel's whole
         value distribution to the style's (first in ``efdm_slices`` rotated bases); ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
-        (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap.'''
+        (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap;
+        ``luminance_only`` stylises the luminance and keeps the content's colours.'''
         s = time.time()
         seen = {}
 
@@ -634,7 +732,8 @@ class WCT(object):
                                  content_mask=content_mask, style_weights=style_weights, style_masks=style_masks,
                                  swap_targets=swap_targets, tile_size=tile_size, ost=ost, seamless=seamless, mst=mst,
                                  mst_smooth=mst_smooth, strength_map=strength_map, content_weights=content_weights,
-                                 mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels, efdm_slices=efdm_slices)
+                                 mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels, efdm_slices=efdm_slices,
+                                 luminance_only=luminance_only)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
