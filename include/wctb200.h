@@ -127,6 +127,15 @@ WCTB200_API int wctb200_luminance_match_u8(const uint8_t* src, int N, long long 
                                            void* stream);
 WCTB200_API int wctb200_luminance_merge_u8(const uint8_t* content, const uint8_t* stylised, int N, long long npix_per_frame,
                                            const float* kb, uint8_t* dst, void* stream);
+/* Coarse-to-fine join (DESIGN.md §3.3.16): content [N][H][W][3], coarse_content and coarse_stylised [N][h][w][3], all uint8
+ * on the device; dst [N][H][W][3] = clip(rint(content + U(coarse_stylised - coarse_content)), 0, 255), the content with its
+ * low band replaced by the stylised one.  U is bilinear upsampling (or downsampling, for h > H) with half-pixel centres: per
+ * axis sy = h / H (one fp32 division), ys = (y + 0.5) sy - 0.5 clamped to [0, h - 1], taps y0 = floor(ys), y1 =
+ * min(y0 + 1, h - 1), weight wy = ys - y0; the same for x.  The four differences are exact; a = d00 + wx (d01 - d00), b
+ * likewise for row y1, v = a + wy (b - a), each a rounded fp32 operation with no contraction, rint half to even.  Frame n's
+ * bytes do not depend on N.  1 <= H, W, h, w <= 2^15, N H W < 2^40, else WCTB200_EINVAL. */
+WCTB200_API int wctb200_coarse_join_u8(const uint8_t* content, const uint8_t* coarse_content, const uint8_t* coarse_stylised,
+                                       int N, int H, int W, int h, int w, uint8_t* dst, void* stream);
 /* Texture synthesis input (--noise, webcam.py:191-192 np.random.randint(0, 256, shape, np.uint8)): N frames of uniform random
  * bytes, out device uint8 [N][H][W][C].  Frame n has the absolute index f = first_index + n; byte j of its H*W*C bytes
  * (row-major HWC) is byte j % 16 of Philox4x32-10 (Random123) with counter (b_lo, b_hi, f_lo, f_hi), b = j / 16 (64-bit), and

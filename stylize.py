@@ -64,6 +64,12 @@ It combines with the options above; not with ``--keep-colors`` or ``--noise``, a
 prepared with ``prepare_styles.py --luminance-only``.  ``--passes`` then run in one call and the colours are merged once,
 after the last.  Output names are unchanged.
 
+Scale control: ``--coarse-to-fine F`` (2..16; 0 is off) stylises a copy of the content at about 1/F of its size at every
+level first, puts that result's low band into the content, and then runs only the fine levels (``--fine-targets``; default
+those of relu3_1, relu2_1 and relu1_1 among ``--relu-targets``) at full size (DESIGN.md §3.3.16).  The style's large
+structures then come out about F times larger on a large image while its fine texture keeps its own scale, and the deep
+levels run on 1/F^2 of the pixels.  Not with the style swap, ``--seamless`` or ``--mst``.  Output names are unchanged.
+
 Which of these options combine is decided by one table, ``wct_tf_b200/options.py``; a rejected combination is a parser error
 naming both flags.
 
@@ -136,6 +142,12 @@ _FLAGS = [
                                help="one 8-bit grayscale soft weight map per --mask-styles entry, in place of --content-mask")),
     (("--luminance-only",), dict(action="store_true", default=False,
                                  help="stylise the luminance only and keep the content's colours (not with --keep-colors)")),
+    (("--coarse-to-fine",), dict(type=int, default=0, metavar="F",
+                                 help="scale control: stylise a 1/F copy at every level, then the --fine-targets at full size "
+                                      "(2..16; 0: off)")),
+    (("--fine-targets",), dict(nargs="+", type=str, default=None, metavar="RELU",
+                               help="with --coarse-to-fine: the levels run at full size (default: relu3_1 relu2_1 relu1_1 "
+                                    "among --relu-targets)")),
     (("--swap-labels",), dict(nargs=2, type=str, default=None, metavar=("CONTENT_MAP", "STYLE_MAP"),
                               help="with --swap5 / --swap-targets: flat-colour label maps of the content and the style; each "
                                    "content patch takes only style patches of its own colour")),
@@ -241,7 +253,8 @@ def check_swap_label_flags(parser, args):
 
 def check_values(parser, args):
     """The values of --tile-size (0: off), --mst / --mst-smooth (which needs --mst and defaults to 0.05 here),
-    --mask-feather, --efdm-slices and --temporal (stylize_video.py), as wct_tf_b200/options.py checks them."""
+    --mask-feather, --efdm-slices, --coarse-to-fine / --fine-targets and --temporal (stylize_video.py), as
+    wct_tf_b200/options.py checks them."""
     from wct_tf_b200 import options
     try:
         if getattr(args, "tile_size", 0):
@@ -255,6 +268,8 @@ def check_values(parser, args):
         if getattr(args, "mask_feather", None) is not None:
             options.check_mask_feather(args.mask_feather, "--mask-feather")
         options.check_efdm_slices(args.efdm_slices, args.efdm, options.CLI)
+        if getattr(args, "coarse_to_fine", 0) or getattr(args, "fine_targets", None) is not None:
+            options.check_coarse_to_fine(args.coarse_to_fine or None, args.fine_targets, args.relu_targets or [], options.CLI)
         if hasattr(args, "temporal"):
             options.check_temporal_strength(args.temporal, "--temporal")
     except ValueError as e:
@@ -272,6 +287,7 @@ def check_options(parser, args):
               mask_feather=getattr(args, "mask_feather", None) is not None, strength_map=args.strength_map is not None,
               tile_size=bool(getattr(args, "tile_size", 0)), seamless=args.seamless is not None,
               temporal=bool(getattr(args, "temporal", 0)), luminance_only=getattr(args, "luminance_only", False),
+              coarse_to_fine=bool(getattr(args, "coarse_to_fine", 0)),
               prepared=bool(style_path) and (is_prepared(style_path) or (os.path.isdir(style_path)
                                                                          and any(is_prepared(f) for f in os.listdir(style_path)))))
     try:
@@ -307,6 +323,13 @@ def read_grey(path):
     """8-bit grayscale map file -> uint8 [H, W] (read as v/255 by the soft spatial-control options)."""
     from PIL import Image
     return np.asarray(Image.open(path).convert("L"), dtype=np.uint8)
+
+
+def scale_kw(args):
+    """predict_batch options of scale control (--coarse-to-fine, --fine-targets) from the parsed flags."""
+    if not getattr(args, "coarse_to_fine", 0):
+        return {}
+    return dict(coarse_to_fine=args.coarse_to_fine, fine_targets=args.fine_targets)
 
 
 def soft_kw(args):
@@ -510,7 +533,7 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw["efdm_slices"] = args.efdm_slices
     if getattr(args, "swap_labels", None):
         kw["swap_labels"] = args.swap_label_maps
-    kw.update(soft_kw(args))
+    kw.update(soft_kw(args), **scale_kw(args))
     return run_passes(model, content_dev, style_dev, args, kw)
 
 
@@ -530,7 +553,7 @@ def _stylize_masked(model, content_dev, styles_dev, labels, args, style_masks=No
     kw = dict(alpha=args.alpha, return_device=True)
     if labels is not None:
         kw["content_mask"] = labels
-    kw.update(soft_kw(args))
+    kw.update(soft_kw(args), **scale_kw(args))
     if args.seamless:
         kw["seamless"] = args.seamless
     if style_masks is not None:
@@ -574,7 +597,8 @@ def main_interp(args, model, io, dimg, t_start):
     """--interp-styles: every content image in the weighted blend of the styles."""
     os.makedirs(args.out_path, exist_ok=True)
     device = model.engine.device
-    kw = dict(alpha=args.alpha, adain=args.adain, return_device=True, style_weights=np.asarray(args.interp_weights, np.float64))
+    kw = dict(alpha=args.alpha, adain=args.adain, return_device=True, style_weights=np.asarray(args.interp_weights, np.float64),
+              **scale_kw(args))
     if args.seamless:
         kw["seamless"] = args.seamless
     written = 0

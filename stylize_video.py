@@ -34,6 +34,9 @@ Colour preservation: ``--luminance-only`` stylises the luminance and keeps each 
 Unlike ``--keep-colors``, which makes every frame its own style, frames of one size stay in batches, and each frame is a
 function of its own content only.  All passes run in one call; the colours are merged after the last.
 
+Scale control: ``--coarse-to-fine F`` with ``--fine-targets`` stylises each frame coarse to fine (DESIGN.md §3.3.16), on
+both paths.
+
 Which of these options combine is decided by one table, ``wct_tf_b200/options.py``, as for stylize.py.
 """
 from __future__ import division, print_function
@@ -68,7 +71,8 @@ _VIDEO_FLAGS = [
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
            "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-patch-size", "--ss-stride", "--adain",
            "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
-           "--mst", "--mst-smooth", "--strength-map", "--efdm", "--efdm-slices", "--luminance-only")
+           "--mst", "--mst-smooth", "--strength-map", "--efdm", "--efdm-slices", "--luminance-only", "--coarse-to-fine",
+           "--fine-targets")
 # flags of the one-style mode that --interp-styles takes no part of
 _INTERP_EXCLUDES = [("style_path", "--style-path"), ("concat", "--concat")]
 
@@ -161,8 +165,10 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
         return dict(style_weights=weights if weights.ndim == 1 else weights[lo:hi])
 
     temporal_kw = {} if temporal is None else dict(temporal=temporal)
-    # --ost, --seamless, --mst, --efdm, --efdm-slices and --luminance-only, on both paths
+    # --ost, --seamless, --mst, --efdm, --efdm-slices, --luminance-only and --coarse-to-fine, on both paths
+    import stylize
     opt_kw = dict(ost=True) if getattr(args, "ost", False) else {}
+    opt_kw.update(stylize.scale_kw(args))
     if getattr(args, "luminance_only", False):
         opt_kw["luminance_only"] = True
     if getattr(args, "efdm", False):
@@ -174,7 +180,6 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
     if getattr(args, "mst", None) is not None:
         opt_kw.update(mst=args.mst, mst_smooth=args.mst_smooth)
     if getattr(args, "strength_map", None):
-        import stylize
         opt_kw["strength_map"] = stylize.read_grey(args.strength_map)   # one map for every frame
 
     def coral(style, fr):

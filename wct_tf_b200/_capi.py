@@ -38,6 +38,7 @@ SIGNATURES = {
     "wctb200_luminance_match_u8": (_i, [_vp, _i, C.c_longlong, _vp, _vp, _vp]),
     "wctb200_luminance_merge_u8": (_i, [_vp, _vp, _i, C.c_longlong, _vp, _vp, _vp]),
     "wctb200_noise_u8": (_i, [_vp, _i, _i, _i, _i, C.c_ulonglong, C.c_longlong, _vp]),
+    "wctb200_coarse_join_u8": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "wctb200_luminance_u8": (_i, [_vp, C.c_longlong, _vp, _vp]),
     "wctb200_flow_pairs_workspace_bytes": (_sz, [_i, _i, _i]),
     "wctb200_flow_pairs": (_i, [_vp, _i, _i, _i, _vp, _vp, _sz, _vp]),

@@ -94,6 +94,8 @@ int launch_luma_merge(const uint8_t* content, const uint8_t* styl, int N, long l
 int launch_coral_apply(const uint8_t* src, long long npix, const double* A, const double* sm, const double* ss, const double* tm,
                        const double* ts, uint8_t* dst, cudaStream_t st);
 int launch_noise_u8(uint8_t* out, int N, long long frame_bytes, unsigned long long seed, long long first_index, cudaStream_t st);
+int launch_coarse_join(const uint8_t* content, const uint8_t* coarse, const uint8_t* styl, int N, int H, int W, int h, int w,
+                       uint8_t* dst, cudaStream_t st);
 int launch_luminance(const uint8_t* rgb, long long npix, float* Y, cudaStream_t st);
 size_t flow_pairs_workspace_bytes(int M, int H, int W);
 int launch_flow_pairs(const float* Y, int M, int H, int W, float* flows, void* ws, size_t ws_bytes, cudaStream_t st);
@@ -330,6 +332,14 @@ int wctb200_luminance_merge_u8(const uint8_t* content, const uint8_t* stylised, 
     WCTB_REQUIRE(((uintptr_t)kb & 7) == 0, "luminance_merge_u8: kb must be 8-byte aligned");
     WCTB_REQUIRE(frames_ok(N, npix_per_frame), "luminance_merge_u8: bad geometry N=%d npix=%lld", N, npix_per_frame);
     return launch_luma_merge(content, stylised, N, npix_per_frame, kb, dst, ST(stream));
+}
+int wctb200_coarse_join_u8(const uint8_t* content, const uint8_t* coarse_content, const uint8_t* coarse_stylised, int N, int H,
+                           int W, int h, int w, uint8_t* dst, void* stream) {
+    WCTB_REQUIRE(content && coarse_content && coarse_stylised && dst, "coarse_join_u8: null pointer");
+    WCTB_REQUIRE(N >= 1 && H >= 1 && W >= 1 && h >= 1 && w >= 1 && H <= (1 << 15) && W <= (1 << 15) && h <= (1 << 15) &&
+                 w <= (1 << 15) && (long long)N * H * W < (1ll << 40),
+                 "coarse_join_u8: bad geometry N=%d %dx%d from %dx%d", N, H, W, h, w);
+    return launch_coarse_join(content, coarse_content, coarse_stylised, N, H, W, h, w, dst, ST(stream));
 }
 int wctb200_coral_apply_u8(const uint8_t* src, long long npix, const double* A, const double* src_mean, const double* src_std,
                            const double* tgt_mean, const double* tgt_std, uint8_t* dst, void* stream) {

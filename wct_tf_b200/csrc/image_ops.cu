@@ -360,6 +360,70 @@ int launch_luma_merge(const uint8_t* content, const uint8_t* styl, int N, long l
 }
 
 // ---------------------------------------------------------------------------
+// Coarse-to-fine join (DESIGN.md §3.3.16)
+// ---------------------------------------------------------------------------
+// One bilinear axis of the join: output coordinate i of n maps to source s = (i + 0.5) sc - 0.5 clamped to [0, m - 1],
+// taps i0 = floor(s) and i1 = min(i0 + 1, m - 1), weight s - i0.  Explicitly rounded fp32, as the NumPy oracle computes it.
+__device__ __forceinline__ void join_taps(int i, float sc, int m, int& i0, int& i1, float& wt) {
+    float s = __fsub_rn(__fmul_rn(__fadd_rn((float)i, 0.5f), sc), 0.5f);
+    s = fminf(fmaxf(s, 0.0f), (float)(m - 1));
+    i0 = (int)s;                                              // s >= 0: truncation is floor
+    i1 = i0 + 1 < m ? i0 + 1 : m - 1;
+    wt = __fsub_rn(s, (float)i0);
+}
+
+// dst = clip(rint(C + U(S - D))): the content with its low band (D, the coarse content) replaced by the stylised low band
+// (S), U the bilinear upsampling from h x w to H x W.  Rows of the N H output rows on y (striding by gridDim.y), columns on
+// x: a warp reads and writes 32 consecutive pixels of one row, and its low-resolution taps are a few pixels of two coarse
+// rows, served by L1 / L2.  Every operation is a rounded fp32 add / sub / mul in a fixed order, so frame n's bytes depend on
+// its own pixels only.
+__global__ void k_coarse_join_u8(const uint8_t* __restrict__ content, const uint8_t* __restrict__ coarse,
+                                 const uint8_t* __restrict__ styl, int N, int H, int W, int h, int w, uint8_t* __restrict__ dst) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= W) return;
+    int x0, x1;
+    float wx;
+    join_taps(x, __fdiv_rn((float)w, (float)W), w, x0, x1, wx);
+    const float sy = __fdiv_rn((float)h, (float)H);
+    const long long rows = (long long)N * H;
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+        const long long n = r / H;
+        const int y = (int)(r - n * H);
+        int y0, y1;
+        float wy;
+        join_taps(y, sy, h, y0, y1, wy);
+        const long long q0 = (n * h + y0) * w, q1 = (n * h + y1) * w;
+        const long long t00 = 3 * (q0 + x0), t01 = 3 * (q0 + x1), t10 = 3 * (q1 + x0), t11 = 3 * (q1 + x1);
+        const long long o = 3 * (r * W + x);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const float d00 = __fsub_rn((float)styl[t00 + c], (float)coarse[t00 + c]);
+            const float d01 = __fsub_rn((float)styl[t01 + c], (float)coarse[t01 + c]);
+            const float d10 = __fsub_rn((float)styl[t10 + c], (float)coarse[t10 + c]);
+            const float d11 = __fsub_rn((float)styl[t11 + c], (float)coarse[t11 + c]);
+            const float a = __fadd_rn(d00, __fmul_rn(wx, __fsub_rn(d01, d00)));
+            const float b = __fadd_rn(d10, __fmul_rn(wx, __fsub_rn(d11, d10)));
+            const float v = __fadd_rn(a, __fmul_rn(wy, __fsub_rn(b, a)));
+            dst[o + c] = round_clip8(__fadd_rn((float)content[o + c], v));
+        }
+    }
+}
+
+int launch_coarse_join(const uint8_t* content, const uint8_t* coarse, const uint8_t* styl, int N, int H, int W, int h, int w,
+                       uint8_t* dst, cudaStream_t st) {
+    const int block = 128;
+    const int gx = cdiv(W, block);
+    const long long rows = (long long)N * H;
+    long long gy = (long long)device_sm_count() * 32 / gx;   // enough resident blocks to cover HBM latency; rows loop
+    if (gy > rows) gy = rows;
+    if (gy > 65535) gy = 65535;
+    if (gy < 1) gy = 1;
+    k_coarse_join_u8<<<dim3((unsigned)gx, (unsigned)gy), block, 0, st>>>(content, coarse, styl, N, H, W, h, w, dst);
+    WCTB_CHECK_LAUNCH("k_coarse_join_u8");
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
 // Noise
 // ---------------------------------------------------------------------------
 // Philox4x32-10 (Salmon et al., SC'11; the Random123 constants)

@@ -250,6 +250,25 @@ def luminance_params(mean_c, sd_c, mean_s, sd_s):
     return (k, mean_s - k * mean_c), (1.0 / k, mean_c - mean_s / k)
 
 
+def coarse_join(content, coarse_content, coarse_stylised):
+    """The join of coarse-to-fine stylisation (DESIGN.md §3.3.16): clip(rint(C + U(S - D))) on the device
+    (``wctb200_coarse_join_u8``), the content frames C [H,W,3] or [N,H,W,3] with their low band, the coarse content D
+    [h,w,3] or [N,h,w,3], replaced by the stylised low band S of D's shape; U is bilinear resampling from h x w to H x W.
+    All uint8 on one CUDA device; returns uint8 of C's shape."""
+    lib = _capi.load()
+    c, d, s = _frames(content), _frames(coarse_content), _frames(coarse_stylised)
+    if d.shape != s.shape or d.shape[0] != c.shape[0] or not (c.device == d.device == s.device):
+        raise ValueError("coarse_join: content %s, coarse content %s and coarse stylised %s frames must be [N,H,W,3], [N,h,w,3] "
+                         "and [N,h,w,3] on one device" % (tuple(c.shape), tuple(d.shape), tuple(s.shape)))
+    N, H, W = c.shape[:3]
+    h, w = d.shape[1:3]
+    with torch.cuda.device(c.device):
+        out = torch.empty_like(c)
+        _capi.check(lib.wctb200_coarse_join_u8(c.data_ptr(), d.data_ptr(), s.data_ptr(), N, H, W, h, w, out.data_ptr(),
+                                               _stream()))
+    return out if content.dim() == 4 else out[0]
+
+
 def noise_u8(count, height, width, seed=0, first_index=0, device="cuda:0"):
     """--noise (webcam.py:191-192, ``np.random.randint(0, 256, shape, np.uint8)``): ``count`` frames of uniform random bytes,
     a uint8 CUDA tensor [count, height, width, 3] made on the device (``wctb200_noise_u8``) on the current stream.  Frame i

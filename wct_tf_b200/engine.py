@@ -805,6 +805,14 @@ class Engine(object):
         return out, None
 
     # ------------------------------------------------------------------ pipeline
+    def run_levels(self, levels=None):
+        """The levels (``model.levels`` entries) a call runs: all for None, else those of ``levels`` in the model's order
+        (``options.check_levels``: ValueError for an empty, repeated or foreign target)."""
+        if levels is None:
+            return self.model.levels
+        keep = options.check_levels(levels, self.model.relu_targets)
+        return [lvl for lvl in self.model.levels if lvl.relu_target in keep]
+
     def swap_levels(self, swap5=False, swap_targets=None):
         """The relu levels a call swaps at: ``swap_targets`` (checked against this model's targets), or relu5_1 for
         ``swap5`` when it is a target (model.py:148).  ValueError for both at once or a level that is not a target."""
@@ -822,7 +830,7 @@ class Engine(object):
     def stylize(self, content_u8, style_u8, alpha=1.0, adain=False, want_info=False, capture=None, swap5=False, ss_alpha=0.6,
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
                 region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05, strength_map=None,
-                content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0):
+                content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0, levels=None):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -889,8 +897,16 @@ class Engine(object):
         K random orthonormal bases of each level's channels, each step rotating the previous one's output, so that the
         joint distribution of the channels approaches the style's; the last step is plain EFDM, and the blend at ``alpha``
         is with the content feature.  K = 0 is plain EFDM.  A ``PreparedStyle`` must come from
-        ``prepare_call(efdm=True, efdm_slices=K)`` with the same K."""
+        ``prepare_call(efdm=True, efdm_slices=K)`` with the same K.
+
+        Level subset (coarse-to-fine stylisation, DESIGN.md §3.3.16): ``levels`` names some of the model's relu targets
+        (``options.check_levels``); only those levels run, in the model's order, each but the last clipped (model.py:86),
+        as in an engine built with only those targets and the same weights.  A style side made for every level serves
+        any subset.  None runs every level.  Not with ``mst``, whose clustering side runs its own level chain."""
         N = content_u8.shape[0]
+        chain = self.run_levels(levels)
+        if levels is not None and mst is not None:
+            raise ValueError("levels does not combine with mst: its clustering side runs its own level chain")
         options.check({name for name, on in (
             ("adain", adain), ("ost", ost), ("efdm", efdm), ("mst", mst is not None), ("swap", swap5 or swap_targets is not None),
             ("content_mask", labels is not None), ("style_masks", region_masks is not None),
@@ -965,7 +981,7 @@ class Engine(object):
                 raise ValueError("interp_weights must be a float32 tensor [1|N, K] on %s" % self.device)
             w = w.contiguous()
             return self._stylize_multi(content_u8, list(interp_styles), alpha, adain, want_info, capture,
-                                       lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]), seamless=seamless)
+                                       lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]), seamless=seamless, run=chain)
         if labels is not None:
             R = len(region_styles) if region_styles is not None else 0
             if not 1 <= R <= 8:
@@ -978,7 +994,8 @@ class Engine(object):
             if region_masks is not None:
                 region_masks = self.check_region_masks(region_masks, region_styles)
             return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
-                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks, seamless=seamless, soft=soft)
+                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks, seamless=seamless, soft=soft,
+                                       run=chain)
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
         if n_style not in (1, N):
@@ -991,7 +1008,8 @@ class Engine(object):
             outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
                                  alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
                                  ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm, efdm_slices=efdm_slices,
-                                 swap_labels=None if swap_labels is None else _frame_labels(swap_labels, i, i + 1))
+                                 swap_labels=None if swap_labels is None else _frame_labels(swap_labels, i, i + 1),
+                                 levels=levels)
                     for i in range(N)]
             return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
@@ -1017,12 +1035,13 @@ class Engine(object):
                     sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
                 return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
                                          seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm, efdm_slices=efdm_slices,
-                                         swap_labels=None if swap_labels is None else _frame_labels(swap_labels, lo, hi))
+                                         swap_labels=None if swap_labels is None else _frame_labels(swap_labels, lo, hi),
+                                         run=chain)
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
                                     swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft, efdm=efdm,
-                                    swap_labels=swap_labels, efdm_slices=efdm_slices)
+                                    swap_labels=swap_labels, efdm_slices=efdm_slices, run=chain)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -1116,10 +1135,12 @@ class Engine(object):
                     m.record_stream(side)
         return sides
 
-    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None, seamless=None, soft=None):
+    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None, seamless=None, soft=None,
+                       run=None):
         """``stylize`` with several styles (spatial control, style interpolation): images are prepared once per call, and
         every style side is shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the
-        label maps or weight rows); ``masks``: the style masks of spatial control (``_region_sides``)."""
+        label maps or weight rows); ``masks``: the style masks of spatial control (``_region_sides``); ``run``: the levels
+        to run (``run_levels``)."""
         N = content_u8.shape[0]
         main = torch.cuda.current_stream(self.device)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
@@ -1130,11 +1151,12 @@ class Engine(object):
             self._group = 0
         if G == 1:
             out = self._stylize_one(content_u8, None, alpha, adain, want_info, capture, multi=per_frame(0, N) + (sides,),
-                                    seamless=seamless, soft=soft)
+                                    seamless=seamless, soft=soft, run=run)
         else:
             out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, adain, False, None,
                                                                                multi=per_frame(lo, hi) + (sides,),
-                                                                               seamless=seamless, soft=_soft_slice(soft, lo, hi)))
+                                                                               seamless=seamless, soft=_soft_slice(soft, lo, hi),
+                                                                               run=run))
         for side in {id(sd.side): sd.side for sd in owned}.values():
             if side is not main:
                 side.wait_stream(main)         # the style states are recycled only after every level used them
@@ -1316,14 +1338,15 @@ class Engine(object):
         return ps.swap[key]
 
     def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
-                     seamless=None, soft=None, efdm=False, swap_labels=None, efdm_slices=0):
+                     seamless=None, soft=None, efdm=False, swap_labels=None, efdm_slices=0, run=None):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
         ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
         optimal-transport transform instead of WCT at the other levels, ``efdm`` exact feature distribution matching (in
         ``efdm_slices`` rotated bases first when > 0);
         ``seamless``: the wrapped axes of the content path
         (the transforms write a reflect halo, which is rewritten before the decoder reads it); ``swap_labels``: the (content
-        [1|N], style [1]) label maps of a labelled swap at the swap levels."""
+        [1|N], style [1]) label maps of a labelled swap at the swap levels; ``run``: the levels to run (``run_levels``;
+        None: all)."""
         wrap = self.wrap_flags(seamless)
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
@@ -1345,8 +1368,8 @@ class Engine(object):
             mode, per_frame, sides = multi
         infos = []
         x = content
-        nlev = len(self.model.levels)
-        for lvl in self.model.levels:
+        run = self.model.levels if run is None else run
+        for lvl in run:
             relu = lvl.relu_target
             self._tag = relu
             cf, _ = self.encode(x, relu, seamless=seamless)
@@ -1399,7 +1422,7 @@ class Engine(object):
                 capture.setdefault("content_feat", []).append(cf)
                 capture.setdefault("transformed", []).append(f)
             # model.py:86: clip between levels; model.py:94: last output unclipped
-            x = self.decode(f, lvl.index, clip=(lvl.index < nlev - 1), seamless=seamless)
+            x = self.decode(f, lvl.index, clip=lvl is not run[-1], seamless=seamless)
             if capture is not None:
                 capture.setdefault("level_output", []).append(x)
         self._tag = None
@@ -1523,15 +1546,16 @@ class Engine(object):
             out[:, y0:oy1, x0:ox1] = dec[:, y0 - cy0:oy1 - cy0, x0 - cx0:ox1 - cx0]
         return out
 
-    def stylize_tiled(self, content_u8, style_u8, alpha=1.0, adain=False, tile_size=1024, ost=False, seamless=None):
+    def stylize_tiled(self, content_u8, style_u8, alpha=1.0, adain=False, tile_size=1024, ost=False, seamless=None, levels=None):
         """``stylize`` in tiles of ``tile_size`` (a positive multiple of 16) at every level, in bounded device memory: the
         working set follows the largest crop, (tile_size + 2 h_B)^2, not the image.  Each level's statistics are those of
         the whole image, so the result is the untiled one up to the order in which the statistics are summed, and byte
         for byte the same when one tile covers the image.  ``style_u8``: a cuda uint8 image batch or a ``PreparedStyle``
         of 1 or N styles.  The frames run one after another, each with its own statistics; the style side is untiled.
         ``ost``: the optimal-transport transform (DESIGN.md §3.3.8) instead of WCT.  ``seamless``: as for
-        ``stylize`` (``tiled_level``)."""
+        ``stylize`` (``tiled_level``).  ``levels``: the subset of levels to run, as for ``stylize``."""
         T = options.check_tile_size(tile_size)
+        run = self.run_levels(levels)
         options.check({name for name, on in (("tile_size", True), ("adain", adain), ("ost", ost),
                                              ("seamless", seamless is not None)) if on}, options.ENGINE)
         N = content_u8.shape[0]
@@ -1544,20 +1568,19 @@ class Engine(object):
             self.check_prepared(style_u8, adain)
         main = torch.cuda.current_stream(self.device)
         side = style_u8 if prepared else self._style_side(style_u8, main, wct=not adain, adain=adain)
-        nlev = len(self.model.levels)
         outs = []
         for i in range(N):
             sd = side if n_style == 1 else self.slice_prepared(side, i, i + 1)
             x = torch.empty((1,) + tuple(content_u8.shape[1:]), dtype=torch.float32, device=self.device)
             self._call("u8_to_f32", 1, self.lib.wctb200_image_u8_to_f32, content_u8[i].data_ptr(), x.numel(), x.data_ptr(),
                        self._stream())
-            for lvl in self.model.levels:
+            for lvl in run:
                 self._tag = lvl.relu_target
                 if sd.side is not main:
                     sd.wait(main, lvl.relu_target)
                 state = sd.adain[lvl.relu_target] if adain else sd.wct[lvl.relu_target]
                 # model.py:86: clip between levels; model.py:94: last output unclipped
-                x = self.tiled_level(x, lvl.index, state, alpha, adain, T, clip=lvl.index < nlev - 1, ost=ost, seamless=seamless)
+                x = self.tiled_level(x, lvl.index, state, alpha, adain, T, clip=lvl is not run[-1], ost=ost, seamless=seamless)
             self._tag = None
             outs.append(x)
         if prepared:

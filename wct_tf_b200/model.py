@@ -113,6 +113,13 @@ def tile_grid(H, W, T):
     return [(y0, min(y0 + T, H), x0, min(x0 + T, W)) for y0 in range(0, H, T) for x0 in range(0, W, T)]
 
 
+def coarse_size(H, W, f, g):
+    """Size (h, w) of the coarse stage of coarse-to-fine stylisation (DESIGN.md §3.3.16) of an H x W content at factor ``f``:
+    each side divided by f and rounded to the nearest multiple of g = 2^(pools to the deepest target), halves up, at least g,
+    so that every level of the coarse stage decodes exactly h x w."""
+    return tuple(g * max(1, (2 * n + f * g) // (2 * f * g)) for n in (H, W))
+
+
 SEAMLESS_MODES = (None, "x", "y", "xy")
 
 

@@ -8,6 +8,10 @@ This is the one statement of that policy.  ``WCT.predict_batch``, ``Engine.styli
 ``swap``, as ``mst_smooth`` is of ``mst``.  It needs the swap, and through it takes the swap's exclusions; it adds none of
 its own.  ``efdm_slices`` (sliced distribution matching, ``check_efdm_slices``) is in the same way a parameter of ``efdm``.
 
+``coarse_to_fine`` (scale control, ``check_coarse_to_fine``) is in ``AROUND`` too: it runs the call on a downscaled
+content at every level, joins the result into the content's low band and runs the fine levels on that at full size.
+``fine_targets`` is its parameter.  The engine's part is ``levels=``, the subset of relu targets a call runs.
+
 ``luminance_only`` (colour preservation) is in ``AROUND``: it runs the whole call on grey frames and merges the colours
 into its uint8 result, so it combines with every option of ``SPELLINGS`` but ``return_float``.
 """
@@ -34,10 +38,11 @@ SPELLINGS = {
     "prepared": ("a prepared style", None, "prepared styles (.wctstyle)"),
     "per_frame_styles": ("one style per frame", None, None),
 }
-# options that act around the stylising call, on its uint8 frames before and after it, and never reach the engine's levels;
-# spelled as SPELLINGS
+# options that act around the stylising call, on its uint8 frames before and after it (coarse-to-fine: before, between and
+# after its two stages); the engine has no such option.  Spelled as SPELLINGS
 AROUND = {
     "luminance_only": ("luminance_only", None, "--luminance-only"),
+    "coarse_to_fine": ("coarse_to_fine", None, "--coarse-to-fine"),
 }
 API, ENGINE, CLI = ({name: s[i] for name, s in list(SPELLINGS.items()) + list(AROUND.items())} for i in range(3))
 
@@ -74,6 +79,9 @@ EXCLUDES = [
     ("style_weights", ("content_mask", "swap"), "interpolation blends the transforms of whole styles"),
     ("content_mask", ("adain", "swap"), "spatial control is WCT only"),
     ("luminance_only", ("return_float",), "the colours are merged into the uint8 frames"),
+    ("coarse_to_fine", ("swap",), "the stride crop and the patch grid depend on the resolution"),
+    ("coarse_to_fine", ("seamless",), "neither the resize nor the join wraps"),
+    ("coarse_to_fine", ("mst",), "its clustering side runs its own level chain"),
 ]
 
 # (option, the options of which it needs one)
@@ -149,6 +157,46 @@ def check_efdm_slices(K, efdm, vocab=API):
     if K and not efdm:
         raise ValueError("%s needs %s: the slices are steps of EFDM" % (name, vocab["efdm"]))
     return int(K)
+
+
+def check_levels(levels, relu_targets, name="levels"):
+    """A subset of the model's ``relu_targets`` (in the model's order) that a call runs: a non-empty sequence of its
+    targets, none repeated.  Returns them as a tuple in the model's order; ValueError otherwise."""
+    if isinstance(levels, str):
+        levels = [levels]
+    levels = [str(r) for r in levels]
+    if not levels:
+        raise ValueError("%s must name at least one relu target" % name)
+    for r in levels:
+        if r not in relu_targets:
+            raise ValueError("%s: %s is not a relu target of this model (%s)" % (name, r, ", ".join(relu_targets)))
+    if len(set(levels)) != len(levels):
+        raise ValueError("%s names a relu target more than once: %s" % (name, ", ".join(levels)))
+    return tuple(r for r in relu_targets if r in levels)
+
+
+# the levels that carry texture and strokes rather than layout (DESIGN.md §3.3.5): the default fine stage
+FINE_TARGETS = ("relu3_1", "relu2_1", "relu1_1")
+
+
+def check_coarse_to_fine(f, fine_targets, relu_targets, vocab=API):
+    """(f, fine levels) of a coarse-to-fine call (DESIGN.md §3.3.16): ``f`` an integer in 2..16, and ``fine_targets`` a
+    subset of ``relu_targets`` (``check_levels``; None: the model's targets among relu3_1, relu2_1 and relu1_1), returned
+    as a tuple in the model's order.  ValueError otherwise, for ``fine_targets`` without ``f``, and for a model with no
+    default fine level, naming the options as ``vocab`` spells them."""
+    name = vocab["coarse_to_fine"]
+    fine_name = "--fine-targets" if vocab is CLI else "fine_targets"
+    if f is None:
+        raise ValueError("%s needs %s" % (fine_name, name))
+    if isinstance(f, bool) or not isinstance(f, (int, np.integer)) or not 2 <= f <= 16:
+        raise ValueError("%s must be an integer factor in 2..16, got %r" % (name, f))
+    if fine_targets is None:
+        fine = tuple(r for r in relu_targets if r in FINE_TARGETS)
+        if not fine:
+            raise ValueError("%s: the model has none of the default fine targets (%s); give %s"
+                             % (name, ", ".join(FINE_TARGETS), fine_name))
+        return int(f), fine
+    return int(f), check_levels(fine_targets, relu_targets, fine_name)
 
 
 def check_tile_size(tile_size, name="tile_size"):

@@ -30,7 +30,9 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
   * ``swap_labels`` is new: the labelled style swap (neural doodle, Champandard 2016), each content patch matched only to
     style patches of its own label;
   * ``luminance_only`` is new: colour preservation (Gatys et al., CVPR 2017, §5), the luminance stylised and the content's
-    colours kept.
+    colours kept;
+  * ``coarse_to_fine`` is new: scale control (Gatys et al., CVPR 2017, §6), the call run on a downscaled content and its
+    result joined into the content's low band before the fine levels run at full size.
 """
 from __future__ import annotations
 
@@ -273,7 +275,7 @@ class WCT(object):
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
                       swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
                       strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None,
-                      efdm_slices=0, luminance_only=False):
+                      efdm_slices=0, luminance_only=False, coarse_to_fine=None, fine_targets=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -373,7 +375,15 @@ class WCT(object):
         luminance in all three channels (``luminance_merge``): the output has the content's YIQ chrominance up to uint8
         rounding.  With several styles the style statistics are those of their mixture: per frame under ``style_weights``,
         pooled over the distinct region styles with a content mask or weights.  ``temporal`` stabilises the merged frames.
-        False changes nothing."""
+        False changes nothing.
+
+        ``coarse_to_fine`` = f in 2..16 (scale control, DESIGN.md §3.3.16): each pass first stylises, at every level, the
+        content D resized to about 1/f of its size (``model.coarse_size``: sides rounded to multiples of 2^pools, at least
+        one), joins the uint8 result S into the content's low band, J = clip(rint(C + U(S - D))) (``device_image.coarse_join``),
+        and stylises J at full size at ``fine_targets`` only (relu targets; default the model's among relu3_1, relu2_1 and
+        relu1_1).  The style keeps its own size in both stages, so the fine texture keeps the style's pixel scale while the
+        coarse structures come out about f times larger; the deep levels also run on 1/f^2 of the pixels.  Both stages apply
+        one style side, made once per call.  ``return_float`` returns the fine stage's float output.  None changes nothing."""
         call = dict(locals()) if luminance_only else None     # every keyword, re-issued on the grey frames
         prepared = isinstance(styles, PreparedStyle)
         per_frame = not prepared and (isinstance(styles, (list, tuple)) or np.ndim(styles) not in (3, 4)
@@ -385,7 +395,11 @@ class WCT(object):
             ("mask_feather", mask_feather is not None), ("strength_map", strength_map is not None),
             ("tile_size", tile_size is not None and tile_size != 0), ("seamless", seamless is not None),
             ("temporal", temporal is not None), ("return_float", return_float), ("prepared", prepared),
-            ("per_frame_styles", per_frame), ("luminance_only", luminance_only)) if on}, options.API)
+            ("per_frame_styles", per_frame), ("luminance_only", luminance_only),
+            ("coarse_to_fine", coarse_to_fine is not None)) if on}, options.API)
+        ctf = None
+        if coarse_to_fine is not None or fine_targets is not None:
+            ctf = options.check_coarse_to_fine(coarse_to_fine, fine_targets, self.model.relu_targets)
         efdm_slices = options.check_efdm_slices(efdm_slices, efdm)
         if mask_feather is not None:
             options.check_mask_feather(mask_feather)
@@ -426,14 +440,16 @@ class WCT(object):
         def to_dev(a):
             return _to_dev(a, dev)
 
+        once = int(passes) > 1 or ctf is not None           # the style side is applied more than once
+
         def style_dev(a):
-            """A style image on the device, or a prepared style as it is.  With several passes an image is prepared once
-            here, and every pass applies it."""
+            """A style image on the device, or a prepared style as it is.  With several passes, or two coarse-to-fine
+            stages, an image is prepared once here, and every pass and stage applies it."""
             if isinstance(a, PreparedStyle):
                 return a
             a = to_dev(a)
             return (eng.prepare_call(a, adain=adain, swap5=swap5, swap_targets=swap_targets, efdm=efdm, efdm_slices=efdm_slices)
-                    if int(passes) > 1 else a)
+                    if once else a)
 
         # wct.py:84-90: with a stride the filter may not fit; centre-crop the content (on the device) to a size it tiles
         Hc0, Wc0 = contents.shape[-3], contents.shape[-2]
@@ -457,9 +473,9 @@ class WCT(object):
                 w_dev = torch.from_numpy(weights).to(dev, non_blocking=True)
                 ist = [style_dev(x) for x in interp_styles]
 
-                def one_pass(x, first):
+                def one_pass(x, first, levels=None):
                     return eng.stylize(x, None, alpha=alpha, adain=adain, interp_styles=ist, interp_weights=w_dev,
-                                       seamless=seamless)
+                                       seamless=seamless, levels=levels)
             elif content_mask is not None and style_masks is not None:
                 lab = mask.to(dev, non_blocking=True)
                 # the same object stays the same object on the device: the engine shares its side
@@ -472,41 +488,48 @@ class WCT(object):
                         on_dev[id(m)] = m.to(dev, non_blocking=True).contiguous()
                 rs = [on_dev[id(x)] for x in region_styles]
                 sm = [None if m is None else on_dev[id(m)] for m in style_masks]
-                if int(passes) > 1:
+                if once:
                     rs, sm = eng.prepare_regions_call(rs, eng.check_region_masks(sm, rs)), None
 
-                def one_pass(x, first):
+                def one_pass(x, first, levels=None):
                     return eng.stylize(x, None, alpha=alpha, labels=None if content_weights is not None else lab, region_styles=rs,
-                                       region_masks=sm, seamless=seamless, **soft_kw)
+                                       region_masks=sm, seamless=seamless, levels=levels, **soft_kw)
             elif content_mask is not None:
                 lab = mask.to(dev, non_blocking=True)
                 rs = [style_dev(x) for x in region_styles]
 
-                def one_pass(x, first):
+                def one_pass(x, first, levels=None):
                     return eng.stylize(x, None, alpha=alpha, labels=None if content_weights is not None else lab, region_styles=rs,
-                                       seamless=seamless, **soft_kw)
+                                       seamless=seamless, levels=levels, **soft_kw)
             elif mst is not None:
                 s = to_dev(styles)
                 if int(passes) > 1:
                     s = eng.prepare_mst_call(s, mst)
 
-                def one_pass(x, first):
+                def one_pass(x, first, levels=None):
                     return eng.stylize(x, s, alpha=alpha, mst=mst, mst_smooth=mst_smooth)
             elif tile_size is not None:
                 s = style_dev(styles)
 
-                def one_pass(x, first):
-                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size, ost=ost, seamless=seamless)
+                def one_pass(x, first, levels=None):
+                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size, ost=ost, seamless=seamless,
+                                             levels=levels)
             else:
                 s = style_dev(styles)
 
-                def one_pass(x, first):
+                def one_pass(x, first, levels=None):
                     # the style swap acts in the first pass only (stylize_video.py:117-121).  A shared style swaps the
                     # whole batch in one call; with one style per frame the engine swaps frame by frame.
                     return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
                                        swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, efdm=efdm,
-                                       efdm_slices=efdm_slices, swap_labels=lab_dev if first else None, **soft_kw)
+                                       efdm_slices=efdm_slices, swap_labels=lab_dev if first else None, levels=levels,
+                                       **soft_kw)
+            if ctf is not None:
+                whole = one_pass
+
+                def one_pass(x, first):
+                    return self._coarse_to_fine(x, first, whole, *ctf)
             out_f = one_pass(c, True)
             out_dev = eng.to_u8(out_f)
             for _ in range(int(passes) - 1):
@@ -522,6 +545,17 @@ class WCT(object):
         if return_float:
             return out_u8, out_f.cpu().numpy()
         return out_u8
+
+    def _coarse_to_fine(self, x, first, one_pass, f, fine):
+        """One coarse-to-fine pass (DESIGN.md §3.3.16) of the uint8 frames ``x`` [N,H,W,3]: ``one_pass(D, first)`` at every
+        level on the coarse content D, the join J of its uint8 result into x's low band, and ``one_pass(J, first, fine)``
+        at full size.  Returns the fine stage's float output."""
+        from .device_image import coarse_join, imresize
+        from .model import RELU_LEVEL, coarse_size
+        g = 2 ** (RELU_LEVEL[self.model.deepest_target] - 1)
+        d = imresize(x, coarse_size(x.shape[1], x.shape[2], f, g))
+        s = self.engine.to_u8(one_pass(d, first))
+        return one_pass(coarse_join(x, d, s), first, fine)
 
     @staticmethod
     def _crop_labels(cl, hw0, hw):
@@ -706,7 +740,7 @@ class WCT(object):
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
                 style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
                 strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0,
-                luminance_only=False):
+                luminance_only=False, coarse_to_fine=None, fine_targets=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
@@ -715,7 +749,8 @@ class WCT(object):
         value distribution to the style's (first in ``efdm_slices`` rotated bases); ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
         (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap;
-        ``luminance_only`` stylises the luminance and keeps the content's colours.'''
+        ``luminance_only`` stylises the luminance and keeps the content's colours; ``coarse_to_fine`` = f stylises a 1/f
+        copy at every level first and ``fine_targets`` at full size (scale control).'''
         s = time.time()
         seen = {}
 
@@ -733,7 +768,7 @@ class WCT(object):
                                  swap_targets=swap_targets, tile_size=tile_size, ost=ost, seamless=seamless, mst=mst,
                                  mst_smooth=mst_smooth, strength_map=strength_map, content_weights=content_weights,
                                  mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels, efdm_slices=efdm_slices,
-                                 luminance_only=luminance_only)
+                                 luminance_only=luminance_only, coarse_to_fine=coarse_to_fine, fine_targets=fine_targets)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
