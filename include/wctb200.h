@@ -480,6 +480,39 @@ WCTB200_API int wctb200_style_swap_apply_labels(const void* content, int Nc, int
                                     void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* label_buf, size_t label_bytes,
                                     void* stream);
 
+/*
+ * Softmax style swap (DESIGN.md §3.3.17): wctb200_style_swap_apply (or _apply_labels when both label maps are given) with
+ * each anchor's arg-max replaced by a softmax over the patches at temperature tau = `temperature`.  With s(a,n) the hard
+ * swap's scores, ||c_a|| the l2 norm of the whitened content over the anchor's window, K = patch*patch*C and n_p the number
+ * of real patches, z(a,n) = s(a,n) / (||c_a|| sqrt(K / n_p)) (0 where ||c_a|| = 0) and
+ * w(a,n) = exp((z(a,n) - M_a) / tau) / sum_{m in A(a)} exp((z(a,m) - M_a) / tau) on the allowed set A(a) (every patch, or
+ * wctb200_style_swap_apply_labels's set), M_a the maximum of z over A(a).  Every anchor pastes sum_n w(a,n) times the raw
+ * whitened patch n; overlaps are averaged, coloured and blended with `alpha` as in the hard swap.  tau -> 0 gives the hard
+ * swap wherever an anchor's maximum is unique; a large tau the mean of A(a).  The state is the hard swap's, unchanged.
+ *   ws: wctb200_style_swap_softmax_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride) bytes run the apply in one chunk;
+ *   down to wctb200_style_swap_softmax_min_workspace_bytes (one block of patches) it runs in chunks of whole blocks, and
+ *   every size gives the same bytes.  The workspace begins with wctb200_style_swap_apply's layout (the offsets of
+ *   wctb200_debug_style_swap_layout hold).  Less than the minimum is WCTB200_EWS.
+ *   content_labels / style_labels: both NULL (every patch allowed) or both given, with label_buf, as for
+ *   wctb200_style_swap_apply_labels.
+ * A temperature that is not a finite, normal float > 0 (a subnormal has no finite 1/tau) is WCTB200_EINVAL; the other errors
+ * are wctb200_style_swap_apply_labels's.  Frame i of an apply is bit-identical to the apply of that frame alone.
+ * wctb200_style_swap_softmax_launches: the number of kernels an apply with ws_bytes of workspace launches (it grows with
+ * the chunks and the patch blocks), counted as the library's other calls count theirs; 0 for a bad geometry or too
+ * small a workspace.
+ */
+WCTB200_API size_t wctb200_style_swap_softmax_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride);
+WCTB200_API size_t wctb200_style_swap_softmax_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch,
+                                                                  int stride);
+WCTB200_API int wctb200_style_swap_softmax_launches(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride,
+                                                    size_t ws_bytes, int labelled);
+WCTB200_API int wctb200_style_swap_apply_softmax(const void* content, int Nc, int Hc, int Wc, int C, const void* state,
+                                     int Hs, int Ws, int patch, int stride, float alpha, float eps_cov, float thresh,
+                                     float temperature, const uint8_t* content_labels, int Ncl, int Hm, int Wm,
+                                     const uint8_t* style_labels, int Hms, int Wms,
+                                     void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* label_buf, size_t label_bytes,
+                                     void* stream);
+
 /* ---- multimodal style transfer (DESIGN.md §3.3.10; mst.cu) ----------------
  * Spherical k-means of one style feature (SPF16 [1,Hs,Ws,C], C in {64,128,256,512}) into K in 1..8 clusters of the unit
  * directions u_p = f_p / max(|f_p|, 1e-12): k-means++ seeding with Philox4x32-10 draws (counter (j, level, 0, 0)), then at

@@ -52,6 +52,11 @@ Sliced distribution matching: ``--efdm-slices K`` (0..32, with ``--efdm``) first
 level's channels, each on the previous one's output, so that how the channels go together is matched too and not only
 each channel's own values (DESIGN.md §3.3.14).  0 is plain ``--efdm``.  Output names are unchanged.
 
+Softmax swap: ``--ss-temperature T`` (T > 0, with ``--swap5`` / ``--swap-targets``) rebuilds every content patch from a
+blend of style patches weighted by a softmax of their scores at temperature T, instead of its single best patch (DESIGN.md
+§3.3.17).  Small T approaches the hard swap; larger T blends more patches, which softens the seams between neighbouring
+patches (about 0.003 blends a few patches per anchor at relu3_1).  Output names are unchanged.
+
 Labelled style swap (neural doodle): ``--swap-labels CONTENT_MAP STYLE_MAP`` with ``--swap5`` / ``--swap-targets`` gives
 the content and the style each a flat-colour label map (RGB or grey PNG, any resolution); every content patch is then
 rebuilt only from style patches of the same colour, or from all of them where the style has none (DESIGN.md §3.3.13).  The
@@ -107,6 +112,9 @@ _FLAGS = [
     (("--swap-targets",), dict(nargs="+", type=str, default=None, metavar="RELU",
                                help="style swap at these --relu-targets levels (e.g. relu3_1 for brush strokes); not with --swap5")),
     (("--ss-alpha",), dict(type=float, default=0.6, help="blend of the style-swapped feature")),
+    (("--ss-temperature",), dict(type=float, default=None, metavar="T",
+                                 help="with --swap5 / --swap-targets: softmax swap, each content patch a blend of style patches "
+                                      "weighted by a softmax of their scores at temperature T > 0 (not in the reference)")),
     (("--ss-patch-size",), dict(type=int, default=3)),
     (("--ss-stride",), dict(type=int, default=1)),
     # not in the reference
@@ -268,6 +276,7 @@ def check_values(parser, args):
         if getattr(args, "mask_feather", None) is not None:
             options.check_mask_feather(args.mask_feather, "--mask-feather")
         options.check_efdm_slices(args.efdm_slices, args.efdm, options.CLI)
+        options.check_ss_temperature(args.ss_temperature, args.swap5 or args.swap_targets is not None, options.CLI)
         if getattr(args, "coarse_to_fine", 0) or getattr(args, "fine_targets", None) is not None:
             options.check_coarse_to_fine(args.coarse_to_fine or None, args.fine_targets, args.relu_targets or [], options.CLI)
         if hasattr(args, "temporal"):
@@ -519,6 +528,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
     kw = dict(alpha=args.alpha, swap5=args.swap5, ss_alpha=args.ss_alpha, adain=args.adain, return_device=True)
     if args.swap_targets:
         kw["swap_targets"] = list(args.swap_targets)
+    if args.ss_temperature is not None:
+        kw["ss_temperature"] = args.ss_temperature
     if args.tile_size:
         kw["tile_size"] = args.tile_size
     if args.ost:

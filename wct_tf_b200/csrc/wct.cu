@@ -7,6 +7,8 @@
 // Stage C  W_c = E_c D_c^-1/2 E_c^T, C_s = E_s D_s^1/2 E_s^T, T = C_s W_c, M = aT + (1-a)I, bias
 // Stage D  out = M x + bias : the 1-tap mode of the wgmma conv kernel (conv_tc.cu) with a
 //          per-frame weight set, so the apply GEMM runs on the tensor cores.
+#include <cfloat>
+#include <cmath>
 #include <cooperative_groups.h>
 
 #include "common.cuh"
@@ -2686,36 +2688,116 @@ struct SwapLabelMaps {
     size_t buf_bytes;
 };
 
+// checks shared by every apply: the style geometry, the content frames, the tiling of the content encoding and, for a
+// labelled call, its maps and label buffer (*LL gets the buffer's layout)
+static int swap_apply_check(int Nc, int Hc, int Wc, int C, int Hs, int Ws, int patch, int stride, const SwapLabelMaps* maps,
+                            SwapLabelWs* LL) {
+    int rc = swap_check_style(C, Hs, Ws, patch, stride);
+    if (rc) return rc;
+    WCTB_REQUIRE(Nc >= 1 && Hc >= patch && Wc >= patch && Hc >= 2 && Wc >= 2,
+                 "style_swap_apply: %d content maps of %dx%d (patch %d)", Nc, Hc, Wc, patch);
+    // the swapped encoding must have the content's size (ops.py:199 reshapes it to [Hc*Wc, C]); wct.py:84-90 crops the content
+    // image beforehand when the stride makes the filter not fit (utils.swap_filter_fit)
+    const int ho = (Hc - patch) / stride + 1, wo = (Wc - patch) / stride + 1;
+    WCTB_REQUIRE((ho - 1) * stride + patch == Hc && (wo - 1) * stride + patch == Wc,
+                 "style_swap: patch %d / stride %d does not tile a %dx%d encoding (refit the content: swap_filter_fit, wct.py:84-90)",
+                 patch, stride, Hc, Wc);
+    if (maps) {
+        WCTB_REQUIRE(maps->content && maps->style && maps->buf, "style_swap_apply_labels: null pointer");
+        WCTB_REQUIRE((maps->Ncl == 1 || maps->Ncl == Nc) && maps->Hm >= 1 && maps->Wm >= 1 && maps->Hms >= 1 && maps->Wms >= 1,
+                     "style_swap_apply_labels: %d content label maps of %dx%d for %d frames, style labels %dx%d", maps->Ncl,
+                     maps->Hm, maps->Wm, Nc, maps->Hms, maps->Wms);
+        *LL = swap_labels_layout(maps->Ncl, Hc, Wc, Hs, Ws, swap_state_layout(C, Hs, Ws, patch, stride).n_patches);
+        if (maps->buf_bytes < LL->total) {
+            set_error("style_swap_apply_labels: label buffer %zu < %zu bytes", maps->buf_bytes, LL->total);
+            return WCTB200_EWS;
+        }
+    }
+    return 0;
+}
+
+// the content side's whitening over Nc frames (ops.py:187): per-frame mean / covariance, eigensolver, W_c, and the whitened
+// content into wc_feat.  `w` is the apply workspace's wct_layout(C, Nc, 0) block; `zeros` [C] is zeroed here.
+static int swap_apply_whiten(const __half* content, int Nc, int Hc, int Wc, int C, uint8_t* w, float* zeros, float eps_cov,
+                             float thresh, __half* wc_feat, cudaStream_t st) {
+    const WctWs L = wct_layout(C, Nc, 0);
+    double* dsum = reinterpret_cast<double*>(w + L.dsum);
+    float* mean = reinterpret_cast<float*>(w + L.mean);
+    float* G = reinterpret_cast<float*>(w + L.G);
+    float* A0 = reinterpret_cast<float*>(w + L.A0);
+    float* lam = reinterpret_cast<float*>(w + L.lam);
+    float* sigma = reinterpret_cast<float*>(w + L.sigma);
+    float* dvec = reinterpret_cast<float*>(w + L.dvec);
+    float* Wcm = reinterpret_cast<float*>(w + L.Wc);
+    __half* msplit = reinterpret_cast<__half*>(w + L.Msplit);
+    int* mexp = reinterpret_cast<int*>(w + L.Mexp);
+    float* bias = reinterpret_cast<float*>(w + L.bias);
+    float* conv = reinterpret_cast<float*>(w + L.conv);
+    int* kc = reinterpret_cast<int*>(w + L.kcount);
+    const long long CC = (long long)C * C;
+
+    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)Nc * 2 * 4, st));
+    WCTB_CUDA(cudaMemsetAsync(zeros, 0, (size_t)C * 4, st));
+    ActGeom gc(Nc, Hc, Wc, C);
+    int rc = launch_mean_cov(content, gc, eps_cov, mean, G, A0, dsum, st);
+    if (rc) return rc;
+    rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, nullptr, thresh);
+    if (rc) return rc;
+    rc = launch_eig_post(G, A0, lam, C, Nc, thresh, 0.f, Nc, sigma, dvec, kc, st);             // S^-1/2 per frame (ops.py:187)
+    if (rc) return rc;
+    k_outer_gemm<<<dim3((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc), 256, 0, st>>>(G, CC, G, CC, dvec, C, Wcm, CC, C);   // W_c
+    WCTB_CHECK_LAUNCH("k_outer_gemm(whiten)");
+    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), (unsigned)Nc), 256, 0, st>>>(Wcm, C, Nc, 1, 1.f, 0, mean, zeros, msplit, mexp, bias);
+    WCTB_CHECK_LAUNCH("k_finalize_transform(whiten)");
+    return launch_conv_apply(content, Nc, Hc, Wc, C, msplit, Nc, mexp, bias, wc_feat, st);
+}
+
+// the sampled label maps, the patch labels and the present set of a labelled apply
+static int swap_labels_setup(const SwapLabelMaps* maps, const SwapLabelWs& LL, int Hc, int Wc, int Hs, int Ws, const SwapGeom& q,
+                             int n_patches, SwapLabels* lab, cudaStream_t st) {
+    uint8_t* lb = static_cast<uint8_t*>(maps->buf);
+    int rc = launch_labels_resize(maps->content, maps->Ncl, maps->Hm, maps->Wm, Hc, Wc, lb + LL.clab, st);
+    if (rc) return rc;
+    rc = launch_labels_resize(maps->style, 1, maps->Hms, maps->Wms, Hs, Ws, lb + LL.slab, st);
+    if (rc) return rc;
+    uint32_t* present = reinterpret_cast<uint32_t*>(lb + LL.present);
+    WCTB_CUDA(cudaMemsetAsync(present, 0, 8 * sizeof(uint32_t), st));
+    k_swap_patch_labels<<<(unsigned)cdiv(n_patches, 256), 256, 0, st>>>(lb + LL.slab, Ws, q, n_patches, lb + LL.plab, present);
+    WCTB_CHECK_LAUNCH("k_swap_patch_labels");
+    *lab = {lb + LL.clab, maps->Ncl == 1 ? 0ll : (long long)Hc * Wc, lb + LL.plab, present};
+    return 0;
+}
+
+// colour the swapped feature with the style (ops.py:203-206), blend with the content (ops.py:210), report k
+static int swap_apply_finish(const __half* ss_feat, const __half* content, int Nc, int Hc, int Wc, int C, const uint8_t* sp,
+                             const SwapState& SL, const int* kc, float alpha, __half* tmp, __half* out, int32_t* k_out,
+                             cudaStream_t st) {
+    int rc = launch_conv_apply(ss_feat, Nc, Hc, Wc, C, reinterpret_cast<const __half*>(sp + SL.cmsplit), 1,
+                               reinterpret_cast<const int*>(sp + SL.cmexp), reinterpret_cast<const float*>(sp + SL.cbias), tmp, st);
+    if (rc) return rc;
+    const ActGeom gc(Nc, Hc, Wc, C);
+    k_blend2<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(tmp, content, gc, alpha, 1.f - alpha, out);   // ops.py:210
+    WCTB_CHECK_LAUNCH("k_blend2");
+    if (k_out) {
+        // k_out: [k_c x Nc | k_s]
+        WCTB_CUDA(cudaMemcpyAsync(k_out, kc, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
+        WCTB_CUDA(cudaMemcpyAsync(k_out + Nc, sp + SL.k, 4, cudaMemcpyDeviceToDevice, st));
+    }
+    return 0;
+}
+
 // Content side over Nc frames against one prepared style: whiten every frame with its own W_c (ops.py:187), correlate all
 // frames with the shared patch filters in one launch, arg-max and gather per frame, colour with the style, blend.  With
 // `maps` the arg-max is the labelled one (DESIGN.md §3.3.13); everything else is the same launch for launch.
 static int style_swap_apply_impl(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
                                  int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws,
                                  size_t ws_bytes, const SwapLabelMaps* maps, cudaStream_t st) {
-    int rc = swap_check_style(C, Hs, Ws, patch, stride);
-    if (rc) return rc;
-    WCTB_REQUIRE(Nc >= 1 && Hc >= patch && Wc >= patch && Hc >= 2 && Wc >= 2,
-                 "style_swap_apply: %d content maps of %dx%d (patch %d)", Nc, Hc, Wc, patch);
-    const SwapState SL = swap_state_layout(C, Hs, Ws, patch, stride);
-    const SwapApplyWs AL = swap_apply_layout(C, Nc, Hc, Wc, patch, stride, SL.cout_pad);
-    // the swapped encoding must have the content's size (ops.py:199 reshapes it to [Hc*Wc, C]); wct.py:84-90 crops the content
-    // image beforehand when the stride makes the filter not fit (utils.swap_filter_fit)
-    WCTB_REQUIRE((AL.ho - 1) * stride + patch == Hc && (AL.wo - 1) * stride + patch == Wc,
-                 "style_swap: patch %d / stride %d does not tile a %dx%d encoding (refit the content: swap_filter_fit, wct.py:84-90)",
-                 patch, stride, Hc, Wc);
     SwapLabels lab = {nullptr, 0, nullptr, nullptr};
     SwapLabelWs LL = {};
-    if (maps) {
-        WCTB_REQUIRE(maps->content && maps->style && maps->buf, "style_swap_apply_labels: null pointer");
-        WCTB_REQUIRE((maps->Ncl == 1 || maps->Ncl == Nc) && maps->Hm >= 1 && maps->Wm >= 1 && maps->Hms >= 1 && maps->Wms >= 1,
-                     "style_swap_apply_labels: %d content label maps of %dx%d for %d frames, style labels %dx%d", maps->Ncl,
-                     maps->Hm, maps->Wm, Nc, maps->Hms, maps->Wms);
-        LL = swap_labels_layout(maps->Ncl, Hc, Wc, Hs, Ws, SL.n_patches);
-        if (maps->buf_bytes < LL.total) {
-            set_error("style_swap_apply_labels: label buffer %zu < %zu bytes", maps->buf_bytes, LL.total);
-            return WCTB200_EWS;
-        }
-    }
+    int rc = swap_apply_check(Nc, Hc, Wc, C, Hs, Ws, patch, stride, maps, &LL);
+    if (rc) return rc;
+    const SwapState SL = swap_state_layout(C, Hs, Ws, patch, stride);
+    const SwapApplyWs AL = swap_apply_layout(C, Nc, Hc, Wc, patch, stride, SL.cout_pad);
     // chunk width: all cout_pad patches when the workspace holds their scores, else the largest multiple of the whole
     // correlation's N tile that fits (the same tile, hence the same kernel variant and k order, for every chunk)
     const int BN = conv_tc_bn(SL.cout_pad);
@@ -2735,43 +2817,15 @@ static int style_swap_apply_impl(const __half* content, int Nc, int Hc, int Wc, 
     const SwapGeom q = {patch, stride, SL.prow, SL.pcol, AL.ho, AL.wo};
     uint8_t* sw = static_cast<uint8_t*>(ws);
     const uint8_t* sp = static_cast<const uint8_t*>(state);
-    const WctWs L = wct_layout(C, Nc, 0);
-    uint8_t* w = sw + AL.base;
-    double* dsum = reinterpret_cast<double*>(w + L.dsum);
-    float* mean = reinterpret_cast<float*>(w + L.mean);
-    float* G = reinterpret_cast<float*>(w + L.G);
-    float* A0 = reinterpret_cast<float*>(w + L.A0);
-    float* lam = reinterpret_cast<float*>(w + L.lam);
-    float* sigma = reinterpret_cast<float*>(w + L.sigma);
-    float* dvec = reinterpret_cast<float*>(w + L.dvec);
-    float* Wcm = reinterpret_cast<float*>(w + L.Wc);
-    __half* msplit = reinterpret_cast<__half*>(w + L.Msplit);
-    int* mexp = reinterpret_cast<int*>(w + L.Mexp);
-    float* bias = reinterpret_cast<float*>(w + L.bias);
-    float* conv = reinterpret_cast<float*>(w + L.conv);
-    int* kc = reinterpret_cast<int*>(w + L.kcount);
-    float* zeros = reinterpret_cast<float*>(sw + AL.zeros);
+    const int* kc = reinterpret_cast<const int*>(sw + AL.base + wct_layout(C, Nc, 0).kcount);
     int* idx = reinterpret_cast<int*>(sw + AL.idx);
     __half* wc_feat = reinterpret_cast<__half*>(sw + AL.wc_feat);
     __half* ss_feat = reinterpret_cast<__half*>(sw + AL.ss_feat);
     __half* tmp = reinterpret_cast<__half*>(sw + AL.tmp);
     __half* scores = reinterpret_cast<__half*>(sw + AL.scores);
-    const long long CC = (long long)C * C;
-
-    WCTB_CUDA(cudaMemsetAsync(kc, 0, (size_t)Nc * 2 * 4, st));
-    WCTB_CUDA(cudaMemsetAsync(zeros, 0, (size_t)C * 4, st));
     ActGeom gc(Nc, Hc, Wc, C), gs(1, Hs, Ws, C);
-    rc = launch_mean_cov(content, gc, eps_cov, mean, G, A0, dsum, st);
-    if (rc) return rc;
-    rc = launch_jacobi(G, C, Nc, conv, kc + Nc, st, nullptr, thresh);
-    if (rc) return rc;
-    rc = launch_eig_post(G, A0, lam, C, Nc, thresh, 0.f, Nc, sigma, dvec, kc, st);             // S^-1/2 per frame (ops.py:187)
-    if (rc) return rc;
-    k_outer_gemm<<<dim3((unsigned)(C / 64), (unsigned)(C / 64), (unsigned)Nc), 256, 0, st>>>(G, CC, G, CC, dvec, C, Wcm, CC, C);   // W_c
-    WCTB_CHECK_LAUNCH("k_outer_gemm(whiten)");
-    k_finalize_transform<<<dim3((unsigned)cdiv(C, 8), (unsigned)Nc), 256, 0, st>>>(Wcm, C, Nc, 1, 1.f, 0, mean, zeros, msplit, mexp, bias);
-    WCTB_CHECK_LAUNCH("k_finalize_transform(whiten)");
-    rc = launch_conv_apply(content, Nc, Hc, Wc, C, msplit, Nc, mexp, bias, wc_feat, st);
+    rc = swap_apply_whiten(content, Nc, Hc, Wc, C, sw + AL.base, reinterpret_cast<float*>(sw + AL.zeros), eps_cov, thresh, wc_feat,
+                           st);
     if (rc) return rc;
     // every style patch is a filter: the P x P correlation of all frames (top-left anchored, all positions; the strided VALID
     // subset is read by the arg-max) runs on the tensor-core conv kernel, `cols` filters (rows n0.. of the state's filter
@@ -2781,17 +2835,8 @@ static int style_swap_apply_impl(const __half* content, int Nc, int Hc, int Wc, 
     float* best_run = reinterpret_cast<float*>(tmp);
     const int npos = AL.ho * AL.wo;
     if (maps) {
-        uint8_t* lb = static_cast<uint8_t*>(maps->buf);
-        rc = launch_labels_resize(maps->content, maps->Ncl, maps->Hm, maps->Wm, Hc, Wc, lb + LL.clab, st);
+        rc = swap_labels_setup(maps, LL, Hc, Wc, Hs, Ws, q, SL.n_patches, &lab, st);
         if (rc) return rc;
-        rc = launch_labels_resize(maps->style, 1, maps->Hms, maps->Wms, Hs, Ws, lb + LL.slab, st);
-        if (rc) return rc;
-        uint32_t* present = reinterpret_cast<uint32_t*>(lb + LL.present);
-        WCTB_CUDA(cudaMemsetAsync(present, 0, 8 * sizeof(uint32_t), st));
-        k_swap_patch_labels<<<(unsigned)cdiv(SL.n_patches, 256), 256, 0, st>>>(lb + LL.slab, Ws, q, SL.n_patches, lb + LL.plab,
-                                                                                present);
-        WCTB_CHECK_LAUNCH("k_swap_patch_labels");
-        lab = {lb + LL.clab, maps->Ncl == 1 ? 0ll : (long long)Hc * Wc, lb + LL.plab, present};
     }
     for (int n0 = 0; n0 < SL.cout_pad; n0 += cols) {
         const int m = SL.cout_pad - n0 < cols ? SL.cout_pad - n0 : cols;
@@ -2808,17 +2853,7 @@ static int style_swap_apply_impl(const __half* content, int Nc, int Hc, int Wc, 
     k_swap_gather<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(reinterpret_cast<const __half*>(sp + SL.feat), gs, q,
                                                                                      idx, gc, ss_feat);
     WCTB_CHECK_LAUNCH("k_swap_gather");
-    rc = launch_conv_apply(ss_feat, Nc, Hc, Wc, C, reinterpret_cast<const __half*>(sp + SL.cmsplit), 1,
-                        reinterpret_cast<const int*>(sp + SL.cmexp), reinterpret_cast<const float*>(sp + SL.cbias), tmp, st);
-    if (rc) return rc;
-    k_blend2<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(tmp, content, gc, alpha, 1.f - alpha, out);   // ops.py:210
-    WCTB_CHECK_LAUNCH("k_blend2");
-    if (k_out) {
-        // k_out: [k_c x Nc | k_s]
-        WCTB_CUDA(cudaMemcpyAsync(k_out, kc, (size_t)Nc * 4, cudaMemcpyDeviceToDevice, st));
-        WCTB_CUDA(cudaMemcpyAsync(k_out + Nc, sp + SL.k, 4, cudaMemcpyDeviceToDevice, st));
-    }
-    return 0;
+    return swap_apply_finish(ss_feat, content, Nc, Hc, Wc, C, sp, SL, kc, alpha, tmp, out, k_out, st);
 }
 int launch_style_swap_apply(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws, int patch,
                             int stride, float alpha, float eps_cov, float thresh, __half* out, int32_t* k_out, void* ws, size_t ws_bytes,
@@ -2833,6 +2868,400 @@ int launch_style_swap_apply_labels(const __half* content, int Nc, int Hc, int Wc
     const SwapLabelMaps maps = {content_labels, Ncl, Hm, Wm, style_labels, Hms, Wms, label_buf, label_bytes};
     return style_swap_apply_impl(content, Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, out, k_out, ws,
                                  ws_bytes, &maps, st);
+}
+
+// ---------------------------------------------------------------------------
+// Softmax style swap (DESIGN.md §3.3.17).  The hard swap's scores s(a,n), from the same correlation launches, become the
+// weights of a softmax over patches:
+//   z(a,n) = s(a,n) r_a,  r_a = 1 / (||c_a|| sqrt(K / n_p))  (0 where ||c_a|| = 0),  ||c_a||^2 = sum of wc^2 over the window
+//   w(a,n) = exp((z - M_a) / tau) / sum_{m in A(a)} exp((z(a,m) - M_a) / tau) on the allowed set A(a), 0 elsewhere
+// and every anchor pastes the w-weighted blend of the raw patches instead of its arg-max; the overlaps are averaged as in
+// k_swap_gather.  The padded patch axis is split into blocks of SOFTMAX_SWAP_BLOCK patches (all of cout_pad when that is
+// smaller).  Pass 1 reduces every (anchor, block) to (max, sum of exp) with a fixed tree and combines the blocks in block
+// order into (M_a, 1/Z_a); pass 2 writes each block's weights into a map and folds them with the patches on the tensor
+// cores.  A chunk is a union of whole blocks, so every workspace size -- hence every batch size -- gives the same bytes.
+// ---------------------------------------------------------------------------
+// B: a multiple of 128 (so every chunk is a multiple of the correlation's N tile); the fold's K = P*P*B stays at 2304 for
+// 3x3 patches, inside the cross-product accumulator bound of DESIGN.md §3.1
+constexpr int SOFTMAX_SWAP_BLOCK = 256;
+// the weights are split to fp16 times 2^15: unscaled, weights below 6e-8 would flush to zero (there are 64 516 patches at
+// relu2_1); the fold's epilogue multiplies by 2^-15, exactly
+constexpr float SOFTMAX_SWAP_WSCALE = 32768.f;
+
+// workspace of a softmax apply: the hard apply's layout with `cols` score columns (wc_feat, ss_feat, tmp -- tmp holds the
+// fold's fp32 sum -- and the scores), then r_a [Nc*ho*wo] | (max, sum) per (anchor, block) | (M_a, 1/Z_a) per anchor | the
+// fold's unscale factor | one block's fold filters [2][C][P*P][B] | the weight map SPF16 [Nc, Hc+P-1, Wc+P-1, B] | the fold
+// of one block SPF16 [Nc, Hc+P-1, Wc+P-1, C]
+struct SwapSoftmaxWs {
+    SwapApplyWs A;
+    size_t ascale, bstat, mz, wscale, filt, wmap, fold, total;
+    int B, nblk;
+};
+static SwapSoftmaxWs swap_softmax_layout(int C, int Nc, int Hc, int Wc, int P, int S, int cout_pad, int cols) {
+    SwapSoftmaxWs L;
+    L.A = swap_apply_layout(C, Nc, Hc, Wc, P, S, cols);
+    L.B = cout_pad < SOFTMAX_SWAP_BLOCK ? cout_pad : SOFTMAX_SWAP_BLOCK;
+    L.nblk = cdiv(cout_pad, L.B);
+    size_t o = L.A.total;
+    auto take = [&](size_t bytes) { size_t r = o; o = align_up(o + bytes, 256); return r; };
+    const size_t na = (size_t)Nc * L.A.ho * L.A.wo;
+    L.ascale = take(na * 4);
+    L.bstat = take(na * L.nblk * sizeof(float2));
+    L.mz = take(na * sizeof(float2));
+    L.wscale = take(4);
+    L.filt = take((size_t)2 * C * P * P * L.B * sizeof(__half));
+    L.wmap = take((size_t)ActGeom(Nc, Hc + P - 1, Wc + P - 1, L.B).plane * 2 * sizeof(__half));
+    L.fold = take((size_t)ActGeom(Nc, Hc + P - 1, Wc + P - 1, C).plane * 2 * sizeof(__half));
+    L.total = o;
+    return L;
+}
+// one chunk (all cout_pad scores), and the least: one block of scores
+size_t style_swap_softmax_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
+    return swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cp).total;
+}
+size_t style_swap_softmax_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
+    return swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cp < SOFTMAX_SWAP_BLOCK ? cp : SOFTMAX_SWAP_BLOCK).total;
+}
+
+// chunk width of a softmax apply in ws_bytes: all cout_pad patches when the workspace holds their scores, else the largest
+// whole number of blocks that fits; 0 when not even one block does
+static int softmax_swap_cols(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, size_t ws_bytes) {
+    const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
+    const SwapSoftmaxWs full = swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cp);
+    if (ws_bytes >= full.total) return cp;
+    int cols = (cp - 1) / full.B * full.B;
+    while (cols >= full.B && swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cols).total > ws_bytes) cols -= full.B;
+    return cols >= full.B ? cols : 0;
+}
+// kernels one softmax apply in ws_bytes launches, counted as the hard apply's 11 are (memsets and copies not counted): the
+// whitening and colouring suffix (8), the anchor factors and the unscale factor (2), per chunk the correlation and the
+// statistics, the combine, the second correlation per chunk when there are several, per block the weights, the filters,
+// the fold and the sum; a labelled apply adds the two label resizes and the patch labels.  0 when ws_bytes is too small.
+int style_swap_softmax_launches(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, size_t ws_bytes, int labelled) {
+    const int cols = softmax_swap_cols(C, Nc, Hc, Wc, Hs, Ws, P, S, ws_bytes);
+    if (cols == 0) return 0;
+    const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
+    const SwapSoftmaxWs L = swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cols);
+    const int chunks = cdiv(cp, cols);
+    return 8 + 2 + 2 * chunks + 1 + (chunks > 1 ? chunks : 0) + 4 * L.nblk + (labelled ? 3 : 0);
+}
+
+// r_a of every anchor of frame blockIdx.y, one warp each: lane l sums wc^2 over the channels l, l+32, .. of every tap in
+// tap order, then a fixed butterfly.  rms_f = sqrt(K / n_p).
+__global__ void k_softmax_swap_anchor_scale(const __half* __restrict__ wc, ActGeom g, SwapGeom q, float rms_f,
+                                            float* __restrict__ ascale) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= q.ho * q.wo) return;
+    const int n = blockIdx.y;
+    const int y = warp / q.wo, x = warp - y * q.wo;
+    float s = 0.f;
+    for (int ky = 0; ky < q.P; ++ky)
+        for (int kx = 0; kx < q.P; ++kx) {
+            const long long pos = ((long long)n * g.Hp + y * q.S + ky + 1) * g.Wp + (x * q.S + kx + 1);
+            for (int c = lane; c < g.C; c += 32) {
+                const float v = merge_f32(wc[pos * g.C + c], wc[g.plane + pos * g.C + c]);
+                s = fmaf(v, v, s);
+            }
+        }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) ascale[(long long)n * q.ho * q.wo + warp] = s > 0.f ? 1.f / (sqrtf(s) * rms_f) : 0.f;
+}
+__global__ void k_softmax_swap_set(float* __restrict__ p, float v) { *p = v; }
+
+// whether patch n (< n_patches) is in the allowed set of an anchor with label l (`any`: no patch carries l)
+template <bool LABELS>
+__device__ __forceinline__ bool softmax_swap_allowed(const SwapLabels& lab, bool any, int l, int n) {
+    if constexpr (LABELS) return any || lab.plab[n] == l;
+    return true;
+}
+// the label of anchor (y, x) of frame n, and whether no patch carries it
+template <bool LABELS>
+__device__ __forceinline__ int softmax_swap_label(const SwapLabels& lab, const ActGeom& g, const SwapGeom& q, int n, int y, int x,
+                                                  bool& any) {
+    any = true;
+    if constexpr (LABELS) {
+        const int o = (q.P - 1) / 2;
+        const int l = lab.clab[n * lab.clab_frame + (long long)(y * q.S + o) * g.W + x * q.S + o];
+        any = ((lab.present[l >> 5] >> (l & 31)) & 1u) == 0u;
+        return l;
+    }
+    return 0;
+}
+
+// z(a,n) = s(a,n) r_a, rounded once.  Pass 1 and pass 2 must form the same z bit for bit, so that z - M_a is exactly 0 at
+// the maximum (w <= 1/Z_a <= 1): with a plain `merge * r - M` the compiler may contract the product into the subtraction
+// (one FFMA, the unrounded product), and at small tau that difference of half an ulp of z becomes a factor exp(delta/tau)
+__device__ __forceinline__ float softmax_swap_z(const __half* __restrict__ scores, const ActGeom& g, long long pos, int j, float r) {
+    return __fmul_rn(merge_f32(scores[pos * g.C + j], scores[g.plane + pos * g.C + j]), r);
+}
+// exp((x - m) / tau), formed the same way wherever it is used
+__device__ __forceinline__ float softmax_swap_exp(float x, float m, float inv_t) { return expf(__fmul_rn(__fsub_rn(x, m), inv_t)); }
+
+constexpr int SOFTMAX_SWAP_PER_LANE = SOFTMAX_SWAP_BLOCK / 32;
+// pass 1: (max_b, sum_b exp((z - max_b) / tau)) over the allowed real patches of each of the `nb` blocks of this chunk
+// (scores of patches [n0, n0 + g.C)), one warp per anchor; lane l takes the block's patches l, l+32, .., then fixed
+// butterflies.  A block without an allowed patch gives (-inf, 0).
+template <bool LABELS>
+__global__ void k_softmax_swap_stats(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n0, int nb, int B, int n_patches,
+                                     const float* __restrict__ ascale, float inv_t, int nblk, float2* __restrict__ bstat,
+                                     SwapLabels lab) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= q.ho * q.wo) return;
+    const int n = blockIdx.y;
+    const int y = warp / q.wo, x = warp - y * q.wo;
+    const long long a = (long long)n * q.ho * q.wo + warp;
+    const long long pos = ((long long)n * g.Hp + y * q.S + 1) * g.Wp + (x * q.S + 1);
+    const float r = ascale[a];
+    bool any;
+    const int l = softmax_swap_label<LABELS>(lab, g, q, n, y, x, any);
+    for (int bi = 0; bi < nb; ++bi) {
+        float z[SOFTMAX_SWAP_PER_LANE];
+        float mx = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < SOFTMAX_SWAP_PER_LANE; ++i) {
+            const int jj = lane + 32 * i, j = bi * B + jj;
+            z[i] = -INFINITY;
+            if (jj < B && n0 + j < n_patches && softmax_swap_allowed<LABELS>(lab, any, l, n0 + j)) {
+                z[i] = softmax_swap_z(scores, g, pos, j, r);
+                mx = fmaxf(mx, z[i]);
+            }
+        }
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        float sum = 0.f;
+        if (mx > -INFINITY) {
+#pragma unroll
+            for (int i = 0; i < SOFTMAX_SWAP_PER_LANE; ++i)
+                if (z[i] > -INFINITY) sum += softmax_swap_exp(z[i], mx, inv_t);
+        }
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        if (lane == 0) bstat[a * nblk + n0 / B + bi] = make_float2(mx, sum);
+    }
+}
+// (M_a, 1/Z_a) from the blocks' (max, sum), in block order
+__global__ void k_softmax_swap_combine(const float2* __restrict__ bstat, long long na, int nblk, float inv_t, float2* __restrict__ mz) {
+    for (long long a = (long long)blockIdx.x * blockDim.x + threadIdx.x; a < na; a += (long long)gridDim.x * blockDim.x) {
+        const float2* t = bstat + a * nblk;
+        float M = -INFINITY;
+        for (int b = 0; b < nblk; ++b) M = fmaxf(M, t[b].x);
+        float Z = 0.f;
+        for (int b = 0; b < nblk; ++b)
+            if (t[b].y > 0.f) Z += t[b].y * softmax_swap_exp(t[b].x, M, inv_t);
+        mz[a] = make_float2(M, 1.f / Z);
+    }
+}
+// pass 2: the weights of block [n0 + c0, n0 + c0 + gm.C) times 2^15, split, at map pixel (y*S + P-1, x*S + P-1) of every
+// anchor; padding, foreign-label and non-patch channels get 0.  One warp per anchor.
+template <bool LABELS>
+__global__ void k_softmax_swap_weights(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n0, int c0, int n_patches,
+                                       const float* __restrict__ ascale, const float2* __restrict__ mz, float inv_t, ActGeom gm,
+                                       __half* __restrict__ wmap, SwapLabels lab) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= q.ho * q.wo) return;
+    const int n = blockIdx.y;
+    const int y = warp / q.wo, x = warp - y * q.wo;
+    const long long a = (long long)n * q.ho * q.wo + warp;
+    const long long pos = ((long long)n * g.Hp + y * q.S + 1) * g.Wp + (x * q.S + 1);
+    const long long mpos = ((long long)n * gm.Hp + y * q.S + q.P) * gm.Wp + (x * q.S + q.P);
+    const float r = ascale[a];
+    const float2 t = mz[a];
+    bool any;
+    const int l = softmax_swap_label<LABELS>(lab, g, q, n, y, x, any);
+    for (int jj = lane; jj < gm.C; jj += 32) {
+        const int j = c0 + jj;
+        float w = 0.f;
+        if (n0 + j < n_patches && softmax_swap_allowed<LABELS>(lab, any, l, n0 + j)) {
+            w = softmax_swap_exp(softmax_swap_z(scores, g, pos, j, r), t.x, inv_t) * t.y * SOFTMAX_SWAP_WSCALE;
+        }
+        __half hi, lo;
+        split_f32(w, hi, lo);
+        wmap[mpos * gm.C + jj] = hi;
+        wmap[gm.plane + mpos * gm.C + jj] = lo;
+    }
+}
+// the fold's filters of the patch block [b0, b0 + B): [plane][c][tap = ky*P + kx][j] = the whitened style (hi, lo as stored)
+// of patch b0 + j at its pixel (P-1-ky, P-1-kx) -- the raw patches, taps flipped; 0 for padding patches
+__global__ void k_softmax_swap_fold_filters(const __half* __restrict__ feat, ActGeom gs, SwapGeom q, int b0, int B, int n_patches,
+                                            __half* __restrict__ filt) {
+    const int PP = q.P * q.P;
+    const long long per = (long long)PP * B, total = per * gs.C;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i / per);
+        const int rem = (int)(i - c * per);
+        const int tap = rem / B, j = rem - tap * B;
+        const int nn = b0 + j;
+        __half hi = __float2half_rn(0.f), lo = hi;
+        if (nn < n_patches) {
+            const int dy = q.P - 1 - tap / q.P, dx = q.P - 1 - tap % q.P;
+            const int py = nn / q.pcol, px = nn - py * q.pcol;
+            const long long pos = ((long long)(py * q.S + dy + 1)) * gs.Wp + (px * q.S + dx + 1);
+            hi = feat[pos * gs.C + c];
+            lo = feat[gs.plane + pos * gs.C + c];
+        }
+        filt[i] = hi;
+        filt[total + i] = lo;
+    }
+}
+// acc (fp32 [Nc][Hc][Wc][C], in the apply's tmp) = / += the fold of one block, read at interior pixel (Y, X) of
+// gf = [Nc, Hc+P-1, Wc+P-1, C]; after the last block the average over the anchors covering (Y, X), split and stored with the
+// halo as k_swap_gather does
+__global__ void k_softmax_swap_accum(const __half* __restrict__ fold, ActGeom gf, SwapGeom q, ActGeom gc, int first, int last,
+                                     float* __restrict__ acc, __half* __restrict__ out) {
+    const int cg = gc.C / 8;
+    const long long hw = (long long)gc.H * gc.W;
+    const long long total = (long long)gc.N * hw * cg;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int c0 = (int)(i % cg) * 8;
+        const long long fp = i / cg;
+        const int n = (int)(fp / hw);
+        const int pix = (int)(fp - n * hw);
+        const int Y = pix / gc.W, X = pix - Y * gc.W;
+        float v[8];
+        load8(fold, gf, ((long long)n * gf.Hp + Y + 1) * gf.Wp + X + 1, c0, v);
+        float4* ap = reinterpret_cast<float4*>(acc + fp * gc.C + c0);
+        if (!first) {
+            const float4 u0 = ap[0], u1 = ap[1];
+            v[0] = u0.x + v[0]; v[1] = u0.y + v[1]; v[2] = u0.z + v[2]; v[3] = u0.w + v[3];
+            v[4] = u1.x + v[4]; v[5] = u1.y + v[5]; v[6] = u1.z + v[6]; v[7] = u1.w + v[7];
+        }
+        if (!last) {
+            ap[0] = make_float4(v[0], v[1], v[2], v[3]);
+            ap[1] = make_float4(v[4], v[5], v[6], v[7]);
+            continue;
+        }
+        int cy = 0, cx = 0;
+        for (int d = 0; d < q.P; ++d) {
+            const int ty = Y - d, tx = X - d;
+            if (ty >= 0 && ty % q.S == 0 && ty / q.S < q.ho) ++cy;
+            if (tx >= 0 && tx % q.S == 0 && tx / q.S < q.wo) ++cx;
+        }
+        const int cnt = cy * cx;
+        const float inv = cnt > 0 ? 1.f / (float)cnt : 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] *= inv;
+        Half8 hi, lo;
+        split8(v, hi, lo);
+        store8_with_halo(out, gc, n, Y, X, c0, hi, lo);
+    }
+}
+
+static int style_swap_apply_softmax_impl(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws,
+                                         int patch, int stride, float alpha, float eps_cov, float thresh, float temperature,
+                                         __half* out, int32_t* k_out, void* ws, size_t ws_bytes, const SwapLabelMaps* maps,
+                                         cudaStream_t st) {
+    // a normal float: a subnormal tau has no finite 1/tau, and (z - M) * inf would be NaN at every maximum
+    WCTB_REQUIRE(std::isfinite(temperature) && temperature >= FLT_MIN && std::isfinite(1.f / temperature),
+                 "style_swap_apply_softmax: temperature %g must be a finite, normal float32 > 0", (double)temperature);
+    SwapLabels lab = {nullptr, 0, nullptr, nullptr};
+    SwapLabelWs LL = {};
+    int rc = swap_apply_check(Nc, Hc, Wc, C, Hs, Ws, patch, stride, maps, &LL);
+    if (rc) return rc;
+    const SwapState SL = swap_state_layout(C, Hs, Ws, patch, stride);
+    const int cp = SL.cout_pad;
+    const int cols = softmax_swap_cols(C, Nc, Hc, Wc, Hs, Ws, patch, stride, ws_bytes);
+    if (cols == 0) {
+        set_error("style_swap_apply_softmax: workspace %zu < %zu bytes", ws_bytes,
+                  style_swap_softmax_min_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride));
+        return WCTB200_EWS;
+    }
+    const SwapSoftmaxWs L = swap_softmax_layout(C, Nc, Hc, Wc, patch, stride, cp, cols);
+    const SwapApplyWs& AL = L.A;
+    const int B = L.B;
+    const SwapGeom q = {patch, stride, SL.prow, SL.pcol, AL.ho, AL.wo};
+    uint8_t* sw = static_cast<uint8_t*>(ws);
+    const uint8_t* sp = static_cast<const uint8_t*>(state);
+    const int* kc = reinterpret_cast<const int*>(sw + AL.base + wct_layout(C, Nc, 0).kcount);
+    __half* wc_feat = reinterpret_cast<__half*>(sw + AL.wc_feat);
+    __half* ss_feat = reinterpret_cast<__half*>(sw + AL.ss_feat);
+    __half* tmp = reinterpret_cast<__half*>(sw + AL.tmp);
+    __half* scores = reinterpret_cast<__half*>(sw + AL.scores);
+    float* ascale = reinterpret_cast<float*>(sw + L.ascale);
+    float2* bstat = reinterpret_cast<float2*>(sw + L.bstat);
+    float2* mz = reinterpret_cast<float2*>(sw + L.mz);
+    float* wscale = reinterpret_cast<float*>(sw + L.wscale);
+    __half* filt = reinterpret_cast<__half*>(sw + L.filt);
+    __half* wmap = reinterpret_cast<__half*>(sw + L.wmap);
+    __half* fold = reinterpret_cast<__half*>(sw + L.fold);
+    const ActGeom gc(Nc, Hc, Wc, C), gs(1, Hs, Ws, C);
+    const ActGeom gm(Nc, Hc + patch - 1, Wc + patch - 1, B), gf(Nc, Hc + patch - 1, Wc + patch - 1, C);
+    rc = swap_apply_whiten(content, Nc, Hc, Wc, C, sw + AL.base, reinterpret_cast<float*>(sw + AL.zeros), eps_cov, thresh, wc_feat,
+                           st);
+    if (rc) return rc;
+    if (maps) {
+        rc = swap_labels_setup(maps, LL, Hc, Wc, Hs, Ws, q, SL.n_patches, &lab, st);
+        if (rc) return rc;
+    }
+    const long long K = (long long)patch * patch * C;
+    const __half* wsplit = reinterpret_cast<const __half*>(sp + SL.wsplit);
+    const int BN = conv_tc_bn(cp);
+    const int npos = AL.ho * AL.wo;
+    const float inv_t = 1.f / temperature;
+    const dim3 agrid((unsigned)cdiv((long long)npos * 32, 256), (unsigned)Nc);
+    k_softmax_swap_anchor_scale<<<agrid, 256, 0, st>>>(wc_feat, gc, q, (float)std::sqrt((double)K / SL.n_patches), ascale);
+    WCTB_CHECK_LAUNCH("k_softmax_swap_anchor_scale");
+    k_softmax_swap_set<<<1, 1, 0, st>>>(wscale, 1.f / SOFTMAX_SWAP_WSCALE);
+    WCTB_CHECK_LAUNCH("k_softmax_swap_set");
+    // pass 1: the correlation (the hard swap's launches and bits) and the statistics of every block
+    for (int n0 = 0; n0 < cp; n0 += cols) {
+        const int m = cp - n0 < cols ? cp - n0 : cols;
+        rc = launch_conv_taps_rows(wc_feat, Nc, Hc, Wc, C, wsplit + (long long)n0 * K, (long long)cp * K, m, BN, scores, st, patch);
+        if (rc) return rc;
+        if (maps)
+            k_softmax_swap_stats<true><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, cdiv(m, B), B, SL.n_patches,
+                                                              ascale, inv_t, L.nblk, bstat, lab);
+        else
+            k_softmax_swap_stats<false><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, cdiv(m, B), B, SL.n_patches,
+                                                               ascale, inv_t, L.nblk, bstat, lab);
+        WCTB_CHECK_LAUNCH("k_softmax_swap_stats");
+    }
+    const long long na = (long long)Nc * npos;
+    k_softmax_swap_combine<<<swap_grid(na, 256), 256, 0, st>>>(bstat, na, L.nblk, inv_t, mz);
+    WCTB_CHECK_LAUNCH("k_softmax_swap_combine");
+    // pass 2: the correlation again when it ran in more than one chunk (the scores are the same bits), then per block the
+    // weight map, the block's filters, the fold on the tensor cores and its sum in block order
+    WCTB_CUDA(cudaMemsetAsync(wmap, 0, (size_t)gm.plane * 2 * sizeof(__half), st));
+    const long long PPCB = (long long)patch * patch * C * B;
+    for (int n0 = 0; n0 < cp; n0 += cols) {
+        const int m = cp - n0 < cols ? cp - n0 : cols;
+        if (cols < cp) {
+            rc = launch_conv_taps_rows(wc_feat, Nc, Hc, Wc, C, wsplit + (long long)n0 * K, (long long)cp * K, m, BN, scores, st, patch);
+            if (rc) return rc;
+        }
+        for (int c0 = 0; c0 < m; c0 += B) {
+            const int b = (n0 + c0) / B;
+            if (maps)
+                k_softmax_swap_weights<true><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, c0, SL.n_patches, ascale,
+                                                                    mz, inv_t, gm, wmap, lab);
+            else
+                k_softmax_swap_weights<false><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, c0, SL.n_patches, ascale,
+                                                                     mz, inv_t, gm, wmap, lab);
+            WCTB_CHECK_LAUNCH("k_softmax_swap_weights");
+            k_softmax_swap_fold_filters<<<swap_grid(PPCB, 256), 256, 0, st>>>(reinterpret_cast<const __half*>(sp + SL.feat), gs, q,
+                                                                              n0 + c0, B, SL.n_patches, filt);
+            WCTB_CHECK_LAUNCH("k_softmax_swap_fold_filters");
+            rc = launch_conv_tc(CONV_TAPS, wmap, Nc, gm.H, gm.W, B, filt, 1, wscale, nullptr, C, 0, fold, st, patch);
+            if (rc) return rc;
+            k_softmax_swap_accum<<<swap_grid((long long)Nc * Hc * Wc * (C / 8), 256), 256, 0, st>>>(
+                fold, gf, q, gc, b == 0, b == L.nblk - 1, reinterpret_cast<float*>(tmp), ss_feat);
+            WCTB_CHECK_LAUNCH("k_softmax_swap_accum");
+        }
+    }
+    return swap_apply_finish(ss_feat, content, Nc, Hc, Wc, C, sp, SL, kc, alpha, tmp, out, k_out, st);
+}
+int launch_style_swap_apply_softmax(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws,
+                                    int patch, int stride, float alpha, float eps_cov, float thresh, float temperature,
+                                    const uint8_t* content_labels, int Ncl, int Hm, int Wm, const uint8_t* style_labels, int Hms,
+                                    int Wms, __half* out, int32_t* k_out, void* ws, size_t ws_bytes, void* label_buf,
+                                    size_t label_bytes, cudaStream_t st) {
+    WCTB_REQUIRE((content_labels == nullptr) == (style_labels == nullptr),
+                 "style_swap_apply_softmax: give both label maps or neither");
+    const SwapLabelMaps maps = {content_labels, Ncl, Hm, Wm, style_labels, Hms, Wms, label_buf, label_bytes};
+    return style_swap_apply_softmax_impl(content, Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, temperature,
+                                         out, k_out, ws, ws_bytes, content_labels ? &maps : nullptr, st);
 }
 
 int launch_style_swap_level(const __half* content, int Hc, int Wc, const __half* style, int Hs, int Ws, int C, int patch, int stride,

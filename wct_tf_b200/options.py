@@ -6,7 +6,8 @@ This is the one statement of that policy.  ``WCT.predict_batch``, ``Engine.styli
 
 ``swap_labels`` (the labelled style swap, ``check_swap_labels``) has no entry in ``SPELLINGS``: it is a parameter of
 ``swap``, as ``mst_smooth`` is of ``mst``.  It needs the swap, and through it takes the swap's exclusions; it adds none of
-its own.  ``efdm_slices`` (sliced distribution matching, ``check_efdm_slices``) is in the same way a parameter of ``efdm``.
+its own.  ``ss_temperature`` (the softmax swap, ``check_ss_temperature``) is a parameter of ``swap`` in the same way.
+``efdm_slices`` (sliced distribution matching, ``check_efdm_slices``) is in the same way a parameter of ``efdm``.
 
 ``coarse_to_fine`` (scale control, ``check_coarse_to_fine``) is in ``AROUND`` too: it runs the call on a downscaled
 content at every level, joins the result into the content's low band and runs the fine levels on that at full size.
@@ -145,6 +146,24 @@ def check_swap_labels(swap_labels, swap, n_frames, n_styles=1, names=("swap_labe
     content = _label_map(swap_labels[0], names[0] + " content labels", (1, n_frames))
     style = _label_map(swap_labels[1], names[0] + " style labels", (1, n_styles))
     return content, style
+
+
+def check_ss_temperature(t, swap, vocab=API):
+    """The temperature of the softmax swap (DESIGN.md §3.3.17): None (the hard swap), or a finite number > 0 that is a
+    normal float32, and only with the style swap (``swap``: whether the call swaps at any level).  Returns it as a float
+    or None; ValueError otherwise, naming the options as ``vocab`` spells them."""
+    name = "--ss-temperature" if vocab is CLI else "ss_temperature"
+    if t is None:
+        return None
+    if isinstance(t, bool) or not isinstance(t, (int, float, np.integer, np.floating)) or not np.isfinite(t) or not t > 0:
+        raise ValueError("%s must be a finite number > 0, got %r" % (name, t))
+    # the device takes tau as a float32 and divides by it: a value that rounds to 0, a subnormal or inf has no finite 1/tau
+    f32 = np.finfo(np.float32)
+    if not float(f32.tiny) <= float(t) <= float(f32.max):
+        raise ValueError("%s must lie in float32's normal range [%g, %g], got %r" % (name, f32.tiny, f32.max, t))
+    if not swap:
+        raise ValueError("%s needs %s: the temperature is the style swap's" % (name, vocab["swap"]))
+    return float(t)
 
 
 def check_efdm_slices(K, efdm, vocab=API):

@@ -31,6 +31,8 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
     style patches of its own label;
   * ``luminance_only`` is new: colour preservation (Gatys et al., CVPR 2017, §5), the luminance stylised and the content's
     colours kept;
+  * ``ss_temperature`` is new: the softmax swap, each content patch rebuilt from a softmax-weighted blend of style
+    patches instead of its single best one;
   * ``coarse_to_fine`` is new: scale control (Gatys et al., CVPR 2017, §6), the call run on a downscaled content and its
     result joined into the content's low band before the fine levels run at full size.
 """
@@ -275,7 +277,7 @@ class WCT(object):
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
                       swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
                       strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None,
-                      efdm_slices=0, luminance_only=False, coarse_to_fine=None, fine_targets=None):
+                      efdm_slices=0, luminance_only=False, coarse_to_fine=None, fine_targets=None, ss_temperature=None):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -367,6 +369,15 @@ class WCT(object):
         stride the content is cropped as for the swap, and a content map of exactly the content's size is cropped with it
         (any other size is stretched over the image as stylised).  Labels act in the first pass only, like the swap.
 
+        ``ss_temperature`` = tau > 0 (softmax swap, DESIGN.md §3.3.17; with ``swap5`` / ``swap_targets``): each content
+        patch is rebuilt from a blend of style patches, weighted by a softmax of their scores at temperature tau, instead of
+        its single best patch.  Small tau approaches the hard swap, large tau the mean of the allowed patches; the useful
+        range is small (with synthetic weights at relu3_1 of a 512^2 style, about 2 to 3 patches per anchor at tau = 0.003
+        and hundreds at 0.01, tools/softmax_swap_bench.py; trained weights may differ), and blending a few close matches softens the seams between neighbouring patches.
+        With ``swap_labels``
+        the blend is over the patches of the anchor's label.  It acts in the first pass only, like the swap.  None is the
+        hard swap.
+
         ``luminance_only`` (colour preservation, DESIGN.md §3.3.15): stylise the luminance only and keep the content's
         colours.  The content frames (after a stride swap's crop) are made grey with the style's luminance mean and spread
         (``device_image.luminance_match``), the call runs with every other option on them against the grey of each style
@@ -401,6 +412,7 @@ class WCT(object):
         if coarse_to_fine is not None or fine_targets is not None:
             ctf = options.check_coarse_to_fine(coarse_to_fine, fine_targets, self.model.relu_targets)
         efdm_slices = options.check_efdm_slices(efdm_slices, efdm)
+        ss_temperature = options.check_ss_temperature(ss_temperature, swap5 or swap_targets is not None)
         if mask_feather is not None:
             options.check_mask_feather(mask_feather)
         if mst is not None:
@@ -524,7 +536,7 @@ class WCT(object):
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
                                        swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, efdm=efdm,
                                        efdm_slices=efdm_slices, swap_labels=lab_dev if first else None, levels=levels,
-                                       **soft_kw)
+                                       ss_temperature=ss_temperature if first else None, **soft_kw)
             if ctf is not None:
                 whole = one_pass
 
@@ -740,7 +752,7 @@ class WCT(object):
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
                 style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
                 strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0,
-                luminance_only=False, coarse_to_fine=None, fine_targets=None):
+                luminance_only=False, coarse_to_fine=None, fine_targets=None, ss_temperature=None):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
@@ -748,8 +760,8 @@ class WCT(object):
         path circularly, ``mst`` = K matches the content to K modes of the style and ``efdm`` matches every channel's whole
         value distribution to the style's (first in ``efdm_slices`` rotated bases); ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
-        (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap;
-        ``luminance_only`` stylises the luminance and keeps the content's colours; ``coarse_to_fine`` = f stylises a 1/f
+        (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap and
+        ``ss_temperature`` makes it the softmax swap; ``luminance_only`` stylises the luminance and keeps the content's colours; ``coarse_to_fine`` = f stylises a 1/f
         copy at every level first and ``fine_targets`` at full size (scale control).'''
         s = time.time()
         seen = {}
@@ -768,7 +780,8 @@ class WCT(object):
                                  swap_targets=swap_targets, tile_size=tile_size, ost=ost, seamless=seamless, mst=mst,
                                  mst_smooth=mst_smooth, strength_map=strength_map, content_weights=content_weights,
                                  mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels, efdm_slices=efdm_slices,
-                                 luminance_only=luminance_only, coarse_to_fine=coarse_to_fine, fine_targets=fine_targets)
+                                 luminance_only=luminance_only, coarse_to_fine=coarse_to_fine, fine_targets=fine_targets,
+                                 ss_temperature=ss_temperature)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
