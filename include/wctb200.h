@@ -513,6 +513,40 @@ WCTB200_API int wctb200_style_swap_apply_softmax(const void* content, int Nc, in
                                      void* out, int32_t* k_out, void* ws, size_t ws_bytes, void* label_buf, size_t label_bytes,
                                      void* stream);
 
+/*
+ * Balanced style swap (DESIGN.md §3.3.18): wctb200_style_swap_apply_softmax with `iters` Sinkhorn iterations that balance
+ * how much each style patch is used.  With z(a,n), tau and the allowed sets A(a) of the softmax swap, the column targets are
+ * c_n = sum_{a : n in A(a)} 1 / |A(a)| (Na / n_p without labels; with labels cnt(l(n)) / np(l(n)) + F / n_p, from exact
+ * counts: cnt the anchors of a label the style carries, np the patches of that label, F the anchors of absent labels).
+ * Potentials h_n (fp32, one per frame and patch, in units of z) start at 0; x(a,n) = z(a,n) + h_n, rounded once.
+ *   row step:    M_a = max_{n in A(a)} x(a,n),  Z_a = sum_{n in A(a)} exp((x(a,n) - M_a) / tau);
+ *   column step: S_n = sum_{a : n in A(a)} exp((x(a,n) - M_a) / tau) / Z_a (a log-sum-exp over anchor blocks of 256 per
+ *                frame, combined in block order),  h_n += tau (log c_n - log S_n) for every n with c_n > 0.
+ * The apply runs the row step of h = 0, `iters` times a column step then a row step, and folds
+ * w(a,n) = exp((x(a,n) - M_a) / tau) / Z_a as the softmax swap folds its weights: rows sum to 1, columns tend to c_n.
+ * iters = 0 is the softmax swap, launch for launch and byte for byte.  Each iteration costs one pass over the scores: the
+ * correlation again when the apply runs in chunks.
+ *   col_sums: NULL, or float [Nc][n_p] that receives S_n of the final plan (one more column pass, no extra correlation).
+ *   ws: wctb200_style_swap_balanced_workspace_bytes run in one chunk, down to _balanced_min_workspace_bytes (one block of
+ *   patches) in chunks of whole blocks, and every size gives the same bytes.  The workspace begins with
+ *   wctb200_style_swap_apply's layout.
+ * iters < 0 or > 256 is WCTB200_EINVAL; the other errors are wctb200_style_swap_apply_softmax's.  Frame i of an apply is
+ * bit-identical to the apply of that frame alone.
+ * wctb200_style_swap_balanced_launches: the kernels an apply with ws_bytes of workspace launches (labelled: label maps
+ * given; want_cols: col_sums given); 0 for a bad geometry, a bad iters or too small a workspace.
+ */
+WCTB200_API size_t wctb200_style_swap_balanced_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride);
+WCTB200_API size_t wctb200_style_swap_balanced_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch,
+                                                                   int stride);
+WCTB200_API int wctb200_style_swap_balanced_launches(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride,
+                                                     size_t ws_bytes, int labelled, int iters, int want_cols);
+WCTB200_API int wctb200_style_swap_apply_balanced(const void* content, int Nc, int Hc, int Wc, int C, const void* state,
+                                      int Hs, int Ws, int patch, int stride, float alpha, float eps_cov, float thresh,
+                                      float temperature, int iters, const uint8_t* content_labels, int Ncl, int Hm, int Wm,
+                                      const uint8_t* style_labels, int Hms, int Wms,
+                                      void* out, int32_t* k_out, float* col_sums, void* ws, size_t ws_bytes, void* label_buf,
+                                      size_t label_bytes, void* stream);
+
 /* ---- multimodal style transfer (DESIGN.md §3.3.10; mst.cu) ----------------
  * Spherical k-means of one style feature (SPF16 [1,Hs,Ws,C], C in {64,128,256,512}) into K in 1..8 clusters of the unit
  * directions u_p = f_p / max(|f_p|, 1e-12): k-means++ seeding with Philox4x32-10 draws (counter (j, level, 0, 0)), then at

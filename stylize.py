@@ -57,6 +57,11 @@ blend of style patches weighted by a softmax of their scores at temperature T, i
 §3.3.17).  Small T approaches the hard swap; larger T blends more patches, which softens the seams between neighbouring
 patches (about 0.003 blends a few patches per anchor at relu3_1).  Output names are unchanged.
 
+Balanced swap: ``--ss-balance T`` (1..256, with ``--ss-temperature``) runs T Sinkhorn iterations on the softmax swap's
+weights, so that the style patches are used about evenly instead of a few of them covering large regions (DESIGN.md
+§3.3.18).  Each iteration costs about one more pass over the patch scores.  0 is the softmax swap.  Output names are
+unchanged.
+
 Labelled style swap (neural doodle): ``--swap-labels CONTENT_MAP STYLE_MAP`` with ``--swap5`` / ``--swap-targets`` gives
 the content and the style each a flat-colour label map (RGB or grey PNG, any resolution); every content patch is then
 rebuilt only from style patches of the same colour, or from all of them where the style has none (DESIGN.md §3.3.13).  The
@@ -115,6 +120,9 @@ _FLAGS = [
     (("--ss-temperature",), dict(type=float, default=None, metavar="T",
                                  help="with --swap5 / --swap-targets: softmax swap, each content patch a blend of style patches "
                                       "weighted by a softmax of their scores at temperature T > 0 (not in the reference)")),
+    (("--ss-balance",), dict(type=int, default=None, metavar="T",
+                             help="with --ss-temperature: balanced swap, T in 1..256 Sinkhorn iterations that spread the "
+                                  "softmax swap's use of the style patches evenly; 0 is the softmax swap (not in the reference)")),
     (("--ss-patch-size",), dict(type=int, default=3)),
     (("--ss-stride",), dict(type=int, default=1)),
     # not in the reference
@@ -277,6 +285,8 @@ def check_values(parser, args):
             options.check_mask_feather(args.mask_feather, "--mask-feather")
         options.check_efdm_slices(args.efdm_slices, args.efdm, options.CLI)
         options.check_ss_temperature(args.ss_temperature, args.swap5 or args.swap_targets is not None, options.CLI)
+        if args.ss_balance is not None:
+            options.check_ss_balance(args.ss_balance, args.ss_temperature, options.CLI)
         if getattr(args, "coarse_to_fine", 0) or getattr(args, "fine_targets", None) is not None:
             options.check_coarse_to_fine(args.coarse_to_fine or None, args.fine_targets, args.relu_targets or [], options.CLI)
         if hasattr(args, "temporal"):
@@ -530,6 +540,8 @@ def _stylize_pair(model, content_dev, style_dev, args):
         kw["swap_targets"] = list(args.swap_targets)
     if args.ss_temperature is not None:
         kw["ss_temperature"] = args.ss_temperature
+    if args.ss_balance is not None:
+        kw["ss_balance"] = args.ss_balance
     if args.tile_size:
         kw["tile_size"] = args.tile_size
     if args.ost:

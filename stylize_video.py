@@ -69,8 +69,9 @@ _VIDEO_FLAGS = [
                                 "predecessor (default 0: off)")),
 ]
 _SHARED = ("--checkpoints", "--relu-targets", "--vgg-path", "--keep-colors", "--style-size", "--crop-size", "--content-size",
-           "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-temperature", "--ss-patch-size",
-           "--ss-stride", "--adain", "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets", "--ost", "--seamless",
+           "--passes", "--device", "--alpha", "--concat", "--swap5", "--ss-alpha", "--ss-temperature", "--ss-balance",
+           "--ss-patch-size", "--ss-stride", "--adain", "--synthetic-weights", "--interp-styles", "--interp-weights", "--swap-targets",
+           "--ost", "--seamless",
            "--mst", "--mst-smooth", "--strength-map", "--efdm", "--efdm-slices", "--luminance-only", "--coarse-to-fine",
            "--fine-targets")
 # flags of the one-style mode that --interp-styles takes no part of
@@ -205,6 +206,8 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 swap_kw = dict(swap_targets=list(args.swap_targets), ss_alpha=args.ss_alpha)
             if args.ss_temperature is not None:
                 swap_kw["ss_temperature"] = args.ss_temperature
+            if args.ss_balance is not None:
+                swap_kw["ss_balance"] = args.ss_balance
             one = weights is not None or not hasattr(style_img, "shape")   # a list of styles, or a prepared style
             out = wct_model.predict_batch(x, style_img if one else style_img[None], alpha=args.alpha,
                                           adain=args.adain, passes=args.passes, return_device=True,
@@ -220,6 +223,8 @@ def stylize_frames(wct_model, in_files, out_files, style_img, args, io, pool, di
                 swap_kw = dict(swap_targets=list(args.swap_targets)) if args.swap_targets else {}
                 if args.ss_temperature is not None:
                     swap_kw["ss_temperature"] = args.ss_temperature
+                if args.ss_balance is not None:
+                    swap_kw["ss_balance"] = args.ss_balance
                 if temporal is not None or "luminance_only" in opt_kw:   # stabilised / merged after the last pass
                     o = wct_model.predict_batch(fr, style_rgb, swap5=args.swap5, passes=args.passes,
                                                 **dict(kw, **swap_kw, **temporal_kw))

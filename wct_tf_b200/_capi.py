@@ -94,6 +94,11 @@ SIGNATURES = {
     "wctb200_style_swap_softmax_launches": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _sz, _i]),
     "wctb200_style_swap_apply_softmax": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _f, _vp, _i, _i, _i, _vp, _i,
                                               _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "wctb200_style_swap_balanced_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i, _i]),
+    "wctb200_style_swap_balanced_min_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i, _i, _i]),
+    "wctb200_style_swap_balanced_launches": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _sz, _i, _i, _i]),
+    "wctb200_style_swap_apply_balanced": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _f, _i, _vp, _i, _i, _i, _vp,
+                                               _i, _i, _vp, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "wctb200_style_swap_apply_labels": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _i, _i, _i, _vp, _i, _i,
                                              _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "wctb200_stats_record_layout": (_sz, [_i, _i, _i, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),

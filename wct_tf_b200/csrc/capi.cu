@@ -134,6 +134,15 @@ int launch_style_swap_apply_softmax(const __half* content, int Nc, int Hc, int W
                                     const uint8_t* content_labels, int Ncl, int Hm, int Wm, const uint8_t* style_labels, int Hms,
                                     int Wms, __half* out, int32_t* k_out, void* ws, size_t ws_bytes, void* label_buf,
                                     size_t label_bytes, cudaStream_t st);
+size_t style_swap_balanced_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S);
+size_t style_swap_balanced_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S);
+int style_swap_balanced_launches(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, size_t ws_bytes, int labelled,
+                                 int iters, int want_cols);
+int launch_style_swap_apply_balanced(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws,
+                                     int patch, int stride, float alpha, float eps_cov, float thresh, float temperature, int iters,
+                                     const uint8_t* content_labels, int Ncl, int Hm, int Wm, const uint8_t* style_labels, int Hms,
+                                     int Wms, __half* out, int32_t* k_out, float* col_sums, void* ws, size_t ws_bytes,
+                                     void* label_buf, size_t label_bytes, cudaStream_t st);
 size_t wct_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_cs, size_t* off_k);
 size_t adain_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_var);
 int launch_adain_style_prepare(const __half* style, int Ns, int Hs, int Ws, int C, void* state, cudaStream_t st);
@@ -768,6 +777,37 @@ int wctb200_style_swap_apply_softmax(const void* content, int Nc, int Hc, int Wc
     return launch_style_swap_apply_softmax(HCP(content), Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh,
                                            temperature, content_labels, Ncl, Hm, Wm, style_labels, Hms, Wms, HP(out), k_out, ws,
                                            ws_bytes, label_buf, label_bytes, ST(stream));
+}
+size_t wctb200_style_swap_balanced_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride) {
+    if (!swap_style_ok(C, Hs, Ws, patch, stride) || !geom_ok(Nc, Hc, Wc, C) || Hc < patch || Wc < patch) return 0;
+    return style_swap_balanced_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride);
+}
+size_t wctb200_style_swap_balanced_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride) {
+    if (!swap_style_ok(C, Hs, Ws, patch, stride) || !geom_ok(Nc, Hc, Wc, C) || Hc < patch || Wc < patch) return 0;
+    return style_swap_balanced_min_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride);
+}
+int wctb200_style_swap_balanced_launches(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int patch, int stride, size_t ws_bytes,
+                                         int labelled, int iters, int want_cols) {
+    if (!swap_style_ok(C, Hs, Ws, patch, stride) || !geom_ok(Nc, Hc, Wc, C) || Hc < patch || Wc < patch) return 0;
+    return style_swap_balanced_launches(C, Nc, Hc, Wc, Hs, Ws, patch, stride, ws_bytes, labelled, iters, want_cols);
+}
+int wctb200_style_swap_apply_balanced(const void* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws,
+                                      int patch, int stride, float alpha, float eps_cov, float thresh, float temperature, int iters,
+                                      const uint8_t* content_labels, int Ncl, int Hm, int Wm, const uint8_t* style_labels, int Hms,
+                                      int Wms, void* out, int32_t* k_out, float* col_sums, void* ws, size_t ws_bytes,
+                                      void* label_buf, size_t label_bytes, void* stream) {
+    WCTB_REQUIRE(content && state && out && ws, "style_swap_apply_balanced: null pointer");
+    WCTB_REQUIRE(Nc >= 1, "style_swap_apply_balanced: Nc=%d < 1", Nc);
+    WCTB_REQUIRE(geom_ok(Nc, Hc, Wc, C) && geom_ok(1, Hs, Ws, C), "style_swap_apply_balanced: bad geometry");
+    if (content_labels || style_labels) {
+        WCTB_REQUIRE(content_labels && style_labels && label_buf, "style_swap_apply_balanced: null label pointer");
+        WCTB_REQUIRE(swap_label_map_ok(Ncl, Hm, Wm) && (Ncl == 1 || Ncl == Nc) && swap_label_map_ok(1, Hms, Wms),
+                     "style_swap_apply_balanced: %d content label maps of %dx%d for %d frames, style labels %dx%d", Ncl, Hm, Wm,
+                     Nc, Hms, Wms);
+    }
+    return launch_style_swap_apply_balanced(HCP(content), Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh,
+                                            temperature, iters, content_labels, Ncl, Hm, Wm, style_labels, Hms, Wms, HP(out), k_out,
+                                            col_sums, ws, ws_bytes, label_buf, label_bytes, ST(stream));
 }
 size_t wctb200_wct_style_state_layout(int C, int Ns, size_t* off_mean, size_t* off_cs, size_t* off_k) {
     if (C < 8 || Ns < 1) return 0;

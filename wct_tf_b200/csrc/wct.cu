@@ -2887,17 +2887,23 @@ constexpr int SOFTMAX_SWAP_BLOCK = 256;
 // the weights are split to fp16 times 2^15: unscaled, weights below 6e-8 would flush to zero (there are 64 516 patches at
 // relu2_1); the fold's epilogue multiplies by 2^-15, exactly
 constexpr float SOFTMAX_SWAP_WSCALE = 32768.f;
+// the most Sinkhorn iterations of a balanced apply (DESIGN.md §3.3.18)
+constexpr int BALANCED_SWAP_MAX_ITERS = 256;
 
 // workspace of a softmax apply: the hard apply's layout with `cols` score columns (wc_feat, ss_feat, tmp -- tmp holds the
 // fold's fp32 sum -- and the scores), then r_a [Nc*ho*wo] | (max, sum) per (anchor, block) | (M_a, 1/Z_a) per anchor | the
 // fold's unscale factor | one block's fold filters [2][C][P*P][B] | the weight map SPF16 [Nc, Hc+P-1, Wc+P-1, B] | the fold
-// of one block SPF16 [Nc, Hc+P-1, Wc+P-1, C]
+// of one block SPF16 [Nc, Hc+P-1, Wc+P-1, C].  A balanced apply (DESIGN.md §3.3.18) adds the potentials h [Nc][cout_pad] |
+// the log column targets [Nc][cout_pad] | (max, sum) per (frame, anchor block, chunk column) [Nc][nablk_a][cols].
 struct SwapSoftmaxWs {
     SwapApplyWs A;
-    size_t ascale, bstat, mz, wscale, filt, wmap, fold, total;
-    int B, nblk;
+    size_t ascale, bstat, mz, wscale, filt, wmap, fold, hpot, logc, cstat, total;
+    int B, nblk, nablk_a;
 };
-static SwapSoftmaxWs swap_softmax_layout(int C, int Nc, int Hc, int Wc, int P, int S, int cout_pad, int cols) {
+// anchors per block of the balanced swap's column statistics (per frame; the last block of a frame may be short)
+constexpr int BALANCED_SWAP_ABLK = 256;
+static SwapSoftmaxWs swap_softmax_layout(int C, int Nc, int Hc, int Wc, int P, int S, int cout_pad, int cols,
+                                         bool balanced = false) {
     SwapSoftmaxWs L;
     L.A = swap_apply_layout(C, Nc, Hc, Wc, P, S, cols);
     L.B = cout_pad < SOFTMAX_SWAP_BLOCK ? cout_pad : SOFTMAX_SWAP_BLOCK;
@@ -2912,6 +2918,13 @@ static SwapSoftmaxWs swap_softmax_layout(int C, int Nc, int Hc, int Wc, int P, i
     L.filt = take((size_t)2 * C * P * P * L.B * sizeof(__half));
     L.wmap = take((size_t)ActGeom(Nc, Hc + P - 1, Wc + P - 1, L.B).plane * 2 * sizeof(__half));
     L.fold = take((size_t)ActGeom(Nc, Hc + P - 1, Wc + P - 1, C).plane * 2 * sizeof(__half));
+    L.nablk_a = cdiv(L.A.ho * L.A.wo, BALANCED_SWAP_ABLK);
+    L.hpot = L.logc = L.cstat = 0;
+    if (balanced) {
+        L.hpot = take((size_t)Nc * cout_pad * 4);
+        L.logc = take((size_t)Nc * cout_pad * 4);
+        L.cstat = take((size_t)Nc * L.nablk_a * cols * sizeof(float2));
+    }
     L.total = o;
     return L;
 }
@@ -2927,12 +2940,12 @@ size_t style_swap_softmax_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int
 
 // chunk width of a softmax apply in ws_bytes: all cout_pad patches when the workspace holds their scores, else the largest
 // whole number of blocks that fits; 0 when not even one block does
-static int softmax_swap_cols(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, size_t ws_bytes) {
+static int softmax_swap_cols(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, size_t ws_bytes, bool balanced = false) {
     const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
-    const SwapSoftmaxWs full = swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cp);
+    const SwapSoftmaxWs full = swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cp, balanced);
     if (ws_bytes >= full.total) return cp;
     int cols = (cp - 1) / full.B * full.B;
-    while (cols >= full.B && swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cols).total > ws_bytes) cols -= full.B;
+    while (cols >= full.B && swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cols, balanced).total > ws_bytes) cols -= full.B;
     return cols >= full.B ? cols : 0;
 }
 // kernels one softmax apply in ws_bytes launches, counted as the hard apply's 11 are (memsets and copies not counted): the
@@ -2946,6 +2959,30 @@ int style_swap_softmax_launches(int C, int Nc, int Hc, int Wc, int Hs, int Ws, i
     const SwapSoftmaxWs L = swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cols);
     const int chunks = cdiv(cp, cols);
     return 8 + 2 + 2 * chunks + 1 + (chunks > 1 ? chunks : 0) + 4 * L.nblk + (labelled ? 3 : 0);
+}
+
+// the balanced swap's workspaces (the softmax layout plus its buffers; one chunk, and one block of scores) and launches:
+// the softmax apply's, plus the targets when iters > 0, per iteration and chunk the column statistics, the column update,
+// the row statistics and -- with several chunks -- the correlation, one combine per iteration, and per chunk the column
+// statistics and their output when `want_cols`.  0 when ws_bytes is too small.
+size_t style_swap_balanced_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
+    return swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cp, true).total;
+}
+size_t style_swap_balanced_min_workspace_bytes(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S) {
+    const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
+    return swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cp < SOFTMAX_SWAP_BLOCK ? cp : SOFTMAX_SWAP_BLOCK, true).total;
+}
+int style_swap_balanced_launches(int C, int Nc, int Hc, int Wc, int Hs, int Ws, int P, int S, size_t ws_bytes, int labelled,
+                                 int iters, int want_cols) {
+    if (iters < 0 || iters > BALANCED_SWAP_MAX_ITERS) return 0;
+    const int cols = softmax_swap_cols(C, Nc, Hc, Wc, Hs, Ws, P, S, ws_bytes, true);
+    if (cols == 0) return 0;
+    const int cp = swap_state_layout(C, Hs, Ws, P, S).cout_pad;
+    const SwapSoftmaxWs L = swap_softmax_layout(C, Nc, Hc, Wc, P, S, cp, cols, true);
+    const int chunks = cdiv(cp, cols);
+    const int base = 8 + 2 + 2 * chunks + 1 + (chunks > 1 ? chunks : 0) + 4 * L.nblk + (labelled ? 3 : 0);
+    return base + (iters > 0 ? 1 : 0) + iters * (chunks * (chunks > 1 ? 4 : 3) + 1) + (want_cols ? 2 * chunks : 0);
 }
 
 // r_a of every anchor of frame blockIdx.y, one warp each: lane l sums wc^2 over the channels l, l+32, .. of every tap in
@@ -3003,11 +3040,12 @@ __device__ __forceinline__ float softmax_swap_exp(float x, float m, float inv_t)
 constexpr int SOFTMAX_SWAP_PER_LANE = SOFTMAX_SWAP_BLOCK / 32;
 // pass 1: (max_b, sum_b exp((z - max_b) / tau)) over the allowed real patches of each of the `nb` blocks of this chunk
 // (scores of patches [n0, n0 + g.C)), one warp per anchor; lane l takes the block's patches l, l+32, .., then fixed
-// butterflies.  A block without an allowed patch gives (-inf, 0).
-template <bool LABELS>
+// butterflies.  A block without an allowed patch gives (-inf, 0).  POT (the balanced swap's row step, DESIGN.md §3.3.18)
+// takes x = z + h_n, rounded once, in place of z; hpot points at h of patch n0 of frame 0, frames `hstride` apart.
+template <bool LABELS, bool POT = false>
 __global__ void k_softmax_swap_stats(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n0, int nb, int B, int n_patches,
                                      const float* __restrict__ ascale, float inv_t, int nblk, float2* __restrict__ bstat,
-                                     SwapLabels lab) {
+                                     SwapLabels lab, const float* __restrict__ hpot = nullptr, int hstride = 0) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= q.ho * q.wo) return;
     const int n = blockIdx.y;
@@ -3026,6 +3064,7 @@ __global__ void k_softmax_swap_stats(const __half* __restrict__ scores, ActGeom 
             z[i] = -INFINITY;
             if (jj < B && n0 + j < n_patches && softmax_swap_allowed<LABELS>(lab, any, l, n0 + j)) {
                 z[i] = softmax_swap_z(scores, g, pos, j, r);
+                if constexpr (POT) z[i] = __fadd_rn(z[i], hpot[(long long)n * hstride + j]);
                 mx = fmaxf(mx, z[i]);
             }
         }
@@ -3055,11 +3094,12 @@ __global__ void k_softmax_swap_combine(const float2* __restrict__ bstat, long lo
     }
 }
 // pass 2: the weights of block [n0 + c0, n0 + c0 + gm.C) times 2^15, split, at map pixel (y*S + P-1, x*S + P-1) of every
-// anchor; padding, foreign-label and non-patch channels get 0.  One warp per anchor.
-template <bool LABELS>
+// anchor; padding, foreign-label and non-patch channels get 0.  One warp per anchor.  POT: x = z + h_n as in the statistics.
+template <bool LABELS, bool POT = false>
 __global__ void k_softmax_swap_weights(const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n0, int c0, int n_patches,
                                        const float* __restrict__ ascale, const float2* __restrict__ mz, float inv_t, ActGeom gm,
-                                       __half* __restrict__ wmap, SwapLabels lab) {
+                                       __half* __restrict__ wmap, SwapLabels lab, const float* __restrict__ hpot = nullptr,
+                                       int hstride = 0) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= q.ho * q.wo) return;
     const int n = blockIdx.y;
@@ -3075,7 +3115,9 @@ __global__ void k_softmax_swap_weights(const __half* __restrict__ scores, ActGeo
         const int j = c0 + jj;
         float w = 0.f;
         if (n0 + j < n_patches && softmax_swap_allowed<LABELS>(lab, any, l, n0 + j)) {
-            w = softmax_swap_exp(softmax_swap_z(scores, g, pos, j, r), t.x, inv_t) * t.y * SOFTMAX_SWAP_WSCALE;
+            float x = softmax_swap_z(scores, g, pos, j, r);
+            if constexpr (POT) x = __fadd_rn(x, hpot[(long long)n * hstride + j]);
+            w = softmax_swap_exp(x, t.x, inv_t) * t.y * SOFTMAX_SWAP_WSCALE;
         }
         __half hi, lo;
         split_f32(w, hi, lo);
@@ -3149,26 +3191,145 @@ __global__ void k_softmax_swap_accum(const __half* __restrict__ fold, ActGeom gf
     }
 }
 
+// ---------------------------------------------------------------------------
+// Balanced style swap (DESIGN.md §3.3.18): Sinkhorn iterations on the softmax swap's plan.  Potentials h_n (units of z,
+// one per frame and patch) enter as x(a,n) = z(a,n) + h_n; the row step is the softmax swap's statistics of x, and the
+// column step moves h_n by tau (log c_n - log S_n), S_n = sum_a exp((x - M_a) / tau) / Z_a over the anchors that may take n.
+// ---------------------------------------------------------------------------
+// log c_n of every patch of frame blockIdx.x: c_n = cnt(l(n)) / np(l(n)) + F / n_p from exact integer histograms (anchors
+// per present label, patches per label, F the anchors whose label the style lacks); without labels cnt = 0, np = 1 and
+// F = Na, so c_n = Na / n_p.  Padding patches and c_n = 0 (no anchor may take n) get -inf.
+template <bool LABELS>
+__global__ void k_balanced_swap_targets(ActGeom g, SwapGeom q, int n_patches, int cp, SwapLabels lab, float* __restrict__ logc) {
+    __shared__ int ha[256], hp[256], fallback;
+    const int n = blockIdx.x, npos = q.ho * q.wo;
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) ha[i] = hp[i] = 0;
+    if (threadIdx.x == 0) fallback = LABELS ? 0 : npos;
+    __syncthreads();
+    if constexpr (LABELS) {
+        for (int a = threadIdx.x; a < npos; a += blockDim.x) {
+            const int y = a / q.wo, x = a - y * q.wo;
+            bool any;
+            const int l = softmax_swap_label<true>(lab, g, q, n, y, x, any);
+            atomicAdd(any ? &fallback : &ha[l], 1);
+        }
+        for (int p = threadIdx.x; p < n_patches; p += blockDim.x) atomicAdd(&hp[lab.plab[p]], 1);
+    }
+    __syncthreads();
+    const float f = __fdiv_rn((float)fallback, (float)n_patches);
+    for (int p = threadIdx.x; p < cp; p += blockDim.x) {
+        float c = 0.f;
+        if (p < n_patches) {
+            const int l = LABELS ? lab.plab[p] : 0;
+            c = __fadd_rn(__fdiv_rn((float)ha[l], (float)(LABELS ? hp[l] : 1)), f);
+        }
+        logc[(long long)n * cp + p] = c > 0.f ? logf(c) : -INFINITY;
+    }
+}
+
+// the column statistics of the chunk's patches [n0, n0 + g.C) over anchor block blockIdx.y of frame blockIdx.z: one thread
+// per patch (the contiguous axis of the scores), the block's anchors in order, an online (max, sum of exp) of
+// e(a,n) = (x(a,n) - M_a) / tau + log(1 / Z_a) over the anchors that may take n.  (-inf, 0) when none may.
+// cstat [Nc][nablk][g.C]; (M_a, 1/Z_a) and r_a of the block's anchors are staged in shared memory.
+template <bool LABELS>
+__global__ void __launch_bounds__(BALANCED_SWAP_ABLK) k_balanced_swap_col_stats(
+    const __half* __restrict__ scores, ActGeom g, SwapGeom q, int n0, int n_patches, const float* __restrict__ ascale,
+    const float2* __restrict__ mz, const float* __restrict__ hpot, int cp, float inv_t, int nablk, float2* __restrict__ cstat,
+    SwapLabels lab) {
+    __shared__ float s_r[BALANCED_SWAP_ABLK], s_m[BALANCED_SWAP_ABLK], s_lz[BALANCED_SWAP_ABLK];
+    __shared__ int s_l[BALANCED_SWAP_ABLK];
+    const int n = blockIdx.z, ab = blockIdx.y, npos = q.ho * q.wo;
+    const int a0 = ab * BALANCED_SWAP_ABLK;
+    const int na = npos - a0 < BALANCED_SWAP_ABLK ? npos - a0 : BALANCED_SWAP_ABLK;
+    for (int i = threadIdx.x; i < na; i += blockDim.x) {
+        const long long a = (long long)n * npos + a0 + i;
+        const float2 t = mz[a];
+        s_r[i] = ascale[a];
+        s_m[i] = t.x;
+        s_lz[i] = logf(t.y);
+        s_l[i] = -1;
+        if constexpr (LABELS) {
+            const int y = (a0 + i) / q.wo, x = (a0 + i) - y * q.wo;
+            bool any;
+            const int l = softmax_swap_label<true>(lab, g, q, n, y, x, any);
+            s_l[i] = any ? -1 : l;
+        }
+    }
+    __syncthreads();
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= g.C || n0 + j >= n_patches) return;
+    const float h = hpot[(long long)n * cp + n0 + j];
+    const int pl = LABELS ? (int)lab.plab[n0 + j] : 0;
+    float mx = -INFINITY, sum = 0.f;
+    for (int i = 0; i < na; ++i) {
+        if (LABELS && s_l[i] >= 0 && s_l[i] != pl) continue;
+        const int y = (a0 + i) / q.wo, x = (a0 + i) - y * q.wo;
+        const long long pos = ((long long)n * g.Hp + y * q.S + 1) * g.Wp + (x * q.S + 1);
+        const float xv = __fadd_rn(softmax_swap_z(scores, g, pos, j, s_r[i]), h);
+        const float e = __fadd_rn(__fmul_rn(__fsub_rn(xv, s_m[i]), inv_t), s_lz[i]);
+        if (e > mx) {
+            sum = sum * expf(mx - e) + 1.f;
+            mx = e;
+        } else {
+            sum += expf(e - mx);
+        }
+    }
+    cstat[((long long)n * nablk + ab) * g.C + j] = make_float2(mx, sum);
+}
+
+// log S_n of the chunk's patches from the anchor blocks' (max, sum), in block order; then either the column step
+// h_n += tau (log c_n - log S_n) (col_sums == nullptr; patches with c_n = 0 are left alone) or S_n into col_sums [Nc][n_p].
+// Grid (patches of the chunk, Nc).
+__global__ void k_balanced_swap_col_update(const float2* __restrict__ cstat, int m, int n0, int n_patches, int cp, int nablk,
+                                           const float* __restrict__ logc, float tau, float* __restrict__ hpot,
+                                           float* __restrict__ col_sums) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x, n = blockIdx.y;
+    if (j >= m || n0 + j >= n_patches) return;
+    const float2* t = cstat + (long long)n * nablk * m + j;
+    float M = -INFINITY;
+    for (int b = 0; b < nablk; ++b) M = fmaxf(M, t[(long long)b * m].x);
+    float S = 0.f;
+    for (int b = 0; b < nablk; ++b) {
+        const float2 v = t[(long long)b * m];
+        if (v.y > 0.f) S += v.y * expf(__fsub_rn(v.x, M));
+    }
+    const float log_s = S > 0.f ? __fadd_rn(M, logf(S)) : -INFINITY;
+    const long long k = (long long)n * cp + n0 + j;
+    if (col_sums) {
+        col_sums[(long long)n * n_patches + n0 + j] = expf(log_s);
+        return;
+    }
+    const float lc = logc[k];
+    if (lc == -INFINITY || log_s == -INFINITY) return;
+    hpot[k] = __fadd_rn(hpot[k], __fmul_rn(tau, __fsub_rn(lc, log_s)));
+}
+
+// The softmax apply and, with `balanced`, the balanced one (DESIGN.md §3.3.18): `iters` Sinkhorn iterations between pass 1
+// and pass 2, each a column step then a row step, and the final plan's column sums into `col_sums` when it is given.  A
+// balanced apply uses the balanced workspace layout; at iters = 0 it runs the softmax apply's launches, and its bytes.
 static int style_swap_apply_softmax_impl(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws,
                                          int patch, int stride, float alpha, float eps_cov, float thresh, float temperature,
                                          __half* out, int32_t* k_out, void* ws, size_t ws_bytes, const SwapLabelMaps* maps,
-                                         cudaStream_t st) {
+                                         cudaStream_t st, bool balanced = false, int iters = 0, float* col_sums = nullptr) {
+    const char* fn = balanced ? "style_swap_apply_balanced" : "style_swap_apply_softmax";
     // a normal float: a subnormal tau has no finite 1/tau, and (z - M) * inf would be NaN at every maximum
     WCTB_REQUIRE(std::isfinite(temperature) && temperature >= FLT_MIN && std::isfinite(1.f / temperature),
-                 "style_swap_apply_softmax: temperature %g must be a finite, normal float32 > 0", (double)temperature);
+                 "%s: temperature %g must be a finite, normal float32 > 0", fn, (double)temperature);
+    WCTB_REQUIRE(iters >= 0 && iters <= BALANCED_SWAP_MAX_ITERS, "%s: iters %d not in 0..%d", fn, iters, BALANCED_SWAP_MAX_ITERS);
     SwapLabels lab = {nullptr, 0, nullptr, nullptr};
     SwapLabelWs LL = {};
     int rc = swap_apply_check(Nc, Hc, Wc, C, Hs, Ws, patch, stride, maps, &LL);
     if (rc) return rc;
     const SwapState SL = swap_state_layout(C, Hs, Ws, patch, stride);
     const int cp = SL.cout_pad;
-    const int cols = softmax_swap_cols(C, Nc, Hc, Wc, Hs, Ws, patch, stride, ws_bytes);
+    const int cols = softmax_swap_cols(C, Nc, Hc, Wc, Hs, Ws, patch, stride, ws_bytes, balanced);
     if (cols == 0) {
-        set_error("style_swap_apply_softmax: workspace %zu < %zu bytes", ws_bytes,
-                  style_swap_softmax_min_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride));
+        set_error("%s: workspace %zu < %zu bytes", fn, ws_bytes,
+                  balanced ? style_swap_balanced_min_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride)
+                           : style_swap_softmax_min_workspace_bytes(C, Nc, Hc, Wc, Hs, Ws, patch, stride));
         return WCTB200_EWS;
     }
-    const SwapSoftmaxWs L = swap_softmax_layout(C, Nc, Hc, Wc, patch, stride, cp, cols);
+    const SwapSoftmaxWs L = swap_softmax_layout(C, Nc, Hc, Wc, patch, stride, cp, cols, balanced);
     const SwapApplyWs& AL = L.A;
     const int B = L.B;
     const SwapGeom q = {patch, stride, SL.prow, SL.pcol, AL.ho, AL.wo};
@@ -3221,6 +3382,53 @@ static int style_swap_apply_softmax_impl(const __half* content, int Nc, int Hc, 
     const long long na = (long long)Nc * npos;
     k_softmax_swap_combine<<<swap_grid(na, 256), 256, 0, st>>>(bstat, na, L.nblk, inv_t, mz);
     WCTB_CHECK_LAUNCH("k_softmax_swap_combine");
+    // the balanced swap's iterations: per chunk (the correlation again when there are several) the column step of its
+    // patches from the previous (M_a, Z_a), then its row statistics with the new h; the rows are combined after the last
+    // chunk.  h = 0 until the first column step, where z + 0 = z: pass 1 is the row step of h = 0.
+    float* hpot = reinterpret_cast<float*>(sw + L.hpot);
+    float* logc = reinterpret_cast<float*>(sw + L.logc);
+    float2* cstat = reinterpret_cast<float2*>(sw + L.cstat);
+    if (iters > 0 || col_sums) WCTB_CUDA(cudaMemsetAsync(hpot, 0, (size_t)Nc * cp * 4, st));
+    if (iters > 0) {
+        if (maps)
+            k_balanced_swap_targets<true><<<(unsigned)Nc, 1024, 0, st>>>(gc, q, SL.n_patches, cp, lab, logc);
+        else
+            k_balanced_swap_targets<false><<<(unsigned)Nc, 1024, 0, st>>>(gc, q, SL.n_patches, cp, lab, logc);
+        WCTB_CHECK_LAUNCH("k_balanced_swap_targets");
+    }
+    // the column statistics of one chunk's patches, then the column step (col_out == nullptr) or the column sums
+    auto column_pass = [&](int n0, int m, float* col_out) {
+        const dim3 cgrid((unsigned)cdiv(m, BALANCED_SWAP_ABLK), (unsigned)L.nablk_a, (unsigned)Nc);
+        if (maps)
+            k_balanced_swap_col_stats<true><<<cgrid, BALANCED_SWAP_ABLK, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, SL.n_patches,
+                                                                                 ascale, mz, hpot, cp, inv_t, L.nablk_a, cstat, lab);
+        else
+            k_balanced_swap_col_stats<false><<<cgrid, BALANCED_SWAP_ABLK, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, SL.n_patches,
+                                                                                  ascale, mz, hpot, cp, inv_t, L.nablk_a, cstat, lab);
+        WCTB_CHECK_LAUNCH("k_balanced_swap_col_stats");
+        k_balanced_swap_col_update<<<dim3((unsigned)cdiv(m, 256), (unsigned)Nc), 256, 0, st>>>(cstat, m, n0, SL.n_patches, cp, L.nablk_a,
+                                                                                             logc, temperature, hpot, col_out);
+        WCTB_CHECK_LAUNCH("k_balanced_swap_col_update");
+    };
+    for (int it = 0; it < iters; ++it) {
+        for (int n0 = 0; n0 < cp; n0 += cols) {
+            const int m = cp - n0 < cols ? cp - n0 : cols;
+            if (cols < cp) {
+                rc = launch_conv_taps_rows(wc_feat, Nc, Hc, Wc, C, wsplit + (long long)n0 * K, (long long)cp * K, m, BN, scores, st, patch);
+                if (rc) return rc;
+            }
+            column_pass(n0, m, nullptr);
+            if (maps)
+                k_softmax_swap_stats<true, true><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, cdiv(m, B), B,
+                                                                        SL.n_patches, ascale, inv_t, L.nblk, bstat, lab, hpot + n0, cp);
+            else
+                k_softmax_swap_stats<false, true><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, cdiv(m, B), B,
+                                                                         SL.n_patches, ascale, inv_t, L.nblk, bstat, lab, hpot + n0, cp);
+            WCTB_CHECK_LAUNCH("k_softmax_swap_stats");
+        }
+        k_softmax_swap_combine<<<swap_grid(na, 256), 256, 0, st>>>(bstat, na, L.nblk, inv_t, mz);
+        WCTB_CHECK_LAUNCH("k_softmax_swap_combine");
+    }
     // pass 2: the correlation again when it ran in more than one chunk (the scores are the same bits), then per block the
     // weight map, the block's filters, the fold on the tensor cores and its sum in block order
     WCTB_CUDA(cudaMemsetAsync(wmap, 0, (size_t)gm.plane * 2 * sizeof(__half), st));
@@ -3231,9 +3439,16 @@ static int style_swap_apply_softmax_impl(const __half* content, int Nc, int Hc, 
             rc = launch_conv_taps_rows(wc_feat, Nc, Hc, Wc, C, wsplit + (long long)n0 * K, (long long)cp * K, m, BN, scores, st, patch);
             if (rc) return rc;
         }
+        if (col_sums) column_pass(n0, m, col_sums);
         for (int c0 = 0; c0 < m; c0 += B) {
             const int b = (n0 + c0) / B;
-            if (maps)
+            if (iters > 0 && maps)
+                k_softmax_swap_weights<true, true><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, c0, SL.n_patches,
+                                                                          ascale, mz, inv_t, gm, wmap, lab, hpot + n0, cp);
+            else if (iters > 0)
+                k_softmax_swap_weights<false, true><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, c0, SL.n_patches,
+                                                                           ascale, mz, inv_t, gm, wmap, lab, hpot + n0, cp);
+            else if (maps)
                 k_softmax_swap_weights<true><<<agrid, 256, 0, st>>>(scores, ActGeom(Nc, Hc, Wc, m), q, n0, c0, SL.n_patches, ascale,
                                                                     mz, inv_t, gm, wmap, lab);
             else
@@ -3262,6 +3477,17 @@ int launch_style_swap_apply_softmax(const __half* content, int Nc, int Hc, int W
     const SwapLabelMaps maps = {content_labels, Ncl, Hm, Wm, style_labels, Hms, Wms, label_buf, label_bytes};
     return style_swap_apply_softmax_impl(content, Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, temperature,
                                          out, k_out, ws, ws_bytes, content_labels ? &maps : nullptr, st);
+}
+int launch_style_swap_apply_balanced(const __half* content, int Nc, int Hc, int Wc, int C, const void* state, int Hs, int Ws,
+                                     int patch, int stride, float alpha, float eps_cov, float thresh, float temperature, int iters,
+                                     const uint8_t* content_labels, int Ncl, int Hm, int Wm, const uint8_t* style_labels, int Hms,
+                                     int Wms, __half* out, int32_t* k_out, float* col_sums, void* ws, size_t ws_bytes,
+                                     void* label_buf, size_t label_bytes, cudaStream_t st) {
+    WCTB_REQUIRE((content_labels == nullptr) == (style_labels == nullptr),
+                 "style_swap_apply_balanced: give both label maps or neither");
+    const SwapLabelMaps maps = {content_labels, Ncl, Hm, Wm, style_labels, Hms, Wms, label_buf, label_bytes};
+    return style_swap_apply_softmax_impl(content, Nc, Hc, Wc, C, state, Hs, Ws, patch, stride, alpha, eps_cov, thresh, temperature,
+                                         out, k_out, ws, ws_bytes, content_labels ? &maps : nullptr, st, true, iters, col_sums);
 }
 
 int launch_style_swap_level(const __half* content, int Hc, int Wc, const __half* style, int Hs, int Ws, int C, int patch, int stride,

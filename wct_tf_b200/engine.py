@@ -366,27 +366,35 @@ class Engine(object):
                    int(stride), sem["eps_cov"], sem["thresh"], state.data_ptr(), None, ws.data_ptr(), ws.numel(), st)
         return state
 
-    def swap_apply(self, content, state, style_hw, ss_alpha, want_info=False, patch=3, stride=1, labels=None, temperature=None):
+    def swap_apply(self, content, state, style_hw, ss_alpha, want_info=False, patch=3, stride=1, labels=None, temperature=None,
+                   balance=0):
         """wct_style_swap (ops.py:145-217) of the N content frames against one prepared style (``swap_prepare``).
         ``labels``: (content labels cuda uint8 [1|N,Hm,Wm], style labels cuda uint8 [1,Hm',Wm']) of a labelled swap
         (DESIGN.md §3.3.13), each anchor matched only to the style patches of its own label.  ``temperature``: the softmax
-        swap at that temperature (DESIGN.md §3.3.17) instead of the arg-max; None is the hard swap."""
+        swap at that temperature (DESIGN.md §3.3.17) instead of the arg-max; None is the hard swap.  ``balance`` = T > 0
+        (with ``temperature``): the balanced swap (DESIGN.md §3.3.18), T Sinkhorn iterations that even out how much each
+        style patch is used; 0 is the softmax swap."""
         st = self._stream()
         C, N = content.C, content.N
         Hs, Ws = style_hw
         out = self._act(N, content.H, content.W, C)
         geom = (C, N, content.H, content.W, Hs, Ws, int(patch), int(stride))
         soft = temperature is not None
+        balance = int(balance)
+        if balance and not soft:
+            raise ValueError("the balanced swap needs a temperature")
         lib = self.lib
-        nbytes = (lib.wctb200_style_swap_softmax_workspace_bytes if soft else lib.wctb200_style_swap_apply_workspace_bytes)(*geom)
+        kind = "balanced" if balance else "softmax" if soft else None
+        nbytes = (getattr(lib, "wctb200_style_swap_%s_workspace_bytes" % kind) if kind
+                  else lib.wctb200_style_swap_apply_workspace_bytes)(*geom)
         if nbytes == 0:
             raise ValueError("style swap needs encodings of at least %dx%d (content %dx%d, style %dx%d)"
                              % (patch, patch, content.H, content.W, Hs, Ws))
         # the scores of the patch correlation are produced in chunks when they would not fit SWAP_WORKSPACE_BYTES; every
         # chunking gives the same bytes (include/wctb200.h: wctb200_style_swap_apply_min_workspace_bytes,
-        # wctb200_style_swap_softmax_min_workspace_bytes)
-        least = (lib.wctb200_style_swap_softmax_min_workspace_bytes if soft else lib.wctb200_style_swap_apply_min_workspace_bytes)(
-            *geom)
+        # wctb200_style_swap_softmax_min_workspace_bytes, wctb200_style_swap_balanced_min_workspace_bytes)
+        least = (getattr(lib, "wctb200_style_swap_%s_min_workspace_bytes" % kind) if kind
+                 else lib.wctb200_style_swap_apply_min_workspace_bytes)(*geom)
         nbytes = min(nbytes, max(least, SWAP_WORKSPACE_BYTES))
         ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         kbuf = torch.empty(N + 1, dtype=torch.int32, device=self.device) if want_info else None
@@ -402,7 +410,13 @@ class Engine(object):
         head = (content.ptr, N, content.H, content.W, C, state.data_ptr(), Hs, Ws, int(patch), int(stride), float(ss_alpha),
                 sem["eps_cov"], sem["thresh"])
         tail = (out.ptr, kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel())
-        if soft:
+        if balance:
+            self._call("style_swap_balanced[C%d]" % C,
+                       lib.wctb200_style_swap_balanced_launches(*geom, nbytes, int(lbuf is not None), balance, 0),
+                       lib.wctb200_style_swap_apply_balanced, *head, float(temperature), balance,
+                       *(lab if lbuf is not None else (None, 0, 0, 0, None, 0, 0)), *tail[:2], None, *tail[2:],
+                       None if lbuf is None else lbuf.data_ptr(), 0 if lbuf is None else lbuf.numel(), st)
+        elif soft:
             self._call("style_swap_softmax[C%d]" % C, lib.wctb200_style_swap_softmax_launches(*geom, nbytes, int(lbuf is not None)),
                        lib.wctb200_style_swap_apply_softmax, *head, float(temperature),
                        *(lab if lbuf is not None else (None, 0, 0, 0, None, 0, 0)), *tail,
@@ -844,7 +858,7 @@ class Engine(object):
                 ss_patch_size=3, ss_stride=1, labels=None, region_styles=None, interp_styles=None, interp_weights=None,
                 region_masks=None, swap_targets=None, ost=False, seamless=None, mst=None, mst_smooth=0.05, strength_map=None,
                 content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0, levels=None,
-                ss_temperature=None):
+                ss_temperature=None, ss_balance=0):
         """content_u8: cuda uint8 [N,H,W,3]; style_u8: cuda uint8 [Ns,Hs,Ws,3] or a ``PreparedStyle`` of Ns styles, Ns in
         {1, N}.  Returns the float32 ``decoded_output`` [N,H',W',3] (unclipped, model.py:94).
         ``capture`` (dict) receives every level's input image / features for parity tests.
@@ -884,7 +898,9 @@ class Engine(object):
         its own label, or on all of them when the style has none of that label.  The other levels are unchanged.
         ``ss_temperature`` = tau > 0 makes every swap level a softmax swap (DESIGN.md §3.3.17): each content patch is
         rebuilt from the blend of the style patches weighted by a softmax of their scores at temperature tau, instead of
-        its single best patch.  None is the hard swap.
+        its single best patch.  None is the hard swap.  ``ss_balance`` = T in 1..256 (with ``ss_temperature``) makes it the
+        balanced swap (DESIGN.md §3.3.18): T Sinkhorn iterations spread the blend's use of the style patches evenly; 0 is
+        the softmax swap.
 
         Optimal-transport transform: ``ost=True`` matches each level's content Gaussian to the style's by the Monge map
         (DESIGN.md §3.3.8) instead of WCT, against the same WCT style states; swap levels still swap.
@@ -932,6 +948,7 @@ class Engine(object):
             ("seamless", seamless is not None)) if on}, options.ENGINE)
         efdm_slices = options.check_efdm_slices(efdm_slices, efdm, options.ENGINE)
         ss_temperature = options.check_ss_temperature(ss_temperature, swap5 or swap_targets is not None, options.ENGINE)
+        ss_balance = options.check_ss_balance(ss_balance, ss_temperature, options.ENGINE)
         if efdm and isinstance(style_u8, PreparedStyle):
             skip = self.swap_levels(swap5, swap_targets)
             if any(relu not in style_u8.efdm and relu not in skip for relu in self.model.style_taps):
@@ -1027,7 +1044,7 @@ class Engine(object):
                                  alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
                                  ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm, efdm_slices=efdm_slices,
                                  swap_labels=None if swap_labels is None else _frame_labels(swap_labels, i, i + 1),
-                                 levels=levels, ss_temperature=ss_temperature)
+                                 levels=levels, ss_temperature=ss_temperature, ss_balance=ss_balance)
                     for i in range(N)]
             return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
@@ -1054,12 +1071,13 @@ class Engine(object):
                 return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
                                          seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm, efdm_slices=efdm_slices,
                                          swap_labels=None if swap_labels is None else _frame_labels(swap_labels, lo, hi),
-                                         run=chain, ss_temperature=ss_temperature)
+                                         run=chain, ss_temperature=ss_temperature, ss_balance=ss_balance)
             out = self._in_groups(N, G, main, run)
         else:
             out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
                                     swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft, efdm=efdm,
-                                    swap_labels=swap_labels, efdm_slices=efdm_slices, run=chain, ss_temperature=ss_temperature)
+                                    swap_labels=swap_labels, efdm_slices=efdm_slices, run=chain, ss_temperature=ss_temperature,
+                                    ss_balance=ss_balance)
         if owned is not None and owned.side is not main:
             owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
             if G == 1:
@@ -1356,7 +1374,8 @@ class Engine(object):
         return ps.swap[key]
 
     def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
-                     seamless=None, soft=None, efdm=False, swap_labels=None, efdm_slices=0, run=None, ss_temperature=None):
+                     seamless=None, soft=None, efdm=False, swap_labels=None, efdm_slices=0, run=None, ss_temperature=None,
+                     ss_balance=0):
         """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
         ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
         optimal-transport transform instead of WCT at the other levels, ``efdm`` exact feature distribution matching (in
@@ -1364,7 +1383,8 @@ class Engine(object):
         ``seamless``: the wrapped axes of the content path
         (the transforms write a reflect halo, which is rewritten before the decoder reads it); ``swap_labels``: the (content
         [1|N], style [1]) label maps of a labelled swap at the swap levels; ``run``: the levels to run (``run_levels``;
-        None: all); ``ss_temperature``: the softmax swap's temperature at the swap levels (None: the hard swap)."""
+        None: all); ``ss_temperature``: the softmax swap's temperature at the swap levels (None: the hard swap);
+        ``ss_balance``: the balanced swap's Sinkhorn iterations (0: the softmax swap)."""
         wrap = self.wrap_flags(seamless)
         lib, st = self.lib, self._stream()
         N = content_u8.shape[0]
@@ -1396,7 +1416,7 @@ class Engine(object):
                 main.wait_event(ev)
                 sf = style.feats[relu]
                 f, kbuf = self.swap_apply(cf, state, (sf.H, sf.W), ss_alpha, want_info, *swap[:2], labels=swap_labels,
-                                          temperature=ss_temperature)
+                                          temperature=ss_temperature, balance=ss_balance)
             else:
                 for sd in sides:
                     if sd.side is not main:

@@ -6,7 +6,8 @@ This is the one statement of that policy.  ``WCT.predict_batch``, ``Engine.styli
 
 ``swap_labels`` (the labelled style swap, ``check_swap_labels``) has no entry in ``SPELLINGS``: it is a parameter of
 ``swap``, as ``mst_smooth`` is of ``mst``.  It needs the swap, and through it takes the swap's exclusions; it adds none of
-its own.  ``ss_temperature`` (the softmax swap, ``check_ss_temperature``) is a parameter of ``swap`` in the same way.
+its own.  ``ss_temperature`` (the softmax swap, ``check_ss_temperature``) is a parameter of ``swap`` in the same way, and
+``ss_balance`` (the balanced swap, ``check_ss_balance``) a parameter of ``ss_temperature``.
 ``efdm_slices`` (sliced distribution matching, ``check_efdm_slices``) is in the same way a parameter of ``efdm``.
 
 ``coarse_to_fine`` (scale control, ``check_coarse_to_fine``) is in ``AROUND`` too: it runs the call on a downscaled
@@ -164,6 +165,18 @@ def check_ss_temperature(t, swap, vocab=API):
     if not swap:
         raise ValueError("%s needs %s: the temperature is the style swap's" % (name, vocab["swap"]))
     return float(t)
+
+
+def check_ss_balance(T, temperature, vocab=API):
+    """The Sinkhorn iterations of the balanced swap (DESIGN.md §3.3.18): an integer in 0..256, and above 0 only with the
+    softmax swap (``temperature``: its checked temperature, or None).  Returns it as an int; ValueError otherwise, naming
+    the options as ``vocab`` spells them."""
+    name, tname = ("--ss-balance", "--ss-temperature") if vocab is CLI else ("ss_balance", "ss_temperature")
+    if isinstance(T, bool) or not isinstance(T, (int, np.integer)) or not 0 <= T <= 256:
+        raise ValueError("%s must be an integer in 0..256, got %r" % (name, T))
+    if T and temperature is None:
+        raise ValueError("%s needs %s: the iterations balance the softmax swap" % (name, tname))
+    return int(T)
 
 
 def check_efdm_slices(K, efdm, vocab=API):

@@ -33,6 +33,8 @@ sm_90a engine (engine.py -> libwctb200.so).  Differences, all explicit:
     colours kept;
   * ``ss_temperature`` is new: the softmax swap, each content patch rebuilt from a softmax-weighted blend of style
     patches instead of its single best one;
+  * ``ss_balance`` is new: the balanced swap, Sinkhorn iterations that spread the softmax swap's use of the style
+    patches evenly;
   * ``coarse_to_fine`` is new: scale control (Gatys et al., CVPR 2017, §6), the call run on a downscaled content and its
     result joined into the content's low band before the fine levels run at full size.
 """
@@ -277,7 +279,8 @@ class WCT(object):
                       passes=1, return_device=False, content_mask=None, style_weights=None, style_masks=None,
                       swap_targets=None, temporal=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
                       strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None,
-                      efdm_slices=0, luminance_only=False, coarse_to_fine=None, fine_targets=None, ss_temperature=None):
+                      efdm_slices=0, luminance_only=False, coarse_to_fine=None, fine_targets=None, ss_temperature=None,
+                      ss_balance=0):
         """contents: uint8 [N,H,W,3]; styles: uint8 [1|N,Hs,Ws,3] (numpy or torch; host buffers --
         ideally pinned -- or device tensors).  Returns uint8 [N,H',W',3] on the host: a numpy array,
         or ``out`` (a pinned uint8 torch tensor of the right shape) filled in place.  The call is
@@ -378,6 +381,12 @@ class WCT(object):
         the blend is over the patches of the anchor's label.  It acts in the first pass only, like the swap.  None is the
         hard swap.
 
+        ``ss_balance`` = T in 1..256 (balanced swap, DESIGN.md §3.3.18; with ``ss_temperature``): T Sinkhorn iterations
+        turn the softmax swap's per-anchor weights into a plan whose columns are balanced too, so that every style patch is
+        used about as much as the uniform blend would use it, instead of a few bland patches covering large regions.
+        Each iteration costs about one more pass over the patch scores.  It acts in the first pass only, like the swap.
+        0 is the softmax swap.
+
         ``luminance_only`` (colour preservation, DESIGN.md §3.3.15): stylise the luminance only and keep the content's
         colours.  The content frames (after a stride swap's crop) are made grey with the style's luminance mean and spread
         (``device_image.luminance_match``), the call runs with every other option on them against the grey of each style
@@ -413,6 +422,7 @@ class WCT(object):
             ctf = options.check_coarse_to_fine(coarse_to_fine, fine_targets, self.model.relu_targets)
         efdm_slices = options.check_efdm_slices(efdm_slices, efdm)
         ss_temperature = options.check_ss_temperature(ss_temperature, swap5 or swap_targets is not None)
+        ss_balance = options.check_ss_balance(ss_balance, ss_temperature)
         if mask_feather is not None:
             options.check_mask_feather(mask_feather)
         if mst is not None:
@@ -536,7 +546,8 @@ class WCT(object):
                                        ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
                                        swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, efdm=efdm,
                                        efdm_slices=efdm_slices, swap_labels=lab_dev if first else None, levels=levels,
-                                       ss_temperature=ss_temperature if first else None, **soft_kw)
+                                       ss_temperature=ss_temperature if first else None,
+                                       ss_balance=ss_balance if first else 0, **soft_kw)
             if ctf is not None:
                 whole = one_pass
 
@@ -752,7 +763,7 @@ class WCT(object):
     def predict(self, content, style, alpha=1, swap5=False, ss_alpha=1, adain=False, content_mask=None, style_weights=None,
                 style_masks=None, swap_targets=None, tile_size=None, ost=False, seamless=None, mst=None, mst_smooth=0.05,
                 strength_map=None, content_weights=None, mask_feather=None, efdm=False, swap_labels=None, efdm_slices=0,
-                luminance_only=False, coarse_to_fine=None, fine_targets=None, ss_temperature=None):
+                luminance_only=False, coarse_to_fine=None, fine_targets=None, ss_temperature=None, ss_balance=0):
         '''Stylize a single content/style pair (wct.py:70-106).  With ``content_mask`` (uint8 [Hm,Wm] label map), ``style``
         is a list of R region styles and region r of the content takes style r (with ``style_masks``, the pixels of style r
         labelled r).  With ``style_weights`` ([K]), ``style`` is a list of K styles and the content takes their weighted
@@ -761,7 +772,7 @@ class WCT(object):
         value distribution to the style's (first in ``efdm_slices`` rotated bases); ``strength_map``, ``content_weights``
         ([K,Hm,Wm], with ``style`` a list of K region styles) and ``mask_feather`` are soft spatial control
         (``predict_batch``); ``swap_labels`` = (content labels [Hm,Wm], style labels [Hm',Wm']) steers the style swap and
-        ``ss_temperature`` makes it the softmax swap; ``luminance_only`` stylises the luminance and keeps the content's colours; ``coarse_to_fine`` = f stylises a 1/f
+        ``ss_temperature`` makes it the softmax swap, ``ss_balance`` the balanced swap; ``luminance_only`` stylises the luminance and keeps the content's colours; ``coarse_to_fine`` = f stylises a 1/f
         copy at every level first and ``fine_targets`` at full size (scale control).'''
         s = time.time()
         seen = {}
@@ -781,7 +792,7 @@ class WCT(object):
                                  mst_smooth=mst_smooth, strength_map=strength_map, content_weights=content_weights,
                                  mask_feather=mask_feather, efdm=efdm, swap_labels=swap_labels, efdm_slices=efdm_slices,
                                  luminance_only=luminance_only, coarse_to_fine=coarse_to_fine, fine_targets=fine_targets,
-                                 ss_temperature=ss_temperature)
+                                 ss_temperature=ss_temperature, ss_balance=ss_balance)
         if self.verbose:
             print("Stylized in:", time.time() - s)   # wct.py:104
         return out[0]
