@@ -6,7 +6,9 @@ hand-written sm_90a kernel behind the C-ABI (include/wctb200.h).
 """
 from __future__ import annotations
 
+import collections
 import ctypes
+import dataclasses
 
 import numpy as np
 import torch
@@ -48,17 +50,46 @@ class Act(object):
         return self.buf.data_ptr()
 
 
-def _frame_labels(swap_labels, lo, hi):
-    """The (content, style) label maps of frames lo..hi of a labelled swap: a stack of one map per frame is sliced, a
-    shared map [1,...] is kept."""
-    return tuple(t if t.shape[0] == 1 else t[lo:hi] for t in swap_labels)
+def style_states(adain=False, efdm=False, efdm_slices=0):
+    """The per-level style states a call applies, as keywords of ``Engine._style_side``: the WCT states (also read by OST),
+    the AdaIN moments, or the EFDM states of ``efdm_slices`` slices."""
+    return dict(wct=not adain and not efdm, adain=adain, efdm=efdm, efdm_slices=efdm_slices)
 
 
-def _soft_slice(soft, lo, hi):
-    """The maps of a soft spatial-control call (strength, weights) for frames [lo, hi)."""
-    if soft is None:
-        return None
-    return tuple(None if m is None else m[lo:hi] for m in soft)
+# the style swap of a call (DESIGN.md §3.3.5, §3.3.13, §3.3.17, §3.3.18): patch and stride, the relu levels it replaces the
+# transform at, ss_alpha, the (content, style) label maps or None, the softmax temperature or None, the Sinkhorn iterations
+Swap = collections.namedtuple("Swap", "patch stride levels alpha labels temperature balance")
+
+
+@dataclasses.dataclass(frozen=True)
+class Plan(object):
+    """What one ``Engine.stylize`` call runs, decided once from its checked arguments."""
+    run: list                       # the levels to run (``run_levels``)
+    alpha: float
+    transform: str = "wct"          # of the levels that do not swap: "wct", "ost", "adain" or "efdm"
+    slices: int = 0                 # with "efdm": the K rotated bases of sliced EFDM
+    swap: Swap = None
+    mode: str = None                # several styles: "regions", "interp" or "mst"; None for one style side
+    labels: torch.Tensor = None     # "regions": the label maps [N,Hm,Wm]
+    masks: list = None              # "regions": the style masks (``check_region_masks``) or None
+    weights: torch.Tensor = None    # "interp": the weight rows [1|N,K]
+    mst: tuple = None               # "mst": (K, lambda)
+    soft: tuple = None              # soft spatial control: (strength [N,Hm,Wm] | None, weights [N,K,Hm,Wm] | None)
+    seamless: str = None
+
+    @property
+    def states(self):
+        return style_states(self.transform == "adain", self.transform == "efdm", self.slices)
+
+    def frames(self, lo, hi):
+        """The plan of frames [lo, hi): the per-frame maps and rows are sliced, a shared one ([1,...]) is kept."""
+        def cut(t):
+            return t if t is None or t.shape[0] == 1 else t[lo:hi]
+        swap = self.swap
+        if swap is not None and swap.labels is not None:
+            swap = swap._replace(labels=tuple(cut(t) for t in swap.labels))
+        return dataclasses.replace(self, swap=swap, labels=cut(self.labels), weights=cut(self.weights),
+                                   soft=None if self.soft is None else tuple(cut(m) for m in self.soft))
 
 
 class Engine(object):
@@ -431,25 +462,6 @@ class Engine(object):
         ws.record_stream(cur)   # freed by the caching allocator only after this stream is done
         return out, kbuf
 
-    def style_swap(self, content, style, ss_alpha, want_info=False, patch=3, stride=1):
-        """wct_style_swap (ops.py:145-217) on one content/style pair with ``patch`` x ``patch`` windows every ``stride``."""
-        assert content.N == 1 and style.N == 1, "style swap works on one content/style pair (ops.py:146)"
-        st = self._stream()
-        C = content.C
-        out = self._act(1, content.H, content.W, C)
-        nbytes = self.lib.wctb200_style_swap_workspace_bytes(C, content.H, content.W, style.H, style.W, int(patch), int(stride))
-        if nbytes == 0:
-            raise ValueError("style swap needs encodings of at least %dx%d (content %dx%d, style %dx%d)"
-                             % (patch, patch, content.H, content.W, style.H, style.W))
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        kbuf = torch.empty(4, dtype=torch.int32, device=self.device) if want_info else None
-        sem = SEMANTICS["tf"]                  # the reference only has the TF graph version of this op
-        self._call("style_swap[C%d]" % C, 22, self.lib.wctb200_style_swap_level, content.ptr, content.H, content.W, style.ptr,
-                   style.H, style.W, C, int(patch), int(stride), float(ss_alpha), sem["eps_cov"], sem["thresh"], out.ptr,
-                   kbuf.data_ptr() if want_info else None, ws.data_ptr(), ws.numel(), st)
-        ws.record_stream(torch.cuda.current_stream(self.device))   # freed by the caching allocator only after this stream is done
-        return out, kbuf
-
     def style_prepare(self, style):
         """Style side of one level (ops.py:48-55,76): means, covariance, eigendecomposition, C_s.
         Returns the device state buffer consumed by ``wct_apply``."""
@@ -684,34 +696,6 @@ class Engine(object):
         style_u8.record_stream(ps.side)
         return ps
 
-    def _stylize_mst(self, content_u8, style, K, lam, alpha, want_info, capture):
-        """``stylize`` with multimodal style transfer: the style side clusters each level's style feature (``_style_side``
-        with ``mst``) unless ``style`` is such a side already, and every sub-batch group labels and transforms its frames."""
-        N = content_u8.shape[0]
-        main = torch.cuda.current_stream(self.device)
-        G = min(self.groups, N) if (capture is None and not want_info) else 1
-        owned = None
-        if isinstance(style, PreparedStyle):
-            ps = style
-        else:
-            self._group = 1 if G > 1 else 0
-            try:
-                ps = owned = self._style_side(style, main, mst=K)
-            finally:
-                self._group = 0
-        multi = ("mst", (lam, ps), ps.entries)
-        if G == 1:
-            out = self._stylize_one(content_u8, None, alpha, False, want_info, capture, multi=multi)
-        else:
-            out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, False, False, None,
-                                                                               multi=multi))
-        if owned is not None and owned.side is not main:
-            owned.side.wait_stream(main)        # the style states are recycled only after every level used them
-            main.wait_stream(owned.side)
-        elif owned is None:
-            ps.record_stream(main)
-        return out
-
     # ------------------------------------------------------------------ exact feature distribution matching (§3.3.12)
     def _efdm_chunk(self, total, per_seg_fn):
         """(segments per chunk, chunks) of an EFDM sort of ``total`` segments within EFDM_WORKSPACE_BYTES."""
@@ -816,20 +800,6 @@ class Engine(object):
                    sem["eps_cov"], sem["eps_eig"], sem["thresh"], sem["readd"], out.ptr, kbuf.data_ptr() if want_info else None,
                    ws.data_ptr(), ws.numel(), st, flops=2.0 * C * C * 2 * N * hwc, bytes_=4.0 * C * 2 * N * hwc)
         return out, kbuf
-
-    def adain_blend(self, content, styles, weights, alpha):
-        """AdaIN against the blend of the K style feature maps ``styles`` (each [1,Hs,Ws,C], any sizes) with the weights of
-        ``weights`` (cuda fp32 [1|N, K])."""
-        st = self._stream()
-        C, N, K, Nw = content.C, content.N, len(styles), weights.shape[0]
-        out = self._act(N, content.H, content.W, C)
-        ws = self._grow_workspace(("adain_blend", C, N, K), self.lib.wctb200_adain_blend_workspace_bytes(C, N, K))
-        hws = sum(s.H * s.W for s in styles)
-        self._call("adain_blend[C%d]" % C, 5 + 3 * K, self.lib.wctb200_adain_blend, content.ptr, N, content.H, content.W, C,
-                   _capi.pointer_array([s.ptr for s in styles]), _capi.int_array([s.H for s in styles]),
-                   _capi.int_array([s.W for s in styles]), K, weights.data_ptr(), Nw, float(alpha), 1e-5, out.ptr, ws.data_ptr(),
-                   ws.numel(), st, bytes_=4.0 * C * (2 * N * content.H * content.W + hws))
-        return out, None
 
     # ------------------------------------------------------------------ pipeline
     def run_levels(self, levels=None):
@@ -949,6 +919,7 @@ class Engine(object):
         efdm_slices = options.check_efdm_slices(efdm_slices, efdm, options.ENGINE)
         ss_temperature = options.check_ss_temperature(ss_temperature, swap5 or swap_targets is not None, options.ENGINE)
         ss_balance = options.check_ss_balance(ss_balance, ss_temperature, options.ENGINE)
+        transform = "adain" if adain else "efdm" if efdm else "ost" if ost else "wct"
         if efdm and isinstance(style_u8, PreparedStyle):
             skip = self.swap_levels(swap5, swap_targets)
             if any(relu not in style_u8.efdm and relu not in skip for relu in self.model.style_taps):
@@ -995,7 +966,7 @@ class Engine(object):
                                      "give the style image")
             elif style_u8.shape[0] != 1:
                 raise ValueError("mst takes one style for the whole batch, got %d" % style_u8.shape[0])
-            return self._stylize_mst(content_u8, style_u8, K, lam, alpha, want_info, capture)
+            return self._stylize_call(content_u8, style_u8, Plan(chain, alpha, mode="mst", mst=(K, lam)), want_info, capture)
         if seamless is not None:
             check_seamless(seamless, content_u8.shape[1], content_u8.shape[2], self.model.relu_targets)
         swap_lv = self.swap_levels(swap5, swap_targets)
@@ -1015,8 +986,8 @@ class Engine(object):
                     or w.shape[1] != K or w.device != self.device):
                 raise ValueError("interp_weights must be a float32 tensor [1|N, K] on %s" % self.device)
             w = w.contiguous()
-            return self._stylize_multi(content_u8, list(interp_styles), alpha, adain, want_info, capture,
-                                       lambda lo, hi: ("interp", w if w.shape[0] == 1 else w[lo:hi]), seamless=seamless, run=chain)
+            return self._stylize_call(content_u8, list(interp_styles), Plan(chain, alpha, transform, mode="interp", weights=w,
+                                                                            seamless=seamless), want_info, capture)
         if labels is not None:
             R = len(region_styles) if region_styles is not None else 0
             if not 1 <= R <= 8:
@@ -1028,60 +999,83 @@ class Engine(object):
             labels = labels.expand(N, -1, -1).contiguous()
             if region_masks is not None:
                 region_masks = self.check_region_masks(region_masks, region_styles)
-            return self._stylize_multi(content_u8, list(region_styles), alpha, False, want_info, capture,
-                                       lambda lo, hi: ("regions", labels[lo:hi]), masks=region_masks, seamless=seamless, soft=soft,
-                                       run=chain)
+            return self._stylize_call(content_u8, list(region_styles), Plan(chain, alpha, mode="regions", labels=labels,
+                                                                            masks=region_masks, soft=soft, seamless=seamless),
+                                      want_info, capture)
         prepared = isinstance(style_u8, PreparedStyle)
         n_style = style_u8.n if prepared else style_u8.shape[0]
         if n_style not in (1, N):
             raise ValueError("%d styles for %d frames: give one style, or one per frame" % (n_style, N))
         if prepared and not efdm:
             self.check_prepared(style_u8, adain, swap_lv)
+        swap = (Swap(int(ss_patch_size), int(ss_stride), swap_lv, ss_alpha, swap_labels, ss_temperature, ss_balance)
+                if swap_lv else None)
+        return self._stylize_call(content_u8, style_u8, Plan(chain, alpha, transform, efdm_slices, swap=swap, soft=soft,
+                                                             seamless=seamless), want_info, capture)
+
+    def _stylize_call(self, content_u8, style, plan, want_info, capture):
+        """Run ``plan`` on the frames ``content_u8`` against ``style``: an image batch or ``PreparedStyle`` of 1 or N styles
+        (one style side, or the MST side), or the list of styles of a "regions" / "interp" call.
+
+        The style sides that serve the whole batch -- those of a multi-style call, and one shared style image that the
+        groups or the swap reuse -- are made here once, on group 1's style stream when the batch is cut into G sub-batch
+        groups.  Otherwise each group prepares, or slices, the styles of its own frames.  With one style per frame and a
+        swap the frames run one by one, each with its own style side."""
+        N = content_u8.shape[0]
+        prepared = isinstance(style, PreparedStyle)
+        if plan.swap is not None and (style.n if prepared else style.shape[0]) > 1:
+            return torch.cat([self._stylize_call(content_u8[i:i + 1], self.slice_prepared(style, i, i + 1) if prepared
+                                                 else style[i:i + 1], plan.frames(i, i + 1), want_info, None)
+                              for i in range(N)], dim=0)
         main = torch.cuda.current_stream(self.device)
-        if swap_lv and n_style > 1:
-            # one style per frame: frame by frame (each frame's swap has its own style side)
-            outs = [self.stylize(content_u8[i:i + 1], self.slice_prepared(style_u8, i, i + 1) if prepared else style_u8[i:i + 1],
-                                 alpha=alpha, adain=adain, want_info=want_info, swap_targets=list(swap_lv), ss_alpha=ss_alpha,
-                                 ss_patch_size=ss_patch_size, ss_stride=ss_stride, ost=ost, efdm=efdm, efdm_slices=efdm_slices,
-                                 swap_labels=None if swap_labels is None else _frame_labels(swap_labels, i, i + 1),
-                                 levels=levels, ss_temperature=ss_temperature, ss_balance=ss_balance)
-                    for i in range(N)]
-            return torch.cat(outs, dim=0)
         G = min(self.groups, N) if (capture is None and not want_info) else 1
-        swap = (int(ss_patch_size), int(ss_stride), swap_lv) if swap_lv else None
-        shared = style_u8 if (prepared and n_style == 1) else None
-        owned = None
-        if n_style == 1 and not prepared and (G > 1 or swap_lv):
-            # ONE style for the whole batch (video, configs[2]): its encoder pass and per-level states are made once, every
-            # sub-batch group waits for the per-level events
-            self._group = 1 if G > 1 else 0
-            try:
-                owned = shared = self._style_side(style_u8, main, wct=not adain and not efdm, adain=adain, keep=swap_lv, skip=swap_lv,
-                                                  efdm=efdm, efdm_slices=efdm_slices)
-            finally:
-                self._group = 0
-        for relu in swap_lv:
-            self.swap_state(shared, relu, *swap[:2])
-        if G > 1:
-            def run(lo, hi):
-                if shared is not None:
-                    sg = shared
-                else:
-                    sg = self.slice_prepared(style_u8, lo, hi) if prepared else style_u8[lo:hi]
-                return self._stylize_one(content_u8[lo:hi], sg, alpha, adain, False, None, swap=swap, ss_alpha=ss_alpha, ost=ost,
-                                         seamless=seamless, soft=_soft_slice(soft, lo, hi), efdm=efdm, efdm_slices=efdm_slices,
-                                         swap_labels=None if swap_labels is None else _frame_labels(swap_labels, lo, hi),
-                                         run=chain, ss_temperature=ss_temperature, ss_balance=ss_balance)
-            out = self._in_groups(N, G, main, run)
-        else:
-            out = self._stylize_one(content_u8, shared if shared is not None else style_u8, alpha, adain, want_info, capture,
-                                    swap=swap, ss_alpha=ss_alpha, ost=ost, seamless=seamless, soft=soft, efdm=efdm,
-                                    swap_labels=swap_labels, efdm_slices=efdm_slices, run=chain, ss_temperature=ss_temperature,
-                                    ss_balance=ss_balance)
-        if owned is not None and owned.side is not main:
-            owned.side.wait_stream(main)        # the shared style states are recycled only after every group used them
-            if G == 1:
-                main.wait_stream(owned.side)
+        sides, owned = None, []
+        self._group = 1 if G > 1 else 0
+        try:
+            if plan.mode == "mst":
+                ps = style if prepared else self._style_side(style, main, mst=plan.mst[0])
+                sides, owned = ps.entries, [] if prepared else [ps]
+            elif plan.mode is not None:
+                sides, owned = self._region_sides(style, plan.masks, main, plan.transform == "adain")
+            elif prepared and style.n == 1:
+                sides = [style]
+            elif not prepared and style.shape[0] == 1 and (G > 1 or plan.swap is not None):
+                # ONE style for the whole batch (video, configs[2]): its encoder pass and per-level states are made once,
+                # every sub-batch group waits for the per-level events
+                keep = plan.swap.levels if plan.swap is not None else ()
+                sides = owned = [self._style_side(style, main, keep=keep, skip=keep, **plan.states)]
+        finally:
+            self._group = 0
+        if plan.swap is not None:
+            for relu in plan.swap.levels:
+                self.swap_state(sides[0], relu, plan.swap.patch, plan.swap.stride)
+
+        def group(lo, hi, want_info, capture):
+            cur = torch.cuda.current_stream(self.device)
+            held, mine = sides, None
+            if held is None and prepared:
+                held = [style if G == 1 else self.slice_prepared(style, lo, hi)]
+            elif held is None:
+                assert style.dtype == torch.uint8 and style.shape[0] in (1, N)
+                mine = self._style_side(style[lo:hi], cur, **plan.states)
+                held = [mine]
+            out = self._stylize_one(content_u8[lo:hi], held, plan.frames(lo, hi), want_info, capture)
+            for sd in held:
+                if sd is not mine:
+                    sd.record_stream(cur)      # a prepared style held by the caller may be dropped while this work is queued
+            if mine is not None and mine.side is not cur:
+                mine.side.wait_stream(cur)     # buffers handed across streams may be recycled only after both are done
+                cur.wait_stream(mine.side)
+            return out
+
+        out = group(0, N, want_info, capture) if G == 1 else self._in_groups(N, G, main, lambda lo, hi: group(lo, hi, False, None))
+        for side in {id(sd.side): sd.side for sd in owned}.values():
+            if side is not main:
+                side.wait_stream(main)         # the style states are recycled only after every group used them
+                if G == 1 or plan.mode is not None:
+                    main.wait_stream(side)
+        if plan.mode == "mst" and prepared:
+            style.record_stream(main)          # the caller's clustered side, whose entries the groups applied
         return out
 
     def _in_groups(self, N, G, main, run):
@@ -1148,7 +1142,7 @@ class Engine(object):
                 self.check_prepared(s, adain)
                 sides.append(s)
             elif masks is None:
-                owned.append(self._style_side(s, main, wct=not adain, adain=adain))
+                owned.append(self._style_side(s, main, **style_states(adain)))
                 sides.append(owned[-1])
             else:
                 key = (id(s), id(m))
@@ -1170,34 +1164,6 @@ class Engine(object):
                 if m is not None:
                     m.record_stream(side)
         return sides
-
-    def _stylize_multi(self, content_u8, styles, alpha, adain, want_info, capture, per_frame, masks=None, seamless=None, soft=None,
-                       run=None):
-        """``stylize`` with several styles (spatial control, style interpolation): images are prepared once per call, and
-        every style side is shared by every sub-batch group.  ``per_frame(lo, hi)`` gives (mode, the frames' slice of the
-        label maps or weight rows); ``masks``: the style masks of spatial control (``_region_sides``); ``run``: the levels
-        to run (``run_levels``)."""
-        N = content_u8.shape[0]
-        main = torch.cuda.current_stream(self.device)
-        G = min(self.groups, N) if (capture is None and not want_info) else 1
-        self._group = 1 if G > 1 else 0
-        try:
-            sides, owned = self._region_sides(styles, masks, main, adain)
-        finally:
-            self._group = 0
-        if G == 1:
-            out = self._stylize_one(content_u8, None, alpha, adain, want_info, capture, multi=per_frame(0, N) + (sides,),
-                                    seamless=seamless, soft=soft, run=run)
-        else:
-            out = self._in_groups(N, G, main, lambda lo, hi: self._stylize_one(content_u8[lo:hi], None, alpha, adain, False, None,
-                                                                               multi=per_frame(lo, hi) + (sides,),
-                                                                               seamless=seamless, soft=_soft_slice(soft, lo, hi),
-                                                                               run=run))
-        for side in {id(sd.side): sd.side for sd in owned}.values():
-            if side is not main:
-                side.wait_stream(main)         # the style states are recycled only after every level used them
-                main.wait_stream(side)
-        return out
 
     def _style_stream(self):
         """This group's style stream (the style side overlaps the content work), or None without overlap."""
@@ -1222,7 +1188,7 @@ class Engine(object):
 
         With ``mst`` = K (one style image) each level's style feature is clustered (``mst_clusters``) and its WCT state is
         the masked prepare of the K clusters under the style's own labels: a prepared style of n = K with ``entries`` as
-        above, and the labels, centres and info of every level in ``mst``.
+        above, and the labels, centres and info of every level in ``mst``, which the entries share.
 
         With ``efdm`` every level also gets its EFDM state (``efdm_prepare``: the style's values sorted per channel) in
         ``efdm``.  With ``efdm_slices`` = K > 0 as well (sliced EFDM, §3.3.14), a side of one style also makes the K
@@ -1242,7 +1208,7 @@ class Engine(object):
         if labels is not None or mst:
             ps.entries = [PreparedStyle(1, ps.semantics, taps) for _ in range(R)]
             for e in ps.entries:
-                e.side, e.events = side, ps.events
+                e.side, e.events, e.mst = side, ps.events, ps.mst
         with torch.cuda.stream(side):
             tag, self._tag = self._tag, "style"
             style = torch.empty(style_u8.shape, dtype=torch.float32, device=self.device)
@@ -1298,8 +1264,7 @@ class Engine(object):
         every slice; the features of the swap levels of ``swap5`` / ``swap_targets``), made once for a call that applies it
         several times (passes)."""
         main = torch.cuda.current_stream(self.device)
-        ps = self._style_side(style_u8, main, wct=not adain and not efdm, adain=adain, keep=self.swap_levels(swap5, swap_targets),
-                              efdm=efdm, efdm_slices=efdm_slices)
+        ps = self._style_side(style_u8, main, keep=self.swap_levels(swap5, swap_targets), **style_states(adain, efdm, efdm_slices))
         style_u8.record_stream(ps.side)
         return ps
 
@@ -1373,86 +1338,21 @@ class Engine(object):
             ps.swap[key] = (state, ev)
         return ps.swap[key]
 
-    def _stylize_one(self, content_u8, style, alpha, adain, want_info, capture, swap=None, ss_alpha=0.6, multi=None, ost=False,
-                     seamless=None, soft=None, efdm=False, swap_labels=None, efdm_slices=0, run=None, ss_temperature=None,
-                     ss_balance=0):
-        """The level chain of one (sub-)batch.  ``style``: a cuda uint8 image batch (prepared here) or a ``PreparedStyle``;
-        ``swap``: (patch, stride, levels) of the style swap (its states are made by ``swap_state`` beforehand); ``ost``: the
-        optimal-transport transform instead of WCT at the other levels, ``efdm`` exact feature distribution matching (in
-        ``efdm_slices`` rotated bases first when > 0);
-        ``seamless``: the wrapped axes of the content path
-        (the transforms write a reflect halo, which is rewritten before the decoder reads it); ``swap_labels``: the (content
-        [1|N], style [1]) label maps of a labelled swap at the swap levels; ``run``: the levels to run (``run_levels``;
-        None: all); ``ss_temperature``: the softmax swap's temperature at the swap levels (None: the hard swap);
-        ``ss_balance``: the balanced swap's Sinkhorn iterations (0: the softmax swap)."""
-        wrap = self.wrap_flags(seamless)
-        lib, st = self.lib, self._stream()
-        N = content_u8.shape[0]
-        main = torch.cuda.current_stream(self.device)
-        owned = None
-        if multi is None:
-            assert content_u8.dtype == torch.uint8
-            if not isinstance(style, PreparedStyle):
-                assert style.dtype == torch.uint8 and style.shape[0] in (1, N)
-                owned = style = self._style_side(style, main, wct=not adain and not efdm, adain=adain, efdm=efdm,
-                                                 efdm_slices=efdm_slices)
-            n_style = style.n
-            sides = [style]
+    def _stylize_one(self, content_u8, sides, plan, want_info, capture):
+        """The level chain of ``plan`` on one (sub-)batch against the style ``sides`` (``_stylize_call``).  With
+        ``plan.seamless`` the transforms write a reflect halo, which is rewritten before the decoder reads it."""
+        assert content_u8.dtype == torch.uint8
+        wrap = self.wrap_flags(plan.seamless)
         content = torch.empty(content_u8.shape, dtype=torch.float32, device=self.device)
-        self._call("u8_to_f32", 1, lib.wctb200_image_u8_to_f32, content_u8.data_ptr(), content_u8.numel(), content.data_ptr(), st)
-        if multi is not None:
-            # ("regions", labels [N,Hm,Wm], R style sides) or ("interp", weight rows [1|N,K], K style sides): _stylize_multi;
-            # ("mst", (lambda, the MST side), its K cluster sides): _stylize_mst
-            mode, per_frame, sides = multi
+        self._call("u8_to_f32", 1, self.lib.wctb200_image_u8_to_f32, content_u8.data_ptr(), content_u8.numel(), content.data_ptr(),
+                   self._stream())
         infos = []
         x = content
-        run = self.model.levels if run is None else run
-        for lvl in run:
+        for lvl in plan.run:
             relu = lvl.relu_target
             self._tag = relu
-            cf, _ = self.encode(x, relu, seamless=seamless)
-            if swap is not None and relu in swap[2]:      # model.py:148-152: style swap wins over AdaIN / WCT at its levels
-                state, ev = style.swap[(relu,) + swap[:2]]
-                main.wait_event(ev)
-                sf = style.feats[relu]
-                f, kbuf = self.swap_apply(cf, state, (sf.H, sf.W), ss_alpha, want_info, *swap[:2], labels=swap_labels,
-                                          temperature=ss_temperature, balance=ss_balance)
-            else:
-                for sd in sides:
-                    if sd.side is not main:
-                        sd.wait(main, relu)
-                if soft is not None and multi is None:
-                    f, kbuf = self.soft_level(cf, soft, style.adain[relu] if adain else style.wct[relu], n_style, alpha, adain, ost)
-                elif soft is not None:             # regions: soft weights, or the hard labels' one-hot planes
-                    f, kbuf = self.soft_level(cf, soft, [sd.wct[relu] for sd in sides], None, alpha,
-                                              labels=per_frame if soft[1] is None else None)
-                elif multi is None:
-                    if adain:
-                        f, kbuf = self.adain_apply(cf, style.adain[relu], n_style, alpha)
-                    elif efdm and efdm_slices:
-                        f, kbuf = self.efdm_sliced_apply(cf, style.efdm[relu], n_style, alpha, style.feats.get(relu))
-                    elif efdm:
-                        f, kbuf = self.efdm_apply(cf, style.efdm[relu], n_style, alpha)
-                    elif ost:
-                        f, kbuf = self.ost_apply(cf, style.wct[relu], n_style, alpha, want_info)
-                    else:
-                        f, kbuf = self.wct_apply(cf, style.wct[relu], n_style, alpha, want_info)
-                elif mode == "regions":
-                    lab = self.labels_resize(per_frame, cf.H, cf.W)
-                    f, kbuf = self.wct_apply_regions(cf, lab, [sd.wct[relu] for sd in sides], alpha, want_info)
-                elif mode == "mst":
-                    lam, ms = per_frame
-                    m = ms.mst[relu]
-                    lab = self.mst_smooth(self.mst_data_term(cf, m["centres"], m["info"]), lam)
-                    f, kbuf = self.wct_apply_regions(cf, lab, [sd.wct[relu] for sd in sides], alpha, want_info)
-                    if capture is not None:
-                        for key, val in (("mst_style_labels", m["labels"]), ("mst_centres", m["centres"]), ("mst_info", m["info"]),
-                                         ("mst_content_labels", lab)):
-                            capture.setdefault(key, []).append(val)
-                elif adain:
-                    f, kbuf = self.adain_apply_blend(cf, [sd.adain[relu] for sd in sides], per_frame, alpha)
-                else:
-                    f, kbuf = self.wct_apply_blend(cf, [sd.wct[relu] for sd in sides], per_frame, alpha, want_info)
+            cf, _ = self.encode(x, relu, seamless=plan.seamless)
+            f, kbuf = self._level(cf, relu, sides, plan, want_info, capture)
             if wrap:
                 self.halo(f, wrap)
             infos.append(kbuf)
@@ -1461,19 +1361,61 @@ class Engine(object):
                 capture.setdefault("content_feat", []).append(cf)
                 capture.setdefault("transformed", []).append(f)
             # model.py:86: clip between levels; model.py:94: last output unclipped
-            x = self.decode(f, lvl.index, clip=lvl is not run[-1], seamless=seamless)
+            x = self.decode(f, lvl.index, clip=lvl is not plan.run[-1], seamless=plan.seamless)
             if capture is not None:
                 capture.setdefault("level_output", []).append(x)
         self._tag = None
-        for sd in sides:
-            if sd is not owned:
-                sd.record_stream(main)         # a prepared style held by the caller may be dropped while this work is queued
-        if owned is not None and owned.side is not main:
-            owned.side.wait_stream(main)       # buffers handed across streams may be recycled only after both are done
-            main.wait_stream(owned.side)
         if want_info:
             self.last_info = infos
         return x
+
+    def _level(self, cf, relu, sides, plan, want_info, capture):
+        """The transform of level ``relu`` of ``plan`` on the content feature ``cf``: the one place that picks it.
+        Returns (the transformed feature, the level's info or None)."""
+        main = torch.cuda.current_stream(self.device)
+        sw, alpha = plan.swap, plan.alpha
+        if sw is not None and relu in sw.levels:      # model.py:148-152: style swap wins over AdaIN / WCT at its levels
+            state, ev = sides[0].swap[(relu, sw.patch, sw.stride)]
+            main.wait_event(ev)
+            sf = sides[0].feats[relu]
+            return self.swap_apply(cf, state, (sf.H, sf.W), sw.alpha, want_info, sw.patch, sw.stride, labels=sw.labels,
+                                   temperature=sw.temperature, balance=sw.balance)
+        for sd in sides:
+            if sd.side is not main:
+                sd.wait(main, relu)
+        adain = plan.transform == "adain"
+        if plan.mode is None:
+            style = sides[0]
+            if plan.soft is not None:
+                return self.soft_level(cf, plan.soft, style.adain[relu] if adain else style.wct[relu], style.n, alpha, adain,
+                                       plan.transform == "ost")
+            if adain:
+                return self.adain_apply(cf, style.adain[relu], style.n, alpha)
+            if plan.transform == "efdm" and plan.slices:
+                return self.efdm_sliced_apply(cf, style.efdm[relu], style.n, alpha, style.feats.get(relu))
+            if plan.transform == "efdm":
+                return self.efdm_apply(cf, style.efdm[relu], style.n, alpha)
+            if plan.transform == "ost":
+                return self.ost_apply(cf, style.wct[relu], style.n, alpha, want_info)
+            return self.wct_apply(cf, style.wct[relu], style.n, alpha, want_info)
+        if plan.soft is not None:              # regions: soft weights, or the hard labels' one-hot planes
+            return self.soft_level(cf, plan.soft, [sd.wct[relu] for sd in sides], None, alpha,
+                                   labels=plan.labels if plan.soft[1] is None else None)
+        if plan.mode == "interp" and adain:
+            return self.adain_apply_blend(cf, [sd.adain[relu] for sd in sides], plan.weights, alpha)
+        if plan.mode == "interp":
+            return self.wct_apply_blend(cf, [sd.wct[relu] for sd in sides], plan.weights, alpha, want_info)
+        if plan.mode == "regions":
+            lab = self.labels_resize(plan.labels, cf.H, cf.W)
+            return self.wct_apply_regions(cf, lab, [sd.wct[relu] for sd in sides], alpha, want_info)
+        m = sides[0].mst[relu]                 # "mst": label each pixel with its cluster, then regions
+        lab = self.mst_smooth(self.mst_data_term(cf, m["centres"], m["info"]), plan.mst[1])
+        out = self.wct_apply_regions(cf, lab, [sd.wct[relu] for sd in sides], alpha, want_info)
+        if capture is not None:
+            for key, val in (("mst_style_labels", m["labels"]), ("mst_centres", m["centres"]), ("mst_info", m["info"]),
+                             ("mst_content_labels", lab)):
+                capture.setdefault(key, []).append(val)
+        return out
 
     # ------------------------------------------------------------------ tiled stylisation (DESIGN.md §3.3.7)
     check_tile_size = staticmethod(options.check_tile_size)     # the tile edge of a tiled call: options.check_tile_size
@@ -1606,7 +1548,7 @@ class Engine(object):
         if prepared:
             self.check_prepared(style_u8, adain)
         main = torch.cuda.current_stream(self.device)
-        side = style_u8 if prepared else self._style_side(style_u8, main, wct=not adain, adain=adain)
+        side = style_u8 if prepared else self._style_side(style_u8, main, **style_states(adain))
         outs = []
         for i in range(N):
             sd = side if n_style == 1 else self.slice_prepared(side, i, i + 1)

@@ -491,13 +491,10 @@ class WCT(object):
                 soft_kw["content_weights"] = cweights.to(dev, non_blocking=True)
             elif mask_feather is not None:
                 soft_kw["mask_feather"] = float(mask_feather)
+            s, style_kw = None, {}
             if style_weights is not None:
                 w_dev = torch.from_numpy(weights).to(dev, non_blocking=True)
-                ist = [style_dev(x) for x in interp_styles]
-
-                def one_pass(x, first, levels=None):
-                    return eng.stylize(x, None, alpha=alpha, adain=adain, interp_styles=ist, interp_weights=w_dev,
-                                       seamless=seamless, levels=levels)
+                style_kw = dict(interp_styles=[style_dev(x) for x in interp_styles], interp_weights=w_dev)
             elif content_mask is not None and style_masks is not None:
                 lab = mask.to(dev, non_blocking=True)
                 # the same object stays the same object on the device: the engine shares its side
@@ -512,42 +509,31 @@ class WCT(object):
                 sm = [None if m is None else on_dev[id(m)] for m in style_masks]
                 if once:
                     rs, sm = eng.prepare_regions_call(rs, eng.check_region_masks(sm, rs)), None
-
-                def one_pass(x, first, levels=None):
-                    return eng.stylize(x, None, alpha=alpha, labels=None if content_weights is not None else lab, region_styles=rs,
-                                       region_masks=sm, seamless=seamless, levels=levels, **soft_kw)
+                style_kw = dict(labels=None if content_weights is not None else lab, region_styles=rs, region_masks=sm)
             elif content_mask is not None:
                 lab = mask.to(dev, non_blocking=True)
-                rs = [style_dev(x) for x in region_styles]
-
-                def one_pass(x, first, levels=None):
-                    return eng.stylize(x, None, alpha=alpha, labels=None if content_weights is not None else lab, region_styles=rs,
-                                       seamless=seamless, levels=levels, **soft_kw)
+                style_kw = dict(labels=None if content_weights is not None else lab,
+                             region_styles=[style_dev(x) for x in region_styles])
             elif mst is not None:
                 s = to_dev(styles)
                 if int(passes) > 1:
                     s = eng.prepare_mst_call(s, mst)
-
-                def one_pass(x, first, levels=None):
-                    return eng.stylize(x, s, alpha=alpha, mst=mst, mst_smooth=mst_smooth)
-            elif tile_size is not None:
-                s = style_dev(styles)
-
-                def one_pass(x, first, levels=None):
-                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size, ost=ost, seamless=seamless,
-                                             levels=levels)
+                style_kw = dict(mst=mst, mst_smooth=mst_smooth)
             else:
                 s = style_dev(styles)
+            # the style swap acts in the first pass only (stylize_video.py:117-121).  A shared style swaps the whole batch
+            # in one call; with one style per frame the engine swaps frame by frame.
+            first_only = dict(swap5=swap5, swap_targets=swap_targets, swap_labels=lab_dev, ss_temperature=ss_temperature,
+                              ss_balance=ss_balance)
+            later = dict(swap5=False, swap_targets=None, swap_labels=None, ss_temperature=None, ss_balance=0)
 
-                def one_pass(x, first, levels=None):
-                    # the style swap acts in the first pass only (stylize_video.py:117-121).  A shared style swaps the
-                    # whole batch in one call; with one style per frame the engine swaps frame by frame.
-                    return eng.stylize(x, s, alpha=alpha, adain=adain, swap5=swap5 and first, ss_alpha=ss_alpha,
-                                       ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
-                                       swap_targets=swap_targets if first else None, ost=ost, seamless=seamless, efdm=efdm,
-                                       efdm_slices=efdm_slices, swap_labels=lab_dev if first else None, levels=levels,
-                                       ss_temperature=ss_temperature if first else None,
-                                       ss_balance=ss_balance if first else 0, **soft_kw)
+            def one_pass(x, first, levels=None):
+                if tile_size is not None:
+                    return eng.stylize_tiled(x, s, alpha=alpha, adain=adain, tile_size=tile_size, ost=ost, seamless=seamless,
+                                             levels=levels)
+                return eng.stylize(x, s, alpha=alpha, adain=adain, ost=ost, efdm=efdm, efdm_slices=efdm_slices, seamless=seamless,
+                                   levels=levels, ss_alpha=ss_alpha, ss_patch_size=self.ss_patch_size, ss_stride=self.ss_stride,
+                                   **style_kw, **soft_kw, **(first_only if first else later))
             if ctf is not None:
                 whole = one_pass
 
